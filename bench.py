@@ -17,6 +17,9 @@ reference runs these from timers) and an L2 flush (a 512 MB memset) -- say so in
          D2H read of the frame statistics inside the timed region.
 `--impl reference` times the reference's own kernel source (oracle/_ref, compiled for the host by
 oracle/build_ref.py with OpenMP + atomics) on all host threads, on a bounded sample of the workload.
+`--dump-outputs DIR` writes the map a caller holds after the last timed frame (elevation_map.npy (7,W,W) and
+normal_map.npy (3,W,W), float32, 40 MB at 1024^2) so that two builds can be compared output for output: the frames
+are generated from fixed seeds, so the same arguments give the same inputs on every run.
 """
 import argparse
 import json
@@ -66,7 +69,7 @@ def make_frames(n_sensors, sensor, n_pool):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / power limit / throttle reasons sampled during the timed region."""
 
     def __init__(self, index=0):
         self.index = index
@@ -76,7 +79,7 @@ class ClockSampler:
     def start(self):
         q = ("timestamp,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
              "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-             "clocks_event_reasons.sw_power_cap")
+             "clocks_event_reasons.sw_power_cap,power.limit")
         try:
             self.proc = subprocess.Popen(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader,nounits",
                                           "-lms", "20", "-i", str(self.index)], stdout=subprocess.PIPE, text=True)
@@ -104,20 +107,21 @@ class ClockSampler:
         except Exception:
             pass
         import datetime
-        sm, mx, reasons, n_all = [], [], set(), 0
+        sm, mx, plim, reasons, n_all = [], [], [], set(), 0
         for r in self.rows:
             try:
                 n_all += 1
                 ts = datetime.datetime.strptime(r[0], "%Y/%m/%d %H:%M:%S.%f").timestamp()
                 if t_begin is not None and not (t_begin - 0.02 <= ts <= t_end + 0.02):
                     continue
-                sm.append(float(r[1])); mx.append(float(r[2]))
+                sm.append(float(r[1])); mx.append(float(r[2])); plim.append(float(r[8]))
                 for name, v in zip(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"), r[4:8]):
                     if v.lower().startswith("active"):
                         reasons.add(name)
             except Exception:
                 pass
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": max(mx) if mx else None,
+                "power_limit_w": max(plim) if plim else None,
                 "reasons": sorted(reasons), "samples": len(sm), "samples_total": n_all,
                 "window_s": None if t_begin is None else round(t_end - t_begin, 3)}
 
@@ -245,7 +249,7 @@ def check_sharded_parity(torch, dist, em, sh, frames, poses0, dev_pts, world, ra
 
 
 def reference_gpu_leg(torch, em, param, frames, dev_pts, between, ms_ours, flush):
-    """The reference's own CUDA kernels (its CUDA-C strings compiled by nvcc for sm_100a into oracle/_ref by
+    """The reference's own CUDA kernels (its CUDA-C strings compiled by nvcc for sm_90a into oracle/_ref by
     oracle/build_ref.py, launched as CuPy would: 128-thread blocks, one element per thread) + torch/cuDNN for the
     traversability filter, on the same GPU, same frames, same pre-frame state, same L2 flush -- the bar SURVEY 2.2 names."""
     sys.path.insert(0, os.path.join(ROOT, "tests"))
@@ -271,7 +275,7 @@ def reference_gpu_leg(torch, em, param, frames, dev_pts, between, ms_ours, flush
         em.input_pointcloud(dev_pts[f], ["x", "y", "z"], R, t, 0.02, 0.02)
     ms_ref = float(np.mean(times))
     return {"ms_per_frame": ms_ref, "mpoints_per_s": PTS_PER_SENSOR / (ms_ref * 1e-3) / 1e6, "speedup": ms_ref / ms_ours,
-            "steps": len(times), "note": "reference kernel source (custom_kernels.py strings) built by nvcc for sm_100a + torch/cuDNN "
+            "steps": len(times), "note": "reference kernel source (custom_kernels.py strings) built by nvcc for sm_90a + torch/cuDNN "
             "traversability, incl. its 2 host syncs per frame; device-resident cloud, cold L2, CUDA events"}
 
 
@@ -310,7 +314,12 @@ def _main():
     ap.add_argument("--config", default="B", choices=["B", "D", "E"],
                     help="BASELINE.json configuration: B = configs[1]/[2] (default, the headline metric), D = configs[3], E = configs[4]")
     ap.add_argument("--no-graph", action="store_true", help="config E: launch the frames eagerly instead of replaying CUDA graphs")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the map after the last timed frame as DIR/<name>.npy (config B)")
     args = ap.parse_args()
+    if args.steps < 1:
+        raise SystemExit("--steps must be at least 1")
+    if args.dump_outputs and args.config != "B":
+        raise SystemExit("--dump-outputs is implemented for config B")
     if args.warmup < 3:
         args.warmup = 3
     if args.impl == "reference":
@@ -433,6 +442,12 @@ def _main():
     # summary keeps the rows stamped inside that GPU-busy window
     t_busy0 = time.time()
     ms, launches = run(args.warmup, args.steps, host=False)
+    if args.dump_outputs and rank == 0:
+        torch.cuda.synchronize()
+        state, normal = em.get_state()
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        np.save(os.path.join(args.dump_outputs, "elevation_map.npy"), state)
+        np.save(os.path.join(args.dump_outputs, "normal_map.npy"), normal)
     # launches inside the timed frames only (exclude move_to / ticks): count one frame precisely
     between(0); torch.cuda.synchronize(); l0 = em.launch_count(); frame(0, dev_pts[0]); torch.cuda.synchronize()
     launches_per_frame = em.launch_count() - l0
@@ -469,13 +484,8 @@ def _main():
     n_total = world * PTS_PER_SENSOR
     value = n_total / (ms * 1e-3) / 1e6
     e2e = n_total / (ms_e2e * 1e-3) / 1e6
-    peaks = {}
-    try:
-        peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        pass
-    hbm = float(peaks.get("hbm_gbs", 6650.0))
-    peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)" if "hbm_gbs" in peaks else "fallback 6650 GB/s (B200_PROFILING.md)"
+    hbm = 3350.0
+    peak_src = "H100 SXM data sheet HBM3 bandwidth (not measured)"
     C = param.cell_n ** 2
     names = ["index+error", "drift", "fusion", "record", "raycast", "finalize", "post(dilate+cnn+normal)"]
     dom = int(np.argmax(stage[:7]))
@@ -489,15 +499,8 @@ def _main():
     dom_name = names[dom]
     ach = alg[dom_name] / (stage[dom] * 1e-3) / 1e9 if stage[dom] > 0 else 0.0
     frame_bytes = 24 * N * world + 80 * C
-    traffic = None          # dram__bytes_read+write of the dominant kernel per launch, from the committed ncu capture
-    try:
-        tr = json.load(open(os.path.join(ROOT, "profiles", "dominant_kernel_traffic.json")))
-        if tr.get("kernel") == dom_name:
-            traffic = tr["dram_bytes_per_launch"]
-    except Exception:
-        pass
     roofline = {"bound": "hbm", "kernel": dom_name, "achieved": ach, "peak": hbm, "unit": "GB/s",
-                "frac": ach / hbm, "traffic": traffic, "peak_source": peak_src,
+                "frac": ach / hbm, "peak_source": peak_src,
                 "kernel_ms": float(stage[dom]), "kernel_share_of_frame": float(stage[dom] / max(stage[7], 1e-9)),
                 "frame_algorithmic_bytes": frame_bytes,
                 "frame_achieved_gbs": frame_bytes / (ms * 1e-3) / 1e9, "frame_frac": frame_bytes / (ms * 1e-3) / 1e9 / hbm,
@@ -507,6 +510,7 @@ def _main():
         cpu = cpu_baseline_port(param, frames0[:4])
     line = {"metric": METRIC, "value": value, "unit": "Mpoints/s", "frames_per_s": 1e3 / ms, "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True, "scaling": "weak",
+            "device": torch.cuda.get_device_name(local_rank),
             "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": workload_string(world),
                        "frames_per_s": 1e3 / ms, "points_per_step": n_total,

@@ -1,4 +1,4 @@
-"""elevation_mapping_cupy_b200 -- B200-native (sm_100a) engine for the point-cloud fusion path of
+"""elevation_mapping_cupy_b200 -- H100-native (sm_90a) engine for the point-cloud fusion path of
 elevation_mapping_cupy, behind the reference's ElevationMap / plugin API."""
 from .parameter import Parameter, core_parameter  # noqa: F401
 

@@ -110,7 +110,7 @@ def load():
         if not os.path.exists(LIB_PATH):
             raise ImportError(
                 f"{LIB_PATH} is missing: build it with `python -m elevation_mapping_cupy_b200.build` "
-                "(nvcc, sm_100a).  There is no CPU fallback.")
+                "(nvcc, sm_90a).  There is no CPU fallback.")
         lib = C.CDLL(LIB_PATH)
         for name, (res, args) in SIGNATURES.items():
             fn = getattr(lib, name)

@@ -1,4 +1,4 @@
-"""Builds libemap.so in-tree with nvcc for sm_100a (no JIT cache: the .so travels with the repo)."""
+"""Builds libemap.so in-tree with nvcc for sm_90a (no JIT cache: the .so travels with the repo)."""
 import os
 import subprocess
 
@@ -7,7 +7,7 @@ CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libemap.so")
 SOURCES = ["emap_api.cu"]
 HEADERS = ["emap_kernels.cuh", "emap_device.cuh", "emap_inpaint.cuh", "emap_semantic.cuh", os.path.join("..", "..", "include", "emap.h")]
-NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared", "-cudart", "shared", "-Xptxas", "-v"]
 
 

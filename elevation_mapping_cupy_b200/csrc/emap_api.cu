@@ -1,5 +1,5 @@
 // emap_api.cu -- C ABI of libemap.so (see include/emap.h) and host-side orchestration.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo -O3 (see elevation_mapping_cupy_b200/build.py)
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 (see elevation_mapping_cupy_b200/build.py)
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -74,7 +74,7 @@ struct emap_handle {
   bool overlap_override = false;
   float overlap_z_override = 0.f;
   i64 pt_cap = 0;
-  int n_sm = 148, rc_blocks_per_sm = 8;
+  int n_sm = 132, rc_blocks_per_sm = 8;
   // last frame description
   std::vector<Pose> poses;
   std::vector<i64> offs;      // n_sensors + 1

@@ -1,4 +1,4 @@
-// emap_device.cuh -- device-side arithmetic of the fusion path (sm_100a).
+// emap_device.cuh -- device-side arithmetic of the fusion path (sm_90a).
 //
 // Every helper states which reference expression it reproduces; paths are relative to
 // /root/reference/elevation_mapping_cupy/script/elevation_mapping_cupy/ (CK.py =
@@ -53,7 +53,7 @@ struct DevCfg {
   u32 lut_lim2;                // half2 {LIM, LIM}: the march clamps fp16 coordinates to [-LIM, LIM] before the cell look-up
   int lut_p2;                  // bytes of one half (positive / negative fp16 patterns) of the shared-memory cell table
   int post_tma;                // k_post stages its tiles with TMA tensor copies (row pitch a multiple of 16 B, map >= one box)
-  float2 wp[3][2][9];          // traversability conv weights: layer, channel pair p, tap -> {w[2p][tap], w[2p+1][tap]} (FFMA2 operands)
+  float2 wp[3][2][9];          // traversability conv weights: layer, channel pair p, tap -> {w[2p][tap], w[2p+1][tap]}
   float wout[12];
 };
 

@@ -1,4 +1,4 @@
-// emap_kernels.cuh -- the per-frame kernels of the fusion path (sm_100a).
+// emap_kernels.cuh -- the per-frame kernels of the fusion path (sm_90a).
 //
 // Frame = elevation_mapping.py:316-391 (update_map_with_kernel) executed under the canonical
 // serialisation of SURVEY.md 8(c):
@@ -869,15 +869,11 @@ k_finalize(const DevCfg c, float* __restrict__ map, const CellScratch s, const F
 #define PT_Y 16
 #endif
 
-// two fp32 FMAs in one instruction (Blackwell FFMA2): acc.{x,y} = fma(w.{x,y}, t, acc.{x,y}), each IEEE round-to-nearest
-// (bit-identical to two fmaf); the scalar tap is broadcast by the instruction's operand modifier.
+// two channels' taps: acc.{x,y} = fma(w.{x,y}, t, acc.{x,y}), each IEEE round-to-nearest.  Hopper has no paired
+// fp32 FMA, so this is two scalar FFMAs (the same rounding, so the same bits).
 __device__ __forceinline__ void ffma2(float2& acc, const float2 w, const float t) {
-  u64 a, ww, tt;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(a) : "f"(acc.x), "f"(acc.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ww) : "f"(w.x), "f"(w.y));
-  asm("mov.b64 %0, {%1, %1};" : "=l"(tt) : "f"(t));
-  asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(a) : "l"(ww), "l"(tt));
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(acc.x), "=f"(acc.y) : "l"(a));
+  acc.x = __fmaf_rn(w.x, t, acc.x);
+  acc.y = __fmaf_rn(w.y, t, acc.y);
 }
 
 // K = dilation_size as a compile-time constant (0 = use c.dilation at run time).
@@ -1070,7 +1066,7 @@ k_post(const DevCfg c, float* __restrict__ map, float* __restrict__ trav_input, 
 #pragma unroll
           for (int qq = 0; qq < 3; qq++) t[p * 3 + qq] = d[(p - 1) * dil * DB + (qq - 1) * dil];
 #pragma unroll
-        for (int cp = 0; cp < 2; cp++) {                           // channels 2cp, 2cp+1: one FFMA2 per tap
+        for (int cp = 0; cp < 2; cp++) {                           // channels 2cp, 2cp+1 of each tap
           float2 s2 = make_float2(0.f, 0.f);
 #pragma unroll
           for (int j = 0; j < 9; j++) ffma2(s2, c.wp[l][cp][j], t[j]);

@@ -1,4 +1,4 @@
-// emap_semantic.cuh -- point-channel semantic fusion of a frame (SURVEY 8(f)2), sm_100a.
+// emap_semantic.cuh -- point-channel semantic fusion of a frame (SURVEY 8(f)2), sm_90a.
 //
 // Reference: semantic_map.py:223-259 (update_layers_pointcloud, called from elevation_mapping.py:371 right after
 // average_map_kernel), fusion/pointcloud_average.py:22-113, fusion/pointcloud_class_average.py, and

@@ -1,4 +1,4 @@
-"""Drop-in `ElevationMap` for the fusion path, implemented over libemap.so (hand-written sm_100a CUDA).
+"""Drop-in `ElevationMap` for the fusion path, implemented over libemap.so (hand-written sm_90a CUDA).
 
 Mirrors the public surface of the reference class
 (elevation_mapping_cupy/script/elevation_mapping_cupy/elevation_mapping.py:49-922, "EM.py" below):

@@ -1,5 +1,5 @@
 /*
- * emap.h -- C ABI of libemap.so, the B200-native (sm_100a) elevation-map fusion engine.
+ * emap.h -- C ABI of libemap.so, the H100-native (sm_90a) elevation-map fusion engine.
  *
  * This is the drop-in boundary for ONE path of leggedrobotics/elevation_mapping_cupy: the
  * per-frame point-cloud -> grid fusion + post-process chain.  Every entry point names the

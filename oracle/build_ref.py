@@ -12,7 +12,7 @@ under /root/reference, into oracle/_ref/ (git-ignored, travels to the GPU box):
     ElementwiseKernel body: `class float16` (cupy/_core/include/cupy/carray.cuh,
     third-party, not under /root/reference), CUDA's mixed-type min/max
     overloads, atomicAdd, and the `for i in range(size)` loop.
-  * `libref_gpu_<tag>.so`  -- the same strings compiled by nvcc for sm_100a
+  * `libref_gpu_<tag>.so`  -- the same strings compiled by nvcc for sm_90a
     (128-thread blocks, one element per thread, as CuPy launches them), so that
     the GPU box can run the real reference kernels next to the new engine.
 
@@ -255,7 +255,7 @@ def build(P, tag=None, gpu=False, verbose=False):
     with open(src_path, "w") as f:
         f.write(generate(P, gpu))
     if gpu:
-        cmd = ["nvcc", "-O3", "-std=c++17", "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo",
+        cmd = ["nvcc", "-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
                "-DREF_SHIM_GPU", "-I", HERE, "-shared", "-Xcompiler", "-fPIC", "-cudart", "shared",
                "-o", so, src_path]
     else:

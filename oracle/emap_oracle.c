@@ -29,8 +29,8 @@
  *
  * Parity pinning.  PINNED against the reference's own kernel source: oracle/build_ref.py compiles the CUDA-C strings
  * of kernels/custom_kernels.py and plugins/{min,max}_filter.py, robot_centric_elevation.py unmodified for the host
- * (and for sm_100a); tests/test_oracle_cpu.py compares this file with that build (live, and through the committed
- * golden vectors of tests/golden/): bit-identical cell indices, <= 1e-6 on every order-independent cell, for the
+ * (and for sm_90a); tests/test_oracle_cpu.py compares this file with that build through the golden vectors
+ * tests/golden/make_golden.py stores from it: bit-identical cell indices, <= 1e-6 on every order-independent cell, for the
  * deployed parameters, the dataclass defaults and four toggle / threshold combinations.  Restated rather than
  * executed (third party, absent here): CuPy's `class float16` (oracle/ref_shim.h), cuDNN's convolution order,
  * cupyx's uniform_filter -- see DESIGN.md section 2.

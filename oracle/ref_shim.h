@@ -2,7 +2,7 @@
 //
 // What CuPy places around the body of an ElementwiseKernel, restated so that the
 // reference's CUDA-C kernel strings (kernels/custom_kernels.py, plugins/min_filter.py)
-// compile unmodified with g++ (host) or nvcc (sm_100a).  See oracle/build_ref.py.
+// compile unmodified with g++ (host) or nvcc (sm_90a).  See oracle/build_ref.py.
 //
 // Third-party arithmetic restated here (NOT under /root/reference): CuPy's
 // `class float16` from cupy/_core/include/cupy/carray.cuh (version unpinned by the

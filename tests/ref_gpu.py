@@ -1,6 +1,6 @@
 """Test helper: the REFERENCE'S OWN CUDA kernels on the GPU.
 
-oracle/build_ref.py compiles the CUDA-C strings of kernels/custom_kernels.py unmodified with nvcc for sm_100a
+oracle/build_ref.py compiles the CUDA-C strings of kernels/custom_kernels.py unmodified with nvcc for sm_90a
 (oracle/_ref/libref_gpu_<tag>.so, 128-thread blocks, one element per thread, as CuPy launches them).  This class
 drives them in the order of elevation_mapping.py:316-391 with torch tensors standing in for the CuPy arrays and
 torch/cuDNN convolutions for traversability_filter.py:15-42 (that IS the reference's traversability path).

@@ -1,6 +1,6 @@
 """CPU tests of the oracle (no GPU): the C restatement against (1) the committed golden vectors produced
 by the REFERENCE'S OWN kernel source, (2) an independent NumPy restatement of the index arithmetic,
-(3) the live reference source when oracle/_ref is buildable here (i.e. /root/reference exists)."""
+(3) stored outputs of the reference's kernel source on further seeded inputs (tests/golden/make_golden.py)."""
 import os
 
 import numpy as np
@@ -8,6 +8,7 @@ import pytest
 
 from elevation_mapping_cupy_b200 import workloads as wl
 from elevation_mapping_cupy_b200.parameter import Parameter, core_parameter
+from helpers import FLAG_CASES, STAR_R, dilation_inputs, drift_frames, semantic_inputs, star_inputs
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
@@ -108,146 +109,82 @@ def test_smooth_matches_scipy(oracle_mod):
 
 
 def test_dilation_and_normal_against_reference_source(oracle_mod):
-    """live pin against the reference's dilation / normal / min_filter kernels (needs oracle/_ref)"""
-    from oracle import build_ref
+    """the reference's dilation / normal / min_filter kernels, stored in tests/golden/refsrc_core130.npz"""
+    g = np.load(os.path.join(GOLD, "refsrc_core130.npz"))
     p = core_parameter(130)
-    try:
-        rm = oracle_mod.RefKernelMap(p, "core130")
-    except FileNotFoundError:
-        pytest.skip("oracle/_ref not prebuilt and /root/reference absent")
-    import ctypes as C
-    rng = np.random.default_rng(3)
     W = 130
-    h = rng.standard_normal((W, W)).astype(np.float32)
-    mask = (rng.random((W, W)) < 0.15).astype(np.float32)
-    mask[:, :4] = (rng.random((W, 4)) < 0.6); mask[:, -4:] = (rng.random((W, 4)) < 0.6)   # exercise the row wrap-around
+    h, mask = dilation_inputs(W)
     ours, _ = oracle_mod.dilation(W, p.dilation_size, h, mask)
-    ref = np.zeros((W, W), np.float32); dummy = np.zeros((W, W), np.float32)
-    _p = oracle_mod._p
-    rm.lib.ref_dilation_filter(C.c_longlong(W * W), _p(h), _p(mask), _p(ref), _p(dummy), C.c_int(0))
-    assert np.array_equal(ours, ref)
-    rm.elevation_map[2] = mask
-    rm.update_normal(ours)
+    assert np.array_equal(ours, g["dilation"])
     # the host build of the reference source has no FMA contraction (g++ -ffp-contract=off) while the oracle
     # follows nvcc's contraction of CK.py:497 (fma(nx,nx, ny*ny) + 1): last-ulp differences only
     on = oracle_mod.normal(W, p.resolution, ours, mask)
-    assert np.array_equal(on != 0, rm.normal_map != 0)
-    assert np.abs(on - rm.normal_map).max() <= 2.4e-7
+    assert np.array_equal(on != 0, g["normal"] != 0)
+    assert np.abs(on - g["normal"]).max() <= 2.4e-7
     # min_filter: the reference updates in place (Gauss-Seidel); with one iteration on a mask whose invalid
     # cells have no invalid neighbours inside the window the two orders coincide
     m2 = np.ones((W, W), np.float32); m2[5:-5:4, 5:-5:4] = 0
-    rm.elevation_map[0] = h; rm.elevation_map[2] = m2
-    ref_mf = rm.min_filter(1)
     ours_mf, _ = oracle_mod.min_filter(W, 1, 1, h, m2)
-    assert np.array_equal(np.nan_to_num(ours_mf), np.nan_to_num(ref_mf))
+    assert np.array_equal(np.nan_to_num(ours_mf), np.nan_to_num(g["min_filter"]))
 
 
 def test_star_plugin_oracles_against_reference_source(oracle_mod):
-    """max_filter / robot_centric_elevation restatements vs the reference's kernels (host build of their source)."""
-    import ctypes as C
+    """max_filter / robot_centric_elevation restatements vs the reference's kernels (stored outputs of the host
+    build of their source)."""
+    g = np.load(os.path.join(GOLD, "refsrc_core130.npz"))
     p = core_parameter(130)
-    try:
-        rm = oracle_mod.RefKernelMap(p, "core130")
-    except FileNotFoundError:
-        pytest.skip("oracle/_ref not prebuilt and /root/reference absent")
     W = 130
-    rng = np.random.default_rng(8)
-    h = rng.standard_normal((W, W)).astype(np.float32)
-    m = (rng.random((W, W)) < 0.3).astype(np.float32)
-    _p = oracle_mod._p
-    # max_filter.py:100-113: every launch reads COPIES of the running arrays
-    cur_h, cur_m = h.copy(), m.copy()
-    for _ in range(4):
-        ih, im = cur_h.copy(), cur_m.copy()
-        rm.lib.ref_max_filter(C.c_longlong(W * W), _p(ih), _p(im), _p(cur_h), _p(cur_m), C.c_int(0))
-        if (cur_m > 0.5).all():
-            break
-    ref = np.where(cur_m > 0.5, cur_h, np.nan)
+    h, m = star_inputs(W)
     ours, _ = oracle_mod.max_filter(W, 1, 4, h, m)
-    assert np.array_equal(np.nan_to_num(ours, nan=-7), np.nan_to_num(ref, nan=-7))
+    assert np.array_equal(np.nan_to_num(ours, nan=-7), np.nan_to_num(g["max_filter"], nan=-7))
     # robot_centric_elevation.py:118-121
-    R = np.array([[0.9, 0.1, -0.2], [0.0, 1.0, 0.1], [0.15, -0.12, 0.97]], np.float32)
-    for thr, fn in ((True, rm.lib.ref_base_elevation_thr), (False, rm.lib.ref_base_elevation_raw)):
-        out = h.copy()
-        fn(C.c_longlong(W * W), _p(h), _p(m), _p(np.ascontiguousarray(R.reshape(9))), _p(out), C.c_int(0))
-        ours = oracle_mod.robot_centric(W, p.resolution, 1.1, thr, h, m, R)
+    for thr in (True, False):
+        out = g["base_elevation_thr" if thr else "base_elevation_raw"]
+        ours = oracle_mod.robot_centric(W, p.resolution, 1.1, thr, h, m, STAR_R)
         if thr:
             assert np.array_equal(ours, out)
         else:       # host build has no FMA contraction: last-ulp differences
             assert np.abs(ours - out).max() <= 5e-7 * max(1.0, np.abs(out).max())
 
 
-def _drift_frames(n=5):
-    out = []
-    for f in range(n):
-        pts, R, t = wl.lidar_cloud(0, f, n_rings=24, n_az=500, max_range=4.0)
-        pts = pts.copy(); pts[:, 2] += np.float32(0.03 * (f % 2))     # alternating 3 cm bias -> non-zero mean error
-        out.append((pts, R, t))
-    return out
-
-
 def test_drift_compensation_against_reference_source(oracle_mod):
-    """EM.py:346-357 fires (error_cnt > min_height_drift_cnt, |mean| < max_drift): oracle vs the reference's kernels"""
+    """EM.py:346-357 fires (error_cnt > min_height_drift_cnt, |mean| < max_drift): oracle vs the reference's kernels
+    (tests/golden/drift_core130.npz; traversability is not compared)"""
     from oracle.configs import DRIFT_OVERRIDES
+    g = np.load(os.path.join(GOLD, "drift_core130.npz"))
     p = core_parameter(130, **DRIFT_OVERRIDES)
-    try:
-        rf = oracle_mod.RefKernelMap(p, "drift130"); rr = oracle_mod.RefKernelMap(p, "drift130")
-    except FileNotFoundError:
-        pytest.skip("oracle/_ref not prebuilt and /root/reference absent")
     om = oracle_mod.OracleElevationMap(p)
     fired = 0
-    for pts, R, t in _drift_frames():
-        for m in (rf, rr):
-            m.elevation_map = om.elevation_map.copy(); m.normal_map = om.normal_map.copy(); m.center = om.center.copy()
-            m.additive_mean_error = om.additive_mean_error
-        for m, pp in ((om, pts), (rf, pts), (rr, pts[::-1].copy())):
-            m.move_to(t, R); m.input_pointcloud(pp, ["x", "y", "z"], R, t, 0.02, 0.02)
-        racy = np.zeros((130, 130), bool)
+    for f, (pts, R, t) in enumerate(drift_frames()):
+        om.move_to(t, R); om.input_pointcloud(pts, ["x", "y", "z"], R, t, 0.02, 0.02)
+        racy = g[f"racy_{f}"]
         for li in (0, 1, 2, 4, 5, 6):
-            racy |= np.abs(rf.elevation_map[li] - rr.elevation_map[li]) > 1e-6
-        for li in (0, 1, 2, 4, 5, 6):
-            assert np.abs(om.elevation_map[li] - rf.elevation_map[li])[~racy].max() <= 1e-6
+            assert np.abs(om.elevation_map[li] - g[f"ref_state_{f}"][li])[~racy].max() <= 1e-6
         if om.stats.drift_applied:
             fired += 1
-            assert abs(om.stats.mean_error - float(np.ravel(rf.mean_error)[0])) < 1e-6
+            assert abs(om.stats.mean_error - float(g[f"mean_error_{f}"])) < 1e-6
         om.update_variance(); om.update_time()
     assert fired >= 3
 
 
-@pytest.mark.parametrize("flags", [
-    dict(enable_edge_sharpen=False),
-    dict(enable_visibility_cleanup=False),
-    dict(enable_overlap_clearance=False, enable_drift_compensation=False),
-    dict(max_ray_length=2.0, cleanup_step=0.01, cleanup_cos_thresh=0.5, wall_num_thresh=3, dilation_size=2,
-         min_valid_distance=0.3, mahalanobis_thresh=1.0),
-])
-def test_flag_combinations_against_reference_source(oracle_mod, flags):
-    """feature toggles and thresholds are baked into the reference's kernel source: build it per combination
-    (needs /root/reference) and compare three frames on the order-independent cells"""
-    from oracle import build_ref
-    from oracle.configs import ref_dict
-    if not os.path.isdir(build_ref.REF_ROOT):
-        pytest.skip("/root/reference absent")
+@pytest.mark.parametrize("case", range(len(FLAG_CASES)), ids=[f"flags{i}" for i in range(len(FLAG_CASES))])
+def test_flag_combinations_against_reference_source(oracle_mod, case):
+    """feature toggles and thresholds are baked into the reference's kernel source: its build per combination,
+    run in input order and reversed (tests/golden/flags<case>_core130.npz), against the oracle for three frames on
+    the order-independent cells"""
+    flags = FLAG_CASES[case]
+    g = np.load(os.path.join(GOLD, f"flags{case}_core130.npz"))
     p = core_parameter(130, **flags)
     om = oracle_mod.OracleElevationMap(p)
     for f in range(3):
         pts, R, t = wl.lidar_cloud(0, f, n_rings=24, n_az=500, max_range=4.0)
-        refs = []
-        for order in (1, -1):
-            rm = oracle_mod.RefKernelMap(p, None)
-            rm.elevation_map = om.elevation_map.copy(); rm.normal_map = om.normal_map.copy(); rm.center = om.center.copy()
-            rm.additive_mean_error = om.additive_mean_error
-            rm.move_to(t, R); rm.input_pointcloud(pts[::order].copy(), ["x", "y", "z"], R, t, 0.02, 0.02)
-            refs.append(rm)
         om.move_to(t, R); om.input_pointcloud(pts, ["x", "y", "z"], R, t, 0.02, 0.02)
-        racy = np.zeros((130, 130), bool)
-        for li in (0, 1, 2, 4, 5, 6):
-            racy |= np.abs(refs[0].elevation_map[li] - refs[1].elevation_map[li]) > 1e-6
+        racy = g[f"racy_{f}"]
         n_cmp = int((~racy).sum())
         for li in (0, 1, 2, 4, 5, 6):
-            d = np.abs(om.elevation_map[li] - refs[0].elevation_map[li])[~racy]
+            d = np.abs(om.elevation_map[li] - g[f"ref_state_{f}"][li])[~racy]
             assert int((d > 1e-6).sum()) <= 3, (flags, f, li, float(d.max()))      # symmetric order-dependent patterns
-        assert np.array_equal(om.last_point_record[0], refs[0].last_point_record[0])
+        assert np.array_equal(om.last_point_record[0], g[f"ref_point_idx_{f}"])
         assert n_cmp > 0.9 * 130 * 130
         om.update_variance(); om.update_time()
 
@@ -255,43 +192,15 @@ def test_flag_combinations_against_reference_source(oracle_mod, flags):
 def test_semantic_fusion_oracle_against_reference_source(oracle_mod):
     """SURVEY 8(f)2: the NumPy restatement of the point-channel fusions (average, class_average, color) against the
     reference's own kernel strings (fusion/pointcloud_average.py, pointcloud_class_average.py, pointcloud_color.py),
-    compiled for the host by oracle/build_ref.py and run one element at a time in input order."""
-    import ctypes as C
-    from oracle import build_ref
-    from oracle.configs import REF_CONFIGS
-    from elevation_mapping_cupy_b200.parameter import core_parameter
-    from elevation_mapping_cupy_b200 import workloads as wl
-    try:
-        L = C.CDLL(build_ref.build(REF_CONFIGS["core130"], tag="core130", gpu=False))
-        L.ref_sem_sum
-    except (FileNotFoundError, AttributeError):
-        pytest.skip("oracle/_ref (with the fusion kernels) not prebuilt and /root/reference absent")
+    compiled for the host by oracle/build_ref.py and run one element at a time in input order (stored outputs)."""
+    g = np.load(os.path.join(GOLD, "refsrc_core130.npz"))
     p = core_parameter(130)
     W = 130
-    rng = np.random.default_rng(3)
-    pts, R, t = wl.uniform_cloud(0, 1, n=6000, half_extent=2.3)
-    idx, valid, inside, _ = oracle_mod.point_index(p, pts, R, t)
-    feats = np.stack([rng.random(len(pts), dtype=np.float32) * 3, rng.random(len(pts), dtype=np.float32),
-                      rng.integers(0, 1 << 24, len(pts)).astype(np.uint32).view(np.float32)], 1)
+    idx, valid, inside, _, feats, cnt = semantic_inputs(p, W)
     kinds = ["average", "class_average", "color"]
-    pall = np.ascontiguousarray(np.concatenate([np.stack([idx, valid, inside], 1).astype(np.float32), feats], 1))
-    cnt = np.bincount(idx[(valid > 0) & (inside > 0)], minlength=W * W).astype(np.float32)
-    cnt[rng.random(W * W) < 0.3] = 0          # as if some cells' points had been rejected by the fusion (CK.py:174-179)
-    new_el = np.zeros((7, W, W), np.float32); new_el[2] = cnt.reshape(W, W)
-    fp = lambda a: a.ctypes.data_as(C.c_void_p)
-    dummy = np.zeros(16, np.float32)
-    sem_ref = np.zeros((3, W, W), np.float32); sem_or = np.zeros((3, W, W), np.float32)
+    sem_or = np.zeros((3, W, W), np.float32)
     for frame in range(2):                    # second frame exercises class_average's running mix
-        newmap = np.zeros((3, W, W), np.float32)
-        for k, kind in enumerate(kinds[:2]):
-            chan = np.array([3 + k], np.int32); lay = np.array([k], np.int32); dims = np.array([pall.shape[1], 1], np.int32)
-            L.ref_sem_sum(C.c_longlong(len(pts)), fp(pall), fp(dummy), fp(dummy), fp(chan), fp(lay), fp(dims), fp(sem_ref), fp(newmap), 0)
-            fn = L.ref_sem_average if kind == "average" else L.ref_sem_class_average
-            fn(C.c_longlong(W * W), fp(newmap), fp(chan), fp(lay), fp(dims), fp(new_el), fp(sem_ref), 0)
-        color_map = np.zeros((4, W, W), np.uint32)
-        chan = np.array([5], np.int32); lay = np.array([2], np.int32); dims = np.array([pall.shape[1], 1], np.int32)
-        L.ref_sem_add_color(C.c_longlong(len(pts)), fp(pall), fp(dummy), fp(dummy), fp(chan), fp(lay), fp(dims), fp(color_map), 0)
-        L.ref_sem_color_average(C.c_longlong(W * W), fp(color_map), fp(chan), fp(lay), fp(dims), fp(sem_ref), 0)
+        sem_ref = g[f"semantic_{frame}"]
         oracle_mod.semantic_fuse(W, idx, valid, inside, feats, kinds, sem_or, cnt, alpha=0.5)
         assert np.array_equal(sem_ref[2].view(np.uint32), sem_or[2].view(np.uint32)), "color"
         for k in (0, 1):

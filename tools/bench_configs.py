@@ -6,21 +6,13 @@ D  configs[3]: 2048 x 2048 grid, 1 M-point dense depth-camera cloud per frame (5
 E  configs[4]: batched replay, 64 independent 512 x 512 maps x 100 k points each, 64 / N maps per GPU, one CUDA stream
    per map, every frame replayed as ONE captured CUDA graph (replicas only: no exchange between maps; SURVEY 8(e)).
 """
-import json
-import os
 import time
 
 import numpy as np
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
 
 def _peaks():
-    try:
-        p = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    except Exception:
-        return 6650.0, "fallback 6650 GB/s (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet HBM3 bandwidth (not measured)"
 
 
 def run_config_d(args, torch, dist, rank, local_rank, world, sampler):
@@ -72,7 +64,7 @@ def run_config_d(args, torch, dist, rank, local_rank, world, sampler):
             dist.barrier()
         torch.cuda.synchronize()
 
-    n_warm, n_steps = max(3, min(args.warmup, 4)), max(3, min(args.steps, 20))
+    n_warm, n_steps = max(3, min(args.warmup, 4)), args.steps
     for it in range(n_warm):
         f = it % n_pool
         between(f); step(f, dev[f])
@@ -129,6 +121,7 @@ def run_config_d(args, torch, dist, rank, local_rank, world, sampler):
     return {"metric": "Mpoints/s fused + map-update frames/s (2048^2 grid, 1M-pt depth frames, full post-process chain incl. inpainting)",
             "value": n_total / (ms * 1e-3) / 1e6, "unit": "Mpoints/s", "frames_per_s": world * 1e3 / ms, "n_gpus": world,
             "steps": n_steps, "warmup": n_warm, "requested_steps": args.steps, "ms_per_step": ms, "higher_is_better": True,
+            "device": torch.cuda.get_device_name(local_rank),
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": "BASELINE configs[3]: 2048x2048 grid, 0.04 m, 1M-pt depth-camera cloud/frame (5% NaN), raycast+overlap-clear+"
                                    "drift on, then min_filter -> smooth -> inpainting(telea) -> erosion on the device, the four layers exported to the host",
@@ -226,7 +219,7 @@ def run_config_e(args, torch, dist, rank, local_rank, world, sampler):
             dist.barrier()
         torch.cuda.synchronize()
 
-    n_warm, n_steps = max(3, args.warmup), max(5, args.steps)
+    n_warm, n_steps = max(3, args.warmup), args.steps
     for it in range(n_warm):
         ticks(it % n_pool); step(it % n_pool)
     barrier()
@@ -268,12 +261,13 @@ def run_config_e(args, torch, dist, rank, local_rank, world, sampler):
     return {"metric": "map-frames/s, batched replay: 64 independent 512^2 maps x 100k-pt frames (one map per stream, one CUDA graph per frame)",
             "value": N_MAPS * 1e3 / ms, "unit": "map-frames/s", "mpoints_per_s": N_MAPS * NPTS / (ms * 1e-3) / 1e6, "n_gpus": world,
             "steps": n_steps, "warmup": n_warm, "ms_per_step": ms, "higher_is_better": True, "scaling": "strong",
+            "device": torch.cuda.get_device_name(local_rank),
             "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": "BASELINE configs[4]: 64 independent 512x512 maps x 100k-pt LiDAR-like frame each per step, raycast+overlap-clear+drift on",
                        "parallelism": f"{n_local} maps per GPU x {world} GPU(s), one stream per map, replicas only (no exchange)",
                        "cuda_graph": bool(use_graph), "maps_per_gpu": n_local,
-                       "l2": "not flushed: the %d maps of a GPU (~30 MB of state + scratch each) exceed the 126 MB L2" % n_local
-                             if n_local * 30 > 126 else "not flushed (working set may fit L2)",
+                       "l2": "not flushed: the %d maps of a GPU (~30 MB of state + scratch each) exceed the 50 MB L2" % n_local
+                             if n_local * 30 > 50 else "not flushed (working set may fit L2)",
                        "untimed_between_steps": "move_to, update_variance, update_time on every map"},
             "e2e": {"value": N_MAPS * 1e3 / ms_e2e, "unit": "map-frames/s", "ms_per_step": ms_e2e, "h2d_bytes_per_step": 0,
                     "d2h_bytes_per_step": 72 * n_local, "note": "device-resident replay clouds (a replay batch lives in HBM); wall clock around graph launches + stats read-back"},

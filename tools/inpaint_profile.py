@@ -1,4 +1,4 @@
-"""One inpainting call on config D's map (2048^2, one 1M-point depth frame): the workload of profiles/*inpaint*."""
+"""One inpainting call on config D's map (2048^2, one 1M-point depth frame): the workload of DESIGN.md §4c."""
 import os, sys, time
 import numpy as np, torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Turn an .ncu-rep (ncu --set full) into the transposed per-kernel CSV kept under profiles/.
+"""Turn an .ncu-rep (ncu --set full) into the transposed per-kernel CSV.
 
-usage: tools/ncu_summary.py gpurun_out/prof_<tag>.ncu-rep profiles/<tag>_ncu_frame_kernels.csv [--first]
+usage: tools/ncu_summary.py <capture>.ncu-rep <tag>_ncu_frame_kernels.csv [--first]
 One column per captured launch (or, with --first, the first launch of each kernel name), one row per metric of
-interest.  Also prints dram bytes per launch of every kernel (for profiles/dominant_kernel_traffic.json)."""
+interest.  Also prints dram bytes per launch of every kernel."""
 import csv
 import io
 import subprocess
