@@ -74,7 +74,6 @@ SIGNATURES = {
     "emap_initialize_map_finish": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
     "emap_get_position": (C.c_int, [C.c_void_p, C.c_void_p]),
     "emap_get_map_with_name": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64]),
-    "emap_export_plane": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int64]),
     "emap_get_layers": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int32),
                                   C.c_void_p, C.c_int64]),
     "emap_layer_device_ptr": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),

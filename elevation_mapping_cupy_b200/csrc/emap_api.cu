@@ -25,9 +25,38 @@ struct StageTimer {
   bool have = false;
 };
 
+// Owner of one device allocation of n elements of T: freed with its owner; grown by replacing it (grow() below).
+// Reads as a T* in kernel launches and pointer arithmetic.
+template <typename T>
+class DevBuf {
+ public:
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { reset(); }
+  operator T*() const { return p_; }
+  size_t size() const { return n_; }
+  cudaError_t alloc(size_t n) {
+    reset();
+    const cudaError_t e = cudaMalloc(&p_, sizeof(T) * n);
+    if (e == cudaSuccess) n_ = n; else p_ = nullptr;
+    return e;
+  }
+  void reset() {
+    if (p_) cudaFree(p_);
+    p_ = nullptr; n_ = 0;
+  }
+  void swap(DevBuf& o) { std::swap(p_, o.p_); std::swap(n_, o.n_); }
+
+ private:
+  T* p_ = nullptr;
+  size_t n_ = 0;
+};
+
 }  // namespace
 
 struct emap_handle {
+  ~emap_handle();
   emap_config cfg;
   DevCfg dc;
   int device = 0;
@@ -37,43 +66,40 @@ struct emap_handle {
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;     // side-stream fork / join of the deferred fusion pushes
   cudaEvent_t ev_order = nullptr;                       // emap_wait_for_stream / emap_stream_wait_for
   // state
-  float* map = nullptr;       // (7,W,W)
-  float* map_alt = nullptr;   // shift target
+  DevBuf<float> map;          // (7,W,W)
+  DevBuf<float> map_alt;      // shift target
   CUtensorMap post_tm[2];     // TMA descriptors of the two state buffers as (W, W, 7) fp32 tensors, box = k_post's staged tile
   const float* post_tm_base[2] = {nullptr, nullptr};
-  float* normal = nullptr;    // (3,W,W)
-  float* trav_input = nullptr;
+  DevBuf<float> normal;       // (3,W,W)
+  DevBuf<float> trav_input;
   float center[3] = {0, 0, 0};        // fp32 like EM.py:61
   float base_rotation[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
   // scratch
   CellScratch sc{};
-  u32* u32_block = nullptr;   // cnt_ai (2 x u32 per cell) | cnt_fo (2 x u32 per cell) | n_ray
-  i64* i64_block = nullptr;   // SH | SV | DV
-  int* ukey_x = nullptr;      // exchange copy of the upper-bound keys (sharded frames)
   FrameScalars* fs = nullptr;
-  float* steps = nullptr;     // device march table: [0] dummy, [1 + k] = s_k, +inf padded to n_tab entries
+  DevBuf<char> xscratch;      // the library's exchange scratch (carve_exchange): sc's per-cell arrays + fs; empty once attached
+  DevBuf<int> ukey_x;         // exchange copy of the upper-bound keys (sharded frames)
+  DevBuf<float> steps;        // device march table: [0] dummy, [1 + k] = s_k, +inf padded to n_tab entries
   int n_tab = 0;
   std::vector<float> steps_host;
-  unsigned short* lut = nullptr;   // cell of every fp16 bit pattern (k_build_lut)
-  unsigned short* step_cnt = nullptr;   // march steps below every non-negative fp16 value (k_build_step_cnt)
-  unsigned char* dirty = nullptr;  // per-cell dirty bytes of single-GPU frames (CellScratch::dirty)
-  u32* tmap = nullptr;             // coarse ray map of the frame: RT x RT tile maxima of thr (keys)
+  DevBuf<unsigned short> lut;        // cell of every fp16 bit pattern (k_build_lut)
+  DevBuf<unsigned short> step_cnt;   // march steps below every non-negative fp16 value (k_build_step_cnt)
+  DevBuf<unsigned char> dirty;       // per-cell dirty bytes of single-GPU frames (CellScratch::dirty)
+  DevBuf<float> thr;                 // CellScratch::thr
+  DevBuf<u32> tmap;                  // coarse ray map of the frame: RT x RT tile maxima of thr (keys)
   size_t rc_smem = 0;
   RcLayout rc_lay{};
   int span_cells = 0;              // cells (per axis) one 31-step warp iteration of the march can span
   // points
-  void* d_in[2] = {nullptr, nullptr};
-  size_t d_in_bytes[2] = {0, 0};
+  DevBuf<char> d_in[2];
   cudaEvent_t in_free[2] = {nullptr, nullptr}, copy_done = nullptr;
   int in_sel = 0;
-  float4* xyzv = nullptr;
-  int* pidx = nullptr;
-  Ray* rays = nullptr;        // compacted rays of the frame, one segment per sensor (at the sensor's point offset)
-  int* ray_ctl = nullptr;     // per sensor: RC_CTL ints {ray count, work-queue counters}; zero between frames (k_finalize)
-  int ray_ctl_cap = 0;        // sensors
+  DevBuf<float4> xyzv;
+  DevBuf<int> pidx;
+  DevBuf<Ray> rays;           // compacted rays of the frame, one segment per sensor (at the sensor's point offset)
+  DevBuf<int> ray_ctl;        // per sensor: RC_CTL ints {ray count, work-queue counters}; zero between frames (k_finalize)
   bool overlap_override = false;
   float overlap_z_override = 0.f;
-  i64 pt_cap = 0;
   int n_sm = 132, rc_blocks_per_sm = 8;
   // last frame description
   std::vector<Pose> poses;
@@ -90,24 +116,20 @@ struct emap_handle {
   int pend_dtype = 0, pend_host = 0;
   bool zero_copy_pending = false;      // the index pass reads the caller's pinned host buffer: sync before returning
   // export staging
-  float* d_export = nullptr;
-  size_t d_export_floats = 0;
+  DevBuf<float> d_export;
   // plugin scratch
-  float* pl[4] = {nullptr, nullptr, nullptr, nullptr};
-  int* pl_cnt = nullptr;
-  int pl_cnt_cap = 0;
+  DevBuf<float> pl[4];
+  DevBuf<int> pl_cnt;
   // C-side communicator of sharded frames (emap_comm_init): NCCL, loaded at run time
   void* nccl_comm = nullptr;
   int comm_rank = 0, comm_nranks = 1;
   // semantic point-channel fusion (emap_semantic_configure): caller-owned layers, library-owned per-frame sums
   SemCfg sem{};
   float* sem_map = nullptr;        // (n_layers, W, W) fp32, device, caller-owned
-  i64* sem_fsum = nullptr;         // one 2^-32 fixed-point sum plane per averaged channel
-  u32* sem_csum = nullptr;         // r, g, b, count planes per colour channel
-  int sem_fslots = 0, sem_cslots = 0;
-  // inpainting scratch (allocated on first use): one block, carved into the arrays of InpaintView + lists + control
-  void* ip_block = nullptr;
-  size_t ip_bytes = 0;
+  DevBuf<i64> sem_fsum;            // one 2^-32 fixed-point sum plane per averaged channel
+  DevBuf<u32> sem_csum;            // r, g, b, count planes per colour channel
+  // inpainting scratch (allocated on first use): one block, carved by inpaint_scratch
+  DevBuf<char> ip_block;
   int ip_grid = 0;
   // misc
   int64_t launches = 0;
@@ -220,31 +242,83 @@ void build_steps(const emap_config& c, float max_len16, std::vector<float>& out)
   }
 }
 
-int ensure_points(emap_handle* h, i64 n) {
-  if (n <= h->pt_cap) return 0;
-  i64 cap = n + n / 4 + 1024;
+// Makes b hold at least n elements.  A smaller buffer is replaced by one of n + slack elements (zero-filled on the
+// handle's stream if `zero`), once every stream of the handle is idle: no queued kernel or copy still uses the old one.
+template <typename T>
+int grow(emap_handle* h, DevBuf<T>& b, size_t n, size_t slack, bool zero) {
+  if (n <= b.size()) return 0;
   CK(cudaStreamSynchronize(h->stream));
-  if (h->xyzv) cudaFree(h->xyzv);
-  if (h->pidx) cudaFree(h->pidx);
-  if (h->rays) cudaFree(h->rays);
-  h->xyzv = nullptr; h->pidx = nullptr; h->rays = nullptr; h->pt_cap = 0;
-  CK(cudaMalloc(&h->xyzv, sizeof(float4) * cap));
-  CK(cudaMalloc(&h->pidx, sizeof(int) * cap));
-  CK(cudaMalloc(&h->rays, sizeof(Ray) * cap));
-  h->pt_cap = cap;
+  CK(cudaStreamSynchronize(h->copy_stream));
+  CK(cudaStreamSynchronize(h->side_stream));
+  CK(b.alloc(n + slack));
+  if (zero) CK(cudaMemsetAsync(b, 0, sizeof(T) * b.size(), h->stream));
   return 0;
 }
 
-int ensure_in(emap_handle* h, int b, size_t bytes) {
-  if (bytes <= h->d_in_bytes[b]) return 0;
-  CK(cudaStreamSynchronize(h->stream));
-  CK(cudaStreamSynchronize(h->copy_stream));
-  if (h->d_in[b]) cudaFree(h->d_in[b]);
-  h->d_in[b] = nullptr; h->d_in_bytes[b] = 0;
-  size_t cap = bytes + bytes / 4 + 4096;
-  CK(cudaMalloc(&h->d_in[b], cap));
-  h->d_in_bytes[b] = cap;
-  return 0;
+// Sequential carving of one device block into 256-byte aligned arrays (`align` bytes: packed behind the previous one).
+// With a null base only the size is added up.
+struct Carver {
+  uintptr_t base;
+  size_t bytes = 0;
+  template <typename T>
+  T* take(size_t n, size_t align = 256) {
+    T* p = (T*)(base + bytes);
+    bytes = (bytes + sizeof(T) * n + align - 1) & ~(align - 1);
+    return p;
+  }
+};
+
+// The per-cell exchange scratch of a frame, one block: what the ranks of a sharded frame reduce.  Carves the block at
+// `base` into sc's exchanged arrays and fs; returns its size.
+size_t carve_exchange(size_t C, void* base, CellScratch& sc, FrameScalars*& fs) {
+  Carver b{(uintptr_t)base};
+  sc.cnt_ai = b.take<u64>(C, 8); sc.cnt_fo = b.take<u64>(C, 8); sc.n_ray = b.take<u32>(C);
+  sc.SH = b.take<i64>(C, 8); sc.SV = b.take<i64>(C, 8); sc.DV = b.take<i64>(C);
+  sc.last = b.take<u64>(C);
+  sc.rec = b.take<uint2>(C);
+  sc.ukv = b.take<u32>(C);
+  fs = b.take<FrameScalars>(1);
+  return b.bytes;
+}
+
+size_t exchange_bytes(size_t C) {
+  CellScratch sc;
+  FrameScalars* fs;
+  return carve_exchange(C, nullptr, sc, fs);
+}
+
+// Moves the exchange scratch of h to `base` in its between-frames state: all zero, upper-bound keys UKEY_NONE.
+cudaError_t place_exchange(emap_handle* h, void* base) {
+  const size_t C = (size_t)h->dc.C;
+  carve_exchange(C, base, h->sc, h->fs);
+  cudaError_t e = cudaMemsetAsync(base, 0, exchange_bytes(C), h->stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(h->sc.ukv, 0xff, sizeof(u32) * C, h->stream);
+  return e;
+}
+
+// The inpainting scratch of a W x W map, one block; N = (W + 2)^2 padded pixels.
+struct InpaintScratch {
+  InpaintView v;
+  int* heap[2];
+  int* children;
+  InpaintCtl* ctl;
+  size_t bytes;
+};
+
+InpaintScratch inpaint_scratch(int W, void* base) {
+  const size_t N = (size_t)(W + 2) * (W + 2);
+  Carver b{(uintptr_t)base};
+  InpaintScratch s;
+  s.v.rows = s.v.cols = W + 2;
+  s.v.f = b.take<uint8_t>(N); s.v.ck = b.take<uint8_t>(N); s.v.vc[0] = b.take<uint8_t>(N); s.v.vc[1] = b.take<uint8_t>(N);
+  s.v.img = b.take<uint8_t>((size_t)W * W);
+  s.v.T = b.take<float>(N); s.v.Tc[0] = b.take<float>(N); s.v.Tc[1] = b.take<float>(N);
+  s.v.ord = b.take<uint32_t>(N);
+  s.heap[0] = b.take<int>(N); s.heap[1] = b.take<int>(N); s.children = b.take<int>(N);
+  s.ctl = b.take<InpaintCtl>(1);
+  s.v.em = b.take<uint32_t>(N);
+  s.bytes = b.bytes;
+  return s;
 }
 
 // NVTX range around the launches of one frame stage (visible in nsys / ncu timelines; a no-op without a tool attached)
@@ -272,7 +346,7 @@ int launch_index(emap_handle* h, const Pose& q, const T* pts, i64 n, i64 stride,
 int frame_begin(emap_handle* h, int32_t n_sensors, const void* const* points, const int64_t* n, int64_t row_stride,
                 int dtype, int is_device_ptr, const float* R, const float* t, int64_t global_off, float pn, float on,
                 bool sharded) {
-  h->sc.dirty = sharded ? nullptr : h->dirty;      // sharded frames derive the marker from the all-reduced counts
+  h->sc.dirty = sharded ? nullptr : (unsigned char*)h->dirty;      // sharded frames derive the marker from the all-reduced counts
   h->fused_drift = !sharded;
   if (n_sensors < 1 || row_stride < 3 || (dtype != EMAP_F32 && dtype != EMAP_F64))
     return fail(h, EMAP_ERR_INVALID, "emap_input: n_sensors >= 1, row_stride >= 3, dtype f32/f64 required");
@@ -285,23 +359,18 @@ int frame_begin(emap_handle* h, int32_t n_sensors, const void* const* points, co
   const i64 N = h->offs[n_sensors];
   if (global_off + N >= (1ll << 31)) return fail(h, EMAP_ERR_INVALID, "emap_input: more than 2^31 points in a frame");
   h->n_points = N; h->global_off = global_off; h->pos_noise = pn; h->ori_noise = on;
-  int rc = ensure_points(h, N);
-  if (rc) return rc;
+  int rc;
+  if ((rc = grow(h, h->xyzv, N, N / 4 + 1024, false)) || (rc = grow(h, h->pidx, N, N / 4 + 1024, false)) ||
+      (rc = grow(h, h->rays, N, N / 4 + 1024, false)))
+    return rc;
   h->poses.resize(n_sensors);
   for (int s = 0; s < n_sensors; s++) {
     float tr[3];
     for (int k = 0; k < 3; k++) tr[k] = t[3 * s + k] - h->center[k];      // EM.py:314,333 (fp32)
     make_pose(R + 9 * s, tr, &h->poses[s]);
   }
-  // frame scalars: keep mean / additive error, zero the accumulators
-  if (n_sensors > h->ray_ctl_cap) {
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->ray_ctl) cudaFree(h->ray_ctl);
-    h->ray_ctl = nullptr; h->ray_ctl_cap = 0;
-    CK(cudaMalloc(&h->ray_ctl, sizeof(int) * RC_CTL * (n_sensors + 8)));
-    CK(cudaMemsetAsync(h->ray_ctl, 0, sizeof(int) * RC_CTL * (n_sensors + 8), h->stream));   // ordered before the frame's kernels
-    h->ray_ctl_cap = n_sensors + 8;
-  }
+  // zero-filled on the stream: ordered before the frame's kernels
+  if ((rc = grow(h, h->ray_ctl, (size_t)RC_CTL * n_sensors, RC_CTL * 8, true))) return rc;
   h->overlap_override = false;
   if (stage_mark(h, 0)) return EMAP_ERR_CUDA;
   const void* dev_pts[64];
@@ -330,8 +399,7 @@ int frame_begin(emap_handle* h, int32_t n_sensors, const void* const* points, co
     const int b = h->in_sel; h->in_sel ^= 1;
     size_t total = 0;
     for (int s = 0; s < n_sensors; s++) total += (size_t)n[s] * row_stride * esz;
-    rc = ensure_in(h, b, total);
-    if (rc) return rc;
+    if ((rc = grow(h, h->d_in[b], total, total / 4 + 4096, false))) return rc;
     CK(cudaStreamWaitEvent(h->copy_stream, h->in_free[b], 0));
     size_t o = 0;
     for (int s = 0; s < n_sensors; s++) {
@@ -558,8 +626,8 @@ int launch_post(emap_handle* h) {
 
 int frame_finish(emap_handle* h) {
   NvtxRange nv("emap:finalize+post");
-  if (h->dc.W % 4 == 0) PDL(k_finalize<4>, cdiv(h->dc.C / 4, 256), 256, 0, h->dc, h->map, h->sc, (const FrameScalars*)h->fs, h->dc.visibility, h->ray_ctl, RC_CTL * h->ray_ctl_cap, h->fused_drift ? h->fs : nullptr, h->tmap);
-  else PDL(k_finalize<1>, cdiv(h->dc.C, 256), 256, 0, h->dc, h->map, h->sc, (const FrameScalars*)h->fs, h->dc.visibility, h->ray_ctl, RC_CTL * h->ray_ctl_cap, h->fused_drift ? h->fs : nullptr, h->tmap);
+  if (h->dc.W % 4 == 0) PDL(k_finalize<4>, cdiv(h->dc.C / 4, 256), 256, 0, h->dc, h->map, h->sc, (const FrameScalars*)h->fs, h->dc.visibility, h->ray_ctl, (int)h->ray_ctl.size(), h->fused_drift ? h->fs : nullptr, h->tmap);
+  else PDL(k_finalize<1>, cdiv(h->dc.C, 256), 256, 0, h->dc, h->map, h->sc, (const FrameScalars*)h->fs, h->dc.visibility, h->ray_ctl, (int)h->ray_ctl.size(), h->fused_drift ? h->fs : nullptr, h->tmap);
   LAUNCH_CHECK();
   if (stage_mark(h, 6)) return EMAP_ERR_CUDA;
   int rc = launch_post(h);
@@ -577,7 +645,10 @@ int layer_index(const char* name) {
 }
 
 int alloc_plugin_scratch(emap_handle* h) {
-  for (int i = 0; i < 4; i++) if (!h->pl[i]) CK(cudaMalloc(&h->pl[i], sizeof(float) * h->dc.C));
+  for (int i = 0; i < 4; i++) {
+    int rc = grow(h, h->pl[i], h->dc.C, 0, false);
+    if (rc) return rc;
+  }
   return 0;
 }
 
@@ -591,6 +662,72 @@ __global__ void k_ukey_merge(int C, u32* __restrict__ ukv, const int* __restrict
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= C) return;
   ukv[i] = ((u32)x[i]) ^ 0x80000000u;
+}
+
+// The arrays the ranks of a sharded frame reduce after phase 1..3 (kinds: see emap_exchange in emap.h).  Phase 3 first
+// extracts the upper-bound keys in s32 order; without visibility cleanup it exchanges nothing.
+int exchange_list(emap_handle* h, int phase, emap_exchange out[3], int32_t* n_out) {
+  const i64 C = h->dc.C;
+  if (phase == 1) {          // after begin: counts (CK.py:334,336) and the drift statistics (CK.py:332-333)
+    out[0] = {h->sc.cnt_ai, 2 * C, 3};          // two 32-bit counters per cell: an int32 SUM keeps them apart
+    out[1] = {&h->fs->E, 2, 0};
+    *n_out = 2;
+  } else if (phase == 2) {   // after fusion: sums, counts, last-writer keys
+    out[0] = {h->sc.SH, 2 * C, 0};
+    out[1] = {h->sc.cnt_fo, 2 * C, 3};
+    out[2] = {h->sc.last, C, 1};
+    *n_out = 3;
+  } else if (h->dc.visibility) {   // after the ray-cast: decrements, counts, upper-bound keys
+    k_ukey_extract<<<cdiv(C, 256), 256, 0, h->stream>>>((int)C, h->sc.ukv, h->ukey_x);
+    LAUNCH_CHECK();
+    out[0] = {h->sc.DV, C, 0};
+    out[1] = {h->sc.n_ray, C, 3};
+    out[2] = {h->ukey_x, C, 2};
+    *n_out = 3;
+    h->phase = 4;
+  } else *n_out = 0;
+  return 0;
+}
+
+// last phase of a sharded frame: the reduced upper-bound keys back to u32 (if phase 3 exchanged them), then finalize
+int shard_finish(emap_handle* h) {
+  if (h->phase == 4) {
+    k_ukey_merge<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc.C, h->sc.ukv, h->ukey_x);
+    LAUNCH_CHECK();
+  }
+  return frame_finish(h);
+}
+
+// export_value's kinds 0..8 (kind 9: a caller plane)
+const char* const kExportNames[] = {"elevation", "variance", "traversability", "time", "upper_bound", "is_upper_bound",
+                                    "normal_x", "normal_y", "normal_z"};
+
+// Layers by one k_export_multi launch, one device-to-host copy and one synchronisation.  names[k]: a name of
+// kExportNames, or planes[k] != NULL: a (W,W) device plane exported with flags[k] (bit 0 fill_nan, bit 1 add the centre height).
+int export_layers(emap_handle* h, int32_t n, const char* const* names, const float* const* planes, const int32_t* flags,
+                  float* out_host, int64_t n_out_total) {
+  if (n < 1 || n > EXPORT_MAX_LAYERS || !out_host) return fail(h, EMAP_ERR_INVALID, "emap_get_layers: 1..24 layers, non-null output");
+  const int Wo = h->dc.W - 2;
+  const size_t per = (size_t)Wo * Wo;
+  if (n_out_total != (int64_t)(per * n)) return fail(h, EMAP_ERR_INVALID, "output must hold n * (cell_n-2)^2 floats");
+  ExportList L;
+  memset(&L, 0, sizeof(L));
+  L.n = n;
+  for (int k = 0; k < n; k++) {
+    if (planes && planes[k]) { L.kind[k] = 9; L.plane[k] = planes[k]; L.flags[k] = flags ? flags[k] : 0; continue; }
+    int kind = -1;
+    if (names && names[k]) for (int i = 0; i < 9; i++) if (!strcmp(names[k], kExportNames[i])) kind = i;
+    if (kind < 0) { h->err = std::string("Layer ") + (names && names[k] ? names[k] : "(null)") + " is not in the map"; return EMAP_ERR_NOLAYER; }
+    L.kind[k] = kind;
+  }
+  int rc = grow(h, h->d_export, per * n, 0, false);
+  if (rc) return rc;
+  k_export_multi<<<dim3(cdiv((i64)per, 256), n), 256, 0, h->stream>>>(h->dc, h->map, h->normal, h->d_export, L, h->center[2],
+                                                                       h->cfg.use_only_above_for_upper_bound);
+  LAUNCH_CHECK();
+  CK(cudaMemcpyAsync(out_host, h->d_export, sizeof(float) * per * n, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return EMAP_OK;
 }
 
 }  // namespace
@@ -614,7 +751,7 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   h->cfg = *cfg; h->device = device;
   auto bail = [&](const char* what, cudaError_t e) {
     g_create_error = std::string(what) + ": " + cudaGetErrorString(e);
-    emap_destroy(h);
+    delete h;
     return (int)EMAP_ERR_CUDA;
   };
   cudaError_t e;
@@ -637,45 +774,32 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   if ((e = cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming)) != cudaSuccess) return bail("event", e);
   if ((e = cudaEventCreateWithFlags(&h->ev_order, cudaEventDisableTiming)) != cudaSuccess) return bail("event", e);
   for (int k = 0; k < 9; k++) if ((e = cudaEventCreate(&h->st.ev[k])) != cudaSuccess) return bail("event", e);
-#define ALLOC(p, bytes) if ((e = cudaMalloc(&(p), (bytes))) != cudaSuccess) return bail("cudaMalloc", e)
+#define ALLOC(buf, n) if ((e = (buf).alloc(n)) != cudaSuccess) return bail("cudaMalloc", e)
 #define TRY(call) if ((e = (call)) != cudaSuccess) return bail(#call, e)
-  ALLOC(h->map, sizeof(float) * 7 * C);
-  ALLOC(h->map_alt, sizeof(float) * 7 * C);
-  ALLOC(h->normal, sizeof(float) * 3 * C);
-  ALLOC(h->trav_input, sizeof(float) * C);
-  ALLOC(h->u32_block, sizeof(u32) * 5 * C);
-  ALLOC(h->i64_block, sizeof(i64) * 3 * C);
-  ALLOC(h->sc.last, sizeof(u64) * C);
-  ALLOC(h->sc.rec, sizeof(uint2) * C);
-  ALLOC(h->sc.thr, sizeof(float) * C);
-  ALLOC(h->sc.ukv, sizeof(u32) * C);
+  ALLOC(h->map, 7 * C);
+  ALLOC(h->map_alt, 7 * C);
+  ALLOC(h->normal, 3 * C);
+  ALLOC(h->trav_input, C);
+  ALLOC(h->xscratch, exchange_bytes(C));
+  ALLOC(h->thr, C);
   ALLOC(h->dirty, C + 16);
-  ALLOC(h->ukey_x, sizeof(int) * C);
-  ALLOC(h->fs, sizeof(FrameScalars));
-  ALLOC(h->lut, sizeof(unsigned short) * 65536);
-  ALLOC(h->tmap, sizeof(u32) * RT * RT);
-  ALLOC(h->step_cnt, sizeof(unsigned short) * (0x7c00 + 8));
-  ALLOC(h->d_export, sizeof(float) * C);
-  h->d_export_floats = C;
+  ALLOC(h->ukey_x, C);
+  ALLOC(h->lut, 65536);
+  ALLOC(h->tmap, RT * RT);
+  ALLOC(h->step_cnt, 0x7c00 + 8);
   // march table as k_raycast reads it: [0] unused (lane 0 of the first warp iteration), [1 + k] = s_k, +inf padding up to
   // a whole number of 31-step warp iterations + one warp of over-read
   h->n_tab = (int)(((h->steps_host.size() + RC_STRIDE - 1) / RC_STRIDE) * RC_STRIDE + 64) & ~1;
-  ALLOC(h->steps, sizeof(float) * h->n_tab);
+  ALLOC(h->steps, h->n_tab);
 #undef ALLOC
-  h->sc.cnt_ai = (u64*)h->u32_block; h->sc.cnt_fo = (u64*)(h->u32_block + 2 * C); h->sc.n_ray = h->u32_block + 4 * C;
-  h->sc.SH = h->i64_block; h->sc.SV = h->i64_block + C; h->sc.DV = h->i64_block + 2 * C;
+  h->sc.thr = h->thr;
   h->sc.dirty = h->dirty;
-  TRY(cudaMemsetAsync(h->u32_block, 0, sizeof(u32) * 5 * C, h->stream));
-  TRY(cudaMemsetAsync(h->i64_block, 0, sizeof(i64) * 3 * C, h->stream));
-  TRY(cudaMemsetAsync(h->sc.last, 0, sizeof(u64) * C, h->stream));
-  TRY(cudaMemsetAsync(h->sc.rec, 0, sizeof(uint2) * C, h->stream));
-  TRY(cudaMemsetAsync(h->sc.thr, 0, sizeof(float) * C, h->stream));
-  TRY(cudaMemsetAsync(h->sc.ukv, 0xff, sizeof(u32) * C, h->stream));      // UKEY_NONE
+  TRY(place_exchange(h, h->xscratch));
+  TRY(cudaMemsetAsync(h->thr, 0, sizeof(float) * C, h->stream));
   TRY(cudaMemsetAsync(h->dirty, 0, C + 16, h->stream));
   TRY(cudaMemsetAsync(h->tmap, 0, sizeof(u32) * RT * RT, h->stream));
   TRY(cudaMemsetAsync(h->normal, 0, sizeof(float) * 3 * C, h->stream));
   TRY(cudaMemsetAsync(h->trav_input, 0, sizeof(float) * C, h->stream));
-  TRY(cudaMemsetAsync(h->fs, 0, sizeof(FrameScalars), h->stream));
   {
     std::vector<float> tab((size_t)h->n_tab, INFINITY);
     tab[0] = NAN;       // "step -1" of lane 0 in a ray's first warp iteration: NaN -> cell (0, 0), see k_raycast
@@ -689,7 +813,7 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   k_init<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc, h->map);
   h->launches += 2;
   if (make_post_tm(h, 0, h->map) || make_post_tm(h, 1, h->map_alt)) {
-    g_create_error = h->err; emap_destroy(h); return EMAP_ERR_CUDA;
+    g_create_error = h->err; delete h; return EMAP_ERR_CUDA;
   }
   if (post_smem(h->dc) > 48 * 1024)
     TRY(cudaFuncSetAttribute(k_post<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)post_smem(h->dc)));
@@ -731,31 +855,33 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   return EMAP_OK;
 }
 
-static void comm_release(emap_handle* h);
-
 int emap_destroy(emap_handle* h) {
-  if (!h) return EMAP_OK;
-  cudaSetDevice(h->device);
-  if (h->stream) cudaStreamSynchronize(h->stream);
-  if (h->copy_stream) cudaStreamSynchronize(h->copy_stream);
-  comm_release(h);
-  if (h->attached) { h->u32_block = nullptr; h->i64_block = nullptr; h->sc.last = nullptr; h->sc.rec = nullptr; h->sc.ukv = nullptr; h->fs = nullptr; }
-  void* ptrs[] = {h->map, h->map_alt, h->normal, h->trav_input, h->u32_block, h->i64_block, h->sc.last, h->sc.rec,
-                  h->sc.ukv, h->ukey_x, h->fs, h->steps, h->d_export, h->d_in[0], h->d_in[1], h->xyzv, h->pidx, h->pl[0], h->pl[1],
-                  h->pl[2], h->pl[3], h->pl_cnt, h->rays, h->ray_ctl, h->sc.thr, h->dirty, h->lut, h->step_cnt, h->tmap, h->ip_block, h->sem_fsum, h->sem_csum};
-  for (void* p : ptrs) if (p) cudaFree(p);
-  for (int b = 0; b < 2; b++) if (h->in_free[b]) cudaEventDestroy(h->in_free[b]);
-  if (h->copy_done) cudaEventDestroy(h->copy_done);
-  if (h->ev_fork) cudaEventDestroy(h->ev_fork);
-  if (h->ev_join) cudaEventDestroy(h->ev_join);
-  if (h->ev_order) cudaEventDestroy(h->ev_order);
-  if (h->side_stream) { cudaStreamSynchronize(h->side_stream); cudaStreamDestroy(h->side_stream); }
-  for (int k = 0; k < 9; k++) if (h->st.ev[k]) cudaEventDestroy(h->st.ev[k]);
-  if (h->own_stream) cudaStreamDestroy(h->own_stream);
-  if (h->copy_stream) cudaStreamDestroy(h->copy_stream);
   delete h;
   return EMAP_OK;
 }
+
+static void comm_release(emap_handle* h);
+
+}  // extern "C"
+
+// the device buffers are released after this body, by their DevBuf members
+emap_handle::~emap_handle() {
+  cudaSetDevice(device);
+  if (stream) cudaStreamSynchronize(stream);
+  if (copy_stream) cudaStreamSynchronize(copy_stream);
+  comm_release(this);
+  for (int b = 0; b < 2; b++) if (in_free[b]) cudaEventDestroy(in_free[b]);
+  if (copy_done) cudaEventDestroy(copy_done);
+  if (ev_fork) cudaEventDestroy(ev_fork);
+  if (ev_join) cudaEventDestroy(ev_join);
+  if (ev_order) cudaEventDestroy(ev_order);
+  if (side_stream) { cudaStreamSynchronize(side_stream); cudaStreamDestroy(side_stream); }
+  for (int k = 0; k < 9; k++) if (st.ev[k]) cudaEventDestroy(st.ev[k]);
+  if (own_stream) cudaStreamDestroy(own_stream);
+  if (copy_stream) cudaStreamDestroy(copy_stream);
+}
+
+extern "C" {
 
 #define ENTER(h)                                               \
   if (!(h)) return EMAP_ERR_INVALID;                           \
@@ -818,22 +944,8 @@ int emap_semantic_configure(emap_handle* h, int32_t n_channels, const int32_t* c
     c.slot[k] = (kind[k] == SEM_COLOR) ? 4 * nc++ : nf++;
   }
   const size_t C = (size_t)h->dc.C;
-  if (nf > h->sem_fslots) {
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->sem_fsum) cudaFree(h->sem_fsum);
-    h->sem_fsum = nullptr; h->sem_fslots = 0;
-    CK(cudaMalloc(&h->sem_fsum, sizeof(i64) * C * nf));
-    CK(cudaMemsetAsync(h->sem_fsum, 0, sizeof(i64) * C * nf, h->stream));
-    h->sem_fslots = nf;
-  }
-  if (nc > h->sem_cslots) {
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->sem_csum) cudaFree(h->sem_csum);
-    h->sem_csum = nullptr; h->sem_cslots = 0;
-    CK(cudaMalloc(&h->sem_csum, sizeof(u32) * C * 4 * nc));
-    CK(cudaMemsetAsync(h->sem_csum, 0, sizeof(u32) * C * 4 * nc, h->stream));
-    h->sem_cslots = nc;
-  }
+  int rc;
+  if ((rc = grow(h, h->sem_fsum, C * nf, 0, true)) || (rc = grow(h, h->sem_csum, C * 4 * nc, 0, true))) return rc;
   h->sem = c; h->sem_map = semantic_map_device;
   return EMAP_OK;
 }
@@ -865,12 +977,9 @@ int emap_shard_begin(emap_handle* h, int32_t n_sensors, const void* const* point
   return rc;
 }
 
-static size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 int64_t emap_shard_scratch_bytes(const emap_handle* h) {
   if (!h) return EMAP_ERR_INVALID;
-  const size_t C = (size_t)h->dc.C;
-  return (int64_t)(al256(4 * 5 * C) + al256(8 * 3 * C) + al256(8 * C) + al256(8 * C) + al256(4 * C) + al256(sizeof(FrameScalars)));
+  return (int64_t)exchange_bytes((size_t)h->dc.C);
 }
 
 int emap_shard_attach(emap_handle* h, void* local_base, void* multicast_base, int64_t bytes) {
@@ -878,24 +987,12 @@ int emap_shard_attach(emap_handle* h, void* local_base, void* multicast_base, in
   if (!local_base || !multicast_base || bytes < emap_shard_scratch_bytes(h))
     return fail(h, EMAP_ERR_INVALID, "emap_shard_attach: need local + multicast base of >= emap_shard_scratch_bytes()");
   CK(cudaStreamSynchronize(h->stream));
-  const size_t C = (size_t)h->dc.C;
-  char* b = (char*)local_base;
   FrameScalars keep;
   CK(cudaMemcpy(&keep, h->fs, sizeof(keep), cudaMemcpyDeviceToHost));
   // the library's own scratch is released; the symmetric block (owned by the caller) replaces it
-  void* old[] = {h->u32_block, h->i64_block, h->sc.last, h->sc.rec, h->sc.ukv, h->fs};
-  for (void* p : old) if (p && !h->attached) cudaFree(p);
-  h->u32_block = (u32*)b; b += al256(4 * 5 * C);
-  h->i64_block = (i64*)b; b += al256(8 * 3 * C);
-  h->sc.last = (u64*)b; b += al256(8 * C);
-  h->sc.rec = (uint2*)b; b += al256(8 * C);
-  h->sc.ukv = (u32*)b; b += al256(4 * C);
-  h->fs = (FrameScalars*)b;
-  h->sc.cnt_ai = (u64*)h->u32_block; h->sc.cnt_fo = (u64*)(h->u32_block + 2 * C); h->sc.n_ray = h->u32_block + 4 * C;
-  h->sc.SH = h->i64_block; h->sc.SV = h->i64_block + C; h->sc.DV = h->i64_block + 2 * C;
+  h->xscratch.reset();
+  CK(place_exchange(h, local_base));
   h->sc.mc_off = (i64)((char*)multicast_base - (char*)local_base);
-  CK(cudaMemsetAsync(local_base, 0, (size_t)emap_shard_scratch_bytes(h), h->stream));
-  CK(cudaMemsetAsync(h->sc.ukv, 0xff, sizeof(u32) * C, h->stream));
   CK(cudaMemcpyAsync(h->fs, &keep, sizeof(keep), cudaMemcpyHostToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   h->attached = true;
@@ -912,31 +1009,11 @@ int emap_shard_set_overlap_z(emap_handle* h, float z_abs) {
 int emap_shard_exchange(emap_handle* h, int32_t phase, emap_exchange* out, int32_t* n_out) {
   ENTER(h);
   if (!out || !n_out || *n_out < 3) return fail(h, EMAP_ERR_INVALID, "emap_shard_exchange: need capacity >= 3");
-  const i64 C = h->dc.C;
-  if (phase == 1) {          // after begin: counts (CK.py:334,336) and the drift statistics (CK.py:332-333)
-    if (h->phase != 1) return fail(h, EMAP_ERR_STATE, "exchange 1 must follow emap_shard_begin");
-    out[0] = {h->sc.cnt_ai, 2 * C, 3};          // two 32-bit counters per cell: an int32 SUM keeps them apart
-    out[1] = {&h->fs->E, 2, 0};
-    *n_out = 2;
-  } else if (phase == 2) {   // after fusion: sums, counts, last-writer keys
-    if (h->phase != 2) return fail(h, EMAP_ERR_STATE, "exchange 2 must follow phase 1");
-    out[0] = {h->sc.SH, 2 * C, 0};
-    out[1] = {h->sc.cnt_fo, 2 * C, 3};
-    out[2] = {h->sc.last, C, 1};
-    *n_out = 3;
-  } else if (phase == 3) {   // after the ray-cast: decrements, counts, upper-bound keys
-    if (h->phase != 3) return fail(h, EMAP_ERR_STATE, "exchange 3 must follow phase 2");
-    if (h->dc.visibility) {
-      k_ukey_extract<<<cdiv(C, 256), 256, 0, h->stream>>>((int)C, h->sc.ukv, h->ukey_x);
-      LAUNCH_CHECK();
-      out[0] = {h->sc.DV, C, 0};
-      out[1] = {h->sc.n_ray, C, 3};
-      out[2] = {h->ukey_x, C, 2};
-      *n_out = 3;
-      h->phase = 4;
-    } else *n_out = 0;
-  } else return fail(h, EMAP_ERR_INVALID, "emap_shard_exchange: phase must be 1..3");
-  return EMAP_OK;
+  if (phase < 1 || phase > 3) return fail(h, EMAP_ERR_INVALID, "emap_shard_exchange: phase must be 1..3");
+  static const char* order[] = {"", "exchange 1 must follow emap_shard_begin", "exchange 2 must follow phase 1",
+                                "exchange 3 must follow phase 2"};
+  if (h->phase != phase) return fail(h, EMAP_ERR_STATE, order[phase]);
+  return exchange_list(h, phase, out, n_out);
 }
 
 int emap_shard_phase(emap_handle* h, int32_t phase) {
@@ -957,11 +1034,7 @@ int emap_shard_phase(emap_handle* h, int32_t phase) {
   }
   if (phase == 3) {
     if (h->phase != 3 && h->phase != 4) return fail(h, EMAP_ERR_STATE, "phase 3 must follow phase 2");
-    if (h->phase == 4) {
-      k_ukey_merge<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc.C, h->sc.ukv, h->ukey_x);
-      LAUNCH_CHECK();
-    }
-    return frame_finish(h);
+    return shard_finish(h);
   }
   return fail(h, EMAP_ERR_INVALID, "emap_shard_phase: phase must be 0..3");
 }
@@ -1021,19 +1094,10 @@ int emap_comm_init(emap_handle* h, const emap_nccl_id* id, int32_t rank, int32_t
 }
 
 static int comm_exchange(emap_handle* h, int phase) {
-  emap_exchange ex[4];
-  int32_t n = 4;
-  // (emap_shard_exchange takes the handle lock itself: this helper runs with it held, so build the list directly)
-  const i64 C = h->dc.C;
-  if (phase == 1) { ex[0] = {h->sc.cnt_ai, 2 * C, 3}; ex[1] = {&h->fs->E, 2, 0}; n = 2; }
-  else if (phase == 2) { ex[0] = {h->sc.SH, 2 * C, 0}; ex[1] = {h->sc.cnt_fo, 2 * C, 3}; ex[2] = {h->sc.last, C, 1}; n = 3; }
-  else {
-    if (!h->dc.visibility) return 0;
-    k_ukey_extract<<<cdiv(C, 256), 256, 0, h->stream>>>((int)C, h->sc.ukv, h->ukey_x);
-    LAUNCH_CHECK();
-    ex[0] = {h->sc.DV, C, 0}; ex[1] = {h->sc.n_ray, C, 3}; ex[2] = {h->ukey_x, C, 2}; n = 3;
-    h->phase = 4;
-  }
+  emap_exchange ex[3];
+  int32_t n = 0;
+  int rc = exchange_list(h, phase, ex, &n);
+  if (rc) return rc;
   NcclApi& a = nccl_api();
   for (int k = 0; k < n; k++) {
     const int dt = (ex[k].kind == 0 || ex[k].kind == 1) ? kNcclInt64 : kNcclInt32;
@@ -1064,11 +1128,7 @@ int emap_input_sensors_sharded(emap_handle* h, int32_t n_sensors, const void* co
   if ((rc = comm_exchange(h, 2))) return rc;
   if ((rc = frame_rays(h))) return rc;
   if ((rc = comm_exchange(h, 3))) return rc;
-  if (h->phase == 4) {
-    k_ukey_merge<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc.C, h->sc.ukv, h->ukey_x);
-    LAUNCH_CHECK();
-  }
-  return frame_finish(h);
+  return shard_finish(h);
 }
 
 // ---- read-backs ------------------------------------------------------------------------------
@@ -1111,7 +1171,7 @@ static int shift_map(emap_handle* h, int sx, int sy, double dz) {
   }
   k_shift<<<nb, 256, 0, h->stream>>>(h->dc, h->map, h->map_alt, sx, sy, dz);
   LAUNCH_CHECK();
-  float* t = h->map; h->map = h->map_alt; h->map_alt = t;
+  h->map.swap(h->map_alt);
   return 0;
 }
 
@@ -1198,69 +1258,15 @@ int emap_get_position(emap_handle* h, double out[3]) {
 int emap_get_map_with_name(emap_handle* h, const char* name, float* out_host, int64_t n_out) {
   ENTER(h);
   if (!name || !out_host) return fail(h, EMAP_ERR_INVALID, "null argument");
-  static const char* names[] = {"elevation", "variance", "traversability", "time", "upper_bound", "is_upper_bound",
-                                "normal_x", "normal_y", "normal_z"};
-  int kind = -1;
-  for (int i = 0; i < 9; i++) if (!strcmp(name, names[i])) kind = i;
-  if (kind < 0) { h->err = std::string("Layer ") + name + " is not in the map"; return EMAP_ERR_NOLAYER; }
-  const int Wo = h->dc.W - 2;
-  if (n_out != (int64_t)Wo * Wo) return fail(h, EMAP_ERR_INVALID, "output must hold (cell_n-2)^2 floats");
-  k_export<<<cdiv((i64)Wo * Wo, 256), 256, 0, h->stream>>>(h->dc, h->map, h->normal, h->d_export, kind, h->center[2],
-                                                              h->cfg.use_only_above_for_upper_bound, nullptr, 0);
-  LAUNCH_CHECK();
-  CK(cudaMemcpyAsync(out_host, h->d_export, sizeof(float) * Wo * Wo, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return EMAP_OK;
-}
-
-int emap_export_plane(emap_handle* h, const float* plane, int fill_nan, int add_z, float* out_host, int64_t n_out) {
-  ENTER(h);
-  if (!plane || !out_host) return fail(h, EMAP_ERR_INVALID, "null argument");
-  const int Wo = h->dc.W - 2;
-  if (n_out != (int64_t)Wo * Wo) return fail(h, EMAP_ERR_INVALID, "output must hold (cell_n-2)^2 floats");
-  k_export<<<cdiv((i64)Wo * Wo, 256), 256, 0, h->stream>>>(h->dc, h->map, h->normal, h->d_export, 9, h->center[2], 0, plane,
-                                                              (fill_nan ? 1 : 0) | (add_z ? 2 : 0));
-  LAUNCH_CHECK();
-  CK(cudaMemcpyAsync(out_host, h->d_export, sizeof(float) * Wo * Wo, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return EMAP_OK;
+  return export_layers(h, 1, &name, nullptr, nullptr, out_host, n_out);
 }
 
 // Several layers in one launch, one device-to-host copy and one synchronisation (WRAP:213-252 get_grid_map exports a list
-// of layers per call).  names[k]: a basic layer name, or NULL / a plugin layer name together with planes[k] != NULL (a (W,W)
-// device plane, exported like emap_export_plane with flags[k]: bit 0 fill_nan, bit 1 add the centre height).
+// of layers per call).
 int emap_get_layers(emap_handle* h, int32_t n, const char* const* names, const float* const* planes, const int32_t* flags,
                     float* out_host, int64_t n_out_total) {
   ENTER(h);
-  if (n < 1 || n > EXPORT_MAX_LAYERS || !out_host) return fail(h, EMAP_ERR_INVALID, "emap_get_layers: 1..24 layers, non-null output");
-  static const char* basic[] = {"elevation", "variance", "traversability", "time", "upper_bound", "is_upper_bound",
-                                "normal_x", "normal_y", "normal_z"};
-  const int Wo = h->dc.W - 2;
-  const size_t per = (size_t)Wo * Wo;
-  if (n_out_total != (int64_t)(per * n)) return fail(h, EMAP_ERR_INVALID, "output must hold n * (cell_n-2)^2 floats");
-  ExportList L;
-  memset(&L, 0, sizeof(L));
-  L.n = n;
-  for (int k = 0; k < n; k++) {
-    if (planes && planes[k]) { L.kind[k] = 9; L.plane[k] = planes[k]; L.flags[k] = flags ? flags[k] : 0; continue; }
-    int kind = -1;
-    if (names && names[k]) for (int i = 0; i < 9; i++) if (!strcmp(names[k], basic[i])) kind = i;
-    if (kind < 0) { h->err = std::string("Layer ") + (names && names[k] ? names[k] : "(null)") + " is not in the map"; return EMAP_ERR_NOLAYER; }
-    L.kind[k] = kind;
-  }
-  if (h->d_export_floats < per * n) {
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->d_export) cudaFree(h->d_export);
-    h->d_export = nullptr; h->d_export_floats = 0;
-    CK(cudaMalloc(&h->d_export, sizeof(float) * per * n));
-    h->d_export_floats = per * n;
-  }
-  k_export_multi<<<dim3(cdiv((i64)per, 256), n), 256, 0, h->stream>>>(h->dc, h->map, h->normal, h->d_export, L, h->center[2],
-                                                                       h->cfg.use_only_above_for_upper_bound);
-  LAUNCH_CHECK();
-  CK(cudaMemcpyAsync(out_host, h->d_export, sizeof(float) * per * n, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return EMAP_OK;
+  return export_layers(h, n, names, planes, flags, out_host, n_out_total);
 }
 
 int emap_layer_device_ptr(emap_handle* h, const char* name, void** ptr) {
@@ -1322,18 +1328,13 @@ int emap_erode(emap_handle* h, const float* layer, float* out, int32_t kernel_si
   ENTER(h);
   if (!layer || !out || kernel_size < 1 || kernel_size > 31 || iterations < 1 || iterations > 64)
     return fail(h, EMAP_ERR_INVALID, "emap_erode: bad argument");
-  int rc = alloc_plugin_scratch(h);
-  if (rc) return rc;
-  if (h->pl_cnt_cap < 2) {
-    if (h->pl_cnt) cudaFree(h->pl_cnt);
-    h->pl_cnt = nullptr; h->pl_cnt_cap = 0;
-    CK(cudaMalloc(&h->pl_cnt, sizeof(int) * 32));
-    h->pl_cnt_cap = 32;
-  }
+  int rc;
+  if ((rc = alloc_plugin_scratch(h)) || (rc = grow(h, h->pl_cnt, 2, 30, false))) return rc;
+  u32* const mm = (u32*)(int*)h->pl_cnt;      // min / max of the layer
   const u32 init[2] = {0xffffffffu, 0u};
-  CK(cudaMemcpyAsync(h->pl_cnt, init, sizeof(init), cudaMemcpyHostToDevice, h->stream));
+  CK(cudaMemcpyAsync(mm, init, sizeof(init), cudaMemcpyHostToDevice, h->stream));
   const int nb = cdiv(h->dc.C, 256);
-  k_layer_minmax<<<nb, 256, 0, h->stream>>>(h->dc, layer, reverse, (u32*)h->pl_cnt);
+  k_layer_minmax<<<nb, 256, 0, h->stream>>>(h->dc, layer, reverse, mm);
   LAUNCH_CHECK();
   const int ks = kernel_size + (iterations - 1) * (kernel_size - 1), anchor = (kernel_size / 2) * iterations;
   const float* src = layer;
@@ -1341,7 +1342,7 @@ int emap_erode(emap_handle* h, const float* layer, float* out, int32_t kernel_si
     CK(cudaMemcpyAsync(h->pl[0], layer, sizeof(float) * (size_t)h->dc.C, cudaMemcpyDeviceToDevice, h->stream));
     src = h->pl[0];
   }
-  k_erode<<<nb, 256, 0, h->stream>>>(h->dc, src, out, ks, anchor, reverse, (const u32*)h->pl_cnt);
+  k_erode<<<nb, 256, 0, h->stream>>>(h->dc, src, out, ks, anchor, reverse, (const u32*)mm);
   LAUNCH_CHECK();
   return EMAP_OK;
 }
@@ -1360,14 +1361,8 @@ static int minmax_filter(emap_handle* h, const float* elevation, const float* is
                          int32_t iteration_n, int32_t* iterations_run, int is_max) {
   if (!elevation || !is_valid || !out || k < 0 || k > 16 || iteration_n < 1)
     return fail(h, EMAP_ERR_INVALID, "emap_min_filter: bad argument");
-  int rc = alloc_plugin_scratch(h);
-  if (rc) return rc;
-  if (h->pl_cnt_cap < iteration_n + 1) {
-    if (h->pl_cnt) cudaFree(h->pl_cnt);
-    h->pl_cnt = nullptr; h->pl_cnt_cap = 0;
-    CK(cudaMalloc(&h->pl_cnt, sizeof(int) * (iteration_n + 1)));
-    h->pl_cnt_cap = iteration_n + 1;
-  }
+  int rc;
+  if ((rc = alloc_plugin_scratch(h)) || (rc = grow(h, h->pl_cnt, (size_t)iteration_n + 1, 0, false))) return rc;
   const size_t B = sizeof(float) * (size_t)h->dc.C;
   float *hA = h->pl[0], *mA = h->pl[1], *hB = h->pl[2], *mB = h->pl[3];
   CK(cudaMemsetAsync(h->pl_cnt, 0, sizeof(int) * (iteration_n + 1), h->stream));
@@ -1409,42 +1404,21 @@ int emap_inpaint(emap_handle* h, const float* elevation, const float* is_valid, 
   NvtxRange nv("emap:inpaint");
   if (!elevation || !is_valid || !out) return fail(h, EMAP_ERR_INVALID, "emap_inpaint: null argument");
   if (method != 0) return fail(h, EMAP_ERR_INVALID, "emap_inpaint: only method 0 (telea) is implemented; 'ns' (Navier-Stokes) is not");
-  const int W = h->dc.W, rows = W + 2, cols = W + 2;
-  const size_t N = (size_t)rows * cols, C = (size_t)W * W;
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  // f, ck, vc0, vc1 (u8 N) | img (u8 C) | T, Tc0, Tc1 (f32 N) | ord (u32 N) | heapA, heapB, children (int N) | ctl | em (u32 N)
-  const size_t need = 4 * al(N) + al(C) + 3 * al(4 * N) + al(4 * N) + 3 * al(4 * N) + al(sizeof(InpaintCtl)) + al(4 * N);
-  if (h->ip_bytes < need) {
-    CK(cudaStreamSynchronize(h->stream));
-    if (h->ip_block) cudaFree(h->ip_block);
-    h->ip_block = nullptr; h->ip_bytes = 0;
-    CK(cudaMalloc(&h->ip_block, need));
-    // once: the march loads a pixel's child fields (ck, Tc, vc) speculatively, before it knows the pixel is a child of the
-    // running round; the values of non-children are never used, but they should not be uninitialised memory
-    CK(cudaMemsetAsync(h->ip_block, 0, need, h->stream));
-    h->ip_bytes = need;
+  const int W = h->dc.W;
+  const size_t N = (size_t)(W + 2) * (W + 2), C = (size_t)W * W;
+  // zero-filled once: the march loads a pixel's child fields (ck, Tc, vc) speculatively, before it knows the pixel is a
+  // child of the running round; the values of non-children are never used, but they should not be uninitialised memory
+  int rc = grow(h, h->ip_block, inpaint_scratch(W, nullptr).bytes, 0, true);
+  if (rc) return rc;
+  if (!h->ip_grid) {
     int nb = 0;
     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_ip_march, IP_MARCH_THREADS, 0));
     if (nb < 1) return fail(h, EMAP_ERR_CUDA, "emap_inpaint: the cooperative kernel does not fit on an SM");
     h->ip_grid = h->n_sm;          // one CTA per SM: the fronts are thin, and a grid barrier costs less with fewer CTAs
   }
-  char* b = (char*)h->ip_block;
-  InpaintView v;
-  v.rows = rows; v.cols = cols;
-  v.f = (uint8_t*)b; b += al(N);
-  v.ck = (uint8_t*)b; b += al(N);
-  v.vc[0] = (uint8_t*)b; b += al(N);
-  v.vc[1] = (uint8_t*)b; b += al(N);
-  v.img = (uint8_t*)b; b += al(C);
-  v.T = (float*)b; b += al(4 * N);
-  v.Tc[0] = (float*)b; b += al(4 * N);
-  v.Tc[1] = (float*)b; b += al(4 * N);
-  v.ord = (uint32_t*)b; b += al(4 * N);
-  int* heapA = (int*)b; b += al(4 * N);
-  int* heapB = (int*)b; b += al(4 * N);
-  int* children = (int*)b; b += al(4 * N);
-  InpaintCtl* ctl = (InpaintCtl*)b; b += al(sizeof(InpaintCtl));
-  v.em = (uint32_t*)b;
+  InpaintScratch s = inpaint_scratch(W, h->ip_block);
+  InpaintView& v = s.v;
+  InpaintCtl* ctl = s.ctl;
   InpaintCtl init;
   memset(&init, 0, sizeof(init));
   init.mm[0] = 0xffffffffu; init.mm[1] = 0u;
@@ -1452,11 +1426,11 @@ int emap_inpaint(emap_handle* h, const float* elevation, const float* is_valid, 
   const int nbC = cdiv((i64)C, 256), nbN = cdiv((i64)N, 256);
   k_ip_minmax<<<nbC, 256, 0, h->stream>>>((int)C, elevation, is_valid, ctl); LAUNCH_CHECK();
   k_ip_init<<<nbN, 256, 0, h->stream>>>(W, elevation, is_valid, v, (const InpaintCtl*)ctl); LAUNCH_CHECK();
-  k_ip_band<<<nbN, 256, 0, h->stream>>>(v, heapA, ctl); LAUNCH_CHECK();
-  k_ip_band_flag<<<nbN, 256, 0, h->stream>>>(v, (const int*)heapA, ctl); LAUNCH_CHECK();
+  k_ip_band<<<nbN, 256, 0, h->stream>>>(v, s.heap[0], ctl); LAUNCH_CHECK();
+  k_ip_band_flag<<<nbN, 256, 0, h->stream>>>(v, (const int*)s.heap[0], ctl); LAUNCH_CHECK();
   {
     int cap = 4096;
-    void* args[] = {(void*)&v, (void*)&heapA, (void*)&heapB, (void*)&children, (void*)&ctl, (void*)&cap};
+    void* args[] = {(void*)&v, (void*)&s.heap[0], (void*)&s.heap[1], (void*)&s.children, (void*)&ctl, (void*)&cap};
     CK(cudaLaunchCooperativeKernel((const void*)k_ip_march, dim3(h->ip_grid), dim3(IP_MARCH_THREADS), args, 0, h->stream));
     h->launches++;
   }
@@ -1468,12 +1442,8 @@ int emap_inpaint(emap_handle* h, const float* elevation, const float* is_valid, 
 int emap_inpaint_stats(emap_handle* h, int32_t* rounds, int32_t* max_jacobi, int32_t* not_converged) {
   ENTER(h);
   if (!h->ip_block) return fail(h, EMAP_ERR_STATE, "emap_inpaint has not run");
-  const int W = h->dc.W;
-  const size_t N = (size_t)(W + 2) * (W + 2), C = (size_t)W * W;
-  auto al = [](size_t x) { return (x + 255) & ~(size_t)255; };
-  const size_t off = 4 * al(N) + al(C) + 3 * al(4 * N) + al(4 * N) + 3 * al(4 * N);
   InpaintCtl c;
-  CK(cudaMemcpyAsync(&c, (char*)h->ip_block + off, sizeof(c), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaMemcpyAsync(&c, inpaint_scratch(h->dc.W, h->ip_block).ctl, sizeof(c), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   if (rounds) *rounds = c.rounds;
   if (max_jacobi) *max_jacobi = c.max_jacobi;

@@ -1218,16 +1218,7 @@ __device__ __forceinline__ float export_value(const DevCfg& c, const float* __re
   return v;
 }
 
-__global__ void __launch_bounds__(256)
-k_export(const DevCfg c, const float* __restrict__ map, const float* __restrict__ normal, float* __restrict__ out,
-         int kind, float center_z, int only_above, const float* __restrict__ plane, int flags) {
-  const int Wo = c.W - 2;
-  const int o = blockIdx.x * blockDim.x + threadIdx.x;
-  if (o >= Wo * Wo) return;
-  out[o] = export_value(c, map, normal, o, kind, center_z, only_above, plane, flags);
-}
-
-// Several layers in one launch (WRAP:213-252 get_grid_map asks for a list of layers): blockIdx.y = layer.
+// One launch exports a list of layers (WRAP:213-252 get_grid_map asks for several): blockIdx.y = layer.
 #define EXPORT_MAX_LAYERS 24
 struct ExportList { int n; int kind[EXPORT_MAX_LAYERS]; int flags[EXPORT_MAX_LAYERS]; const float* plane[EXPORT_MAX_LAYERS]; };
 __global__ void __launch_bounds__(256)

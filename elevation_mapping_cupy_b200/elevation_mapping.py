@@ -327,60 +327,59 @@ class ElevationMap:
         self.plugin_manager.update_with_name(name, self.elevation_map, self.layer_names, self.semantic_map.semantic_map,
                                              self.semantic_map.layer_names, self.base_rotation, self.semantic_map.elements_to_shift)
 
+    def _export_source(self, name):
+        """(name, device plane, flags, tensor to keep alive) of an exportable layer, None if the map has none by that name.
+        Basic layers are exported by name; semantic layers as they are (EM.py:747-748: cropped, flipped, no NaN fill, no z
+        offset); plugin layers with their fill_nan / is_height_layer (EM.py:762-775: flags bit 0 / bit 1)."""
+        if name in EXPORT_NAMES:
+            return name, None, 0, None
+        if name in self.semantic_map.layer_names:
+            m = self.semantic_map.semantic_map[self.semantic_map.layer_names.index(name)]
+            return name, m.data_ptr(), 0, m
+        if name in self.plugin_manager.layer_names:
+            self._update_plugin(name)
+            m = self.plugin_manager.get_map_with_name(name)
+            p = self.plugin_manager.get_param_with_name(name)
+            return name, m.data_ptr(), int(bool(p.fill_nan)) | (int(bool(p.is_height_layer)) << 1), m
+        return None
+
+    def _export(self, sources, data):
+        """Writes the layers of `sources` (_export_source results) into `data`, a caller-owned (len(sources), cell_n-2,
+        cell_n-2) float32 array: one kernel, one D2H copy, one sync.  Runs under map_lock."""
+        n = len(sources)
+        n_out = (self.cell_n - 2) ** 2
+        direct = isinstance(data, np.ndarray) and data.dtype == np.float32 and data.flags.c_contiguous and data.size == n * n_out
+        buf = data if direct else (self._export_tmp if n == 1 else np.zeros((n, n_out), np.float32))
+        c_names = (C.c_char_p * n)(*[s[0].encode() for s in sources])
+        planes = (C.c_void_p * n)(*[s[1] for s in sources])
+        flags = (C.c_int32 * n)(*[s[2] for s in sources])
+        if any(s[3] is not None for s in sources):
+            self._after_framework()
+        self._check(self._L.emap_get_layers(self._h, n, c_names, planes, flags, buf.ctypes.data, n * n_out))
+        if not direct:
+            data[...] = buf.reshape(data.shape)
+
     def get_map_with_name_ref(self, name, data):
         """EM.py:720-775: write layer `name` (NaN-filled, z-shifted, cropped, flipped) into `data`,
         a caller-owned (cell_n-2, cell_n-2) float32 array."""
-        n_out = (self.cell_n - 2) ** 2
-        direct = isinstance(data, np.ndarray) and data.dtype == np.float32 and data.flags.c_contiguous and data.size == n_out
-        buf = data if direct else self._export_tmp
         with self.map_lock:
-            if name in EXPORT_NAMES:
-                self._check(self._L.emap_get_map_with_name(self._h, name.encode(), buf.ctypes.data, n_out))
-            elif name in self.semantic_map.layer_names:
-                # EM.py:747-748: semantic layers are exported as they are (cropped, flipped), no NaN fill, no z offset
-                m = self.semantic_map.semantic_map[self.semantic_map.layer_names.index(name)]
-                self._after_framework()
-                self._check(self._L.emap_export_plane(self._h, m.data_ptr(), 0, 0, buf.ctypes.data, n_out))
-            elif name in self.plugin_manager.layer_names:
-                self._update_plugin(name)
-                m = self.plugin_manager.get_map_with_name(name)
-                p = self.plugin_manager.get_param_with_name(name)
-                self._after_framework()
-                self._check(self._L.emap_export_plane(self._h, m.data_ptr(), int(p.fill_nan), int(p.is_height_layer),
-                                                      buf.ctypes.data, n_out))
-            else:
+            src = self._export_source(name)
+            if src is None:
                 print("Layer {} is not in the map".format(name))
                 return
-        if not direct:
-            data[...] = buf.reshape(data.shape)
+            self._export([src], data)
 
     def get_maps_with_names_ref(self, names, data):
         """Several layers at once (what the C++ bridge's get_grid_map does one by one, elevation_mapping_wrapper.cpp:213-252):
         `data` is a caller-owned (len(names), cell_n-2, cell_n-2) float32 array.  One kernel, one D2H copy, one sync."""
-        n = len(names)
-        n_out = (self.cell_n - 2) ** 2
-        direct = isinstance(data, np.ndarray) and data.dtype == np.float32 and data.flags.c_contiguous and data.size == n * n_out
-        buf = data if direct else np.zeros((n, self.cell_n - 2, self.cell_n - 2), np.float32)
-        c_names = (C.c_char_p * n)(); planes = (C.c_void_p * n)(); flags = (C.c_int32 * n)()
-        keep = []
         with self.map_lock:
-            for k, name in enumerate(names):
-                if name in EXPORT_NAMES:
-                    c_names[k] = name.encode(); planes[k] = None
-                elif name in self.plugin_manager.layer_names:
-                    self._update_plugin(name)
-                    m = self.plugin_manager.get_map_with_name(name)
-                    p = self.plugin_manager.get_param_with_name(name)
-                    keep.append(m)
-                    c_names[k] = name.encode(); planes[k] = m.data_ptr()
-                    flags[k] = int(bool(p.fill_nan)) | (int(bool(p.is_height_layer)) << 1)
-                else:
+            sources = []
+            for name in names:
+                src = self._export_source(name)
+                if src is None:
                     raise KeyError("Layer {} is not in the map".format(name))
-            if keep:
-                self._after_framework()
-            self._check(self._L.emap_get_layers(self._h, n, c_names, planes, flags, buf.ctypes.data, n * n_out))
-        if not direct:
-            data[...] = buf.reshape(data.shape)
+                sources.append(src)
+            self._export(sources, data)
 
     def get_state(self):
         """Host copies (map (7,W,W), normal (3,W,W)) -- tests / checkpointing."""

@@ -196,14 +196,11 @@ int emap_get_position(emap_handle* h, double out[3]);          /* EM.py:130-137 
  * border ring, flip both axes; writes (cell_n-2)^2 floats to caller memory.  Names: elevation,
  * variance, traversability, time, upper_bound, is_upper_bound, normal_x, normal_y, normal_z. ---- */
 int emap_get_map_with_name(emap_handle* h, const char* name, float* out_host, int64_t n_out);
-/* EM.py:579-596,762-775 for a plugin layer: process_map_for_publish(fill_nan, add_z) of an arbitrary
- * (W,W) fp32 device plane, then crop + flip + copy to the host. */
-int emap_export_plane(emap_handle* h, const float* plane_device, int fill_nan, int add_z, float* out_host,
-                      int64_t n_out);
 /* Batched export: what WRAP:213-252 (ElevationMappingWrapper::get_grid_map) does layer by layer -- n layers with ONE
  * kernel, one device-to-host copy, one synchronisation.  names[k] is a basic layer of emap_get_map_with_name, or
- * planes[k] a (W,W) device plane (plugin layer) exported with flags[k] (bit 0: fill_nan, bit 1: add the centre height).
- * out_host holds n consecutive (cell_n-2)^2 planes. */
+ * planes[k] a (W,W) fp32 device plane (plugin or semantic layer) exported with flags[k]: EM.py:579-596,762-775
+ * process_map_for_publish, bit 0: fill_nan, bit 1: add the centre height.  out_host holds n consecutive (cell_n-2)^2
+ * planes. */
 int emap_get_layers(emap_handle* h, int32_t n, const char* const* names, const float* const* planes_device,
                     const int32_t* flags, float* out_host, int64_t n_out_total);
 /* EM.py:807-835 get_layer / raw state access: device pointer of a (W,W) fp32 plane.  Names: the 7

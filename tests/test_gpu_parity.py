@@ -416,6 +416,9 @@ def test_semantic_point_fusion_matches_oracle(oracle_mod):
     out = np.zeros((W - 2, W - 2), np.float32)
     em.get_map_with_name_ref("person", out)
     assert np.array_equal(out, np.flip(sem_or[1][1:-1, 1:-1], (0, 1)))
+    batched = np.zeros((2, W - 2, W - 2), np.float32)
+    em.get_maps_with_names_ref(["elevation", "person"], batched)
+    assert np.array_equal(batched[1], out)
     # the layers travel with the map (EM.py:221) and clear() empties them (EM.py:126)
     em.move(np.array([0.08, -0.12, 0.0]))
     moved = em.get_layer("person").cpu().numpy()
