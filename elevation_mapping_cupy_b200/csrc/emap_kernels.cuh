@@ -580,19 +580,27 @@ k_raycast(const DevCfg c, const Pose q, const Ray* __restrict__ rays, int* __res
   const u32 s_t8_o = s_t8_a - 4u * (u32)(g.ta * RT + g.tb);      // address of the (virtual) entry of tile (0, 0)
   int n_steps_done = 0, n_visits = 0;
   // Work queue: one global counter; a warp draws RC_BATCH consecutive rays per atomic (all warps hammering ONE address
-  // serialise at ~0.8 ns per atomic, which bounded the kernel at one ray per atomic) and prefetches its next batch
-  // while it marches the current one.
+  // serialise at ~0.8 ns per atomic, which bounded the kernel at one ray per atomic) and draws its next batch when it
+  // starts the last ray of the current one, so the atomic's latency is hidden by that ray's march.  Drawing at the start
+  // of the batch instead reserved a whole batch ahead: when the queue ran dry, warps still held up to 2 batches and
+  // finished over the last ~22 us of the kernel (per-warp %globaltimer stamps: 17 % of warp time idle at the end).
   // (Measured and dropped: several queues with rays dealt round-robin -- 4 % to 20 % slower, consecutive rays share cells
   // and belong in one warp; batches of 8 -- 11 % slower at config B, the tail gets ragged; a two-level queue, CTA chunks
   // from the global counter + shared-memory atomics per warp -- 2 % slower at B, 15 % at D: the prefetched global atomic
-  // below hides its latency under the march, a shared-memory draw at the start of every batch does not.)
+  // below hides its latency under the march, a shared-memory draw at the start of every batch does not.
+  // On one H100 80GB HBM3 at 400 W, config B, raycast stage in bench.py: parent (draw at the batch start) 69.7-70.2 us,
+  // this draw 63.8-64.0 us.  Two march iterations in flight per warp (two thr gathers per lane, 58-60 registers, one
+  // 1024-thread CTA per SM) with this draw: 68.5-69.5 us at B and 325 us against 284 us at config D -- fewer warps cost
+  // more latency hiding than the second gather gives; with the draw at the batch start 73.8-74.3 us (512 x 2: 77.3-78.2).
+  // Loading a batch's four direction records at once and the next batch's after its first ray: no gain at B, and the
+  // extra registers spill at 768 x 2.  Batches of 2 with this draw: 81.5-81.8 us, the single counter saturates.)
   int* next = ray_ctl + 32;
   int pend = 0;
   if (lane == 0) pend = atomicAdd(next, RC_BATCH);
   int rbase = __shfl_sync(0xffffffffu, pend, 0);
   while (rbase < n_rays) {
-    if (lane == 0) pend = atomicAdd(next, RC_BATCH);              // next batch: latency hidden by this one's march
    for (int r = rbase; r < min(rbase + RC_BATCH, n_rays); r++) {
+    if (lane == 0 && (r + 1 == rbase + RC_BATCH || r + 1 == n_rays)) pend = atomicAdd(next, RC_BATCH);   // next batch
     const float4 rb = __ldg(reinterpret_cast<const float4*>(rays + r) + 1);
     const float rx = rb.x, ry = rb.y, rz = rb.z;
     const int n_act = (int)(__float_as_uint(rb.w) & 0xffffu), k_far = (int)(__float_as_uint(rb.w) >> 16);
