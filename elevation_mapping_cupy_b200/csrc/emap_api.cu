@@ -177,6 +177,13 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
     if (le_ != cudaSuccess) { h->err = std::string("kernel launch: ") + cudaGetErrorString(le_); return EMAP_ERR_CUDA; } \
   } while (0)
 
+// plain launch of a per-cell kernel (one thread per map cell) on the handle's stream
+#define PER_CELL(kern, ...)                                                                       \
+  do {                                                                                            \
+    kern<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(__VA_ARGS__);                                 \
+    LAUNCH_CHECK();                                                                               \
+  } while (0)
+
 inline float h16_host(float x) { return __half2float(__float2half_rn(x)); }
 
 inline int cdiv(i64 a, int b) { return (int)((a + b - 1) / b); }
@@ -333,11 +340,23 @@ int stage_mark(emap_handle* h, int k) {
   return 0;
 }
 
+// f(pts, s) for the cloud of every sensor s of the pending frame, with pts typed by pend_dtype (float or double);
+// stops at the first non-zero return
+template <typename F>
+int each_cloud(emap_handle* h, F&& f) {
+  for (int s = 0; s < (int)h->pend_pts.size(); s++) {
+    const int rc = h->pend_dtype == EMAP_F32 ? f((const float*)h->pend_pts[s], s) : f((const double*)h->pend_pts[s], s);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
 template <typename T>
-int launch_index(emap_handle* h, const Pose& q, const T* pts, i64 n, i64 stride, i64 off, int sensor) {
+int launch_index(emap_handle* h, const T* pts, int s) {
+  const i64 n = h->pend_n[s], off = h->offs[s];
   if (n <= 0) return 0;
-  PDL(k_index_error<T>, cdiv(n, 256), 256, 0, h->dc, q, pts, n, stride, h->xyzv + off, h->pidx + off, (const float*)h->map,
-      h->sc, h->fs, h->rays + off, h->ray_ctl + RC_CTL * sensor, (const unsigned short*)h->step_cnt);
+  PDL(k_index_error<T>, cdiv(n, 256), 256, 0, h->dc, h->poses[s], pts, n, h->pend_stride, h->xyzv + off, h->pidx + off,
+      (const float*)h->map, h->sc, h->fs, h->rays + off, h->ray_ctl + RC_CTL * s, (const unsigned short*)h->step_cnt);
   LAUNCH_CHECK();
   return 0;
 }
@@ -421,13 +440,7 @@ int frame_begin(emap_handle* h, int32_t n_sensors, const void* const* points, co
 // index + error-count pass of every sensor (CK.py:280-345)
 int frame_index(emap_handle* h) {
   NvtxRange nv("emap:index+error");
-  const int n_sensors = (int)h->pend_pts.size();
-  for (int s = 0; s < n_sensors; s++) {
-    int rc = h->pend_dtype == EMAP_F32
-                 ? launch_index<float>(h, h->poses[s], (const float*)h->pend_pts[s], h->pend_n[s], h->pend_stride, h->offs[s], s)
-                 : launch_index<double>(h, h->poses[s], (const double*)h->pend_pts[s], h->pend_n[s], h->pend_stride, h->offs[s], s);
-    if (rc) return rc;
-  }
+  if (int rc = each_cloud(h, [h](auto pts, int s) { return launch_index(h, pts, s); })) return rc;
   if (h->pend_host) CK(cudaEventRecord(h->in_free[h->in_sel ^ 1], h->stream));
   if (h->zero_copy_pending) CK(cudaEventRecord(h->copy_done, h->stream));      // caller's buffer is free after this point
   if (stage_mark(h, 1)) return EMAP_ERR_CUDA;
@@ -468,9 +481,11 @@ int frame_fuse(emap_handle* h) {
 // semantic point-channel fusion of the frame (semantic_map.py:223-259 after EM.py:369-371): needs the fused counts of
 // k_fuse and must run before k_finalize re-zeroes them
 template <typename T>
-int launch_sem_sum(emap_handle* h, const T* pts, i64 n, i64 stride, i64 off) {
+int launch_sem_sum(emap_handle* h, const T* pts, int s) {
+  const i64 n = h->pend_n[s];
   if (n <= 0) return 0;
-  k_sem_sum<T><<<cdiv(n, 256), 256, 0, h->stream>>>(h->dc, h->sem, pts, n, stride, (const int*)(h->pidx + off), h->sem_fsum, h->sem_csum);
+  k_sem_sum<T><<<cdiv(n, 256), 256, 0, h->stream>>>(h->dc, h->sem, pts, n, h->pend_stride, (const int*)(h->pidx + h->offs[s]),
+                                                     h->sem_fsum, h->sem_csum);
   LAUNCH_CHECK();
   return 0;
 }
@@ -478,17 +493,11 @@ int launch_sem_sum(emap_handle* h, const T* pts, i64 n, i64 stride, i64 off) {
 int frame_semantic(emap_handle* h) {
   if (h->sem.n_ch <= 0 || !h->sem_map) return 0;
   NvtxRange nv("emap:semantic");
-  for (size_t s = 0; s < h->pend_pts.size(); s++) {
-    int rc = h->pend_dtype == EMAP_F32
-                 ? launch_sem_sum<float>(h, (const float*)h->pend_pts[s], h->pend_n[s], h->pend_stride, h->offs[s])
-                 : launch_sem_sum<double>(h, (const double*)h->pend_pts[s], h->pend_n[s], h->pend_stride, h->offs[s]);
-    if (rc) return rc;
-  }
+  if (int rc = each_cloud(h, [h](auto pts, int s) { return launch_sem_sum(h, pts, s); })) return rc;
   // the cloud (staging buffer or the caller's pinned memory) is free only now
   if (h->pend_host) CK(cudaEventRecord(h->in_free[h->in_sel ^ 1], h->stream));
   if (h->zero_copy_pending) CK(cudaEventRecord(h->copy_done, h->stream));
-  k_sem_apply<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc, h->sem, (const u64*)h->sc.cnt_fo, h->sem_fsum, h->sem_csum, h->sem_map);
-  LAUNCH_CHECK();
+  PER_CELL(k_sem_apply, h->dc, h->sem, (const u64*)h->sc.cnt_fo, h->sem_fsum, h->sem_csum, h->sem_map);
   return 0;
 }
 
@@ -650,6 +659,32 @@ int alloc_plugin_scratch(emap_handle* h) {
     if (rc) return rc;
   }
   return 0;
+}
+
+// emap_min_filter / emap_max_filter: `iteration_n` Jacobi passes ping-ponging between two plane pairs, then the select
+template <bool MAX>
+int minmax_filter(emap_handle* h, const float* elevation, const float* is_valid, float* out, int32_t k, int32_t iteration_n,
+                  int32_t* iterations_run) {
+  if (!elevation || !is_valid || !out || k < 0 || k > 16 || iteration_n < 1)
+    return fail(h, EMAP_ERR_INVALID, "emap_min_filter: bad argument");
+  int rc;
+  if ((rc = alloc_plugin_scratch(h)) || (rc = grow(h, h->pl_cnt, (size_t)iteration_n + 1, 0, false))) return rc;
+  const size_t B = sizeof(float) * (size_t)h->dc.C;
+  float *hA = h->pl[0], *mA = h->pl[1], *hB = h->pl[2], *mB = h->pl[3];
+  CK(cudaMemsetAsync(h->pl_cnt, 0, sizeof(int) * (iteration_n + 1), h->stream));
+  CK(cudaMemcpyAsync(hA, elevation, B, cudaMemcpyDeviceToDevice, h->stream));      // min_filter.py:105-106
+  CK(cudaMemcpyAsync(mA, is_valid, B, cudaMemcpyDeviceToDevice, h->stream));
+  for (int it = 0; it < iteration_n; it++) {
+    const bool even = (it & 1) == 0;
+    PER_CELL(k_fill_filter_iter<MAX>, h->dc, k, is_valid, even ? hA : hB, even ? mA : mB, even ? hB : hA, even ? mB : mA,
+             h->pl_cnt, it);
+  }
+  PER_CELL(k_min_filter_final, h->dc, hA, mA, hB, mB, h->pl_cnt, iteration_n, out, h->pl_cnt + iteration_n);
+  if (iterations_run) {
+    CK(cudaMemcpyAsync(iterations_run, h->pl_cnt + iteration_n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+  }
+  return EMAP_OK;
 }
 
 // upper-bound keys of a sharded frame (NCCL mode): u32 keys <-> the s32 order an int32 MIN all-reduce needs
@@ -1163,14 +1198,11 @@ int emap_set_ray_counting(emap_handle* h, int enable) { ENTER(h); h->count_rays 
 
 // ---- pose / time -----------------------------------------------------------------------------
 static int shift_map(emap_handle* h, int sx, int sy, double dz) {
-  const int nb = cdiv(h->dc.C, 256);
   if (sx == 0 && sy == 0) {                                    // EM.py:208-209 early return, then shift_map_z
-    k_shift_z<<<nb, 256, 0, h->stream>>>(h->dc, h->map, dz);
-    LAUNCH_CHECK();
+    PER_CELL(k_shift_z, h->dc, h->map, dz);
     return 0;
   }
-  k_shift<<<nb, 256, 0, h->stream>>>(h->dc, h->map, h->map_alt, sx, sy, dz);
-  LAUNCH_CHECK();
+  PER_CELL(k_shift, h->dc, h->map, h->map_alt, sx, sy, dz);
   h->map.swap(h->map_alt);
   return 0;
 }
@@ -1200,30 +1232,26 @@ int emap_move(emap_handle* h, const double d[3]) {
 
 int emap_clear(emap_handle* h) {
   ENTER(h);
-  k_clear<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc, h->map);
-  LAUNCH_CHECK();
+  PER_CELL(k_clear, h->dc, h->map);
   CK(cudaMemsetAsync(&h->fs->mean_error, 0, 2 * sizeof(float), h->stream));     // EM.py:127-128
   return EMAP_OK;
 }
 
 int emap_update_variance(emap_handle* h) {
   ENTER(h);
-  k_update_variance<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc, h->map);
-  LAUNCH_CHECK();
+  PER_CELL(k_update_variance, h->dc, h->map);
   return EMAP_OK;
 }
 
 int emap_update_time(emap_handle* h) {
   ENTER(h);
-  k_update_time<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc, h->map);
-  LAUNCH_CHECK();
+  PER_CELL(k_update_time, h->dc, h->map);
   return EMAP_OK;
 }
 
 int emap_update_normal(emap_handle* h, const float* dilated) {
   ENTER(h);
-  k_normal<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc, dilated ? dilated : h->trav_input, h->map + 2 * (size_t)h->dc.C, h->normal);
-  LAUNCH_CHECK();
+  PER_CELL(k_normal, h->dc, dilated ? dilated : h->trav_input, h->map + 2 * (size_t)h->dc.C, h->normal);
   return EMAP_OK;
 }
 
@@ -1236,14 +1264,11 @@ int emap_initialize_map_finish(emap_handle* h, int32_t dilation_size, int32_t it
   int rc = alloc_plugin_scratch(h);
   if (rc) return rc;
   const size_t B = sizeof(float) * (size_t)h->dc.C;
-  const int nb = cdiv(h->dc.C, 256);
   const int passes = dilation_size > 0 ? iterations : 0;
   for (int it = 0; it < std::max(passes, 1); it++) {
     CK(cudaMemcpyAsync(h->pl[0], h->map, B, cudaMemcpyDeviceToDevice, h->stream));
     CK(cudaMemcpyAsync(h->pl[1], h->map + 2 * (size_t)h->dc.C, B, cudaMemcpyDeviceToDevice, h->stream));
-    k_init_dilate<<<nb, 256, 0, h->stream>>>(h->dc, h->pl[0], h->pl[1], h->map, passes ? dilation_size : 0,
-                                              it == std::max(passes, 1) - 1);
-    LAUNCH_CHECK();
+    PER_CELL(k_init_dilate, h->dc, h->pl[0], h->pl[1], h->map, passes ? dilation_size : 0, it == std::max(passes, 1) - 1);
   }
   return EMAP_OK;
 }
@@ -1309,19 +1334,16 @@ int emap_set_state(emap_handle* h, const float* map_host, const float* normal_ho
 }
 
 // ---- plugins ---------------------------------------------------------------------------------
-static int minmax_filter(emap_handle* h, const float* elevation, const float* is_valid, float* out, int32_t k,
-                         int32_t iteration_n, int32_t* iterations_run, int is_max);
-
 int emap_min_filter(emap_handle* h, const float* elevation, const float* is_valid, float* out, int32_t k, int32_t iteration_n,
                     int32_t* iterations_run) {
   ENTER(h);
-  return minmax_filter(h, elevation, is_valid, out, k, iteration_n, iterations_run, 0);
+  return minmax_filter<false>(h, elevation, is_valid, out, k, iteration_n, iterations_run);
 }
 
 int emap_max_filter(emap_handle* h, const float* elevation, const float* is_valid, float* out, int32_t k, int32_t iteration_n,
                     int32_t* iterations_run) {
   ENTER(h);
-  return minmax_filter(h, elevation, is_valid, out, k, iteration_n, iterations_run, 1);
+  return minmax_filter<true>(h, elevation, is_valid, out, k, iteration_n, iterations_run);
 }
 
 int emap_erode(emap_handle* h, const float* layer, float* out, int32_t kernel_size, int32_t iterations, int32_t reverse) {
@@ -1333,17 +1355,14 @@ int emap_erode(emap_handle* h, const float* layer, float* out, int32_t kernel_si
   u32* const mm = (u32*)(int*)h->pl_cnt;      // min / max of the layer
   const u32 init[2] = {0xffffffffu, 0u};
   CK(cudaMemcpyAsync(mm, init, sizeof(init), cudaMemcpyHostToDevice, h->stream));
-  const int nb = cdiv(h->dc.C, 256);
-  k_layer_minmax<<<nb, 256, 0, h->stream>>>(h->dc, layer, reverse, mm);
-  LAUNCH_CHECK();
+  PER_CELL(k_layer_minmax, h->dc, layer, reverse, mm);
   const int ks = kernel_size + (iterations - 1) * (kernel_size - 1), anchor = (kernel_size / 2) * iterations;
   const float* src = layer;
   if (layer == out) {        // in-place call: erode from a copy
     CK(cudaMemcpyAsync(h->pl[0], layer, sizeof(float) * (size_t)h->dc.C, cudaMemcpyDeviceToDevice, h->stream));
     src = h->pl[0];
   }
-  k_erode<<<nb, 256, 0, h->stream>>>(h->dc, src, out, ks, anchor, reverse, (const u32*)mm);
-  LAUNCH_CHECK();
+  PER_CELL(k_erode, h->dc, src, out, ks, anchor, reverse, (const u32*)mm);
   return EMAP_OK;
 }
 
@@ -1351,36 +1370,7 @@ int emap_robot_centric_elevation(emap_handle* h, const float* elevation, const f
                                  double resolution, double threshold, int32_t use_threshold) {
   ENTER(h);
   if (!elevation || !is_valid || !R || !out) return fail(h, EMAP_ERR_INVALID, "null argument");
-  k_robot_centric<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc, elevation, is_valid, out, R[6], R[7], R[8], resolution,
-                                                              threshold, use_threshold);
-  LAUNCH_CHECK();
-  return EMAP_OK;
-}
-
-static int minmax_filter(emap_handle* h, const float* elevation, const float* is_valid, float* out, int32_t k,
-                         int32_t iteration_n, int32_t* iterations_run, int is_max) {
-  if (!elevation || !is_valid || !out || k < 0 || k > 16 || iteration_n < 1)
-    return fail(h, EMAP_ERR_INVALID, "emap_min_filter: bad argument");
-  int rc;
-  if ((rc = alloc_plugin_scratch(h)) || (rc = grow(h, h->pl_cnt, (size_t)iteration_n + 1, 0, false))) return rc;
-  const size_t B = sizeof(float) * (size_t)h->dc.C;
-  float *hA = h->pl[0], *mA = h->pl[1], *hB = h->pl[2], *mB = h->pl[3];
-  CK(cudaMemsetAsync(h->pl_cnt, 0, sizeof(int) * (iteration_n + 1), h->stream));
-  CK(cudaMemcpyAsync(hA, elevation, B, cudaMemcpyDeviceToDevice, h->stream));      // min_filter.py:105-106
-  CK(cudaMemcpyAsync(mA, is_valid, B, cudaMemcpyDeviceToDevice, h->stream));
-  const int nb = cdiv(h->dc.C, 256);
-  for (int it = 0; it < iteration_n; it++) {
-    const bool even = (it & 1) == 0;
-    k_min_filter_iter<<<nb, 256, 0, h->stream>>>(h->dc, k, is_valid, even ? hA : hB, even ? mA : mB, even ? hB : hA,
-                                                  even ? mB : mA, h->pl_cnt, it, is_max);
-    LAUNCH_CHECK();
-  }
-  k_min_filter_final<<<nb, 256, 0, h->stream>>>(h->dc, hA, mA, hB, mB, h->pl_cnt, iteration_n, out, h->pl_cnt + iteration_n);
-  LAUNCH_CHECK();
-  if (iterations_run) {
-    CK(cudaMemcpyAsync(iterations_run, h->pl_cnt + iteration_n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-  }
+  PER_CELL(k_robot_centric, h->dc, elevation, is_valid, out, R[6], R[7], R[8], resolution, threshold, use_threshold);
   return EMAP_OK;
 }
 
@@ -1389,11 +1379,10 @@ int emap_smooth_filter(emap_handle* h, const float* in, float* out) {
   if (!in || !out) return fail(h, EMAP_ERR_INVALID, "null argument");
   int rc = alloc_plugin_scratch(h);
   if (rc) return rc;
-  const int nb = cdiv(h->dc.C, 256);
-  k_box3<<<nb, 256, 0, h->stream>>>(h->dc, in, h->pl[0], 0); LAUNCH_CHECK();
-  k_box3<<<nb, 256, 0, h->stream>>>(h->dc, h->pl[0], h->pl[1], 1); LAUNCH_CHECK();
-  k_box3<<<nb, 256, 0, h->stream>>>(h->dc, h->pl[1], h->pl[0], 0); LAUNCH_CHECK();
-  k_box3<<<nb, 256, 0, h->stream>>>(h->dc, h->pl[0], out, 1); LAUNCH_CHECK();
+  PER_CELL(k_box3, h->dc, in, h->pl[0], 0);
+  PER_CELL(k_box3, h->dc, h->pl[0], h->pl[1], 1);
+  PER_CELL(k_box3, h->dc, h->pl[1], h->pl[0], 0);
+  PER_CELL(k_box3, h->dc, h->pl[0], out, 1);
   return EMAP_OK;
 }
 
@@ -1423,8 +1412,8 @@ int emap_inpaint(emap_handle* h, const float* elevation, const float* is_valid, 
   memset(&init, 0, sizeof(init));
   init.mm[0] = 0xffffffffu; init.mm[1] = 0u;
   CK(cudaMemcpyAsync(ctl, &init, sizeof(init), cudaMemcpyHostToDevice, h->stream));     // pageable: staged before return
-  const int nbC = cdiv((i64)C, 256), nbN = cdiv((i64)N, 256);
-  k_ip_minmax<<<nbC, 256, 0, h->stream>>>((int)C, elevation, is_valid, ctl); LAUNCH_CHECK();
+  const int nbN = cdiv((i64)N, 256);
+  PER_CELL(k_ip_minmax, (int)C, elevation, is_valid, ctl);
   k_ip_init<<<nbN, 256, 0, h->stream>>>(W, elevation, is_valid, v, (const InpaintCtl*)ctl); LAUNCH_CHECK();
   k_ip_band<<<nbN, 256, 0, h->stream>>>(v, s.heap[0], ctl); LAUNCH_CHECK();
   k_ip_band_flag<<<nbN, 256, 0, h->stream>>>(v, (const int*)s.heap[0], ctl); LAUNCH_CHECK();
@@ -1434,7 +1423,7 @@ int emap_inpaint(emap_handle* h, const float* elevation, const float* is_valid, 
     CK(cudaLaunchCooperativeKernel((const void*)k_ip_march, dim3(h->ip_grid), dim3(IP_MARCH_THREADS), args, 0, h->stream));
     h->launches++;
   }
-  k_ip_finish<<<nbC, 256, 0, h->stream>>>((int)C, (const uint8_t*)v.img, elevation, out, (const InpaintCtl*)ctl); LAUNCH_CHECK();
+  PER_CELL(k_ip_finish, (int)C, (const uint8_t*)v.img, elevation, out, (const InpaintCtl*)ctl);
   return EMAP_OK;
 }
 

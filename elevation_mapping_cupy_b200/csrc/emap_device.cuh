@@ -146,6 +146,30 @@ __device__ __forceinline__ bool cell_inside(int W, int ix, int iy) {
   return ix != 0 && ix != W - 1 && iy != 0 && iy != W - 1;
 }
 
+// CK.py:403-410: the (2k+1)^2 window of cell i, dy then dx ascending.  The neighbour (dy, dx) is the FLAT index
+// idx = i + W*dy + dx (a column offset past the map's edge wraps into the adjacent row); it counts only inside [0, C)
+// and off the border ring.  f(idx, dy, dx) runs for each neighbour that counts.
+template <typename F>
+__device__ __forceinline__ void for_window(int W, int C, int i, int k, F&& f) {
+  for (int dy = -k; dy <= k; dy++)
+    for (int dx = -k; dx <= k; dx++) {
+      const int idx = i + W * dy + dx;
+      if (idx < 0 || idx >= C) continue;
+      const int ix = idx / W, iy = idx - ix * W;
+      if (ix <= 0 || ix >= W - 1 || iy <= 0 || iy >= W - 1) continue;
+      f(idx, dy, dx);
+    }
+}
+
+// CK.py:486-501: unit normal of a cell from its height h and the heights of its neighbours in the next column (h_col)
+// and the next row (h_row)
+__device__ __forceinline__ float3 surface_normal(float h, float h_col, float h_row, float res) {
+  const float dzdx = __fsub_rn(h_col, h), dzdy = __fsub_rn(h_row, h);
+  const float nx = __fdiv_rn(-dzdy, res), ny = __fdiv_rn(-dzdx, res);
+  const float nn = __fsqrt_rn(__fadd_rn(__fmaf_rn(nx, nx, __fmul_rn(ny, ny)), 1.0f));
+  return make_float3(__fdiv_rn(nx, nn), __fdiv_rn(ny, nn), __fdiv_rn(1.0f, nn));
+}
+
 // CK.py:68-81 is_valid; X,Y,Z are the fp16-rounded transformed point.
 __device__ __forceinline__ bool point_valid(const DevCfg& c, const Pose& q, float X, float Y, float Z) {
   float dx = X - q.t16[0], dy = Y - q.t16[1], dz = Z - q.t16[2];

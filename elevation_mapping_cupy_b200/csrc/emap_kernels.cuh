@@ -69,6 +69,31 @@ __device__ __forceinline__ void red_min(u32* p, u32 v, i64 mc) {
 __device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
+// Bulk copies (TMA) into shared memory that complete on one mbarrier: one thread arms the barrier with the bytes the
+// copies will deliver (bar_expect) and issues them; the CTA waits for the barrier's phase (bar_wait) only after every
+// thread can see the initialised barrier (a __syncthreads in between).
+__device__ __forceinline__ void bar_expect(u32 bar, u32 bytes) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
+  asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void bar_wait(u32 bar, u32 parity) {
+  u32 ok = 0;
+  while (!ok)
+    asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
+                 : "=r"(ok) : "r"(bar), "r"(parity) : "memory");
+}
+// `bytes` (a multiple of 16) from global `src` to shared `dst` (both 16-byte aligned)
+__device__ __forceinline__ void bulk_copy(u32 dst, const void* src, u32 bytes, u32 bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+// the box of tensor map `tm` at element coordinates (x, y, z) to shared `dst`; elements outside the tensor arrive as zeros
+__device__ __forceinline__ void tensor_copy_3d(u32 dst, const CUtensorMap* tm, int x, int y, int z, u32 bar) {
+  asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+               ::"r"(dst), "l"(tm), "r"(x), "r"(y), "r"(z), "r"(bar) : "memory");
+}
+
 #ifndef FUSE_AGG
 #define FUSE_AGG 1                // single-GPU frames: warp-aggregate the per-cell atomics of a warp that has runs (0: never)
 #endif
@@ -540,13 +565,9 @@ k_raycast(const DevCfg c, const Pose q, const Ray* __restrict__ rays, int* __res
   pdl_trigger();
   // static tables (written once at emap_create): staged before the dependency wait, under the previous kernel's tail
   if (tid == 0) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(sbar));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sbar), "r"(2 * P2) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(s_lut), "l"(lut), "r"(P2), "r"(sbar) : "memory");
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(s_lut + 65536u), "l"(lut + 32768), "r"(P2), "r"(sbar) : "memory");
+    bar_expect(sbar, 2 * P2);
+    bulk_copy(s_lut, lut, P2, sbar);
+    bulk_copy(s_lut + 65536u, lut + 32768, P2, sbar);
   }
   for (int k = tid; k < n_tab; k += RC_THREADS) s_steps[k] = steps_tab[k];
   pdl_wait();
@@ -564,12 +585,7 @@ k_raycast(const DevCfg c, const Pose q, const Ray* __restrict__ rays, int* __res
     s_t16[k] = m;
   }
   __syncthreads();
-  {
-    u32 ok = 0;
-    while (!ok)
-      asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                   : "=r"(ok) : "r"(sbar), "r"(0) : "memory");
-  }
+  bar_wait(sbar, 0);
   const int n_rays = ray_ctl[0];
   const int W = c.W, C = c.C;
   const float tx = q.t[0], ty = q.t[1], tz = q.t[2];
@@ -915,21 +931,14 @@ k_post(const DevCfg c, float* __restrict__ map, float* __restrict__ trav_input, 
   if (bulk) {
     const u32 sbar = (u32)__cvta_generic_to_shared(s_bar);
     if (tid == 0) {
-      asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(sbar));
-      asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-      asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(sbar), "r"(3 * A * B * 4) : "memory");
+      bar_expect(sbar, 3 * A * B * 4);
 #pragma unroll
-      for (int pl = 0; pl < 3; pl++) {
-        const u32 dst = (u32)__cvta_generic_to_shared(pl == 0 ? s_up : pl == 1 ? s_mask : s_iu);
-        asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-                     ::"r"(dst), "l"(&tm), "r"(c0 - HLX), "r"(r0 - HL), "r"(pl == 0 ? 5 : pl == 1 ? 2 : 6), "r"(sbar) : "memory");
-      }
+      for (int pl = 0; pl < 3; pl++)
+        tensor_copy_3d((u32)__cvta_generic_to_shared(pl == 0 ? s_up : pl == 1 ? s_mask : s_iu), &tm, c0 - HLX, r0 - HL,
+                       pl == 0 ? 5 : pl == 1 ? 2 : 6, sbar);
     }
     __syncthreads();                             // the barrier is initialised before anyone polls it
-    u32 ok = 0;
-    while (!ok)
-      asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }"
-                   : "=r"(ok) : "r"(sbar), "r"(0) : "memory");
+    bar_wait(sbar, 0);
   }
   // raw mask + per staged row one 64-bit word whose bit b says "cell (a,b) may be SELECTED as a neighbour"
   // (CK.py:432-434: is_inside && mask > 0.5), built with warp ballots (B <= 64)
@@ -1032,21 +1041,25 @@ k_post(const DevCfg c, float* __restrict__ map, float* __restrict__ trav_input, 
       const int i = r * W + cc;
       float out = up[i];
       if (__fadd_rn(valid[i], isup[i]) < 0.5f) {
+        // row and column of the flat index i + W*dy + dx of for_window: one wrap step finds them, as |dx| <= K <= 8 <= W
+        auto wrap = [&](int dy, int dx) {
+          int rr = r + dy, c2 = cc + dx;
+          if (c2 < 0) { c2 += W; rr -= 1; } else if (c2 >= W) { c2 -= W; rr += 1; }
+          return make_int2(rr, c2);
+        };
         u32 best = 0xffffffffu;
         for (int cand = lane; cand < side * side; cand += 32) {
           const int dy = cand / side - K, dx = cand - (dy + K) * side - K;
-          int rr = r + dy, c2 = cc + dx;
-          if (c2 < 0) { c2 += W; rr -= 1; } else if (c2 >= W) { c2 -= W; rr += 1; }   // idx / W, idx % W of CK.py:409-410
-          if (rr <= 0 || rr >= W - 1 || c2 <= 0 || c2 >= W - 1) continue;
-          const int idx = rr * W + c2;
+          const int2 n = wrap(dy, dx);
+          if (n.x <= 0 || n.x >= W - 1 || n.y <= 0 || n.y >= W - 1) continue;
+          const int idx = n.x * W + n.y;
           if (__fadd_rn(valid[idx], isup[idx]) > 0.5f) best = min(best, (u32)((dx + dy + 2 * K) << 8 | (dy + K)));
         }
         best = __reduce_min_sync(0xffffffffu, best);
         if (best != 0xffffffffu) {
           const int dy = (int)(best & 255u) - K, dx = (int)(best >> 8) - 2 * K - dy;
-          int rr = r + dy, c2 = cc + dx;
-          if (c2 < 0) { c2 += W; rr -= 1; } else if (c2 >= W) { c2 -= W; rr += 1; }
-          out = up[rr * W + c2];
+          const int2 n = wrap(dy, dx);
+          out = up[n.x * W + n.y];
         }
       }
       if (lane == 0) s_dil[e] = out;
@@ -1085,14 +1098,9 @@ k_post(const DevCfg c, float* __restrict__ map, float* __restrict__ trav_input, 
       map[3 * C + gi] = expf(-acc);
     }
     // normals CK.py:486-501 (normal_map is cleared first, EM.py:571)
-    float n0 = 0.f, n1 = 0.f, n2 = 0.f;
-    if (__ldg(valid + gi) > 0.5f && r >= 1 && r <= W - 3 && cc >= 1 && cc <= W - 3) {
-      const float dzdx = __fsub_rn(d[1], h), dzdy = __fsub_rn(d[DB], h);
-      const float nx = __fdiv_rn(-dzdy, c.res_f), ny = __fdiv_rn(-dzdx, c.res_f);
-      const float nn = __fsqrt_rn(__fadd_rn(__fmaf_rn(nx, nx, __fmul_rn(ny, ny)), 1.0f));
-      n0 = __fdiv_rn(nx, nn); n1 = __fdiv_rn(ny, nn); n2 = __fdiv_rn(1.0f, nn);
-    }
-    normal[gi] = n0; normal[C + gi] = n1; normal[2 * C + gi] = n2;
+    float3 n = make_float3(0.f, 0.f, 0.f);
+    if (__ldg(valid + gi) > 0.5f && r >= 1 && r <= W - 3 && cc >= 1 && cc <= W - 3) n = surface_normal(h, d[1], d[DB], c.res_f);
+    normal[gi] = n.x; normal[C + gi] = n.y; normal[2 * C + gi] = n.z;
   }
 }
 
@@ -1102,15 +1110,9 @@ k_normal(const DevCfg c, const float* __restrict__ dil, const float* __restrict_
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= c.C) return;
   const int W = c.W, r = i / W, cc = i - r * W;
-  float n0 = 0.f, n1 = 0.f, n2 = 0.f;
-  if (valid[i] > 0.5f && r >= 1 && r <= W - 3 && cc >= 1 && cc <= W - 3) {
-    const float h = dil[i];
-    const float dzdx = __fsub_rn(dil[i + 1], h), dzdy = __fsub_rn(dil[i + W], h);
-    const float nx = __fdiv_rn(-dzdy, c.res_f), ny = __fdiv_rn(-dzdx, c.res_f);
-    const float nn = __fsqrt_rn(__fadd_rn(__fmaf_rn(nx, nx, __fmul_rn(ny, ny)), 1.0f));
-    n0 = __fdiv_rn(nx, nn); n1 = __fdiv_rn(ny, nn); n2 = __fdiv_rn(1.0f, nn);
-  }
-  normal[i] = n0; normal[c.C + i] = n1; normal[2 * c.C + i] = n2;
+  float3 n = make_float3(0.f, 0.f, 0.f);
+  if (valid[i] > 0.5f && r >= 1 && r <= W - 3 && cc >= 1 && cc <= W - 3) n = surface_normal(dil[i], dil[i + 1], dil[i + W], c.res_f);
+  normal[i] = n.x; normal[c.C + i] = n.y; normal[2 * c.C + i] = n.z;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1178,14 +1180,9 @@ k_init_dilate(const DevCfg c, const float* __restrict__ src_h, const float* __re
   float h = src_h[i], valid = src_valid[i];
   if (valid < 0.5f) {
     float distance = 100.f, near_value = 0.f;
-    for (int dy = -k; dy <= k; dy++)
-      for (int dx = -k; dx <= k; dx++) {
-        const int idx = i + W * dy + dx;                          // flat index, as the reference (no row wrap handling)
-        if (idx < 0 || idx >= C) continue;
-        const int ix = idx / W, iy = idx - ix * W;
-        if (ix <= 0 || ix >= W - 1 || iy <= 0 || iy >= W - 1) continue;
-        if (src_valid[idx] > 0.5f && (float)(dx + dy) < distance) { distance = (float)(dx + dy); near_value = src_h[idx]; }
-      }
+    for_window(W, C, i, k, [&](int idx, int dy, int dx) {
+      if ((src_valid[idx] > 0.5f) & ((float)(dx + dy) < distance)) { distance = (float)(dx + dy); near_value = src_h[idx]; }
+    });
     if (distance < 100.f) { h = near_value; valid = 1.0f; }
   }
   map[i] = h; map[2 * C + i] = valid;
@@ -1244,44 +1241,26 @@ k_export_multi(const DevCfg c, const float* __restrict__ map, const float* __res
 // plugins/min_filter.py:57-82 with Jacobi order (reads iteration k-1, writes iteration k).
 // `unfilled[it]` counts cells whose mask is still <= 0.5 after iteration it; an iteration whose
 // predecessor left none is skipped on the device (min_filter.py:115 breaks on the host instead).
-// is_max = 1: plugins/max_filter.py:68-88 -- same stencil with max, and the fill test looks at the CURRENT mask
+// MAX: plugins/max_filter.py:68-88 -- same stencil with max, and the fill test looks at the CURRENT mask
 // (max_filter.py:102-108 passes copies of the running arrays), where min_filter keeps testing the ORIGINAL one.
+template <bool MAX>
 __global__ void __launch_bounds__(256)
-k_min_filter_iter(const DevCfg c, int k, const float* __restrict__ mask0, const float* __restrict__ in_h,
-                  const float* __restrict__ in_m, float* __restrict__ out_h, float* __restrict__ out_m,
-                  int* __restrict__ unfilled, int it, int is_max) {
+k_fill_filter_iter(const DevCfg c, int k, const float* __restrict__ mask0, const float* __restrict__ in_h,
+                   const float* __restrict__ in_m, float* __restrict__ out_h, float* __restrict__ out_m,
+                   int* __restrict__ unfilled, int it) {
   if (it > 0 && unfilled[it - 1] == 0) { if (blockIdx.x == 0 && threadIdx.x == 0) unfilled[it] = 0; return; }
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   int miss = 0;
   if (i < c.C) {
-    const int W = c.W;
     float h = in_h[i], m = in_m[i];
-    if (is_max) {
-      if (m < 0.5f) {
-        float mv = -1000000.0f;
-        for (int dy = -k; dy <= k; dy++)
-          for (int dx = -k; dx <= k; dx++) {
-            const int idx = i + W * dy + dx;
-            if (idx < 0 || idx >= c.C) continue;
-            const int ix = idx / W, iy = idx - ix * W;
-            if (ix <= 0 || ix >= W - 1 || iy <= 0 || iy >= W - 1) continue;
-            const float val = in_h[idx];
-            if (in_m[idx] > 0.5f && val > mv) mv = val;
-          }
-        if (mv > -1000000.f + 1.f) { h = mv; m = 0.6f; }
-      }
-    } else if (mask0[i] < 0.5f) {
-      float mv = 1000000.0f;
-      for (int dy = -k; dy <= k; dy++)
-        for (int dx = -k; dx <= k; dx++) {
-          const int idx = i + W * dy + dx;
-          if (idx < 0 || idx >= c.C) continue;
-          const int ix = idx / W, iy = idx - ix * W;
-          if (ix <= 0 || ix >= W - 1 || iy <= 0 || iy >= W - 1) continue;
-          const float val = in_h[idx];
-          if (in_m[idx] > 0.5f && val < mv) mv = val;
-        }
-      if (mv < 1000000.f - 1.f) { h = mv; m = 0.6f; }
+    if ((MAX ? m : mask0[i]) < 0.5f) {
+      const float none = MAX ? -1000000.0f : 1000000.0f;
+      float mv = none;
+      for_window(c.W, c.C, i, k, [&](int idx, int, int) {
+        const float val = in_h[idx];
+        if (in_m[idx] > 0.5f && (MAX ? val > mv : val < mv)) mv = val;
+      });
+      if (MAX ? mv > none + 1.f : mv < none - 1.f) { h = mv; m = 0.6f; }
     }
     out_h[i] = h; out_m[i] = m;
     miss = !(m > 0.5f);

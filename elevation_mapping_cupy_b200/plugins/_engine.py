@@ -1,6 +1,5 @@
 """Helpers shared by the built-in plugins: call a libemap.so stencil on torch CUDA tensors.
 Ordering with the caller's torch stream is by stream waits (ElevationMap._after_framework / _before_framework), never a host sync."""
-import ctypes as C
 
 
 def require_engine(engine, who):
@@ -16,3 +15,33 @@ def as_plane(t):
     if not t.is_cuda:
         raise TypeError("plugin layers must be CUDA tensors")
     return t.to(torch.float32).contiguous()
+
+
+def run_plugin(eng, entry, planes, *args, ptrs=()):
+    """Runs the library entry point `entry` of the engine `eng` (require_engine) as `entry(handle, *planes, *ptrs, out,
+    *args)` and returns `out`, a new (W,W) plane.  `planes` are (W,W) CUDA layers, `ptrs` raw pointers the entry point
+    takes before the output.  The call runs after the torch work queued so far and before the torch work queued next."""
+    import torch
+    planes = [as_plane(p) for p in planes]
+    out = torch.empty_like(planes[0])
+    eng._after_framework()
+    eng._check(getattr(eng._L, entry)(eng._h, *(p.data_ptr() for p in planes), *ptrs, out.data_ptr(), *args))
+    eng._before_framework()
+    return out
+
+
+class FillFilter:
+    """Body of MinFilter and MaxFilter (`ENTRY`: emap_min_filter / emap_max_filter).  Not a PluginBase subclass:
+    PluginManager instantiates every PluginBase subclass a plugin module holds, imported ones included."""
+    ENTRY = None
+
+    def __init__(self, cell_n: int = 100, dilation_size: int = 5, iteration_n: int = 5, engine=None, **kwargs):
+        super().__init__()
+        self.iteration_n = int(iteration_n)
+        self.dilation_size = int(dilation_size)
+        self.width = self.height = cell_n
+        self.engine = engine
+
+    def __call__(self, elevation_map, layer_names, plugin_layers, plugin_layer_names, *args):
+        eng = require_engine(self.engine, type(self).__name__)
+        return run_plugin(eng, self.ENTRY, (elevation_map[0], elevation_map[2]), self.dilation_size, self.iteration_n, None)

@@ -4,7 +4,7 @@ to the host and calls cv2.erode).  Here the same arithmetic runs on the device (
 from typing import List
 
 from .plugin_manager import PluginBase
-from ._engine import require_engine, as_plane
+from ._engine import require_engine, run_plugin
 
 
 class Erosion(PluginBase):
@@ -20,7 +20,6 @@ class Erosion(PluginBase):
 
     def __call__(self, elevation_map, layer_names: List[str], plugin_layers, plugin_layer_names: List[str],
                  semantic_map, semantic_layer_names: List[str], *args):
-        import torch
         eng = require_engine(self.engine, "Erosion")
         semantic_layer_names = semantic_layer_names or []
         layer = None
@@ -30,10 +29,4 @@ class Erosion(PluginBase):
             if layer is not None:
                 break
             print(f"No layers are found, using {self.default_layer_name}!")
-        layer = as_plane(layer)
-        out = torch.empty_like(layer)
-        eng._after_framework()
-        eng._check(eng._L.emap_erode(eng._h, layer.data_ptr(), out.data_ptr(), self.kernel_size, self.iterations,
-                                     int(self.reverse)))
-        eng._before_framework()
-        return out
+        return run_plugin(eng, "emap_erode", (layer,), self.kernel_size, self.iterations, int(self.reverse))

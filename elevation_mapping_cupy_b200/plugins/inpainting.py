@@ -9,7 +9,7 @@ call on large maps and without the two PCIe copies.  `method="ns"` (Navier-Stoke
 from typing import List
 
 from .plugin_manager import PluginBase
-from ._engine import require_engine, as_plane
+from ._engine import require_engine, run_plugin
 
 
 class Inpainting(PluginBase):
@@ -20,13 +20,7 @@ class Inpainting(PluginBase):
         self.engine = engine
 
     def __call__(self, elevation_map, layer_names: List[str], plugin_layers, plugin_layer_names: List[str], *args):
-        import torch
         eng = require_engine(self.engine, "Inpainting")
         if self.method != 0:
             raise NotImplementedError("Inpainting(method='ns'): the Navier-Stokes variant is not implemented on the device")
-        h = as_plane(elevation_map[0]); m = as_plane(elevation_map[2])
-        out = torch.empty_like(h)
-        eng._after_framework()
-        eng._check(eng._L.emap_inpaint(eng._h, h.data_ptr(), m.data_ptr(), out.data_ptr(), self.method))
-        eng._before_framework()
-        return out
+        return run_plugin(eng, "emap_inpaint", (elevation_map[0], elevation_map[2]), self.method)

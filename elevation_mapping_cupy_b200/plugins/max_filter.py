@@ -1,27 +1,9 @@
 """max_filter plugin: fill invalid cells with the maximum of their valid neighbours, iterated (Jacobi)
 (reference: elevation_mapping_cupy/script/elevation_mapping_cupy/plugins/max_filter.py:12-113).
 Runs in libemap.so (`emap_max_filter`)."""
-from typing import List
-
 from .plugin_manager import PluginBase
-from ._engine import require_engine, as_plane
+from ._engine import FillFilter
 
 
-class MaxFilter(PluginBase):
-    def __init__(self, cell_n: int = 100, dilation_size: int = 5, iteration_n: int = 5, engine=None, **kwargs):
-        super().__init__()
-        self.iteration_n = int(iteration_n)
-        self.dilation_size = int(dilation_size)
-        self.width = self.height = cell_n
-        self.engine = engine
-
-    def __call__(self, elevation_map, layer_names: List[str], plugin_layers, plugin_layer_names: List[str], *args):
-        import torch
-        eng = require_engine(self.engine, "MaxFilter")
-        h = as_plane(elevation_map[0]); m = as_plane(elevation_map[2])
-        out = torch.empty_like(h)
-        eng._after_framework()
-        eng._check(eng._L.emap_max_filter(eng._h, h.data_ptr(), m.data_ptr(), out.data_ptr(), self.dilation_size,
-                                          self.iteration_n, None))
-        eng._before_framework()
-        return out
+class MaxFilter(FillFilter, PluginBase):
+    ENTRY = "emap_max_filter"

@@ -6,7 +6,7 @@ from typing import List
 import numpy as np
 
 from .plugin_manager import PluginBase
-from ._engine import require_engine, as_plane
+from ._engine import require_engine, run_plugin
 
 
 class RobotCentricElevation(PluginBase):
@@ -21,14 +21,8 @@ class RobotCentricElevation(PluginBase):
 
     def __call__(self, elevation_map, layer_names: List[str], plugin_layers, plugin_layer_names: List[str],
                  semantic_map, semantic_layer_names: List[str], rotation, *args):
-        import torch
         eng = require_engine(self.engine, "RobotCentricElevation")
-        h = as_plane(elevation_map[0]); m = as_plane(elevation_map[2])
         R = rotation.detach().cpu().numpy() if hasattr(rotation, "detach") else np.asarray(rotation)
         R = np.ascontiguousarray(R, dtype=np.float32).reshape(9)
-        out = torch.empty_like(h)
-        eng._after_framework()
-        eng._check(eng._L.emap_robot_centric_elevation(eng._h, h.data_ptr(), m.data_ptr(), R.ctypes.data, out.data_ptr(),
-                                                       self.resolution, self.threshold, self.use_threshold))
-        eng._before_framework()
-        return out
+        return run_plugin(eng, "emap_robot_centric_elevation", (elevation_map[0], elevation_map[2]), self.resolution,
+                          self.threshold, self.use_threshold, ptrs=(R.ctypes.data,))

@@ -8,7 +8,7 @@ layer, with the reference's message, when `input_layer_name` is unknown.
 from typing import List
 
 from .plugin_manager import PluginBase
-from ._engine import require_engine, as_plane
+from ._engine import require_engine, run_plugin
 
 
 class SmoothFilter(PluginBase):
@@ -26,11 +26,5 @@ class SmoothFilter(PluginBase):
         return elevation_map[0]
 
     def __call__(self, elevation_map, layer_names: List[str], plugin_layers, plugin_layer_names: List[str], *args):
-        import torch
         eng = require_engine(self.engine, "SmoothFilter")
-        src = as_plane(self._source(elevation_map, layer_names, plugin_layers, plugin_layer_names))
-        dst = torch.empty_like(src)
-        eng._after_framework()
-        eng._check(eng._L.emap_smooth_filter(eng._h, src.data_ptr(), dst.data_ptr()))
-        eng._before_framework()
-        return dst
+        return run_plugin(eng, "emap_smooth_filter", (self._source(elevation_map, layer_names, plugin_layers, plugin_layer_names),))

@@ -38,6 +38,28 @@ def test_min_filter_matches_oracle(oracle_mod, k, iters, valid_frac):
     assert np.array_equal(np.nan_to_num(out), np.nan_to_num(ref))
 
 
+# (k, iteration_n, valid fraction, exits early): at half the cells valid every cell is filled after 2 of 30 passes; at
+# 0.1 % valid, 5 passes never fill the map
+@pytest.mark.parametrize("k,iters,valid_frac,early", [(1, 30, 0.5, True), (2, 3, 0.05, False), (1, 5, 0.001, False)])
+def test_fill_filters_iterations_run_match_oracle(oracle_mod, k, iters, valid_frac, early):
+    """iterations_run of emap_min_filter / emap_max_filter: the passes up to the first one that leaves no cell unfilled"""
+    import ctypes as C
+    import torch
+    from elevation_mapping_cupy_b200.parameter import core_parameter
+    em = _mk(core_parameter(202))
+    st = _random_state(202, 5, valid_frac)
+    h = torch.from_numpy(st[0]).cuda(); m = torch.from_numpy(st[2]).cuda(); o = torch.empty_like(h)
+    em._after_framework()
+    for entry, oracle_filter in (("emap_min_filter", oracle_mod.min_filter), ("emap_max_filter", oracle_mod.max_filter)):
+        n = C.c_int32(-1)
+        em._check(getattr(em._L, entry)(em._h, h.data_ptr(), m.data_ptr(), o.data_ptr(), k, iters, C.byref(n)))
+        ref_out, ref_n = oracle_filter(202, k, iters, st[0], st[2])
+        assert (ref_n < iters) == early, (entry, ref_n)
+        assert n.value == ref_n, entry
+        assert np.array_equal(np.nan_to_num(o.cpu().numpy(), nan=-7), np.nan_to_num(ref_out, nan=-7)), entry
+    em._before_framework()
+
+
 def test_smooth_filter_matches_oracle_and_scipy(oracle_mod):
     from scipy import ndimage
     from elevation_mapping_cupy_b200.parameter import core_parameter
@@ -52,6 +74,21 @@ def test_smooth_filter_matches_oracle_and_scipy(oracle_mod):
     assert np.array_equal(out, ref)
     sp = ndimage.uniform_filter(ndimage.uniform_filter(st[0], size=3), size=3)   # smooth_filter.py:57-58 on the host
     assert np.abs(out - sp).max() < 1e-6
+
+
+def test_update_normal_of_a_plane_matches_oracle(oracle_mod):
+    """update_normal(plane) (EM.py:564-577) on an arbitrary device plane: the normals of that plane over the valid cells"""
+    import torch
+    from elevation_mapping_cupy_b200.parameter import core_parameter
+    W = 202
+    p = core_parameter(W)
+    em = _mk(p)
+    st = _random_state(W, 9)
+    em.set_state(st)
+    plane = np.random.default_rng(4).standard_normal((W, W)).astype(np.float32)
+    em.update_normal(torch.from_numpy(plane).cuda())
+    _, normal = em.get_state()
+    assert np.array_equal(normal, oracle_mod.normal(W, p.resolution, plane, st[2]))
 
 
 def test_reference_api_surface_smoke():
