@@ -15,6 +15,7 @@
 #include "emap_kernels.cuh"
 #include "emap_inpaint.cuh"
 #include "emap_semantic.cuh"
+#include "emap_polygon.cuh"
 
 namespace {
 
@@ -131,6 +132,10 @@ struct emap_handle {
   // inpainting scratch (allocated on first use): one block, carved by inpaint_scratch
   DevBuf<char> ip_block;
   int ip_grid = 0;
+  // polygon safety check scratch (allocated on first use): one device block carved by carve_polygon, and its pinned
+  // host staging (the vertices on the way in, the result and the ring on the way out)
+  DevBuf<char> pg_block;
+  char* pg_host = nullptr;
   // misc
   int64_t launches = 0;
   int count_rays = 0;
@@ -765,6 +770,59 @@ int export_layers(emap_handle* h, int32_t n, const char* const* names, const flo
   return EMAP_OK;
 }
 
+// ---- polygon safety check --------------------------------------------------------------------
+constexpr int kRingHead = 256;     // ring vertices read back with the result; a longer ring takes a second copy
+
+struct PolyScratch {
+  float2* xy;                      // EMAP_POLYGON_MAX_VERTICES clipped vertices
+  PolyPartial* part;               // one per k_polygon CTA
+  int *col_min, *col_max;          // W - 2 each
+  PolyResult* res;                 // followed directly by ring, so that one copy reads both
+  double2* ring;                   // 2 (W - 2) + 1 vertices at most
+};
+
+dim3 polygon_grid(int W) { return dim3(cdiv(W, PG_COLS), cdiv(W, PG_ROWS)); }
+size_t ring_capacity(int W) { return 2 * (size_t)(W - 2) + 1; }
+
+size_t carve_polygon(int W, void* base, PolyScratch& s) {
+  const dim3 g = polygon_grid(W);
+  Carver b{(uintptr_t)base};
+  s.xy = b.take<float2>(EMAP_POLYGON_MAX_VERTICES);
+  s.part = b.take<PolyPartial>((size_t)g.x * g.y);
+  s.col_min = b.take<int>(W - 2);
+  s.col_max = b.take<int>(W - 2);
+  s.res = b.take<PolyResult>(1, 16);
+  s.ring = b.take<double2>(ring_capacity(W), 16);
+  return b.bytes;
+}
+
+int alloc_polygon_scratch(emap_handle* h, PolyScratch& s) {
+  const int W = h->dc.W;
+  if (!h->pg_host) {
+    CK(h->pg_block.alloc(carve_polygon(W, nullptr, s)));
+    carve_polygon(W, h->pg_block, s);
+    CK(cudaMemsetAsync(s.col_min, 0x7f, sizeof(int) * (W - 2), h->stream));    // "no cell yet": k_hull restores it
+    CK(cudaMemsetAsync(s.col_max, 0xff, sizeof(int) * (W - 2), h->stream));
+    CK(cudaMallocHost(&h->pg_host, sizeof(float2) * EMAP_POLYGON_MAX_VERTICES + sizeof(PolyResult) +
+                                        sizeof(double2) * ring_capacity(W)));
+  }
+  carve_polygon(W, h->pg_block, s);
+  return 0;
+}
+
+// traversability_polygon.py:46-51 calculate_area on fp32 vertices: every operation in fp32, terms in order i = 0..n-1
+// with p1 = polygon[i - 1], the absolute value at the end
+float shoelace_f32(const float* xy, int n) {
+  float area = 0.0f;
+  for (int i = 0; i < n; i++) {
+    const int j = i ? i - 1 : n - 1;
+    const float a = xy[2 * j] * xy[2 * i + 1];
+    const float b = xy[2 * j + 1] * xy[2 * i];
+    area = area + (a - b) / 2.0f;
+  }
+  return std::fabs(area);
+}
+
 }  // namespace
 
 // =============================================================================================
@@ -914,6 +972,7 @@ emap_handle::~emap_handle() {
   for (int k = 0; k < 9; k++) if (st.ev[k]) cudaEventDestroy(st.ev[k]);
   if (own_stream) cudaStreamDestroy(own_stream);
   if (copy_stream) cudaStreamDestroy(copy_stream);
+  if (pg_host) cudaFreeHost(pg_host);
 }
 
 extern "C" {
@@ -1312,6 +1371,80 @@ int emap_layer_device_ptr(emap_handle* h, const char* name, void** ptr) {
 int emap_exists_layer(const emap_handle* h, const char* name) {
   if (!h || !name) return 0;
   return layer_index(name) >= 0 ? 1 : 0;
+}
+
+// EM.py:837-889 get_polygon_traversability (WRAP:254-281): area, clip and bounding box on the host in fp32, then
+// k_polygon + k_hull, one device-to-host copy and one synchronisation.
+int emap_polygon_traversability(emap_handle* h, const float* polygon_xy, int32_t n_vertices, const float* checker_plane,
+                                double safe_thresh, double safe_min_thresh, int32_t max_unsafe_n, double result[3],
+                                double* hull_xy, int32_t* n_hull, float* mask) {
+  ENTER(h);
+  if (!polygon_xy || !result || !n_hull || *n_hull < 0 || (*n_hull > 0 && !hull_xy))
+    return fail(h, EMAP_ERR_INVALID, "emap_polygon_traversability: null argument or negative hull capacity");
+  if (n_vertices < 3 || n_vertices > EMAP_POLYGON_MAX_VERTICES)
+    return fail(h, EMAP_ERR_INVALID, "emap_polygon_traversability: 3 to EMAP_POLYGON_MAX_VERTICES vertices required");
+  const int W = h->dc.W;
+  const size_t C = (size_t)h->dc.C;
+  PolyScratch s;
+  int rc = alloc_polygon_scratch(h, s);
+  if (rc) return rc;
+  const float area = shoelace_f32(polygon_xy, n_vertices);
+  // EM.py:847-854: each coordinate clipped to [center - map_length/2 + resolution, center + map_length/2 - resolution],
+  // fp32 throughout; map_length is the map's true length (cell_n - 2) * resolution
+  const float half = (float)(0.5 * (double)(W - 2) * h->cfg.resolution), res_f = h->dc.res_f;
+  float lo[2], hi[2], bmin[2], bmax[2];
+  for (int k = 0; k < 2; k++) {
+    lo[k] = (h->center[k] - half) + res_f;
+    hi[k] = (h->center[k] + half) - res_f;
+  }
+  float2* xy = (float2*)h->pg_host;
+  for (int i = 0; i < n_vertices; i++) {
+    float v[2];
+    for (int k = 0; k < 2; k++) {
+      v[k] = std::min(std::max(polygon_xy[2 * i + k], lo[k]), hi[k]);
+      bmin[k] = i ? std::min(bmin[k], v[k]) : v[k];
+      bmax[k] = i ? std::max(bmax[k], v[k]) : v[k];
+    }
+    xy[i] = make_float2(v[0], v[1]);
+  }
+  const float clipped_area = shoelace_f32((const float*)xy, n_vertices);
+  PolyArgs a;
+  a.xy = s.xy; a.n = n_vertices; a.cx = h->center[0]; a.cy = h->center[1];
+  a.bbox[0] = bmin[0]; a.bbox[1] = bmin[1]; a.bbox[2] = bmax[0]; a.bbox[3] = bmax[1];
+  a.thr_over = (float)(1.0 - safe_thresh); a.thr_max = (float)(1.0 - safe_min_thresh);    // traversability_polygon.py:25-26
+  a.max_unsafe_n = max_unsafe_n;
+  CK(cudaMemcpyAsync(s.xy, xy, sizeof(float2) * n_vertices, cudaMemcpyHostToDevice, h->stream));
+  const dim3 grid = polygon_grid(W);
+  k_polygon<<<grid, PG_THREADS, 0, h->stream>>>(W, res_f, a, h->map + L_VALID * C,
+                                                checker_plane ? checker_plane : h->map + L_TRAV * C, mask, s.part,
+                                                s.col_min, s.col_max);
+  LAUNCH_CHECK();
+  k_hull<<<1, HULL_THREADS, 0, h->stream>>>(W, h->cfg.resolution, a, s.part, (int)(grid.x * grid.y), s.col_min, s.col_max,
+                                            s.res, s.ring);
+  LAUNCH_CHECK();
+  char* back = h->pg_host + sizeof(float2) * EMAP_POLYGON_MAX_VERTICES;
+  const size_t head = std::min((size_t)kRingHead, ring_capacity(W));
+  CK(cudaMemcpyAsync(back, s.res, sizeof(PolyResult) + sizeof(double2) * head, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  PolyResult r;
+  memcpy(&r, back, sizeof(r));
+  const double2* ring = (const double2*)(back + sizeof(PolyResult));
+  if (r.n_ring > (int)head) {
+    CK(cudaMemcpyAsync(back + sizeof(PolyResult) + sizeof(double2) * head, s.ring + head,
+                       sizeof(double2) * (r.n_ring - head), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+  }
+  // EM.py:884-887: a polygon (almost) entirely outside the map is unsafe
+  result[0] = (r.is_safe && !(clipped_area < 0.001f)) ? 1.0 : 0.0;
+  result[1] = r.t;
+  result[2] = (double)area;
+  if (r.n_ring > *n_hull) {
+    *n_hull = r.n_ring;
+    return fail(h, EMAP_ERR_INVALID, "emap_polygon_traversability: hull capacity too small (needed length in *n_hull)");
+  }
+  for (int k = 0; k < r.n_ring; k++) { hull_xy[2 * k] = ring[k].x; hull_xy[2 * k + 1] = ring[k].y; }
+  *n_hull = r.n_ring;
+  return EMAP_OK;
 }
 
 int emap_get_state(emap_handle* h, float* map_host, float* normal_host) {

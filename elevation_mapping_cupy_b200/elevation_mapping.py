@@ -9,7 +9,8 @@ happens in the library; this module only marshals arguments.  Device arrays are 
 CUDA tensors that alias the library's memory (they also expose `__cuda_array_interface__`).
 
 Point-cloud semantic layers (average / class_average / color fusion) are fused inside the frame (semantic_map.py).
-Out of scope (SURVEY.md section 8): image input, image / bayesian semantic fusion, polygon safety check.
+The polygon safety check (get_polygon_traversability) is one library call: mask, statistics and hull on the device.
+Out of scope (SURVEY.md section 8): image input, image / bayesian semantic fusion.
 """
 import ctypes as C
 import threading
@@ -98,6 +99,10 @@ class ElevationMap:
         self.semantic_map = SemanticMap(param, engine=self)              # EM.py:106
         self.base_rotation = np.eye(3, dtype=np.float32)
         self._export_tmp = np.zeros((self.cell_n - 2, self.cell_n - 2), np.float32)
+        # polygon safety check (EM.py:110, 239): the last ring, the library's ring buffer, the mask (made on first use)
+        self.untraversable_polygon = np.zeros((1, 2))
+        self._ring = np.zeros((2 * (self.cell_n - 2) + 1, 2), np.float64)
+        self._mask = None
 
     # ---- plumbing -------------------------------------------------------------------------
     def _check(self, rc):
@@ -411,8 +416,41 @@ class ElevationMap:
     def input_image(self, *a, **k):
         raise NotImplementedError("image input is outside the fusion path (SURVEY.md section 8)")
 
-    def get_polygon_traversability(self, *a, **k):
-        raise NotImplementedError("polygon safety check is outside the fusion path (SURVEY.md section 8)")
+    def get_polygon_traversability(self, polygon, result):
+        """EM.py:837-889: is the (N, 2) polygon (any array framework, cast to float32 as the C++ bridge passes it) safe to
+        stand on?  Writes [is_safe, t, area] into `result`, keeps the convex hull of the polygon's untraversable cells
+        for get_untraversable_polygon and returns its ring length (0: no such polygon).  The polygon mask is left in
+        `self.mask`.  One kernel pass over the map, one small hull kernel, one device-to-host copy, one sync."""
+        poly = np.ascontiguousarray(_to_host(polygon), dtype=np.float32).reshape(-1, 2)
+        checker = None
+        if self.param.checker_layer != "traversability":
+            checker = self.get_layer(self.param.checker_layer)     # None: the layer is absent, traversability is used
+        mask = self.mask
+        res = np.zeros(3, np.float64)
+        n_ring = C.c_int32(len(self._ring))
+        with self.map_lock:
+            self._after_framework()
+            self._check(self._L.emap_polygon_traversability(
+                self._h, poly.ctypes.data, poly.shape[0], None if checker is None else checker.data_ptr(),
+                float(self.param.safe_thresh), float(self.param.safe_min_thresh), int(self.param.max_unsafe_n),
+                res.ctypes.data, self._ring.ctypes.data, C.byref(n_ring), mask.data_ptr()))
+        if _clipped_area(poly, self.center, self.cell_n, self.resolution) < np.float32(0.001):
+            print("requested polygon is outside of the map")
+        result[...] = res
+        self.untraversable_polygon = self._ring[:n_ring.value].copy()
+        return n_ring.value
+
+    def get_untraversable_polygon(self, untraversable_polygon):
+        """EM.py:891-897: copy the ring of the last get_polygon_traversability into the caller's (n, 2) array."""
+        untraversable_polygon[...] = self.untraversable_polygon
+
+    @property
+    def mask(self):
+        """(W, W) float32 polygon mask of the last get_polygon_traversability (EM.py:239 `self.mask`), a torch CUDA tensor."""
+        if self._mask is None:
+            import torch
+            self._mask = torch.zeros((self.cell_n, self.cell_n), dtype=torch.float32, device=f"cuda:{self.device}")
+        return self._mask
 
     def initialize_map(self, points, method="cubic"):
         """EM.py:899-922 + map_initializer.py:25-62: clear the map, interpolate the given (x, y, z) points (map frame) over
@@ -452,6 +490,18 @@ def _to_host(x):
     if hasattr(x, "get"):                                # cupy array
         return x.get()
     return np.asarray(x)
+
+
+def _clipped_area(poly, center, cell_n, resolution):
+    """Shoelace area of the fp32 polygon after the clip of EM.py:847-851 (what emap_polygon_traversability tests against
+    0.001 to declare the polygon outside of the map); every operation in fp32."""
+    f = np.float32
+    half, res = f(0.5 * (cell_n - 2) * resolution), f(resolution)
+    c = np.asarray(center, np.float32)[:2]
+    p = np.clip(poly, (c - half) + res, (c + half) - res).astype(np.float32)
+    q = np.roll(p, 1, axis=0)                                          # q[i] = p[i - 1]
+    terms = (q[:, 0] * p[:, 1] - q[:, 1] * p[:, 0]) / f(2)
+    return abs(np.cumsum(terms, dtype=np.float32)[-1])                 # in order i = 0..n-1
 
 
 def _framework_stream():

@@ -212,6 +212,21 @@ int emap_exists_layer(const emap_handle* h, const char* name);  /* EM.py:702-718
 int emap_get_state(emap_handle* h, float* map_host, float* normal_host);
 int emap_set_state(emap_handle* h, const float* map_host, const float* normal_host, const double center[3]);
 
+/* ---- polygon safety check: EM.py:837-897 get_polygon_traversability / get_untraversable_polygon (WRAP:254-281, the
+ * ROS node's check_safety service).  polygon_xy: n_vertices (x, y) fp32 pairs in host memory, 3 <= n_vertices <=
+ * EMAP_POLYGON_MAX_VERTICES.  checker_plane_device: the (W,W) fp32 plane of param.checker_layer, NULL for the
+ * traversability layer.  result = {is_safe (1/0), mean untraversability t, shoelace area of the polygon as given}.
+ * hull_xy receives the closed ring (first vertex repeated at the end) of the convex hull of the interior cells whose
+ * masked untraversability exceeds 1 - safe_thresh, in metres, as rows of (x, y) doubles; *n_hull is its capacity in rows
+ * on entry and the ring length on return (0: no polygon).  A capacity below the ring length returns EMAP_ERR_INVALID
+ * with the needed length in *n_hull (result is written).  mask_device: optional (W,W) fp32 output of the polygon mask.
+ * One device-to-host copy and one synchronisation per call. */
+#define EMAP_POLYGON_MAX_VERTICES 1024
+int emap_polygon_traversability(emap_handle* h, const float* polygon_xy, int32_t n_vertices,
+                                const float* checker_plane_device, double safe_thresh, double safe_min_thresh,
+                                int32_t max_unsafe_n, double result[3], double* hull_xy, int32_t* n_hull,
+                                float* mask_device);
+
 /* ---- plugin stencils on device planes (W,W fp32); replace the CuPy / OpenCV / cupyx bodies of
  * plugins/min_filter.py:57-118, plugins/smooth_filter.py:57-58, plugins/inpainting.py:53-63 ---- */
 int emap_min_filter(emap_handle* h, const float* elevation, const float* is_valid, float* out, int32_t dilation_size,
