@@ -568,6 +568,10 @@ int frame_rays(emap_handle* h) {
     for (size_t s = 0; s + 1 < h->offs.size(); s++) {
       const i64 n = h->offs[s + 1] - h->offs[s];
       if (n <= 0 || h->dc.n_steps == 0) continue;
+      // No map cell within reach of the frame's sensors (empty box): every sample clamps to the border ring, on which no
+      // ray acts, and k_raycast<false>'s fine-tile address would lie outside its coarse map.  The counting variant reads
+      // no coarse map and still counts the march steps.
+      if (!h->count_rays && (box.r1 <= box.r0 || box.c1 <= box.c0)) continue;
       // persistent grid: enough CTAs to fill every SM, never more than one warp per possible ray
       const int grid = (int)std::min<i64>((i64)h->n_sm * h->rc_blocks_per_sm, (n + RC_THREADS / 32 - 1) / (RC_THREADS / 32));
       if (h->count_rays)

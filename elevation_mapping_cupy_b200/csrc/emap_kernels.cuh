@@ -664,7 +664,8 @@ k_raycast(const DevCfg c, const Pose q, const Ray* __restrict__ rays, int* __res
         if (COUNT) n_steps_done += ((unsigned)k < (unsigned)n_act) && lane != 0;
         if (nidx == prev) continue;                               // CK.py:209 (CK.py:211: border cells are skipped via thr = -inf)
         const float nz = __fmaf_rn(rz, sk, tz);
-        if (!COUNT) {   // coarse level: the fine tile's maximum (every cell a ray of this frame reaches lies in the tiled box)
+        if (!COUNT) {   // coarse level: the fine tile's maximum (every cell a ray reaches lies in the tiled box: frame_rays
+                        // launches no march when that box is empty)
           float m;
           asm volatile("ld.shared.f32 %0, [%1];" : "=f"(m) : "r"(s_t8_o + (ix >> ts) * (4u * RT) + ((iy >> ts) << 2)));
           if (nz > m) continue;
@@ -677,7 +678,7 @@ k_raycast(const DevCfg c, const Pose q, const Ray* __restrict__ rays, int* __res
             float d = __fmul_rn(ddy, ddy); d = __fmaf_rn(ddx, ddx, d); d = __fmaf_rn(ddz, ddz, d);
             near = h16(d) < 0.1f;
           }
-          if (!near) n_visits++;
+          if (!near && cell_inside(W, (int)ix, (int)iy)) n_visits++;   // border cells are skipped first (CK.py:211)
         }
         if (nz > __ldg(s.thr + nidx)) continue;                   // first level: the sample cannot act on this cell
         // ---- second level (rare): the exact tests of CK.py:225-256
