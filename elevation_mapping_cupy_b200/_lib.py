@@ -90,6 +90,9 @@ SIGNATURES = {
                                                C.c_double, C.c_double, C.c_int32]),
     "emap_inpaint": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32]),
     "emap_inpaint_stats": (C.c_int, [C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32)]),
+    "emap_semantic_filter": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "emap_semantic_traversability": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "emap_features_pca": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "emap_polygon_traversability": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_double,
                                               C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p]),
     "emap_sync": (C.c_int, [C.c_void_p]),

@@ -16,6 +16,7 @@
 #include "emap_inpaint.cuh"
 #include "emap_semantic.cuh"
 #include "emap_polygon.cuh"
+#include "emap_semantic_plugins.cuh"
 
 namespace {
 
@@ -136,6 +137,8 @@ struct emap_handle {
   // host staging (the vertices on the way in, the result and the ring on the way out)
   DevBuf<char> pg_block;
   char* pg_host = nullptr;
+  // features_pca scratch (allocated on first use): one device block carved by carve_pca
+  DevBuf<char> pca_block;
   // misc
   int64_t launches = 0;
   int count_rays = 0;
@@ -825,6 +828,30 @@ float shoelace_f32(const float* xy, int n) {
     area = area + (a - b) / 2.0f;
   }
   return std::fabs(area);
+}
+
+// ---- features_pca ------------------------------------------------------------------------------
+struct PcaScratch {
+  PcaResult* res;
+  double* part;                    // pca_entries(PCA_MAX_F) per k_pca_stats CTA
+  double* proj;                    // 3 planes of C projections
+};
+
+int pca_stats_grid(emap_handle* h) { return std::min(cdiv(h->dc.C, 32), 2 * h->n_sm); }   // 32 <= tile cells
+
+size_t carve_pca(emap_handle* h, void* base, PcaScratch& s) {
+  Carver b{(uintptr_t)base};
+  s.res = b.take<PcaResult>(1);
+  s.part = b.take<double>((size_t)pca_stats_grid(h) * PCA_MAX_ENTRIES);
+  s.proj = b.take<double>(3 * (size_t)h->dc.C);
+  return b.bytes;
+}
+
+// the planes of a semantic plugin call: a non-null host array of n non-null device pointers
+bool planes_ok(int32_t n, const float* const* planes) {
+  if (n > 0 && !planes) return false;
+  for (int l = 0; l < n; l++) if (!planes[l]) return false;
+  return true;
 }
 
 }  // namespace
@@ -1561,6 +1588,72 @@ int emap_inpaint(emap_handle* h, const float* elevation, const float* is_valid, 
     h->launches++;
   }
   PER_CELL(k_ip_finish, (int)C, (const uint8_t*)v.img, elevation, out, (const InpaintCtl*)ctl);
+  return EMAP_OK;
+}
+
+// plugins/semantic_filter.py:89-133: argmax over the planes, palette entry of the class id (bits)
+int emap_semantic_filter(emap_handle* h, int32_t n_layers, const float* const* planes, float* out) {
+  ENTER(h);
+  if (!out || n_layers < 0 || n_layers > EMAP_SEMANTIC_FILTER_MAX_LAYERS || !planes_ok(n_layers, planes))
+    return fail(h, EMAP_ERR_INVALID, "emap_semantic_filter: 0 to EMAP_SEMANTIC_FILTER_MAX_LAYERS non-null planes and a non-null output required");
+  SemFilterArgs a;
+  memset(&a, 0, sizeof(a));
+  a.n = n_layers;
+  for (int l = 0; l < n_layers; l++) a.plane[l] = planes[l];
+  PER_CELL(k_semantic_filter, h->dc.C, a, (u32*)out);
+  return EMAP_OK;
+}
+
+// plugins/semantic_traversability.py:59-83: per-layer threshold votes (fp64 comparisons), fp32(0.1) or 1
+int emap_semantic_traversability(emap_handle* h, int32_t n_layers, const float* const* planes, const double* thresholds,
+                                 const int32_t* is_traversability_type, float* out) {
+  ENTER(h);
+  if (!out || n_layers < 0 || n_layers > EMAP_SEMANTIC_TRAVERSABILITY_MAX_LAYERS || !planes_ok(n_layers, planes) ||
+      (n_layers > 0 && (!thresholds || !is_traversability_type)))
+    return fail(h, EMAP_ERR_INVALID, "emap_semantic_traversability: 0 to EMAP_SEMANTIC_TRAVERSABILITY_MAX_LAYERS non-null planes, "
+                                     "thresholds, types and a non-null output required");
+  SemTravArgs a;
+  memset(&a, 0, sizeof(a));
+  a.n = n_layers;
+  for (int l = 0; l < n_layers; l++) {
+    a.plane[l] = planes[l];
+    a.thr[l] = thresholds[l];
+    if (is_traversability_type[l]) a.is_trav[l >> 5] |= 1u << (l & 31);
+  }
+  PER_CELL(k_semantic_traversability, h->dc.C, a, out);
+  return EMAP_OK;
+}
+
+// plugins/features_pca.py:44-96: exact 3-component PCA of the clipped features on the device, packed to colour bits.
+// Four launches and one synchronisation, at the end, to read the NaN flag.
+int emap_features_pca(emap_handle* h, int32_t n_features, const float* const* planes, float* out) {
+  ENTER(h);
+  NvtxRange nv("emap:features_pca");
+  if (!out || n_features < 3 || n_features > EMAP_PCA_MAX_FEATURES || !planes_ok(n_features, planes))
+    return fail(h, EMAP_ERR_INVALID, "emap_features_pca: 3 to EMAP_PCA_MAX_FEATURES non-null planes and a non-null output required");
+  PcaScratch s;
+  int rc = grow(h, h->pca_block, carve_pca(h, nullptr, s), 0, false);
+  if (rc) return rc;
+  carve_pca(h, h->pca_block, s);
+  const int C = h->dc.C, F = n_features;
+  PcaArgs a;
+  memset(&a, 0, sizeof(a));
+  a.F = F;
+  for (int f = 0; f < F; f++) a.plane[f] = planes[f];
+  const size_t eig_smem = sizeof(double) * 2 * F * (F + 1);
+  CK(cudaFuncSetAttribute(k_pca_eigen, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eig_smem));
+  CK(cudaMemsetAsync(&s.res->nan, 0, sizeof(int), h->stream));
+  const int grid = pca_stats_grid(h);
+  k_pca_stats<<<grid, PCA_THREADS, 0, h->stream>>>(C, a, s.part, s.res);
+  LAUNCH_CHECK();
+  k_pca_eigen<<<1, PCA_THREADS, eig_smem, h->stream>>>(C, F, grid, s.part, s.res);
+  LAUNCH_CHECK();
+  PER_CELL(k_pca_project, C, a, s.res, s.proj);
+  PER_CELL(k_pca_pack, C, (const PcaResult*)s.res, (const double*)s.proj, (u32*)out);
+  int nan = 0;
+  CK(cudaMemcpyAsync(&nan, &s.res->nan, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  if (nan) return fail(h, EMAP_ERR_INVALID, "emap_features_pca: NaN in the input features");
   return EMAP_OK;
 }
 

@@ -17,17 +17,33 @@ def as_plane(t):
     return t.to(torch.float32).contiguous()
 
 
-def run_plugin(eng, entry, planes, *args, ptrs=()):
+def run_plugin(eng, entry, planes, *args, ptrs=(), like=None):
     """Runs the library entry point `entry` of the engine `eng` (require_engine) as `entry(handle, *planes, *ptrs, out,
-    *args)` and returns `out`, a new (W,W) plane.  `planes` are (W,W) CUDA layers, `ptrs` raw pointers the entry point
-    takes before the output.  The call runs after the torch work queued so far and before the torch work queued next."""
+    *args)` and returns `out`, a new (W,W) plane shaped like planes[0] (or `like` when `planes` is empty).  `planes` are
+    (W,W) CUDA layers, `ptrs` raw pointers the entry point takes before the output.  The call runs after the torch work
+    queued so far and before the torch work queued next."""
     import torch
     planes = [as_plane(p) for p in planes]
-    out = torch.empty_like(planes[0])
+    out = torch.empty_like(as_plane(planes[0] if planes else like))
     eng._after_framework()
     eng._check(getattr(eng._L, entry)(eng._h, *(p.data_ptr() for p in planes), *ptrs, out.data_ptr(), *args))
     eng._before_framework()
     return out
+
+
+def select_planes(patterns, stores):
+    """The planes whose layer name `re.match`es one of `patterns`, store by store and in layer order within a store
+    (semantic_filter.py:77-89, 116-122 of the reference).  `stores`: (layers, names) pairs; layers may be None when
+    `names` is empty (no semantic layer yet)."""
+    import re
+    return [as_plane(layers[i]) for layers, names in stores for i, name in enumerate(names or [])
+            if any(re.match(p, name) for p in patterns)]
+
+
+def pointer_array(planes):
+    """ctypes host array of the planes' device pointers (None for no plane)"""
+    import ctypes as C
+    return (C.c_void_p * len(planes))(*(p.data_ptr() for p in planes)) if planes else None
 
 
 class FillFilter:

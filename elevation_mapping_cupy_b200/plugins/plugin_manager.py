@@ -82,8 +82,8 @@ class PluginManager(object):
             try:
                 module = importlib.import_module("." + spec.name, package=self.package)
             except ImportError as e:
-                # a YAML written for the reference may name a plugin this package does not provide (semantic / image
-                # plugins are outside the fusion path): keep the layer slot, say so, and fail only if it is evaluated
+                # a YAML written for the reference may name a plugin module this package does not provide: keep the
+                # layer slot, say so, and fail only if it is evaluated
                 print(f"plugin {spec.name!r} is not provided by {self.package} ({e}); its layer will raise when requested")
                 self.plugins.append(_MissingPlugin(spec.name))
                 continue

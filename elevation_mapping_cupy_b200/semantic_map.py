@@ -6,7 +6,8 @@ Mirrors the point-cloud half of the reference class
 frame's point record: `average` (fusion/pointcloud_average.py), `class_average` (fusion/pointcloud_class_average.py, the
 reference's default) and `color` (fusion/pointcloud_color.py).  The kernels are csrc/emap_semantic.cuh; this class only
 decides which column of the cloud goes to which layer and hands the layer buffer to the engine
-(`emap_semantic_configure`).  Image fusion, bayesian / class-max fusion and the feature extractors are out of scope.
+(`emap_semantic_configure`).  The plugins that consume these layers (semantic_filter, semantic_traversability,
+features_pca) are in plugins/.  Image fusion, bayesian / class-max fusion and the image feature extractors are out of scope.
 """
 import ctypes as C
 import re

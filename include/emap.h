@@ -248,6 +248,28 @@ int emap_inpaint(emap_handle* h, const float* elevation, const float* is_valid, 
 /* diagnostics of the last emap_inpaint: fast-marching rounds, longest fixed-point iteration, rounds that hit the cap */
 int emap_inpaint_stats(emap_handle* h, int32_t* rounds, int32_t* max_jacobi, int32_t* not_converged);
 
+/* ---- semantic plugins: plugins/semantic_filter.py:13-133, plugins/semantic_traversability.py:12-83 and
+ * plugins/features_pca.py:13-96.  planes_device is a HOST array of n device pointers to (W,W) fp32 planes; out is a (W,W)
+ * fp32 device plane.  The caller selects the planes (the reference's regex / name look-up over its layer stores). ----
+ * emap_semantic_filter: per cell the class id = numpy.argmax over the planes (first maximum wins; a NaN is the maximum,
+ * the first NaN wins; 0 with no plane), written as the bits of the reference palette entry color_map(255)[id]
+ * (r << 16 | g << 8 | b; many are fp32 denormals: read them as uint32). */
+#define EMAP_SEMANTIC_FILTER_MAX_LAYERS 255
+int emap_semantic_filter(emap_handle* h, int32_t n_layers, const float* const* planes_device, float* out);
+/* emap_semantic_traversability: a layer votes where v <= thresholds[l] (is_traversability_type[l] != 0) or v >= thresholds[l]
+ * (otherwise), compared in fp64 (the fp32 value widened); NaN never votes.  out = fp32(0.1) where no layer votes, else 1. */
+#define EMAP_SEMANTIC_TRAVERSABILITY_MAX_LAYERS 128
+int emap_semantic_traversability(emap_handle* h, int32_t n_layers, const float* const* planes_device,
+                                 const double* thresholds, const int32_t* is_traversability_type, float* out);
+/* emap_features_pca: exact PCA (3 components) of the n_features planes clipped to [-1, 1], every cell a sample,
+ * 3 <= n_features <= EMAP_PCA_MAX_FEATURES.  Statistics, eigen-decomposition (Jacobi) and projection in fp64 and in a
+ * fixed order (the result is the same every call); each component's largest-|entry| coordinate is positive (sklearn's
+ * svd_flip).  out = bits of uint8(trunc((p - min) / (max - min) * 255)) per component packed r << 16 | g << 8 | b; a
+ * component of range 0 gives channel 0.  NaN input returns EMAP_ERR_INVALID.  Four kernels and ONE synchronisation, at
+ * the end of the call, to read the NaN flag. */
+#define EMAP_PCA_MAX_FEATURES 64
+int emap_features_pca(emap_handle* h, int32_t n_features, const float* const* planes_device, float* out);
+
 /* ---- plumbing ---- */
 int emap_sync(emap_handle* h);
 int emap_stream(emap_handle* h, void** cuda_stream);
