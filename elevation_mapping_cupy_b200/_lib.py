@@ -95,6 +95,9 @@ SIGNATURES = {
     "emap_features_pca": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "emap_polygon_traversability": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_double,
                                               C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p]),
+    "emap_polygon_traversability_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                    C.c_double, C.c_double, C.c_int32, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_sync": (C.c_int, [C.c_void_p]),
     "emap_stream": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "emap_set_stream": (C.c_int, [C.c_void_p, C.c_void_p]),

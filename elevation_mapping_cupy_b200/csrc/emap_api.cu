@@ -55,6 +55,11 @@ class DevBuf {
   size_t n_ = 0;
 };
 
+// sizes of the polygon check's scratch (carve_polygon): upload bytes, partials, column extremes, read-back bytes
+struct PolySizes {
+  size_t up = 0, items = 0, cols = 0, down = 0;
+};
+
 }  // namespace
 
 struct emap_handle {
@@ -133,10 +138,12 @@ struct emap_handle {
   // inpainting scratch (allocated on first use): one block, carved by inpaint_scratch
   DevBuf<char> ip_block;
   int ip_grid = 0;
-  // polygon safety check scratch (allocated on first use): one device block carved by carve_polygon, and its pinned
-  // host staging (the vertices on the way in, the result and the ring on the way out)
+  // polygon safety check scratch (allocated on first use, grown to the largest call): one device block carved by
+  // carve_polygon, and its pinned host staging (the upload region on the way in, the read-back region on the way out)
   DevBuf<char> pg_block;
+  PolySizes pg_cap{};
   char* pg_host = nullptr;
+  size_t pg_host_bytes = 0;
   // features_pca scratch (allocated on first use): one device block carved by carve_pca
   DevBuf<char> pca_block;
   // misc
@@ -778,43 +785,103 @@ int export_layers(emap_handle* h, int32_t n, const char* const* names, const flo
 }
 
 // ---- polygon safety check --------------------------------------------------------------------
-constexpr int kRingHead = 256;     // ring vertices read back with the result; a longer ring takes a second copy
+constexpr int kRingHead = 256;     // ring vertices of a single call read back with its result
+constexpr size_t kBatchRingHead = 4096;    // ring rows of a batch read back with its results
+// (longer rings take a second copy)
 
 struct PolyScratch {
-  float2* xy;                      // EMAP_POLYGON_MAX_VERTICES clipped vertices
-  PolyPartial* part;               // one per k_polygon CTA
-  int *col_min, *col_max;          // W - 2 each
-  PolyResult* res;                 // followed directly by ring, so that one copy reads both
-  double2* ring;                   // 2 (W - 2) + 1 vertices at most
+  char* up;                        // upload region: poison counts, descriptors, clipped vertices (PolyStage)
+  PolyPartial* part;               // one per k_polygon work item
+  int *col_min, *col_max;          // the polygons' column windows, back to back
+  char* down;                      // read-back region: one PolyResult per polygon, then the rings (PolyStage)
 };
+
+// One call's layout of the upload and read-back regions, the same in device and in pinned host memory, so that each
+// region moves in one copy.  The two poison counts sit at offset 0 of the upload, the results at offset 0 of the read-back.
+struct PolyStage {
+  size_t desc, xy, up_bytes;
+  size_t ring, down_bytes;
+};
+
+PolyStage poly_stage(size_t n_poly, size_t n_vert, size_t ring_rows) {
+  PolyStage s;
+  s.desc = 16;
+  s.xy = s.desc + sizeof(PolyDesc) * n_poly;
+  s.up_bytes = s.xy + sizeof(float2) * n_vert;
+  s.ring = sizeof(PolyResult) * n_poly;
+  s.down_bytes = s.ring + sizeof(double2) * ring_rows;
+  return s;
+}
 
 dim3 polygon_grid(int W) { return dim3(cdiv(W, PG_COLS), cdiv(W, PG_ROWS)); }
 size_t ring_capacity(int W) { return 2 * (size_t)(W - 2) + 1; }
 
-size_t carve_polygon(int W, void* base, PolyScratch& s) {
-  const dim3 g = polygon_grid(W);
+size_t carve_polygon(const PolySizes& z, void* base, PolyScratch& s) {
   Carver b{(uintptr_t)base};
-  s.xy = b.take<float2>(EMAP_POLYGON_MAX_VERTICES);
-  s.part = b.take<PolyPartial>((size_t)g.x * g.y);
-  s.col_min = b.take<int>(W - 2);
-  s.col_max = b.take<int>(W - 2);
-  s.res = b.take<PolyResult>(1, 16);
-  s.ring = b.take<double2>(ring_capacity(W), 16);
+  s.up = b.take<char>(z.up);
+  s.part = b.take<PolyPartial>(z.items);
+  s.col_min = b.take<int>(z.cols);
+  s.col_max = b.take<int>(z.cols);
+  s.down = b.take<char>(z.down);
   return b.bytes;
 }
 
-int alloc_polygon_scratch(emap_handle* h, PolyScratch& s) {
-  const int W = h->dc.W;
-  if (!h->pg_host) {
-    CK(h->pg_block.alloc(carve_polygon(W, nullptr, s)));
-    carve_polygon(W, h->pg_block, s);
-    CK(cudaMemsetAsync(s.col_min, 0x7f, sizeof(int) * (W - 2), h->stream));    // "no cell yet": k_hull restores it
-    CK(cudaMemsetAsync(s.col_max, 0xff, sizeof(int) * (W - 2), h->stream));
-    CK(cudaMallocHost(&h->pg_host, sizeof(float2) * EMAP_POLYGON_MAX_VERTICES + sizeof(PolyResult) +
-                                        sizeof(double2) * ring_capacity(W)));
+// Carves the scratch of a call of sizes z, growing the device block and the pinned staging (upload region, then
+// read-back region) to the largest call so far.
+int alloc_polygon_scratch(emap_handle* h, const PolySizes& z, PolyScratch& s) {
+  PolySizes& c = h->pg_cap;
+  if (!h->pg_block || z.up > c.up || z.items > c.items || z.cols > c.cols || z.down > c.down) {
+    // the read-back region follows the upload region in pinned memory: keep it aligned for its double2 rings
+    c.up = std::max(c.up, (z.up + 255) & ~(size_t)255); c.items = std::max(c.items, z.items);
+    c.cols = std::max(c.cols, z.cols); c.down = std::max(c.down, z.down);
+    CK(h->pg_block.alloc(carve_polygon(c, nullptr, s)));
+    carve_polygon(c, h->pg_block, s);
+    CK(cudaMemsetAsync(s.col_min, 0x7f, sizeof(int) * c.cols, h->stream));    // "no cell yet": k_hull restores it
+    CK(cudaMemsetAsync(s.col_max, 0xff, sizeof(int) * c.cols, h->stream));
   }
-  carve_polygon(W, h->pg_block, s);
+  if (h->pg_host_bytes < c.up + c.down) {
+    if (h->pg_host) CK(cudaFreeHost(h->pg_host));
+    h->pg_host = nullptr; h->pg_host_bytes = 0;
+    CK(cudaMallocHost(&h->pg_host, c.up + c.down));
+    h->pg_host_bytes = c.up + c.down;
+  }
+  carve_polygon(c, h->pg_block, s);
   return 0;
+}
+
+// EM.py:847-854: each coordinate clipped to [center - map_length/2 + resolution, center + map_length/2 - resolution],
+// fp32 throughout; map_length is the map's true length (cell_n - 2) * resolution.  Writes the clipped vertices (unless
+// out is NULL) and their bounding box.
+void clip_polygon(const emap_handle* h, const float* xy, int n, float2* out, float bbox[4]) {
+  const float half = (float)(0.5 * (double)(h->dc.W - 2) * h->cfg.resolution), res_f = h->dc.res_f;
+  float lo[2], hi[2], bmin[2], bmax[2];
+  for (int k = 0; k < 2; k++) {
+    lo[k] = (h->center[k] - half) + res_f;
+    hi[k] = (h->center[k] + half) - res_f;
+  }
+  for (int i = 0; i < n; i++) {
+    float v[2];
+    for (int k = 0; k < 2; k++) {
+      v[k] = std::min(std::max(xy[2 * i + k], lo[k]), hi[k]);
+      bmin[k] = i ? std::min(bmin[k], v[k]) : v[k];
+      bmax[k] = i ? std::max(bmax[k], v[k]) : v[k];
+    }
+    if (out) out[i] = make_float2(v[0], v[1]);
+  }
+  bbox[0] = bmin[0]; bbox[1] = bmin[1]; bbox[2] = bmax[0]; bbox[3] = bmax[1];
+}
+
+// The tiles of k_polygon's grid that meet the polygon's cell bounding box (CK.py:609-615, the cells k_polygon tests)
+// and the interior columns of that box, the only ones that can hold its over-threshold cells.
+void polygon_tiles(const emap_handle* h, PolyDesc& d) {
+  const int W = h->dc.W;
+  const float rf = h->dc.res_f;
+  const int bx0 = poly_axis_cell(d.bbox[0], h->center[0], rf, W), bx1 = poly_axis_cell(d.bbox[2], h->center[0], rf, W);
+  const int by0 = poly_axis_cell(d.bbox[1], h->center[1], rf, W), by1 = poly_axis_cell(d.bbox[3], h->center[1], rf, W);
+  d.tr0 = bx0 / PG_ROWS; d.n_tr = bx1 / PG_ROWS - d.tr0 + 1;
+  d.tc0 = by0 / PG_COLS; d.n_tc = by1 / PG_COLS - d.tc0 + 1;
+  d.col0 = std::max(by0, 1) - 1;
+  d.n_col = std::max(0, std::min(by1, W - 2) - std::max(by0, 1) + 1);
 }
 
 // traversability_polygon.py:46-51 calculate_area on fp32 vertices: every operation in fp32, terms in order i = 0..n-1
@@ -828,6 +895,54 @@ float shoelace_f32(const float* xy, int n) {
     area = area + (a - b) / 2.0f;
   }
   return std::fabs(area);
+}
+
+// The device part of a call whose n_poly polygons (n_items work items) are staged in the upload region of h->pg_host:
+// one upload copy, k_poly_poison (with `poison`), k_polygon, k_hull, one copy of the results and the first `head` ring
+// rows into the read-back region of h->pg_host, one synchronisation; one more copy and synchronisation only if a ring
+// ends beyond `head`.
+int run_polygons(emap_handle* h, const PolyScratch& s, const PolyStage& st, int n_poly, int n_items, bool poison,
+                 const float* checker_plane, double safe_thresh, double safe_min_thresh, int32_t max_unsafe_n,
+                 float* mask, bool hulls, size_t head) {
+  const int W = h->dc.W;
+  const size_t C = (size_t)h->dc.C;
+  const dim3 g = polygon_grid(W);
+  const float* valid = h->map + L_VALID * C;
+  const float* checker = checker_plane ? checker_plane : h->map + L_TRAV * C;
+  PolyArgs a;
+  a.poly = (const PolyDesc*)(s.up + st.desc); a.n_poly = n_poly; a.xy = (const float2*)(s.up + st.xy);
+  a.cx = h->center[0]; a.cy = h->center[1];
+  a.thr_over = (float)(1.0 - safe_thresh); a.thr_max = (float)(1.0 - safe_min_thresh);    // traversability_polygon.py:25-26
+  a.max_unsafe_n = max_unsafe_n;
+  a.poison = poison ? (const int*)s.up : nullptr;
+  memcpy(&a.one, h->pg_host + st.desc, sizeof(PolyDesc));
+  CK(cudaMemcpyAsync(s.up, h->pg_host, st.up_bytes, cudaMemcpyHostToDevice, h->stream));
+  if (poison) {
+    k_poly_poison<<<std::min(cdiv((i64)C, 256), 4 * h->n_sm), 256, 0, h->stream>>>(W, valid, checker, (int*)s.up);
+    LAUNCH_CHECK();
+  }
+  (poison ? k_polygon<true> : k_polygon<false>)<<<n_items, PG_THREADS, 0, h->stream>>>(
+      W, h->dc.res_f, a, valid, checker, mask, s.part, hulls ? s.col_min : nullptr, hulls ? s.col_max : nullptr);
+  LAUNCH_CHECK();
+  k_hull<<<n_poly, HULL_THREADS, 0, h->stream>>>(W, h->cfg.resolution, a, (int)g.x, (int)g.y, s.part, s.col_min,
+                                                 s.col_max, (PolyResult*)s.down,
+                                                 hulls ? (double2*)(s.down + st.ring) : nullptr);
+  LAUNCH_CHECK();
+  char* back = h->pg_host + h->pg_cap.up;
+  head = std::min(head, (st.down_bytes - st.ring) / sizeof(double2));
+  CK(cudaMemcpyAsync(back, s.down, st.ring + sizeof(double2) * head, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  const PolyResult* r = (const PolyResult*)back;
+  const PolyDesc* d = (const PolyDesc*)(h->pg_host + st.desc);
+  size_t end = 0;
+  for (int i = 0; i < n_poly; i++)
+    if (r[i].n_ring) end = std::max(end, (size_t)d[i].ring_off + r[i].n_ring);
+  if (end > head) {
+    const size_t off = st.ring + sizeof(double2) * head;
+    CK(cudaMemcpyAsync(back + off, s.down + off, sizeof(double2) * (end - head), cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+  }
+  return EMAP_OK;
 }
 
 // ---- features_pca ------------------------------------------------------------------------------
@@ -1404,8 +1519,9 @@ int emap_exists_layer(const emap_handle* h, const char* name) {
   return layer_index(name) >= 0 ? 1 : 0;
 }
 
-// EM.py:837-889 get_polygon_traversability (WRAP:254-281): area, clip and bounding box on the host in fp32, then
-// k_polygon + k_hull, one device-to-host copy and one synchronisation.
+// EM.py:837-889 get_polygon_traversability (WRAP:254-281): area, clip and bounding box on the host in fp32, then a
+// batch of one polygon whose work items are every tile of the grid (the mask is written everywhere, and the statistics
+// need no poison pass), one device-to-host copy and one synchronisation.
 int emap_polygon_traversability(emap_handle* h, const float* polygon_xy, int32_t n_vertices, const float* checker_plane,
                                 double safe_thresh, double safe_min_thresh, int32_t max_unsafe_n, double result[3],
                                 double* hull_xy, int32_t* n_hull, float* mask) {
@@ -1415,56 +1531,29 @@ int emap_polygon_traversability(emap_handle* h, const float* polygon_xy, int32_t
   if (n_vertices < 3 || n_vertices > EMAP_POLYGON_MAX_VERTICES)
     return fail(h, EMAP_ERR_INVALID, "emap_polygon_traversability: 3 to EMAP_POLYGON_MAX_VERTICES vertices required");
   const int W = h->dc.W;
-  const size_t C = (size_t)h->dc.C;
+  const dim3 g = polygon_grid(W);
+  const PolyStage st = poly_stage(1, n_vertices, ring_capacity(W));
+  PolySizes z;
+  z.up = st.up_bytes; z.items = (size_t)g.x * g.y; z.cols = W - 2; z.down = st.down_bytes;
   PolyScratch s;
-  int rc = alloc_polygon_scratch(h, s);
+  int rc = alloc_polygon_scratch(h, z, s);
   if (rc) return rc;
   const float area = shoelace_f32(polygon_xy, n_vertices);
-  // EM.py:847-854: each coordinate clipped to [center - map_length/2 + resolution, center + map_length/2 - resolution],
-  // fp32 throughout; map_length is the map's true length (cell_n - 2) * resolution
-  const float half = (float)(0.5 * (double)(W - 2) * h->cfg.resolution), res_f = h->dc.res_f;
-  float lo[2], hi[2], bmin[2], bmax[2];
-  for (int k = 0; k < 2; k++) {
-    lo[k] = (h->center[k] - half) + res_f;
-    hi[k] = (h->center[k] + half) - res_f;
-  }
-  float2* xy = (float2*)h->pg_host;
-  for (int i = 0; i < n_vertices; i++) {
-    float v[2];
-    for (int k = 0; k < 2; k++) {
-      v[k] = std::min(std::max(polygon_xy[2 * i + k], lo[k]), hi[k]);
-      bmin[k] = i ? std::min(bmin[k], v[k]) : v[k];
-      bmax[k] = i ? std::max(bmax[k], v[k]) : v[k];
-    }
-    xy[i] = make_float2(v[0], v[1]);
-  }
+  PolyDesc d = {};
+  float2* xy = (float2*)(h->pg_host + st.xy);
+  clip_polygon(h, polygon_xy, n_vertices, xy, d.bbox);
   const float clipped_area = shoelace_f32((const float*)xy, n_vertices);
-  PolyArgs a;
-  a.xy = s.xy; a.n = n_vertices; a.cx = h->center[0]; a.cy = h->center[1];
-  a.bbox[0] = bmin[0]; a.bbox[1] = bmin[1]; a.bbox[2] = bmax[0]; a.bbox[3] = bmax[1];
-  a.thr_over = (float)(1.0 - safe_thresh); a.thr_max = (float)(1.0 - safe_min_thresh);    // traversability_polygon.py:25-26
-  a.max_unsafe_n = max_unsafe_n;
-  CK(cudaMemcpyAsync(s.xy, xy, sizeof(float2) * n_vertices, cudaMemcpyHostToDevice, h->stream));
-  const dim3 grid = polygon_grid(W);
-  k_polygon<<<grid, PG_THREADS, 0, h->stream>>>(W, res_f, a, h->map + L_VALID * C,
-                                                checker_plane ? checker_plane : h->map + L_TRAV * C, mask, s.part,
-                                                s.col_min, s.col_max);
-  LAUNCH_CHECK();
-  k_hull<<<1, HULL_THREADS, 0, h->stream>>>(W, h->cfg.resolution, a, s.part, (int)(grid.x * grid.y), s.col_min, s.col_max,
-                                            s.res, s.ring);
-  LAUNCH_CHECK();
-  char* back = h->pg_host + sizeof(float2) * EMAP_POLYGON_MAX_VERTICES;
-  const size_t head = std::min((size_t)kRingHead, ring_capacity(W));
-  CK(cudaMemcpyAsync(back, s.res, sizeof(PolyResult) + sizeof(double2) * head, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  d.v0 = 0; d.n = n_vertices; d.item0 = 0;
+  d.tr0 = 0; d.tc0 = 0; d.n_tr = g.y; d.n_tc = g.x;
+  d.col0 = 0; d.n_col = W - 2; d.col_off = 0; d.ring_off = 0;
+  memcpy(h->pg_host + st.desc, &d, sizeof(d));
+  rc = run_polygons(h, s, st, 1, (int)z.items, false, checker_plane, safe_thresh, safe_min_thresh, max_unsafe_n, mask,
+                    true, kRingHead);
+  if (rc) return rc;
+  const char* back = h->pg_host + h->pg_cap.up;
   PolyResult r;
   memcpy(&r, back, sizeof(r));
-  const double2* ring = (const double2*)(back + sizeof(PolyResult));
-  if (r.n_ring > (int)head) {
-    CK(cudaMemcpyAsync(back + sizeof(PolyResult) + sizeof(double2) * head, s.ring + head,
-                       sizeof(double2) * (r.n_ring - head), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-  }
+  const double2* ring = (const double2*)(back + st.ring);
   // EM.py:884-887: a polygon (almost) entirely outside the map is unsafe
   result[0] = (r.is_safe && !(clipped_area < 0.001f)) ? 1.0 : 0.0;
   result[1] = r.t;
@@ -1475,6 +1564,101 @@ int emap_polygon_traversability(emap_handle* h, const float* polygon_xy, int32_t
   }
   for (int k = 0; k < r.n_ring; k++) { hull_xy[2 * k] = ring[k].x; hull_xy[2 * k + 1] = ring[k].y; }
   *n_hull = r.n_ring;
+  return EMAP_OK;
+}
+
+// The check_safety service (CheckSafety.srv) in one call: every polygon's answer is emap_polygon_traversability's.  The
+// work items are only the tiles of each polygon's cell bounding box; k_poly_poison carries the map-wide NaN rule to
+// the cells outside them.  One upload, one read-back copy and one synchronisation (plus one for long rings).
+int emap_polygon_traversability_batch(emap_handle* h, int32_t n_polygons, const int32_t* n_vertices,
+                                      const float* polygon_xy, const float* checker_plane, double safe_thresh,
+                                      double safe_min_thresh, int32_t max_unsafe_n, double* results, double* hull_xy,
+                                      int64_t* hull_offsets, int64_t* hull_rows) {
+  ENTER(h);
+  if (n_polygons < 1 || n_polygons > EMAP_POLYGON_MAX_BATCH)
+    return fail(h, EMAP_ERR_INVALID, "emap_polygon_traversability_batch: 1 to EMAP_POLYGON_MAX_BATCH polygons required");
+  if (!n_vertices || !polygon_xy || !results || (hull_xy && (!hull_offsets || !hull_rows)) ||
+      (hull_rows && *hull_rows < 0))
+    return fail(h, EMAP_ERR_INVALID, "emap_polygon_traversability_batch: null argument or negative hull capacity");
+  size_t n_vert = 0;
+  for (int i = 0; i < n_polygons; i++) {
+    if (n_vertices[i] < 3 || n_vertices[i] > EMAP_POLYGON_MAX_VERTICES)
+      return fail(h, EMAP_ERR_INVALID,
+                  "emap_polygon_traversability_batch: 3 to EMAP_POLYGON_MAX_VERTICES vertices required per polygon");
+    n_vert += n_vertices[i];
+  }
+  const bool hulls = hull_xy != nullptr;
+  // traversability_polygon.py:25 compares the whole interior: with fp32(1 - safe_thresh) < 0 the masked 0 of every cell
+  // outside a polygon is over too, so its count and hull take the whole map.  Every polygon then brings every tile and
+  // the whole column window, as the single call does.
+  const bool whole_map = (float)(1.0 - safe_thresh) < 0.0f;
+  const dim3 g = polygon_grid(h->dc.W);
+  // each polygon's tiles (its work items and partials), column window and ring slot
+  std::vector<PolyDesc> desc(n_polygons);
+  size_t items = 0, cols = 0, rows = 0, v0 = 0;
+  for (int i = 0; i < n_polygons; i++) {
+    PolyDesc& d = desc[i];
+    clip_polygon(h, polygon_xy + 2 * v0, n_vertices[i], nullptr, d.bbox);
+    polygon_tiles(h, d);
+    if (whole_map) {
+      d.tr0 = 0; d.tc0 = 0; d.n_tr = g.y; d.n_tc = g.x;
+      d.col0 = 0; d.n_col = h->dc.W - 2;
+    }
+    if (!hulls) d.n_col = 0;
+    d.v0 = (int)v0; d.n = n_vertices[i]; d.item0 = (int)items; d.col_off = (int)cols; d.ring_off = (int)rows;
+    items += (size_t)d.n_tr * d.n_tc;
+    cols += d.n_col;
+    rows += d.n_col ? 2 * (size_t)d.n_col + 1 : 0;
+    v0 += n_vertices[i];
+  }
+  const PolyStage st = poly_stage(n_polygons, n_vert, rows);
+  PolySizes z;
+  z.up = st.up_bytes; z.items = items; z.cols = cols; z.down = st.down_bytes;
+  PolyScratch s;
+  int rc = alloc_polygon_scratch(h, z, s);
+  if (rc) return rc;
+  memset(h->pg_host, 0, st.desc);                                   // the poison counts start at zero
+  memcpy(h->pg_host + st.desc, desc.data(), sizeof(PolyDesc) * n_polygons);
+  float2* xy = (float2*)(h->pg_host + st.xy);
+  std::vector<float> area(n_polygons), clipped_area(n_polygons);
+  for (int i = 0; i < n_polygons; i++) {
+    const PolyDesc& d = desc[i];
+    area[i] = shoelace_f32(polygon_xy + 2 * (size_t)d.v0, d.n);
+    float bbox[4];
+    clip_polygon(h, polygon_xy + 2 * (size_t)d.v0, d.n, xy + d.v0, bbox);
+    clipped_area[i] = shoelace_f32((const float*)(xy + d.v0), d.n);
+  }
+  rc = run_polygons(h, s, st, n_polygons, (int)items, true, checker_plane, safe_thresh, safe_min_thresh, max_unsafe_n,
+                    nullptr, hulls, kBatchRingHead);
+  if (rc) return rc;
+  const char* back = h->pg_host + h->pg_cap.up;
+  const PolyResult* r = (const PolyResult*)back;
+  const double2* ring = (const double2*)(back + st.ring);
+  int64_t total = 0;
+  for (int i = 0; i < n_polygons; i++) {
+    // EM.py:884-887: a polygon (almost) entirely outside the map is unsafe
+    results[3 * i] = (r[i].is_safe && !(clipped_area[i] < 0.001f)) ? 1.0 : 0.0;
+    results[3 * i + 1] = r[i].t;
+    results[3 * i + 2] = (double)area[i];
+    if (hull_offsets) hull_offsets[i] = total;
+    total += r[i].n_ring;
+  }
+  if (hull_offsets) hull_offsets[n_polygons] = total;
+  if (!hulls) {
+    if (hull_rows) *hull_rows = 0;
+    return EMAP_OK;
+  }
+  if (total > *hull_rows) {
+    *hull_rows = total;
+    return fail(h, EMAP_ERR_INVALID,
+                "emap_polygon_traversability_batch: hull capacity too small (needed rows in *hull_rows)");
+  }
+  for (int i = 0; i < n_polygons; i++) {
+    const double2* src = ring + desc[i].ring_off;
+    double* dst = hull_xy + 2 * hull_offsets[i];
+    for (int k = 0; k < r[i].n_ring; k++) { dst[2 * k] = src[k].x; dst[2 * k + 1] = src[k].y; }
+  }
+  *hull_rows = total;
   return EMAP_OK;
 }
 

@@ -9,7 +9,8 @@ happens in the library; this module only marshals arguments.  Device arrays are 
 CUDA tensors that alias the library's memory (they also expose `__cuda_array_interface__`).
 
 Point-cloud semantic layers (average / class_average / color fusion) are fused inside the frame (semantic_map.py).
-The polygon safety check (get_polygon_traversability) is one library call: mask, statistics and hull on the device.
+The polygon safety check (get_polygon_traversability) is one library call: mask, statistics and hull on the device;
+get_polygons_traversability checks a batch of polygons in one call.
 Out of scope (SURVEY.md section 8): image input, image / bayesian semantic fusion.
 """
 import ctypes as C
@@ -103,6 +104,7 @@ class ElevationMap:
         self.untraversable_polygon = np.zeros((1, 2))
         self._ring = np.zeros((2 * (self.cell_n - 2) + 1, 2), np.float64)
         self._mask = None
+        self._batch_hull = np.zeros((4096, 2), np.float64)      # rings of get_polygons_traversability, grown on demand
 
     # ---- plumbing -------------------------------------------------------------------------
     def _check(self, rc):
@@ -439,6 +441,46 @@ class ElevationMap:
         result[...] = res
         self.untraversable_polygon = self._ring[:n_ring.value].copy()
         return n_ring.value
+
+    def get_polygons_traversability(self, polygons, results, compute_untraversable_polygon=True):
+        """The check_safety service (CheckSafety.srv) in one library call: row i of the (B, 3) float64 `results` gets what
+        get_polygon_traversability writes for polygons[i] (an (n_i, 2) array of any framework, cast to float32), and
+        the returned list holds polygon i's untraversable ring as a float64 (n, 2) array ((0, 2) if none, and for every
+        polygon when compute_untraversable_polygon is False).  self.mask and the single call's ring are left as they were."""
+        polys = [np.ascontiguousarray(_to_host(p), dtype=np.float32).reshape(-1, 2) for p in polygons]
+        n_vert = np.array([len(p) for p in polys], np.int32)
+        xy = np.ascontiguousarray(np.concatenate(polys) if polys else np.zeros((0, 2), np.float32))
+        checker = None
+        if self.param.checker_layer != "traversability":
+            checker = self.get_layer(self.param.checker_layer)     # None: the layer is absent, traversability is used
+        B = len(polys)
+        res = np.zeros((B, 3), np.float64)
+        offsets = np.zeros(B + 1, np.int64)
+        rows = C.c_int64(0)
+        hull = None
+        with self.map_lock:
+            self._after_framework()
+            while True:
+                if compute_untraversable_polygon:
+                    hull = self._batch_hull
+                    rows.value = len(hull)
+                rc = self._L.emap_polygon_traversability_batch(
+                    self._h, B, n_vert.ctypes.data, xy.ctypes.data, None if checker is None else checker.data_ptr(),
+                    float(self.param.safe_thresh), float(self.param.safe_min_thresh), int(self.param.max_unsafe_n),
+                    res.ctypes.data, None if hull is None else hull.ctypes.data, offsets.ctypes.data, C.byref(rows))
+                if rc == -1 and hull is not None and rows.value > len(hull):
+                    self._batch_hull = np.zeros((rows.value, 2), np.float64)     # same map state, same answer
+                    continue
+                self._check(rc)
+                break
+        center = self.center
+        for p in polys:
+            if _clipped_area(p, center, self.cell_n, self.resolution) < np.float32(0.001):
+                print("requested polygon is outside of the map")
+        results[...] = res
+        if hull is None:
+            return [np.zeros((0, 2), np.float64) for _ in polys]
+        return [hull[offsets[i]:offsets[i + 1]].copy() for i in range(B)]
 
     def get_untraversable_polygon(self, untraversable_polygon):
         """EM.py:891-897: copy the ring of the last get_polygon_traversability into the caller's (n, 2) array."""

@@ -226,6 +226,22 @@ int emap_polygon_traversability(emap_handle* h, const float* polygon_xy, int32_t
                                 const float* checker_plane_device, double safe_thresh, double safe_min_thresh,
                                 int32_t max_unsafe_n, double result[3], double* hull_xy, int32_t* n_hull,
                                 float* mask_device);
+/* A batch of polygons in one call (CheckSafety.srv's polygons[], is_safe[], traversability[], untraversable_polygons[]).
+ * Polygon i has n_vertices[i] vertices (3 to EMAP_POLYGON_MAX_VERTICES); polygon_xy holds all of them as (x, y) fp32
+ * pairs, back to back.  results[3i .. 3i + 2] and ring i are what emap_polygon_traversability returns for polygon i
+ * on the same map.  hull_xy NULL: no hulls (every ring is empty, less device work); hull_offsets and hull_rows may then
+ * be NULL too.  Otherwise ring i is rows [hull_offsets[i], hull_offsets[i + 1]) of hull_xy ((x, y) doubles) and
+ * *hull_rows is the capacity in rows on entry and the total on return; a capacity below the total returns
+ * EMAP_ERR_INVALID with the needed total in *hull_rows (results and hull_offsets are written).  No mask is written.
+ * One host-to-device copy, one device-to-host copy and one synchronisation per call (one more of each of the last two
+ * when the rings are long).  The work is proportional to the polygons' bounding boxes plus one pass over the map,
+ * except when fp32(1 - safe_thresh) < 0: every cell outside a polygon is then over-threshold too, and every polygon
+ * takes the whole map, as the single call does. */
+#define EMAP_POLYGON_MAX_BATCH 4096
+int emap_polygon_traversability_batch(emap_handle* h, int32_t n_polygons, const int32_t* n_vertices,
+                                      const float* polygon_xy, const float* checker_plane_device, double safe_thresh,
+                                      double safe_min_thresh, int32_t max_unsafe_n, double* results, double* hull_xy,
+                                      int64_t* hull_offsets, int64_t* hull_rows);
 
 /* ---- plugin stencils on device planes (W,W fp32); replace the CuPy / OpenCV / cupyx bodies of
  * plugins/min_filter.py:57-118, plugins/smooth_filter.py:57-58, plugins/inpainting.py:53-63 ---- */
