@@ -93,6 +93,9 @@ SIGNATURES = {
     "emap_semantic_filter": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
     "emap_semantic_traversability": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "emap_features_pca": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]),
+    "emap_input_image": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                   C.c_int32, C.c_char_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_int32]),
     "emap_polygon_traversability": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_void_p, C.c_double, C.c_double,
                                               C.c_int32, C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.c_void_p]),
     "emap_polygon_traversability_batch": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -17,6 +17,7 @@
 #include "emap_semantic.cuh"
 #include "emap_polygon.cuh"
 #include "emap_semantic_plugins.cuh"
+#include "emap_image.cuh"
 
 namespace {
 
@@ -146,6 +147,12 @@ struct emap_handle {
   size_t pg_host_bytes = 0;
   // features_pca scratch (allocated on first use): one device block carved by carve_pca
   DevBuf<char> pca_block;
+  // emap_input_image with a host image (allocated on first use, grown to the largest image): pinned staging, the device
+  // copy the kernel reads, and the event after which the staging may be overwritten
+  DevBuf<float> img_dev;
+  float* img_host = nullptr;
+  size_t img_host_n = 0;
+  cudaEvent_t img_staged = nullptr;
   // misc
   int64_t launches = 0;
   int count_rays = 0;
@@ -1119,6 +1126,8 @@ emap_handle::~emap_handle() {
   if (own_stream) cudaStreamDestroy(own_stream);
   if (copy_stream) cudaStreamDestroy(copy_stream);
   if (pg_host) cudaFreeHost(pg_host);
+  if (img_staged) { cudaEventSynchronize(img_staged); cudaEventDestroy(img_staged); }
+  if (img_host) cudaFreeHost(img_host);
 }
 
 extern "C" {
@@ -1838,6 +1847,67 @@ int emap_features_pca(emap_handle* h, int32_t n_features, const float* const* pl
   CK(cudaMemcpyAsync(&nan, &s.res->nan, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
   if (nan) return fail(h, EMAP_ERR_INVALID, "emap_features_pca: NaN in the input features");
+  return EMAP_OK;
+}
+
+// EM.py:468-562 input_image + semantic_map.py:261-309 update_layers_image: the host part (image_camera) and one
+// k_image_fuse launch.  A host image is copied into pinned staging and from there, once, to the device; a device image
+// is read in place, with no host synchronisation.
+int emap_input_image(emap_handle* h, int32_t n_planes, const float* image, int is_device_ptr, int32_t height, int32_t width,
+                     const float K[9], const float* D, int32_t n_D, const char* distortion_model, const float R[9],
+                     const float t[3], int32_t n_fused, const int32_t* plane, const int32_t* kind, const int32_t* layer,
+                     float* semantic_map_device, int32_t n_layers) {
+  ENTER(h);
+  NvtxRange nv("emap:input_image");
+  if (!image || !K || !R || !t || !distortion_model || (n_D > 0 && !D) || n_D < 0 ||
+      (n_fused > 0 && (!plane || !kind || !layer || !semantic_map_device)))
+    return fail(h, EMAP_ERR_INVALID, "emap_input_image: null argument");
+  if (n_planes < 1 || height < 1 || width < 1 || (int64_t)height * width > (1ll << 24))
+    return fail(h, EMAP_ERR_INVALID, "emap_input_image: n_planes >= 1 and 1 <= height * width <= 2^24 required");
+  if (n_fused < 0 || n_fused > EMAP_IMAGE_MAX_CHANNELS)
+    return fail(h, EMAP_ERR_INVALID, "emap_input_image: 0 to EMAP_IMAGE_MAX_CHANNELS fused channels required");
+  ImageArgs a;
+  memset(&a, 0, sizeof(a));
+  for (int k = 0; k < n_fused; k++) {
+    if (kind[k] != EMAP_IMAGE_COLOR && kind[k] != EMAP_IMAGE_EXPONENTIAL)
+      return fail(h, EMAP_ERR_INVALID, "emap_input_image: kind must be EMAP_IMAGE_COLOR or EMAP_IMAGE_EXPONENTIAL");
+    if (plane[k] < 0 || plane[k] >= n_planes || (kind[k] == EMAP_IMAGE_COLOR && n_planes < 3))
+      return fail(h, EMAP_ERR_INVALID, "emap_input_image: plane outside the image, or a colour channel with fewer than 3 planes");
+    if (layer[k] < 0 || layer[k] >= n_layers)
+      return fail(h, EMAP_ERR_INVALID, "emap_input_image: layer outside [0, n_layers)");
+    a.plane[k] = plane[k];
+    a.kind[k] = kind[k] == EMAP_IMAGE_COLOR ? IMG_COLOR : IMG_EXPONENTIAL;
+    a.layer[k] = layer[k];
+  }
+  const int cam = image_camera(K, D, n_D, distortion_model, R, t, h->center, h->dc.W, h->cfg.resolution, &a.cam);
+  if (cam == IMG_CAM_NONFINITE) return fail(h, EMAP_ERR_INVALID, "emap_input_image: non-finite K, R or t");
+  if (cam == IMG_CAM_OUTSIDE)
+    return fail(h, EMAP_ERR_INVALID, "emap_input_image: camera cell cell_n / 2 + t / resolution outside [0, 2^24)");
+  if (n_fused == 0) return EMAP_OK;       // the correspondence alone changes nothing
+  const size_t plane_sz = (size_t)height * width, n_img = plane_sz * n_planes;
+  const float* img = image;
+  if (!is_device_ptr) {
+    int rc = grow(h, h->img_dev, n_img, 0, false);
+    if (rc) return rc;
+    if (!h->img_staged) CK(cudaEventCreateWithFlags(&h->img_staged, cudaEventDisableTiming));
+    else CK(cudaEventSynchronize(h->img_staged));         // the previous image has left the staging
+    if (h->img_host_n < n_img) {
+      if (h->img_host) { cudaFreeHost(h->img_host); h->img_host = nullptr; h->img_host_n = 0; }
+      CK(cudaHostAlloc((void**)&h->img_host, sizeof(float) * n_img, cudaHostAllocDefault));
+      h->img_host_n = n_img;
+    }
+    memcpy(h->img_host, image, sizeof(float) * n_img);   // the caller's buffer is free from here on
+    CK(cudaMemcpyAsync(h->img_dev, h->img_host, sizeof(float) * n_img, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaEventRecord(h->img_staged, h->stream));
+    img = h->img_dev;
+  }
+  for (int k = 0; k < 3; k++) a.center[k] = h->center[k];
+  a.res = h->cfg.resolution;
+  a.W = h->dc.W; a.C = h->dc.C;
+  a.img_w = (float)width; a.img_h = (float)height;
+  a.n_img = (long long)n_img; a.plane_sz = (long long)plane_sz;
+  a.image = img; a.sem = semantic_map_device; a.n = n_fused;
+  PER_CELL(k_image_fuse, a, (const float*)h->map);
   return EMAP_OK;
 }
 

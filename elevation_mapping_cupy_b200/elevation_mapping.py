@@ -11,7 +11,10 @@ CUDA tensors that alias the library's memory (they also expose `__cuda_array_int
 Point-cloud semantic layers (average / class_average / color fusion) are fused inside the frame (semantic_map.py).
 The polygon safety check (get_polygon_traversability) is one library call: mask, statistics and hull on the device;
 get_polygons_traversability checks a batch of polygons in one call.
-Out of scope (SURVEY.md section 8): image input, image / bayesian semantic fusion.
+Camera images (input_image) fuse into the semantic layers with the reference's `color` and `exponential` image fusions:
+one kernel projects every map cell into the image, tests occlusion along the line to the camera and writes every fused
+channel (csrc/emap_image.cuh), bit-identical to the reference's kernels on the same card.
+Out of scope (SURVEY.md section 8): bayesian semantic fusion and the image feature extractors.
 """
 import ctypes as C
 import threading
@@ -414,9 +417,36 @@ class ElevationMap:
         self._check(self._L.emap_get_stage_ms(self._h, out.ctypes.data))
         return out
 
+    def input_image(self, image, channels: List[str], R, t, K, D, distortion_model: str, image_height: int,
+                    image_width: int):
+        """EM.py:468-562 (WRAP:180-185): fuse a camera image into the semantic layers.  `image` is a list of (H, W) arrays
+        or a (C, H, W) array of any framework, host or device; channel j of the processed channel list reads plane j.
+        R, t: map -> camera optical frame; K: 3x3 intrinsics; D: distortion coefficients, used for "radtan" only.
+        One library call, one kernel (semantic_map.py update_layers_image picks the fusions and layers)."""
+        dev, img = _image_stack(image, self.device)
+        n_planes, H, W = img.shape
+        if (H, W) != (int(image_height), int(image_width)):
+            raise ValueError(f"image is {H}x{W}, image_height x image_width is {image_height}x{image_width}")
+        f32 = lambda x, n: np.ascontiguousarray(_to_host(x), dtype=np.float32).reshape(n)
+        Rm, tv, Km = f32(R, 9), f32(t, 3), f32(K, 9)
+        Dv = np.ascontiguousarray(_to_host(D), dtype=np.float32).reshape(-1)
+        with self.map_lock:
+            planes, kinds, layers = self.semantic_map.update_layers_image(list(channels))
+            n = len(planes)
+            arr = lambda v: (C.c_int32 * max(n, 1))(*v)
+            sem = self.semantic_map.semantic_map
+            self._after_framework()       # the stacked image and any layer the channels added are complete
+            rc = self._L.emap_input_image(
+                self._h, n_planes, img.data_ptr() if dev else img.ctypes.data, int(dev), H, W, Km.ctypes.data,
+                Dv.ctypes.data if Dv.size else None, int(Dv.size), str(distortion_model).encode(), Rm.ctypes.data,
+                tv.ctypes.data, n, arr(planes), arr(kinds), arr(layers), None if sem is None else sem.data_ptr(),
+                len(self.semantic_map.layer_names))
+            # framework work queued from here on sees the fused layers, and releases or rewrites a device image only after
+            # the kernel has read it (no host sync)
+            self._before_framework()
+            self._check(rc)
+
     # ---- not on the per-frame path ---------------------------------------------------------------
-    def input_image(self, *a, **k):
-        raise NotImplementedError("image input is outside the fusion path (SURVEY.md section 8)")
 
     def get_polygon_traversability(self, polygon, result):
         """EM.py:837-889: is the (N, 2) polygon (any array framework, cast to float32 as the C++ bridge passes it) safe to
@@ -532,6 +562,31 @@ def _to_host(x):
     if hasattr(x, "get"):                                # cupy array
         return x.get()
     return np.asarray(x)
+
+
+def _is_device(x):
+    return getattr(x, "__cuda_array_interface__", None) is not None if not hasattr(x, "is_cuda") else bool(x.is_cuda)
+
+
+def _image_stack(image, device):
+    """(on_device, contiguous fp32 (C, H, W) array) of an input_image image (EM.py:504-509: np.stack, then a 2-D result
+    gets a leading axis).  Device input stays on the device (a torch tensor); host input becomes a NumPy array."""
+    parts = list(image) if isinstance(image, (list, tuple)) else None
+    if any(_is_device(x) for x in (parts if parts is not None else [image])):
+        import torch
+        as_t = lambda x: torch.as_tensor(x, device=f"cuda:{device}")
+        img = torch.stack([as_t(x) for x in parts]) if parts is not None else as_t(image)
+        if img.dim() == 2:
+            img = img[None]
+        if img.dim() != 3:
+            raise ValueError("image must be (C, H, W) or a list of (H, W) planes")
+        return True, img.to(torch.float32).contiguous()
+    img = np.stack([_to_host(x) for x in parts]) if parts is not None else _to_host(image)
+    if img.ndim == 2:
+        img = img[None]
+    if img.ndim != 3:
+        raise ValueError("image must be (C, H, W) or a list of (H, W) planes")
+    return False, np.ascontiguousarray(img, dtype=np.float32)
 
 
 def _clipped_area(poly, center, cell_n, resolution):

@@ -25,7 +25,7 @@ class Parameter:
     additional_layers: list = field(default_factory=list)
     fusion_algorithms: list = field(default_factory=list)
     pointcloud_channel_fusions: dict = field(default_factory=lambda: {"rgb": "color", "default": "class_average"})  # parameter.py:160
-    image_channel_fusions: dict = field(default_factory=dict)
+    image_channel_fusions: dict = field(default_factory=lambda: {"rgb": "color", "default": "exponential"})  # parameter.py:161
     data_type: str = np.float32
     average_weight: float = 0.5
 

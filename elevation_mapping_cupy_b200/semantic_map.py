@@ -7,7 +7,12 @@ frame's point record: `average` (fusion/pointcloud_average.py), `class_average` 
 reference's default) and `color` (fusion/pointcloud_color.py).  The kernels are csrc/emap_semantic.cuh; this class only
 decides which column of the cloud goes to which layer and hands the layer buffer to the engine
 (`emap_semantic_configure`).  The plugins that consume these layers (semantic_filter, semantic_traversability,
-features_pca) are in plugins/.  Image fusion, bayesian / class-max fusion and the image feature extractors are out of scope.
+features_pca) are in plugins/.
+Camera images (ElevationMap.input_image) fuse into the same layers: `update_layers_image` picks each channel's fusion
+(`image_channel_fusions`: `color`, fusion/image_color.py, or `exponential`, fusion/image_exponential.py) and layer, and
+one library call (`emap_input_image`, csrc/emap_image.cuh) projects, tests occlusion and writes every channel.  A layer
+an image adds reallocates the buffer; the point-channel registration is moved to the new buffer at once.
+Bayesian / class-max fusion and the image feature extractors are out of scope.
 """
 import ctypes as C
 import re
@@ -16,6 +21,7 @@ from typing import Dict, List
 import numpy as np
 
 KINDS = {"average": 0, "class_average": 1, "color": 2}
+IMAGE_KINDS = {"color": 0, "exponential": 1}          # EMAP_IMAGE_COLOR, EMAP_IMAGE_EXPONENTIAL
 
 
 class SemanticMap:
@@ -23,9 +29,11 @@ class SemanticMap:
         self.param = param
         self.engine = engine
         self.layer_specs_points: Dict[str, str] = {}
+        self.layer_specs_image: Dict[str, str] = {}
         self.layer_names: List[str] = []
         self.semantic_map = None           # torch (n_layers, W, W) float32 on the engine's device, grown by add_layer
         self._configured = None
+        self._registered = None            # (columns, kinds, layers) the engine fuses point channels with, or None
         self.elements_to_shift = {}
 
     # ---- layer bookkeeping (semantic_map.py:47-99) ----------------------------------------------------------------
@@ -44,8 +52,13 @@ class SemanticMap:
             return
         self.layer_names.append(name)
         new = self._alloc(1)
-        self.semantic_map = new if self.semantic_map is None else torch.cat([self.semantic_map, new], 0)
-        self._configured = None            # the buffer moved: re-register with the engine
+        if self.semantic_map is None:
+            self.semantic_map = new
+        else:
+            self.engine._before_framework()        # the engine's queued writes to the old buffer come first
+            self.semantic_map = torch.cat([self.semantic_map, new], 0)
+        if self._registered is not None:           # the old buffer is freed: point the engine's fusion at the new one
+            self._register(*self._registered)
 
     def get_matching_fusion(self, channel: str, fusion_algs: Dict[str, str]):
         for pattern, alg in fusion_algs.items():          # semantic_map.py:186-191
@@ -79,9 +92,8 @@ class SemanticMap:
         key = tuple(channels)
         if self._configured == key:
             return
-        eng = self.engine
         if not feats:
-            eng._check(eng._L.emap_semantic_configure(eng._h, 0, None, None, None, None, 0, 0.0))
+            self._register(None)
             self._configured = key
             return
         fusions = getattr(self.param, "pointcloud_channel_fusions", None) or {"rgb": "color", "default": "class_average"}
@@ -94,16 +106,40 @@ class SemanticMap:
                 print(f"Layer {ch} not found, adding it to the semantic map")
                 self.add_layer(ch)
             cols.append(3 + feats.index(ch)); kinds.append(KINDS[alg]); layers.append(self.layer_names.index(ch))
-        n = len(cols)
-        if n == 0:                          # no channel has a fusion: nothing to fuse
+        self._register(cols, kinds, layers)        # no channel has a fusion: nothing to fuse
+        self._configured = tuple(channels)
+
+    def _register(self, cols, kinds=None, layers=None):
+        """Hands the point-channel fusion (or None: no fusion) and the current layer buffer to the engine."""
+        eng = self.engine
+        if not cols:
             eng._check(eng._L.emap_semantic_configure(eng._h, 0, None, None, None, None, 0, 0.0))
-            self._configured = key
+            self._registered = None
             return
+        n = len(cols)
         arr = lambda v: (C.c_int32 * n)(*v)
         eng._check(eng._L.emap_semantic_configure(eng._h, n, arr(cols), arr(kinds), arr(layers),
                                                   C.c_void_p(self.semantic_map.data_ptr()), len(self.layer_names),
                                                   float(getattr(self.param, "average_weight", 0.5))))
-        self._configured = tuple(channels)
+        self._registered = (cols, kinds, layers)
+
+    # ---- the image hook (semantic_map.py:261-309) ----------------------------------------------------------------------
+    def update_layers_image(self, channels: List[str]):
+        """The channel selection of update_layers_image: (planes, kinds, layers) of the channels the image fuses.  Channel j
+        of the processed list reads image plane j; a missing layer is added; a fusion other than color / exponential
+        prints the reference's warning and is skipped (its layer is still added)."""
+        fusions = getattr(self.param, "image_channel_fusions", None) or {"rgb": "color", "default": "exponential"}
+        process, fusion = self.get_fusion(channels, fusions, self.layer_specs_image)
+        planes, kinds, layers = [], [], []
+        for j, (alg, ch) in enumerate(zip(fusion, process)):
+            if ch not in self.layer_names:
+                print(f"Layer {ch} not found, adding it to the semantic map")
+                self.add_layer(ch)
+            if alg not in IMAGE_KINDS:
+                print(f"[WARNING] Plugin image_{alg} is not in the list: {['image_' + k for k in IMAGE_KINDS]}")
+                continue
+            planes.append(j); kinds.append(IMAGE_KINDS[alg]); layers.append(self.layer_names.index(ch))
+        return planes, kinds, layers
 
     # ---- queries (semantic_map.py:318-385) ----------------------------------------------------------------------------
     def get_map_with_name(self, name):

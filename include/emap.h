@@ -286,6 +286,30 @@ int emap_semantic_traversability(emap_handle* h, int32_t n_layers, const float* 
 #define EMAP_PCA_MAX_FEATURES 64
 int emap_features_pca(emap_handle* h, int32_t n_features, const float* const* planes_device, float* out);
 
+/* ---- camera image fusion: EM.py:468-562 input_image (WRAP:180-185) with semantic_map.py:261-309 update_layers_image,
+ * kernels/custom_image_kernels.py:9-157 and fusion/image_color.py / image_exponential.py.
+ * image: (n_planes, height, width) fp32, host (is_device_ptr 0) or device memory; height * width <= 2^24.
+ * K (3x3 row-major), R (3x3, map -> camera optical frame, row-major), t (3): fp32.  D: n_D distortion coefficients,
+ * padded / truncated to 5 (fewer than 4: none) and used only when distortion_model is "radtan".
+ * The library computes P = K [R | t] and the camera cell uint32(cell_n / 2 + (-R^T t - center) / resolution) in fp32
+ * (products rounded, sums left to right).  A cell is fused where its is_valid is exactly 1, it projects in front of the
+ * camera into the image (radtan applied when D is not all zero), and no valid cell on the Bresenham line to the camera
+ * cell rises more than 0.10 above the ray.  Fused channel k then writes layer[k] of the caller's (n_layers, W, W) fp32
+ * device buffer at that cell, from pixel int(u) + int(v) * width:
+ *   EMAP_IMAGE_COLOR:       bits (r << 16) + (g << 8) + b of planes 0, 1, 2 (each converted float -> uint32);
+ *   EMAP_IMAGE_EXPONENTIAL: fp32(layer * (1 - 0.7) + 0.7 * image[plane[k]]), in double.
+ * Every other cell keeps its value.  Channels are applied in order.  Bit-identical to the reference's kernels built by
+ * nvcc for sm_90a.  EMAP_ERR_INVALID for NULL arguments, height * width > 2^24, a colour channel with fewer than 3
+ * planes, a plane >= n_planes, a layer outside [0, n_layers), non-finite K, R or t, and a camera cell outside [0, 2^24).
+ * One kernel per call.  A host image is copied into pinned staging (the caller may reuse its buffer on return) and to
+ * the device once; a device image is read in place and the call does not synchronise with the host. */
+#define EMAP_IMAGE_MAX_CHANNELS 64
+enum { EMAP_IMAGE_COLOR = 0, EMAP_IMAGE_EXPONENTIAL = 1 };
+int emap_input_image(emap_handle* h, int32_t n_planes, const float* image, int is_device_ptr, int32_t height, int32_t width,
+                     const float K[9], const float* D, int32_t n_D, const char* distortion_model, const float R[9],
+                     const float t[3], int32_t n_fused, const int32_t* plane, const int32_t* kind, const int32_t* layer,
+                     float* semantic_map_device, int32_t n_layers);
+
 /* ---- plumbing ---- */
 int emap_sync(emap_handle* h);
 int emap_stream(emap_handle* h, void** cuda_stream);
