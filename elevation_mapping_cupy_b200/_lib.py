@@ -49,6 +49,8 @@ SIGNATURES = {
     "emap_get_point_record": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]),
     "emap_semantic_configure": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                           C.c_double]),
+    "emap_semantic_configure_ext": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                              C.c_int32, C.c_double, C.c_void_p, C.c_void_p, C.c_int32]),
     "emap_point_record_device_ptr": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]),
     "emap_get_frame_stats": (C.c_int, [C.c_void_p, C.POINTER(EmapFrameStats)]),
     "emap_set_ray_counting": (C.c_int, [C.c_void_p, C.c_int]),

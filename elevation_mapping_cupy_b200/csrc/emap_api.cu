@@ -136,6 +136,9 @@ struct emap_handle {
   float* sem_map = nullptr;        // (n_layers, W, W) fp32, device, caller-owned
   DevBuf<i64> sem_fsum;            // one 2^-32 fixed-point sum plane per averaged channel
   DevBuf<u32> sem_csum;            // r, g, b, count planes per colour channel
+  // class_max scratch (SemMax): per-cell words (cnt, off, occ), control words + bitmaps + U list, the per-record table
+  DevBuf<u32> cm_cell, cm_ctl, cm_key, cm_flag;
+  DevBuf<i64> cm_sum;
   // inpainting scratch (allocated on first use): one block, carved by inpaint_scratch
   DevBuf<char> ip_block;
   int ip_grid = 0;
@@ -502,12 +505,35 @@ int frame_fuse(emap_handle* h) {
 
 // semantic point-channel fusion of the frame (semantic_map.py:223-259 after EM.py:369-371): needs the fused counts of
 // k_fuse and must run before k_finalize re-zeroes them
+// the class_max scratch as the kernels see it (pointers into the handle's buffers)
+SemMax sem_max(emap_handle* h) {
+  const size_t C = (size_t)h->dc.C;
+  SemMax m;
+  m.cnt = h->cm_cell; m.off = h->cm_cell + C; m.occ = h->cm_cell + 2 * C;
+  m.ctl = h->cm_ctl; m.ulist = h->cm_ctl + CM_CTL + (1 + SEM_MAX_CH) * CM_WORDS;
+  m.key = h->cm_key; m.flag = h->cm_flag; m.sum = h->cm_sum;
+  return m;
+}
+
 template <typename T>
 int launch_sem_sum(emap_handle* h, const T* pts, int s) {
   const i64 n = h->pend_n[s];
   if (n <= 0) return 0;
   k_sem_sum<T><<<cdiv(n, 256), 256, 0, h->stream>>>(h->dc, h->sem, pts, n, h->pend_stride, (const int*)(h->pidx + h->offs[s]),
-                                                     h->sem_fsum, h->sem_csum);
+                                                     h->sem_fsum, h->sem_csum, sem_max(h));
+  LAUNCH_CHECK();
+  return 0;
+}
+
+// class_max before the scatter: U and the records per cell over every cloud (id_max read once, with the first cloud)
+template <typename T>
+int launch_cm_count(emap_handle* h, const T* pts, int s) {
+  const i64 n = h->pend_n[s], n_idm = s == 0 ? (i64)h->sem.n_id_max * h->dc.C : 0;
+  const i64 work = std::max(n, n_idm);
+  if (work <= 0) return 0;
+  const int grid = (int)std::min<i64>(cdiv(work, 256), (i64)h->n_sm * 4);
+  k_cm_count<T><<<grid, 256, 0, h->stream>>>(h->sem, pts, n, h->pend_stride, (const int*)(h->pidx + h->offs[s]),
+                                             (const int*)h->sem.id_max, n_idm, sem_max(h));
   LAUNCH_CHECK();
   return 0;
 }
@@ -515,11 +541,36 @@ int launch_sem_sum(emap_handle* h, const T* pts, int s) {
 int frame_semantic(emap_handle* h) {
   if (h->sem.n_ch <= 0 || !h->sem_map) return 0;
   NvtxRange nv("emap:semantic");
+  const int n_max = h->sem.n_max;
+  if (n_max > 0) {
+    // table slots: n_max per valid + inside point at most (grown like the frame's other point buffers)
+    const size_t slots = (size_t)h->n_points * n_max;
+    int rc;
+    if ((rc = grow(h, h->cm_key, slots, slots / 4 + 1024, true)) || (rc = grow(h, h->cm_flag, slots, slots / 4 + 1024, true)) ||
+        (rc = grow(h, h->cm_sum, slots, slots / 4 + 1024, true)))
+      return rc;
+    CK(cudaMemsetAsync(h->cm_ctl, 0, sizeof(u32) * (CM_CTL + (1 + n_max) * CM_WORDS), h->stream));
+    if ((rc = each_cloud(h, [h](auto pts, int s) { return launch_cm_count(h, pts, s); }))) return rc;
+    PER_CELL(k_cm_alloc, h->dc.C, sem_max(h));
+    k_cm_ulist<<<1, 1024, 0, h->stream>>>(sem_max(h));
+    LAUNCH_CHECK();
+  }
   if (int rc = each_cloud(h, [h](auto pts, int s) { return launch_sem_sum(h, pts, s); })) return rc;
   // the cloud (staging buffer or the caller's pinned memory) is free only now
   if (h->pend_host) CK(cudaEventRecord(h->in_free[h->in_sel ^ 1], h->stream));
   if (h->zero_copy_pending) CK(cudaEventRecord(h->copy_done, h->stream));
-  PER_CELL(k_sem_apply, h->dc, h->sem, (const u64*)h->sc.cnt_fo, h->sem_fsum, h->sem_csum, h->sem_map);
+  if (n_max > 0) {
+    // occupied cells: at most one per valid + inside point
+    const int grid = std::max(1, cdiv(std::min<i64>(h->dc.C, h->n_points), 256));
+    for (int k = 0, j = 0; k < h->sem.n_ch; k++) {
+      if (h->sem.kind[k] != SEM_CLASS_MAX) continue;
+      k_cm_round<<<grid, 256, 0, h->stream>>>(h->dc.C, j, j == n_max - 1, sem_max(h), h->sem_map + (size_t)h->sem.layer[k] * h->dc.C,
+                                              h->sem.id_max + (size_t)j * h->dc.C);
+      LAUNCH_CHECK();
+      j++;
+    }
+  }
+  PER_CELL(k_sem_apply, h->dc, h->sem, (const u64*)h->sc.cnt_fo, h->sem_fsum, h->sem_csum, h->sem_map, sem_max(h));
   return 0;
 }
 
@@ -1176,27 +1227,59 @@ int emap_input_pointcloud(emap_handle* h, const void* points, int64_t n, int64_t
 }
 
 // ---- semantic point-channel fusion ------------------------------------------------------------
-int emap_semantic_configure(emap_handle* h, int32_t n_channels, const int32_t* column, const int32_t* kind, const int32_t* layer,
-                            float* semantic_map_device, int32_t n_layers, double average_weight) {
-  ENTER(h);
+namespace {
+int semantic_configure(emap_handle* h, const char* fn, int max_kind, int32_t n_channels, const int32_t* column,
+                       const int32_t* kind, const int32_t* layer, float* semantic_map_device, int32_t n_layers,
+                       double average_weight, float* variance_device, int32_t* id_max_device, int32_t n_id_max) {
+  char msg[200];
   if (n_channels <= 0) { h->sem.n_ch = 0; h->sem_map = nullptr; return EMAP_OK; }
-  if (n_channels > SEM_MAX_CH || !column || !kind || !layer || !semantic_map_device || n_layers < 1)
-    return fail(h, EMAP_ERR_INVALID, "emap_semantic_configure: 1..16 channels, non-null arrays and layer buffer");
+  if (n_channels > SEM_MAX_CH || !column || !kind || !layer || !semantic_map_device || n_layers < 1) {
+    snprintf(msg, sizeof(msg), "%s: 1..16 channels, non-null arrays and layer buffer", fn);
+    return fail(h, EMAP_ERR_INVALID, msg);
+  }
   SemCfg c;
   memset(&c, 0, sizeof(c));
   c.n_ch = n_channels; c.alpha = average_weight;
-  int nf = 0, nc = 0;
+  int nf = 0, nc = 0, nm = 0, nb = 0;
   for (int k = 0; k < n_channels; k++) {
-    if (column[k] < 3 || layer[k] < 0 || layer[k] >= n_layers || kind[k] < SEM_AVERAGE || kind[k] > SEM_COLOR)
-      return fail(h, EMAP_ERR_INVALID, "emap_semantic_configure: column >= 3, 0 <= layer < n_layers, kind 0..2 required");
+    if (column[k] < 3 || layer[k] < 0 || layer[k] >= n_layers || kind[k] < SEM_AVERAGE || kind[k] > max_kind) {
+      snprintf(msg, sizeof(msg), "%s: column >= 3, 0 <= layer < n_layers, kind 0..%d required", fn, max_kind);
+      return fail(h, EMAP_ERR_INVALID, msg);
+    }
     c.col[k] = column[k]; c.kind[k] = kind[k]; c.layer[k] = layer[k];
-    c.slot[k] = (kind[k] == SEM_COLOR) ? 4 * nc++ : nf++;
+    c.slot[k] = (kind[k] == SEM_COLOR) ? 4 * nc++ : (kind[k] == SEM_CLASS_MAX) ? nm++ : nf++;
+    nb += kind[k] == SEM_BAYESIAN_INFERENCE;
   }
+  if (nb > 0 && !variance_device)
+    return fail(h, EMAP_ERR_INVALID, "emap_semantic_configure_ext: bayesian_inference needs the variance planes");
+  if (nm > 0 && (!id_max_device || n_id_max < nm))
+    return fail(h, EMAP_ERR_INVALID, "emap_semantic_configure_ext: class_max needs id_max with one plane per class_max channel");
+  c.n_max = nm; c.sigma = nb ? variance_device : nullptr;
+  c.id_max = nm ? id_max_device : nullptr; c.n_id_max = nm ? n_id_max : 0;
   const size_t C = (size_t)h->dc.C;
   int rc;
   if ((rc = grow(h, h->sem_fsum, C * nf, 0, true)) || (rc = grow(h, h->sem_csum, C * 4 * nc, 0, true))) return rc;
+  if (nm > 0 && ((rc = grow(h, h->cm_cell, 3 * C, 0, true)) ||
+                 (rc = grow(h, h->cm_ctl, (size_t)CM_CTL + (1 + SEM_MAX_CH) * CM_WORDS + 65536, 0, true))))
+    return rc;
   h->sem = c; h->sem_map = semantic_map_device;
   return EMAP_OK;
+}
+}  // namespace
+
+int emap_semantic_configure(emap_handle* h, int32_t n_channels, const int32_t* column, const int32_t* kind, const int32_t* layer,
+                            float* semantic_map_device, int32_t n_layers, double average_weight) {
+  ENTER(h);
+  return semantic_configure(h, "emap_semantic_configure", SEM_COLOR, n_channels, column, kind, layer, semantic_map_device,
+                            n_layers, average_weight, nullptr, nullptr, 0);
+}
+
+int emap_semantic_configure_ext(emap_handle* h, int32_t n_channels, const int32_t* column, const int32_t* kind,
+                                const int32_t* layer, float* semantic_map_device, int32_t n_layers, double average_weight,
+                                float* variance_device, int32_t* id_max_device, int32_t n_id_max) {
+  ENTER(h);
+  return semantic_configure(h, "emap_semantic_configure_ext", SEM_CLASS_MAX, n_channels, column, kind, layer,
+                            semantic_map_device, n_layers, average_weight, variance_device, id_max_device, n_id_max);
 }
 
 // device-resident write-back of the last frame (CK.py:260-262): packed (cell index | flags) per input row, see

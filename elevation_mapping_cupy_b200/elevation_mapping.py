@@ -8,13 +8,14 @@ same method names, positional signatures and error behaviour, so the C++ bridge
 happens in the library; this module only marshals arguments.  Device arrays are handed out as torch
 CUDA tensors that alias the library's memory (they also expose `__cuda_array_interface__`).
 
-Point-cloud semantic layers (average / class_average / color fusion) are fused inside the frame (semantic_map.py).
+Point-cloud semantic layers are fused inside the frame with every point-cloud fusion of the reference (average,
+class_average, color, class_bayesian, bayesian_inference, class_max; semantic_map.py).
 The polygon safety check (get_polygon_traversability) is one library call: mask, statistics and hull on the device;
 get_polygons_traversability checks a batch of polygons in one call.
 Camera images (input_image) fuse into the semantic layers with the reference's `color` and `exponential` image fusions:
 one kernel projects every map cell into the image, tests occlusion along the line to the camera and writes every fused
 channel (csrc/emap_image.cuh), bit-identical to the reference's kernels on the same card.
-Out of scope (SURVEY.md section 8): bayesian semantic fusion and the image feature extractors.
+Out of scope (SURVEY.md section 8): the image feature extractors.
 """
 import ctypes as C
 import threading
@@ -243,7 +244,8 @@ class ElevationMap:
     def input_pointcloud(self, raw_points, channels: List[str], R, t, position_noise: float, orientation_noise: float):
         """EM.py:434-466.  raw_points: (N, 3+k) host (numpy / torch CPU, float32 or float64) or device
         (torch CUDA / cupy) array.  Channels beyond x, y, z are fused into semantic layers inside the frame
-        (semantic_map.py:223-259; algorithms average / class_average / color)."""
+        (semantic_map.py:223-259; algorithms average / class_average / color / class_bayesian / bayesian_inference /
+        class_max)."""
         if channels is not None and (len(channels) > 3 or self.semantic_map._configured is not None):
             self.semantic_map.configure_for(list(channels))
         Rm = np.ascontiguousarray(_to_host(R), dtype=np.float32).reshape(9)

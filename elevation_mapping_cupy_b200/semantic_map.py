@@ -6,13 +6,19 @@ Mirrors the point-cloud half of the reference class
 frame's point record: `average` (fusion/pointcloud_average.py), `class_average` (fusion/pointcloud_class_average.py, the
 reference's default) and `color` (fusion/pointcloud_color.py).  The kernels are csrc/emap_semantic.cuh; this class only
 decides which column of the cloud goes to which layer and hands the layer buffer to the engine
-(`emap_semantic_configure`).  The plugins that consume these layers (semantic_filter, semantic_traversability,
+(`emap_semantic_configure_ext`).  The plugins that consume these layers (semantic_filter, semantic_traversability,
 features_pca) are in plugins/.
+The reference's three other point-cloud fusions fuse in the same frame: `class_bayesian`
+(fusion/pointcloud_class_bayesian.py), `bayesian_inference` (pointcloud_bayesian_inference.py) and `class_max`
+(pointcloud_class_max.py), as DESIGN §4d defines them.  `bayesian_inference` keeps a variance plane per layer
+(`variance`, 1.0 at the start, reset to 1.0 by `clear`, moved with the map and padded with 1.0); `class_max` keeps the
+class id of each of its rounds in `elements_to_shift["id_max"]` ((n_class_max, W, W) int32, 0 at the start, moved with
+the map and padded with 0, kept by `clear`).
 Camera images (ElevationMap.input_image) fuse into the same layers: `update_layers_image` picks each channel's fusion
 (`image_channel_fusions`: `color`, fusion/image_color.py, or `exponential`, fusion/image_exponential.py) and layer, and
 one library call (`emap_input_image`, csrc/emap_image.cuh) projects, tests occlusion and writes every channel.  A layer
 an image adds reallocates the buffer; the point-channel registration is moved to the new buffer at once.
-Bayesian / class-max fusion and the image feature extractors are out of scope.
+The image feature extractors are out of scope.
 """
 import ctypes as C
 import re
@@ -20,7 +26,8 @@ from typing import Dict, List
 
 import numpy as np
 
-KINDS = {"average": 0, "class_average": 1, "color": 2}
+KINDS = {"average": 0, "class_average": 1, "color": 2,            # EMAP_SEM_*
+         "class_bayesian": 3, "bayesian_inference": 4, "class_max": 5}
 IMAGE_KINDS = {"color": 0, "exponential": 1}          # EMAP_IMAGE_COLOR, EMAP_IMAGE_EXPONENTIAL
 
 
@@ -34,7 +41,8 @@ class SemanticMap:
         self.semantic_map = None           # torch (n_layers, W, W) float32 on the engine's device, grown by add_layer
         self._configured = None
         self._registered = None            # (columns, kinds, layers) the engine fuses point channels with, or None
-        self.elements_to_shift = {}
+        self.variance = None               # (n_layers, W, W) float32 variance planes of bayesian_inference, made on first use
+        self.elements_to_shift = {}        # "id_max": (n_class_max, W, W) int32, made when a class_max channel is configured
 
     # ---- layer bookkeeping (semantic_map.py:47-99) ----------------------------------------------------------------
     def _alloc(self, n):
@@ -45,6 +53,8 @@ class SemanticMap:
     def clear(self):
         if self.semantic_map is not None:
             self.semantic_map.zero_()
+        if self.variance is not None:
+            self.variance.fill_(1.0)
 
     def add_layer(self, name):
         import torch
@@ -57,6 +67,8 @@ class SemanticMap:
         else:
             self.engine._before_framework()        # the engine's queued writes to the old buffer come first
             self.semantic_map = torch.cat([self.semantic_map, new], 0)
+            if self.variance is not None:
+                self.variance = torch.cat([self.variance, torch.ones_like(new)], 0)
         if self._registered is not None:           # the old buffer is freed: point the engine's fusion at the new one
             self._register(*self._registered)
 
@@ -106,21 +118,43 @@ class SemanticMap:
                 print(f"Layer {ch} not found, adding it to the semantic map")
                 self.add_layer(ch)
             cols.append(3 + feats.index(ch)); kinds.append(KINDS[alg]); layers.append(self.layer_names.index(ch))
+        self._alloc_state(kinds)
         self._register(cols, kinds, layers)        # no channel has a fusion: nothing to fuse
         self._configured = tuple(channels)
 
+    def _alloc_state(self, kinds):
+        """The variance planes (first bayesian_inference channel) and id_max (grown to this cloud's class_max channels;
+        new planes start at 0)."""
+        import torch
+        if KINDS["bayesian_inference"] in kinds and self.variance is None:
+            self.engine._before_framework()
+            self.variance = torch.ones_like(self.semantic_map)
+        n_max = kinds.count(KINDS["class_max"])
+        old = self.elements_to_shift.get("id_max")
+        if n_max and (old is None or old.shape[0] < n_max):
+            W = self.param.cell_n
+            new = torch.zeros((n_max, W, W), dtype=torch.int32, device=self.semantic_map.device)
+            if old is not None:
+                self.engine._before_framework()
+                new[:old.shape[0]] = old
+            self.elements_to_shift["id_max"] = new
+
     def _register(self, cols, kinds=None, layers=None):
-        """Hands the point-channel fusion (or None: no fusion) and the current layer buffer to the engine."""
+        """Hands the point-channel fusion (or None: no fusion), the current layer buffer and the fusion state (variance
+        planes, id_max) to the engine."""
         eng = self.engine
         if not cols:
-            eng._check(eng._L.emap_semantic_configure(eng._h, 0, None, None, None, None, 0, 0.0))
+            eng._check(eng._L.emap_semantic_configure_ext(eng._h, 0, None, None, None, None, 0, 0.0, None, None, 0))
             self._registered = None
             return
         n = len(cols)
         arr = lambda v: (C.c_int32 * n)(*v)
-        eng._check(eng._L.emap_semantic_configure(eng._h, n, arr(cols), arr(kinds), arr(layers),
-                                                  C.c_void_p(self.semantic_map.data_ptr()), len(self.layer_names),
-                                                  float(getattr(self.param, "average_weight", 0.5))))
+        id_max = self.elements_to_shift.get("id_max")
+        eng._check(eng._L.emap_semantic_configure_ext(
+            eng._h, n, arr(cols), arr(kinds), arr(layers), C.c_void_p(self.semantic_map.data_ptr()), len(self.layer_names),
+            float(getattr(self.param, "average_weight", 0.5)),
+            None if self.variance is None else C.c_void_p(self.variance.data_ptr()),
+            None if id_max is None else C.c_void_p(id_max.data_ptr()), 0 if id_max is None else id_max.shape[0]))
         self._registered = (cols, kinds, layers)
 
     # ---- the image hook (semantic_map.py:261-309) ----------------------------------------------------------------------
@@ -148,15 +182,24 @@ class SemanticMap:
     def get_index(self, name):
         return self.layer_names.index(name) if name in self.layer_names else -1
 
-    def shift_map_xy(self, shift_value):
-        """semantic_map.py:131-148: roll + zero padding, applied with the elevation map's shift."""
+    @staticmethod
+    def _shift(buf, sx, sy, pad):
         import torch
+        m = torch.roll(buf, (sx, sy), dims=(1, 2))
+        if sx > 0: m[:, :sx, :] = pad
+        elif sx < 0: m[:, sx:, :] = pad
+        if sy > 0: m[:, :, :sy] = pad
+        elif sy < 0: m[:, :, sy:] = pad
+        buf.copy_(m)
+
+    def shift_map_xy(self, shift_value):
+        """semantic_map.py:131-148: roll + zero padding, applied with the elevation map's shift.  The variance planes
+        are padded with 1.0 (their initial value), id_max with 0."""
         if self.semantic_map is None or (shift_value[0] == 0 and shift_value[1] == 0):
             return
         sx, sy = int(shift_value[0]), int(shift_value[1])
-        m = torch.roll(self.semantic_map, (sx, sy), dims=(1, 2))
-        if sx > 0: m[:, :sx, :] = 0.0
-        elif sx < 0: m[:, sx:, :] = 0.0
-        if sy > 0: m[:, :, :sy] = 0.0
-        elif sy < 0: m[:, :, sy:] = 0.0
-        self.semantic_map.copy_(m)
+        self._shift(self.semantic_map, sx, sy, 0.0)
+        if self.variance is not None:
+            self._shift(self.variance, sx, sy, 1.0)
+        if "id_max" in self.elements_to_shift:
+            self._shift(self.elements_to_shift["id_max"], sx, sy, 0)

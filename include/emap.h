@@ -131,6 +131,31 @@ int emap_set_ray_counting(emap_handle* h, int enable);
  * n_channels = 0 switches it off.  Not applied to sharded frames. */
 int emap_semantic_configure(emap_handle* h, int32_t n_channels, const int32_t* column, const int32_t* kind,
                             const int32_t* layer, float* semantic_map_device, int32_t n_layers, double average_weight);
+/* The kinds of emap_semantic_configure (0..2) and of emap_semantic_configure_ext (0..5). */
+#define EMAP_SEM_AVERAGE 0
+#define EMAP_SEM_CLASS_AVERAGE 1
+#define EMAP_SEM_COLOR 2
+#define EMAP_SEM_CLASS_BAYESIAN 3
+#define EMAP_SEM_BAYESIAN_INFERENCE 4
+#define EMAP_SEM_CLASS_MAX 5
+/* emap_semantic_configure with every point-cloud fusion of the reference, and the state two of them keep.  The arguments
+ * of emap_semantic_configure mean the same; kind may also be
+ *   3 = fusion/pointcloud_class_bayesian.py: per frame, the sum of the channel's values >= 0 at each cell, divided by the
+ *       sum over the class_bayesian channels (1 where that is 0), in every cell;
+ *   4 = fusion/pointcloud_bayesian_inference.py: where the frame fused n > 0 points, m' = m/(n*s + 1) + n*s*mean/(n*s + 1)
+ *       and s' = s/(n*s + 1) in fp32, with the variance s of the layer read from and written to variance_device
+ *       ((n_layers, W, W) fp32, device, caller-owned, indexed by layer like semantic_map_device; start it at 1.0);
+ *   5 = fusion/pointcloud_class_max.py: the feature's bits are an fp16 probability (low 16) and a class id (high 16).
+ *       For the j-th class_max channel, each cell takes the largest per-class probability sum over the ids of the frame's
+ *       rows and of id_max (absent or earlier-won ids count 0, ties to the smallest id, NaN is the largest); the id goes
+ *       to plane j of id_max_device ((n_id_max, W, W) int32, device, caller-owned, n_id_max >= the class_max channels),
+ *       and every id that won anywhere counts 0 in the later channels.  The layers hold the maxima divided by their
+ *       sum over the class_max channels (1 where that is 0), in every cell.
+ * variance_device may be NULL without a kind 4 channel, id_max_device without a kind 5 channel.  Sums are exact fixed
+ * point (DESIGN.md §4d).  emap_semantic_configure_ext(h, 0, ...) switches the fusion off. */
+int emap_semantic_configure_ext(emap_handle* h, int32_t n_channels, const int32_t* column, const int32_t* kind,
+                                const int32_t* layer, float* semantic_map_device, int32_t n_layers, double average_weight,
+                                float* variance_device, int32_t* id_max_device, int32_t n_id_max);
 /* CK.py:260-262 write-back of the last frame, on the DEVICE: one packed int32 per input row (bits 0..23 cell index,
  * bit 28 valid, bit 29 inside, bit 30 row dropped as NaN); valid until the next frame. */
 int emap_point_record_device_ptr(emap_handle* h, const int32_t** packed_device, int64_t* n);
