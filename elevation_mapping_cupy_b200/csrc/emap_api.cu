@@ -18,6 +18,7 @@
 #include "emap_polygon.cuh"
 #include "emap_semantic_plugins.cuh"
 #include "emap_image.cuh"
+#include "emap_submap.cuh"
 
 namespace {
 
@@ -814,8 +815,24 @@ int shard_finish(emap_handle* h) {
 const char* const kExportNames[] = {"elevation", "variance", "traversability", "time", "upper_bound", "is_upper_bound",
                                     "normal_x", "normal_y", "normal_z"};
 
-// Layers by one k_export_multi launch, one device-to-host copy and one synchronisation.  names[k]: a name of
-// kExportNames, or planes[k] != NULL: a (W,W) device plane exported with flags[k] (bit 0 fill_nan, bit 1 add the centre height).
+// The n (<= EXPORT_MAX_LAYERS) layers of an export call.  names[k]: a name of kExportNames, or planes[k] != NULL: a (W,W)
+// device plane exported with flags[k] (bit 0 fill_nan, bit 1 add the centre height).  Returns false, with the message
+// in h->err, for an unknown name.
+bool export_list(emap_handle* h, int32_t n, const char* const* names, const float* const* planes, const int32_t* flags,
+                 ExportList& L) {
+  memset(&L, 0, sizeof(L));
+  L.n = n;
+  for (int k = 0; k < n; k++) {
+    if (planes && planes[k]) { L.kind[k] = 9; L.plane[k] = planes[k]; L.flags[k] = flags ? flags[k] : 0; continue; }
+    int kind = -1;
+    if (names && names[k]) for (int i = 0; i < 9; i++) if (!strcmp(names[k], kExportNames[i])) kind = i;
+    if (kind < 0) { h->err = std::string("Layer ") + (names && names[k] ? names[k] : "(null)") + " is not in the map"; return false; }
+    L.kind[k] = kind;
+  }
+  return true;
+}
+
+// Layers by one k_export_multi launch, one device-to-host copy and one synchronisation (layers as export_list).
 int export_layers(emap_handle* h, int32_t n, const char* const* names, const float* const* planes, const int32_t* flags,
                   float* out_host, int64_t n_out_total) {
   if (n < 1 || n > EXPORT_MAX_LAYERS || !out_host) return fail(h, EMAP_ERR_INVALID, "emap_get_layers: 1..24 layers, non-null output");
@@ -823,15 +840,7 @@ int export_layers(emap_handle* h, int32_t n, const char* const* names, const flo
   const size_t per = (size_t)Wo * Wo;
   if (n_out_total != (int64_t)(per * n)) return fail(h, EMAP_ERR_INVALID, "output must hold n * (cell_n-2)^2 floats");
   ExportList L;
-  memset(&L, 0, sizeof(L));
-  L.n = n;
-  for (int k = 0; k < n; k++) {
-    if (planes && planes[k]) { L.kind[k] = 9; L.plane[k] = planes[k]; L.flags[k] = flags ? flags[k] : 0; continue; }
-    int kind = -1;
-    if (names && names[k]) for (int i = 0; i < 9; i++) if (!strcmp(names[k], kExportNames[i])) kind = i;
-    if (kind < 0) { h->err = std::string("Layer ") + (names && names[k] ? names[k] : "(null)") + " is not in the map"; return EMAP_ERR_NOLAYER; }
-    L.kind[k] = kind;
-  }
+  if (!export_list(h, n, names, planes, flags, L)) return EMAP_ERR_NOLAYER;
   int rc = grow(h, h->d_export, per * n, 0, false);
   if (rc) return rc;
   k_export_multi<<<dim3(cdiv((i64)per, 256), n), 256, 0, h->stream>>>(h->dc, h->map, h->normal, h->d_export, L, h->center[2],
@@ -1589,6 +1598,83 @@ int emap_get_layers(emap_handle* h, int32_t n, const char* const* names, const f
                     float* out_host, int64_t n_out_total) {
   ENTER(h);
   return export_layers(h, n, names, planes, flags, out_host, n_out_total);
+}
+
+static_assert(EMAP_SUBMAP_MAX_WINDOWS == SUBMAP_MAX_WINDOWS && EMAP_SUBMAP_MAX_LAYERS == EXPORT_MAX_LAYERS,
+              "emap.h states the kernel's limits");
+
+static bool submap_lengths_ok(int64_t n, const double* windows) {
+  for (int64_t w = 0; w < n; w++)
+    for (int a = 2; a < 4; a++)
+      if (!(std::isfinite(windows[4 * w + a]) && windows[4 * w + a] >= 0.0)) return false;
+  return true;
+}
+
+// The host part of emap_get_submaps on its own (no handle, no device): submap_window for every request.
+int emap_submap_windows(int32_t cell_n, double resolution, const double center[2], int32_t n_windows,
+                        const double* windows, int32_t* info, double* centres) {
+  if (!center || !windows || !info || !centres || cell_n < 3 || !(std::isfinite(resolution) && resolution > 0.0) ||
+      n_windows < 0 || !submap_lengths_ok(n_windows, windows))
+    return EMAP_ERR_INVALID;
+  for (int32_t w = 0; w < n_windows; w++) submap_window(cell_n, resolution, center, windows + 4 * w, info + 5 * w, centres + 2 * w);
+  return EMAP_OK;
+}
+
+// The get_raw_submap service (elevation_mapping_ros.cpp:507-553) for a batch of windows: the windows on the host
+// (submap_window), every (window, layer, row) of the batch in one k_submap launch whose table is its parameters.  Host
+// output: one device-to-host copy and one synchronisation; device output: stream-ordered, no synchronisation.  Every
+// check runs before anything is written or launched.
+int emap_get_submaps(emap_handle* h, int32_t n_windows, const double* windows, int32_t n_layers, const char* const* names,
+                     const float* const* planes_device, const int32_t* flags, float* out, int32_t out_is_device,
+                     int64_t out_floats, int32_t* info, double* centres) {
+  ENTER(h);
+  NvtxRange nv("emap:get_submaps");
+  if (!windows || !names || !out || !info || !centres) return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: null argument");
+  if (n_windows < 1 || n_windows > EMAP_SUBMAP_MAX_WINDOWS)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: 1 to EMAP_SUBMAP_MAX_WINDOWS windows required");
+  if (n_layers < 1 || n_layers > EMAP_SUBMAP_MAX_LAYERS)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: 1 to EMAP_SUBMAP_MAX_LAYERS layers required");
+  if (!submap_lengths_ok(n_windows, windows))
+    return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: lengths must be finite and >= 0");
+  SubmapArgs a;
+  if (!export_list(h, n_layers, names, planes_device, flags, a.L)) return EMAP_ERR_INVALID;
+  const int W = h->dc.W;
+  const double m[2] = {h->center[0], h->center[1]};
+  std::vector<int32_t> inf(5 * (size_t)n_windows);
+  std::vector<double> cen(2 * (size_t)n_windows);
+  a.n_win = 0;
+  int tiles = 0;
+  long long total = 0;
+  for (int w = 0; w < n_windows; w++) {
+    const int32_t* q = &inf[5 * w];
+    submap_window(W, h->cfg.resolution, m, windows + 4 * w, &inf[5 * w], &cen[2 * w]);
+    if (!q[0]) continue;
+    SubmapWin& s = a.win[a.n_win++];
+    s.r0 = (int16_t)(W - 2 - q[1]); s.c0 = (int16_t)(W - 2 - q[2]);
+    s.rows = (int16_t)q[3]; s.cols = (int16_t)q[4];
+    s.tile0 = tiles; s.off = total;
+    tiles += cdiv(q[3], SUBMAP_ROWS);
+    total += (long long)n_layers * q[3] * q[4];
+  }
+  if (total > out_floats)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: out_floats is below the layers times the windows' cells");
+  memcpy(info, inf.data(), sizeof(int32_t) * inf.size());
+  memcpy(centres, cen.data(), sizeof(double) * cen.size());
+  if (!a.n_win) return EMAP_OK;
+  float* dst = out;
+  if (!out_is_device) {
+    const int rc = grow(h, h->d_export, (size_t)total, 0, false);
+    if (rc) return rc;
+    dst = h->d_export;
+  }
+  k_submap<<<dim3(tiles, n_layers), dim3(32, SUBMAP_ROWS), 0, h->stream>>>(h->dc, h->map, h->normal, dst, a, h->center[2],
+                                                                           h->cfg.use_only_above_for_upper_bound);
+  LAUNCH_CHECK();
+  if (!out_is_device) {
+    CK(cudaMemcpyAsync(out, dst, sizeof(float) * total, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+  }
+  return EMAP_OK;
 }
 
 int emap_layer_device_ptr(emap_handle* h, const char* name, void** ptr) {

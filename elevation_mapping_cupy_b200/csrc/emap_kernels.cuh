@@ -1194,12 +1194,10 @@ k_init_dilate(const DevCfg c, const float* __restrict__ src_h, const float* __re
 // export EM.py:579-670,720-775: NaN-fill, +center_z, crop the border ring, flip both axes.
 // kind: 0 elevation, 1 variance, 2 traversability, 3 time, 4 upper_bound, 5 is_upper_bound, 6..8 normal xyz
 // kind 9: arbitrary plane with flags (bit0 fill_nan, bit1 add_z) = process_map_for_publish (EM.py:579-596)
-__device__ __forceinline__ float export_value(const DevCfg& c, const float* __restrict__ map, const float* __restrict__ normal,
-                                              int o, int kind, float center_z, int only_above, const float* __restrict__ plane,
-                                              int flags) {
-  const int Wo = c.W - 2;
-  const int orow = o / Wo, ocol = o - orow * Wo;
-  const int r = Wo - 1 - orow + 1, cc = Wo - 1 - ocol + 1;         // flip(0), flip(1) of m[1:-1,1:-1]
+// export_cell: the value of state cell (r, cc); export_value: of exported cell o (row-major over the (W-2)^2 output).
+__device__ __forceinline__ float export_cell(const DevCfg& c, const float* __restrict__ map, const float* __restrict__ normal,
+                                             int r, int cc, int kind, float center_z, int only_above,
+                                             const float* __restrict__ plane, int flags) {
   const int i = r * c.W + cc, C = c.C;
   const float nanv = __int_as_float(0x7fc00000);
   const float valid = map[2 * C + i], isup = map[6 * C + i], upper = map[5 * C + i];
@@ -1222,6 +1220,14 @@ __device__ __forceinline__ float export_value(const DevCfg& c, const float* __re
     default: v = normal[(size_t)(kind - 6) * C + i]; break;
   }
   return v;
+}
+__device__ __forceinline__ float export_value(const DevCfg& c, const float* __restrict__ map, const float* __restrict__ normal,
+                                              int o, int kind, float center_z, int only_above, const float* __restrict__ plane,
+                                              int flags) {
+  const int Wo = c.W - 2;
+  const int orow = o / Wo, ocol = o - orow * Wo;
+  const int r = Wo - 1 - orow + 1, cc = Wo - 1 - ocol + 1;         // flip(0), flip(1) of m[1:-1,1:-1]
+  return export_cell(c, map, normal, r, cc, kind, center_z, only_above, plane, flags);
 }
 
 // One launch exports a list of layers (WRAP:213-252 get_grid_map asks for several): blockIdx.y = layer.

@@ -15,6 +15,8 @@ get_polygons_traversability checks a batch of polygons in one call.
 Camera images (input_image) fuse into the semantic layers with the reference's `color` and `exponential` image fusions:
 one kernel projects every map cell into the image, tests occlusion along the line to the camera and writes every fused
 channel (csrc/emap_image.cuh), bit-identical to the reference's kernels on the same card.
+Windows of the exported map (get_submap / get_submaps, the node's get_raw_submap service) come from one library call
+and one kernel per batch (csrc/emap_submap.cuh).
 Out of scope (SURVEY.md section 8): the image feature extractors.
 """
 import ctypes as C
@@ -392,6 +394,70 @@ class ElevationMap:
                     raise KeyError("Layer {} is not in the map".format(name))
                 sources.append(src)
             self._export(sources, data)
+
+    def get_submap(self, position, length, layers, out=None):
+        """The get_raw_submap service (elevation_mapping_ros.cpp:507-553) in the map frame: the window of the exported
+        map around `position` (x, y) of `length` (x, y) metres, as get_submaps returns it for one request."""
+        return self.get_submaps([(position, length)], layers, out)[0]
+
+    def get_submaps(self, requests, layers, out=None):
+        """Windows of the exported map (get_maps_with_names_ref's coordinates: the interior, flipped on both axes) for
+        `requests`, a list of (position, length) pairs of (x, y) metres in the map frame, in one library call
+        (emap_get_submaps; include/emap.h states the window rule).  `layers` are named as for get_maps_with_names_ref
+        and evaluated once per call.  `out`: None (a new NumPy array), a float32 C-contiguous NumPy array or a float32
+        contiguous torch CUDA tensor of at least len(layers) * the windows' cells; with a CUDA tensor the call does not
+        synchronise with the host and the results stay on the device.  Returns one dict per request: "layers" maps each
+        name to a (rows, cols) view of `out`, "index" is (row0, col0), "size" (rows, cols), "centre" the centre of the
+        window's cells and "success" whether the position lies in the map (a failed window has (0, 0) layers)."""
+        names = list(layers)
+        for name in names:
+            if not (name in EXPORT_NAMES or name in self.semantic_map.layer_names
+                    or name in self.plugin_manager.layer_names):
+                raise KeyError("Layer {} is not in the map".format(name))
+        req = np.zeros((len(requests), 4), np.float64)
+        for w, (pos, ln) in enumerate(requests):
+            req[w, :2] = np.asarray(_to_host(pos), np.float64).reshape(-1)[:2]
+            req[w, 2:] = np.asarray(_to_host(ln), np.float64).reshape(-1)[:2]
+        n, nl = len(req), len(names)
+        info = np.zeros((n, 5), np.int32)
+        centres = np.zeros((n, 2), np.float64)
+        device = out is not None and _is_device(out)
+        with self.map_lock:
+            if out is None:
+                c = self.center.astype(np.float64)
+                self._check(self._L.emap_submap_windows(self.cell_n, float(self.resolution), c.ctypes.data, n,
+                                                        req.ctypes.data, info.ctypes.data, centres.ctypes.data))
+                out = np.zeros(nl * int((info[:, 3].astype(np.int64) * info[:, 4]).sum()), np.float32)
+            if device:
+                import torch
+                if out.dtype != torch.float32 or not out.is_contiguous():
+                    raise TypeError("a device `out` must be a contiguous float32 torch CUDA tensor")
+                ptr, size = out.data_ptr(), out.numel()
+            else:
+                if out.dtype != np.float32 or not out.flags.c_contiguous:
+                    raise TypeError("a host `out` must be a C-contiguous float32 NumPy array")
+                ptr, size = out.ctypes.data, out.size
+            sources = [self._export_source(name) for name in names]
+            c_names = (C.c_char_p * nl)(*[s[0].encode() for s in sources])
+            planes = (C.c_void_p * nl)(*[s[1] for s in sources])
+            flags = (C.c_int32 * nl)(*[s[2] for s in sources])
+            if device or any(s[3] is not None for s in sources):
+                self._after_framework()       # the planes and the output buffer are complete / free
+            self._check(self._L.emap_get_submaps(self._h, n, req.ctypes.data, nl, c_names, planes, flags, ptr,
+                                                 int(device), size, info.ctypes.data, centres.ctypes.data))
+            if device:
+                self._before_framework()      # framework reads of `out` run after the kernel (no host sync)
+        flat = out.reshape(-1)
+        result, off = [], 0
+        for w in range(n):
+            ok, r0, c0, rows, cols = (int(v) for v in info[w])
+            views = {}
+            for name in names:
+                views[name] = flat[off:off + rows * cols].reshape(rows, cols)
+                off += rows * cols
+            result.append({"layers": views, "index": (r0, c0), "size": (rows, cols), "centre": centres[w].copy(),
+                           "success": bool(ok)})
+        return result
 
     def get_state(self):
         """Host copies (map (7,W,W), normal (3,W,W)) -- tests / checkpointing."""

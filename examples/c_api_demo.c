@@ -37,9 +37,21 @@ int main(void) {
   const int wo = emap_cell_n(h) - 2;
   float* layer = (float*)malloc(sizeof(float) * (size_t)wo * wo);
   if (!rc) rc = emap_get_map_with_name(h, "elevation", layer, (int64_t)wo * wo);
+  /* the get_raw_submap service: a 2 m x 2 m window around the map centre with two layers, sized on the host first */
+  double centre[3] = {0, 0, 0}, win[4] = {0, 0, 2.0, 2.0}, win_centre[2];
+  int32_t info[5] = {0, 0, 0, 0, 0};
+  const char* names[2] = {"elevation", "traversability"};
+  float* sub = NULL;
+  if (!rc) rc = emap_get_position(h, centre);
+  win[0] = centre[0]; win[1] = centre[1];
+  if (!rc) rc = emap_submap_windows(emap_cell_n(h), cfg.resolution, centre, 1, win, info, win_centre);
+  const int64_t sub_n = 2 * (int64_t)info[3] * info[4];
+  if (!rc && sub_n) sub = (float*)malloc(sizeof(float) * (size_t)sub_n);
+  if (!rc && sub) rc = emap_get_submaps(h, 1, win, 2, names, NULL, NULL, sub, 0, sub_n, info, win_centre);
   if (rc) fprintf(stderr, "error %d: %s\n", rc, emap_last_error(h));
-  else printf("centre cell elevation: %f, kernels launched: %lld\n", layer[(wo / 2) * wo + wo / 2], (long long)emap_launch_count(h));
-  free(layer); free(pts);
+  else printf("centre cell elevation: %f, window %d x %d at row %d, column %d, kernels launched: %lld\n",
+              layer[(wo / 2) * wo + wo / 2], info[3], info[4], info[1], info[2], (long long)emap_launch_count(h));
+  free(sub); free(layer); free(pts);
   emap_destroy(h);
   return rc ? 1 : 0;
 }

@@ -228,6 +228,37 @@ int emap_get_map_with_name(emap_handle* h, const char* name, float* out_host, in
  * planes. */
 int emap_get_layers(emap_handle* h, int32_t n, const char* const* names, const float* const* planes_device,
                     const int32_t* flags, float* out_host, int64_t n_out_total);
+/* ---- windows of the exported map: the ROS node's get_raw_submap service (elevation_mapping_ros.cpp:507-553, grid_map's
+ * GridMap::getSubmap on the exported layers).  Coordinates are those of emap_get_layers' output: the (cell_n-2)^2
+ * interior, flipped on both axes, so row 0 is the +x edge and column 0 the +y edge; rows follow x, columns y.
+ * windows[4w .. 4w+3] = (position_x, position_y, length_x, length_y) in the map frame, lengths finite and >= 0.
+ * A coordinate p lies in state cell floor((p - center) / resolution + cell_n / 2) (EM.py's index, in double, half-open:
+ * a coordinate on a cell boundary belongs to the cell on its +x / +y side), state cell i is output index cell_n - 2 - i.
+ * Window w is the inclusive cell rectangle between the cell holding position + length / 2 and the cell holding
+ * position - length / 2, each clipped to the exported area; a length of 0 gives one cell.  It fails when the position's
+ * own cell is outside the exported area (or the position is not a number).
+ * info[5w .. 5w+4] = {success (1/0), row0, col0, rows, cols}, all 0 on failure; centres[2w .. 2w+1] = the centre of the
+ * window's cells in the map frame (NaN on failure).
+ * emap_submap_windows: that arithmetic alone, on the host, for a map of cell_n cells at `resolution` centred at
+ * center; no handle, no device.  EMAP_ERR_INVALID for NULL arguments, cell_n < 3, a resolution that is not finite and
+ * > 0, n_windows < 0 and a length that is not finite and >= 0. */
+int emap_submap_windows(int32_t cell_n, double resolution, const double center[2], int32_t n_windows,
+                        const double* windows, int32_t* info, double* centres);
+/* emap_get_submaps: the windows of the handle's map, with n_layers layers each, named as for emap_get_layers (names[k],
+ * or planes_device[k] != NULL with flags[k]); every value is bit-identical to the same cell of emap_get_layers.
+ * out receives, window after window, each successful window's layers one after another, each rows x cols row-major
+ * (failed windows take no space): out_floats must be at least n_layers times the sum of rows * cols.  out is host memory
+ * (out_is_device 0: one device-to-host copy and one synchronisation) or device memory (out_is_device != 0: no host
+ * synchronisation; the work is queued on the handle's stream, see emap_wait_for_stream / emap_stream_wait_for, and the
+ * call can be captured into a CUDA graph: its window table travels in the kernel's parameters).  One kernel per call.
+ * EMAP_ERR_INVALID, with nothing written or launched, for a NULL windows / names / out / info / centres, n_windows
+ * outside [1, EMAP_SUBMAP_MAX_WINDOWS], n_layers outside [1, EMAP_SUBMAP_MAX_LAYERS], a length that is not finite and
+ * >= 0, an unknown layer name and an output too small. */
+#define EMAP_SUBMAP_MAX_WINDOWS 1024
+#define EMAP_SUBMAP_MAX_LAYERS 24
+int emap_get_submaps(emap_handle* h, int32_t n_windows, const double* windows, int32_t n_layers, const char* const* names,
+                     const float* const* planes_device, const int32_t* flags, float* out, int32_t out_is_device,
+                     int64_t out_floats, int32_t* info, double* centres);
 /* EM.py:807-835 get_layer / raw state access: device pointer of a (W,W) fp32 plane.  Names: the 7
  * layers of EM.py:69-77, normal_x/y/z, traversability_input.  `elevation_map` returns the (7,W,W)
  * base, `normal_map` the (3,W,W) base.  Pointers stay valid until the next emap_move / emap_move_to / emap_destroy. */
