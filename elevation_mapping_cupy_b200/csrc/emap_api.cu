@@ -19,6 +19,7 @@
 #include "emap_semantic_plugins.cuh"
 #include "emap_image.cuh"
 #include "emap_submap.cuh"
+#include "emap_mapcloud.cuh"
 
 namespace {
 
@@ -157,6 +158,11 @@ struct emap_handle {
   float* img_host = nullptr;
   size_t img_host_n = 0;
   cudaEvent_t img_staged = nullptr;
+  // emap_get_map_points / emap_get_normal_arrows (allocated on first use): the count and offset tables, the kept cells'
+  // payload (grown to the largest call) and a pinned word for the count
+  DevBuf<int> mc_table;
+  DevBuf<char> mc_out;
+  int* mc_count_host = nullptr;
   // misc
   int64_t launches = 0;
   int count_rays = 0;
@@ -811,9 +817,15 @@ int shard_finish(emap_handle* h) {
   return frame_finish(h);
 }
 
-// export_value's kinds 0..8 (kind 9: a caller plane)
+// export_value's named kinds: kExportNames[k] is kind k, except the last, normal_color (kind EXPORT_KIND_PLANE is a
+// caller plane)
 const char* const kExportNames[] = {"elevation", "variance", "traversability", "time", "upper_bound", "is_upper_bound",
-                                    "normal_x", "normal_y", "normal_z"};
+                                    "normal_x", "normal_y", "normal_z", "normal_color"};
+constexpr int kNumExportNames = sizeof(kExportNames) / sizeof(kExportNames[0]);
+static_assert(kNumExportNames == EXPORT_KIND_PLANE + 1, "kinds 0..8 are named in order, then normal_color");
+inline int export_kind(int name_index) {
+  return name_index == kNumExportNames - 1 ? EXPORT_KIND_NORMAL_COLOR : name_index;
+}
 
 // The n (<= EXPORT_MAX_LAYERS) layers of an export call.  names[k]: a name of kExportNames, or planes[k] != NULL: a (W,W)
 // device plane exported with flags[k] (bit 0 fill_nan, bit 1 add the centre height).  Returns false, with the message
@@ -823,9 +835,13 @@ bool export_list(emap_handle* h, int32_t n, const char* const* names, const floa
   memset(&L, 0, sizeof(L));
   L.n = n;
   for (int k = 0; k < n; k++) {
-    if (planes && planes[k]) { L.kind[k] = 9; L.plane[k] = planes[k]; L.flags[k] = flags ? flags[k] : 0; continue; }
+    if (planes && planes[k]) {
+      L.kind[k] = EXPORT_KIND_PLANE; L.plane[k] = planes[k]; L.flags[k] = flags ? flags[k] : 0;
+      continue;
+    }
     int kind = -1;
-    if (names && names[k]) for (int i = 0; i < 9; i++) if (!strcmp(names[k], kExportNames[i])) kind = i;
+    if (names && names[k])
+      for (int i = 0; i < kNumExportNames; i++) if (!strcmp(names[k], kExportNames[i])) kind = export_kind(i);
     if (kind < 0) { h->err = std::string("Layer ") + (names && names[k] ? names[k] : "(null)") + " is not in the map"; return false; }
     L.kind[k] = kind;
   }
@@ -843,10 +859,61 @@ int export_layers(emap_handle* h, int32_t n, const char* const* names, const flo
   if (!export_list(h, n, names, planes, flags, L)) return EMAP_ERR_NOLAYER;
   int rc = grow(h, h->d_export, per * n, 0, false);
   if (rc) return rc;
-  k_export_multi<<<dim3(cdiv((i64)per, 256), n), 256, 0, h->stream>>>(h->dc, h->map, h->normal, h->d_export, L, h->center[2],
-                                                                       h->cfg.use_only_above_for_upper_bound);
+  const auto kern = export_has_colour(L) ? k_export_multi<true> : k_export_multi<false>;
+  kern<<<dim3(cdiv((i64)per, 256), n), 256, 0, h->stream>>>(h->dc, h->map, h->normal, h->d_export, L, h->center[2],
+                                                             h->cfg.use_only_above_for_upper_bound);
   LAUNCH_CHECK();
   CK(cudaMemcpyAsync(out_host, h->d_export, sizeof(float) * per * n, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return EMAP_OK;
+}
+
+// emap_get_map_points (ARROWS false) / emap_get_normal_arrows (true): the count pass and the scan, one synchronisation
+// for the total; then, if the caller's capacity holds it, the write pass, the payload's copies and one more
+// synchronisation.  Nothing reaches the caller's rows when the capacity is too small.
+template <bool ARROWS>
+int map_cloud(emap_handle* h, int64_t* n_rows, float* xyz, int32_t* ids, double* seg) {
+  const int Wo = h->dc.W - 2;
+  const int n_chunks = cdiv(Wo, MC_TILE), n_tiles = cdiv(Wo, MC_TILE);
+  const int n = Wo * n_chunks, span = MC_TILE * n_chunks;      // count entries; entries of one scan CTA
+  static_assert(MC_TILE % 4 == 0, "k_mapcloud_scan reads whole spans as int4");
+  // cell_n <= 2049 (emap_create): at most 64 chunks, a span of at most 2048 entries, two per scan thread
+  if (span > 2 * 1024) return fail(h, EMAP_ERR_INVALID, "map point cloud: cell_n too large for k_mapcloud_scan");
+  int rc = grow(h, h->mc_table, 2 * (size_t)n + 1, 0, false);
+  if (rc) return rc;
+  if (!h->mc_count_host) CK(cudaMallocHost(&h->mc_count_host, sizeof(int)));
+  int* cnt = h->mc_table;
+  int* off = cnt + n;
+  const dim3 grid(n_tiles, n_chunks);
+  const MapCloudGeom g = {(double)h->center[0], (double)h->center[1], h->cfg.resolution};
+  MapCloudOut o = {nullptr, nullptr, nullptr};
+  k_mapcloud<ARROWS, false><<<grid, MC_THREADS, 0, h->stream>>>(h->dc, h->map, h->normal, h->center[2], cnt, nullptr, g, o);
+  LAUNCH_CHECK();
+  k_mapcloud_scan<<<cdiv(n, span), 1024, 0, h->stream>>>(cnt, off, n, span);
+  LAUNCH_CHECK();
+  CK(cudaMemcpyAsync(h->mc_count_host, off + n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  const int64_t total = *h->mc_count_host;
+  if (total > *n_rows) {
+    *n_rows = total;
+    return fail(h, EMAP_ERR_INVALID, "map point cloud: capacity too small (needed rows in the count argument)");
+  }
+  *n_rows = total;
+  if (!total) return EMAP_OK;
+  const size_t id_bytes = ARROWS ? (sizeof(int32_t) * (size_t)total + 255) & ~(size_t)255 : 0;
+  const size_t row_bytes = ARROWS ? 6 * sizeof(double) : 3 * sizeof(float);
+  rc = grow(h, h->mc_out, id_bytes + row_bytes * (size_t)total, 0, false);
+  if (rc) return rc;
+  char* base = h->mc_out;
+  o.xyz = (float*)base; o.ids = (int32_t*)base; o.seg = (double*)(base + id_bytes);
+  k_mapcloud<ARROWS, true><<<grid, MC_THREADS, 0, h->stream>>>(h->dc, h->map, h->normal, h->center[2], cnt, off, g, o);
+  LAUNCH_CHECK();
+  if (ARROWS) {
+    CK(cudaMemcpyAsync(ids, o.ids, sizeof(int32_t) * total, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(seg, o.seg, 6 * sizeof(double) * total, cudaMemcpyDeviceToHost, h->stream));
+  } else {
+    CK(cudaMemcpyAsync(xyz, o.xyz, 3 * sizeof(float) * total, cudaMemcpyDeviceToHost, h->stream));
+  }
   CK(cudaStreamSynchronize(h->stream));
   return EMAP_OK;
 }
@@ -1188,6 +1255,7 @@ emap_handle::~emap_handle() {
   if (pg_host) cudaFreeHost(pg_host);
   if (img_staged) { cudaEventSynchronize(img_staged); cudaEventDestroy(img_staged); }
   if (img_host) cudaFreeHost(img_host);
+  if (mc_count_host) cudaFreeHost(mc_count_host);
 }
 
 extern "C" {
@@ -1667,14 +1735,33 @@ int emap_get_submaps(emap_handle* h, int32_t n_windows, const double* windows, i
     if (rc) return rc;
     dst = h->d_export;
   }
-  k_submap<<<dim3(tiles, n_layers), dim3(32, SUBMAP_ROWS), 0, h->stream>>>(h->dc, h->map, h->normal, dst, a, h->center[2],
-                                                                           h->cfg.use_only_above_for_upper_bound);
+  const auto kern = export_has_colour(a.L) ? k_submap<true> : k_submap<false>;
+  kern<<<dim3(tiles, n_layers), dim3(32, SUBMAP_ROWS), 0, h->stream>>>(h->dc, h->map, h->normal, dst, a, h->center[2],
+                                                                       h->cfg.use_only_above_for_upper_bound);
   LAUNCH_CHECK();
   if (!out_is_device) {
     CK(cudaMemcpyAsync(out, dst, sizeof(float) * total, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
   }
   return EMAP_OK;
+}
+
+// The node's publishAsPointCloud (elevation_mapping_ros.cpp:501-505): the points of the exported elevation (map_cloud).
+int emap_get_map_points(emap_handle* h, float* xyz_host, int64_t* n_points) {
+  ENTER(h);
+  NvtxRange nv("emap:get_map_points");
+  if (!n_points || *n_points < 0 || (*n_points > 0 && !xyz_host))
+    return fail(h, EMAP_ERR_INVALID, "emap_get_map_points: null argument or negative capacity");
+  return map_cloud<false>(h, n_points, xyz_host, nullptr, nullptr);
+}
+
+// The node's publishNormalAsArrow (elevation_mapping_ros.cpp:751-778): the arrows of the exported normals (map_cloud).
+int emap_get_normal_arrows(emap_handle* h, int32_t* ids_host, double* segments_host, int64_t* n_arrows) {
+  ENTER(h);
+  NvtxRange nv("emap:get_normal_arrows");
+  if (!n_arrows || *n_arrows < 0 || (*n_arrows > 0 && (!ids_host || !segments_host)))
+    return fail(h, EMAP_ERR_INVALID, "emap_get_normal_arrows: null argument or negative capacity");
+  return map_cloud<true>(h, n_arrows, nullptr, ids_host, segments_host);
 }
 
 int emap_layer_device_ptr(emap_handle* h, const char* name, void** ptr) {

@@ -69,6 +69,7 @@ inline void submap_window(int cell_n, double res, const double m[2], const doubl
 // One CTA per (window row tile, layer): warp y writes output row SUBMAP_ROWS * tile + y of the window, lane by lane
 // along the row.  Lane k reads state column c0 - k: the warp's 32 addresses are the same 128-byte span as a forward
 // read, and the memory system coalesces by address, not by lane order, so neither reads nor writes need staging.
+template <bool COLOUR>
 __global__ void __launch_bounds__(32 * SUBMAP_ROWS)
 k_submap(const DevCfg c, const float* __restrict__ map, const float* __restrict__ normal, float* __restrict__ out,
          const __grid_constant__ SubmapArgs a, float center_z, int only_above) {
@@ -87,5 +88,5 @@ k_submap(const DevCfg c, const float* __restrict__ map, const float* __restrict_
   float* dst = out + w.off + ((long long)l * rows + rr) * cols;
   const int sr = w.r0 - rr;
   for (int cc = (int)threadIdx.x; cc < cols; cc += 32)
-    dst[cc] = export_cell(c, map, normal, sr, w.c0 - cc, kind, center_z, only_above, plane, flags);
+    dst[cc] = export_cell<COLOUR>(c, map, normal, sr, w.c0 - cc, kind, center_z, only_above, plane, flags);
 }

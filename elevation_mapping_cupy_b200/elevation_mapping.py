@@ -17,6 +17,9 @@ one kernel projects every map cell into the image, tests occlusion along the lin
 channel (csrc/emap_image.cuh), bit-identical to the reference's kernels on the same card.
 Windows of the exported map (get_submap / get_submaps, the node's get_raw_submap service) come from one library call
 and one kernel per batch (csrc/emap_submap.cuh).
+The rest of the node's map timer is served too: the normals (get_normal_maps / get_normal_ref), the bridge's normal
+colour as the exported layer `normal_color`, and the exported map as a point cloud (get_map_points) and as normal arrows
+(get_normal_arrows), compacted in grid_map's cell order on the device (csrc/emap_mapcloud.cuh).
 Out of scope (SURVEY.md section 8): the image feature extractors.
 """
 import ctypes as C
@@ -32,7 +35,7 @@ from .semantic_map import SemanticMap
 
 LAYER_NAMES = ["elevation", "variance", "is_valid", "traversability", "time", "upper_bound", "is_upper_bound"]
 EXPORT_NAMES = ["elevation", "variance", "traversability", "time", "upper_bound", "is_upper_bound",
-                "normal_x", "normal_y", "normal_z"]
+                "normal_x", "normal_y", "normal_z", "normal_color"]
 
 
 def config_from_parameter(param: Parameter) -> _lib.EmapConfig:
@@ -111,6 +114,9 @@ class ElevationMap:
         self._ring = np.zeros((2 * (self.cell_n - 2) + 1, 2), np.float64)
         self._mask = None
         self._batch_hull = np.zeros((4096, 2), np.float64)      # rings of get_polygons_traversability, grown on demand
+        # rows of get_map_points / get_normal_arrows, grown on demand
+        self._mc_points = [np.zeros((0, 3), np.float32)]
+        self._mc_arrows = [np.zeros(0, np.int32), np.zeros((0, 6), np.float64)]
 
     # ---- plumbing -------------------------------------------------------------------------
     def _check(self, rc):
@@ -458,6 +464,53 @@ class ElevationMap:
             result.append({"layers": views, "index": (r0, c0), "size": (rows, cols), "centre": centres[w].copy(),
                            "success": bool(ok)})
         return result
+
+    def get_normal_maps(self):
+        """EM.py:777-791: a new (3, cell_n-2, cell_n-2) float32 array of the exported normal_x, normal_y, normal_z.  One
+        kernel, one D2H copy, one sync."""
+        n = self.cell_n - 2
+        maps = np.zeros((3, n, n), np.float32)
+        with self.map_lock:
+            self._export([self._export_source(name) for name in ("normal_x", "normal_y", "normal_z")], maps)
+        return maps
+
+    def get_normal_ref(self, normal_x_data, normal_y_data, normal_z_data):
+        """EM.py:793-805 (WRAP:239-247 with enable_normal_color): the exported normals into three caller-owned
+        (cell_n-2, cell_n-2) arrays."""
+        maps = self.get_normal_maps()
+        normal_x_data[...] = maps[0]
+        normal_y_data[...] = maps[1]
+        normal_z_data[...] = maps[2]
+
+    def _map_cloud(self, attr, call):
+        """Runs emap_get_map_points / emap_get_normal_arrows into the grow-only buffers in self.<attr> (`call(bufs, n)`
+        issues the library call), growing them and retrying once when the map has more rows than they hold.  Returns
+        the number of rows."""
+        with self.map_lock:
+            self._after_framework()
+            for attempt in range(2):
+                bufs = getattr(self, attr)
+                n = C.c_int64(len(bufs[0]))
+                rc = call(bufs, n)
+                if rc == 0 or attempt or n.value <= len(bufs[0]):
+                    self._check(rc)
+                    return n.value
+                setattr(self, attr, [np.zeros((n.value,) + b.shape[1:], b.dtype) for b in bufs])
+
+    def get_map_points(self):
+        """The node's publishAsPointCloud (elevation_mapping_ros.cpp:501-505): an (M, 3) float32 array of (x, y, z), one
+        row per cell of the exported map whose elevation is finite, in grid_map's column-major cell order (include/emap.h
+        states the rule).  On the device, with the count and the rows read back once each."""
+        m = self._map_cloud("_mc_points", lambda b, n: self._L.emap_get_map_points(self._h, b[0].ctypes.data, C.byref(n)))
+        return self._mc_points[0][:m].copy()
+
+    def get_normal_arrows(self):
+        """The node's publishNormalAsArrow (elevation_mapping_ros.cpp:751-778): (ids, segments), an (M,) int32 array of
+        marker ids (the cells' column-major linear index) and an (M, 6) float64 array of (start, end) = ((x, y, z),
+        (x, y, z) + 0.1 * normal), one row per valid cell whose normal is not shorter than 0.1 (include/emap.h)."""
+        m = self._map_cloud("_mc_arrows", lambda b, n: self._L.emap_get_normal_arrows(self._h, b[0].ctypes.data,
+                                                                                       b[1].ctypes.data, C.byref(n)))
+        return self._mc_arrows[0][:m].copy(), self._mc_arrows[1][:m].copy()
 
     def get_state(self):
         """Host copies (map (7,W,W), normal (3,W,W)) -- tests / checkpointing."""

@@ -219,7 +219,14 @@ int emap_get_position(emap_handle* h, double out[3]);          /* EM.py:130-137 
 
 /* ---- export: EM.py:720-775 get_map_with_name_ref (WRAP:205-252): NaN-fill, +center_z, crop the
  * border ring, flip both axes; writes (cell_n-2)^2 floats to caller memory.  Names: elevation,
- * variance, traversability, time, upper_bound, is_upper_bound, normal_x, normal_y, normal_z. ---- */
+ * variance, traversability, time, upper_bound, is_upper_bound, normal_x, normal_y, normal_z, normal_color.
+ * normal_color is the C++ bridge's addNormalColorLayer (WRAP:296-314, enable_normal_color), which the bridge stores as
+ * its `color` layer, for every exported cell, from the exported normal_x/y/z: cx = float((nx + 1.0) / 2.0),
+ * cy = float((ny + 1.0) / 2.0) (computed in double), cz = nz; each channel is int(c * 255.0f) (a float product truncated
+ * toward zero); the value is the float whose bits are (r << 16) | (g << 8) | b (grid_map's colorVectorToValue).  Where
+ * the reference leaves it undefined: a channel whose product is NaN is 0, one beyond the int32 range saturates, and a
+ * negative channel contributes its 32-bit two's complement to the OR.  This is restated from grid_map's published
+ * source and was not checked against a grid_map build. ---- */
 int emap_get_map_with_name(emap_handle* h, const char* name, float* out_host, int64_t n_out);
 /* Batched export: what WRAP:213-252 (ElevationMappingWrapper::get_grid_map) does layer by layer -- n layers with ONE
  * kernel, one device-to-host copy, one synchronisation.  names[k] is a basic layer of emap_get_map_with_name, or
@@ -259,6 +266,27 @@ int emap_submap_windows(int32_t cell_n, double resolution, const double center[2
 int emap_get_submaps(emap_handle* h, int32_t n_windows, const double* windows, int32_t n_layers, const char* const* names,
                      const float* const* planes_device, const int32_t* flags, float* out, int32_t out_is_device,
                      int64_t out_floats, int32_t* info, double* centres);
+/* ---- the exported map as a point cloud and as normal arrows: the ROS node's publishAsPointCloud
+ * (elevation_mapping_ros.cpp:501-505, grid_map's toPointCloud(map, {"elevation"}, "elevation")) and publishNormalAsArrow
+ * (:751-778), restated from grid_map's published source (not checked against a grid_map build).  Coordinates are those of
+ * emap_get_layers' output (exported cell (r, c) is state cell (cell_n-2-r, cell_n-2-c)).  Cells are visited in grid_map's
+ * storage order, column-major over the exported map: linear index i = c * (cell_n-2) + r.  A cell's position, in double:
+ *   x = (cx + (0.5 * L - 0.5 * res)) - res * r,   y = (cy + (0.5 * L - 0.5 * res)) - res * c,
+ * with (cx, cy) the handle's fp32 centre widened to double, res the resolution and L = (cell_n-2) * res
+ * (getPositionFromIndex with the geometry get_grid_map sets).
+ * emap_get_map_points: one row (float x, float y, float z) per cell whose exported elevation is finite, in that order;
+ * x and y are the positions rounded to float, z is the exported elevation bit for bit.
+ * emap_get_normal_arrows: one arrow per cell whose exported elevation is finite and whose exported normal n is not
+ * shorter than 0.1 (skipped when sqrt((nx^2 + ny^2) + nz^2) < 0.1 in double, the reference's test, so a normal that is
+ * not a number keeps its arrow; the frame never writes one), in that order.  ids[k] = the cell's linear index i (the
+ * marker id); segments[6k .. 6k+5] = (start, end) in double: start = (x, y, elevation), end = start + n * 0.1 per component.
+ * *n_points / *n_arrows: the capacity in rows on entry, the number of rows on return.  A capacity below it returns
+ * EMAP_ERR_INVALID with the needed number in *n_points / *n_arrows and writes nothing to the rows.  The outputs may be
+ * NULL when the capacity is 0 (a count query).  EMAP_ERR_INVALID for a NULL count, a negative capacity or a NULL output
+ * with a capacity above 0.  Host output: two synchronisations per call (one for the count, one for the rows); the work
+ * is ordered on the handle's stream like the other exports and leaves the map state unchanged. */
+int emap_get_map_points(emap_handle* h, float* xyz_host, int64_t* n_points);
+int emap_get_normal_arrows(emap_handle* h, int32_t* ids_host, double* segments_host, int64_t* n_arrows);
 /* EM.py:807-835 get_layer / raw state access: device pointer of a (W,W) fp32 plane.  Names: the 7
  * layers of EM.py:69-77, normal_x/y/z, traversability_input.  `elevation_map` returns the (7,W,W)
  * base, `normal_map` the (3,W,W) base.  Pointers stay valid until the next emap_move / emap_move_to / emap_destroy. */
