@@ -51,7 +51,6 @@ class DevBuf {
     if (p_) cudaFree(p_);
     p_ = nullptr; n_ = 0;
   }
-  void swap(DevBuf& o) { std::swap(p_, o.p_); std::swap(n_, o.n_); }
 
  private:
   T* p_ = nullptr;
@@ -76,10 +75,9 @@ struct emap_handle {
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;     // side-stream fork / join of the deferred fusion pushes
   cudaEvent_t ev_order = nullptr;                       // emap_wait_for_stream / emap_stream_wait_for
   // state
-  DevBuf<float> map;          // (7,W,W)
-  DevBuf<float> map_alt;      // shift target
-  CUtensorMap post_tm[2];     // TMA descriptors of the two state buffers as (W, W, 7) fp32 tensors, box = k_post's staged tile
-  const float* post_tm_base[2] = {nullptr, nullptr};
+  DevBuf<float> map;          // (7,W,W); the same buffer for the handle's lifetime (captured frames bind it)
+  DevBuf<float> map_alt;      // shift target, copied back into map
+  CUtensorMap post_tm;        // TMA descriptor of map as a (W, W, 7) fp32 tensor, box = k_post's staged tile
   DevBuf<float> normal;       // (3,W,W)
   DevBuf<float> trav_input;
   float center[3] = {0, 0, 0};        // fp32 like EM.py:61
@@ -670,10 +668,10 @@ size_t post_smem(const DevCfg& d) {
   return sizeof(float) * (3 * plane + (size_t)(PT_Y + 6) * (PT_X + 6) + 2) + sizeof(unsigned long long) * (size_t)(PT_Y + 2 * HL + 2);
 }
 
-// TMA descriptor of one state buffer for k_post: tensor (x = column, y = row, z = layer), box = staged tile + halo of one
+// TMA descriptor of the state buffer for k_post: tensor (x = column, y = row, z = layer), box = staged tile + halo of one
 // layer; out-of-range elements are filled with zeros.  cuTensorMapEncodeTiled is fetched from the driver at run time
 // (no link-time dependency on libcuda).
-int make_post_tm(emap_handle* h, int which, const float* base) {
+int make_post_tm(emap_handle* h) {
   typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -685,8 +683,7 @@ int make_post_tm(emap_handle* h, int which, const float* base) {
       return fail(h, EMAP_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
     enc = (encode_fn)fn;
   }
-  memset(&h->post_tm[which], 0, sizeof(CUtensorMap));
-  h->post_tm_base[which] = base;
+  memset(&h->post_tm, 0, sizeof(CUtensorMap));
   const int W = h->dc.W;
   const int HL = h->dc.dilation + 3, HLX = (HL + 3) & ~3;
   // plain loads instead when the row pitch is not a multiple of 16 bytes, or the map is smaller than one staged box
@@ -696,7 +693,7 @@ int make_post_tm(emap_handle* h, int which, const float* base) {
   const cuuint64_t strides[2] = {(cuuint64_t)W * 4, (cuuint64_t)W * W * 4};
   const cuuint32_t box[3] = {(cuuint32_t)(PT_X + 2 * HLX), (cuuint32_t)(PT_Y + 2 * HL), 1};
   const cuuint32_t es[3] = {1, 1, 1};
-  const CUresult r = enc(&h->post_tm[which], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)base, dims, strides, box, es,
+  const CUresult r = enc(&h->post_tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void*)(float*)h->map, dims, strides, box, es,
                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(h, EMAP_ERR_CUDA, "cuTensorMapEncodeTiled failed");
@@ -706,7 +703,7 @@ int make_post_tm(emap_handle* h, int which, const float* base) {
 int launch_post(emap_handle* h) {
   dim3 grid(cdiv(h->dc.W, PT_X), cdiv(h->dc.W, PT_Y));
   const size_t sm = post_smem(h->dc);
-  const CUtensorMap& tm = h->post_tm[h->post_tm_base[1] == h->map ? 1 : 0];
+  const CUtensorMap& tm = h->post_tm;
   switch (h->dc.dilation) {
     case 1: PDL(k_post<1>, grid, 256, sm, h->dc, h->map, h->trav_input, h->normal, tm); break;
     case 2: PDL(k_post<2>, grid, 256, sm, h->dc, h->map, h->trav_input, h->normal, tm); break;
@@ -1185,7 +1182,7 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   k_build_step_cnt<<<cdiv(0x7c01, 256), 256, 0, h->stream>>>((const float*)(h->steps + 1), h->dc.n_steps, h->step_cnt);
   k_init<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc, h->map);
   h->launches += 2;
-  if (make_post_tm(h, 0, h->map) || make_post_tm(h, 1, h->map_alt)) {
+  if (make_post_tm(h)) {
     g_create_error = h->err; delete h; return EMAP_ERR_CUDA;
   }
   if (post_smem(h->dc) > 48 * 1024)
@@ -1291,7 +1288,12 @@ int emap_input_sensors(emap_handle* h, int32_t n_sensors, const void* const* poi
   if ((rc = frame_semantic(h))) return rc;
   if ((rc = frame_rays(h))) return rc;
   if ((rc = frame_finish(h))) return rc;
-  if (!is_device_ptr || h->zero_copy_pending) CK(cudaEventSynchronize(h->copy_done));   // caller may reuse its host buffers on return
+  if (!is_device_ptr || h->zero_copy_pending) {      // caller may reuse its host buffers on return
+    // a captured frame runs nothing yet: it reads the caller's pinned cloud at every replay instead
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    CK(cudaStreamIsCapturing(h->stream, &cs));
+    if (cs == cudaStreamCaptureStatusNone) CK(cudaEventSynchronize(h->copy_done));
+  }
   h->zero_copy_pending = false;
   return EMAP_OK;
 }
@@ -1576,8 +1578,9 @@ static int shift_map(emap_handle* h, int sx, int sy, double dz) {
     PER_CELL(k_shift_z, h->dc, h->map, dz);
     return 0;
   }
+  // shifted into map_alt and copied back: map keeps its address, which captured frames and the caller's views hold
   PER_CELL(k_shift, h->dc, h->map, h->map_alt, sx, sy, dz);
-  h->map.swap(h->map_alt);
+  CK(cudaMemcpyAsync(h->map, h->map_alt, sizeof(float) * 7 * (size_t)h->dc.C, cudaMemcpyDeviceToDevice, h->stream));
   return 0;
 }
 

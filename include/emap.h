@@ -398,7 +398,22 @@ int emap_input_image(emap_handle* h, int32_t n_planes, const float* image, int i
 int emap_sync(emap_handle* h);
 int emap_stream(emap_handle* h, void** cuda_stream);
 /* Run this handle's work on a caller-owned stream (e.g. the framework's current stream); NULL restores
- * the handle's own stream. */
+ * the handle's own stream.
+ *
+ * A frame (emap_input_pointcloud / emap_input_sensors) from device memory makes no host synchronisation, and one from
+ * page-locked host memory waits only for the kernel that reads the cloud (not while the stream is being captured), so
+ * either can be captured into a CUDA graph on that stream.  The graph binds, at capture:
+ *   - the cloud pointer(s), row counts, row stride and dtype (a replay reads the same memory again: keep it alive and
+ *     write the next cloud into it; a page-locked host cloud is read over PCIe at every replay);
+ *   - the sensor pose relative to the map centre at capture (and the ray box derived from it);
+ *   - the semantic configuration (emap_semantic_configure*) and ray counting (emap_set_ray_counting).
+ * The state buffer itself keeps its address for the handle's lifetime (moves shift it in place), so moves, ticks and
+ * other calls may run between capture and replay.  A replay is valid only at the capture centre, bit for bit: move back
+ * to it (emap_get_position) before replaying.  A replay runs after what is already queued on the stream it is launched
+ * on; order it after the caller's other streams, as emap_wait_for_stream does for eager calls.
+ * Invalidates a graph: any call that grows the handle's buffers (a frame with more points or sensors than any frame
+ * before it, a new semantic configuration, more class_max slots): run an eager frame of the largest size and
+ * configuration first, then capture.  Cannot be captured: pageable host clouds (staged with a synchronising copy). */
 int emap_set_stream(emap_handle* h, void* cuda_stream);
 /* Stream ordering WITHOUT host synchronisation between the handle's stream and a stream of the caller's framework
  * (torch / CuPy current stream; NULL = the legacy default stream): after emap_wait_for_stream the handle's next work runs

@@ -20,6 +20,26 @@ def compare_state(eng_map, eng_normal, om, trav_tol=2e-6, exact_layers=(0, 1, 2,
     assert np.array_equal(eng_normal, om.normal_map), f"{label} normals differ: max {np.abs(eng_normal - om.normal_map).max()}"
 
 
+def check_frame(em, om, n, label, counted=False, nan_rows=None):
+    """state, point record and frame statistics of the last frame of `em` against the oracle's"""
+    state, normal = em.get_state()
+    compare_state(state, normal, om, label=label)
+    idx, valid, inside = em.get_point_record(n)
+    oi, ov, oin = om.last_point_record
+    ok = np.ones(n, bool) if nan_rows is None else ~nan_rows
+    assert np.array_equal(idx[ok], oi[ok]), label
+    assert np.array_equal(valid, ov) and np.array_equal(inside, oin), label
+    st = em.get_frame_stats()
+    assert st.n_points == n, label
+    assert st.n_valid_points == int(ov.sum()), label
+    assert st.error_cnt == om.stats.error_cnt and st.drift_applied == om.stats.drift_applied, label
+    if om.stats.drift_evaluated:
+        assert np.float32(st.mean_error) == np.float32(om.stats.mean_error), label
+    if counted:
+        assert (st.ray_steps, st.ray_visits) == (om.stats.ray_steps, om.stats.ray_visits), label
+    return st, state, normal
+
+
 # Seeded inputs of the comparisons with the reference's kernel source (tests/test_oracle_cpu.py); the reference's
 # outputs on them are stored under tests/golden/ by tests/golden/make_golden.py.
 STAR_R = np.array([[0.9, 0.1, -0.2], [0.0, 1.0, 0.1], [0.15, -0.12, 0.97]], np.float32)

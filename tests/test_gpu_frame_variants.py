@@ -8,7 +8,7 @@ import numpy as np
 import pytest
 
 import frame_variants as fv
-from helpers import compare_state
+from helpers import check_frame as _check_frame, compare_state
 
 pytestmark = pytest.mark.gpu
 
@@ -38,26 +38,6 @@ def _random_state(W, seed, valid_frac=0.2):
     st[5] = rng.standard_normal((W, W)); st[6] = (rng.random((W, W)) < 0.1) * (st[2] < 0.5)
     st[0] *= st[2]
     return st
-
-
-def _check_frame(em, om, n, label, counted=False, nan_rows=None):
-    """state, point record and frame statistics of the last frame of `em` against the oracle's"""
-    state, normal = em.get_state()
-    compare_state(state, normal, om, label=label)
-    idx, valid, inside = em.get_point_record(n)
-    oi, ov, oin = om.last_point_record
-    ok = np.ones(n, bool) if nan_rows is None else ~nan_rows
-    assert np.array_equal(idx[ok], oi[ok]), label
-    assert np.array_equal(valid, ov) and np.array_equal(inside, oin), label
-    st = em.get_frame_stats()
-    assert st.n_points == n, label
-    assert st.n_valid_points == int(ov.sum()), label
-    assert st.error_cnt == om.stats.error_cnt and st.drift_applied == om.stats.drift_applied, label
-    if om.stats.drift_evaluated:
-        assert np.float32(st.mean_error) == np.float32(om.stats.mean_error), label
-    if counted:
-        assert (st.ray_steps, st.ray_visits) == (om.stats.ray_steps, om.stats.ray_visits), label
-    return st, state, normal
 
 
 # ---- A: resolution, ray length and map size -------------------------------------------------------------------------
