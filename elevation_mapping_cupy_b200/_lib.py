@@ -74,6 +74,8 @@ SIGNATURES = {
     "emap_update_time": (C.c_int, [C.c_void_p]),
     "emap_update_normal": (C.c_int, [C.c_void_p, C.c_void_p]),
     "emap_initialize_map_finish": (C.c_int, [C.c_void_p, C.c_int32, C.c_int32]),
+    "emap_initialize_map": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p,
+                                      C.c_double, C.c_int32]),
     "emap_get_position": (C.c_int, [C.c_void_p, C.c_void_p]),
     "emap_get_map_with_name": (C.c_int, [C.c_void_p, C.c_char_p, C.c_void_p, C.c_int64]),
     "emap_get_layers": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int32),

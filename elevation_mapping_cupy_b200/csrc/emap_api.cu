@@ -20,6 +20,7 @@
 #include "emap_image.cuh"
 #include "emap_submap.cuh"
 #include "emap_mapcloud.cuh"
+#include "emap_initialize.cuh"
 
 namespace {
 
@@ -161,6 +162,12 @@ struct emap_handle {
   DevBuf<int> mc_table;
   DevBuf<char> mc_out;
   int* mc_count_host = nullptr;
+  // emap_initialize_map (allocated on first use, grown to the largest call): the device copy of the upload, its pinned
+  // staging and the event after which the staging may be overwritten
+  DevBuf<char> init_dev;
+  char* init_host = nullptr;
+  size_t init_host_bytes = 0;
+  cudaEvent_t init_staged = nullptr;
   // misc
   int64_t launches = 0;
   int count_rays = 0;
@@ -1253,6 +1260,32 @@ emap_handle::~emap_handle() {
   if (img_staged) { cudaEventSynchronize(img_staged); cudaEventDestroy(img_staged); }
   if (img_host) cudaFreeHost(img_host);
   if (mc_count_host) cudaFreeHost(mc_count_host);
+  if (init_staged) { cudaEventSynchronize(init_staged); cudaEventDestroy(init_staged); }
+  if (init_host) cudaFreeHost(init_host);
+}
+
+// EM.py:119-128 clear
+int clear_map(emap_handle* h) {
+  PER_CELL(k_clear, h->dc, h->map);
+  CK(cudaMemsetAsync(&h->fs->mean_error, 0, 2 * sizeof(float), h->stream));     // EM.py:127-128
+  return EMAP_OK;
+}
+
+// EM.py:913-922 after the interpolation: `iterations` Jacobi passes of the initialiser dilation, then
+// upper_bound <- elevation on valid cells
+int initialize_finish(emap_handle* h, int32_t dilation_size, int32_t iterations) {
+  if (dilation_size < 0 || dilation_size > 64 || iterations < 0 || iterations > 16)
+    return fail(h, EMAP_ERR_INVALID, "emap_initialize_map_finish: 0 <= dilation_size <= 64, 0 <= iterations <= 16");
+  int rc = alloc_plugin_scratch(h);
+  if (rc) return rc;
+  const size_t B = sizeof(float) * (size_t)h->dc.C;
+  const int passes = dilation_size > 0 ? iterations : 0;
+  for (int it = 0; it < std::max(passes, 1); it++) {
+    CK(cudaMemcpyAsync(h->pl[0], h->map, B, cudaMemcpyDeviceToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->pl[1], h->map + 2 * (size_t)h->dc.C, B, cudaMemcpyDeviceToDevice, h->stream));
+    PER_CELL(k_init_dilate, h->dc, h->pl[0], h->pl[1], h->map, passes ? dilation_size : 0, it == std::max(passes, 1) - 1);
+  }
+  return EMAP_OK;
 }
 
 extern "C" {
@@ -1609,9 +1642,7 @@ int emap_move(emap_handle* h, const double d[3]) {
 
 int emap_clear(emap_handle* h) {
   ENTER(h);
-  PER_CELL(k_clear, h->dc, h->map);
-  CK(cudaMemsetAsync(&h->fs->mean_error, 0, 2 * sizeof(float), h->stream));     // EM.py:127-128
-  return EMAP_OK;
+  return clear_map(h);
 }
 
 int emap_update_variance(emap_handle* h) {
@@ -1636,18 +1667,133 @@ int emap_update_normal(emap_handle* h, const float* dilated) {
 // `iterations` Jacobi passes of the initialiser dilation, then upper_bound <- elevation on valid cells.
 int emap_initialize_map_finish(emap_handle* h, int32_t dilation_size, int32_t iterations) {
   ENTER(h);
-  if (dilation_size < 0 || dilation_size > 64 || iterations < 0 || iterations > 16)
-    return fail(h, EMAP_ERR_INVALID, "emap_initialize_map_finish: 0 <= dilation_size <= 64, 0 <= iterations <= 16");
-  int rc = alloc_plugin_scratch(h);
+  return initialize_finish(h, dilation_size, iterations);
+}
+
+// EM.py:899-922 + map_initializer.py:25-62 on the device (include/emap.h, csrc/emap_initialize.cuh): clear, snap, the
+// host part (triangulation, gradients, coefficients, tile lists), one upload, one interpolation kernel, then the
+// dilation passes and the upper-bound fill of emap_initialize_map_finish.
+int emap_initialize_map(emap_handle* h, const float* xyz_host, int32_t n_points, int32_t method,
+                        const int32_t* triangles_host, int32_t n_triangles, const double* gradients_host,
+                        double initialized_variance, int32_t dilation_size_initialize) {
+  ENTER(h);
+  NvtxRange nv("emap:initialize_map");
+  int rc = clear_map(h);                 // EM.py:906: every failure below leaves the map cleared
   if (rc) return rc;
-  const size_t B = sizeof(float) * (size_t)h->dc.C;
-  const int passes = dilation_size > 0 ? iterations : 0;
-  for (int it = 0; it < std::max(passes, 1); it++) {
-    CK(cudaMemcpyAsync(h->pl[0], h->map, B, cudaMemcpyDeviceToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->pl[1], h->map + 2 * (size_t)h->dc.C, B, cudaMemcpyDeviceToDevice, h->stream));
-    PER_CELL(k_init_dilate, h->dc, h->pl[0], h->pl[1], h->map, passes ? dilation_size : 0, it == std::max(passes, 1) - 1);
+  if (!xyz_host) return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: null points");
+  if (n_points <= 3) return fail(h, EMAP_ERR_INVALID, "Initialization points must be more than 3.");
+  if (n_points > EMAP_INIT_MAX_POINTS)
+    return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: more than EMAP_INIT_MAX_POINTS points");
+  if (method < 0 || method > 2) return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: method must be 0 (nearest), 1 (linear) or 2 (cubic)");
+  if (triangles_host && (n_triangles < 1 || n_triangles > 2 * EMAP_INIT_MAX_POINTS))
+    return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: 1 to 2 * EMAP_INIT_MAX_POINTS triangles required");
+  if (dilation_size_initialize < 0 || dilation_size_initialize > 64 || !std::isfinite(initialized_variance))
+    return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: 0 <= dilation_size_initialize <= 64 and a finite variance required");
+  // transform_to_map_index as elevation_mapping.py applies it, in fp32: ((xy - center) / res + W / 2), truncated
+  const int W = h->dc.W, n = n_points;
+  const float res_f = (float)h->cfg.resolution, half_f = (float)(0.5 * W);
+  std::vector<long long> xy(2 * (size_t)n);
+  std::vector<double> z(n);
+  bool narrow = true;
+  for (int i = 0; i < n; i++) {
+    const float* q = xyz_host + 3 * (size_t)i;
+    if (!std::isfinite(q[0]) || !std::isfinite(q[1]) || !std::isfinite(q[2]))
+      return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: non-finite point");
+    for (int d = 0; d < 2; d++) {
+      const float v = (q[d] - h->center[d]) / res_f;
+      const float c = v + half_f;
+      if (!(c >= -2147483648.f && c < 2147483648.f))
+        return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: a point's cell index is outside the int32 range");
+      xy[2 * i + d] = (long long)(int32_t)c;
+      narrow &= std::llabs(xy[2 * i + d]) <= INIT_NARROW;
+    }
+    z[i] = (double)(float)(q[2] - h->center[2]);
   }
-  return EMAP_OK;
+  InitArgs a;
+  memset(&a, 0, sizeof(a));
+  a.W = W; a.C = h->dc.C; a.tiles_x = (W + INIT_TILE - 1) / INIT_TILE;
+  a.var = (float)initialized_variance;
+  // the upload: one block, 256-byte aligned arrays, the same layout in pinned and in device memory
+  std::vector<int> tri, nb, off, list;
+  std::vector<double> grad, coef;
+  size_t bytes = 0;
+  auto carve = [&](size_t n_bytes) { const size_t o = bytes; bytes += (n_bytes + 255) & ~(size_t)255; return o; };
+  size_t o_pxy = 0, o_pz = 0, o_txy = 0, o_coef = 0, o_off = 0, o_list = 0;
+  if (method == 0) {
+    a.n = n;
+    o_pxy = carve(sizeof(int2) * n);
+    o_pz = carve(sizeof(float) * n);
+  } else {
+    if (triangles_host) {
+      tri.assign(triangles_host, triangles_host + 3 * (size_t)n_triangles);
+      for (int t = 0; t < n_triangles; t++) {
+        int* v = &tri[3 * (size_t)t];
+        if (v[0] < 0 || v[0] >= n || v[1] < 0 || v[1] >= n || v[2] < 0 || v[2] >= n)
+          return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: triangle index outside [0, n_points)");
+        const int o = init_host::orient_sign(&xy[2 * (size_t)v[0]], &xy[2 * (size_t)v[1]], &xy[2 * (size_t)v[2]]);
+        if (o == 0) return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: a triangle of zero area");
+        if (o < 0) std::swap(v[1], v[2]);
+      }
+    } else if (!init_host::delaunay(xy, tri)) {
+      return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: the points are collinear (no triangulation)");
+    }
+    const int T = (int)(tri.size() / 3);
+    a.n = T;
+    if (method == 2) {
+      init_host::neighbours(tri, nb);
+      if (!gradients_host) init_host::estimate_gradients(xy, z, tri, grad);
+      coef.resize((size_t)INIT_CT * T);
+      init_host::ct_coefficients(xy, z, gradients_host ? gradients_host : grad.data(), tri, nb, coef.data());
+    } else {
+      coef.resize(3 * (size_t)T);
+      for (size_t k = 0; k < coef.size(); k++) coef[k] = z[tri[k]];
+    }
+    init_host::bin_tiles(W, xy, tri, off, list);
+    o_txy = carve(sizeof(int) * 6 * (size_t)T);
+    o_coef = carve(sizeof(double) * coef.size());
+    o_off = carve(sizeof(int) * off.size());
+    o_list = carve(sizeof(int) * std::max<size_t>(list.size(), 1));
+  }
+  rc = grow(h, h->init_dev, bytes, 0, false);
+  if (rc) return rc;
+  if (!h->init_staged) CK(cudaEventCreateWithFlags(&h->init_staged, cudaEventDisableTiming));
+  else CK(cudaEventSynchronize(h->init_staged));          // the previous call's upload has left the staging
+  if (h->init_host_bytes < bytes) {
+    if (h->init_host) { cudaFreeHost(h->init_host); h->init_host = nullptr; h->init_host_bytes = 0; }
+    CK(cudaHostAlloc((void**)&h->init_host, bytes, cudaHostAllocDefault));
+    h->init_host_bytes = bytes;
+  }
+  char* hb = h->init_host;
+  char* db = h->init_dev;
+  if (method == 0) {
+    int2* pxy = (int2*)(hb + o_pxy);
+    float* pz = (float*)(hb + o_pz);
+    for (int i = 0; i < n; i++) { pxy[i] = make_int2((int)xy[2 * i], (int)xy[2 * i + 1]); pz[i] = (float)z[i]; }
+    a.pxy = (const int2*)(db + o_pxy); a.pz = (const float*)(db + o_pz);
+  } else {
+    int* txy = (int*)(hb + o_txy);
+    for (size_t k = 0; k < tri.size(); k++) { txy[2 * k] = (int)xy[2 * (size_t)tri[k]]; txy[2 * k + 1] = (int)xy[2 * (size_t)tri[k] + 1]; }
+    memcpy(hb + o_coef, coef.data(), sizeof(double) * coef.size());
+    memcpy(hb + o_off, off.data(), sizeof(int) * off.size());
+    if (!list.empty()) memcpy(hb + o_list, list.data(), sizeof(int) * list.size());
+    a.txy = (const int*)(db + o_txy); a.coef = (const double*)(db + o_coef);
+    a.tile_off = (const int*)(db + o_off); a.tile_tri = (const int*)(db + o_list);
+  }
+  CK(cudaMemcpyAsync(db, hb, bytes, cudaMemcpyHostToDevice, h->stream));
+  CK(cudaEventRecord(h->init_staged, h->stream));
+  const int grid = a.tiles_x * a.tiles_x;
+  if (method == 0) {
+    if (narrow) k_init_nearest<long long><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
+    else k_init_nearest<__int128><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
+  } else if (method == 1) {
+    if (narrow) k_init_interp<long long, false><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
+    else k_init_interp<__int128, false><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
+  } else {
+    if (narrow) k_init_interp<long long, true><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
+    else k_init_interp<__int128, true><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
+  }
+  LAUNCH_CHECK();
+  return initialize_finish(h, dilation_size_initialize, 2);
 }
 
 int emap_get_position(emap_handle* h, double out[3]) {

@@ -36,6 +36,7 @@ from .semantic_map import SemanticMap
 LAYER_NAMES = ["elevation", "variance", "is_valid", "traversability", "time", "upper_bound", "is_upper_bound"]
 EXPORT_NAMES = ["elevation", "variance", "traversability", "time", "upper_bound", "is_upper_bound",
                 "normal_x", "normal_y", "normal_z", "normal_color"]
+INIT_METHODS = {"nearest": 0, "linear": 1, "cubic": 2}          # emap_initialize_map's method codes
 
 
 def config_from_parameter(param: Parameter) -> _lib.EmapConfig:
@@ -647,32 +648,33 @@ class ElevationMap:
 
     def initialize_map(self, points, method="cubic"):
         """EM.py:899-922 + map_initializer.py:25-62: clear the map, interpolate the given (x, y, z) points (map frame) over
-        the grid with scipy.interpolate.griddata ON THE HOST -- exactly what the reference does (it copies to NumPy for
-        griddata) -- then, on the device, dilate twice with dilation_size_initialize and set upper_bound to the elevation
-        of the valid cells.  Start-up path, not on the per-frame path."""
-        from scipy.interpolate import griddata
-        self.clear()
-        pts = np.array(_to_host(points), dtype=np.float32, copy=True)
-        center = self.center
-        W = self.cell_n
-        # transform_to_map_index (traversability_polygon.py:61-63): truncation toward zero, like astype(int32)
-        idx = ((pts[:, :2] - center[:2].reshape(1, 2)) / np.float32(self.resolution) + W / 2).astype(np.int32)
-        pts[:, :2] = idx.astype(np.float32)
-        pts[:, 2] -= center[2]
-        state, normal = self.get_state()
-        vi = np.where(state[2] > 0.5)
-        points_idx = np.vstack([np.stack(vi).T.astype(np.float32), pts[:, :2]])
-        values = np.hstack([state[0][vi], pts[:, 2]])
-        assert points_idx.shape[0] > 3, "Initialization points must be more than 3."
-        gx, gy = np.mgrid[0:W, 0:W]
-        interp = griddata(points_idx, values, (gx, gy), method=method)
-        ok = ~np.isnan(interp)
-        state[0] = np.nan_to_num(interp).astype(np.float32)
-        state[1] = np.where(ok, np.float32(self.param.initialized_variance), np.float32(self.param.initial_variance))
-        state[2] = ok.astype(np.float32)
+        the grid, dilate twice with dilation_size_initialize and set upper_bound to the elevation of the valid cells.
+        One library call (emap_initialize_map, include/emap.h) does it on the device.  linear / cubic use the
+        reference's own triangulation, scipy.spatial.Delaunay of the snapped points, and cubic SciPy's
+        Clough-Tocher gradients on it: O(points) host work."""
+        self.clear()                                           # EM.py:906; failures below leave the map cleared
+        pts = np.ascontiguousarray(_to_host(points), dtype=np.float32).reshape(-1, 3)
+        assert pts.shape[0] > 3, "Initialization points must be more than 3."
+        if method not in INIT_METHODS:
+            raise ValueError(f"Unknown interpolation method {method!r} for 2-D data")
+        tri = grad = None
+        if method != "nearest":
+            from scipy.spatial import Delaunay
+            # transform_to_map_index (traversability_polygon.py:61-63), as the library snaps: truncation toward zero
+            c = self.center
+            idx = ((pts[:, :2] - c[:2].reshape(1, 2)) / np.float32(self.resolution) + self.cell_n / 2).astype(np.int32)
+            d = Delaunay(idx.astype(np.float64))
+            tri = np.ascontiguousarray(d.simplices, dtype=np.int32)
+            if method == "cubic":
+                from scipy.interpolate import CloughTocher2DInterpolator
+                z = pts[:, 2] - c[2]
+                grad = np.ascontiguousarray(CloughTocher2DInterpolator(d, z.astype(np.float64)).grad[:, 0, :], np.float64)
         with self.map_lock:
-            self.set_state(state)
-            self._check(self._L.emap_initialize_map_finish(self._h, int(self.param.dilation_size_initialize), 2))
+            self._after_framework()
+            self._check(self._L.emap_initialize_map(
+                self._h, pts.ctypes.data, pts.shape[0], INIT_METHODS[method], None if tri is None else tri.ctypes.data,
+                0 if tri is None else tri.shape[0], None if grad is None else grad.ctypes.data,
+                float(self.param.initialized_variance), int(self.param.dilation_size_initialize)))
 
 
 def _to_host(x):

@@ -31,6 +31,9 @@ int main(void) {
   const float R[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, t[3] = {0, 0, 1.0f};
   const double pos[3] = {0, 0, 0};
   int rc = emap_move_to(h, pos, R);
+  /* the node's use_initializer_at_start: the base and the corners of a 1 m square, cubic, the library triangulates */
+  const float feet[15] = {0, 0, -1, -0.5f, -0.5f, -1, 0.5f, -0.5f, -1, 0.5f, 0.5f, -1, -0.5f, 0.5f, -1};
+  if (!rc) rc = emap_initialize_map(h, feet, 5, 2, NULL, 0, NULL, 10.0, 2);
   if (!rc) rc = emap_input_pointcloud(h, pts, N, 3, EMAP_F64, 0, R, t, 0.02f, 0.02f);
   if (!rc) rc = emap_update_variance(h);
   if (!rc) rc = emap_update_time(h);

@@ -210,11 +210,39 @@ int emap_update_time(emap_handle* h);
 /* EM.py:564-577 update_normal(dilated_map): device pointer to a (W,W) fp32 plane, or NULL for
  * the engine's own traversability_input. */
 int emap_update_normal(emap_handle* h, const float* dilated_map_device);
-/* EM.py:899-922 initialize_map, device half: after the caller has written the interpolated elevation / variance /
- * is_valid planes (emap_set_state; the interpolation itself is SciPy's griddata on the host in the reference too,
- * map_initializer.py:25-62), run `iterations` passes of the initialiser's dilation (CK.py:392-449 with
- * dilation_size_initialize, mask = is_valid) and update_upper_bound_with_valid_elevation (EM.py:428-432). */
+/* EM.py:899-922 initialize_map, device half only: after the caller has written interpolated elevation / variance /
+ * is_valid planes (emap_set_state), run `iterations` passes of the initialiser's dilation (CK.py:392-449 with
+ * dilation_size_initialize, mask = is_valid) and update_upper_bound_with_valid_elevation (EM.py:428-432).
+ * emap_initialize_map below does the whole initialisation, interpolation included, and runs this as its last step. */
 int emap_initialize_map_finish(emap_handle* h, int32_t dilation_size_initialize, int32_t iterations);
+/* EM.py:899-922 + map_initializer.py:25-62 initialize_map, on the device: clear the map (as emap_clear), then
+ * interpolate n_points (x, y, z) fp32 points in the map frame over every cell, then two passes of
+ * emap_initialize_map_finish with dilation_size_initialize.
+ *  - Snap: cell = (int32)((xy - center_xy) / (float)resolution + cell_n / 2) and z - center_z, all in fp32 (the
+ *    reference's transform_to_map_index).  Cell (i, j) is state element [i * cell_n + j].
+ *  - method 0 nearest: the point at the least squared cell distance, the lowest input index on a tie (SciPy's k-d tree
+ *    agrees whenever there are at most 10 points).  1 linear / 2 cubic: barycentric / Clough-Tocher (SciPy's
+ *    LinearNDInterpolator / CloughTocher2DInterpolator) over the triangles, in fp64.  A cell takes the lowest-index
+ *    triangle that contains it, edges and vertices included; cells outside every triangle keep the cleared values.
+ *  - Cells with a value get elevation = (float)value, variance = initialized_variance, is_valid = 1.
+ *  - triangles_host: (n_triangles, 3) indices into the points, either orientation, or NULL.  With NULL the library
+ *    triangulates: exact integer predicates, Bowyer-Watson inserting the points in input order from the seed (point
+ *    0, the first point that differs from it, the first point not collinear with those two); a point equal to an
+ *    earlier one is skipped; a point ON a triangle's circumcircle does not break it, so among four or more cocircular
+ *    points the triangles of the earlier points stay.  Triangles are then numbered in order of (lowest vertex, next
+ *    vertex counter-clockwise, last).
+ *  - gradients_host (cubic only): (n_points, 2) fp64 vertex gradients, or NULL for SciPy's
+ *    estimate_gradients_2d_global (tol 1e-6, maxiter 400, vertices in index order).
+ * EMAP_ERR_INVALID, with the map cleared: NULL points, n_points <= 3 (the reference's assertion), more than
+ * EMAP_INIT_MAX_POINTS, an unknown method, a non-finite point or one whose cell is outside the int32 range, collinear
+ * points (linear / cubic without triangles), a triangle index outside [0, n_points), a triangle of zero area,
+ * n_triangles outside [1, 2 * EMAP_INIT_MAX_POINTS].  One host-to-device upload of the points or of the triangles, their
+ * coefficients and tile lists, and kernels on the handle's stream: no device-to-host copy and no host synchronisation
+ * (except when the upload's staging grows, and a wait for the previous call's upload to leave it). */
+#define EMAP_INIT_MAX_POINTS 65536
+int emap_initialize_map(emap_handle* h, const float* xyz_host, int32_t n_points, int32_t method,
+                        const int32_t* triangles_host, int32_t n_triangles, const double* gradients_host,
+                        double initialized_variance, int32_t dilation_size_initialize);
 int emap_get_position(emap_handle* h, double out[3]);          /* EM.py:130-137 */
 
 /* ---- export: EM.py:720-775 get_map_with_name_ref (WRAP:205-252): NaN-fill, +center_z, crop the
