@@ -26,14 +26,9 @@ namespace {
 
 thread_local std::string g_create_error;
 
-struct StageTimer {
-  cudaEvent_t ev[9];
-  bool have = false;
-};
-
-// Owner of one device allocation of n elements of T: freed with its owner; grown by replacing it (grow() below).
-// Reads as a T* in kernel launches and pointer arithmetic.
-template <typename T>
+// Owner of one allocation of n elements of T, in device memory or (PINNED) in page-locked host memory: freed with its
+// owner; grown by replacing it (grow() below for device memory).  Reads as a T* in kernel launches and pointer arithmetic.
+template <typename T, bool PINNED = false>
 class DevBuf {
  public:
   DevBuf() = default;
@@ -44,18 +39,54 @@ class DevBuf {
   size_t size() const { return n_; }
   cudaError_t alloc(size_t n) {
     reset();
-    const cudaError_t e = cudaMalloc(&p_, sizeof(T) * n);
+    const cudaError_t e = PINNED ? cudaHostAlloc((void**)&p_, sizeof(T) * n, cudaHostAllocDefault)
+                                 : cudaMalloc(&p_, sizeof(T) * n);
     if (e == cudaSuccess) n_ = n; else p_ = nullptr;
     return e;
   }
   void reset() {
-    if (p_) cudaFree(p_);
+    if (p_) PINNED ? cudaFreeHost(p_) : cudaFree(p_);
     p_ = nullptr; n_ = 0;
   }
 
  private:
   T* p_ = nullptr;
   size_t n_ = 0;
+};
+
+template <typename T>
+using PinnedBuf = DevBuf<T, true>;
+
+// Owner of one stream or event: destroyed with its owner.  Reads as the raw cudaStream_t / cudaEvent_t.
+template <typename H, cudaError_t (*Create)(H*, unsigned), cudaError_t (*Destroy)(H)>
+class CudaHandle {
+ public:
+  CudaHandle() = default;
+  CudaHandle(const CudaHandle&) = delete;
+  CudaHandle& operator=(const CudaHandle&) = delete;
+  ~CudaHandle() { if (h_) Destroy(h_); }
+  operator H() const { return h_; }
+  cudaError_t create(unsigned flags) { return Create(&h_, flags); }
+
+ private:
+  H h_ = nullptr;
+};
+using Stream = CudaHandle<cudaStream_t, cudaStreamCreateWithFlags, cudaStreamDestroy>;
+using Event = CudaHandle<cudaEvent_t, cudaEventCreateWithFlags, cudaEventDestroy>;
+
+struct StageTimer {
+  Event ev[9];
+  bool have = false;
+};
+
+// A host-to-device upload through pinned staging, each buffer grown to the largest upload: the device copy kernels
+// read, its staging, and the event after which the staging may be overwritten.
+struct StagedUpload {
+  DevBuf<char> dev;
+  PinnedBuf<char> host;
+  Event staged;
+  int room(emap_handle* h, size_t n);      // both buffers hold n bytes, and the previous upload has left the staging
+  int send(emap_handle* h, size_t n);      // queues the upload of the first n staged bytes on the handle's stream
 };
 
 // sizes of the polygon check's scratch (carve_polygon): upload bytes, partials, column extremes, read-back bytes
@@ -72,9 +103,10 @@ struct emap_handle {
   int device = 0;
   std::mutex mu;
   std::string err;
-  cudaStream_t stream = nullptr, copy_stream = nullptr, own_stream = nullptr, side_stream = nullptr;
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;     // side-stream fork / join of the deferred fusion pushes
-  cudaEvent_t ev_order = nullptr;                       // emap_wait_for_stream / emap_stream_wait_for
+  cudaStream_t stream = nullptr;                        // own_stream or the caller's (emap_set_stream)
+  Stream own_stream, copy_stream, side_stream;
+  Event ev_fork, ev_join;                               // side-stream fork / join of the deferred fusion pushes
+  Event ev_order;                                       // emap_wait_for_stream / emap_stream_wait_for
   // state
   DevBuf<float> map;          // (7,W,W); the same buffer for the handle's lifetime (captured frames bind it)
   DevBuf<float> map_alt;      // shift target, copied back into map
@@ -101,7 +133,7 @@ struct emap_handle {
   int span_cells = 0;              // cells (per axis) one 31-step warp iteration of the march can span
   // points
   DevBuf<char> d_in[2];
-  cudaEvent_t in_free[2] = {nullptr, nullptr}, copy_done = nullptr;
+  Event in_free[2], copy_done;
   int in_sel = 0;
   DevBuf<float4> xyzv;
   DevBuf<int> pidx;
@@ -147,27 +179,18 @@ struct emap_handle {
   // carve_polygon, and its pinned host staging (the upload region on the way in, the read-back region on the way out)
   DevBuf<char> pg_block;
   PolySizes pg_cap{};
-  char* pg_host = nullptr;
-  size_t pg_host_bytes = 0;
+  PinnedBuf<char> pg_host;
   // features_pca scratch (allocated on first use): one device block carved by carve_pca
   DevBuf<char> pca_block;
-  // emap_input_image with a host image (allocated on first use, grown to the largest image): pinned staging, the device
-  // copy the kernel reads, and the event after which the staging may be overwritten
-  DevBuf<float> img_dev;
-  float* img_host = nullptr;
-  size_t img_host_n = 0;
-  cudaEvent_t img_staged = nullptr;
+  // emap_input_image with a host image (allocated on first use)
+  StagedUpload img_up;
   // emap_get_map_points / emap_get_normal_arrows (allocated on first use): the count and offset tables, the kept cells'
   // payload (grown to the largest call) and a pinned word for the count
   DevBuf<int> mc_table;
   DevBuf<char> mc_out;
-  int* mc_count_host = nullptr;
-  // emap_initialize_map (allocated on first use, grown to the largest call): the device copy of the upload, its pinned
-  // staging and the event after which the staging may be overwritten
-  DevBuf<char> init_dev;
-  char* init_host = nullptr;
-  size_t init_host_bytes = 0;
-  cudaEvent_t init_staged = nullptr;
+  PinnedBuf<int> mc_count_host;
+  // emap_initialize_map's arrays (allocated on first use)
+  StagedUpload init_up;
   // misc
   int64_t launches = 0;
   int count_rays = 0;
@@ -296,6 +319,19 @@ int grow(emap_handle* h, DevBuf<T>& b, size_t n, size_t slack, bool zero) {
   CK(cudaStreamSynchronize(h->side_stream));
   CK(b.alloc(n + slack));
   if (zero) CK(cudaMemsetAsync(b, 0, sizeof(T) * b.size(), h->stream));
+  return 0;
+}
+
+// Waits only for the previous upload (a staged event that was never recorded is complete) and when a buffer grows.
+int StagedUpload::room(emap_handle* h, size_t n) {
+  CK(cudaEventSynchronize(staged));
+  if (host.size() < n) CK(host.alloc(n));
+  return grow(h, dev, n, 0, false);
+}
+
+int StagedUpload::send(emap_handle* h, size_t n) {
+  CK(cudaMemcpyAsync(dev, host, n, cudaMemcpyHostToDevice, h->stream));
+  CK(cudaEventRecord(staged, h->stream));
   return 0;
 }
 
@@ -885,7 +921,7 @@ int map_cloud(emap_handle* h, int64_t* n_rows, float* xyz, int32_t* ids, double*
   if (span > 2 * 1024) return fail(h, EMAP_ERR_INVALID, "map point cloud: cell_n too large for k_mapcloud_scan");
   int rc = grow(h, h->mc_table, 2 * (size_t)n + 1, 0, false);
   if (rc) return rc;
-  if (!h->mc_count_host) CK(cudaMallocHost(&h->mc_count_host, sizeof(int)));
+  if (!h->mc_count_host) CK(h->mc_count_host.alloc(1));
   int* cnt = h->mc_table;
   int* off = cnt + n;
   const dim3 grid(n_tiles, n_chunks);
@@ -977,12 +1013,7 @@ int alloc_polygon_scratch(emap_handle* h, const PolySizes& z, PolyScratch& s) {
     CK(cudaMemsetAsync(s.col_min, 0x7f, sizeof(int) * c.cols, h->stream));    // "no cell yet": k_hull restores it
     CK(cudaMemsetAsync(s.col_max, 0xff, sizeof(int) * c.cols, h->stream));
   }
-  if (h->pg_host_bytes < c.up + c.down) {
-    if (h->pg_host) CK(cudaFreeHost(h->pg_host));
-    h->pg_host = nullptr; h->pg_host_bytes = 0;
-    CK(cudaMallocHost(&h->pg_host, c.up + c.down));
-    h->pg_host_bytes = c.up + c.down;
-  }
+  if (h->pg_host.size() < c.up + c.down) CK(h->pg_host.alloc(c.up + c.down));
   carve_polygon(c, h->pg_block, s);
   return 0;
 }
@@ -1138,19 +1169,14 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   h->dc.n_steps = (int)h->steps_host.size();
   h->dc.first_step = h->steps_host.empty() ? INFINITY : h->steps_host[0];
   const size_t C = (size_t)h->dc.C;
-  if ((e = cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
+  for (Stream* s : {&h->own_stream, &h->copy_stream, &h->side_stream})
+    if ((e = s->create(cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
   h->stream = h->own_stream;
-  if ((e = cudaStreamCreateWithFlags(&h->copy_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
-  for (int b = 0; b < 2; b++) {
-    if ((e = cudaEventCreateWithFlags(&h->in_free[b], cudaEventDisableTiming)) != cudaSuccess) return bail("event", e);
-    if ((e = cudaEventRecord(h->in_free[b], h->stream)) != cudaSuccess) return bail("event", e);
-  }
-  if ((e = cudaEventCreateWithFlags(&h->copy_done, cudaEventDisableTiming)) != cudaSuccess) return bail("event", e);
-  if ((e = cudaStreamCreateWithFlags(&h->side_stream, cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
-  if ((e = cudaEventCreateWithFlags(&h->ev_fork, cudaEventDisableTiming)) != cudaSuccess) return bail("event", e);
-  if ((e = cudaEventCreateWithFlags(&h->ev_join, cudaEventDisableTiming)) != cudaSuccess) return bail("event", e);
-  if ((e = cudaEventCreateWithFlags(&h->ev_order, cudaEventDisableTiming)) != cudaSuccess) return bail("event", e);
-  for (int k = 0; k < 9; k++) if ((e = cudaEventCreate(&h->st.ev[k])) != cudaSuccess) return bail("event", e);
+  for (Event* ev : {&h->in_free[0], &h->in_free[1], &h->copy_done, &h->ev_fork, &h->ev_join, &h->ev_order,
+                    &h->img_up.staged, &h->init_up.staged})
+    if ((e = ev->create(cudaEventDisableTiming)) != cudaSuccess) return bail("event", e);
+  for (Event& ev : h->st.ev) if ((e = ev.create(cudaEventDefault)) != cudaSuccess) return bail("event", e);
+  for (int b = 0; b < 2; b++) if ((e = cudaEventRecord(h->in_free[b], h->stream)) != cudaSuccess) return bail("event", e);
 #define ALLOC(buf, n) if ((e = (buf).alloc(n)) != cudaSuccess) return bail("cudaMalloc", e)
 #define TRY(call) if ((e = (call)) != cudaSuccess) return bail(#call, e)
   ALLOC(h->map, 7 * C);
@@ -1241,27 +1267,14 @@ static void comm_release(emap_handle* h);
 
 }  // extern "C"
 
-// the device buffers are released after this body, by their DevBuf members
+// The members release the memory, streams and events after this body, once no queued work uses them (emap_set_stream
+// synchronises the stream it replaces, so the current one holds everything queued on the handle's behalf).
 emap_handle::~emap_handle() {
   cudaSetDevice(device);
   if (stream) cudaStreamSynchronize(stream);
   if (copy_stream) cudaStreamSynchronize(copy_stream);
+  if (side_stream) cudaStreamSynchronize(side_stream);
   comm_release(this);
-  for (int b = 0; b < 2; b++) if (in_free[b]) cudaEventDestroy(in_free[b]);
-  if (copy_done) cudaEventDestroy(copy_done);
-  if (ev_fork) cudaEventDestroy(ev_fork);
-  if (ev_join) cudaEventDestroy(ev_join);
-  if (ev_order) cudaEventDestroy(ev_order);
-  if (side_stream) { cudaStreamSynchronize(side_stream); cudaStreamDestroy(side_stream); }
-  for (int k = 0; k < 9; k++) if (st.ev[k]) cudaEventDestroy(st.ev[k]);
-  if (own_stream) cudaStreamDestroy(own_stream);
-  if (copy_stream) cudaStreamDestroy(copy_stream);
-  if (pg_host) cudaFreeHost(pg_host);
-  if (img_staged) { cudaEventSynchronize(img_staged); cudaEventDestroy(img_staged); }
-  if (img_host) cudaFreeHost(img_host);
-  if (mc_count_host) cudaFreeHost(mc_count_host);
-  if (init_staged) { cudaEventSynchronize(init_staged); cudaEventDestroy(init_staged); }
-  if (init_host) cudaFreeHost(init_host);
 }
 
 // EM.py:119-128 clear
@@ -1716,13 +1729,12 @@ int emap_initialize_map(emap_handle* h, const float* xyz_host, int32_t n_points,
   // the upload: one block, 256-byte aligned arrays, the same layout in pinned and in device memory
   std::vector<int> tri, nb, off, list;
   std::vector<double> grad, coef;
-  size_t bytes = 0;
-  auto carve = [&](size_t n_bytes) { const size_t o = bytes; bytes += (n_bytes + 255) & ~(size_t)255; return o; };
+  Carver up{0};           // base 0: take() returns byte offsets
   size_t o_pxy = 0, o_pz = 0, o_txy = 0, o_coef = 0, o_off = 0, o_list = 0;
   if (method == 0) {
     a.n = n;
-    o_pxy = carve(sizeof(int2) * n);
-    o_pz = carve(sizeof(float) * n);
+    o_pxy = (size_t)up.take<int2>(n);
+    o_pz = (size_t)up.take<float>(n);
   } else {
     if (triangles_host) {
       tri.assign(triangles_host, triangles_host + 3 * (size_t)n_triangles);
@@ -1749,22 +1761,14 @@ int emap_initialize_map(emap_handle* h, const float* xyz_host, int32_t n_points,
       for (size_t k = 0; k < coef.size(); k++) coef[k] = z[tri[k]];
     }
     init_host::bin_tiles(W, xy, tri, off, list);
-    o_txy = carve(sizeof(int) * 6 * (size_t)T);
-    o_coef = carve(sizeof(double) * coef.size());
-    o_off = carve(sizeof(int) * off.size());
-    o_list = carve(sizeof(int) * std::max<size_t>(list.size(), 1));
+    o_txy = (size_t)up.take<int>(6 * (size_t)T);
+    o_coef = (size_t)up.take<double>(coef.size());
+    o_off = (size_t)up.take<int>(off.size());
+    o_list = (size_t)up.take<int>(std::max<size_t>(list.size(), 1));
   }
-  rc = grow(h, h->init_dev, bytes, 0, false);
-  if (rc) return rc;
-  if (!h->init_staged) CK(cudaEventCreateWithFlags(&h->init_staged, cudaEventDisableTiming));
-  else CK(cudaEventSynchronize(h->init_staged));          // the previous call's upload has left the staging
-  if (h->init_host_bytes < bytes) {
-    if (h->init_host) { cudaFreeHost(h->init_host); h->init_host = nullptr; h->init_host_bytes = 0; }
-    CK(cudaHostAlloc((void**)&h->init_host, bytes, cudaHostAllocDefault));
-    h->init_host_bytes = bytes;
-  }
-  char* hb = h->init_host;
-  char* db = h->init_dev;
+  if ((rc = h->init_up.room(h, up.bytes))) return rc;
+  char* hb = h->init_up.host;
+  char* db = h->init_up.dev;
   if (method == 0) {
     int2* pxy = (int2*)(hb + o_pxy);
     float* pz = (float*)(hb + o_pz);
@@ -1779,8 +1783,7 @@ int emap_initialize_map(emap_handle* h, const float* xyz_host, int32_t n_points,
     a.txy = (const int*)(db + o_txy); a.coef = (const double*)(db + o_coef);
     a.tile_off = (const int*)(db + o_off); a.tile_tri = (const int*)(db + o_list);
   }
-  CK(cudaMemcpyAsync(db, hb, bytes, cudaMemcpyHostToDevice, h->stream));
-  CK(cudaEventRecord(h->init_staged, h->stream));
+  if ((rc = h->init_up.send(h, up.bytes))) return rc;
   const int grid = a.tiles_x * a.tiles_x;
   if (method == 0) {
     if (narrow) k_init_nearest<long long><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
@@ -2292,19 +2295,11 @@ int emap_input_image(emap_handle* h, int32_t n_planes, const float* image, int i
   const size_t plane_sz = (size_t)height * width, n_img = plane_sz * n_planes;
   const float* img = image;
   if (!is_device_ptr) {
-    int rc = grow(h, h->img_dev, n_img, 0, false);
-    if (rc) return rc;
-    if (!h->img_staged) CK(cudaEventCreateWithFlags(&h->img_staged, cudaEventDisableTiming));
-    else CK(cudaEventSynchronize(h->img_staged));         // the previous image has left the staging
-    if (h->img_host_n < n_img) {
-      if (h->img_host) { cudaFreeHost(h->img_host); h->img_host = nullptr; h->img_host_n = 0; }
-      CK(cudaHostAlloc((void**)&h->img_host, sizeof(float) * n_img, cudaHostAllocDefault));
-      h->img_host_n = n_img;
-    }
-    memcpy(h->img_host, image, sizeof(float) * n_img);   // the caller's buffer is free from here on
-    CK(cudaMemcpyAsync(h->img_dev, h->img_host, sizeof(float) * n_img, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaEventRecord(h->img_staged, h->stream));
-    img = h->img_dev;
+    const size_t bytes = sizeof(float) * n_img;
+    if (int rc = h->img_up.room(h, bytes)) return rc;
+    memcpy(h->img_up.host, image, bytes);                // the caller's buffer is free from here on
+    if (int rc = h->img_up.send(h, bytes)) return rc;
+    img = (const float*)(char*)h->img_up.dev;
   }
   for (int k = 0; k < 3; k++) a.center[k] = h->center[k];
   a.res = h->cfg.resolution;
