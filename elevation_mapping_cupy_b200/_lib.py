@@ -32,6 +32,15 @@ class EmapFrameStats(C.Structure):
                 ("ray_steps", C.c_int64), ("ray_visits", C.c_int64)]
 
 
+class EmapDepthCamera(C.Structure):
+    _fields_ = [("height", C.c_int32), ("width", C.c_int32), ("depth", C.c_void_p), ("confidence", C.c_void_p),
+                ("rgb", C.c_void_p), ("features", C.c_void_p), ("fx", C.c_double), ("fy", C.c_double),
+                ("cx", C.c_double), ("cy", C.c_double), ("R", C.c_float * 9), ("t", C.c_float * 3)]
+
+
+EMAP_DEPTH_MAX_CAMERAS = 16
+
+
 class EmapExchange(C.Structure):
     _fields_ = [("ptr", C.c_void_p), ("count", C.c_int64), ("kind", C.c_int32)]
 
@@ -51,6 +60,10 @@ SIGNATURES = {
                                           C.c_double]),
     "emap_semantic_configure_ext": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                               C.c_int32, C.c_double, C.c_void_p, C.c_void_p, C.c_int32]),
+    "emap_input_depth_images": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(EmapDepthCamera), C.c_int, C.c_int32, C.c_void_p,
+                                          C.c_int32, C.c_float, C.c_float, C.c_float, C.c_float]),
+    "emap_input_depth_image": (C.c_int, [C.c_void_p, C.POINTER(EmapDepthCamera), C.c_int, C.c_int32, C.c_void_p, C.c_int32,
+                                         C.c_float, C.c_float, C.c_float, C.c_float]),
     "emap_point_record_device_ptr": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_int64)]),
     "emap_get_frame_stats": (C.c_int, [C.c_void_p, C.POINTER(EmapFrameStats)]),
     "emap_set_ray_counting": (C.c_int, [C.c_void_p, C.c_int]),

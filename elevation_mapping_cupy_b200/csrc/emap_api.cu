@@ -22,6 +22,8 @@
 #include "emap_mapcloud.cuh"
 #include "emap_initialize.cuh"
 
+static_assert(EMAP_DEPTH_MAX_CHANNELS == SEM_MAX_CH, "emap.h and the semantic kernels disagree on the channel count");
+
 namespace {
 
 thread_local std::string g_create_error;
@@ -156,6 +158,8 @@ struct emap_handle {
   int64_t pend_stride = 0;
   int pend_dtype = 0, pend_host = 0;
   bool zero_copy_pending = false;      // the index pass reads the caller's pinned host buffer: sync before returning
+  bool depth_frame = false;            // the last frame reads depth images (pend_cams) instead of clouds
+  std::vector<DepthSource> pend_cams;
   // export staging
   DevBuf<float> d_export;
   // plugin scratch
@@ -413,43 +417,81 @@ int stage_mark(emap_handle* h, int k) {
   return 0;
 }
 
-// f(pts, s) for the cloud of every sensor s of the pending frame, with pts typed by pend_dtype (float or double);
-// stops at the first non-zero return
+// f(src, s) for the point source of every sensor s of the pending frame: its cloud rows typed by pend_dtype (float or
+// double), or its depth camera; stops at the first non-zero return
 template <typename F>
 int each_cloud(emap_handle* h, F&& f) {
-  for (int s = 0; s < (int)h->pend_pts.size(); s++) {
-    const int rc = h->pend_dtype == EMAP_F32 ? f((const float*)h->pend_pts[s], s) : f((const double*)h->pend_pts[s], s);
+  for (int s = 0; s < (int)h->pend_n.size(); s++) {
+    const int rc = h->depth_frame ? f(h->pend_cams[s], s)
+                 : h->pend_dtype == EMAP_F32 ? f(RowSource<float>{(const float*)h->pend_pts[s], h->pend_stride}, s)
+                                             : f(RowSource<double>{(const double*)h->pend_pts[s], h->pend_stride}, s);
     if (rc) return rc;
   }
   return 0;
 }
 
-template <typename T>
-int launch_index(emap_handle* h, const T* pts, int s) {
+template <typename Src>
+int launch_index(emap_handle* h, const Src& src, int s) {
   const i64 n = h->pend_n[s], off = h->offs[s];
   if (n <= 0) return 0;
-  PDL(k_index_error<T>, cdiv(n, 256), 256, 0, h->dc, h->poses[s], pts, n, h->pend_stride, h->xyzv + off, h->pidx + off,
+  PDL(k_index_error<Src>, cdiv(n, 256), 256, 0, h->dc, h->poses[s], src, n, h->xyzv + off, h->pidx + off,
       (const float*)h->map, h->sc, h->fs, h->rays + off, h->ray_ctl + RC_CTL * s, (const unsigned short*)h->step_cnt);
   LAUNCH_CHECK();
   return 0;
 }
 
-// phase 0: upload + index/error pass for every sensor
-int frame_begin(emap_handle* h, int32_t n_sensors, const void* const* points, const int64_t* n, int64_t row_stride,
-                int dtype, int is_device_ptr, const float* R, const float* t, int64_t global_off, float pn, float on,
-                bool sharded) {
+// Makes the frame's n_buf input buffers (bytes[k] bytes at ptrs[k], host or device memory) readable by its kernels, at
+// dp[k].  Device memory is read in place.  Host buffers that are all page-locked (cudaHostAlloc / cudaHostRegister /
+// torch pin_memory) are read by the kernels directly over PCIe (zero-copy): no staging copy, no copy-engine round trip.
+// Otherwise every buffer is staged, 256-byte aligned, into one of two device buffers on the copy stream.
+int stage_inputs(emap_handle* h, int n_buf, const void* const* ptrs, const size_t* bytes, int is_device_ptr,
+                 const void** dp) {
+  bool zero_copy = false;
+  if (!is_device_ptr) {
+    zero_copy = true;
+    for (int k = 0; k < n_buf && zero_copy; k++) {
+      if (bytes[k] == 0) { dp[k] = ptrs[k]; continue; }
+      cudaPointerAttributes at;
+      if (cudaPointerGetAttributes(&at, ptrs[k]) != cudaSuccess || at.type != cudaMemoryTypeHost || !at.devicePointer) {
+        cudaGetLastError(); zero_copy = false;
+      } else dp[k] = at.devicePointer;
+    }
+  }
+  h->pend_host = 0;
+  if (is_device_ptr) {
+    for (int k = 0; k < n_buf; k++) dp[k] = ptrs[k];
+  } else if (zero_copy) {
+    h->zero_copy_pending = true;             // nothing to stage; the caller's buffers are read until the frame's last reader
+  } else {
+    const int b = h->in_sel; h->in_sel ^= 1;
+    const auto aligned = [](size_t x) { return (x + 255) & ~(size_t)255; };
+    size_t total = 0;
+    for (int k = 0; k < n_buf; k++) total += aligned(bytes[k]);
+    int rc;
+    if ((rc = grow(h, h->d_in[b], total, total / 4 + 4096, false))) return rc;
+    CK(cudaStreamWaitEvent(h->copy_stream, h->in_free[b], 0));
+    size_t o = 0;
+    for (int k = 0; k < n_buf; k++) {
+      if (bytes[k]) CK(cudaMemcpyAsync((char*)h->d_in[b] + o, ptrs[k], bytes[k], cudaMemcpyHostToDevice, h->copy_stream));
+      dp[k] = (char*)h->d_in[b] + o;
+      o += aligned(bytes[k]);
+    }
+    CK(cudaEventRecord(h->copy_done, h->copy_stream));
+    CK(cudaStreamWaitEvent(h->stream, h->copy_done, 0));
+    h->pend_host = 1;
+  }
+  return 0;
+}
+
+// The frame's row counts (rows of sensor s at offs[s]), sensor poses and per-row buffers; the caller has validated n
+// (every n[s] >= 0, fewer than 2^31 rows in all).
+int frame_setup(emap_handle* h, int32_t n_sensors, const int64_t* n, const float* R, const float* t, int64_t global_off,
+                float pn, float on, bool sharded) {
   h->sc.dirty = sharded ? nullptr : (unsigned char*)h->dirty;      // sharded frames derive the marker from the all-reduced counts
   h->fused_drift = !sharded;
-  if (n_sensors < 1 || row_stride < 3 || (dtype != EMAP_F32 && dtype != EMAP_F64))
-    return fail(h, EMAP_ERR_INVALID, "emap_input: n_sensors >= 1, row_stride >= 3, dtype f32/f64 required");
-  const size_t esz = dtype == EMAP_F32 ? 4 : 8;
   h->offs.assign(n_sensors + 1, 0);
-  for (int s = 0; s < n_sensors; s++) {
-    if (n[s] < 0 || (n[s] > 0 && !points[s])) return fail(h, EMAP_ERR_INVALID, "emap_input: bad point array");
-    h->offs[s + 1] = h->offs[s] + n[s];
-  }
+  for (int s = 0; s < n_sensors; s++) h->offs[s + 1] = h->offs[s] + n[s];
   const i64 N = h->offs[n_sensors];
-  if (global_off + N >= (1ll << 31)) return fail(h, EMAP_ERR_INVALID, "emap_input: more than 2^31 points in a frame");
   h->n_points = N; h->global_off = global_off; h->pos_noise = pn; h->ori_noise = on;
   int rc;
   if ((rc = grow(h, h->xyzv, N, N / 4 + 1024, false)) || (rc = grow(h, h->pidx, N, N / 4 + 1024, false)) ||
@@ -464,48 +506,31 @@ int frame_begin(emap_handle* h, int32_t n_sensors, const void* const* points, co
   // zero-filled on the stream: ordered before the frame's kernels
   if ((rc = grow(h, h->ray_ctl, (size_t)RC_CTL * n_sensors, RC_CTL * 8, true))) return rc;
   h->overlap_override = false;
-  if (stage_mark(h, 0)) return EMAP_ERR_CUDA;
-  const void* dev_pts[64];
-  std::vector<const void*> dev_vec;
-  const void** dp = dev_pts;
-  if (n_sensors > 64) { dev_vec.resize(n_sensors); dp = dev_vec.data(); }
-  // Host clouds in page-locked memory (cudaHostAlloc / cudaHostRegister / torch pin_memory) are read by the index
-  // kernel directly over PCIe (zero-copy): no staging copy, no copy-engine round trip.  Pageable memory is staged.
-  bool zero_copy = false;
-  if (!is_device_ptr) {
-    zero_copy = true;
-    for (int s = 0; s < n_sensors && zero_copy; s++) {
-      if (n[s] == 0) { dp[s] = points[s]; continue; }
-      cudaPointerAttributes at;
-      if (cudaPointerGetAttributes(&at, points[s]) != cudaSuccess || at.type != cudaMemoryTypeHost || !at.devicePointer) {
-        cudaGetLastError(); zero_copy = false;
-      } else dp[s] = at.devicePointer;
-    }
-  }
-  if (is_device_ptr) {
-    for (int s = 0; s < n_sensors; s++) dp[s] = points[s];
-  } else if (zero_copy) {
-    is_device_ptr = 1;                       // nothing to stage; the caller's buffer is read until the index pass ends
-    h->zero_copy_pending = true;
-  } else {
-    const int b = h->in_sel; h->in_sel ^= 1;
-    size_t total = 0;
-    for (int s = 0; s < n_sensors; s++) total += (size_t)n[s] * row_stride * esz;
-    if ((rc = grow(h, h->d_in[b], total, total / 4 + 4096, false))) return rc;
-    CK(cudaStreamWaitEvent(h->copy_stream, h->in_free[b], 0));
-    size_t o = 0;
-    for (int s = 0; s < n_sensors; s++) {
-      const size_t bytes = (size_t)n[s] * row_stride * esz;
-      if (bytes) CK(cudaMemcpyAsync((char*)h->d_in[b] + o, points[s], bytes, cudaMemcpyHostToDevice, h->copy_stream));
-      dp[s] = (char*)h->d_in[b] + o;
-      o += bytes;
-    }
-    CK(cudaEventRecord(h->copy_done, h->copy_stream));
-    CK(cudaStreamWaitEvent(h->stream, h->copy_done, 0));
-  }
-  h->pend_pts.assign(dp, dp + n_sensors);
   h->pend_n.assign(n, n + n_sensors);
-  h->pend_stride = row_stride; h->pend_dtype = dtype; h->pend_host = !is_device_ptr;
+  if (stage_mark(h, 0)) return EMAP_ERR_CUDA;
+  return 0;
+}
+
+// phase 0: upload + index/error pass for every sensor
+int frame_begin(emap_handle* h, int32_t n_sensors, const void* const* points, const int64_t* n, int64_t row_stride,
+                int dtype, int is_device_ptr, const float* R, const float* t, int64_t global_off, float pn, float on,
+                bool sharded) {
+  if (n_sensors < 1 || row_stride < 3 || (dtype != EMAP_F32 && dtype != EMAP_F64))
+    return fail(h, EMAP_ERR_INVALID, "emap_input: n_sensors >= 1, row_stride >= 3, dtype f32/f64 required");
+  const size_t esz = dtype == EMAP_F32 ? 4 : 8;
+  i64 N = 0;
+  for (int s = 0; s < n_sensors; s++) {
+    if (n[s] < 0 || (n[s] > 0 && !points[s])) return fail(h, EMAP_ERR_INVALID, "emap_input: bad point array");
+    N += n[s];
+  }
+  if (global_off + N >= (1ll << 31)) return fail(h, EMAP_ERR_INVALID, "emap_input: more than 2^31 points in a frame");
+  int rc;
+  if ((rc = frame_setup(h, n_sensors, n, R, t, global_off, pn, on, sharded))) return rc;
+  std::vector<size_t> bytes(n_sensors);
+  for (int s = 0; s < n_sensors; s++) bytes[s] = (size_t)n[s] * row_stride * esz;
+  h->pend_pts.resize(n_sensors);
+  if ((rc = stage_inputs(h, n_sensors, points, bytes.data(), is_device_ptr, h->pend_pts.data()))) return rc;
+  h->pend_stride = row_stride; h->pend_dtype = dtype; h->depth_frame = false;
   h->phase = -1;                                                   // index pass pending
   return 0;
 }
@@ -563,25 +588,25 @@ SemMax sem_max(emap_handle* h) {
   return m;
 }
 
-template <typename T>
-int launch_sem_sum(emap_handle* h, const T* pts, int s) {
+template <typename Src>
+int launch_sem_sum(emap_handle* h, const Src& src, int s) {
   const i64 n = h->pend_n[s];
   if (n <= 0) return 0;
-  k_sem_sum<T><<<cdiv(n, 256), 256, 0, h->stream>>>(h->dc, h->sem, pts, n, h->pend_stride, (const int*)(h->pidx + h->offs[s]),
-                                                     h->sem_fsum, h->sem_csum, sem_max(h));
+  k_sem_sum<Src><<<cdiv(n, 256), 256, 0, h->stream>>>(h->dc, h->sem, src, n, (const int*)(h->pidx + h->offs[s]),
+                                                       h->sem_fsum, h->sem_csum, sem_max(h));
   LAUNCH_CHECK();
   return 0;
 }
 
 // class_max before the scatter: U and the records per cell over every cloud (id_max read once, with the first cloud)
-template <typename T>
-int launch_cm_count(emap_handle* h, const T* pts, int s) {
+template <typename Src>
+int launch_cm_count(emap_handle* h, const Src& src, int s) {
   const i64 n = h->pend_n[s], n_idm = s == 0 ? (i64)h->sem.n_id_max * h->dc.C : 0;
   const i64 work = std::max(n, n_idm);
   if (work <= 0) return 0;
   const int grid = (int)std::min<i64>(cdiv(work, 256), (i64)h->n_sm * 4);
-  k_cm_count<T><<<grid, 256, 0, h->stream>>>(h->sem, pts, n, h->pend_stride, (const int*)(h->pidx + h->offs[s]),
-                                             (const int*)h->sem.id_max, n_idm, sem_max(h));
+  k_cm_count<Src><<<grid, 256, 0, h->stream>>>(h->sem, src, n, (const int*)(h->pidx + h->offs[s]),
+                                               (const int*)h->sem.id_max, n_idm, sem_max(h));
   LAUNCH_CHECK();
   return 0;
 }
@@ -1301,6 +1326,25 @@ int initialize_finish(emap_handle* h, int32_t dilation_size, int32_t iterations)
   return EMAP_OK;
 }
 
+// The frame after its inputs are in place (frame_begin or the depth-image set-up): every pass, then, for host inputs, the
+// wait after which the caller may reuse them
+int frame_run(emap_handle* h, int is_device_ptr) {
+  int rc;
+  if ((rc = frame_index(h))) return rc;
+  if ((rc = frame_fuse(h))) return rc;
+  if ((rc = frame_semantic(h))) return rc;
+  if ((rc = frame_rays(h))) return rc;
+  if ((rc = frame_finish(h))) return rc;
+  if (!is_device_ptr || h->zero_copy_pending) {      // caller may reuse its host buffers on return
+    // a captured frame runs nothing yet: it reads the caller's pinned cloud at every replay instead
+    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+    CK(cudaStreamIsCapturing(h->stream, &cs));
+    if (cs == cudaStreamCaptureStatusNone) CK(cudaEventSynchronize(h->copy_done));
+  }
+  h->zero_copy_pending = false;
+  return EMAP_OK;
+}
+
 extern "C" {
 
 #define ENTER(h)                                               \
@@ -1327,21 +1371,8 @@ int emap_input_sensors(emap_handle* h, int32_t n_sensors, const void* const* poi
   ENTER(h);
   if (!points || !n || !R || !t) return fail(h, EMAP_ERR_INVALID, "emap_input: null argument");
   if (h->attached) return fail(h, EMAP_ERR_STATE, "handle is attached to a sharded scratch: use the emap_shard_* calls");
-  int rc = frame_begin(h, n_sensors, points, n, row_stride, dtype, is_device_ptr, R, t, 0, pn, on, false);
-  if (rc) return rc;
-  if ((rc = frame_index(h))) return rc;
-  if ((rc = frame_fuse(h))) return rc;
-  if ((rc = frame_semantic(h))) return rc;
-  if ((rc = frame_rays(h))) return rc;
-  if ((rc = frame_finish(h))) return rc;
-  if (!is_device_ptr || h->zero_copy_pending) {      // caller may reuse its host buffers on return
-    // a captured frame runs nothing yet: it reads the caller's pinned cloud at every replay instead
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    CK(cudaStreamIsCapturing(h->stream, &cs));
-    if (cs == cudaStreamCaptureStatusNone) CK(cudaEventSynchronize(h->copy_done));
-  }
-  h->zero_copy_pending = false;
-  return EMAP_OK;
+  const int rc = frame_begin(h, n_sensors, points, n, row_stride, dtype, is_device_ptr, R, t, 0, pn, on, false);
+  return rc ? rc : frame_run(h, is_device_ptr);
 }
 
 int emap_input_pointcloud(emap_handle* h, const void* points, int64_t n, int64_t row_stride, int dtype, int is_device_ptr,
@@ -1349,6 +1380,86 @@ int emap_input_pointcloud(emap_handle* h, const void* points, int64_t n, int64_t
   const void* p[1] = {points};
   int64_t nn[1] = {n};
   return emap_input_sensors(h, 1, p, nn, row_stride, dtype, is_device_ptr, R, t, pn, on);
+}
+
+int emap_input_depth_images(emap_handle* h, int32_t n_cameras, const emap_depth_camera* cams, int is_device_ptr,
+                            int32_t n_channels, const int32_t* channel_source, int32_t n_features,
+                            float confidence_threshold, float max_depth, float pn, float on) {
+  ENTER(h);
+  if (h->attached) return fail(h, EMAP_ERR_STATE, "handle is attached to a sharded scratch: use the emap_shard_* calls");
+  if (!cams || n_cameras < 1 || n_cameras > EMAP_DEPTH_MAX_CAMERAS)
+    return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: 1 <= n_cameras <= EMAP_DEPTH_MAX_CAMERAS cameras required");
+  if (n_channels < 0 || n_channels > SEM_MAX_CH || (n_channels > 0 && !channel_source) || n_features < 0 ||
+      n_features > EMAP_DEPTH_MAX_FEATURES)
+    return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: 0..16 channels with their sources, 0..255 feature planes required");
+  int n_color = 0, n_feat_used = 0;
+  for (int j = 0; j < n_channels; j++) {
+    if (channel_source[j] < -1 || channel_source[j] >= n_features)
+      return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: a channel source outside [-1, n_features)");
+    n_color += channel_source[j] == -1;
+    n_feat_used += channel_source[j] >= 0;
+  }
+  if (n_color > 1) return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: more than one colour channel");
+  if (h->sem.n_ch > 0 && h->sem_map)
+    for (int k = 0; k < h->sem.n_ch; k++)
+      if (h->sem.col[k] >= 3 + n_channels)
+        return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: a configured semantic column beyond 3 + n_channels");
+  int64_t n[EMAP_DEPTH_MAX_CAMERAS];      // at most 16 * 2^24 = 2^28 pixels: below the frame's 2^31 rows
+  float R[9 * EMAP_DEPTH_MAX_CAMERAS], t[3 * EMAP_DEPTH_MAX_CAMERAS];
+  for (int s = 0; s < n_cameras; s++) {
+    const emap_depth_camera& c = cams[s];
+    bool finite = std::isfinite(c.fx) && std::isfinite(c.fy) && c.fx != 0.0 && c.fy != 0.0 && std::isfinite(c.cx) &&
+                  std::isfinite(c.cy);
+    for (int k = 0; k < 9; k++) finite = finite && std::isfinite(c.R[k]);
+    for (int k = 0; k < 3; k++) finite = finite && std::isfinite(c.t[k]);
+    if (!c.depth || c.height <= 0 || c.width <= 0 || (i64)c.height * c.width > (1ll << 24))
+      return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: a depth image, 0 < height * width <= 2^24 required");
+    if (!finite) return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: non-finite or zero fx / fy, or non-finite cx, cy, R, t");
+    if ((n_color && !c.rgb) || (n_feat_used && !c.features))
+      return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: a colour channel needs rgb, a feature channel the feature planes");
+    n[s] = (i64)c.height * c.width;
+    memcpy(R + 9 * s, c.R, sizeof(c.R));
+    memcpy(t + 3 * s, c.t, sizeof(c.t));
+  }
+  int rc;
+  if ((rc = frame_setup(h, n_cameras, n, R, t, 0, pn, on, false))) return rc;
+  // per camera: depth, confidence, rgb, feature planes (the ones the channels read)
+  const void* ptrs[4 * EMAP_DEPTH_MAX_CAMERAS];
+  const void* dp[4 * EMAP_DEPTH_MAX_CAMERAS];
+  size_t bytes[4 * EMAP_DEPTH_MAX_CAMERAS];
+  for (int s = 0; s < n_cameras; s++) {
+    const emap_depth_camera& c = cams[s];
+    const size_t P = (size_t)n[s];
+    ptrs[4 * s] = c.depth; bytes[4 * s] = 4 * P;
+    ptrs[4 * s + 1] = c.confidence; bytes[4 * s + 1] = c.confidence ? 4 * P : 0;
+    ptrs[4 * s + 2] = c.rgb; bytes[4 * s + 2] = n_color ? 3 * P : 0;
+    ptrs[4 * s + 3] = c.features; bytes[4 * s + 3] = n_feat_used ? 4 * P * n_features : 0;
+  }
+  if ((rc = stage_inputs(h, 4 * n_cameras, ptrs, bytes, is_device_ptr, dp))) return rc;
+  h->pend_cams.resize(n_cameras);
+  for (int s = 0; s < n_cameras; s++) {
+    const emap_depth_camera& c = cams[s];
+    DepthSource& d = h->pend_cams[s];
+    memset(&d, 0, sizeof(d));
+    d.depth = (const float*)dp[4 * s];
+    d.conf = c.confidence ? (const float*)dp[4 * s + 1] : nullptr;
+    d.rgb = (const unsigned char*)dp[4 * s + 2];
+    d.feat = (const float*)dp[4 * s + 3];
+    d.plane = n[s]; d.width = c.width;
+    d.conf_min = confidence_threshold; d.max_depth = max_depth;
+    d.fx = c.fx; d.fy = c.fy; d.cx = c.cx; d.cy = c.cy;
+    for (int j = 0; j < n_channels; j++) d.src[j / 8] |= (u64)(channel_source[j] + 1) << (8 * (j % 8));
+  }
+  h->depth_frame = true;
+  h->phase = -1;                                                   // index pass pending
+  return frame_run(h, is_device_ptr);
+}
+
+int emap_input_depth_image(emap_handle* h, const emap_depth_camera* camera, int is_device_ptr, int32_t n_channels,
+                           const int32_t* channel_source, int32_t n_features, float confidence_threshold, float max_depth,
+                           float pn, float on) {
+  return emap_input_depth_images(h, 1, camera, is_device_ptr, n_channels, channel_source, n_features, confidence_threshold,
+                                 max_depth, pn, on);
 }
 
 // ---- semantic point-channel fusion ------------------------------------------------------------
@@ -1612,7 +1723,7 @@ int emap_get_frame_stats(emap_handle* h, emap_frame_stats* out) {
   CK(cudaStreamSynchronize(h->stream));
   out->mean_error = f.mean_error; out->additive_mean_error = f.additive_mean_error; out->shift_applied = f.shift;
   out->error_sum = f.error_sum; out->error_cnt = f.ecnt_last; out->drift_applied = f.applied; out->drift_evaluated = f.evaluated;
-  out->n_points = h->n_points; out->n_valid_points = f.nvalid_last; out->ray_steps = f.ray_steps; out->ray_visits = f.ray_visits;
+  out->n_points = h->depth_frame ? f.nkept_last : h->n_points; out->n_valid_points = f.nvalid_last; out->ray_steps = f.ray_steps; out->ray_visits = f.ray_visits;
   return EMAP_OK;
 }
 

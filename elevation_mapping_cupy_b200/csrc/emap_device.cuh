@@ -79,6 +79,7 @@ struct FrameScalars {          // device-resident scalars of the running frame
   float mean_error, additive_mean_error, error_sum;
   float overlap_tz;            // t[2] of sensor 0 relative to the map centre (elevation_mapping.py:400-401)
   i64 ecnt_last, nvalid_last;  // copies for emap_get_frame_stats (the accumulators are re-zeroed inside the frame)
+  i64 nkept, nkept_last;       // kept pixels of a depth-image frame (DepthSource), and its copy
 };
 
 __device__ __forceinline__ float h16(float x) { return __half2float(__float2half_rn(x)); }

@@ -15,7 +15,7 @@
 // oracle/emap_oracle.c; they are within one fp32 rounding of some order of the reference atomics.
 #pragma once
 #include <cuda.h>                 // CUtensorMap (type only; the encoder is fetched at run time, emap_api.cu)
-#include "emap_device.cuh"
+#include "emap_sources.cuh"
 
 // ------------------------------------------------------------------------------------------
 // per-cell scratch of a frame; all zero between frames (k_finalize re-zeroes what it consumed)
@@ -135,45 +135,29 @@ __device__ __forceinline__ int count_below(const float* __restrict__ t, int n, f
   return lo;
 }
 
-// One point's xyz.  fp32 rows padded to 4 floats (16-byte aligned): one 128-bit read-only load per point; other
-// layouts: three scalar loads (a warp's rows are contiguous, so they coalesce into the same sectors).
-template <typename T>
-__device__ __forceinline__ void load_point(const T* __restrict__ pts, i64 i, i64 stride, float& x, float& y, float& z) {
-  const T* p = pts + i * stride;
-  x = (float)p[0]; y = (float)p[1]; z = (float)p[2];
-}
-template <>
-__device__ __forceinline__ void load_point<float>(const float* __restrict__ pts, i64 i, i64 stride, float& x, float& y, float& z) {
-  const float* p = pts + i * stride;
-  if (stride == 4 && (reinterpret_cast<uintptr_t>(pts) & 15) == 0) {
-    const float4 v = __ldg(reinterpret_cast<const float4*>(p));
-    x = v.x; y = v.y; z = v.z;
-  } else {
-    x = p[0]; y = p[1]; z = p[2];
-  }
-}
-
 // ------------------------------------------------------------------------------------------
-template <typename T>
+// Src: a point source of emap_sources.cuh (the caller's cloud rows, or a depth image read pixel by pixel)
+template <typename Src>
 __global__ void __launch_bounds__(256)
-k_index_error(const DevCfg c, const Pose q, const T* __restrict__ pts, const i64 n, const i64 stride,
+k_index_error(const DevCfg c, const Pose q, const Src src, const i64 n,
               float4* __restrict__ xyzv, int* __restrict__ pidx, const float* __restrict__ map,
               const CellScratch s, FrameScalars* fs, Ray* __restrict__ rays, int* __restrict__ ray_ctl,
               const unsigned short* __restrict__ step_cnt) {
   pdl_trigger(); pdl_wait();
   const i64 i = blockIdx.x * (i64)blockDim.x + threadIdx.x;
-  i64 e = 0; int ec = 0, nv = 0;
+  i64 e = 0; int ec = 0, nv = 0, nk = 0;
   Ray ray; ray.len = -1.f; ray.counts = 0;
   int cell_key = -1 - (int)(threadIdx.x & 31);                    // cell receiving this point's count (unique negative: none)
   bool is_inl = false;
   if (i < n) {
     float px, py, pz;                                             // EM.py:456 cast to fp32
-    load_point(pts, i, stride, px, py, pz);
+    const bool kept = src.load(i, px, py, pz);
     int rec;
     float4 o = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (px != px || py != py || pz != pz) {                       // EM.py:458 drop NaN rows
+    if (!kept || px != px || py != py || pz != pz) {              // EM.py:458 drop NaN rows (and masked pixels)
       rec = PT_SKIP | PT_IDX_MASK;
     } else {
+      nk = 1;
       Geom g; point_geom(c, q, px, py, pz, g);
       const int idx = g.ix * c.W + g.iy;
       rec = idx | (g.valid ? PT_VALID : 0) | (g.inside ? PT_INSIDE : 0);
@@ -238,6 +222,7 @@ k_index_error(const DevCfg c, const Pose q, const T* __restrict__ pts, const i64
   const u32 ray_bal = __ballot_sync(0xffffffffu, has_ray);
   if ((threadIdx.x & 31) == 0) s_rc[threadIdx.x >> 5] = __popc(ray_bal);
   // block reduction -> one integer atomic per block (order independent)
+  if (Src::kCountsKept) nv |= nk << 16;                           // a block has 256 rows: both counts fit in one int
   for (int o = 16; o > 0; o >>= 1) {
     e += __shfl_down_sync(0xffffffffu, e, o);
     ec += __shfl_down_sync(0xffffffffu, ec, o);
@@ -251,6 +236,10 @@ k_index_error(const DevCfg c, const Pose q, const T* __restrict__ pts, const i64
     for (int k = 1; k < 8; k++) { e += s_e[k]; ec += s_c[k]; nv += s_v[k]; }
     if (e != 0) red_add((u64*)&fs->E, (u64)e, s.mc_off);
     if (ec) red_add((u64*)&fs->ecnt, (u64)ec, s.mc_off);
+    if (Src::kCountsKept) {
+      if (nv >> 16) atomicAdd((u64*)&fs->nkept, (u64)(nv >> 16));
+      nv &= 0xffff;
+    }
     if (nv) atomicAdd((u64*)&fs->nvalid, (u64)nv);
     int tot = 0;
     for (int k = 0; k < 8; k++) tot += s_rc[k];
@@ -289,7 +278,7 @@ __device__ __forceinline__ DriftDecision drift_decide(const DevCfg& c, const i64
 // one thread: publish the decision and the frame statistics (emap_get_frame_stats), reset the ray-march counters
 __device__ __forceinline__ void drift_publish(FrameScalars* fs, const DriftDecision& d, const i64 ecnt, const float overlap_tz,
                                               const int set_overlap) {
-  fs->nvalid_last = fs->nvalid;
+  fs->nvalid_last = fs->nvalid; fs->nkept_last = fs->nkept;
   fs->ray_steps = 0; fs->ray_visits = 0;
   fs->ecnt_last = ecnt;
   if (set_overlap) fs->overlap_tz = overlap_tz;
@@ -308,7 +297,7 @@ __global__ void k_drift(const DevCfg c, FrameScalars* fs, float position_noise, 
   const i64 ecnt = fs->ecnt;
   const DriftDecision d = drift_decide(c, fs->E, ecnt, position_noise, orientation_noise);
   drift_publish(fs, d, ecnt, overlap_tz, set_overlap);
-  fs->E = 0; fs->ecnt = 0; fs->nvalid = 0;
+  fs->E = 0; fs->ecnt = 0; fs->nvalid = 0; fs->nkept = 0;
 }
 
 // CK.py:168-197 fusion half; every load is of the pre-frame snapshot (+ drift shift)
@@ -812,7 +801,7 @@ k_finalize(const DevCfg c, float* __restrict__ map, const CellScratch s, const F
   if (blockIdx.x == 0) for (int k = threadIdx.x; k < n_ctl; k += blockDim.x) ray_ctl[k] = 0;   // consumed by k_raycast: next frame's
   if (fs_reset && blockIdx.x == 1 % gridDim.x) {     // frames without k_drift: the housekeeping it would do for the next frame
     for (int k = threadIdx.x; k < RT * RT; k += blockDim.x) tmap[k] = 0u;
-    if (threadIdx.x == 0) { fs_reset->E = 0; fs_reset->ecnt = 0; fs_reset->nvalid = 0; }
+    if (threadIdx.x == 0) { fs_reset->E = 0; fs_reset->ecnt = 0; fs_reset->nvalid = 0; fs_reset->nkept = 0; }
   }
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int i0 = (blockIdx.x * blockDim.x + threadIdx.x) * V;

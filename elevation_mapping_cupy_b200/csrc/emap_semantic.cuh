@@ -7,7 +7,7 @@
 // integer sums for a colour channel -- and a dense kernel over (cell, channel) that writes the layer from the sums and
 // the frame's fused-point count new_map[2] (CK.py:185).
 // Here: ONE scatter kernel over the frame's points for all channels of all algorithms (it reads the packed
-// (idx, valid, inside) record k_index_error left on the device and the feature columns of the caller's cloud), and ONE
+// (idx, valid, inside) record k_index_error left on the device and the feature columns of the frame's point source), and ONE
 // per-cell kernel, both inside the frame (after k_fuse, before k_finalize re-zeroes the counts).  Float sums are
 // accumulated in 2^-32 fixed point like the height sums: order-independent, deterministic, within one rounding of any
 // order of the reference's float atomics.
@@ -16,11 +16,10 @@
 // zeroed everywhere for the later rounds), so it adds its own passes between them, see "class_max" below.  DESIGN §4d
 // defines all three where the reference crashes or degenerates.
 #pragma once
-#include "emap_device.cuh"
+#include "emap_sources.cuh"
 
 enum { SEM_AVERAGE = 0, SEM_CLASS_AVERAGE = 1, SEM_COLOR = 2, SEM_CLASS_BAYESIAN = 3, SEM_BAYESIAN_INFERENCE = 4,
        SEM_CLASS_MAX = 5 };
-#define SEM_MAX_CH 16
 
 struct SemCfg {
   int n_ch;                      // channels fused this frame (0: semantic fusion off)
@@ -71,19 +70,18 @@ __device__ __forceinline__ float cm_value(u32 f, i64 s) {
 // scatter: fusion/pointcloud_average.py:41-52 (sum_kernel), fusion/pointcloud_color.py:51-61 (add_color_kernel)
 // fusion/pointcloud_class_bayesian.py alpha_kernel (theta >= 0 only), pointcloud_bayesian_inference.py
 // sum_compact_kernel and pointcloud_class_max.py sum_max_kernel (into the cell's hash table), every (point, channel)
-template <typename T>
+template <typename Src>
 __global__ void __launch_bounds__(256)
-k_sem_sum(const DevCfg c, const SemCfg sc, const T* __restrict__ pts, const i64 n, const i64 stride,
+k_sem_sum(const DevCfg c, const SemCfg sc, const Src src, const i64 n,
           const int* __restrict__ pidx, i64* __restrict__ fsum, u32* __restrict__ csum, const SemMax ms) {
   const i64 i = blockIdx.x * (i64)blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int rec = pidx[i];
   if ((rec & (PT_VALID | PT_INSIDE | PT_SKIP)) != (PT_VALID | PT_INSIDE)) return;     // `if (valid) if (inside)`
   const int idx = rec & PT_IDX_MASK;
-  const T* row = pts + i * stride;
   const size_t C = (size_t)c.C;
   for (int k = 0; k < sc.n_ch; k++) {
-    const float feat = (float)row[sc.col[k]];                     // points_all is float32 (EM.py:456)
+    const float feat = src.feature(i, sc.col[k]);
     if (sc.kind[k] == SEM_COLOR) {
       const u32 color = __float_as_uint(feat);                    // pointcloud_color.py:56-60
       u32* p = csum + (size_t)sc.slot[k] * C + idx;
@@ -114,9 +112,9 @@ k_sem_sum(const DevCfg c, const SemCfg sc, const T* __restrict__ pts, const i64 
 
 // class_max, before the scatter: U (ids of every non-dropped row, and of the first n_idm entries of id_max) and the
 // records per cell.  Grid-stride; each block ORs into a shared bitmap and flushes its non-zero words once.
-template <typename T>
+template <typename Src>
 __global__ void __launch_bounds__(256)
-k_cm_count(const SemCfg sc, const T* __restrict__ pts, const i64 n, const i64 stride, const int* __restrict__ pidx,
+k_cm_count(const SemCfg sc, const Src src, const i64 n, const int* __restrict__ pidx,
            const int* __restrict__ idm, const i64 n_idm, const SemMax ms) {
   __shared__ u32 bm[CM_WORDS];
   for (int w = threadIdx.x; w < CM_WORDS; w += blockDim.x) bm[w] = 0;
@@ -125,10 +123,9 @@ k_cm_count(const SemCfg sc, const T* __restrict__ pts, const i64 n, const i64 st
   for (i64 i = blockIdx.x * (i64)blockDim.x + threadIdx.x; i < n; i += step) {
     const int rec = pidx[i];
     if (rec & PT_SKIP) continue;                                  // EM.py:458 dropped the row: not in points_all
-    const T* row = pts + i * stride;
     for (int k = 0; k < sc.n_ch; k++) {
       if (sc.kind[k] != SEM_CLASS_MAX) continue;
-      const u32 id = __float_as_uint((float)row[sc.col[k]]) >> 16;
+      const u32 id = __float_as_uint(src.feature(i, sc.col[k])) >> 16;
       atomicOr(bm + (id >> 5), 1u << (id & 31));
     }
     if ((rec & (PT_VALID | PT_INSIDE)) == (PT_VALID | PT_INSIDE)) atomicAdd(ms.cnt + (rec & PT_IDX_MASK), (u32)sc.n_max);

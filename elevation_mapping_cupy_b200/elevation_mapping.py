@@ -20,6 +20,8 @@ and one kernel per batch (csrc/emap_submap.cuh).
 The rest of the node's map timer is served too: the normals (get_normal_maps / get_normal_ref), the bridge's normal
 colour as the exported layer `normal_color`, and the exported map as a point cloud (get_map_points) and as normal arrows
 (get_normal_arrows), compacted in grid_map's cell order on the device (csrc/emap_mapcloud.cuh).
+Depth cameras (input_depth_image / input_depth_images) fuse without the semantic sensor node's intermediate cloud: the
+frame reads the depth, confidence, rgb and feature planes itself (csrc/emap_sources.cuh).
 Out of scope (SURVEY.md section 8): the image feature extractors.
 """
 import ctypes as C
@@ -311,6 +313,70 @@ class ElevationMap:
             self._check(self._L.emap_input_sensors(self._h, ns, ptrs, counts, stride, dt, int(bool(device_ptrs)),
                                                    Rm.ctypes.data, tm.ctypes.data, float(position_noise),
                                                    float(orientation_noise)))
+
+    def input_depth_image(self, depth, P, R, t, position_noise: float, orientation_noise: float, channels=(), rgb=None,
+                          features=None, confidence=None, confidence_threshold: float = 10.0, max_depth: float = 8.0):
+        """A depth camera frame: the semantic sensor node's create_pcl_from_image (pointcloud_node.py:205-274) and
+        input_pointcloud of its cloud in one library call, with no intermediate cloud (emap_input_depth_image).
+        depth: (H, W) metres; P: CameraInfo P (3x4) or K (3x3); R, t: optical frame -> map; confidence: (H, W), pixels
+        below `confidence_threshold` are dropped (pointcloud_parameters.py:42), as are pixels that are not finite, <= 0
+        or >= `max_depth` (the node's 8 m).  `channels` are the cloud's extra channel names: one whose fusion is `color`
+        reads `rgb` ((H, W, 3) uint8), the others read the planes of `features` ((n, H, W) float32) in order.  Arrays of
+        any framework; all host or all device."""
+        self.input_depth_images([dict(depth=depth, P=P, R=R, t=t, rgb=rgb, features=features, confidence=confidence)],
+                                position_noise, orientation_noise, channels, confidence_threshold, max_depth)
+
+    def input_depth_images(self, cameras, position_noise: float, orientation_noise: float, channels=(),
+                           confidence_threshold: float = 10.0, max_depth: float = 8.0):
+        """Several depth cameras of one time slice fused against the same snapshot, as input_sensors fuses clouds.
+        `cameras`: dicts with the keys depth, P, R, t and optionally rgb, features, confidence (see input_depth_image);
+        `channels` is shared by every camera."""
+        channels = list(channels)
+        if channels or self.semantic_map._configured is not None:
+            self.semantic_map.configure_for(["x", "y", "z"] + channels)
+        sources, k = [], 0
+        for ch in channels:                       # the node's rule: the `color` channel takes rgb, the others the planes
+            if self.semantic_map.layer_specs_points.get(ch) == "color":
+                sources.append(-1)
+            else:
+                sources.append(k); k += 1
+        n = len(cameras)
+        if not 1 <= n <= _lib.EMAP_DEPTH_MAX_CAMERAS:
+            raise ValueError(f"1 to {_lib.EMAP_DEPTH_MAX_CAMERAS} cameras per call")
+        dev = _on_device(cameras[0]["depth"])
+        keep, cams, n_features = [], (_lib.EmapDepthCamera * n)(), 0
+        for i, cam in enumerate(cameras):
+            depth = _depth_input(cam["depth"], np.float32, dev, self.device, keep)
+            if depth.ndim != 2:
+                raise ValueError("depth must be an (H, W) array")
+            H, W = depth.shape
+            c = cams[i]
+            c.height, c.width, c.depth = H, W, _address(depth)
+            for name, dtype, shape in (("confidence", np.float32, (H, W)), ("rgb", np.uint8, (H, W, 3)),
+                                       ("features", np.float32, None)):
+                if cam.get(name) is None:
+                    continue
+                a = _depth_input(cam[name], dtype, dev, self.device, keep)
+                if tuple(a.shape) != shape and not (shape is None and a.ndim == 3 and tuple(a.shape[1:]) == (H, W)):
+                    raise ValueError(f"{name} has shape {tuple(a.shape)} for a {H}x{W} depth image")
+                setattr(c, name, _address(a))
+                if name == "features":
+                    n_features = a.shape[0] if i == 0 else min(n_features, a.shape[0])
+            Pm = np.asarray(_to_host(cam["P"]), np.float64)
+            c.fx, c.fy, c.cx, c.cy = Pm[0, 0], Pm[1, 1], Pm[0, 2], Pm[1, 2]
+            c.R[:] = np.asarray(_to_host(cam["R"]), np.float32).reshape(9).tolist()
+            c.t[:] = np.asarray(_to_host(cam["t"]), np.float32).reshape(3).tolist()
+        src = (C.c_int32 * max(len(sources), 1))(*sources)
+        with self.map_lock:
+            self._after_framework()       # framework work writing the images or reading the aliased layers comes first
+            rc = self._L.emap_input_depth_images(self._h, n, cams, int(dev), len(sources), src, n_features,
+                                                 float(confidence_threshold), float(max_depth), float(position_noise),
+                                                 float(orientation_noise))
+            # framework work queued from here on sees the fused map, and the device images (the caller's, or the
+            # converted copies in `keep`, freed on return) are released or rewritten only after the frame has read them
+            # (no host sync)
+            self._before_framework()
+            self._check(rc)
 
     # ---- queries -------------------------------------------------------------------------------
     def get_additive_mean_error(self):
@@ -689,6 +755,38 @@ def _to_host(x):
 
 def _is_device(x):
     return getattr(x, "__cuda_array_interface__", None) is not None if not hasattr(x, "is_cuda") else bool(x.is_cuda)
+
+
+def _depth_input(x, dtype, dev, device, keep):
+    """One input of input_depth_images as a contiguous array of `dtype` (a list of planes is stacked): a torch CUDA tensor
+    when the call's inputs are on the device, else a NumPy array (a pinned torch CPU tensor stays in its pinned memory).
+    The array is appended to `keep` for the duration of the call."""
+    if _on_device(x) != dev:
+        raise ValueError("depth-image inputs must be all host or all device arrays")
+    if dev:
+        import torch
+        td = torch.uint8 if dtype == np.uint8 else torch.float32
+        as_t = lambda p: torch.as_tensor(p, device=f"cuda:{device}")
+        a = (torch.stack([as_t(p) for p in x]) if isinstance(x, (list, tuple)) else as_t(x)).to(td).contiguous()
+    else:
+        a = np.ascontiguousarray(np.stack([_to_host(p) for p in x]) if isinstance(x, (list, tuple)) else _to_host(x),
+                                 dtype=dtype)
+    keep.append(a)
+    return a
+
+
+def _on_device(x):
+    """Is x (an array, or a list of planes that are all host or all device arrays) in device memory?"""
+    if isinstance(x, (list, tuple)):
+        kinds = {_is_device(p) for p in x}
+        if len(kinds) != 1:
+            raise ValueError("a list of planes must be all host or all device arrays")
+        return kinds.pop()
+    return _is_device(x)
+
+
+def _address(a):
+    return a.data_ptr() if hasattr(a, "data_ptr") else a.ctypes.data
 
 
 def _image_stack(image, device):

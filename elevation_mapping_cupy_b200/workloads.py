@@ -128,3 +128,27 @@ def reference_test_cloud(seed, n=100000, n_ch=3):
     rng = np.random.default_rng(seed)
     return (rng.random((n, n_ch), dtype=np.float32), rng.random((3, 3), dtype=np.float32),
             rng.random(3, dtype=np.float32))
+
+
+def depth_image(frame, width=640, height=480, max_range=10.0, hole_frac=0.03, sensor=0):
+    """Depth image (32FC1 metres) of the terrain from an optical camera (x right, y down, z forward) 1.0 m above the
+    ground, pitched 30 deg down, with a 90 deg horizontal field of view; rays that hit nothing within max_range read
+    max_range, and a fraction of pixels are holes (NaN, 0 or -inf).  Returns (depth (H, W) f32, P (3x4) f64, R, t), R, t
+    the optical -> map pose in fp32.  `sensor` turns the camera by 90 deg about z per step."""
+    f = float(frame)
+    rng = rng_for(9, frame, sensor)
+    fx = fy = 0.5 * width
+    cx, cy = 0.5 * (width - 1) + 0.25, 0.5 * (height - 1) - 0.25
+    P = np.array([[fx, 0, cx, 0], [0, fy, cy, 0], [0, 0, 1, 0]], np.float64)
+    R_opt = np.array([[0, 0, 1], [-1, 0, 0], [0, -1, 0]], np.float64)       # optical axes in the body frame
+    R = (_rot_z(0.01 * f + 0.5 * np.pi * sensor) @ _rot_y(np.deg2rad(30.0)) @ R_opt).astype(np.float32)
+    t = np.array([0.04 * f + 0.2 * sensor, 0.02 * f, 1.0 + terrain(0.04 * f, 0.02 * f)], np.float32)
+    u, v = np.meshgrid(np.arange(width), np.arange(height), indexing="xy")
+    d_o = np.stack([(u - cx) / fx, (v - cy) / fy, np.ones_like(u, np.float64)], -1).reshape(-1, 3)
+    norm = np.linalg.norm(d_o, axis=1)
+    rr = _ray_terrain(t.astype(np.float64), (d_o / norm[:, None]) @ R.astype(np.float64).T, max_range, coarse=0.1)
+    depth = (rr / norm).astype(np.float32).reshape(height, width)
+    depth += rng.normal(0.0, 0.003, depth.shape).astype(np.float32)
+    holes = rng.random(depth.shape) < hole_frac
+    depth[holes] = rng.choice(np.array([np.nan, 0.0, -np.inf], np.float32), int(holes.sum()))
+    return depth, P, R, t

@@ -88,7 +88,7 @@ typedef struct emap_frame_stats {
   int64_t error_cnt;           /* EM.py:329 */
   int32_t drift_applied;
   int32_t drift_evaluated;
-  int64_t n_points;            /* points in the frame (NaN rows included) */
+  int64_t n_points;            /* points in the frame (NaN rows included; a depth-image frame: its kept pixels) */
   int64_t n_valid_points;      /* points passing is_valid (CK.py:68-81) */
   int64_t ray_steps;           /* ray-march iterations (CK.py:203), 0 unless counting is enabled */
   int64_t ray_visits;          /* cells examined by rays past the skips of CK.py:209-226 */
@@ -159,6 +159,55 @@ int emap_semantic_configure_ext(emap_handle* h, int32_t n_channels, const int32_
 /* CK.py:260-262 write-back of the last frame, on the DEVICE: one packed int32 per input row (bits 0..23 cell index,
  * bit 28 valid, bit 29 inside, bit 30 row dropped as NaN); valid until the next frame. */
 int emap_point_record_device_ptr(emap_handle* h, const int32_t** packed_device, int64_t* n);
+
+/* ---- depth cameras: the semantic sensor node's depth-image -> cloud step (sensor_processing/semantic_sensor/script/
+ * semantic_sensor/pointcloud_node.py:205-274 create_pcl_from_image, get_coordinates, process_image) fused into the frame
+ * with no intermediate cloud.  Per camera: depth (height, width) fp32 metres (the node's 32FC1 `passthrough`), optional
+ * confidence (height, width) fp32, optional rgb (height, width, 3) uint8, optional features (n_features, height, width)
+ * fp32; fx, fy, cx, cy = CameraInfo P[0], P[5], P[2], P[6]; R (3x3 row-major), t: the optical frame -> map pose, fp32 as
+ * for emap_input_sensors.
+ *  1. Mask: pixel (v, u) is kept iff isfinite(d) && d > 0 && d < max_depth && (no confidence || q >= confidence_threshold),
+ *     compared in fp32 (the node's max(rint(fin + pos + conf + low - 2.6), 0) is this AND; its max_depth is 8).
+ *  2. The kept pixels in row-major order (v, then u: nonzero's order), camera after camera, are the rows of the cloud.
+ *  3. x = fp32(((double)u - cx) * (double)d / fx), y = fp32(((double)v - cy) * (double)d / fy), each operation rounded
+ *     once in double, no contraction; z = d.
+ *  4. Extra channel j (column 3 + j of the row, as emap_semantic_configure* addresses it) reads channel_source[j]: -1 the
+ *     packed colour (r << 16) | (g << 8) | b as fp32 bits (at most one channel), k >= 0 feature plane k, bits as they are.
+ *  5. The frame is bit for bit emap_input_sensors(h, n_cameras, clouds, ..., R, t, ...) of the clouds of steps 1-4
+ *     (state, normals, semantic layers and their fusion state, emap_get_frame_stats; n_points = the kept pixels).
+ *  6. Point record: one row per PIXEL, camera after camera; masked pixels are dropped rows (idx -1, bit 30 on the device
+ *     record), the kept ones equal the cloud frame's record.
+ * Inputs are all host memory or all device memory (is_device_ptr), staged as clouds are: device images are read in place
+ * (no host synchronisation, capturable into a CUDA graph under the rules of emap_set_stream, which binds the image
+ * pointers, sizes, intrinsics and channel sources too), page-locked host images over PCIe, pageable ones are staged;
+ * host images are free to reuse on return.  Kernel launches: those of the cloud frame with the same channel
+ * configuration.  Not applied to sharded frames.
+ * EMAP_ERR_INVALID, with nothing launched and the state unchanged, for: n_cameras outside [1, EMAP_DEPTH_MAX_CAMERAS], a
+ * NULL depth, height or width <= 0 or height * width > 2^24 (so a frame has fewer than 2^31 pixels), non-finite or zero fx / fy,
+ * non-finite cx / cy / R / t, n_channels outside [0, EMAP_DEPTH_MAX_CHANNELS], n_features outside
+ * [0, EMAP_DEPTH_MAX_FEATURES], a source outside [-1, n_features), more
+ * than one colour channel, a colour channel without rgb or a feature channel without features, and a configured semantic
+ * column >= 3 + n_channels.  EMAP_ERR_STATE on a handle attached to sharded scratch. */
+#define EMAP_DEPTH_MAX_CAMERAS 16
+#define EMAP_DEPTH_MAX_CHANNELS 16
+#define EMAP_DEPTH_MAX_FEATURES 255
+typedef struct emap_depth_camera {
+  int32_t height, width;
+  const float* depth;
+  const float* confidence;       /* or NULL */
+  const uint8_t* rgb;            /* or NULL */
+  const float* features;         /* or NULL */
+  double fx, fy, cx, cy;
+  float R[9];
+  float t[3];
+} emap_depth_camera;
+int emap_input_depth_images(emap_handle* h, int32_t n_cameras, const emap_depth_camera* cameras, int is_device_ptr,
+                            int32_t n_channels, const int32_t* channel_source, int32_t n_features,
+                            float confidence_threshold, float max_depth, float position_noise, float orientation_noise);
+/* emap_input_depth_images with one camera. */
+int emap_input_depth_image(emap_handle* h, const emap_depth_camera* camera, int is_device_ptr, int32_t n_channels,
+                           const int32_t* channel_source, int32_t n_features, float confidence_threshold, float max_depth,
+                           float position_noise, float orientation_noise);
 
 /* ---- sharded frame (one rank per GPU, replicated grid; SURVEY 8(e)).  Between the phases the
  * caller all-reduces the exchange buffers in place (SUM for the int64/uint32 words named
