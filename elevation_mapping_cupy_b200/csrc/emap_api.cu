@@ -102,6 +102,7 @@ struct emap_handle {
   ~emap_handle();
   emap_config cfg;
   DevCfg dc;
+  FramePlan plan;             // make_plan: march table, kernel variants, shared-memory layouts
   int device = 0;
   std::mutex mu;
   std::string err;
@@ -122,17 +123,12 @@ struct emap_handle {
   FrameScalars* fs = nullptr;
   DevBuf<char> xscratch;      // the library's exchange scratch (carve_exchange): sc's per-cell arrays + fs; empty once attached
   DevBuf<int> ukey_x;         // exchange copy of the upper-bound keys (sharded frames)
-  DevBuf<float> steps;        // device march table: [0] dummy, [1 + k] = s_k, +inf padded to n_tab entries
-  int n_tab = 0;
-  std::vector<float> steps_host;
+  DevBuf<float> steps;        // device march table: [0] dummy, [1 + k] = s_k, +inf padded to plan.n_tab entries
   DevBuf<unsigned short> lut;        // cell of every fp16 bit pattern (k_build_lut)
   DevBuf<unsigned short> step_cnt;   // march steps below every non-negative fp16 value (k_build_step_cnt)
   DevBuf<unsigned char> dirty;       // per-cell dirty bytes of single-GPU frames (CellScratch::dirty)
   DevBuf<float> thr;                 // CellScratch::thr
   DevBuf<u32> tmap;                  // coarse ray map of the frame: RT x RT tile maxima of thr (keys)
-  size_t rc_smem = 0;
-  RcLayout rc_lay{};
-  int span_cells = 0;              // cells (per axis) one 31-step warp iteration of the march can span
   // points
   DevBuf<char> d_in[2];
   Event in_free[2], copy_done;
@@ -248,8 +244,6 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
     LAUNCH_CHECK();                                                                               \
   } while (0)
 
-inline float h16_host(float x) { return __half2float(__float2half_rn(x)); }
-
 inline int cdiv(i64 a, int b) { return (int)((a + b - 1) / b); }
 
 int fail(emap_handle* h, int code, const char* msg) {
@@ -260,57 +254,6 @@ int fail(emap_handle* h, int code, const char* msg) {
 void make_pose(const float* R, const float* t_rel, Pose* q) {
   for (int i = 0; i < 9; i++) q->R16[i] = h16_host(R[i]);
   for (int i = 0; i < 3; i++) { q->t16[i] = h16_host(t_rel[i]); q->t[i] = t_rel[i]; }
-}
-
-void fill_devcfg(const emap_config& c, DevCfg& d) {
-  memset(&d, 0, sizeof(d));
-  d.W = c.cell_n; d.C = c.cell_n * c.cell_n;
-  d.dilation = c.dilation_size; d.edge_sharpen = c.enable_edge_sharpen; d.drift_en = c.enable_drift_compensation;
-  d.visibility = c.enable_visibility_cleanup; d.overlap = c.enable_overlap_clearance;
-  // EM.py:87-91
-  int cell_range = (int)(c.overlap_clear_range_xy / c.resolution);
-  if (cell_range < 0) cell_range = 0;
-  if (cell_range > c.cell_n) cell_range = c.cell_n;
-  d.cell_min = c.cell_n / 2 - cell_range / 2; d.cell_max = c.cell_n / 2 + cell_range / 2;
-  d.resolution = c.resolution; d.half_w = 0.5 * (double)c.cell_n;
-  d.snf = c.sensor_noise_factor; d.mahal = c.mahalanobis_thresh; d.outlier_var = c.outlier_variance;
-  d.inlier_var_half = c.drift_compensation_variance_inlier / 2.0; d.trav_inlier = c.traversability_inlier;
-  d.wall_thresh = c.wall_num_thresh; d.min_drift_cnt = c.min_height_drift_cnt;
-  d.max_ray_length = c.max_ray_length; d.cleanup_step = c.cleanup_step; d.cos_thresh = c.cleanup_cos_thresh;
-  d.mvd2 = c.min_valid_distance * c.min_valid_distance; d.max_height = c.max_height_range;
-  d.ramp_a = c.ramped_height_range_a; d.ramp_b = c.ramped_height_range_b; d.ramp_c = c.ramped_height_range_c;
-  d.max_variance = c.max_variance; d.pos_thresh = c.position_noise_thresh; d.ori_thresh = c.orientation_noise_thresh;
-  d.inv_res_f = (float)(1.0 / c.resolution); d.half_w_f = (float)(0.5 * (double)c.cell_n);
-  d.c_out = (float)c.outlier_variance; d.init_var = (float)c.initial_variance;
-  d.max_drift_f = (float)c.max_drift; d.drift_alpha_f = (float)c.drift_compensation_alpha;
-  d.max_len16 = h16_host((float)c.max_ray_length);
-  d.w_plus_half_f = (float)c.cell_n + 0.5f;
-  d.res_f = (float)c.resolution;
-  d.overlap_z_f = (float)c.overlap_clear_range_z; d.time_var_f = (float)c.time_variance;
-  d.time_int_f = (float)c.time_interval;
-  // ray-march cell table: fp16 coordinates are clamped to [-LIM, LIM], LIM = the first fp16 value >= (W/2 + 1) * resolution;
-  // every value at or beyond +-LIM maps to cell W-1 / 0, so only the bit patterns [0, P) and [0x8000, 0x8000 + P) are staged
-  {
-    const double want = (0.5 * (double)c.cell_n + 1.0) * c.resolution;
-    __half hl = __float2half_ru((float)std::min(want, 60000.0));
-    unsigned short bits = __half_as_ushort(hl);
-    if (bits > 0x7bff) bits = 0x7bff;
-    d.lut_lim2 = ((u32)bits << 16) | bits;
-    d.lut_p2 = (int)(((size_t)(bits + 1) * 2 + 15) & ~(size_t)15);
-  }
-}
-
-// CK.py:203,268: the fp16 march variable, identical for every ray
-void build_steps(const emap_config& c, float max_len16, std::vector<float>& out) {
-  const double ray_step = c.resolution / std::sqrt(2.0);
-  out.clear();
-  float s = h16_host((float)ray_step);
-  while (s < max_len16 && out.size() < 65535) {
-    out.push_back(s);
-    float nx = h16_host((float)((double)s + ray_step));
-    if (!(nx > s)) break;      // fp16 spacing exceeded the step: the reference would spin forever
-    s = nx;
-  }
 }
 
 // Makes b hold at least n elements.  A smaller buffer is replaced by one of n + slack elements (zero-filled on the
@@ -647,43 +590,6 @@ int frame_semantic(emap_handle* h) {
   return 0;
 }
 
-// Cells a ray of this frame can reach.  A sample is t + ray*s with |ray| <= 1 per axis and s < len <= max_len16, so it
-// lies within max_len16 of the sensor on each axis; its fp16 rounding moves it by at most 2^-11 of its magnitude.
-// Rows [r0, r1) x columns [c0, c1), columns aligned to `align`; union over the frame's sensors, two cells of slack.
-// Tile size 2^ts: at most RT tiles per axis, and a double-size tile at least half the span of one warp iteration
-// (so that an iteration starting anywhere in a double tile stays inside the 3 x 3 block k_raycast tests).
-RayGrid ray_grid(const emap_handle* h, int align) {
-  const int W = h->dc.W;
-  int r0 = W, r1 = 0, c0 = W, c1 = 0;
-  const double L = (double)h->dc.max_len16;
-  for (const Pose& q : h->poses) {
-    for (int ax = 0; ax < 2; ax++) {
-      const double tc = (double)q.t[ax];
-      const double e = (std::fabs(tc) + L) * (1.0 / 2048.0) + 1e-4;
-      double lo = std::floor((tc - L - e) / h->dc.resolution + h->dc.half_w) - 2.0;
-      double hi = std::floor((tc + L + e) / h->dc.resolution + h->dc.half_w) + 3.0;
-      if (!(lo == lo) || !(hi == hi)) { lo = 0; hi = W; }         // NaN pose: whole map
-      const int a = (int)std::min(std::max(lo, 0.0), (double)W), b = (int)std::min(std::max(hi, 0.0), (double)W);
-      if (ax == 0) { r0 = std::min(r0, a); r1 = std::max(r1, b); } else { c0 = std::min(c0, a); c1 = std::max(c1, b); }
-    }
-  }
-  RayGrid g{0, 0, 0, 0, 3, 0, 0};
-  if (r1 <= r0 || c1 <= c0) return g;
-  c0 = (c0 / align) * align; c1 = std::min(W, ((c1 + align - 1) / align) * align);
-  g.r0 = r0; g.r1 = r1; g.c0 = c0; g.c1 = c1;
-  // tiles are aligned to the map (tile = cell >> ts) and the coarse maps start at a double-tile boundary at or before
-  // (r0, c0): RT tiles per axis must reach the far edge of the box from there
-  for (int ts = 2;; ts++) {
-    const int al = 2 << ts;
-    const int r0a = (r0 / al) * al, c0a = (c0 / al) * al;
-    if ((RT << ts) >= std::max(r1 - r0a, c1 - c0a) && (4 << ts) >= h->span_cells + 1) {
-      g.ts = ts; g.ta = r0a >> ts; g.tb = c0a >> ts;
-      break;
-    }
-  }
-  return g;
-}
-
 int frame_rays(emap_handle* h) {
   NvtxRange nv("emap:record+raycast");
   const bool deferred = h->attached && h->n_points > 0;
@@ -697,8 +603,8 @@ int frame_rays(emap_handle* h) {
     CK(cudaEventRecord(h->ev_join, h->side_stream));
   }
   if (h->dc.visibility) {
-    const int V = (h->dc.W % 4 == 0) ? 4 : 1;
-    const RayGrid box = ray_grid(h, V);
+    const int V = h->plan.cells_per_thread;
+    const RayGrid box = ray_box(h->dc, h->plan, h->poses.data(), (int)h->poses.size());
     const i64 nthreads = (i64)(box.r1 - box.r0) * ((box.c1 - box.c0) / V);
     if (nthreads > 0) {
       if (V == 4) PDL(k_record<4>, cdiv(nthreads, 256), 256, 0, h->dc, (const float*)h->map, h->sc, (const FrameScalars*)h->fs, box, h->tmap);
@@ -708,19 +614,15 @@ int frame_rays(emap_handle* h) {
     if (stage_mark(h, 4)) return EMAP_ERR_CUDA;
     for (size_t s = 0; s + 1 < h->offs.size(); s++) {
       const i64 n = h->offs[s + 1] - h->offs[s];
-      if (n <= 0 || h->dc.n_steps == 0) continue;
-      // No map cell within reach of the frame's sensors (empty box): every sample clamps to the border ring, on which no
-      // ray acts, and k_raycast<false>'s fine-tile address would lie outside its coarse map.  The counting variant reads
-      // no coarse map and still counts the march steps.
-      if (!h->count_rays && (box.r1 <= box.r0 || box.c1 <= box.c0)) continue;
+      if (!raycast_runs(box, n, h->dc.n_steps, h->count_rays != 0)) continue;
       // persistent grid: enough CTAs to fill every SM, never more than one warp per possible ray
       const int grid = (int)std::min<i64>((i64)h->n_sm * h->rc_blocks_per_sm, (n + RC_THREADS / 32 - 1) / (RC_THREADS / 32));
       if (h->count_rays)
-        PDL(k_raycast<true>, grid, RC_THREADS, h->rc_smem, h->dc, h->poses[s], (const Ray*)(h->rays + h->offs[s]), h->ray_ctl + RC_CTL * (int)s,
-            (const float*)h->map, (const float*)h->normal, h->sc, (const float*)h->steps, h->n_tab, (const unsigned short*)h->lut, box, (const u32*)h->tmap, h->rc_lay, h->fs);
+        PDL(k_raycast<true>, grid, RC_THREADS, h->plan.rc_smem, h->dc, h->poses[s], (const Ray*)(h->rays + h->offs[s]), h->ray_ctl + RC_CTL * (int)s,
+            (const float*)h->map, (const float*)h->normal, h->sc, (const float*)h->steps, h->plan.n_tab, (const unsigned short*)h->lut, box, (const u32*)h->tmap, h->plan.rc_lay, h->fs);
       else
-        PDL(k_raycast<false>, grid, RC_THREADS, h->rc_smem, h->dc, h->poses[s], (const Ray*)(h->rays + h->offs[s]), h->ray_ctl + RC_CTL * (int)s,
-            (const float*)h->map, (const float*)h->normal, h->sc, (const float*)h->steps, h->n_tab, (const unsigned short*)h->lut, box, (const u32*)h->tmap, h->rc_lay, h->fs);
+        PDL(k_raycast<false>, grid, RC_THREADS, h->plan.rc_smem, h->dc, h->poses[s], (const Ray*)(h->rays + h->offs[s]), h->ray_ctl + RC_CTL * (int)s,
+            (const float*)h->map, (const float*)h->normal, h->sc, (const float*)h->steps, h->plan.n_tab, (const unsigned short*)h->lut, box, (const u32*)h->tmap, h->plan.rc_lay, h->fs);
       LAUNCH_CHECK();
     }
   } else if (stage_mark(h, 4)) return EMAP_ERR_CUDA;
@@ -730,16 +632,12 @@ int frame_rays(emap_handle* h) {
   return 0;
 }
 
-size_t post_smem(const DevCfg& d) {
-  const int HL = d.dilation + 3, HLX = (HL + 3) & ~3;
-  const size_t plane = (size_t)(((PT_Y + 2 * HL) * (PT_X + 2 * HLX) + 31) & ~31);
-  return sizeof(float) * (3 * plane + (size_t)(PT_Y + 6) * (PT_X + 6) + 2) + sizeof(unsigned long long) * (size_t)(PT_Y + 2 * HL + 2);
-}
-
 // TMA descriptor of the state buffer for k_post: tensor (x = column, y = row, z = layer), box = staged tile + halo of one
-// layer; out-of-range elements are filled with zeros.  cuTensorMapEncodeTiled is fetched from the driver at run time
-// (no link-time dependency on libcuda).
+// layer; out-of-range elements are filled with zeros.  Encoded only when the plan stages k_post's tiles with TMA.
+// cuTensorMapEncodeTiled is fetched from the driver at run time (no link-time dependency on libcuda).
 int make_post_tm(emap_handle* h) {
+  memset(&h->post_tm, 0, sizeof(CUtensorMap));
+  if (!h->dc.post_tma) return 0;
   typedef CUresult (*encode_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -751,12 +649,8 @@ int make_post_tm(emap_handle* h) {
       return fail(h, EMAP_ERR_CUDA, "cuTensorMapEncodeTiled not available from the driver");
     enc = (encode_fn)fn;
   }
-  memset(&h->post_tm, 0, sizeof(CUtensorMap));
   const int W = h->dc.W;
   const int HL = h->dc.dilation + 3, HLX = (HL + 3) & ~3;
-  // plain loads instead when the row pitch is not a multiple of 16 bytes, or the map is smaller than one staged box
-  h->dc.post_tma = (W % 4 == 0 && W >= PT_X + 2 * HLX && W >= PT_Y + 2 * HL) ? 1 : 0;
-  if (!h->dc.post_tma) return 0;
   const cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)W, 7};
   const cuuint64_t strides[2] = {(cuuint64_t)W * 4, (cuuint64_t)W * W * 4};
   const cuuint32_t box[3] = {(cuuint32_t)(PT_X + 2 * HLX), (cuuint32_t)(PT_Y + 2 * HL), 1};
@@ -770,9 +664,9 @@ int make_post_tm(emap_handle* h) {
 
 int launch_post(emap_handle* h) {
   dim3 grid(cdiv(h->dc.W, PT_X), cdiv(h->dc.W, PT_Y));
-  const size_t sm = post_smem(h->dc);
+  const size_t sm = h->plan.post_smem;
   const CUtensorMap& tm = h->post_tm;
-  switch (h->dc.dilation) {
+  switch (h->plan.post_instance) {
     case 1: PDL(k_post<1>, grid, 256, sm, h->dc, h->map, h->trav_input, h->normal, tm); break;
     case 2: PDL(k_post<2>, grid, 256, sm, h->dc, h->map, h->trav_input, h->normal, tm); break;
     case 3: PDL(k_post<3>, grid, 256, sm, h->dc, h->map, h->trav_input, h->normal, tm); break;
@@ -784,7 +678,7 @@ int launch_post(emap_handle* h) {
 
 int frame_finish(emap_handle* h) {
   NvtxRange nv("emap:finalize+post");
-  if (h->dc.W % 4 == 0) PDL(k_finalize<4>, cdiv(h->dc.C / 4, 256), 256, 0, h->dc, h->map, h->sc, (const FrameScalars*)h->fs, h->dc.visibility, h->ray_ctl, (int)h->ray_ctl.size(), h->fused_drift ? h->fs : nullptr, h->tmap);
+  if (h->plan.cells_per_thread == 4) PDL(k_finalize<4>, cdiv(h->dc.C / 4, 256), 256, 0, h->dc, h->map, h->sc, (const FrameScalars*)h->fs, h->dc.visibility, h->ray_ctl, (int)h->ray_ctl.size(), h->fused_drift ? h->fs : nullptr, h->tmap);
   else PDL(k_finalize<1>, cdiv(h->dc.C, 256), 256, 0, h->dc, h->map, h->sc, (const FrameScalars*)h->fs, h->dc.visibility, h->ray_ctl, (int)h->ray_ctl.size(), h->fused_drift ? h->fs : nullptr, h->tmap);
   LAUNCH_CHECK();
   if (stage_mark(h, 6)) return EMAP_ERR_CUDA;
@@ -1043,54 +937,6 @@ int alloc_polygon_scratch(emap_handle* h, const PolySizes& z, PolyScratch& s) {
   return 0;
 }
 
-// EM.py:847-854: each coordinate clipped to [center - map_length/2 + resolution, center + map_length/2 - resolution],
-// fp32 throughout; map_length is the map's true length (cell_n - 2) * resolution.  Writes the clipped vertices (unless
-// out is NULL) and their bounding box.
-void clip_polygon(const emap_handle* h, const float* xy, int n, float2* out, float bbox[4]) {
-  const float half = (float)(0.5 * (double)(h->dc.W - 2) * h->cfg.resolution), res_f = h->dc.res_f;
-  float lo[2], hi[2], bmin[2], bmax[2];
-  for (int k = 0; k < 2; k++) {
-    lo[k] = (h->center[k] - half) + res_f;
-    hi[k] = (h->center[k] + half) - res_f;
-  }
-  for (int i = 0; i < n; i++) {
-    float v[2];
-    for (int k = 0; k < 2; k++) {
-      v[k] = std::min(std::max(xy[2 * i + k], lo[k]), hi[k]);
-      bmin[k] = i ? std::min(bmin[k], v[k]) : v[k];
-      bmax[k] = i ? std::max(bmax[k], v[k]) : v[k];
-    }
-    if (out) out[i] = make_float2(v[0], v[1]);
-  }
-  bbox[0] = bmin[0]; bbox[1] = bmin[1]; bbox[2] = bmax[0]; bbox[3] = bmax[1];
-}
-
-// The tiles of k_polygon's grid that meet the polygon's cell bounding box (CK.py:609-615, the cells k_polygon tests)
-// and the interior columns of that box, the only ones that can hold its over-threshold cells.
-void polygon_tiles(const emap_handle* h, PolyDesc& d) {
-  const int W = h->dc.W;
-  const float rf = h->dc.res_f;
-  const int bx0 = poly_axis_cell(d.bbox[0], h->center[0], rf, W), bx1 = poly_axis_cell(d.bbox[2], h->center[0], rf, W);
-  const int by0 = poly_axis_cell(d.bbox[1], h->center[1], rf, W), by1 = poly_axis_cell(d.bbox[3], h->center[1], rf, W);
-  d.tr0 = bx0 / PG_ROWS; d.n_tr = bx1 / PG_ROWS - d.tr0 + 1;
-  d.tc0 = by0 / PG_COLS; d.n_tc = by1 / PG_COLS - d.tc0 + 1;
-  d.col0 = std::max(by0, 1) - 1;
-  d.n_col = std::max(0, std::min(by1, W - 2) - std::max(by0, 1) + 1);
-}
-
-// traversability_polygon.py:46-51 calculate_area on fp32 vertices: every operation in fp32, terms in order i = 0..n-1
-// with p1 = polygon[i - 1], the absolute value at the end
-float shoelace_f32(const float* xy, int n) {
-  float area = 0.0f;
-  for (int i = 0; i < n; i++) {
-    const int j = i ? i - 1 : n - 1;
-    const float a = xy[2 * j] * xy[2 * i + 1];
-    const float b = xy[2 * j + 1] * xy[2 * i];
-    area = area + (a - b) / 2.0f;
-  }
-  return std::fabs(area);
-}
-
 // The device part of a call whose n_poly polygons (n_items work items) are staged in the upload region of h->pg_host:
 // one upload copy, k_poly_poison (with `poison`), k_polygon, k_hull, one copy of the results and the first `head` ring
 // rows into the read-back region of h->pg_host, one synchronisation; one more copy and synchronisation only if a ring
@@ -1189,10 +1035,7 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   };
   cudaError_t e;
   if ((e = cudaSetDevice(device)) != cudaSuccess) return bail("cudaSetDevice", e);
-  fill_devcfg(*cfg, h->dc);
-  build_steps(*cfg, h->dc.max_len16, h->steps_host);
-  h->dc.n_steps = (int)h->steps_host.size();
-  h->dc.first_step = h->steps_host.empty() ? INFINITY : h->steps_host[0];
+  make_plan(*cfg, h->dc, h->plan);
   const size_t C = (size_t)h->dc.C;
   for (Stream* s : {&h->own_stream, &h->copy_stream, &h->side_stream})
     if ((e = s->create(cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
@@ -1215,10 +1058,7 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   ALLOC(h->lut, 65536);
   ALLOC(h->tmap, RT * RT);
   ALLOC(h->step_cnt, 0x7c00 + 8);
-  // march table as k_raycast reads it: [0] unused (lane 0 of the first warp iteration), [1 + k] = s_k, +inf padding up to
-  // a whole number of 31-step warp iterations + one warp of over-read
-  h->n_tab = (int)(((h->steps_host.size() + RC_STRIDE - 1) / RC_STRIDE) * RC_STRIDE + 64) & ~1;
-  ALLOC(h->steps, h->n_tab);
+  ALLOC(h->steps, h->plan.n_tab);
 #undef ALLOC
   h->sc.thr = h->thr;
   h->sc.dirty = h->dirty;
@@ -1229,9 +1069,9 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   TRY(cudaMemsetAsync(h->normal, 0, sizeof(float) * 3 * C, h->stream));
   TRY(cudaMemsetAsync(h->trav_input, 0, sizeof(float) * C, h->stream));
   {
-    std::vector<float> tab((size_t)h->n_tab, INFINITY);
+    std::vector<float> tab((size_t)h->plan.n_tab, INFINITY);
     tab[0] = NAN;       // "step -1" of lane 0 in a ray's first warp iteration: NaN -> cell (0, 0), see k_raycast
-    for (size_t k = 0; k < h->steps_host.size(); k++) tab[1 + k] = h->steps_host[k];
+    for (size_t k = 0; k < h->plan.steps.size(); k++) tab[1 + k] = h->plan.steps[k];
     // pageable source: the copy is staged before the call returns, and the stream is synchronised below
     TRY(cudaMemcpyAsync(h->steps, tab.data(), sizeof(float) * tab.size(), cudaMemcpyHostToDevice, h->stream));
     TRY(cudaStreamSynchronize(h->stream));
@@ -1243,39 +1083,16 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   if (make_post_tm(h)) {
     g_create_error = h->err; delete h; return EMAP_ERR_CUDA;
   }
-  if (post_smem(h->dc) > 48 * 1024)
-    TRY(cudaFuncSetAttribute(k_post<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)post_smem(h->dc)));
-  {
-    {   // one warp iteration of the march: 30 steps between its first and last new sample, in cells (+1: fp16 coordinates)
-      double span = 0;
-      const std::vector<float>& st = h->steps_host;
-      for (size_t k = 0; k + 1 < st.size(); k++) {
-        const size_t e = std::min(st.size() - 1, k + RC_STRIDE - 1);
-        span = std::max(span, ((double)st[e] - (double)st[k]) / cfg->resolution);
-      }
-      h->span_cells = (int)std::ceil(span) + 2;
-    }
-    {   // shared-memory layout of k_raycast: coarse maps + march table in the gap between the two halves of the cell
-        // table when they fit there, else behind the second half
-      const size_t P2 = (size_t)h->dc.lut_p2;
-      const size_t need = sizeof(float) * (RT * RT + (RT / 2) * (RT / 2) + (size_t)h->n_tab) + 16;
-      size_t base = (P2 + 15) & ~(size_t)15, end = 65536 + P2;
-      if (base + need > 65536) { base = (end + 15) & ~(size_t)15; end = base + need; }
-      h->rc_lay.off_t8 = (int)base;
-      h->rc_lay.off_t16 = (int)(base + sizeof(float) * RT * RT);
-      h->rc_lay.off_steps = (int)(base + sizeof(float) * (RT * RT + (RT / 2) * (RT / 2)));
-      h->rc_lay.off_bar = (int)((base + need - 16 + 7) & ~(size_t)7);
-      h->rc_smem = end;
-    }
-    TRY(cudaFuncSetAttribute(k_raycast<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->rc_smem));
-    TRY(cudaFuncSetAttribute(k_raycast<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->rc_smem));
-    cudaDeviceProp prop;
-    if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) h->n_sm = prop.multiProcessorCount;
-    int nb = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_raycast<false>, RC_THREADS, h->rc_smem) == cudaSuccess && nb > 0)
-      h->rc_blocks_per_sm = nb;
-    else h->rc_blocks_per_sm = 1;
-  }
+  if (h->plan.post_smem > 48 * 1024)
+    TRY(cudaFuncSetAttribute(k_post<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->plan.post_smem));
+  TRY(cudaFuncSetAttribute(k_raycast<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->plan.rc_smem));
+  TRY(cudaFuncSetAttribute(k_raycast<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)h->plan.rc_smem));
+  cudaDeviceProp prop;
+  if (cudaGetDeviceProperties(&prop, device) == cudaSuccess) h->n_sm = prop.multiProcessorCount;
+  int nb = 0;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_raycast<false>, RC_THREADS, h->plan.rc_smem) == cudaSuccess && nb > 0)
+    h->rc_blocks_per_sm = nb;
+  else h->rc_blocks_per_sm = 1;
   TRY(cudaStreamSynchronize(h->stream));
   TRY(cudaGetLastError());
 #undef TRY
@@ -2069,7 +1886,7 @@ int emap_polygon_traversability(emap_handle* h, const float* polygon_xy, int32_t
   const float area = shoelace_f32(polygon_xy, n_vertices);
   PolyDesc d = {};
   float2* xy = (float2*)(h->pg_host + st.xy);
-  clip_polygon(h, polygon_xy, n_vertices, xy, d.bbox);
+  clip_polygon(W, h->cfg.resolution, h->center, polygon_xy, n_vertices, xy, d.bbox);
   const float clipped_area = shoelace_f32((const float*)xy, n_vertices);
   d.v0 = 0; d.n = n_vertices; d.item0 = 0;
   d.tr0 = 0; d.tc0 = 0; d.n_tr = g.y; d.n_tc = g.x;
@@ -2126,8 +1943,8 @@ int emap_polygon_traversability_batch(emap_handle* h, int32_t n_polygons, const 
   size_t items = 0, cols = 0, rows = 0, v0 = 0;
   for (int i = 0; i < n_polygons; i++) {
     PolyDesc& d = desc[i];
-    clip_polygon(h, polygon_xy + 2 * v0, n_vertices[i], nullptr, d.bbox);
-    polygon_tiles(h, d);
+    clip_polygon(h->dc.W, h->cfg.resolution, h->center, polygon_xy + 2 * v0, n_vertices[i], nullptr, d.bbox);
+    polygon_tiles(h->dc.W, h->cfg.resolution, h->center, d);
     if (whole_map) {
       d.tr0 = 0; d.tc0 = 0; d.n_tr = g.y; d.n_tc = g.x;
       d.col0 = 0; d.n_col = h->dc.W - 2;
@@ -2153,7 +1970,7 @@ int emap_polygon_traversability_batch(emap_handle* h, int32_t n_polygons, const 
     const PolyDesc& d = desc[i];
     area[i] = shoelace_f32(polygon_xy + 2 * (size_t)d.v0, d.n);
     float bbox[4];
-    clip_polygon(h, polygon_xy + 2 * (size_t)d.v0, d.n, xy + d.v0, bbox);
+    clip_polygon(h->dc.W, h->cfg.resolution, h->center, polygon_xy + 2 * (size_t)d.v0, d.n, xy + d.v0, bbox);
     clipped_area[i] = shoelace_f32((const float*)(xy + d.v0), d.n);
   }
   rc = run_polygons(h, s, st, n_polygons, (int)items, true, checker_plane, safe_thresh, safe_min_thresh, max_unsafe_n,

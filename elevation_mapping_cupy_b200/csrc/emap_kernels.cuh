@@ -15,6 +15,7 @@
 // oracle/emap_oracle.c; they are within one fp32 rounding of some order of the reference atomics.
 #pragma once
 #include <cuda.h>                 // CUtensorMap (type only; the encoder is fetched at run time, emap_api.cu)
+#include "emap_plan.cuh"         // RT, RayGrid, RC_STRIDE, RcLayout, PT_X, PT_Y
 #include "emap_sources.cuh"
 
 // ------------------------------------------------------------------------------------------
@@ -38,12 +39,6 @@ struct CellScratch {
                    // (0 = single GPU).  Non-zero: every accumulation is one multimem.red that the NVSwitch
                    // applies to the replicas of ALL ranks (this one included) -- scatter and collective fused.
 };
-
-// Geometry of the cells a ray of this frame can reach, and of the coarse maps over them (ray_box in emap_api.cu):
-// rows [r0, r1) x columns [c0, c1) (c0, c1 multiples of 4 when W is); fine tiles of 2^ts x 2^ts cells aligned to the
-// map (tile of a cell = cell >> ts), at most RT x RT of them from tile (ta, tb) on, covering the whole box.
-#define RT 64                     // fine tiles per axis of the coarse ray maps
-struct RayGrid { int r0, r1, c0, c1, ts, ta, tb; };   // (ta, tb): tile coordinates (cell >> ts) of the coarse maps' origin, both even
 
 // accumulate into the per-cell scratch: local L2 atomic, or one in-switch multicast reduction
 __device__ __forceinline__ void red_add(u32* p, u32 v, i64 mc) {
@@ -516,12 +511,10 @@ __global__ void __launch_bounds__(256) k_build_lut(const DevCfg c, unsigned shor
 //     take the exact second level.  The effects of a visit are commutative integer atomics, so neither lane
 //     nor ray order matters.
 #define RC_THREADS 768
-#define RC_STRIDE 31              // new march steps per warp iteration
 #define RC_CTL 64                 // ints of control state per sensor: [0] ray count, [32] the work counter (128 B apart)
 #ifndef RC_BATCH
 #define RC_BATCH 4                // rays a warp draws from the work counter at a time
 #endif
-struct RcLayout { int off_t8, off_t16, off_steps, off_bar; };     // byte offsets of the shared-memory regions (host: rc_layout)
 
 // cell of the sample t + ray*s (CK.py:205-207 -> 26-33) through the staged table; all lanes must pass in-range addresses
 __device__ __forceinline__ void rc_cell(const u32 s_lut, const u32 lim2, const u32 nlim2, const float nx, const float ny,
@@ -877,11 +870,8 @@ k_finalize(const DevCfg c, float* __restrict__ map, const CellScratch s, const F
 // (EM.py:376-383) -> traversability_input; traversability CNN (traversability_filter.py:15-42)
 // -> map[3][3:-3,3:-3] (EM.py:385-388); normals of the dilated map (CK.py:452-506, EM.py:564-577).
 // One CTA per PT_Y x PT_X tile; the (tile + halo) of the two input planes is staged in shared
-// memory once, the dilated tile (+3 halo) stays in shared memory for the CNN and the normals.
-#define PT_X 32
-#ifndef PT_Y
-#define PT_Y 16
-#endif
+// memory once, the dilated tile (+3 halo) stays in shared memory for the CNN and the normals.  The tile size and the
+// shared-memory size are in emap_plan.cuh.
 
 // two channels' taps: acc.{x,y} = fma(w.{x,y}, t, acc.{x,y}), each IEEE round-to-nearest.  Hopper has no paired
 // fp32 FMA, so this is two scalar FFMAs (the same rounding, so the same bits).

@@ -13,6 +13,9 @@
 // k_hull: one CTA per polygon sums its partials in a fixed order (the result does not depend on scheduling) and builds
 // the convex hull of its over-threshold cells (traversability_polygon.py:46-53) from the column extremes.
 #pragma once
+#include <algorithm>
+#include <cmath>
+
 #include "emap_device.cuh"
 
 #define PG_COLS 32               // columns per k_polygon tile (one warp wide: coalesced rows)
@@ -80,6 +83,54 @@ __host__ __device__ __forceinline__ int poly_axis_cell(float v, float c, float r
   const int i = q != q ? 0 : (q >= 2147483647.0 ? 2147483647 : (q <= -2147483648.0 ? (-2147483647 - 1) : (int)q));
   return i < 0 ? 0 : (i > W - 1 ? W - 1 : i);
 #endif
+}
+
+// EM.py:847-854: each coordinate clipped to [center - map_length/2 + resolution, center + map_length/2 - resolution],
+// fp32 throughout; map_length is the map's true length (W - 2) * resolution.  Writes the clipped vertices (unless out
+// is NULL) and their bounding box.
+inline void clip_polygon(int W, double resolution, const float* center, const float* xy, int n, float2* out,
+                         float bbox[4]) {
+  const float half = (float)(0.5 * (double)(W - 2) * resolution), res_f = (float)resolution;
+  float lo[2], hi[2], bmin[2], bmax[2];
+  for (int k = 0; k < 2; k++) {
+    lo[k] = (center[k] - half) + res_f;
+    hi[k] = (center[k] + half) - res_f;
+  }
+  for (int i = 0; i < n; i++) {
+    float v[2];
+    for (int k = 0; k < 2; k++) {
+      v[k] = std::min(std::max(xy[2 * i + k], lo[k]), hi[k]);
+      bmin[k] = i ? std::min(bmin[k], v[k]) : v[k];
+      bmax[k] = i ? std::max(bmax[k], v[k]) : v[k];
+    }
+    if (out) out[i] = make_float2(v[0], v[1]);
+  }
+  bbox[0] = bmin[0]; bbox[1] = bmin[1]; bbox[2] = bmax[0]; bbox[3] = bmax[1];
+}
+
+// The tiles of k_polygon's grid that meet the polygon's cell bounding box d.bbox (CK.py:609-615, the cells k_polygon
+// tests) and the interior columns of that box, the only ones that can hold its over-threshold cells.
+inline void polygon_tiles(int W, double resolution, const float* center, PolyDesc& d) {
+  const float rf = (float)resolution;
+  const int bx0 = poly_axis_cell(d.bbox[0], center[0], rf, W), bx1 = poly_axis_cell(d.bbox[2], center[0], rf, W);
+  const int by0 = poly_axis_cell(d.bbox[1], center[1], rf, W), by1 = poly_axis_cell(d.bbox[3], center[1], rf, W);
+  d.tr0 = bx0 / PG_ROWS; d.n_tr = bx1 / PG_ROWS - d.tr0 + 1;
+  d.tc0 = by0 / PG_COLS; d.n_tc = by1 / PG_COLS - d.tc0 + 1;
+  d.col0 = std::max(by0, 1) - 1;
+  d.n_col = std::max(0, std::min(by1, W - 2) - std::max(by0, 1) + 1);
+}
+
+// traversability_polygon.py:46-51 calculate_area on fp32 vertices: every operation in fp32, terms in order i = 0..n-1
+// with p1 = polygon[i - 1], the absolute value at the end
+inline float shoelace_f32(const float* xy, int n) {
+  float area = 0.0f;
+  for (int i = 0; i < n; i++) {
+    const int j = i ? i - 1 : n - 1;
+    const float a = xy[2 * j] * xy[2 * i + 1];
+    const float b = xy[2 * j + 1] * xy[2 * i];
+    area = area + (a - b) / 2.0f;
+  }
+  return std::fabs(area);
 }
 
 // CK.py:513-560: orientation of the ordered integer triplet (0 collinear, 1 clockwise, 2 counter-clockwise) and the

@@ -1,18 +1,14 @@
-"""The host-side decisions of a frame, restated in NumPy, and the cases of the frame-variant tests.
+"""The cases of the frame-variant tests and the oracles that check the ray box against march samples.
 
 The host picks kernel variants and shared-memory layouts from cell_n, resolution, max_ray_length, dilation_size, the
-sensor poses and the input buffer (elevation_mapping_cupy_b200/csrc/emap_api.cu).  Each function below restates one of
-those choices and cites the lines it restates, so that the tests can say which side of every choice a case is on
-(tests/test_frame_variants_cpu.py checks that each side has a case) and can check the ray box against march samples
-computed independently of the engine.
+sensor poses and the input buffer (make_plan, ray_box and raycast_runs in elevation_mapping_cupy_b200/csrc/emap_plan.cuh,
+called through tests/plan_host.py).  tests/test_frame_variants_cpu.py checks that every side of each choice has a case
+below, and that the ray box holds the march samples computed here independently of the engine.
 """
-import math
-
 import numpy as np
 
-RT = 64               # fine tiles per axis of the coarse ray maps (emap_kernels.cuh RT)
-RC_STRIDE = 31        # new march steps per warp iteration (emap_kernels.cuh RC_STRIDE)
-PT_X, PT_Y = 32, 16   # k_post tile (emap_kernels.cuh PT_X, PT_Y)
+import plan_host
+
 CORE_RES, CORE_RAY = 0.04, 10.0       # resolution and max_ray_length of core_parameter()
 
 
@@ -21,148 +17,16 @@ def h16(x):
     return float(np.float16(np.float32(x)))
 
 
-def _h16_up(x):
-    """__float2half_ru of an fp32 value."""
-    x = np.float32(x)
-    h = np.float16(x)
-    if np.float32(h) < x:
-        h = np.nextafter(h, np.float16(np.inf))
-    return h
-
-
-# ---- k_post ---------------------------------------------------------------------------------------------------------
-def post_tma(W, K):
-    """emap_api.cu:616-618 make_post_tm: k_post stages its tiles with TMA tensor copies when the row pitch is a multiple of
-    16 bytes and the map holds one staged box; plain loads otherwise."""
-    HL = K + 3
-    HLX = (HL + 3) & ~3
-    return W % 4 == 0 and W >= PT_X + 2 * HLX and W >= PT_Y + 2 * HL
-
-
-def post_instance(K):
-    """emap_api.cu:635-640 launch_post: the k_post<K> instantiation (0 = dilation read at run time)."""
-    return K if K in (1, 2, 3) else 0
-
-
-def record_v(W):
-    """emap_api.cu:559 and 647-648: cells per thread of k_record and k_finalize (and the ray box's column alignment)."""
-    return 4 if W % 4 == 0 else 1
-
-
-# ---- ray-march tables and the k_raycast shared-memory layout ----------------------------------------------------------
-def max_len16(max_ray_length):
-    """emap_api.cu:227 fill_devcfg max_len16"""
-    return h16(max_ray_length)
-
-
-def lut_p2(W, res):
-    """emap_api.cu:232-241 fill_devcfg: bytes of one half of the staged cell table (fp16 patterns [0, LIM])."""
-    want = (0.5 * W + 1.0) * res
-    bits = int(np.array(_h16_up(min(want, 60000.0))).view(np.uint16))
-    bits = min(bits, 0x7BFF)
-    return ((bits + 1) * 2 + 15) & ~15
-
-
-def march_steps(res, max_ray_length):
-    """emap_api.cu:244-255 build_steps: the fp16 march variable s_k < max_len16 (CK.py:203,268)."""
-    step = res / math.sqrt(2.0)
-    L = max_len16(max_ray_length)
-    out = []
-    s = h16(step)
-    while s < L and len(out) < 65535:
-        out.append(s)
-        nx = h16(s + step)
-        if not nx > s:
-            break
-        s = nx
-    return np.array(out, np.float32)
-
-
-def n_steps(res, max_ray_length):
-    return len(march_steps(res, max_ray_length))
-
-
-def n_tab(n):
-    """emap_api.cu:889: floats of the march table as k_raycast stages it"""
-    return (((n + RC_STRIDE - 1) // RC_STRIDE) * RC_STRIDE + 64) & ~1
-
-
-def span_cells(res, max_ray_length):
-    """emap_api.cu:918-926: cells per axis one 31-step warp iteration of the march can span"""
-    st = march_steps(res, max_ray_length).astype(np.float64)
-    span = 0.0
-    for k in range(len(st) - 1):
-        e = min(len(st) - 1, k + RC_STRIDE - 1)
-        span = max(span, (st[e] - st[k]) / res)
-    return int(math.ceil(span)) + 2
-
-
-def rc_layout(W, res, max_ray_length):
-    """emap_api.cu:927-938 emap_create: byte offsets of k_raycast's shared-memory regions.  The coarse maps and the march
-    table sit in the gap between the two halves of the cell table when they fit there ("gap"), else behind the second
-    half ("behind")."""
-    P2 = lut_p2(W, res)
-    need = 4 * (RT * RT + (RT // 2) * (RT // 2) + n_tab(n_steps(res, max_ray_length))) + 16
-    base, end = (P2 + 15) & ~15, 65536 + P2
-    where = "gap"
-    if base + need > 65536:
-        base = (end + 15) & ~15
-        end = base + need
-        where = "behind"
-    return dict(where=where, p2=P2, off_t8=base, off_t16=base + 4 * RT * RT,
-                off_steps=base + 4 * (RT * RT + (RT // 2) * (RT // 2)), rc_smem=end)
-
-
 # ---- the ray box ----------------------------------------------------------------------------------------------------
-def ray_grid(W, res, max_ray_length, t_rel):
-    """emap_api.cu:509-544 ray_grid: (r0, r1, c0, c1, ts, ta, tb), the box of cells the rays of a frame can reach and its
-    tiling.  t_rel: the sensors' positions relative to the map centre (fp32, as emap_api.cu:393 computes them)."""
-    align = record_v(W)
-    L = float(np.float32(max_len16(max_ray_length)))
-    half_w = 0.5 * W
-    r0, r1, c0, c1 = W, 0, W, 0
-    for t in t_rel:
-        for ax in range(2):
-            tc = float(np.float32(t[ax]))
-            e = (abs(tc) + L) * (1.0 / 2048.0) + 1e-4
-            lo = math.floor((tc - L - e) / res + half_w) - 2.0
-            hi = math.floor((tc + L + e) / res + half_w) + 3.0
-            a, b = int(min(max(lo, 0.0), W)), int(min(max(hi, 0.0), W))
-            if ax == 0:
-                r0, r1 = min(r0, a), max(r1, b)
-            else:
-                c0, c1 = min(c0, a), max(c1, b)
-    if r1 <= r0 or c1 <= c0:
-        return (0, 0, 0, 0, 3, 0, 0)
-    c0 = (c0 // align) * align
-    c1 = min(W, ((c1 + align - 1) // align) * align)
-    sp = span_cells(res, max_ray_length)
-    ts = 2
-    while True:
-        al = 2 << ts
-        r0a, c0a = (r0 // al) * al, (c0 // al) * al
-        if (RT << ts) >= max(r1 - r0a, c1 - c0a) and (4 << ts) >= sp + 1:
-            return (r0, r1, c0, c1, ts, r0a >> ts, c0a >> ts)
-        ts += 1
-
-
 def box_empty(box):
     return box[1] <= box[0] or box[3] <= box[2]
 
 
-def raycast_launched(box, n_rays, n_steps_, count_rays=False):
-    """emap_api.cu:568-574 frame_rays: whether k_raycast runs for a sensor.  The counting variant (emap_set_ray_counting) reads no
-    coarse map and runs for every sensor with rays; the march itself only where the box holds a cell."""
-    if n_rays <= 0 or n_steps_ == 0:
-        return False
-    return count_rays or not box_empty(box)
-
-
-def t8_address(layout, box, ix, iy):
-    """emap_kernels.cuh:596,670: the shared-memory byte address of the fine-tile maximum k_raycast<false> reads for cell
-    (ix, iy)"""
+def t8_address(plan, box, ix, iy):
+    """k_raycast: the shared-memory byte address of the fine-tile maximum k_raycast<false> reads for cell (ix, iy)"""
     _, _, _, _, ts, ta, tb = box
-    return layout["off_t8"] + 4 * (((np.asarray(ix) >> ts) - ta) * RT + ((np.asarray(iy) >> ts) - tb))
+    RT = plan_host.constants()["RT"]
+    return plan["off_t8"] + 4 * (((np.asarray(ix) >> ts) - ta) * RT + ((np.asarray(iy) >> ts) - tb))
 
 
 # ---- rays and march samples -----------------------------------------------------------------------------------------
@@ -176,7 +40,7 @@ def rays_of(t_rel, points, max_ray_length):
     norm = f16(np.sqrt((v[:, 0] * v[:, 0] + v[:, 1] * v[:, 1]) + v[:, 2] * v[:, 2]))
     with np.errstate(invalid="ignore", divide="ignore"):
         r = np.where(norm[:, None] > 0, f16(v / norm[:, None]), np.float32(0))
-    length = np.minimum(norm, np.float32(max_len16(max_ray_length)))
+    length = np.minimum(norm, np.float32(h16(max_ray_length)))
     return r[:, 0], r[:, 1], r[:, 2], length
 
 
@@ -197,7 +61,7 @@ def march_cells(W, res, steps, t_rel, rx, ry, length):
 
 def address_samples(W, ix, iy, live):
     """The samples at which k_raycast forms a fine-tile address: a cell different from the previous sample's
-    (emap_kernels.cuh:662-665; before the first sample lane 0 supplies cell (0, 0), emap_api.cu:902)."""
+    (k_raycast; before the first sample lane 0 supplies cell (0, 0), the NaN entry [0] of the march table)."""
     nidx = ix * W + iy
     prev = np.concatenate([np.zeros((nidx.shape[0], 1), np.int64), nidx[:, :-1]], 1)
     return live & (nidx != prev)
@@ -255,12 +119,12 @@ LAYOUTS = ["f32-host", "f32x4-device", "f32x4-device-unaligned", "f32-pinned", "
 
 def layout_path(layout):
     """(where the index pass reads the rows, whether it takes the 16-byte vector load) of a layout:
-    emap_api.cu:404-437 frame_begin (staged copy, zero-copy, device) and emap_kernels.cuh:146-154 load_point<float>"""
+    frame_begin / stage_inputs (staged copy, zero-copy, device) and load_point<float> (emap_sources.cuh)"""
     where = {"f32-host": "staged", "f32-pinned": "zero-copy", "f64-pinned": "zero-copy"}.get(layout, "device")
     return where, layout == "f32x4-device"
 
 
-MANY_SENSORS = 70     # more than the 64 sensor pointers frame_begin keeps on the stack (emap_api.cu:400-403)
+MANY_SENSORS = 70     # more than 64 sensors in one frame
 
 
 def frame_params(case):

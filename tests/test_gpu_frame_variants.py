@@ -1,7 +1,7 @@
 """GPU: whole frames at the configurations the other frame tests never reach, against OracleElevationMap.  Bar as in
 tests/test_gpu_parity.py: every state plane bit-identical except traversability (2e-6), plus the point record and the
-frame statistics.  The cases and the host decisions each group is meant to reach come from tests/frame_variants.py
-(checked without a GPU by tests/test_frame_variants_cpu.py); every group also asserts them here."""
+frame statistics.  The cases come from tests/frame_variants.py; tests/test_frame_variants_cpu.py checks without a GPU
+that each group reaches the host decisions it is meant to reach."""
 import types
 
 import numpy as np
@@ -45,10 +45,6 @@ def _random_state(W, seed, valid_frac=0.2):
 def test_frames_at_other_resolutions_ray_lengths_and_sizes(oracle_mod, case):
     from elevation_mapping_cupy_b200 import workloads as wl
     W, res, L = fv.frame_params(case)
-    lay = fv.rc_layout(W, res, L)
-    assert lay["where"] == ("behind" if case["id"] in ("res0.1-2048", "ray40-1024") else "gap"), lay
-    assert (res == fv.CORE_RES) == (case["id"] in ("ray0.5-1024", "ray40-1024", "odd-2049"))
-    assert fv.record_v(W) == (1 if W % 4 else 4)
     p = _param(W, **case["kw"])
     em = _mk(p); om = oracle_mod.OracleElevationMap(p, nthreads=0)
     half = 0.5 * (W - 2) * res
@@ -73,12 +69,7 @@ def test_frames_at_other_resolutions_ray_lengths_and_sizes(oracle_mod, case):
 def test_post_every_dilation_on_random_state(oracle_mod, W):
     """dilation K = 0..8 (the flat-index row wrap on populated border columns) + CNN + normals, driven by an empty
     cloud, with TMA staging or plain loads as the host picks them"""
-    paths = set()
     for K in fv.POST_KS:
-        tma = fv.post_tma(W, K)
-        paths.add((tma, fv.post_instance(K)))
-        if W == 48:
-            assert tma == (K <= 5)
         p = _param(W, dilation_size=K, enable_visibility_cleanup=(K % 2 == 0))
         em = _mk(p); om = oracle_mod.OracleElevationMap(p, nthreads=0)
         st = _random_state(W, 1000 * W + K)
@@ -88,9 +79,8 @@ def test_post_every_dilation_on_random_state(oracle_mod, W):
         em.input_pointcloud(empty, ["x", "y", "z"], R, t, 0.0, 0.0)
         om.input_pointcloud(empty, ["x", "y", "z"], R, t, 0.0, 0.0)
         state, normal = em.get_state()
-        compare_state(state, normal, om, label=f"post {W}/K{K} ({'TMA' if tma else 'plain loads'})")
+        compare_state(state, normal, om, label=f"post {W}/K{K}")
         assert np.array_equal(em.traversability_input.cpu().numpy(), om.traversability_input), (W, K)
-    assert len({k for _, k in paths}) == 4 and len({t for t, _ in paths}) == (2 if W == 48 else 1), paths
 
 
 # ---- C: sensor poses at and beyond the map edge ---------------------------------------------------------------------
@@ -110,11 +100,7 @@ def test_sensor_poses_at_and_beyond_the_map_edge(oracle_mod, W):
     beyond an edge within and beyond max_ray_length (an empty ray box), two sensors far apart and a sensor below the
     terrain; once with the march and once with the step-counting march, whose statistics must equal the oracle's"""
     p = _param(W)
-    sides = set()
     for k, (cid, ts) in enumerate(fv.pose_cases(W)):
-        box = fv.ray_grid(W, fv.CORE_RES, fv.CORE_RAY, ts)
-        sides.add(fv.box_empty(box))
-        assert fv.box_empty(box) == cid.startswith("beyond-far"), (cid, box)
         rng = np.random.default_rng(W + k)
         clouds = [_pose_cloud(t, rng) for t in ts]
         Rs = [np.eye(3, dtype=np.float32)] * len(ts)
@@ -135,7 +121,6 @@ def test_sensor_poses_at_and_beyond_the_map_edge(oracle_mod, W):
             assert stc.ray_steps > 0, cid
             for m in (em, emc, om):
                 m.update_time()
-    assert sides == {True, False}
 
 
 # ---- D: input layouts -----------------------------------------------------------------------------------------------

@@ -1,7 +1,8 @@
 """The batch polygon check's work list (no GPU needed): emap_polygon_traversability_batch gives each polygon only the
 k_polygon tiles (PG_COLS = 32 columns by PG_ROWS = 64 rows, aligned to the map) that meet its cell bounding box, and
-keeps its column extremes over the box's interior columns.  Restated here in NumPy, the enumeration must hold every cell
-of the oracle's mask, so that no polygon loses a cell to a tile it was not given."""
+keeps its column extremes over the box's interior columns.  The library's enumeration (clip_polygon and polygon_tiles in
+emap_polygon.cuh, through tests/plan_host.py) must hold every cell of the oracle's mask, so that no polygon loses a cell
+to a tile it was not given."""
 import os
 import sys
 
@@ -10,20 +11,8 @@ import pytest
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, HERE)
+import plan_host as ph               # noqa: E402
 import polygon_oracle as PO          # noqa: E402
-
-PG_COLS, PG_ROWS = 32, 64
-
-
-def tiles(poly, center, W, resolution):
-    """polygon_tiles() in emap_api.cu: (tile rows, tile columns, interior column window [col0, col0 + n_col))."""
-    _, bbox = PO.clip_polygon(poly, center, W, resolution)
-    bx0, bx1 = PO.vertex_cells(bbox[[0, 2]], np.float32(center[0]), resolution, W)
-    by0, by1 = PO.vertex_cells(bbox[[1, 3]], np.float32(center[1]), resolution, W)
-    rows = range(bx0 // PG_ROWS, bx1 // PG_ROWS + 1)
-    cols = range(by0 // PG_COLS, by1 // PG_COLS + 1)
-    col0 = max(by0, 1) - 1
-    return rows, cols, col0, max(0, min(by1, W - 2) - max(by0, 1) + 1)
 
 
 def _polygons(W, resolution, rng):
@@ -43,11 +32,13 @@ def _polygons(W, resolution, rng):
 def test_enumerated_tiles_hold_every_mask_cell(W):
     resolution = 0.04
     rng = np.random.default_rng(W)
+    k = ph.constants()
+    PG_COLS, PG_ROWS = k["PG_COLS"], k["PG_ROWS"]
     n_cells = 0
     for poly, center in _polygons(W, resolution, rng):
         clipped, bbox = PO.clip_polygon(poly, center, W, resolution)
         mask = PO.polygon_mask(clipped, bbox, center, resolution, W)
-        rows, cols, col0, n_col = tiles(poly, center, W, resolution)
+        rows, cols, col0, n_col = ph.polygon_tiles(poly, center, W, resolution)
         cover = np.zeros((W, W), bool)
         for r in rows:
             for c in cols:
