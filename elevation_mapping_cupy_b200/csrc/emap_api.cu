@@ -91,6 +91,45 @@ struct StagedUpload {
   int send(emap_handle* h, size_t n);      // queues the upload of the first n staged bytes on the handle's stream
 };
 
+// The input of a frame: where its kernels read every sensor's points, and when the caller may reuse its host memory.
+// A frame describes it (kind, rows, the caller's buffers); stage() makes the buffers readable by the kernels, each()
+// hands every sensor's point source to a launch, read_done() follows each pass that reads them, and wait_free()
+// returns once the caller may reuse them.
+struct FrameInput {
+  enum Kind { F32_ROWS, F64_ROWS, DEPTH };
+  enum Residence { DEVICE, STAGED, ZERO_COPY };    // the caller's device memory, a staged copy, page-locked host memory
+  DevBuf<char> staging[2];                         // used by alternate staged frames
+  Event staging_free[2], copied, host_free;        // staging block b reusable; staged copies done; zero-copy input read
+  int buf = 1;                                     // staging block of the last staged frame
+  Kind kind = F32_ROWS;                // the current frame's kind and residence
+  Residence res = DEVICE;
+  bool read = false, held = false;     // read_done() has run; wait_free() has yet to wait
+  std::vector<int64_t> n;              // rows of sensor s
+  // bytes[k] bytes at bufs[k] as the caller passed them (rows: sensor s's at k = s; DEPTH: camera s's depth,
+  // confidence, rgb and feature planes at k = 4s .. 4s + 3), read by the kernels at readable[k] (stage)
+  std::vector<const void*> bufs, readable;
+  std::vector<size_t> bytes;
+  int64_t stride = 0;                  // rows: elements from one row to the next
+  std::vector<DepthSource> cams;       // DEPTH: camera s, pointed at its planes by stage() (a null conf stays null)
+  int stage(emap_handle* h, int is_device_ptr);
+  int read_done(emap_handle* h);
+  int wait_free(emap_handle* h);
+  template <typename F>     // f(src, s) for the point source of every sensor s (float or double rows, or a camera)
+  int each(F&& f) const {   // until one returns non-zero
+    for (int s = 0; s < (int)n.size(); s++) {
+      const int rc = kind == DEPTH ? f(cams[s], s)
+                   : kind == F32_ROWS ? f(RowSource<float>{(const float*)readable[s], stride}, s)
+                                      : f(RowSource<double>{(const double*)readable[s], stride}, s);
+      if (rc) return rc;
+    }
+    return 0;
+  }
+};
+
+// How far the current frame has come (a sharded frame's caller drives it one call at a time): none, input staged, the
+// index / fusion / ray-cast pass queued, or exchange 3 took the upper-bound keys (the finish merges them back first)
+enum class Progress { IDLE, BEGUN, INDEXED, FUSED, RAYS_CAST, KEYS_EXCHANGED };
+
 // sizes of the polygon check's scratch (carve_polygon): upload bytes, partials, column extremes, read-back bytes
 struct PolySizes {
   size_t up = 0, items = 0, cols = 0, down = 0;
@@ -130,9 +169,7 @@ struct emap_handle {
   DevBuf<float> thr;                 // CellScratch::thr
   DevBuf<u32> tmap;                  // coarse ray map of the frame: RT x RT tile maxima of thr (keys)
   // points
-  DevBuf<char> d_in[2];
-  Event in_free[2], copy_done;
-  int in_sel = 0;
+  FrameInput in;
   DevBuf<float4> xyzv;
   DevBuf<int> pidx;
   DevBuf<Ray> rays;           // compacted rays of the frame, one segment per sensor (at the sensor's point offset)
@@ -145,17 +182,10 @@ struct emap_handle {
   std::vector<i64> offs;      // n_sensors + 1
   i64 n_points = 0, global_off = 0;
   float pos_noise = 0, ori_noise = 0;
-  int phase = 0;              // sharded-frame state machine
+  Progress progress = Progress::IDLE;
   bool fused_drift = false;   // single-GPU frame: no k_drift launch (k_fuse decides, k_finalize resets)
   // multicast-attached scratch (sharded frames over NVLink multicast, emap_shard_attach)
   bool attached = false;
-  std::vector<const void*> pend_pts;   // device pointers of the frame's clouds (index pass deferred to phase 0)
-  std::vector<int64_t> pend_n;
-  int64_t pend_stride = 0;
-  int pend_dtype = 0, pend_host = 0;
-  bool zero_copy_pending = false;      // the index pass reads the caller's pinned host buffer: sync before returning
-  bool depth_frame = false;            // the last frame reads depth images (pend_cams) instead of clouds
-  std::vector<DepthSource> pend_cams;
   // export staging
   DevBuf<float> d_export;
   // plugin scratch
@@ -360,22 +390,9 @@ int stage_mark(emap_handle* h, int k) {
   return 0;
 }
 
-// f(src, s) for the point source of every sensor s of the pending frame: its cloud rows typed by pend_dtype (float or
-// double), or its depth camera; stops at the first non-zero return
-template <typename F>
-int each_cloud(emap_handle* h, F&& f) {
-  for (int s = 0; s < (int)h->pend_n.size(); s++) {
-    const int rc = h->depth_frame ? f(h->pend_cams[s], s)
-                 : h->pend_dtype == EMAP_F32 ? f(RowSource<float>{(const float*)h->pend_pts[s], h->pend_stride}, s)
-                                             : f(RowSource<double>{(const double*)h->pend_pts[s], h->pend_stride}, s);
-    if (rc) return rc;
-  }
-  return 0;
-}
-
 template <typename Src>
 int launch_index(emap_handle* h, const Src& src, int s) {
-  const i64 n = h->pend_n[s], off = h->offs[s];
+  const i64 n = h->in.n[s], off = h->offs[s];
   if (n <= 0) return 0;
   PDL(k_index_error<Src>, cdiv(n, 256), 256, 0, h->dc, h->poses[s], src, n, h->xyzv + off, h->pidx + off,
       (const float*)h->map, h->sc, h->fs, h->rays + off, h->ray_ctl + RC_CTL * s, (const unsigned short*)h->step_cnt);
@@ -383,57 +400,74 @@ int launch_index(emap_handle* h, const Src& src, int s) {
   return 0;
 }
 
-// Makes the frame's n_buf input buffers (bytes[k] bytes at ptrs[k], host or device memory) readable by its kernels, at
-// dp[k].  Device memory is read in place.  Host buffers that are all page-locked (cudaHostAlloc / cudaHostRegister /
-// torch pin_memory) are read by the kernels directly over PCIe (zero-copy): no staging copy, no copy-engine round trip.
-// Otherwise every buffer is staged, 256-byte aligned, into one of two device buffers on the copy stream.
-int stage_inputs(emap_handle* h, int n_buf, const void* const* ptrs, const size_t* bytes, int is_device_ptr,
-                 const void** dp) {
-  bool zero_copy = false;
-  if (!is_device_ptr) {
-    zero_copy = true;
-    for (int k = 0; k < n_buf && zero_copy; k++) {
-      if (bytes[k] == 0) { dp[k] = ptrs[k]; continue; }
-      cudaPointerAttributes at;
-      if (cudaPointerGetAttributes(&at, ptrs[k]) != cudaSuccess || at.type != cudaMemoryTypeHost || !at.devicePointer) {
-        cudaGetLastError(); zero_copy = false;
-      } else dp[k] = at.devicePointer;
-    }
+// Makes the frame's buffers readable by its kernels at readable[k], and points the depth cameras there.  Device
+// memory is read in place.  Host buffers that are all page-locked (cudaHostAlloc / cudaHostRegister / torch pin_memory)
+// are read by the kernels directly over PCIe (zero-copy): no staging copy, no copy-engine round trip.  Otherwise every
+// buffer is staged, 256-byte aligned, into the staging block the last staged frame did not use, on the copy stream.
+int FrameInput::stage(emap_handle* h, int is_device_ptr) {
+  readable = bufs;
+  res = is_device_ptr ? DEVICE : ZERO_COPY; read = false; held = !is_device_ptr;
+  for (size_t k = 0; k < bufs.size() && res == ZERO_COPY; k++) {
+    if (bytes[k] == 0) continue;
+    cudaPointerAttributes at;
+    if (cudaPointerGetAttributes(&at, bufs[k]) != cudaSuccess || at.type != cudaMemoryTypeHost || !at.devicePointer) {
+      cudaGetLastError(); res = STAGED;
+    } else readable[k] = at.devicePointer;
   }
-  h->pend_host = 0;
-  if (is_device_ptr) {
-    for (int k = 0; k < n_buf; k++) dp[k] = ptrs[k];
-  } else if (zero_copy) {
-    h->zero_copy_pending = true;             // nothing to stage; the caller's buffers are read until the frame's last reader
-  } else {
-    const int b = h->in_sel; h->in_sel ^= 1;
+  if (res == STAGED) {
+    buf ^= 1;
     const auto aligned = [](size_t x) { return (x + 255) & ~(size_t)255; };
     size_t total = 0;
-    for (int k = 0; k < n_buf; k++) total += aligned(bytes[k]);
-    int rc;
-    if ((rc = grow(h, h->d_in[b], total, total / 4 + 4096, false))) return rc;
-    CK(cudaStreamWaitEvent(h->copy_stream, h->in_free[b], 0));
+    for (size_t b : bytes) total += aligned(b);
+    if (int rc = grow(h, staging[buf], total, total / 4 + 4096, false)) return rc;
+    CK(cudaStreamWaitEvent(h->copy_stream, staging_free[buf], 0));
     size_t o = 0;
-    for (int k = 0; k < n_buf; k++) {
-      if (bytes[k]) CK(cudaMemcpyAsync((char*)h->d_in[b] + o, ptrs[k], bytes[k], cudaMemcpyHostToDevice, h->copy_stream));
-      dp[k] = (char*)h->d_in[b] + o;
+    for (size_t k = 0; k < bufs.size(); k++) {
+      if (bytes[k]) CK(cudaMemcpyAsync((char*)staging[buf] + o, bufs[k], bytes[k], cudaMemcpyHostToDevice, h->copy_stream));
+      readable[k] = (char*)staging[buf] + o;
       o += aligned(bytes[k]);
     }
-    CK(cudaEventRecord(h->copy_done, h->copy_stream));
-    CK(cudaStreamWaitEvent(h->stream, h->copy_done, 0));
-    h->pend_host = 1;
+    CK(cudaEventRecord(copied, h->copy_stream));
+    CK(cudaStreamWaitEvent(h->stream, copied, 0));
+  }
+  for (size_t s = 0; kind == DEPTH && s < cams.size(); s++) {
+    const void* const* p = &readable[4 * s];
+    DepthSource& d = cams[s];
+    d.depth = (const float*)p[0]; d.conf = d.conf ? (const float*)p[1] : nullptr;
+    d.rgb = (const unsigned char*)p[2]; d.feat = (const float*)p[3];
   }
   return 0;
 }
 
-// The frame's row counts (rows of sensor s at offs[s]), sensor poses and per-row buffers; the caller has validated n
-// (every n[s] >= 0, fewer than 2^31 rows in all).
-int frame_setup(emap_handle* h, int32_t n_sensors, const int64_t* n, const float* R, const float* t, int64_t global_off,
-                float pn, float on, bool sharded) {
+// After a pass that reads the input: its staging block or the caller's page-locked memory is free from here on the stream
+int FrameInput::read_done(emap_handle* h) {
+  if (res == STAGED) CK(cudaEventRecord(staging_free[buf], h->stream));
+  else if (res == ZERO_COPY) CK(cudaEventRecord(host_free, h->stream));
+  read = true;
+  return 0;
+}
+
+// Returns once the caller may reuse its host memory: staged input once its copy has finished, zero-copy input once its
+// last reader is queued (read_done) and has run, device input at once.  No wait while the stream is captured: the
+// graph reads the caller's page-locked memory at every replay.  After one wait, the frame's later calls return at once.
+int FrameInput::wait_free(emap_handle* h) {
+  if (!held || (res == ZERO_COPY && !read)) return 0;
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  CK(cudaStreamIsCapturing(h->stream, &cs));
+  if (cs == cudaStreamCaptureStatusNone) CK(cudaEventSynchronize(res == STAGED ? copied : host_free));
+  held = false;
+  return 0;
+}
+
+// Starts a frame on the input that h->in describes: the row offsets, sensor poses and per-row buffers, then the input
+// staged, with the index pass pending.  The caller has validated the rows (every n[s] >= 0, fewer than 2^31 in all).
+int frame_start(emap_handle* h, int is_device_ptr, const float* R, const float* t, int64_t global_off, float pn,
+                float on, bool sharded) {
+  const int n_sensors = (int)h->in.n.size();
   h->sc.dirty = sharded ? nullptr : (unsigned char*)h->dirty;      // sharded frames derive the marker from the all-reduced counts
   h->fused_drift = !sharded;
   h->offs.assign(n_sensors + 1, 0);
-  for (int s = 0; s < n_sensors; s++) h->offs[s + 1] = h->offs[s] + n[s];
+  for (int s = 0; s < n_sensors; s++) h->offs[s + 1] = h->offs[s] + h->in.n[s];
   const i64 N = h->offs[n_sensors];
   h->n_points = N; h->global_off = global_off; h->pos_noise = pn; h->ori_noise = on;
   int rc;
@@ -449,12 +483,13 @@ int frame_setup(emap_handle* h, int32_t n_sensors, const int64_t* n, const float
   // zero-filled on the stream: ordered before the frame's kernels
   if ((rc = grow(h, h->ray_ctl, (size_t)RC_CTL * n_sensors, RC_CTL * 8, true))) return rc;
   h->overlap_override = false;
-  h->pend_n.assign(n, n + n_sensors);
   if (stage_mark(h, 0)) return EMAP_ERR_CUDA;
+  if ((rc = h->in.stage(h, is_device_ptr))) return rc;
+  h->progress = Progress::BEGUN;
   return 0;
 }
 
-// phase 0: upload + index/error pass for every sensor
+// A frame of point clouds: sensor s has n[s] rows of row_stride elements of dtype at points[s]
 int frame_begin(emap_handle* h, int32_t n_sensors, const void* const* points, const int64_t* n, int64_t row_stride,
                 int dtype, int is_device_ptr, const float* R, const float* t, int64_t global_off, float pn, float on,
                 bool sharded) {
@@ -467,25 +502,20 @@ int frame_begin(emap_handle* h, int32_t n_sensors, const void* const* points, co
     N += n[s];
   }
   if (global_off + N >= (1ll << 31)) return fail(h, EMAP_ERR_INVALID, "emap_input: more than 2^31 points in a frame");
-  int rc;
-  if ((rc = frame_setup(h, n_sensors, n, R, t, global_off, pn, on, sharded))) return rc;
-  std::vector<size_t> bytes(n_sensors);
-  for (int s = 0; s < n_sensors; s++) bytes[s] = (size_t)n[s] * row_stride * esz;
-  h->pend_pts.resize(n_sensors);
-  if ((rc = stage_inputs(h, n_sensors, points, bytes.data(), is_device_ptr, h->pend_pts.data()))) return rc;
-  h->pend_stride = row_stride; h->pend_dtype = dtype; h->depth_frame = false;
-  h->phase = -1;                                                   // index pass pending
-  return 0;
+  FrameInput& in = h->in;
+  in.kind = dtype == EMAP_F32 ? FrameInput::F32_ROWS : FrameInput::F64_ROWS; in.stride = row_stride;
+  in.n.assign(n, n + n_sensors); in.bufs.assign(points, points + n_sensors); in.bytes.resize(n_sensors);
+  for (int s = 0; s < n_sensors; s++) in.bytes[s] = (size_t)n[s] * row_stride * esz;
+  return frame_start(h, is_device_ptr, R, t, global_off, pn, on, sharded);
 }
 
 // index + error-count pass of every sensor (CK.py:280-345)
 int frame_index(emap_handle* h) {
   NvtxRange nv("emap:index+error");
-  if (int rc = each_cloud(h, [h](auto pts, int s) { return launch_index(h, pts, s); })) return rc;
-  if (h->pend_host) CK(cudaEventRecord(h->in_free[h->in_sel ^ 1], h->stream));
-  if (h->zero_copy_pending) CK(cudaEventRecord(h->copy_done, h->stream));      // caller's buffer is free after this point
+  if (int rc = h->in.each([h](auto pts, int s) { return launch_index(h, pts, s); })) return rc;
+  if (int rc = h->in.read_done(h)) return rc;
   if (stage_mark(h, 1)) return EMAP_ERR_CUDA;
-  h->phase = 1;
+  h->progress = Progress::INDEXED;
   return 0;
 }
 
@@ -515,7 +545,7 @@ int frame_fuse(emap_handle* h) {
     LAUNCH_CHECK();
   }
   if (stage_mark(h, 3)) return EMAP_ERR_CUDA;
-  h->phase = 2;
+  h->progress = Progress::FUSED;
   return 0;
 }
 
@@ -533,7 +563,7 @@ SemMax sem_max(emap_handle* h) {
 
 template <typename Src>
 int launch_sem_sum(emap_handle* h, const Src& src, int s) {
-  const i64 n = h->pend_n[s];
+  const i64 n = h->in.n[s];
   if (n <= 0) return 0;
   k_sem_sum<Src><<<cdiv(n, 256), 256, 0, h->stream>>>(h->dc, h->sem, src, n, (const int*)(h->pidx + h->offs[s]),
                                                        h->sem_fsum, h->sem_csum, sem_max(h));
@@ -544,7 +574,7 @@ int launch_sem_sum(emap_handle* h, const Src& src, int s) {
 // class_max before the scatter: U and the records per cell over every cloud (id_max read once, with the first cloud)
 template <typename Src>
 int launch_cm_count(emap_handle* h, const Src& src, int s) {
-  const i64 n = h->pend_n[s], n_idm = s == 0 ? (i64)h->sem.n_id_max * h->dc.C : 0;
+  const i64 n = h->in.n[s], n_idm = s == 0 ? (i64)h->sem.n_id_max * h->dc.C : 0;
   const i64 work = std::max(n, n_idm);
   if (work <= 0) return 0;
   const int grid = (int)std::min<i64>(cdiv(work, 256), (i64)h->n_sm * 4);
@@ -566,15 +596,13 @@ int frame_semantic(emap_handle* h) {
         (rc = grow(h, h->cm_sum, slots, slots / 4 + 1024, true)))
       return rc;
     CK(cudaMemsetAsync(h->cm_ctl, 0, sizeof(u32) * (CM_CTL + (1 + n_max) * CM_WORDS), h->stream));
-    if ((rc = each_cloud(h, [h](auto pts, int s) { return launch_cm_count(h, pts, s); }))) return rc;
+    if ((rc = h->in.each([h](auto pts, int s) { return launch_cm_count(h, pts, s); }))) return rc;
     PER_CELL(k_cm_alloc, h->dc.C, sem_max(h));
     k_cm_ulist<<<1, 1024, 0, h->stream>>>(sem_max(h));
     LAUNCH_CHECK();
   }
-  if (int rc = each_cloud(h, [h](auto pts, int s) { return launch_sem_sum(h, pts, s); })) return rc;
-  // the cloud (staging buffer or the caller's pinned memory) is free only now
-  if (h->pend_host) CK(cudaEventRecord(h->in_free[h->in_sel ^ 1], h->stream));
-  if (h->zero_copy_pending) CK(cudaEventRecord(h->copy_done, h->stream));
+  if (int rc = h->in.each([h](auto pts, int s) { return launch_sem_sum(h, pts, s); })) return rc;
+  if (int rc = h->in.read_done(h)) return rc;      // the input is free only now
   if (n_max > 0) {
     // occupied cells: at most one per valid + inside point
     const int grid = std::max(1, cdiv(std::min<i64>(h->dc.C, h->n_points), 256));
@@ -628,7 +656,7 @@ int frame_rays(emap_handle* h) {
   } else if (stage_mark(h, 4)) return EMAP_ERR_CUDA;
   if (deferred) CK(cudaStreamWaitEvent(h->stream, h->ev_join, 0));   // before the cross-rank barrier that follows this phase
   if (stage_mark(h, 5)) return EMAP_ERR_CUDA;
-  h->phase = 3;
+  h->progress = Progress::RAYS_CAST;
   return 0;
 }
 
@@ -686,7 +714,7 @@ int frame_finish(emap_handle* h) {
   if (rc) return rc;
   if (stage_mark(h, 7)) return EMAP_ERR_CUDA;
   h->st.have = h->timing != 0;
-  h->phase = 0;
+  h->progress = Progress::IDLE;
   return 0;
 }
 
@@ -762,14 +790,14 @@ int exchange_list(emap_handle* h, int phase, emap_exchange out[3], int32_t* n_ou
     out[1] = {h->sc.n_ray, C, 3};
     out[2] = {h->ukey_x, C, 2};
     *n_out = 3;
-    h->phase = 4;
+    h->progress = Progress::KEYS_EXCHANGED;
   } else *n_out = 0;
   return 0;
 }
 
 // last phase of a sharded frame: the reduced upper-bound keys back to u32 (if phase 3 exchanged them), then finalize
 int shard_finish(emap_handle* h) {
-  if (h->phase == 4) {
+  if (h->progress == Progress::KEYS_EXCHANGED) {
     k_ukey_merge<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc.C, h->sc.ukv, h->ukey_x);
     LAUNCH_CHECK();
   }
@@ -1040,11 +1068,10 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   for (Stream* s : {&h->own_stream, &h->copy_stream, &h->side_stream})
     if ((e = s->create(cudaStreamNonBlocking)) != cudaSuccess) return bail("stream", e);
   h->stream = h->own_stream;
-  for (Event* ev : {&h->in_free[0], &h->in_free[1], &h->copy_done, &h->ev_fork, &h->ev_join, &h->ev_order,
-                    &h->img_up.staged, &h->init_up.staged})
+  for (Event* ev : {&h->in.staging_free[0], &h->in.staging_free[1], &h->in.copied, &h->in.host_free, &h->ev_fork,
+                    &h->ev_join, &h->ev_order, &h->img_up.staged, &h->init_up.staged})
     if ((e = ev->create(cudaEventDisableTiming)) != cudaSuccess) return bail("event", e);
   for (Event& ev : h->st.ev) if ((e = ev.create(cudaEventDefault)) != cudaSuccess) return bail("event", e);
-  for (int b = 0; b < 2; b++) if ((e = cudaEventRecord(h->in_free[b], h->stream)) != cudaSuccess) return bail("event", e);
 #define ALLOC(buf, n) if ((e = (buf).alloc(n)) != cudaSuccess) return bail("cudaMalloc", e)
 #define TRY(call) if ((e = (call)) != cudaSuccess) return bail(#call, e)
   ALLOC(h->map, 7 * C);
@@ -1143,23 +1170,13 @@ int initialize_finish(emap_handle* h, int32_t dilation_size, int32_t iterations)
   return EMAP_OK;
 }
 
-// The frame after its inputs are in place (frame_begin or the depth-image set-up): every pass, then, for host inputs, the
-// wait after which the caller may reuse them
-int frame_run(emap_handle* h, int is_device_ptr) {
+// The frame after frame_start: every pass, then the wait after which the caller may reuse its host memory
+int frame_run(emap_handle* h) {
   int rc;
-  if ((rc = frame_index(h))) return rc;
-  if ((rc = frame_fuse(h))) return rc;
-  if ((rc = frame_semantic(h))) return rc;
-  if ((rc = frame_rays(h))) return rc;
-  if ((rc = frame_finish(h))) return rc;
-  if (!is_device_ptr || h->zero_copy_pending) {      // caller may reuse its host buffers on return
-    // a captured frame runs nothing yet: it reads the caller's pinned cloud at every replay instead
-    cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-    CK(cudaStreamIsCapturing(h->stream, &cs));
-    if (cs == cudaStreamCaptureStatusNone) CK(cudaEventSynchronize(h->copy_done));
-  }
-  h->zero_copy_pending = false;
-  return EMAP_OK;
+  if ((rc = frame_index(h)) || (rc = frame_fuse(h)) || (rc = frame_semantic(h)) || (rc = frame_rays(h)) ||
+      (rc = frame_finish(h)))
+    return rc;
+  return h->in.wait_free(h);
 }
 
 extern "C" {
@@ -1189,7 +1206,7 @@ int emap_input_sensors(emap_handle* h, int32_t n_sensors, const void* const* poi
   if (!points || !n || !R || !t) return fail(h, EMAP_ERR_INVALID, "emap_input: null argument");
   if (h->attached) return fail(h, EMAP_ERR_STATE, "handle is attached to a sharded scratch: use the emap_shard_* calls");
   const int rc = frame_begin(h, n_sensors, points, n, row_stride, dtype, is_device_ptr, R, t, 0, pn, on, false);
-  return rc ? rc : frame_run(h, is_device_ptr);
+  return rc ? rc : frame_run(h);
 }
 
 int emap_input_pointcloud(emap_handle* h, const void* points, int64_t n, int64_t row_stride, int dtype, int is_device_ptr,
@@ -1238,38 +1255,25 @@ int emap_input_depth_images(emap_handle* h, int32_t n_cameras, const emap_depth_
     memcpy(R + 9 * s, c.R, sizeof(c.R));
     memcpy(t + 3 * s, c.t, sizeof(c.t));
   }
-  int rc;
-  if ((rc = frame_setup(h, n_cameras, n, R, t, 0, pn, on, false))) return rc;
   // per camera: depth, confidence, rgb, feature planes (the ones the channels read)
-  const void* ptrs[4 * EMAP_DEPTH_MAX_CAMERAS];
-  const void* dp[4 * EMAP_DEPTH_MAX_CAMERAS];
-  size_t bytes[4 * EMAP_DEPTH_MAX_CAMERAS];
+  FrameInput& in = h->in;
+  in.kind = FrameInput::DEPTH; in.n.assign(n, n + n_cameras);
+  in.bufs.resize(4 * n_cameras); in.bytes.resize(4 * n_cameras); in.cams.assign(n_cameras, DepthSource{});
   for (int s = 0; s < n_cameras; s++) {
     const emap_depth_camera& c = cams[s];
     const size_t P = (size_t)n[s];
-    ptrs[4 * s] = c.depth; bytes[4 * s] = 4 * P;
-    ptrs[4 * s + 1] = c.confidence; bytes[4 * s + 1] = c.confidence ? 4 * P : 0;
-    ptrs[4 * s + 2] = c.rgb; bytes[4 * s + 2] = n_color ? 3 * P : 0;
-    ptrs[4 * s + 3] = c.features; bytes[4 * s + 3] = n_feat_used ? 4 * P * n_features : 0;
-  }
-  if ((rc = stage_inputs(h, 4 * n_cameras, ptrs, bytes, is_device_ptr, dp))) return rc;
-  h->pend_cams.resize(n_cameras);
-  for (int s = 0; s < n_cameras; s++) {
-    const emap_depth_camera& c = cams[s];
-    DepthSource& d = h->pend_cams[s];
-    memset(&d, 0, sizeof(d));
-    d.depth = (const float*)dp[4 * s];
-    d.conf = c.confidence ? (const float*)dp[4 * s + 1] : nullptr;
-    d.rgb = (const unsigned char*)dp[4 * s + 2];
-    d.feat = (const float*)dp[4 * s + 3];
-    d.plane = n[s]; d.width = c.width;
+    in.bufs[4 * s] = c.depth; in.bytes[4 * s] = 4 * P;
+    in.bufs[4 * s + 1] = c.confidence; in.bytes[4 * s + 1] = c.confidence ? 4 * P : 0;
+    in.bufs[4 * s + 2] = c.rgb; in.bytes[4 * s + 2] = n_color ? 3 * P : 0;
+    in.bufs[4 * s + 3] = c.features; in.bytes[4 * s + 3] = n_feat_used ? 4 * P * n_features : 0;
+    DepthSource& d = in.cams[s];
+    d.conf = c.confidence; d.plane = n[s]; d.width = c.width;
     d.conf_min = confidence_threshold; d.max_depth = max_depth;
     d.fx = c.fx; d.fy = c.fy; d.cx = c.cx; d.cy = c.cy;
     for (int j = 0; j < n_channels; j++) d.src[j / 8] |= (u64)(channel_source[j] + 1) << (8 * (j % 8));
   }
-  h->depth_frame = true;
-  h->phase = -1;                                                   // index pass pending
-  return frame_run(h, is_device_ptr);
+  const int rc = frame_start(h, is_device_ptr, R, t, 0, pn, on, false);
+  return rc ? rc : frame_run(h);
 }
 
 int emap_input_depth_image(emap_handle* h, const emap_depth_camera* camera, int is_device_ptr, int32_t n_channels,
@@ -1352,14 +1356,11 @@ int emap_shard_begin(emap_handle* h, int32_t n_sensors, const void* const* point
   ENTER(h);
   if (!points || !n || !R || !t) return fail(h, EMAP_ERR_INVALID, "emap_shard_begin: null argument");
   int rc = frame_begin(h, n_sensors, points, n, row_stride, dtype, is_device_ptr, R, t, global_point_offset, pn, on, true);
-  if (rc) return rc;
-  if (!is_device_ptr && !h->zero_copy_pending) CK(cudaEventSynchronize(h->copy_done));   // staged copy done: host buffers reusable
+  if (rc || (rc = h->in.wait_free(h))) return rc;
   // multicast mode: every rank must have reset its frame scalars before anyone pushes -> the caller runs a
   // cross-rank barrier and then emap_shard_phase(h, 0); NCCL mode: index right away
   if (h->attached) return 0;
-  rc = frame_index(h);
-  if (!rc && h->zero_copy_pending) { CK(cudaEventSynchronize(h->copy_done)); h->zero_copy_pending = false; }
-  return rc;
+  return (rc = frame_index(h)) ? rc : h->in.wait_free(h);
 }
 
 int64_t emap_shard_scratch_bytes(const emap_handle* h) {
@@ -1386,7 +1387,8 @@ int emap_shard_attach(emap_handle* h, void* local_base, void* multicast_base, in
 
 int emap_shard_set_overlap_z(emap_handle* h, float z_abs) {
   ENTER(h);
-  if (h->phase != 1 && h->phase != -1) return fail(h, EMAP_ERR_STATE, "emap_shard_set_overlap_z must follow emap_shard_begin");
+  if (h->progress != Progress::BEGUN && h->progress != Progress::INDEXED)
+    return fail(h, EMAP_ERR_STATE, "emap_shard_set_overlap_z must follow emap_shard_begin");
   h->overlap_override = true; h->overlap_z_override = z_abs - h->center[2];     // consumed by k_drift (phase 1)
   return EMAP_OK;
 }
@@ -1397,28 +1399,28 @@ int emap_shard_exchange(emap_handle* h, int32_t phase, emap_exchange* out, int32
   if (phase < 1 || phase > 3) return fail(h, EMAP_ERR_INVALID, "emap_shard_exchange: phase must be 1..3");
   static const char* order[] = {"", "exchange 1 must follow emap_shard_begin", "exchange 2 must follow phase 1",
                                 "exchange 3 must follow phase 2"};
-  if (h->phase != phase) return fail(h, EMAP_ERR_STATE, order[phase]);
+  static const Progress after[] = {Progress::IDLE, Progress::INDEXED, Progress::FUSED, Progress::RAYS_CAST};
+  if (h->progress != after[phase]) return fail(h, EMAP_ERR_STATE, order[phase]);
   return exchange_list(h, phase, out, n_out);
 }
 
 int emap_shard_phase(emap_handle* h, int32_t phase) {
   ENTER(h);
   if (phase == 0) {
-    if (h->phase != -1) return fail(h, EMAP_ERR_STATE, "phase 0 must follow emap_shard_begin on an attached handle");
-    int rc0 = frame_index(h);
-    if (!rc0 && h->zero_copy_pending) { CK(cudaEventSynchronize(h->copy_done)); h->zero_copy_pending = false; }
-    return rc0;
+    if (h->progress != Progress::BEGUN) return fail(h, EMAP_ERR_STATE, "phase 0 must follow emap_shard_begin on an attached handle");
+    const int rc = frame_index(h);
+    return rc ? rc : h->in.wait_free(h);
   }
   if (phase == 1) {
-    if (h->phase != 1) return fail(h, EMAP_ERR_STATE, "phase 1 must follow emap_shard_begin");
+    if (h->progress != Progress::INDEXED) return fail(h, EMAP_ERR_STATE, "phase 1 must follow emap_shard_begin");
     return frame_fuse(h);
   }
   if (phase == 2) {
-    if (h->phase != 2) return fail(h, EMAP_ERR_STATE, "phase 2 must follow phase 1");
+    if (h->progress != Progress::FUSED) return fail(h, EMAP_ERR_STATE, "phase 2 must follow phase 1");
     return frame_rays(h);
   }
   if (phase == 3) {
-    if (h->phase != 3 && h->phase != 4) return fail(h, EMAP_ERR_STATE, "phase 3 must follow phase 2");
+    if (h->progress != Progress::RAYS_CAST && h->progress != Progress::KEYS_EXCHANGED) return fail(h, EMAP_ERR_STATE, "phase 3 must follow phase 2");
     return shard_finish(h);
   }
   return fail(h, EMAP_ERR_INVALID, "emap_shard_phase: phase must be 0..3");
@@ -1503,10 +1505,7 @@ int emap_input_sensors_sharded(emap_handle* h, int32_t n_sensors, const void* co
   if (h->attached) return fail(h, EMAP_ERR_STATE, "handle is attached to a multicast scratch: use the emap_shard_* calls");
   if (!points || !n || !R || !t) return fail(h, EMAP_ERR_INVALID, "emap_input_sensors_sharded: null argument");
   int rc = frame_begin(h, n_sensors, points, n, row_stride, dtype, is_device_ptr, R, t, global_point_offset, pn, on, true);
-  if (rc) return rc;
-  if (!is_device_ptr && !h->zero_copy_pending) CK(cudaEventSynchronize(h->copy_done));
-  if ((rc = frame_index(h))) return rc;
-  if (h->zero_copy_pending) { CK(cudaEventSynchronize(h->copy_done)); h->zero_copy_pending = false; }
+  if (rc || (rc = h->in.wait_free(h)) || (rc = frame_index(h)) || (rc = h->in.wait_free(h))) return rc;
   h->overlap_override = true; h->overlap_z_override = overlap_sensor_z_absolute - h->center[2];
   if ((rc = comm_exchange(h, 1))) return rc;
   if ((rc = frame_fuse(h))) return rc;
@@ -1540,7 +1539,7 @@ int emap_get_frame_stats(emap_handle* h, emap_frame_stats* out) {
   CK(cudaStreamSynchronize(h->stream));
   out->mean_error = f.mean_error; out->additive_mean_error = f.additive_mean_error; out->shift_applied = f.shift;
   out->error_sum = f.error_sum; out->error_cnt = f.ecnt_last; out->drift_applied = f.applied; out->drift_evaluated = f.evaluated;
-  out->n_points = h->depth_frame ? f.nkept_last : h->n_points; out->n_valid_points = f.nvalid_last; out->ray_steps = f.ray_steps; out->ray_visits = f.ray_visits;
+  out->n_points = h->in.kind == FrameInput::DEPTH ? f.nkept_last : h->n_points; out->n_valid_points = f.nvalid_last; out->ray_steps = f.ray_steps; out->ray_visits = f.ray_visits;
   return EMAP_OK;
 }
 

@@ -79,6 +79,34 @@ def _device_pointer(x):
     return int(cai["data"][0]), int(n), int(row), (_lib.EMAP_F32 if esz == 4 else _lib.EMAP_F64), x
 
 
+def _cloud(x, device):
+    """(ptr, n_rows, row_stride, dtype_code, keepalive) of one point cloud: a device array read in place (device=True),
+    or a host array (a device array is copied there), float32 unless float64, C-contiguous."""
+    if device:
+        dev = _device_pointer(x)
+        if dev is None:
+            raise ValueError("device_ptrs=True needs every point cloud in device memory")
+        return dev
+    a = _to_host(x)
+    if a.dtype not in (np.float32, np.float64):
+        a = a.astype(np.float32)
+    if a.ndim != 2 or a.shape[1] < 3:
+        raise ValueError("raw_points must be (N, >=3)")
+    if not a.flags.c_contiguous:
+        a = np.ascontiguousarray(a)
+    return a.ctypes.data, a.shape[0], a.shape[1], (_lib.EMAP_F32 if a.dtype == np.float32 else _lib.EMAP_F64), a
+
+
+def _clouds(clouds, device):
+    """(ptrs, counts, row_stride, dtype_code, keepalive) of one frame's clouds (_cloud each), which must share row stride
+    and dtype"""
+    cs = [_cloud(c, device) for c in clouds]
+    if len({c[2:4] for c in cs}) > 1:
+        raise ValueError("all sensor clouds must share row stride and dtype")
+    stride, dt = cs[0][2:4] if cs else (None, None)
+    return (C.c_void_p * len(cs))(*[c[0] for c in cs]), (C.c_int64 * len(cs))(*[c[1] for c in cs]), stride, dt, cs
+
+
 class ElevationMap:
     """Core elevation mapping class (EM.py:49)."""
 
@@ -262,57 +290,26 @@ class ElevationMap:
         Rm = np.ascontiguousarray(_to_host(R), dtype=np.float32).reshape(9)
         tv = np.ascontiguousarray(_to_host(t), dtype=np.float32).reshape(3)
         dev = _device_pointer(raw_points)
+        ptr, n, row, dt, _keep = dev if dev is not None else _cloud(raw_points, False)
         with self.map_lock:
-            if dev is not None:
-                ptr, n, row, dt, _keep = dev
-                self._after_framework()
-                rc = self._L.emap_input_pointcloud(self._h, ptr, n, row, dt, 1, Rm.ctypes.data, tv.ctypes.data,
-                                                   float(position_noise), float(orientation_noise))
-            else:
-                pts = _to_host(raw_points)
-                if pts.dtype not in (np.float32, np.float64):
-                    pts = pts.astype(np.float32)
-                if pts.ndim != 2 or pts.shape[1] < 3:
-                    raise ValueError("raw_points must be (N, >=3)")
-                if not pts.flags.c_contiguous:
-                    pts = np.ascontiguousarray(pts)
-                dt = _lib.EMAP_F32 if pts.dtype == np.float32 else _lib.EMAP_F64
-                self._after_framework()       # framework kernels still reading the aliased layers finish first
-                rc = self._L.emap_input_pointcloud(self._h, pts.ctypes.data, pts.shape[0], pts.shape[1], dt, 0,
-                                                   Rm.ctypes.data, tv.ctypes.data, float(position_noise),
-                                                   float(orientation_noise))
-            self._check(rc)
+            self._after_framework()       # framework work writing the cloud or reading the aliased layers comes first
+            self._check(self._L.emap_input_pointcloud(self._h, ptr, n, row, dt, int(dev is not None), Rm.ctypes.data,
+                                                      tv.ctypes.data, float(position_noise), float(orientation_noise)))
 
     # the pure-Python ROS node of the reference still calls `.input(...)` (elevation_mapping_ros.py:212)
     input = input_pointcloud
 
     def input_sensors(self, clouds, Rs, ts, position_noise, orientation_noise, device_ptrs=False):
-        """Several sensors of one time slice fused against the same snapshot (SURVEY 8(e))."""
-        ns = len(clouds)
-        keep, ptrs, counts = [], (C.c_void_p * ns)(), (C.c_int64 * ns)()
-        stride = dt = None
-        for i, c in enumerate(clouds):
-            dev = _device_pointer(c) if device_ptrs else None
-            if dev is not None:
-                ptr, n, row, d, k = dev
-            else:
-                a = np.ascontiguousarray(_to_host(c))
-                if a.dtype not in (np.float32, np.float64):
-                    a = a.astype(np.float32)
-                ptr, n, row, d, k = a.ctypes.data, a.shape[0], a.shape[1], (_lib.EMAP_F32 if a.dtype == np.float32 else _lib.EMAP_F64), a
-            if stride is None:
-                stride, dt = row, d
-            elif (stride, dt) != (row, d):
-                raise ValueError("all sensor clouds must share row stride and dtype")
-            keep.append(k); ptrs[i] = ptr; counts[i] = n
+        """Several sensors of one time slice fused against the same snapshot (SURVEY 8(e)).  device_ptrs=True: every
+        cloud is a device array, read in place; otherwise every cloud is read from the host."""
+        ptrs, counts, stride, dt, _keep = _clouds(clouds, device_ptrs)
         Rm = np.ascontiguousarray(np.stack([np.asarray(_to_host(r), np.float32).reshape(9) for r in Rs]))
         tm = np.ascontiguousarray(np.stack([np.asarray(_to_host(t), np.float32).reshape(3) for t in ts]))
-        if device_ptrs:
-            self._after_framework()
         with self.map_lock:
-            self._check(self._L.emap_input_sensors(self._h, ns, ptrs, counts, stride, dt, int(bool(device_ptrs)),
-                                                   Rm.ctypes.data, tm.ctypes.data, float(position_noise),
-                                                   float(orientation_noise)))
+            self._after_framework()       # framework work writing the clouds or reading the aliased layers comes first
+            self._check(self._L.emap_input_sensors(self._h, len(counts), ptrs, counts, stride, dt,
+                                                   int(bool(device_ptrs)), Rm.ctypes.data, tm.ctypes.data,
+                                                   float(position_noise), float(orientation_noise)))
 
     def input_depth_image(self, depth, P, R, t, position_noise: float, orientation_noise: float, channels=(), rgb=None,
                           features=None, confidence=None, confidence_threshold: float = 10.0, max_depth: float = 8.0):

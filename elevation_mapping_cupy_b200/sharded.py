@@ -146,24 +146,9 @@ class ShardedElevationMap:
     def input_sensors(self, clouds, Rs, ts, position_noise, orientation_noise, device_ptrs=False, overlap_z=None):
         """`overlap_z`: absolute z of the frame's first sensor (rank 0's), the same value on every rank."""
         em = self.em
-        ns = len(clouds)
-        keep, ptrs, counts = [], (C.c_void_p * ns)(), (C.c_int64 * ns)()
-        stride = dt = None
-        from .elevation_mapping import _device_pointer, _to_host
-        for i, c in enumerate(clouds):
-            dev = _device_pointer(c) if device_ptrs else None
-            if dev is not None:
-                ptr, n, row, d, k = dev
-            else:
-                a = np.ascontiguousarray(_to_host(c))
-                if a.dtype not in (np.float32, np.float64):
-                    a = a.astype(np.float32)
-                ptr, n, row, d, k = a.ctypes.data, a.shape[0], a.shape[1], (_lib.EMAP_F32 if a.dtype == np.float32 else _lib.EMAP_F64), a
-            if stride is None:
-                stride, dt = row, d
-            elif (row, d) != (stride, dt):           # same check as ElevationMap.input_sensors
-                raise ValueError("all clouds of one frame must share dtype and column count")
-            keep.append(k); ptrs[i] = ptr; counts[i] = n
+        from .elevation_mapping import _clouds, _to_host
+        ptrs, counts, stride, dt, _keep = _clouds(clouds, device_ptrs)
+        ns = len(counts)
         total_local = sum(int(c) for c in counts)
         off, _total = self.static_offsets if self.static_offsets else global_point_offsets(total_local, self.group)
         Rm = np.ascontiguousarray(np.stack([np.asarray(_to_host(r), np.float32).reshape(9) for r in Rs]))

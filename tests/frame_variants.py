@@ -119,7 +119,7 @@ LAYOUTS = ["f32-host", "f32x4-device", "f32x4-device-unaligned", "f32-pinned", "
 
 def layout_path(layout):
     """(where the index pass reads the rows, whether it takes the 16-byte vector load) of a layout:
-    frame_begin / stage_inputs (staged copy, zero-copy, device) and load_point<float> (emap_sources.cuh)"""
+    FrameInput::stage (staged copy, zero-copy, device; emap_api.cu) and load_point<float> (emap_sources.cuh)"""
     where = {"f32-host": "staged", "f32-pinned": "zero-copy", "f64-pinned": "zero-copy"}.get(layout, "device")
     return where, layout == "f32x4-device"
 

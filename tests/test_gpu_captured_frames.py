@@ -298,11 +298,12 @@ def test_semantic_channels_in_a_captured_frame():
 
 
 # ---- E: eager frames and ticks on a caller stream, without host syncs -----------------------------------------------
-def test_eager_frames_and_edits_on_a_caller_stream(oracle_mod):
+def _eager_frames_and_edits_on_a_caller_stream(oracle_mod, frame):
     """the handle on its own stream, torch on a side stream.  Before each frame the side stream sleeps and then edits the
-    aliased state (a block of variance, a block of cleared is_valid); then input_pointcloud, move_to and update_time.
-    After the last call a layer is cloned on the side stream before any synchronisation.  A library call that overtook
-    the edits, or a clone that read the view before the frame finished, gives a state other than the oracle's."""
+    aliased state (a block of variance, a block of cleared is_valid); then frame(em, host cloud, device cloud, R, t),
+    move_to and update_time.  After the last call a layer is cloned on the side stream before any synchronisation.  A
+    library call that overtook the edits, or a clone that read the view before the frame finished, gives a state other
+    than the oracle's."""
     import torch
     from elevation_mapping_cupy_b200 import workloads as wl
     from elevation_mapping_cupy_b200.parameter import core_parameter
@@ -322,7 +323,7 @@ def test_eager_frames_and_edits_on_a_caller_stream(oracle_mod):
             om.elevation_map[1, r0:r0 + 40, 60:150] = 0.25
             om.elevation_map[2, 120:170, r0:r0 + 50] = 0.0
             move = np.asarray(t, np.float64) + [0.33, -0.21, 0.05]
-            em.input_pointcloud(src[f], XYZ, R, t, 0.02, 0.02); em.move_to(move, R); em.update_time()
+            frame(em, pts, src[f], R, t); em.move_to(move, R); em.update_time()
             for m in (om, unedited):
                 m.input_pointcloud(pts, XYZ, R, t, 0.02, 0.02); m.move_to(move, R); m.update_time()
         elevation = em.get_layer("elevation").clone()
@@ -333,3 +334,15 @@ def test_eager_frames_and_edits_on_a_caller_stream(oracle_mod):
     changed = [int((om.elevation_map[li] != unedited.elevation_map[li]).sum()) for li in (0, 1, 2)]
     assert changed[0] > 100 and changed[1] > 100 and changed[2] > 0, changed     # the edits matter to the frames
     check_frame(em, om, len(frames[-1][0]), "side stream")
+
+
+def test_eager_frames_and_edits_on_a_caller_stream(oracle_mod):
+    """E with input_pointcloud of device clouds"""
+    _eager_frames_and_edits_on_a_caller_stream(
+        oracle_mod, lambda em, pts, dev, R, t: em.input_pointcloud(dev, XYZ, R, t, 0.02, 0.02))
+
+
+def test_eager_host_sensor_frames_and_edits_on_a_caller_stream(oracle_mod):
+    """E with input_sensors of host clouds: the staged frame too runs after the caller's queued edits"""
+    _eager_frames_and_edits_on_a_caller_stream(
+        oracle_mod, lambda em, pts, dev, R, t: em.input_sensors([pts], [R], [t], 0.02, 0.02))
