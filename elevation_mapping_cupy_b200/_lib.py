@@ -96,6 +96,11 @@ SIGNATURES = {
     "emap_submap_windows": (C.c_int, [C.c_int32, C.c_double, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "emap_get_submaps": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_void_p),
                                    C.POINTER(C.c_int32), C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
+    "emap_transformed_submap_windows": (C.c_int, [C.c_int32, C.c_double, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
+                                                  C.c_void_p, C.c_void_p]),
+    "emap_get_transformed_submaps": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_double, C.c_int32,
+                                               C.POINTER(C.c_char_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int32),
+                                               C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
     "emap_get_map_points": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_get_normal_arrows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_layer_device_ptr": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),

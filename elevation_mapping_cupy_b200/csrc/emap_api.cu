@@ -188,6 +188,9 @@ struct emap_handle {
   bool attached = false;
   // export staging
   DevBuf<float> d_export;
+  // emap_get_transformed_submaps' per-cell keys (grown to the largest call, zero between calls: k_tsub_gather resets)
+  DevBuf<u32> ts_key1;
+  DevBuf<u64> ts_key2;
   // plugin scratch
   DevBuf<float> pl[4];
   DevBuf<int> pl_cnt;
@@ -1820,6 +1823,126 @@ int emap_get_submaps(emap_handle* h, int32_t n_windows, const double* windows, i
   LAUNCH_CHECK();
   if (!out_is_device) {
     CK(cudaMemcpyAsync(out, dst, sizeof(float) * total, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+  }
+  return EMAP_OK;
+}
+
+static_assert(EMAP_TRANSFORM_TOLERANCE == TSUB_ORTHO_TOL && EMAP_TRANSFORMED_WINDOWS_PER_LAUNCH == TSUB_MAX_WINDOWS,
+              "emap.h states the transformed windows' limits");
+
+static bool transforms_ok(int64_t n, const double* transforms) {
+  for (int64_t w = 0; w < n; w++)
+    if (!tsub_transform_ok(transforms + 12 * w)) return false;
+  return true;
+}
+
+// The host part of emap_get_transformed_submaps on its own (no handle, no device): transformed_window for every request.
+int emap_transformed_submap_windows(int32_t cell_n, double resolution, const double center[2], int32_t n_windows,
+                                    const double* windows, const double* transforms, int32_t* info, double* geometry) {
+  if (!center || !windows || !transforms || !info || !geometry || cell_n < 3 ||
+      !(std::isfinite(resolution) && resolution > 0.0) || n_windows < 0 || !submap_lengths_ok(n_windows, windows) ||
+      !transforms_ok(n_windows, transforms))
+    return EMAP_ERR_INVALID;
+  for (int32_t w = 0; w < n_windows; w++) {
+    TSubGeom g;
+    transformed_window(cell_n, resolution, center, windows + 4 * w, transforms + 12 * w, g);
+    info[3 * w] = g.win[0]; info[3 * w + 1] = g.size[0]; info[3 * w + 2] = g.size[1];
+    for (int a = 0; a < 2; a++) { geometry[4 * w + a] = g.pos[a]; geometry[4 * w + 2 + a] = g.len[a]; }
+  }
+  return EMAP_OK;
+}
+
+// get_raw_submap with a request frame other than the map frame (elevation_mapping_ros.cpp:507-553 with grid_map's
+// getTransformedMap): the geometry on the host (transformed_window), then per launch of up to TSUB_MAX_WINDOWS windows
+// the two scatter passes and the gather (csrc/emap_submap.cuh), each launch's table in its parameters.  Output, stream
+// and graph rules as emap_get_submaps; every check runs before anything is written or launched.
+int emap_get_transformed_submaps(emap_handle* h, int32_t n_windows, const double* windows, const double* transforms,
+                                 double sample_ratio, int32_t n_layers, const char* const* names,
+                                 const float* const* planes_device, const int32_t* flags, float* out,
+                                 int32_t out_is_device, int64_t out_floats, int32_t* info, double* geometry) {
+  ENTER(h);
+  NvtxRange nv("emap:get_transformed_submaps");
+  if (!windows || !transforms || !names || !out || !info || !geometry)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: null argument");
+  if (n_windows < 1 || n_windows > EMAP_SUBMAP_MAX_WINDOWS)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: 1 to EMAP_SUBMAP_MAX_WINDOWS windows required");
+  if (n_layers < 1 || n_layers > EMAP_SUBMAP_MAX_LAYERS)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: 1 to EMAP_SUBMAP_MAX_LAYERS layers required");
+  if (!submap_lengths_ok(n_windows, windows))
+    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: lengths must be finite and >= 0");
+  if (!transforms_ok(n_windows, transforms))
+    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: a transform is not finite or its R is not "
+                                     "orthonormal within EMAP_TRANSFORM_TOLERANCE");
+  if (!(std::isfinite(sample_ratio) && sample_ratio >= 0.0))
+    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: sample_ratio must be finite and >= 0");
+  ExportList L;
+  if (!export_list(h, n_layers, names, planes_device, flags, L)) return EMAP_ERR_INVALID;
+  const int W = h->dc.W;
+  const double res = h->cfg.resolution;
+  const double m[2] = {h->center[0], h->center[1]};
+  std::vector<TSubGeom> g(n_windows);
+  long long cells = 0;
+  for (int w = 0; w < n_windows; w++) {
+    transformed_window(W, res, m, windows + 4 * w, transforms + 12 * w, g[w]);
+    const long long n = (long long)g[w].size[0] * g[w].size[1];
+    if (n > INT32_MAX - TSUB_THREADS)
+      return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: a new map of 2^31 cells or more");
+    cells += n;
+  }
+  if (n_layers * cells > out_floats)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: out_floats is below the layers times the new maps' cells");
+  for (int w = 0; w < n_windows; w++) {
+    info[3 * w] = g[w].win[0]; info[3 * w + 1] = g[w].size[0]; info[3 * w + 2] = g[w].size[1];
+    for (int a = 0; a < 2; a++) { geometry[4 * w + a] = g[w].pos[a]; geometry[4 * w + 2 + a] = g[w].len[a]; }
+  }
+  if (!cells) return EMAP_OK;
+  int rc;
+  if ((rc = grow(h, h->ts_key1, (size_t)cells, 0, true)) || (rc = grow(h, h->ts_key2, (size_t)cells, 0, true))) return rc;
+  float* dst = out;
+  if (!out_is_device) {
+    if ((rc = grow(h, h->d_export, (size_t)(n_layers * cells), 0, false))) return rc;
+    dst = h->d_export;
+  }
+  const bool colour = export_has_colour(L);
+  TSubArgs a;
+  a.L = L;
+  a.n_samples = sample_ratio > 0.0 ? 5 : 1;
+  a.res = res;
+  a.s = res * sample_ratio;
+  long long cell0 = 0;
+  for (int w0 = 0; w0 < n_windows;) {
+    a.n_win = 0;
+    int blk_src = 0, blk_dst = 0;
+    for (; w0 < n_windows && a.n_win < TSUB_MAX_WINDOWS; w0++) {
+      const TSubGeom& q = g[w0];
+      if (!q.win[0] || !q.size[0] || !q.size[1]) continue;
+      TSubWin& s = a.win[a.n_win++];
+      for (int k = 0; k < 9; k++) s.R[k] = transforms[12 * w0 + k];
+      for (int k = 0; k < 3; k++) s.t[k] = transforms[12 * w0 + 9 + k];
+      s.x0 = q.centre[0] + (0.5 * (q.win[3] * res) - 0.5 * res);
+      s.y0 = q.centre[1] + (0.5 * (q.win[4] * res) - 0.5 * res);
+      for (int k = 0; k < 2; k++) { s.pos[k] = q.pos[k]; s.len[k] = q.len[k]; }
+      s.r0 = (int16_t)(W - 2 - q.win[1]); s.c0 = (int16_t)(W - 2 - q.win[2]);
+      s.rows = (int16_t)q.win[3]; s.cols = (int16_t)q.win[4];
+      s.nrows = q.size[0]; s.ncols = q.size[1];
+      s.blk_src = blk_src; s.blk_dst = blk_dst; s.cell0 = cell0;
+      blk_src += cdiv((i64)q.win[3] * q.win[4], TSUB_THREADS);
+      blk_dst += cdiv((i64)q.size[0] * q.size[1], TSUB_THREADS);
+      cell0 += (long long)q.size[0] * q.size[1];
+    }
+    if (!a.n_win) continue;
+    k_tsub_scatter<1><<<blk_src, TSUB_THREADS, 0, h->stream>>>(h->dc, h->map, h->ts_key1, h->ts_key2, a, h->center[2]);
+    LAUNCH_CHECK();
+    k_tsub_scatter<2><<<blk_src, TSUB_THREADS, 0, h->stream>>>(h->dc, h->map, h->ts_key1, h->ts_key2, a, h->center[2]);
+    LAUNCH_CHECK();
+    const auto gather = colour ? k_tsub_gather<true> : k_tsub_gather<false>;
+    gather<<<blk_dst, TSUB_THREADS, 0, h->stream>>>(h->dc, h->map, h->normal, h->ts_key1, h->ts_key2, dst, a,
+                                                    h->center[2], h->cfg.use_only_above_for_upper_bound);
+    LAUNCH_CHECK();
+  }
+  if (!out_is_device) {
+    CK(cudaMemcpyAsync(out, dst, sizeof(float) * n_layers * cells, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
   }
   return EMAP_OK;

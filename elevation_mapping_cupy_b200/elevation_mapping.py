@@ -16,7 +16,8 @@ Camera images (input_image) fuse into the semantic layers with the reference's `
 one kernel projects every map cell into the image, tests occlusion along the line to the camera and writes every fused
 channel (csrc/emap_image.cuh), bit-identical to the reference's kernels on the same card.
 Windows of the exported map (get_submap / get_submaps, the node's get_raw_submap service) come from one library call
-and one kernel per batch (csrc/emap_submap.cuh).
+and one kernel per batch (csrc/emap_submap.cuh); get_transformed_submap(s) serve them in a requester's frame, as grid_map's
+getTransformedMap does, in three kernels per batch.
 The rest of the node's map timer is served too: the normals (get_normal_maps / get_normal_ref), the bridge's normal
 colour as the exported layer `normal_color`, and the exported map as a point cloud (get_map_points) and as normal arrows
 (get_normal_arrows), compacted in grid_map's cell order on the device (csrc/emap_mapcloud.cuh).
@@ -479,25 +480,86 @@ class ElevationMap:
         synchronise with the host and the results stay on the device.  Returns one dict per request: "layers" maps each
         name to a (rows, cols) view of `out`, "index" is (row0, col0), "size" (rows, cols), "centre" the centre of the
         window's cells and "success" whether the position lies in the map (a failed window has (0, 0) layers)."""
+        req = np.zeros((len(requests), 4), np.float64)
+        for w, (pos, ln) in enumerate(requests):
+            req[w] = _xy(pos) + _xy(ln)
+        n = len(req)
+        info = np.zeros((n, 5), np.int32)
+        centres = np.zeros((n, 2), np.float64)
+
+        def cells():
+            c = self.center.astype(np.float64)
+            self._check(self._L.emap_submap_windows(self.cell_n, float(self.resolution), c.ctypes.data, n,
+                                                    req.ctypes.data, info.ctypes.data, centres.ctypes.data))
+            return int((info[:, 3].astype(np.int64) * info[:, 4]).sum())
+
+        def call(nl, c_names, planes, flags, ptr, device, size):
+            self._check(self._L.emap_get_submaps(self._h, n, req.ctypes.data, nl, c_names, planes, flags, ptr,
+                                                 device, size, info.ctypes.data, centres.ctypes.data))
+
+        views = self._window_views(layers, out, cells, call, info[:, 3:5])
+        return [{"layers": views[w], "index": (int(info[w, 1]), int(info[w, 2])),
+                 "size": (int(info[w, 3]), int(info[w, 4])), "centre": centres[w].copy(), "success": bool(info[w, 0])}
+                for w in range(n)]
+
+    def get_transformed_submap(self, position, length, layers, transform, sample_ratio=0.0, out=None):
+        """The get_raw_submap service with a request frame other than the map frame, for one request: see
+        get_transformed_submaps."""
+        return self.get_transformed_submaps([(position, length, transform)], layers, out, sample_ratio)[0]
+
+    def get_transformed_submaps(self, requests, layers, out=None, sample_ratio=0.0):
+        """The get_raw_submap service (elevation_mapping_ros.cpp:507-553) in a requester's frame, in one library call
+        (emap_get_transformed_submaps; include/emap.h states the rules).  `requests` is a list of (position, length,
+        transform): position (x, y) in the request frame, length (x, y) metres, and transform the map -> request frame
+        isometry (lookupTransform(frame_id, map_frame)) as a 4 x 4 array or an (R, t) pair.  Each window is the one
+        get_submaps cuts at the map-frame position, carried into the request frame as grid_map's getTransformedMap
+        does, with `sample_ratio` (>= 0; the node uses 0).  `layers` and `out` as for get_submaps, with each window's
+        cells those of its new map.  Returns one dict per request: "layers" maps each name to a (rows, cols) view of
+        `out` (row r, column c is grid_map index (r, c) of the new map), "size" (rows, cols), "frame_centre" the new
+        map's centre (x, y) in the request frame, "length" its length (x, y), and "success" whether the map-frame
+        position lies in the map (a failed window has (0, 0) layers)."""
+        n = len(requests)
+        req = np.zeros((n, 4), np.float64)
+        tf = np.zeros((n, 12), np.float64)
+        for w, (pos, ln, T) in enumerate(requests):
+            req[w] = _xy(pos) + _xy(ln)
+            tf[w] = _isometry(T)
+        info = np.zeros((n, 3), np.int32)
+        geometry = np.zeros((n, 4), np.float64)
+
+        def cells():
+            c = self.center.astype(np.float64)
+            self._check(self._L.emap_transformed_submap_windows(self.cell_n, float(self.resolution), c.ctypes.data, n,
+                                                                req.ctypes.data, tf.ctypes.data, info.ctypes.data,
+                                                                geometry.ctypes.data))
+            return int((info[:, 1].astype(np.int64) * info[:, 2]).sum())
+
+        def call(nl, c_names, planes, flags, ptr, device, size):
+            self._check(self._L.emap_get_transformed_submaps(self._h, n, req.ctypes.data, tf.ctypes.data,
+                                                             float(sample_ratio), nl, c_names, planes, flags, ptr,
+                                                             device, size, info.ctypes.data, geometry.ctypes.data))
+
+        views = self._window_views(layers, out, cells, call, info[:, 1:3])
+        return [{"layers": views[w], "size": (int(info[w, 1]), int(info[w, 2])),
+                 "frame_centre": geometry[w, :2].copy(), "length": geometry[w, 2:].copy(), "success": bool(info[w, 0])}
+                for w in range(n)]
+
+    def _window_views(self, layers, out, cells, call, sizes):
+        """What get_submaps and get_transformed_submaps share: checks the layer names (KeyError before anything runs),
+        sizes a new host `out` with cells() (the host window arithmetic, which fills `sizes`), checks `out`, orders the
+        library call `call(n_layers, names, planes, flags, out pointer, is device, out floats)` after the caller's
+        stream and the caller's later work after it (device output), and returns per window a dict of (rows, cols)
+        views of `out` per layer, rows and cols read from `sizes` after the call."""
         names = list(layers)
         for name in names:
             if not (name in EXPORT_NAMES or name in self.semantic_map.layer_names
                     or name in self.plugin_manager.layer_names):
                 raise KeyError("Layer {} is not in the map".format(name))
-        req = np.zeros((len(requests), 4), np.float64)
-        for w, (pos, ln) in enumerate(requests):
-            req[w, :2] = np.asarray(_to_host(pos), np.float64).reshape(-1)[:2]
-            req[w, 2:] = np.asarray(_to_host(ln), np.float64).reshape(-1)[:2]
-        n, nl = len(req), len(names)
-        info = np.zeros((n, 5), np.int32)
-        centres = np.zeros((n, 2), np.float64)
+        nl = len(names)
         device = out is not None and _is_device(out)
         with self.map_lock:
             if out is None:
-                c = self.center.astype(np.float64)
-                self._check(self._L.emap_submap_windows(self.cell_n, float(self.resolution), c.ctypes.data, n,
-                                                        req.ctypes.data, info.ctypes.data, centres.ctypes.data))
-                out = np.zeros(nl * int((info[:, 3].astype(np.int64) * info[:, 4]).sum()), np.float32)
+                out = np.zeros(nl * cells(), np.float32)
             if device:
                 import torch
                 if out.dtype != torch.float32 or not out.is_contiguous():
@@ -513,20 +575,18 @@ class ElevationMap:
             flags = (C.c_int32 * nl)(*[s[2] for s in sources])
             if device or any(s[3] is not None for s in sources):
                 self._after_framework()       # the planes and the output buffer are complete / free
-            self._check(self._L.emap_get_submaps(self._h, n, req.ctypes.data, nl, c_names, planes, flags, ptr,
-                                                 int(device), size, info.ctypes.data, centres.ctypes.data))
+            call(nl, c_names, planes, flags, ptr, int(device), size)
             if device:
                 self._before_framework()      # framework reads of `out` run after the kernel (no host sync)
         flat = out.reshape(-1)
         result, off = [], 0
-        for w in range(n):
-            ok, r0, c0, rows, cols = (int(v) for v in info[w])
+        for rows, cols in sizes:
+            rows, cols = int(rows), int(cols)
             views = {}
             for name in names:
                 views[name] = flat[off:off + rows * cols].reshape(rows, cols)
                 off += rows * cols
-            result.append({"layers": views, "index": (r0, c0), "size": (rows, cols), "centre": centres[w].copy(),
-                           "success": bool(ok)})
+            result.append(views)
         return result
 
     def get_normal_maps(self):
@@ -752,6 +812,24 @@ def _to_host(x):
 
 def _is_device(x):
     return getattr(x, "__cuda_array_interface__", None) is not None if not hasattr(x, "is_cuda") else bool(x.is_cuda)
+
+
+def _xy(v):
+    """The first two values of a position or length, as a list of two floats."""
+    return list(np.asarray(_to_host(v), np.float64).reshape(-1)[:2])
+
+
+def _isometry(T):
+    """The 12 doubles (R row-major, then t) of a 4 x 4 homogeneous transform or an (R, t) pair."""
+    if isinstance(T, (tuple, list)) and len(T) == 2:
+        R = np.asarray(_to_host(T[0]), np.float64).reshape(3, 3)
+        t = np.asarray(_to_host(T[1]), np.float64).reshape(3)
+    else:
+        M = np.asarray(_to_host(T), np.float64)
+        if M.shape != (4, 4):
+            raise ValueError("a transform is a 4 x 4 array or an (R, t) pair")
+        R, t = M[:3, :3], M[:3, 3]
+    return np.concatenate([R.reshape(-1), t])
 
 
 def _depth_input(x, dtype, dev, device, keep):

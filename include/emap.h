@@ -343,6 +343,56 @@ int emap_submap_windows(int32_t cell_n, double resolution, const double center[2
 int emap_get_submaps(emap_handle* h, int32_t n_windows, const double* windows, int32_t n_layers, const char* const* names,
                      const float* const* planes_device, const int32_t* flags, float* out, int32_t out_is_device,
                      int64_t out_floats, int32_t* info, double* centres);
+/* ---- windows in the requester's frame: get_raw_submap with a frame_id other than the map frame
+ * (elevation_mapping_ros.cpp:507-553): the window around T^-1 * position, then grid_map's
+ * GridMap::getTransformedMap(T, "elevation", frame_id, sample_ratio) on it.  Restated from grid_map's published source
+ * (GridMap::getTransformedMap, GridMapMath.cpp); not checked against a grid_map build.
+ * transforms[12w .. 12w+11] = T of window w: R row-major (9), then t (3), in double; T maps map-frame points into the
+ * request frame (lookupTransform(frame_id, map_frame)).  R must be finite and orthonormal: every entry of R^T R - I
+ * within EMAP_TRANSFORM_TOLERANCE; t finite.  windows[4w .. 4w+3] = (position_x, position_y) in the request frame and
+ * (length_x, length_y), finite and >= 0.  Every product and sum below is one IEEE double operation, nothing is fused,
+ * and a matrix-vector product is ((R_k0 x + R_k1 y) + R_k2 z) (+ t_k) per component (Eigen on x86-64 SSE2).
+ *  1. Window: the map-frame position is R' (px, py, 0) + t' with R' = R^T, t' = -(R' t) (Isometry3d::inverse()); the
+ *     length is not transformed.  The window is the one emap_get_submaps cuts there: same cells, centre c, length
+ *     L = (rows, cols) * resolution.  A failed window fails here too (info {0, 0, 0}, geometry NaN, no cells).
+ *  2. New map: the corners (c_x + L_x / 2, c_y + L_y / 2, 0), (+, -), (-, +), (-, -), in that order, go through T; the
+ *     new centre is 0.25 * ((((0 + e0) + e1) + e2) + e3), the new length 2 * max |e_k - centre| per axis; size =
+ *     round(length / resolution) (half away from zero), length = size * resolution.  Every cell starts as NaN.
+ *  3. Scatter: the window's cells in grid_map order, column-major (i = col * rows + row); a cell whose exported
+ *     elevation h is NaN is skipped.  Its samples are p = (x, y, h) with x = (c_x + (0.5 L_x - 0.5 res)) - res * row,
+ *     y likewise with col (emap_get_map_points' formula on the window's geometry), and with sample_ratio > 0 four more,
+ *     in order (x - s, y, h), (x + s, y, h), (x, y - s, h), (x, y + s, h), s = resolution * sample_ratio (the
+ *     unchanged components + 0.0).  Each goes to q = R p + t.  With o = 0.5 * length per axis of the new map and its
+ *     centre m: q is inside when 0 <= -((q - m) - o) < length on both axes (checkIfPositionWithinMap), and then lands
+ *     on output index trunc(-(((q - o) - m) / resolution)) per axis (getIndexFromPosition), clamped to [0, size - 1]
+ *     (grid_map wraps an index of `size`, which only rounding can produce; parity on exact cell boundaries is not
+ *     claimed).  A sample is skipped when the target's stored elevation is not NaN and > q.z (the stored float
+ *     widened); otherwise the target's elevation becomes float(q.z) and every other layer takes the source cell's
+ *     exported value as it is (normals are copied, not rotated, as grid_map does).
+ *  The result is that sequential loop's, computed in parallel: a target's elevation is M = max float(q.z) over the
+ *  samples that reach it, and its winner is the last sample (in visit order, j = 5 i + k, or i with one sample) with
+ *  q.z >= M, else the first with float(q.z) = M.  The node passes sample_ratio 0, which leaves NaN holes at angles other
+ *  than multiples of 90 degrees (grid_map's behaviour); e.g. 0.5 fills them.
+ * info[3w .. 3w+2] = {success, rows, cols} of the new map; geometry[4w .. 4w+3] = its centre (x, y) in the request
+ * frame and its length (x, y).  Output row r, column c of window w is grid_map index (r, c) of its new map (row 0 is the
+ * +x edge, column 0 the +y edge of the request frame).  out, out_is_device, out_floats, layers, limits and the stream
+ * and graph rules are those of emap_get_submaps, with rows x cols the new map's size; the elevation layer drives the
+ * scatter whether or not it is asked for.  Three kernels per EMAP_TRANSFORMED_WINDOWS_PER_LAUNCH windows (their table
+ * travels in the kernels' parameters).  The per-cell scratch is the handle's and grows to the largest call (a call
+ * that grows it synchronises and cannot be captured: capture after an eager call of the largest size).
+ * EMAP_ERR_INVALID, with nothing written or launched, for what emap_get_submaps rejects, a NULL transforms / geometry,
+ * a transform as above, a sample_ratio that is not finite and >= 0, and a new map of 2^31 cells or more.
+ * emap_transformed_submap_windows: steps 1 and 2 alone, on the host (info and geometry as above), for a map of cell_n
+ * cells at `resolution` centred at center; no handle, no device; EMAP_ERR_INVALID for what emap_submap_windows
+ * rejects and a transform as above. */
+#define EMAP_TRANSFORM_TOLERANCE 1e-6
+#define EMAP_TRANSFORMED_WINDOWS_PER_LAUNCH 128
+int emap_transformed_submap_windows(int32_t cell_n, double resolution, const double center[2], int32_t n_windows,
+                                    const double* windows, const double* transforms, int32_t* info, double* geometry);
+int emap_get_transformed_submaps(emap_handle* h, int32_t n_windows, const double* windows, const double* transforms,
+                                 double sample_ratio, int32_t n_layers, const char* const* names,
+                                 const float* const* planes_device, const int32_t* flags, float* out,
+                                 int32_t out_is_device, int64_t out_floats, int32_t* info, double* geometry);
 /* ---- the exported map as a point cloud and as normal arrows: the ROS node's publishAsPointCloud
  * (elevation_mapping_ros.cpp:501-505, grid_map's toPointCloud(map, {"elevation"}, "elevation")) and publishNormalAsArrow
  * (:751-778), restated from grid_map's published source (not checked against a grid_map build).  Coordinates are those of
