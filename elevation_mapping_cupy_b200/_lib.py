@@ -32,6 +32,13 @@ class EmapFrameStats(C.Structure):
                 ("ray_steps", C.c_int64), ("ray_visits", C.c_int64)]
 
 
+class EmapPlaneParams(C.Structure):
+    _fields_ = [("median_kernel", C.c_int32), ("median_repeats", C.c_int32), ("resolution", C.c_double),
+                ("kernel_size", C.c_int32), ("opening", C.c_int32), ("min_points", C.c_int32),
+                ("connectivity", C.c_int32), ("plane_inclination_cos", C.c_double),
+                ("local_inclination_cos", C.c_double), ("patch_error", C.c_double), ("ransac", C.c_int32)]
+
+
 class EmapDepthCamera(C.Structure):
     _fields_ = [("height", C.c_int32), ("width", C.c_int32), ("depth", C.c_void_p), ("confidence", C.c_void_p),
                 ("rgb", C.c_void_p), ("features", C.c_void_p), ("fx", C.c_double), ("fy", C.c_double),
@@ -101,6 +108,9 @@ SIGNATURES = {
     "emap_get_transformed_submaps": (C.c_int, [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_double, C.c_int32,
                                                C.POINTER(C.c_char_p), C.POINTER(C.c_void_p), C.POINTER(C.c_int32),
                                                C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_void_p]),
+    "emap_plane_capacity": (C.c_int64, [C.c_int64, C.c_int64, C.c_void_p]),
+    "emap_segment_planes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p,
+                                      C.c_int64, C.c_void_p]),
     "emap_get_map_points": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_get_normal_arrows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_layer_device_ptr": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),

@@ -8,7 +8,7 @@ LIB = os.path.join(PKG, "libemap.so")
 SOURCES = ["emap_api.cu"]
 HEADERS = ["emap_kernels.cuh", "emap_device.cuh", "emap_inpaint.cuh", "emap_semantic.cuh", "emap_polygon.cuh",
            "emap_semantic_plugins.cuh", "emap_image.cuh", "emap_submap.cuh", "emap_mapcloud.cuh", "emap_initialize.cuh",
-           "emap_sources.cuh", "emap_plan.cuh", os.path.join("..", "..", "include", "emap.h")]
+           "emap_sources.cuh", "emap_plan.cuh", "emap_planes.cuh", os.path.join("..", "..", "include", "emap.h")]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo",
               "-Xcompiler", "-fPIC", "-shared", "-cudart", "shared", "-Xptxas", "-v"]
 

@@ -19,6 +19,7 @@
 #include "emap_semantic_plugins.cuh"
 #include "emap_image.cuh"
 #include "emap_submap.cuh"
+#include "emap_planes.cuh"
 #include "emap_mapcloud.cuh"
 #include "emap_initialize.cuh"
 
@@ -191,6 +192,9 @@ struct emap_handle {
   // emap_get_transformed_submaps' per-cell keys (grown to the largest call, zero between calls: k_tsub_gather resets)
   DevBuf<u32> ts_key1;
   DevBuf<u64> ts_key2;
+  // emap_segment_planes' scratch (grown to the largest window): one device block carved by carve_planes
+  DevBuf<char> pl_block;
+  PinnedBuf<char> pl_host;    // its host output's staging: info, plane table and layers, as one copy of the block's tail
   // plugin scratch
   DevBuf<float> pl[4];
   DevBuf<int> pl_cnt;
@@ -1770,6 +1774,17 @@ int emap_submap_windows(int32_t cell_n, double resolution, const double center[2
   return EMAP_OK;
 }
 
+// Appends the successful window q = submap_window's info to k_submap's table: its first work item is `tiles` and its
+// first output float `total`, both advanced past it.
+static void submap_add(SubmapArgs& a, int W, const int32_t q[5], int n_layers, int& tiles, long long& total) {
+  SubmapWin& s = a.win[a.n_win++];
+  s.r0 = (int16_t)(W - 2 - q[1]); s.c0 = (int16_t)(W - 2 - q[2]);
+  s.rows = (int16_t)q[3]; s.cols = (int16_t)q[4];
+  s.tile0 = tiles; s.off = total;
+  tiles += cdiv(q[3], SUBMAP_ROWS);
+  total += (long long)n_layers * q[3] * q[4];
+}
+
 // The get_raw_submap service (elevation_mapping_ros.cpp:507-553) for a batch of windows: the windows on the host
 // (submap_window), every (window, layer, row) of the batch in one k_submap launch whose table is its parameters.  Host
 // output: one device-to-host copy and one synchronisation; device output: stream-ordered, no synchronisation.  Every
@@ -1798,13 +1813,7 @@ int emap_get_submaps(emap_handle* h, int32_t n_windows, const double* windows, i
   for (int w = 0; w < n_windows; w++) {
     const int32_t* q = &inf[5 * w];
     submap_window(W, h->cfg.resolution, m, windows + 4 * w, &inf[5 * w], &cen[2 * w]);
-    if (!q[0]) continue;
-    SubmapWin& s = a.win[a.n_win++];
-    s.r0 = (int16_t)(W - 2 - q[1]); s.c0 = (int16_t)(W - 2 - q[2]);
-    s.rows = (int16_t)q[3]; s.cols = (int16_t)q[4];
-    s.tile0 = tiles; s.off = total;
-    tiles += cdiv(q[3], SUBMAP_ROWS);
-    total += (long long)n_layers * q[3] * q[4];
+    if (q[0]) submap_add(a, W, q, n_layers, tiles, total);
   }
   if (total > out_floats)
     return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: out_floats is below the layers times the windows' cells");
@@ -1944,6 +1953,215 @@ int emap_get_transformed_submaps(emap_handle* h, int32_t n_windows, const double
   if (!out_is_device) {
     CK(cudaMemcpyAsync(out, dst, sizeof(float) * n_layers * cells, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
+  }
+  return EMAP_OK;
+}
+
+// ---- plane segmentation of one window (emap_segment_planes, csrc/emap_planes.cuh) ----------------------------------
+
+// The scratch of a window of n cells with `slots` label slots, one block: the window, two image planes (fill / median
+// ping-pong), union-find parents, flags and ranks, fill keys, the planarity masks, scan block sums, the header words,
+// the label statistics and decisions, and the host output's staging (info, plane table, layers).
+namespace {
+
+struct PlaneScratch {
+  float *raw, *img[2];
+  int *parent, *flag, *rank, *lab, *bsum, *hdr, *keep;
+  unsigned* key;
+  unsigned char *bin, *tmp, *bg;
+  unsigned long long* st;
+  int32_t* info;
+  double* planes;
+  float* layers;
+};
+
+size_t carve_planes(int64_t n, int64_t slots, int64_t plane_rows, bool host_out, void* base, PlaneScratch& s) {
+  Carver c{(uintptr_t)base};
+  const int64_t m = std::max(n, slots);
+  s.raw = c.take<float>(n); s.img[0] = c.take<float>(n); s.img[1] = c.take<float>(n);
+  s.parent = c.take<int>(n); s.flag = c.take<int>(m); s.rank = c.take<int>(m); s.lab = c.take<int>(n);
+  s.bsum = c.take<int>(m / PL_SCAN + 1); s.hdr = c.take<int>(8); s.keep = c.take<int>(slots);
+  s.key = c.take<unsigned>(n);
+  s.bin = c.take<unsigned char>(n); s.tmp = c.take<unsigned char>(n); s.bg = c.take<unsigned char>(slots);
+  s.st = c.take<unsigned long long>(slots * PL_STAT);
+  s.info = c.take<int32_t>(host_out ? 8 : 0);
+  s.planes = c.take<double>(host_out ? 7 * plane_rows : 0);
+  s.layers = c.take<float>(host_out ? 4 * n : 0);
+  return c.bytes;
+}
+
+// Raster-order ranks of the n flags in s.flag into s.rank, the count into *total (three launches).
+int plane_scan(emap_handle* h, const PlaneScratch& s, int64_t n, int* total) {
+  const int nb = cdiv(n, PL_SCAN);
+  k_pl_scan_blocks<<<nb, PL_SCAN, 0, h->stream>>>(s.flag, (int)n, s.bsum);
+  LAUNCH_CHECK();
+  k_pl_scan_top<<<1, PL_SCAN, 0, h->stream>>>(s.bsum, nb, total);
+  LAUNCH_CHECK();
+  k_pl_scan_rank<<<nb, PL_SCAN, 0, h->stream>>>(s.flag, (int)n, s.bsum, s.rank);
+  LAUNCH_CHECK();
+  return 0;
+}
+
+// Union-find merge and flatten of the cells whose parent is >= 0.
+int plane_components(emap_handle* h, const PlaneScratch& s, int rows, int cols, int conn8) {
+  const int64_t n = (int64_t)rows * cols;
+  k_pl_uf_merge<<<cdiv(n, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.parent, rows, cols, conn8);
+  LAUNCH_CHECK();
+  k_pl_uf_flatten<<<cdiv(n, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.parent, (int)n);
+  LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace
+
+static_assert(EMAP_PLANE_EIGEN_MIN == PL_EIG_MIN, "emap.h states the fit's threshold");
+
+// Why p is rejected (nullptr: accepted) for a map of resolution `res`.
+static const char* plane_params_error(const emap_plane_params& p, double res) {
+  if (p.ransac) return "emap_segment_planes: RANSAC refinement is not supported (ransac must be 0)";
+  const int mk = std::max(1, std::min(p.median_kernel, 5));
+  if (mk != 1 && mk != 3 && mk != 5) return "emap_segment_planes: the median kernel must clamp to 1, 3 or 5";
+  if (p.median_repeats < 0 || p.median_repeats > EMAP_PLANE_MAX_REPEATS)
+    return "emap_segment_planes: median_repeats must be in [0, EMAP_PLANE_MAX_REPEATS]";
+  if (std::isnan(p.resolution) || (p.resolution > 0.0 && !(std::fabs(res - p.resolution) < 1e-6)))
+    return "emap_segment_planes: resampling is not supported (resolution must be <= 0 or the map's)";
+  if (p.kernel_size < 3 || p.kernel_size % 2 == 0 || p.kernel_size > EMAP_PLANE_MAX_KERNEL)
+    return "emap_segment_planes: kernel_size must be odd, >= 3 and <= EMAP_PLANE_MAX_KERNEL";
+  if (p.opening < 0 || p.opening > EMAP_PLANE_MAX_OPENING)
+    return "emap_segment_planes: opening must be in [0, EMAP_PLANE_MAX_OPENING]";
+  if (p.connectivity != 4 && p.connectivity != 8) return "emap_segment_planes: connectivity must be 4 or 8";
+  if (!std::isfinite(p.plane_inclination_cos) || !std::isfinite(p.local_inclination_cos) ||
+      !std::isfinite(p.patch_error))
+    return "emap_segment_planes: the inclination cosines and the patch error must be finite";
+  return nullptr;
+}
+
+int64_t emap_plane_capacity(int64_t rows, int64_t cols, const emap_plane_params* params) {
+  if (!params || rows < 0 || cols < 0) return -1;
+  return rows * cols / std::max(params->min_points, 3);
+}
+
+// The plane decomposition node's segmented planes map for one window (ConvexPlaneDecompositionRos.cpp:115-149 up to
+// SlidingWindowPlaneExtractor, without RANSAC): the window by k_submap, then the passes of csrc/emap_planes.cuh.  Host
+// output: the copies and one synchronisation; device output: stream-ordered, no synchronisation.  Every check runs
+// before anything is written or launched.
+int emap_segment_planes(emap_handle* h, const double window[4], const emap_plane_params* params, float* layers_out,
+                        int32_t out_is_device, int64_t out_floats, double* planes_out, int64_t planes_capacity,
+                        int32_t* info) {
+  ENTER(h);
+  NvtxRange nv("emap:segment_planes");
+  if (!window || !params || !layers_out || !planes_out || !info)
+    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: null argument");
+  if (!submap_lengths_ok(1, window)) return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: lengths must be finite and >= 0");
+  const emap_plane_params p = *params;
+  const double res = h->cfg.resolution;
+  if (const char* e = plane_params_error(p, res)) return fail(h, EMAP_ERR_INVALID, e);
+  const int W = h->dc.W;
+  const double m[2] = {h->center[0], h->center[1]};
+  int32_t q[5];
+  double centre[2];
+  submap_window(W, res, m, window, q, centre);
+  const int rows = q[3], cols = q[4];
+  const int64_t n = (int64_t)rows * cols;
+  if (q[0] && out_floats < 4 * n)
+    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: out_floats is below 4 * rows * cols");
+  const int64_t plane_rows = emap_plane_capacity(rows, cols, &p);
+  if (q[0] && planes_capacity < plane_rows)
+    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: planes_capacity is below emap_plane_capacity()");
+  if (!q[0]) {
+    if (out_is_device) CK(cudaMemsetAsync(info, 0, 5 * sizeof(int32_t), h->stream));
+    else memset(info, 0, 5 * sizeof(int32_t));
+    return EMAP_OK;
+  }
+  // labels are at most ceil(n / 2) (a 4-connected checkerboard), plus 0.  The statistics are sized and zeroed for that
+  // worst case (128 bytes a slot) because the label count is known only on the device.
+  const int64_t slots = n / 2 + 2;
+  PlaneScratch s;
+  int rc = grow(h, h->pl_block, carve_planes(n, slots, plane_rows, !out_is_device, nullptr, s), 0, false);
+  if (rc) return rc;
+  const size_t used = carve_planes(n, slots, plane_rows, !out_is_device, h->pl_block, s);
+  float* dst = out_is_device ? layers_out : s.layers;
+  double* dst_planes = out_is_device ? planes_out : s.planes;
+  int32_t* dst_info = out_is_device ? info : s.info;
+  // the window: k_submap's elevation layer into s.raw
+  SubmapArgs a;
+  const char* elevation = "elevation";
+  if (!export_list(h, 1, &elevation, nullptr, nullptr, a.L)) return EMAP_ERR_CUDA;
+  a.n_win = 0;
+  int tiles = 0;
+  long long total = 0;
+  submap_add(a, W, q, 1, tiles, total);
+  k_submap<false><<<dim3(tiles, 1), dim3(32, SUBMAP_ROWS), 0, h->stream>>>(h->dc, h->map, h->normal, s.raw, a, h->center[2],
+                                                                           h->cfg.use_only_above_for_upper_bound);
+  LAUNCH_CHECK();
+  CK(cudaMemsetAsync(s.hdr, 0, 8 * sizeof(int), h->stream));
+  CK(cudaMemsetAsync(s.st, 0, sizeof(unsigned long long) * slots * PL_STAT, h->stream));
+  const int cb = cdiv(n, PL_THREADS);
+  // fill: minValues' fixed point per NaN component
+  k_pl_fill_init<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, s.hdr, (int)n);
+  LAUNCH_CHECK();
+  if ((rc = plane_components(h, s, rows, cols, 0))) return rc;
+  k_pl_fill_min<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, rows, cols);
+  LAUNCH_CHECK();
+  k_pl_fill_write<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, s.img[0], (int)n);
+  LAUNCH_CHECK();
+  // median, numberOfRepeats times
+  const int mk = std::max(1, std::min(p.median_kernel, 5));
+  int cur = 0;
+  if (mk > 1)
+    for (int r = 0; r < p.median_repeats; r++, cur ^= 1) {
+      (mk == 3 ? k_pl_median<3> : k_pl_median<5>)<<<cb, PL_THREADS, 0, h->stream>>>(s.img[cur], s.img[cur ^ 1], rows, cols);
+      LAUNCH_CHECK();
+    }
+  const float* img = s.img[cur];
+  // sliding-window planarity, opening, labels
+  k_pl_fit<<<cb, PL_THREADS, 0, h->stream>>>(img, s.bin, rows, cols, p.kernel_size, res, p.patch_error * p.patch_error,
+                                             p.local_inclination_cos);
+  LAUNCH_CHECK();
+  if (p.opening > 0) {
+    k_pl_morph<false><<<cb, PL_THREADS, 0, h->stream>>>(s.bin, s.tmp, rows, cols, p.opening);
+    LAUNCH_CHECK();
+    k_pl_morph<true><<<cb, PL_THREADS, 0, h->stream>>>(s.tmp, s.bin, rows, cols, p.opening);
+    LAUNCH_CHECK();
+  }
+  k_pl_cc_init<<<cb, PL_THREADS, 0, h->stream>>>(s.bin, s.parent, s.key, s.flag, (int)n);
+  LAUNCH_CHECK();
+  const bool conn8 = p.connectivity == 8;
+  if ((rc = plane_components(h, s, rows, cols, conn8))) return rc;
+  (conn8 ? k_pl_first<2> : k_pl_first<1>)<<<cb, PL_THREADS, 0, h->stream>>>(s.parent, s.key, rows, cols);
+  LAUNCH_CHECK();
+  k_pl_first_flag<<<cb, PL_THREADS, 0, h->stream>>>(s.parent, s.key, s.flag, (int)n);
+  LAUNCH_CHECK();
+  const int64_t n_blocks = conn8 ? (int64_t)cdiv(rows, 2) * cdiv(cols, 2) : n;
+  if ((rc = plane_scan(h, s, n_blocks, s.hdr + 1))) return rc;
+  k_pl_label<<<cb, PL_THREADS, 0, h->stream>>>(s.parent, s.key, s.rank, s.lab, (int)n);
+  LAUNCH_CHECK();
+  // per-label planes
+  k_pl_stats<<<cdiv(cdiv(n, PL_RUN), PL_THREADS), PL_THREADS, 0, h->stream>>>(img, s.lab, s.st, rows, cols);
+  LAUNCH_CHECK();
+  const PlaneLabelArgs la = {centre[0] + (0.5 * (rows * res) - 0.5 * res), centre[1] + (0.5 * (cols * res) - 0.5 * res),
+                             res, p.plane_inclination_cos, p.min_points};
+  k_pl_decide<<<cdiv(slots, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.st, s.hdr, s.flag, s.bg, (int)slots, la);
+  LAUNCH_CHECK();
+  if ((rc = plane_scan(h, s, slots, s.hdr + 2))) return rc;
+  k_pl_planes<<<cdiv(slots, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.st, s.rank, s.hdr, dst_planes, (int)slots, la);
+  LAUNCH_CHECK();
+  k_pl_out<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, img, s.lab, s.bg, s.hdr, dst, dst_info, rows, cols);
+  LAUNCH_CHECK();
+  if (!out_is_device) {
+    // info, the plane table and the layers are the block's tail: one copy, one synchronisation, and the caller's
+    // buffers take the layers and planes only when the window had a finite cell
+    const size_t off = (char*)s.info - (char*)h->pl_block, bytes = used - off;
+    if (h->pl_host.size() < bytes) CK(h->pl_host.alloc(bytes));
+    CK(cudaMemcpyAsync(h->pl_host, s.info, bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    PlaneScratch t;
+    carve_planes(n, slots, plane_rows, true, (char*)h->pl_host - off, t);
+    memcpy(info, t.info, 5 * sizeof(int32_t));
+    if (info[0]) {
+      memcpy(planes_out, t.planes, sizeof(double) * 7 * info[4]);
+      memcpy(layers_out, t.layers, sizeof(float) * 4 * n);
+    }
   }
   return EMAP_OK;
 }

@@ -544,6 +544,58 @@ class ElevationMap:
                  "frame_centre": geometry[w, :2].copy(), "length": geometry[w, 2:].copy(), "success": bool(info[w, 0])}
                 for w in range(n)]
 
+    def segment_planes(self, position, length, params=None, out=None):
+        """The plane decomposition node's segmented planes map for the get_submap window around `position` (x, y) of
+        `length` (x, y) metres, in one library call (emap_segment_planes; include/emap.h states every step).  `params` is
+        a PlaneSegmentationParams (None: the node's parameters.yaml without RANSAC refinement).  `out`: None (new NumPy
+        arrays) or a contiguous float32 torch CUDA tensor of at least 4 * rows * cols floats; with a tensor the layers
+        and the plane table stay on the device, and only the five info words are read back.  Returns a dict: "layers"
+        maps elevation_raw, elevation, segmentation and plane_classification to (rows, cols) views; "planes" is an
+        (n, 7) float64 array (label, support xyz, normal xyz); "highest_label", "origin" (the centre of window cell
+        (0, 0)), "resolution", "size" and "success" (False when the window is outside the map or has no finite cell;
+        its layers are then not written)."""
+        from .plane_segmentation import PlaneSegmentationParams
+        p = (params or PlaneSegmentationParams()).to_c()
+        req = np.array(_xy(position) + _xy(length), np.float64)
+        win = np.zeros(5, np.int32)
+        centre = np.zeros(2, np.float64)
+        device = out is not None and _is_device(out)
+        names = ["elevation_raw", "elevation", "segmentation", "plane_classification"]
+        with self.map_lock:
+            c = self.center.astype(np.float64)
+            self._check(self._L.emap_submap_windows(self.cell_n, float(self.resolution), c.ctypes.data, 1,
+                                                    req.ctypes.data, win.ctypes.data, centre.ctypes.data))
+            rows, cols = int(win[3]), int(win[4])
+            cap = max(int(self._L.emap_plane_capacity(rows, cols, C.byref(p))), 1)
+            if device:
+                import torch
+                if out.dtype != torch.float32 or not out.is_contiguous():
+                    raise TypeError("a device `out` must be a contiguous float32 torch CUDA tensor")
+                planes = torch.empty((cap, 7), dtype=torch.float64, device=out.device)
+                info = torch.zeros(5, dtype=torch.int32, device=out.device)
+                ptrs = (out.data_ptr(), out.numel(), planes.data_ptr(), info.data_ptr())
+                self._after_framework()
+            else:
+                if out is None:
+                    out = np.zeros(4 * rows * cols, np.float32)
+                if out.dtype != np.float32 or not out.flags.c_contiguous:
+                    raise TypeError("a host `out` must be a C-contiguous float32 NumPy array")
+                planes = np.zeros((cap, 7), np.float64)
+                info = np.zeros(5, np.int32)
+                ptrs = (out.ctypes.data, out.size, planes.ctypes.data, info.ctypes.data)
+            self._check(self._L.emap_segment_planes(self._h, req.ctypes.data, C.byref(p), ptrs[0], int(device),
+                                                    ptrs[1], ptrs[2], cap, ptrs[3]))
+            if device:
+                self._before_framework()
+        info_h = info.cpu().numpy() if device else info
+        n = rows * cols
+        flat = out.reshape(-1)
+        res = float(self.resolution)
+        return {"layers": {name: flat[k * n:(k + 1) * n].reshape(rows, cols) for k, name in enumerate(names)},
+                "planes": planes[:int(info_h[4])], "highest_label": int(info_h[3]),
+                "origin": centre + (0.5 * (np.array([rows, cols]) * res) - 0.5 * res), "resolution": res,
+                "size": (rows, cols), "success": bool(info_h[0])}
+
     def _window_views(self, layers, out, cells, call, sizes):
         """What get_submaps and get_transformed_submaps share: checks the layer names (KeyError before anything runs),
         sizes a new host `out` with cells() (the host window arithmetic, which fills `sizes`), checks `out`, orders the

@@ -393,6 +393,70 @@ int emap_get_transformed_submaps(emap_handle* h, int32_t n_windows, const double
                                  double sample_ratio, int32_t n_layers, const char* const* names,
                                  const float* const* planes_device, const int32_t* flags, float* out,
                                  int32_t out_is_device, int64_t out_floats, int32_t* info, double* geometry);
+/* ---- plane segmentation of one window: the plane decomposition node's segmented planes map
+ * (convex_plane_decomposition_ros: ConvexPlaneDecompositionRos.cpp:115-149, GridMapPreprocessing, then
+ * SlidingWindowPlaneExtractor without RANSAC refinement), for one window of the exported elevation.
+ *  Window: the one emap_get_submaps cuts for window = (position_x, position_y, length_x, length_y), with its clipping,
+ *    success flag and orientation (row 0 the +x edge, column 0 the +y edge); origin = the centre of window cell (0, 0),
+ *    centre + (0.5 * n * resolution - 0.5 * resolution) per axis with n = rows / cols (grid_map's getPosition(Index(0, 0))).
+ *  Fill (inpainting::minValues): every NaN cell of a 4-connected NaN component takes the minimum of the non-NaN
+ *    4-neighbours of the component.  Only NaN is missing; +-inf are values.  -0.0 counts as below +0.0 (minValues'
+ *    `<` treats them as equal and keeps the one its scan meets first), so a filled zero may differ in its sign bit.
+ *    A window with no finite cell gives info {0, rows, cols, 0, 0} and leaves the layers and the plane table
+ *    unwritten; the kernels are launched all the same (they find that out on the device).
+ *  Median (smoothing::median): k = max(1, min(median_kernel, 5)), which must be 1, 3 or 5; median_repeats times the
+ *    exact median of the k x k values around each cell, border replicated (cv::medianBlur on CV_32F).
+ *  Resolution: `resolution` <= 0, or within 1e-6 of the map's, means no resampling; anything else is rejected.
+ *  Per-cell fit: the kernel_size x kernel_size window (odd, >= 3) around each cell, cells outside the window and
+ *    non-finite heights skipped, points (-kr * res, -kc * res, h) for window row kr, column kc, summed in double.  With
+ *    n < 3 points, or the middle eigenvalue of S / n - mean mean^T <= EMAP_PLANE_EIGEN_MIN, the fit is (UnitZ, 1e30);
+ *    else the normal is the smallest eigenvalue's eigenvector flipped to z >= 0 and the error that eigenvalue clamped
+ *    at 0.  A cell is planar iff its height is finite, error < patch_error^2 and normal.z > local_inclination_cos.
+ *  Opening: with opening = r > 0, MORPH_OPEN once with a (2r + 1) cross, border replicated.
+ *  Labels: cv::connectedComponents(planar, connectivity 4 or 8): background 0, components 1 .. N - 1 in raster order of
+ *    their first cell with connectivity 4, of their first 2 x 2 cell block (blocks in raster order) with 8, as
+ *    OpenCV's SAUF and Spaghetti scans number them; highest_label = N - 1.
+ *  Per-label fit: the finite cells of label L as points (origin_x - row * res, origin_y - col * res, h).  With fewer
+ *    than max(min_points, 3) points the label stays and gets no plane.  Else support = the mean and normal as in the
+ *    per-cell fit; normal.z > plane_inclination_cos appends (L, support, normal), labels ascending; otherwise every
+ *    cell of L becomes 0.  The sums are exact integer (fixed-point) sums, so support and normal agree with a double
+ *    evaluation of the same formulas to rounding (the tests hold them to 1e-9); every other output is exact.
+ * layers_out: 4 planes of rows x cols row-major: elevation_raw (the window), elevation (filled and denoised),
+ * segmentation (the labels as float) and plane_classification (1.0 where the label is > 0, else 0.0); out_floats >=
+ * 4 * rows * cols.  planes_out: 7 doubles per plane (label, support xyz, normal xyz), planes_capacity >=
+ * emap_plane_capacity(rows, cols, params) rows (rows * cols always suffices).  info = {success, rows, cols,
+ * highest_label, n_planes}; a failed window gives all 0 and writes nothing else.
+ * Host output (out_is_device 0): info, the plane table and the layers come back in one device-to-host copy (through
+ * the handle's pinned staging) and one synchronisation; only the n_planes rows of planes_out are written.  Device output: layers_out, planes_out and info are device memory, the work is queued on the handle's
+ * stream with no host synchronisation (see emap_wait_for_stream / emap_stream_wait_for).  The kernels launched depend on
+ * the parameters only, not on the scene.  The map state is not changed.  The scratch is the handle's and grows to the
+ * largest window (a call that grows it synchronises).
+ * EMAP_ERR_INVALID, with nothing written or launched, for a NULL argument, a length that is not finite and >= 0,
+ * ransac != 0, a median kernel or repeat count, resolution, kernel_size, opening or connectivity as above, non-finite
+ * cosines or patch error, and an output too small. */
+typedef struct emap_plane_params {
+  int32_t median_kernel;           /* preprocessing/kernelSize */
+  int32_t median_repeats;          /* preprocessing/numberOfRepeats, 0 .. EMAP_PLANE_MAX_REPEATS */
+  double resolution;               /* preprocessing/resolution */
+  int32_t kernel_size;             /* sliding_window_plane_extractor/kernel_size, odd, 3 .. EMAP_PLANE_MAX_KERNEL */
+  int32_t opening;                 /* planarity_opening_filter, 0 .. EMAP_PLANE_MAX_OPENING */
+  int32_t min_points;              /* min_number_points_per_label */
+  int32_t connectivity;            /* 4 or 8 */
+  double plane_inclination_cos;    /* cos(plane_inclination_threshold_degrees) */
+  double local_inclination_cos;    /* cos(local_plane_inclination_threshold_degrees) */
+  double patch_error;              /* plane_patch_error_threshold [m] */
+  int32_t ransac;                  /* include_ransac_refinement: must be 0 */
+} emap_plane_params;
+#define EMAP_PLANE_EIGEN_MIN 1e-8
+#define EMAP_PLANE_MAX_REPEATS 64
+#define EMAP_PLANE_MAX_KERNEL 63
+#define EMAP_PLANE_MAX_OPENING 64
+/* The least planes_capacity for a rows x cols window: rows * cols / max(min_points, 3) (every plane has that many
+ * cells); -1 for a NULL params or a negative size. */
+int64_t emap_plane_capacity(int64_t rows, int64_t cols, const emap_plane_params* params);
+int emap_segment_planes(emap_handle* h, const double window[4], const emap_plane_params* params, float* layers_out,
+                        int32_t out_is_device, int64_t out_floats, double* planes_out, int64_t planes_capacity,
+                        int32_t* info);
 /* ---- the exported map as a point cloud and as normal arrows: the ROS node's publishAsPointCloud
  * (elevation_mapping_ros.cpp:501-505, grid_map's toPointCloud(map, {"elevation"}, "elevation")) and publishNormalAsArrow
  * (:751-778), restated from grid_map's published source (not checked against a grid_map build).  Coordinates are those of
