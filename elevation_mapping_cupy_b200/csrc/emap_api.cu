@@ -1,411 +1,14 @@
-// emap_api.cu -- C ABI of libemap.so (see include/emap.h) and host-side orchestration.
+// emap_api.cu -- C ABI of libemap.so (see include/emap.h): the handle, frames (point clouds, depth images, sharded
+// frames and their NCCL exchange), semantic configuration, read-backs, pose, time and state, streams and stage timing.
+// The other calls are in emap_export_api.cu, emap_polygon_api.cu and emap_plugins_api.cu (see emap_handle.cuh).
 // Build: nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo -O3 (see elevation_mapping_cupy_b200/build.py)
-#include <cmath>
-#include <cstdio>
-#include <cstdlib>
-#include <cstring>
-#include <mutex>
-#include <string>
-#include <vector>
-
 #include <dlfcn.h>
-#include <nvtx3/nvToolsExt.h>
 
-#include "../../include/emap.h"
+#include "emap_handle.cuh"
 #include "emap_kernels.cuh"
-#include "emap_inpaint.cuh"
 #include "emap_semantic.cuh"
-#include "emap_polygon.cuh"
-#include "emap_semantic_plugins.cuh"
-#include "emap_image.cuh"
-#include "emap_submap.cuh"
-#include "emap_planes.cuh"
-#include "emap_mapcloud.cuh"
-#include "emap_initialize.cuh"
 
 static_assert(EMAP_DEPTH_MAX_CHANNELS == SEM_MAX_CH, "emap.h and the semantic kernels disagree on the channel count");
-
-namespace {
-
-thread_local std::string g_create_error;
-
-// Owner of one allocation of n elements of T, in device memory or (PINNED) in page-locked host memory: freed with its
-// owner; grown by replacing it (grow() below for device memory).  Reads as a T* in kernel launches and pointer arithmetic.
-template <typename T, bool PINNED = false>
-class DevBuf {
- public:
-  DevBuf() = default;
-  DevBuf(const DevBuf&) = delete;
-  DevBuf& operator=(const DevBuf&) = delete;
-  ~DevBuf() { reset(); }
-  operator T*() const { return p_; }
-  size_t size() const { return n_; }
-  cudaError_t alloc(size_t n) {
-    reset();
-    const cudaError_t e = PINNED ? cudaHostAlloc((void**)&p_, sizeof(T) * n, cudaHostAllocDefault)
-                                 : cudaMalloc(&p_, sizeof(T) * n);
-    if (e == cudaSuccess) n_ = n; else p_ = nullptr;
-    return e;
-  }
-  void reset() {
-    if (p_) PINNED ? cudaFreeHost(p_) : cudaFree(p_);
-    p_ = nullptr; n_ = 0;
-  }
-
- private:
-  T* p_ = nullptr;
-  size_t n_ = 0;
-};
-
-template <typename T>
-using PinnedBuf = DevBuf<T, true>;
-
-// Owner of one stream or event: destroyed with its owner.  Reads as the raw cudaStream_t / cudaEvent_t.
-template <typename H, cudaError_t (*Create)(H*, unsigned), cudaError_t (*Destroy)(H)>
-class CudaHandle {
- public:
-  CudaHandle() = default;
-  CudaHandle(const CudaHandle&) = delete;
-  CudaHandle& operator=(const CudaHandle&) = delete;
-  ~CudaHandle() { if (h_) Destroy(h_); }
-  operator H() const { return h_; }
-  cudaError_t create(unsigned flags) { return Create(&h_, flags); }
-
- private:
-  H h_ = nullptr;
-};
-using Stream = CudaHandle<cudaStream_t, cudaStreamCreateWithFlags, cudaStreamDestroy>;
-using Event = CudaHandle<cudaEvent_t, cudaEventCreateWithFlags, cudaEventDestroy>;
-
-struct StageTimer {
-  Event ev[9];
-  bool have = false;
-};
-
-// A host-to-device upload through pinned staging, each buffer grown to the largest upload: the device copy kernels
-// read, its staging, and the event after which the staging may be overwritten.
-struct StagedUpload {
-  DevBuf<char> dev;
-  PinnedBuf<char> host;
-  Event staged;
-  int room(emap_handle* h, size_t n);      // both buffers hold n bytes, and the previous upload has left the staging
-  int send(emap_handle* h, size_t n);      // queues the upload of the first n staged bytes on the handle's stream
-};
-
-// The input of a frame: where its kernels read every sensor's points, and when the caller may reuse its host memory.
-// A frame describes it (kind, rows, the caller's buffers); stage() makes the buffers readable by the kernels, each()
-// hands every sensor's point source to a launch, read_done() follows each pass that reads them, and wait_free()
-// returns once the caller may reuse them.
-struct FrameInput {
-  enum Kind { F32_ROWS, F64_ROWS, DEPTH };
-  enum Residence { DEVICE, STAGED, ZERO_COPY };    // the caller's device memory, a staged copy, page-locked host memory
-  DevBuf<char> staging[2];                         // used by alternate staged frames
-  Event staging_free[2], copied, host_free;        // staging block b reusable; staged copies done; zero-copy input read
-  int buf = 1;                                     // staging block of the last staged frame
-  Kind kind = F32_ROWS;                // the current frame's kind and residence
-  Residence res = DEVICE;
-  bool read = false, held = false;     // read_done() has run; wait_free() has yet to wait
-  std::vector<int64_t> n;              // rows of sensor s
-  // bytes[k] bytes at bufs[k] as the caller passed them (rows: sensor s's at k = s; DEPTH: camera s's depth,
-  // confidence, rgb and feature planes at k = 4s .. 4s + 3), read by the kernels at readable[k] (stage)
-  std::vector<const void*> bufs, readable;
-  std::vector<size_t> bytes;
-  int64_t stride = 0;                  // rows: elements from one row to the next
-  std::vector<DepthSource> cams;       // DEPTH: camera s, pointed at its planes by stage() (a null conf stays null)
-  int stage(emap_handle* h, int is_device_ptr);
-  int read_done(emap_handle* h);
-  int wait_free(emap_handle* h);
-  template <typename F>     // f(src, s) for the point source of every sensor s (float or double rows, or a camera)
-  int each(F&& f) const {   // until one returns non-zero
-    for (int s = 0; s < (int)n.size(); s++) {
-      const int rc = kind == DEPTH ? f(cams[s], s)
-                   : kind == F32_ROWS ? f(RowSource<float>{(const float*)readable[s], stride}, s)
-                                      : f(RowSource<double>{(const double*)readable[s], stride}, s);
-      if (rc) return rc;
-    }
-    return 0;
-  }
-};
-
-// How far the current frame has come (a sharded frame's caller drives it one call at a time): none, input staged, the
-// index / fusion / ray-cast pass queued, or exchange 3 took the upper-bound keys (the finish merges them back first)
-enum class Progress { IDLE, BEGUN, INDEXED, FUSED, RAYS_CAST, KEYS_EXCHANGED };
-
-// sizes of the polygon check's scratch (carve_polygon): upload bytes, partials, column extremes, read-back bytes
-struct PolySizes {
-  size_t up = 0, items = 0, cols = 0, down = 0;
-};
-
-}  // namespace
-
-struct emap_handle {
-  ~emap_handle();
-  emap_config cfg;
-  DevCfg dc;
-  FramePlan plan;             // make_plan: march table, kernel variants, shared-memory layouts
-  int device = 0;
-  std::mutex mu;
-  std::string err;
-  cudaStream_t stream = nullptr;                        // own_stream or the caller's (emap_set_stream)
-  Stream own_stream, copy_stream, side_stream;
-  Event ev_fork, ev_join;                               // side-stream fork / join of the deferred fusion pushes
-  Event ev_order;                                       // emap_wait_for_stream / emap_stream_wait_for
-  // state
-  DevBuf<float> map;          // (7,W,W); the same buffer for the handle's lifetime (captured frames bind it)
-  DevBuf<float> map_alt;      // shift target, copied back into map
-  CUtensorMap post_tm;        // TMA descriptor of map as a (W, W, 7) fp32 tensor, box = k_post's staged tile
-  DevBuf<float> normal;       // (3,W,W)
-  DevBuf<float> trav_input;
-  float center[3] = {0, 0, 0};        // fp32 like EM.py:61
-  float base_rotation[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1};
-  // scratch
-  CellScratch sc{};
-  FrameScalars* fs = nullptr;
-  DevBuf<char> xscratch;      // the library's exchange scratch (carve_exchange): sc's per-cell arrays + fs; empty once attached
-  DevBuf<int> ukey_x;         // exchange copy of the upper-bound keys (sharded frames)
-  DevBuf<float> steps;        // device march table: [0] dummy, [1 + k] = s_k, +inf padded to plan.n_tab entries
-  DevBuf<unsigned short> lut;        // cell of every fp16 bit pattern (k_build_lut)
-  DevBuf<unsigned short> step_cnt;   // march steps below every non-negative fp16 value (k_build_step_cnt)
-  DevBuf<unsigned char> dirty;       // per-cell dirty bytes of single-GPU frames (CellScratch::dirty)
-  DevBuf<float> thr;                 // CellScratch::thr
-  DevBuf<u32> tmap;                  // coarse ray map of the frame: RT x RT tile maxima of thr (keys)
-  // points
-  FrameInput in;
-  DevBuf<float4> xyzv;
-  DevBuf<int> pidx;
-  DevBuf<Ray> rays;           // compacted rays of the frame, one segment per sensor (at the sensor's point offset)
-  DevBuf<int> ray_ctl;        // per sensor: RC_CTL ints {ray count, work-queue counters}; zero between frames (k_finalize)
-  bool overlap_override = false;
-  float overlap_z_override = 0.f;
-  int n_sm = 132, rc_blocks_per_sm = 8;
-  // last frame description
-  std::vector<Pose> poses;
-  std::vector<i64> offs;      // n_sensors + 1
-  i64 n_points = 0, global_off = 0;
-  float pos_noise = 0, ori_noise = 0;
-  Progress progress = Progress::IDLE;
-  bool fused_drift = false;   // single-GPU frame: no k_drift launch (k_fuse decides, k_finalize resets)
-  // multicast-attached scratch (sharded frames over NVLink multicast, emap_shard_attach)
-  bool attached = false;
-  // export staging
-  DevBuf<float> d_export;
-  // emap_get_transformed_submaps' per-cell keys (grown to the largest call, zero between calls: k_tsub_gather resets)
-  DevBuf<u32> ts_key1;
-  DevBuf<u64> ts_key2;
-  // emap_segment_planes' scratch (grown to the largest window): one device block carved by carve_planes
-  DevBuf<char> pl_block;
-  PinnedBuf<char> pl_host;    // its host output's staging: info, plane table and layers, as one copy of the block's tail
-  // plugin scratch
-  DevBuf<float> pl[4];
-  DevBuf<int> pl_cnt;
-  // C-side communicator of sharded frames (emap_comm_init): NCCL, loaded at run time
-  void* nccl_comm = nullptr;
-  int comm_rank = 0, comm_nranks = 1;
-  // semantic point-channel fusion (emap_semantic_configure): caller-owned layers, library-owned per-frame sums
-  SemCfg sem{};
-  float* sem_map = nullptr;        // (n_layers, W, W) fp32, device, caller-owned
-  DevBuf<i64> sem_fsum;            // one 2^-32 fixed-point sum plane per averaged channel
-  DevBuf<u32> sem_csum;            // r, g, b, count planes per colour channel
-  // class_max scratch (SemMax): per-cell words (cnt, off, occ), control words + bitmaps + U list, the per-record table
-  DevBuf<u32> cm_cell, cm_ctl, cm_key, cm_flag;
-  DevBuf<i64> cm_sum;
-  // inpainting scratch (allocated on first use): one block, carved by inpaint_scratch
-  DevBuf<char> ip_block;
-  int ip_grid = 0;
-  // polygon safety check scratch (allocated on first use, grown to the largest call): one device block carved by
-  // carve_polygon, and its pinned host staging (the upload region on the way in, the read-back region on the way out)
-  DevBuf<char> pg_block;
-  PolySizes pg_cap{};
-  PinnedBuf<char> pg_host;
-  // features_pca scratch (allocated on first use): one device block carved by carve_pca
-  DevBuf<char> pca_block;
-  // emap_input_image with a host image (allocated on first use)
-  StagedUpload img_up;
-  // emap_get_map_points / emap_get_normal_arrows (allocated on first use): the count and offset tables, the kept cells'
-  // payload (grown to the largest call) and a pinned word for the count
-  DevBuf<int> mc_table;
-  DevBuf<char> mc_out;
-  PinnedBuf<int> mc_count_host;
-  // emap_initialize_map's arrays (allocated on first use)
-  StagedUpload init_up;
-  // misc
-  int64_t launches = 0;
-  int count_rays = 0;
-  int timing = 0;
-  StageTimer st;
-  float stage_ms[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-};
-
-namespace {
-
-#define CK(call)                                                                          \
-  do {                                                                                    \
-    cudaError_t e_ = (call);                                                              \
-    if (e_ != cudaSuccess) {                                                              \
-      h->err = std::string(#call) + ": " + cudaGetErrorString(e_);                        \
-      return EMAP_ERR_CUDA;                                                               \
-    }                                                                                     \
-  } while (0)
-
-#define LAUNCH_CHECK()                                                                    \
-  do {                                                                                    \
-    h->launches++;                                                                        \
-    cudaError_t e_ = cudaGetLastError();                                                  \
-    if (e_ != cudaSuccess) {                                                              \
-      h->err = std::string("kernel launch: ") + cudaGetErrorString(e_);                   \
-      return EMAP_ERR_CUDA;                                                               \
-    }                                                                                     \
-  } while (0)
-
-// launch with programmatic stream serialisation (PDL), see pdl_trigger / pdl_wait in emap_kernels.cuh
-template <typename... KArgs, typename... Args>
-cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-  cudaLaunchAttribute at[1];
-  at[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  at[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = at; cfg.numAttrs = 1;
-  return cudaLaunchKernelEx(&cfg, kern, KArgs(std::forward<Args>(args))...);
-}
-#define PDL(kern, grid, block, smem, ...)                                                         \
-  do {                                                                                            \
-    cudaError_t le_ = launch_pdl(kern, dim3(grid), dim3(block), (size_t)(smem), h->stream, __VA_ARGS__); \
-    if (le_ != cudaSuccess) { h->err = std::string("kernel launch: ") + cudaGetErrorString(le_); return EMAP_ERR_CUDA; } \
-  } while (0)
-
-// plain launch of a per-cell kernel (one thread per map cell) on the handle's stream
-#define PER_CELL(kern, ...)                                                                       \
-  do {                                                                                            \
-    kern<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(__VA_ARGS__);                                 \
-    LAUNCH_CHECK();                                                                               \
-  } while (0)
-
-inline int cdiv(i64 a, int b) { return (int)((a + b - 1) / b); }
-
-int fail(emap_handle* h, int code, const char* msg) {
-  if (h) h->err = msg;
-  return code;
-}
-
-void make_pose(const float* R, const float* t_rel, Pose* q) {
-  for (int i = 0; i < 9; i++) q->R16[i] = h16_host(R[i]);
-  for (int i = 0; i < 3; i++) { q->t16[i] = h16_host(t_rel[i]); q->t[i] = t_rel[i]; }
-}
-
-// Makes b hold at least n elements.  A smaller buffer is replaced by one of n + slack elements (zero-filled on the
-// handle's stream if `zero`), once every stream of the handle is idle: no queued kernel or copy still uses the old one.
-template <typename T>
-int grow(emap_handle* h, DevBuf<T>& b, size_t n, size_t slack, bool zero) {
-  if (n <= b.size()) return 0;
-  CK(cudaStreamSynchronize(h->stream));
-  CK(cudaStreamSynchronize(h->copy_stream));
-  CK(cudaStreamSynchronize(h->side_stream));
-  CK(b.alloc(n + slack));
-  if (zero) CK(cudaMemsetAsync(b, 0, sizeof(T) * b.size(), h->stream));
-  return 0;
-}
-
-// Waits only for the previous upload (a staged event that was never recorded is complete) and when a buffer grows.
-int StagedUpload::room(emap_handle* h, size_t n) {
-  CK(cudaEventSynchronize(staged));
-  if (host.size() < n) CK(host.alloc(n));
-  return grow(h, dev, n, 0, false);
-}
-
-int StagedUpload::send(emap_handle* h, size_t n) {
-  CK(cudaMemcpyAsync(dev, host, n, cudaMemcpyHostToDevice, h->stream));
-  CK(cudaEventRecord(staged, h->stream));
-  return 0;
-}
-
-// Sequential carving of one device block into 256-byte aligned arrays (`align` bytes: packed behind the previous one).
-// With a null base only the size is added up.
-struct Carver {
-  uintptr_t base;
-  size_t bytes = 0;
-  template <typename T>
-  T* take(size_t n, size_t align = 256) {
-    T* p = (T*)(base + bytes);
-    bytes = (bytes + sizeof(T) * n + align - 1) & ~(align - 1);
-    return p;
-  }
-};
-
-// The per-cell exchange scratch of a frame, one block: what the ranks of a sharded frame reduce.  Carves the block at
-// `base` into sc's exchanged arrays and fs; returns its size.
-size_t carve_exchange(size_t C, void* base, CellScratch& sc, FrameScalars*& fs) {
-  Carver b{(uintptr_t)base};
-  sc.cnt_ai = b.take<u64>(C, 8); sc.cnt_fo = b.take<u64>(C, 8); sc.n_ray = b.take<u32>(C);
-  sc.SH = b.take<i64>(C, 8); sc.SV = b.take<i64>(C, 8); sc.DV = b.take<i64>(C);
-  sc.last = b.take<u64>(C);
-  sc.rec = b.take<uint2>(C);
-  sc.ukv = b.take<u32>(C);
-  fs = b.take<FrameScalars>(1);
-  return b.bytes;
-}
-
-size_t exchange_bytes(size_t C) {
-  CellScratch sc;
-  FrameScalars* fs;
-  return carve_exchange(C, nullptr, sc, fs);
-}
-
-// Moves the exchange scratch of h to `base` in its between-frames state: all zero, upper-bound keys UKEY_NONE.
-cudaError_t place_exchange(emap_handle* h, void* base) {
-  const size_t C = (size_t)h->dc.C;
-  carve_exchange(C, base, h->sc, h->fs);
-  cudaError_t e = cudaMemsetAsync(base, 0, exchange_bytes(C), h->stream);
-  if (e == cudaSuccess) e = cudaMemsetAsync(h->sc.ukv, 0xff, sizeof(u32) * C, h->stream);
-  return e;
-}
-
-// The inpainting scratch of a W x W map, one block; N = (W + 2)^2 padded pixels.
-struct InpaintScratch {
-  InpaintView v;
-  int* heap[2];
-  int* children;
-  InpaintCtl* ctl;
-  size_t bytes;
-};
-
-InpaintScratch inpaint_scratch(int W, void* base) {
-  const size_t N = (size_t)(W + 2) * (W + 2);
-  Carver b{(uintptr_t)base};
-  InpaintScratch s;
-  s.v.rows = s.v.cols = W + 2;
-  s.v.f = b.take<uint8_t>(N); s.v.ck = b.take<uint8_t>(N); s.v.vc[0] = b.take<uint8_t>(N); s.v.vc[1] = b.take<uint8_t>(N);
-  s.v.img = b.take<uint8_t>((size_t)W * W);
-  s.v.T = b.take<float>(N); s.v.Tc[0] = b.take<float>(N); s.v.Tc[1] = b.take<float>(N);
-  s.v.ord = b.take<uint32_t>(N);
-  s.heap[0] = b.take<int>(N); s.heap[1] = b.take<int>(N); s.children = b.take<int>(N);
-  s.ctl = b.take<InpaintCtl>(1);
-  s.v.em = b.take<uint32_t>(N);
-  s.bytes = b.bytes;
-  return s;
-}
-
-// NVTX range around the launches of one frame stage (visible in nsys / ncu timelines; a no-op without a tool attached)
-struct NvtxRange {
-  explicit NvtxRange(const char* name) { nvtxRangePushA(name); }
-  ~NvtxRange() { nvtxRangePop(); }
-};
-
-int stage_mark(emap_handle* h, int k) {
-  if (!h->timing) return 0;
-  CK(cudaEventRecord(h->st.ev[k], h->stream));
-  return 0;
-}
-
-template <typename Src>
-int launch_index(emap_handle* h, const Src& src, int s) {
-  const i64 n = h->in.n[s], off = h->offs[s];
-  if (n <= 0) return 0;
-  PDL(k_index_error<Src>, cdiv(n, 256), 256, 0, h->dc, h->poses[s], src, n, h->xyzv + off, h->pidx + off,
-      (const float*)h->map, h->sc, h->fs, h->rays + off, h->ray_ctl + RC_CTL * s, (const unsigned short*)h->step_cnt);
-  LAUNCH_CHECK();
-  return 0;
-}
 
 // Makes the frame's buffers readable by its kernels at readable[k], and points the depth cameras there.  Device
 // memory is read in place.  Host buffers that are all page-locked (cudaHostAlloc / cudaHostRegister / torch pin_memory)
@@ -463,6 +66,59 @@ int FrameInput::wait_free(emap_handle* h) {
   CK(cudaStreamIsCapturing(h->stream, &cs));
   if (cs == cudaStreamCaptureStatusNone) CK(cudaEventSynchronize(res == STAGED ? copied : host_free));
   held = false;
+  return 0;
+}
+
+namespace {
+
+thread_local std::string g_create_error;
+
+void make_pose(const float* R, const float* t_rel, Pose* q) {
+  for (int i = 0; i < 9; i++) q->R16[i] = h16_host(R[i]);
+  for (int i = 0; i < 3; i++) { q->t16[i] = h16_host(t_rel[i]); q->t[i] = t_rel[i]; }
+}
+
+// The per-cell exchange scratch of a frame, one block: what the ranks of a sharded frame reduce.  Carves the block at
+// `base` into sc's exchanged arrays and fs; returns its size.
+size_t carve_exchange(size_t C, void* base, CellScratch& sc, FrameScalars*& fs) {
+  Carver b{(uintptr_t)base};
+  sc.cnt_ai = b.take<u64>(C, 8); sc.cnt_fo = b.take<u64>(C, 8); sc.n_ray = b.take<u32>(C);
+  sc.SH = b.take<i64>(C, 8); sc.SV = b.take<i64>(C, 8); sc.DV = b.take<i64>(C);
+  sc.last = b.take<u64>(C);
+  sc.rec = b.take<uint2>(C);
+  sc.ukv = b.take<u32>(C);
+  fs = b.take<FrameScalars>(1);
+  return b.bytes;
+}
+
+size_t exchange_bytes(size_t C) {
+  CellScratch sc;
+  FrameScalars* fs;
+  return carve_exchange(C, nullptr, sc, fs);
+}
+
+// Moves the exchange scratch of h to `base` in its between-frames state: all zero, upper-bound keys UKEY_NONE.
+cudaError_t place_exchange(emap_handle* h, void* base) {
+  const size_t C = (size_t)h->dc.C;
+  carve_exchange(C, base, h->sc, h->fs);
+  cudaError_t e = cudaMemsetAsync(base, 0, exchange_bytes(C), h->stream);
+  if (e == cudaSuccess) e = cudaMemsetAsync(h->sc.ukv, 0xff, sizeof(u32) * C, h->stream);
+  return e;
+}
+
+int stage_mark(emap_handle* h, int k) {
+  if (!h->timing) return 0;
+  CK(cudaEventRecord(h->st.ev[k], h->stream));
+  return 0;
+}
+
+template <typename Src>
+int launch_index(emap_handle* h, const Src& src, int s) {
+  const i64 n = h->in.n[s], off = h->offs[s];
+  if (n <= 0) return 0;
+  PDL(k_index_error<Src>, cdiv(n, 256), 256, 0, h->dc, h->poses[s], src, n, h->xyzv + off, h->pidx + off,
+      (const float*)h->map, h->sc, h->fs, h->rays + off, h->ray_ctl + RC_CTL * s, (const unsigned short*)h->step_cnt);
+  LAUNCH_CHECK();
   return 0;
 }
 
@@ -724,47 +380,6 @@ int frame_finish(emap_handle* h) {
   h->progress = Progress::IDLE;
   return 0;
 }
-
-int layer_index(const char* name) {
-  static const char* names[] = {"elevation", "variance", "is_valid", "traversability", "time", "upper_bound", "is_upper_bound"};
-  for (int i = 0; i < 7; i++) if (!strcmp(name, names[i])) return i;
-  return -1;
-}
-
-int alloc_plugin_scratch(emap_handle* h) {
-  for (int i = 0; i < 4; i++) {
-    int rc = grow(h, h->pl[i], h->dc.C, 0, false);
-    if (rc) return rc;
-  }
-  return 0;
-}
-
-// emap_min_filter / emap_max_filter: `iteration_n` Jacobi passes ping-ponging between two plane pairs, then the select
-template <bool MAX>
-int minmax_filter(emap_handle* h, const float* elevation, const float* is_valid, float* out, int32_t k, int32_t iteration_n,
-                  int32_t* iterations_run) {
-  if (!elevation || !is_valid || !out || k < 0 || k > 16 || iteration_n < 1)
-    return fail(h, EMAP_ERR_INVALID, "emap_min_filter: bad argument");
-  int rc;
-  if ((rc = alloc_plugin_scratch(h)) || (rc = grow(h, h->pl_cnt, (size_t)iteration_n + 1, 0, false))) return rc;
-  const size_t B = sizeof(float) * (size_t)h->dc.C;
-  float *hA = h->pl[0], *mA = h->pl[1], *hB = h->pl[2], *mB = h->pl[3];
-  CK(cudaMemsetAsync(h->pl_cnt, 0, sizeof(int) * (iteration_n + 1), h->stream));
-  CK(cudaMemcpyAsync(hA, elevation, B, cudaMemcpyDeviceToDevice, h->stream));      // min_filter.py:105-106
-  CK(cudaMemcpyAsync(mA, is_valid, B, cudaMemcpyDeviceToDevice, h->stream));
-  for (int it = 0; it < iteration_n; it++) {
-    const bool even = (it & 1) == 0;
-    PER_CELL(k_fill_filter_iter<MAX>, h->dc, k, is_valid, even ? hA : hB, even ? mA : mB, even ? hB : hA, even ? mB : mA,
-             h->pl_cnt, it);
-  }
-  PER_CELL(k_min_filter_final, h->dc, hA, mA, hB, mB, h->pl_cnt, iteration_n, out, h->pl_cnt + iteration_n);
-  if (iterations_run) {
-    CK(cudaMemcpyAsync(iterations_run, h->pl_cnt + iteration_n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-  }
-  return EMAP_OK;
-}
-
 // upper-bound keys of a sharded frame (NCCL mode): u32 keys <-> the s32 order an int32 MIN all-reduce needs
 __global__ void k_ukey_extract(int C, const u32* __restrict__ ukv, int* __restrict__ x) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -809,239 +424,6 @@ int shard_finish(emap_handle* h) {
     LAUNCH_CHECK();
   }
   return frame_finish(h);
-}
-
-// export_value's named kinds: kExportNames[k] is kind k, except the last, normal_color (kind EXPORT_KIND_PLANE is a
-// caller plane)
-const char* const kExportNames[] = {"elevation", "variance", "traversability", "time", "upper_bound", "is_upper_bound",
-                                    "normal_x", "normal_y", "normal_z", "normal_color"};
-constexpr int kNumExportNames = sizeof(kExportNames) / sizeof(kExportNames[0]);
-static_assert(kNumExportNames == EXPORT_KIND_PLANE + 1, "kinds 0..8 are named in order, then normal_color");
-inline int export_kind(int name_index) {
-  return name_index == kNumExportNames - 1 ? EXPORT_KIND_NORMAL_COLOR : name_index;
-}
-
-// The n (<= EXPORT_MAX_LAYERS) layers of an export call.  names[k]: a name of kExportNames, or planes[k] != NULL: a (W,W)
-// device plane exported with flags[k] (bit 0 fill_nan, bit 1 add the centre height).  Returns false, with the message
-// in h->err, for an unknown name.
-bool export_list(emap_handle* h, int32_t n, const char* const* names, const float* const* planes, const int32_t* flags,
-                 ExportList& L) {
-  memset(&L, 0, sizeof(L));
-  L.n = n;
-  for (int k = 0; k < n; k++) {
-    if (planes && planes[k]) {
-      L.kind[k] = EXPORT_KIND_PLANE; L.plane[k] = planes[k]; L.flags[k] = flags ? flags[k] : 0;
-      continue;
-    }
-    int kind = -1;
-    if (names && names[k])
-      for (int i = 0; i < kNumExportNames; i++) if (!strcmp(names[k], kExportNames[i])) kind = export_kind(i);
-    if (kind < 0) { h->err = std::string("Layer ") + (names && names[k] ? names[k] : "(null)") + " is not in the map"; return false; }
-    L.kind[k] = kind;
-  }
-  return true;
-}
-
-// Layers by one k_export_multi launch, one device-to-host copy and one synchronisation (layers as export_list).
-int export_layers(emap_handle* h, int32_t n, const char* const* names, const float* const* planes, const int32_t* flags,
-                  float* out_host, int64_t n_out_total) {
-  if (n < 1 || n > EXPORT_MAX_LAYERS || !out_host) return fail(h, EMAP_ERR_INVALID, "emap_get_layers: 1..24 layers, non-null output");
-  const int Wo = h->dc.W - 2;
-  const size_t per = (size_t)Wo * Wo;
-  if (n_out_total != (int64_t)(per * n)) return fail(h, EMAP_ERR_INVALID, "output must hold n * (cell_n-2)^2 floats");
-  ExportList L;
-  if (!export_list(h, n, names, planes, flags, L)) return EMAP_ERR_NOLAYER;
-  int rc = grow(h, h->d_export, per * n, 0, false);
-  if (rc) return rc;
-  const auto kern = export_has_colour(L) ? k_export_multi<true> : k_export_multi<false>;
-  kern<<<dim3(cdiv((i64)per, 256), n), 256, 0, h->stream>>>(h->dc, h->map, h->normal, h->d_export, L, h->center[2],
-                                                             h->cfg.use_only_above_for_upper_bound);
-  LAUNCH_CHECK();
-  CK(cudaMemcpyAsync(out_host, h->d_export, sizeof(float) * per * n, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return EMAP_OK;
-}
-
-// emap_get_map_points (ARROWS false) / emap_get_normal_arrows (true): the count pass and the scan, one synchronisation
-// for the total; then, if the caller's capacity holds it, the write pass, the payload's copies and one more
-// synchronisation.  Nothing reaches the caller's rows when the capacity is too small.
-template <bool ARROWS>
-int map_cloud(emap_handle* h, int64_t* n_rows, float* xyz, int32_t* ids, double* seg) {
-  const int Wo = h->dc.W - 2;
-  const int n_chunks = cdiv(Wo, MC_TILE), n_tiles = cdiv(Wo, MC_TILE);
-  const int n = Wo * n_chunks, span = MC_TILE * n_chunks;      // count entries; entries of one scan CTA
-  static_assert(MC_TILE % 4 == 0, "k_mapcloud_scan reads whole spans as int4");
-  // cell_n <= 2049 (emap_create): at most 64 chunks, a span of at most 2048 entries, two per scan thread
-  if (span > 2 * 1024) return fail(h, EMAP_ERR_INVALID, "map point cloud: cell_n too large for k_mapcloud_scan");
-  int rc = grow(h, h->mc_table, 2 * (size_t)n + 1, 0, false);
-  if (rc) return rc;
-  if (!h->mc_count_host) CK(h->mc_count_host.alloc(1));
-  int* cnt = h->mc_table;
-  int* off = cnt + n;
-  const dim3 grid(n_tiles, n_chunks);
-  const MapCloudGeom g = {(double)h->center[0], (double)h->center[1], h->cfg.resolution};
-  MapCloudOut o = {nullptr, nullptr, nullptr};
-  k_mapcloud<ARROWS, false><<<grid, MC_THREADS, 0, h->stream>>>(h->dc, h->map, h->normal, h->center[2], cnt, nullptr, g, o);
-  LAUNCH_CHECK();
-  k_mapcloud_scan<<<cdiv(n, span), 1024, 0, h->stream>>>(cnt, off, n, span);
-  LAUNCH_CHECK();
-  CK(cudaMemcpyAsync(h->mc_count_host, off + n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  const int64_t total = *h->mc_count_host;
-  if (total > *n_rows) {
-    *n_rows = total;
-    return fail(h, EMAP_ERR_INVALID, "map point cloud: capacity too small (needed rows in the count argument)");
-  }
-  *n_rows = total;
-  if (!total) return EMAP_OK;
-  const size_t id_bytes = ARROWS ? (sizeof(int32_t) * (size_t)total + 255) & ~(size_t)255 : 0;
-  const size_t row_bytes = ARROWS ? 6 * sizeof(double) : 3 * sizeof(float);
-  rc = grow(h, h->mc_out, id_bytes + row_bytes * (size_t)total, 0, false);
-  if (rc) return rc;
-  char* base = h->mc_out;
-  o.xyz = (float*)base; o.ids = (int32_t*)base; o.seg = (double*)(base + id_bytes);
-  k_mapcloud<ARROWS, true><<<grid, MC_THREADS, 0, h->stream>>>(h->dc, h->map, h->normal, h->center[2], cnt, off, g, o);
-  LAUNCH_CHECK();
-  if (ARROWS) {
-    CK(cudaMemcpyAsync(ids, o.ids, sizeof(int32_t) * total, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaMemcpyAsync(seg, o.seg, 6 * sizeof(double) * total, cudaMemcpyDeviceToHost, h->stream));
-  } else {
-    CK(cudaMemcpyAsync(xyz, o.xyz, 3 * sizeof(float) * total, cudaMemcpyDeviceToHost, h->stream));
-  }
-  CK(cudaStreamSynchronize(h->stream));
-  return EMAP_OK;
-}
-
-// ---- polygon safety check --------------------------------------------------------------------
-constexpr int kRingHead = 256;     // ring vertices of a single call read back with its result
-constexpr size_t kBatchRingHead = 4096;    // ring rows of a batch read back with its results
-// (longer rings take a second copy)
-
-struct PolyScratch {
-  char* up;                        // upload region: poison counts, descriptors, clipped vertices (PolyStage)
-  PolyPartial* part;               // one per k_polygon work item
-  int *col_min, *col_max;          // the polygons' column windows, back to back
-  char* down;                      // read-back region: one PolyResult per polygon, then the rings (PolyStage)
-};
-
-// One call's layout of the upload and read-back regions, the same in device and in pinned host memory, so that each
-// region moves in one copy.  The two poison counts sit at offset 0 of the upload, the results at offset 0 of the read-back.
-struct PolyStage {
-  size_t desc, xy, up_bytes;
-  size_t ring, down_bytes;
-};
-
-PolyStage poly_stage(size_t n_poly, size_t n_vert, size_t ring_rows) {
-  PolyStage s;
-  s.desc = 16;
-  s.xy = s.desc + sizeof(PolyDesc) * n_poly;
-  s.up_bytes = s.xy + sizeof(float2) * n_vert;
-  s.ring = sizeof(PolyResult) * n_poly;
-  s.down_bytes = s.ring + sizeof(double2) * ring_rows;
-  return s;
-}
-
-dim3 polygon_grid(int W) { return dim3(cdiv(W, PG_COLS), cdiv(W, PG_ROWS)); }
-size_t ring_capacity(int W) { return 2 * (size_t)(W - 2) + 1; }
-
-size_t carve_polygon(const PolySizes& z, void* base, PolyScratch& s) {
-  Carver b{(uintptr_t)base};
-  s.up = b.take<char>(z.up);
-  s.part = b.take<PolyPartial>(z.items);
-  s.col_min = b.take<int>(z.cols);
-  s.col_max = b.take<int>(z.cols);
-  s.down = b.take<char>(z.down);
-  return b.bytes;
-}
-
-// Carves the scratch of a call of sizes z, growing the device block and the pinned staging (upload region, then
-// read-back region) to the largest call so far.
-int alloc_polygon_scratch(emap_handle* h, const PolySizes& z, PolyScratch& s) {
-  PolySizes& c = h->pg_cap;
-  if (!h->pg_block || z.up > c.up || z.items > c.items || z.cols > c.cols || z.down > c.down) {
-    // the read-back region follows the upload region in pinned memory: keep it aligned for its double2 rings
-    c.up = std::max(c.up, (z.up + 255) & ~(size_t)255); c.items = std::max(c.items, z.items);
-    c.cols = std::max(c.cols, z.cols); c.down = std::max(c.down, z.down);
-    CK(h->pg_block.alloc(carve_polygon(c, nullptr, s)));
-    carve_polygon(c, h->pg_block, s);
-    CK(cudaMemsetAsync(s.col_min, 0x7f, sizeof(int) * c.cols, h->stream));    // "no cell yet": k_hull restores it
-    CK(cudaMemsetAsync(s.col_max, 0xff, sizeof(int) * c.cols, h->stream));
-  }
-  if (h->pg_host.size() < c.up + c.down) CK(h->pg_host.alloc(c.up + c.down));
-  carve_polygon(c, h->pg_block, s);
-  return 0;
-}
-
-// The device part of a call whose n_poly polygons (n_items work items) are staged in the upload region of h->pg_host:
-// one upload copy, k_poly_poison (with `poison`), k_polygon, k_hull, one copy of the results and the first `head` ring
-// rows into the read-back region of h->pg_host, one synchronisation; one more copy and synchronisation only if a ring
-// ends beyond `head`.
-int run_polygons(emap_handle* h, const PolyScratch& s, const PolyStage& st, int n_poly, int n_items, bool poison,
-                 const float* checker_plane, double safe_thresh, double safe_min_thresh, int32_t max_unsafe_n,
-                 float* mask, bool hulls, size_t head) {
-  const int W = h->dc.W;
-  const size_t C = (size_t)h->dc.C;
-  const dim3 g = polygon_grid(W);
-  const float* valid = h->map + L_VALID * C;
-  const float* checker = checker_plane ? checker_plane : h->map + L_TRAV * C;
-  PolyArgs a;
-  a.poly = (const PolyDesc*)(s.up + st.desc); a.n_poly = n_poly; a.xy = (const float2*)(s.up + st.xy);
-  a.cx = h->center[0]; a.cy = h->center[1];
-  a.thr_over = (float)(1.0 - safe_thresh); a.thr_max = (float)(1.0 - safe_min_thresh);    // traversability_polygon.py:25-26
-  a.max_unsafe_n = max_unsafe_n;
-  a.poison = poison ? (const int*)s.up : nullptr;
-  memcpy(&a.one, h->pg_host + st.desc, sizeof(PolyDesc));
-  CK(cudaMemcpyAsync(s.up, h->pg_host, st.up_bytes, cudaMemcpyHostToDevice, h->stream));
-  if (poison) {
-    k_poly_poison<<<std::min(cdiv((i64)C, 256), 4 * h->n_sm), 256, 0, h->stream>>>(W, valid, checker, (int*)s.up);
-    LAUNCH_CHECK();
-  }
-  (poison ? k_polygon<true> : k_polygon<false>)<<<n_items, PG_THREADS, 0, h->stream>>>(
-      W, h->dc.res_f, a, valid, checker, mask, s.part, hulls ? s.col_min : nullptr, hulls ? s.col_max : nullptr);
-  LAUNCH_CHECK();
-  k_hull<<<n_poly, HULL_THREADS, 0, h->stream>>>(W, h->cfg.resolution, a, (int)g.x, (int)g.y, s.part, s.col_min,
-                                                 s.col_max, (PolyResult*)s.down,
-                                                 hulls ? (double2*)(s.down + st.ring) : nullptr);
-  LAUNCH_CHECK();
-  char* back = h->pg_host + h->pg_cap.up;
-  head = std::min(head, (st.down_bytes - st.ring) / sizeof(double2));
-  CK(cudaMemcpyAsync(back, s.down, st.ring + sizeof(double2) * head, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  const PolyResult* r = (const PolyResult*)back;
-  const PolyDesc* d = (const PolyDesc*)(h->pg_host + st.desc);
-  size_t end = 0;
-  for (int i = 0; i < n_poly; i++)
-    if (r[i].n_ring) end = std::max(end, (size_t)d[i].ring_off + r[i].n_ring);
-  if (end > head) {
-    const size_t off = st.ring + sizeof(double2) * head;
-    CK(cudaMemcpyAsync(back + off, s.down + off, sizeof(double2) * (end - head), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-  }
-  return EMAP_OK;
-}
-
-// ---- features_pca ------------------------------------------------------------------------------
-struct PcaScratch {
-  PcaResult* res;
-  double* part;                    // pca_entries(PCA_MAX_F) per k_pca_stats CTA
-  double* proj;                    // 3 planes of C projections
-};
-
-int pca_stats_grid(emap_handle* h) { return std::min(cdiv(h->dc.C, 32), 2 * h->n_sm); }   // 32 <= tile cells
-
-size_t carve_pca(emap_handle* h, void* base, PcaScratch& s) {
-  Carver b{(uintptr_t)base};
-  s.res = b.take<PcaResult>(1);
-  s.part = b.take<double>((size_t)pca_stats_grid(h) * PCA_MAX_ENTRIES);
-  s.proj = b.take<double>(3 * (size_t)h->dc.C);
-  return b.bytes;
-}
-
-// the planes of a semantic plugin call: a non-null host array of n non-null device pointers
-bool planes_ok(int32_t n, const float* const* planes) {
-  if (n > 0 && !planes) return false;
-  for (int l = 0; l < n; l++) if (!planes[l]) return false;
-  return true;
 }
 
 }  // namespace
@@ -1153,27 +535,9 @@ emap_handle::~emap_handle() {
   comm_release(this);
 }
 
-// EM.py:119-128 clear
 int clear_map(emap_handle* h) {
   PER_CELL(k_clear, h->dc, h->map);
   CK(cudaMemsetAsync(&h->fs->mean_error, 0, 2 * sizeof(float), h->stream));     // EM.py:127-128
-  return EMAP_OK;
-}
-
-// EM.py:913-922 after the interpolation: `iterations` Jacobi passes of the initialiser dilation, then
-// upper_bound <- elevation on valid cells
-int initialize_finish(emap_handle* h, int32_t dilation_size, int32_t iterations) {
-  if (dilation_size < 0 || dilation_size > 64 || iterations < 0 || iterations > 16)
-    return fail(h, EMAP_ERR_INVALID, "emap_initialize_map_finish: 0 <= dilation_size <= 64, 0 <= iterations <= 16");
-  int rc = alloc_plugin_scratch(h);
-  if (rc) return rc;
-  const size_t B = sizeof(float) * (size_t)h->dc.C;
-  const int passes = dilation_size > 0 ? iterations : 0;
-  for (int it = 0; it < std::max(passes, 1); it++) {
-    CK(cudaMemcpyAsync(h->pl[0], h->map, B, cudaMemcpyDeviceToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->pl[1], h->map + 2 * (size_t)h->dc.C, B, cudaMemcpyDeviceToDevice, h->stream));
-    PER_CELL(k_init_dilate, h->dc, h->pl[0], h->pl[1], h->map, passes ? dilation_size : 0, it == std::max(passes, 1) - 1);
-  }
   return EMAP_OK;
 }
 
@@ -1187,14 +551,6 @@ int frame_run(emap_handle* h) {
 }
 
 extern "C" {
-
-#define ENTER(h)                                               \
-  if (!(h)) return EMAP_ERR_INVALID;                           \
-  std::lock_guard<std::mutex> lock_((h)->mu);                  \
-  {                                                            \
-    cudaError_t e_ = cudaSetDevice((h)->device);               \
-    if (e_ != cudaSuccess) { (h)->err = cudaGetErrorString(e_); return EMAP_ERR_CUDA; } \
-  }
 
 int emap_set_traversability_weights(emap_handle* h, const float* w1, const float* w2, const float* w3, const float* w_out) {
   ENTER(h);
@@ -1609,741 +965,9 @@ int emap_update_normal(emap_handle* h, const float* dilated) {
   PER_CELL(k_normal, h->dc, dilated ? dilated : h->trav_input, h->map + 2 * (size_t)h->dc.C, h->normal);
   return EMAP_OK;
 }
-
-// EM.py:913-922: the device half of initialize_map, after the caller wrote the interpolated planes (emap_set_state):
-// `iterations` Jacobi passes of the initialiser dilation, then upper_bound <- elevation on valid cells.
-int emap_initialize_map_finish(emap_handle* h, int32_t dilation_size, int32_t iterations) {
-  ENTER(h);
-  return initialize_finish(h, dilation_size, iterations);
-}
-
-// EM.py:899-922 + map_initializer.py:25-62 on the device (include/emap.h, csrc/emap_initialize.cuh): clear, snap, the
-// host part (triangulation, gradients, coefficients, tile lists), one upload, one interpolation kernel, then the
-// dilation passes and the upper-bound fill of emap_initialize_map_finish.
-int emap_initialize_map(emap_handle* h, const float* xyz_host, int32_t n_points, int32_t method,
-                        const int32_t* triangles_host, int32_t n_triangles, const double* gradients_host,
-                        double initialized_variance, int32_t dilation_size_initialize) {
-  ENTER(h);
-  NvtxRange nv("emap:initialize_map");
-  int rc = clear_map(h);                 // EM.py:906: every failure below leaves the map cleared
-  if (rc) return rc;
-  if (!xyz_host) return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: null points");
-  if (n_points <= 3) return fail(h, EMAP_ERR_INVALID, "Initialization points must be more than 3.");
-  if (n_points > EMAP_INIT_MAX_POINTS)
-    return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: more than EMAP_INIT_MAX_POINTS points");
-  if (method < 0 || method > 2) return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: method must be 0 (nearest), 1 (linear) or 2 (cubic)");
-  if (triangles_host && (n_triangles < 1 || n_triangles > 2 * EMAP_INIT_MAX_POINTS))
-    return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: 1 to 2 * EMAP_INIT_MAX_POINTS triangles required");
-  if (dilation_size_initialize < 0 || dilation_size_initialize > 64 || !std::isfinite(initialized_variance))
-    return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: 0 <= dilation_size_initialize <= 64 and a finite variance required");
-  // transform_to_map_index as elevation_mapping.py applies it, in fp32: ((xy - center) / res + W / 2), truncated
-  const int W = h->dc.W, n = n_points;
-  const float res_f = (float)h->cfg.resolution, half_f = (float)(0.5 * W);
-  std::vector<long long> xy(2 * (size_t)n);
-  std::vector<double> z(n);
-  bool narrow = true;
-  for (int i = 0; i < n; i++) {
-    const float* q = xyz_host + 3 * (size_t)i;
-    if (!std::isfinite(q[0]) || !std::isfinite(q[1]) || !std::isfinite(q[2]))
-      return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: non-finite point");
-    for (int d = 0; d < 2; d++) {
-      const float v = (q[d] - h->center[d]) / res_f;
-      const float c = v + half_f;
-      if (!(c >= -2147483648.f && c < 2147483648.f))
-        return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: a point's cell index is outside the int32 range");
-      xy[2 * i + d] = (long long)(int32_t)c;
-      narrow &= std::llabs(xy[2 * i + d]) <= INIT_NARROW;
-    }
-    z[i] = (double)(float)(q[2] - h->center[2]);
-  }
-  InitArgs a;
-  memset(&a, 0, sizeof(a));
-  a.W = W; a.C = h->dc.C; a.tiles_x = (W + INIT_TILE - 1) / INIT_TILE;
-  a.var = (float)initialized_variance;
-  // the upload: one block, 256-byte aligned arrays, the same layout in pinned and in device memory
-  std::vector<int> tri, nb, off, list;
-  std::vector<double> grad, coef;
-  Carver up{0};           // base 0: take() returns byte offsets
-  size_t o_pxy = 0, o_pz = 0, o_txy = 0, o_coef = 0, o_off = 0, o_list = 0;
-  if (method == 0) {
-    a.n = n;
-    o_pxy = (size_t)up.take<int2>(n);
-    o_pz = (size_t)up.take<float>(n);
-  } else {
-    if (triangles_host) {
-      tri.assign(triangles_host, triangles_host + 3 * (size_t)n_triangles);
-      for (int t = 0; t < n_triangles; t++) {
-        int* v = &tri[3 * (size_t)t];
-        if (v[0] < 0 || v[0] >= n || v[1] < 0 || v[1] >= n || v[2] < 0 || v[2] >= n)
-          return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: triangle index outside [0, n_points)");
-        const int o = init_host::orient_sign(&xy[2 * (size_t)v[0]], &xy[2 * (size_t)v[1]], &xy[2 * (size_t)v[2]]);
-        if (o == 0) return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: a triangle of zero area");
-        if (o < 0) std::swap(v[1], v[2]);
-      }
-    } else if (!init_host::delaunay(xy, tri)) {
-      return fail(h, EMAP_ERR_INVALID, "emap_initialize_map: the points are collinear (no triangulation)");
-    }
-    const int T = (int)(tri.size() / 3);
-    a.n = T;
-    if (method == 2) {
-      init_host::neighbours(tri, nb);
-      if (!gradients_host) init_host::estimate_gradients(xy, z, tri, grad);
-      coef.resize((size_t)INIT_CT * T);
-      init_host::ct_coefficients(xy, z, gradients_host ? gradients_host : grad.data(), tri, nb, coef.data());
-    } else {
-      coef.resize(3 * (size_t)T);
-      for (size_t k = 0; k < coef.size(); k++) coef[k] = z[tri[k]];
-    }
-    init_host::bin_tiles(W, xy, tri, off, list);
-    o_txy = (size_t)up.take<int>(6 * (size_t)T);
-    o_coef = (size_t)up.take<double>(coef.size());
-    o_off = (size_t)up.take<int>(off.size());
-    o_list = (size_t)up.take<int>(std::max<size_t>(list.size(), 1));
-  }
-  if ((rc = h->init_up.room(h, up.bytes))) return rc;
-  char* hb = h->init_up.host;
-  char* db = h->init_up.dev;
-  if (method == 0) {
-    int2* pxy = (int2*)(hb + o_pxy);
-    float* pz = (float*)(hb + o_pz);
-    for (int i = 0; i < n; i++) { pxy[i] = make_int2((int)xy[2 * i], (int)xy[2 * i + 1]); pz[i] = (float)z[i]; }
-    a.pxy = (const int2*)(db + o_pxy); a.pz = (const float*)(db + o_pz);
-  } else {
-    int* txy = (int*)(hb + o_txy);
-    for (size_t k = 0; k < tri.size(); k++) { txy[2 * k] = (int)xy[2 * (size_t)tri[k]]; txy[2 * k + 1] = (int)xy[2 * (size_t)tri[k] + 1]; }
-    memcpy(hb + o_coef, coef.data(), sizeof(double) * coef.size());
-    memcpy(hb + o_off, off.data(), sizeof(int) * off.size());
-    if (!list.empty()) memcpy(hb + o_list, list.data(), sizeof(int) * list.size());
-    a.txy = (const int*)(db + o_txy); a.coef = (const double*)(db + o_coef);
-    a.tile_off = (const int*)(db + o_off); a.tile_tri = (const int*)(db + o_list);
-  }
-  if ((rc = h->init_up.send(h, up.bytes))) return rc;
-  const int grid = a.tiles_x * a.tiles_x;
-  if (method == 0) {
-    if (narrow) k_init_nearest<long long><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
-    else k_init_nearest<__int128><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
-  } else if (method == 1) {
-    if (narrow) k_init_interp<long long, false><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
-    else k_init_interp<__int128, false><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
-  } else {
-    if (narrow) k_init_interp<long long, true><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
-    else k_init_interp<__int128, true><<<grid, INIT_THREADS, 0, h->stream>>>(a, h->map);
-  }
-  LAUNCH_CHECK();
-  return initialize_finish(h, dilation_size_initialize, 2);
-}
-
 int emap_get_position(emap_handle* h, double out[3]) {
   ENTER(h);
   for (int k = 0; k < 3; k++) out[k] = h->center[k];
-  return EMAP_OK;
-}
-
-// ---- export ----------------------------------------------------------------------------------
-int emap_get_map_with_name(emap_handle* h, const char* name, float* out_host, int64_t n_out) {
-  ENTER(h);
-  if (!name || !out_host) return fail(h, EMAP_ERR_INVALID, "null argument");
-  return export_layers(h, 1, &name, nullptr, nullptr, out_host, n_out);
-}
-
-// Several layers in one launch, one device-to-host copy and one synchronisation (WRAP:213-252 get_grid_map exports a list
-// of layers per call).
-int emap_get_layers(emap_handle* h, int32_t n, const char* const* names, const float* const* planes, const int32_t* flags,
-                    float* out_host, int64_t n_out_total) {
-  ENTER(h);
-  return export_layers(h, n, names, planes, flags, out_host, n_out_total);
-}
-
-static_assert(EMAP_SUBMAP_MAX_WINDOWS == SUBMAP_MAX_WINDOWS && EMAP_SUBMAP_MAX_LAYERS == EXPORT_MAX_LAYERS,
-              "emap.h states the kernel's limits");
-
-static bool submap_lengths_ok(int64_t n, const double* windows) {
-  for (int64_t w = 0; w < n; w++)
-    for (int a = 2; a < 4; a++)
-      if (!(std::isfinite(windows[4 * w + a]) && windows[4 * w + a] >= 0.0)) return false;
-  return true;
-}
-
-// The host part of emap_get_submaps on its own (no handle, no device): submap_window for every request.
-int emap_submap_windows(int32_t cell_n, double resolution, const double center[2], int32_t n_windows,
-                        const double* windows, int32_t* info, double* centres) {
-  if (!center || !windows || !info || !centres || cell_n < 3 || !(std::isfinite(resolution) && resolution > 0.0) ||
-      n_windows < 0 || !submap_lengths_ok(n_windows, windows))
-    return EMAP_ERR_INVALID;
-  for (int32_t w = 0; w < n_windows; w++) submap_window(cell_n, resolution, center, windows + 4 * w, info + 5 * w, centres + 2 * w);
-  return EMAP_OK;
-}
-
-// Appends the successful window q = submap_window's info to k_submap's table: its first work item is `tiles` and its
-// first output float `total`, both advanced past it.
-static void submap_add(SubmapArgs& a, int W, const int32_t q[5], int n_layers, int& tiles, long long& total) {
-  SubmapWin& s = a.win[a.n_win++];
-  s.r0 = (int16_t)(W - 2 - q[1]); s.c0 = (int16_t)(W - 2 - q[2]);
-  s.rows = (int16_t)q[3]; s.cols = (int16_t)q[4];
-  s.tile0 = tiles; s.off = total;
-  tiles += cdiv(q[3], SUBMAP_ROWS);
-  total += (long long)n_layers * q[3] * q[4];
-}
-
-// The get_raw_submap service (elevation_mapping_ros.cpp:507-553) for a batch of windows: the windows on the host
-// (submap_window), every (window, layer, row) of the batch in one k_submap launch whose table is its parameters.  Host
-// output: one device-to-host copy and one synchronisation; device output: stream-ordered, no synchronisation.  Every
-// check runs before anything is written or launched.
-int emap_get_submaps(emap_handle* h, int32_t n_windows, const double* windows, int32_t n_layers, const char* const* names,
-                     const float* const* planes_device, const int32_t* flags, float* out, int32_t out_is_device,
-                     int64_t out_floats, int32_t* info, double* centres) {
-  ENTER(h);
-  NvtxRange nv("emap:get_submaps");
-  if (!windows || !names || !out || !info || !centres) return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: null argument");
-  if (n_windows < 1 || n_windows > EMAP_SUBMAP_MAX_WINDOWS)
-    return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: 1 to EMAP_SUBMAP_MAX_WINDOWS windows required");
-  if (n_layers < 1 || n_layers > EMAP_SUBMAP_MAX_LAYERS)
-    return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: 1 to EMAP_SUBMAP_MAX_LAYERS layers required");
-  if (!submap_lengths_ok(n_windows, windows))
-    return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: lengths must be finite and >= 0");
-  SubmapArgs a;
-  if (!export_list(h, n_layers, names, planes_device, flags, a.L)) return EMAP_ERR_INVALID;
-  const int W = h->dc.W;
-  const double m[2] = {h->center[0], h->center[1]};
-  std::vector<int32_t> inf(5 * (size_t)n_windows);
-  std::vector<double> cen(2 * (size_t)n_windows);
-  a.n_win = 0;
-  int tiles = 0;
-  long long total = 0;
-  for (int w = 0; w < n_windows; w++) {
-    const int32_t* q = &inf[5 * w];
-    submap_window(W, h->cfg.resolution, m, windows + 4 * w, &inf[5 * w], &cen[2 * w]);
-    if (q[0]) submap_add(a, W, q, n_layers, tiles, total);
-  }
-  if (total > out_floats)
-    return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: out_floats is below the layers times the windows' cells");
-  memcpy(info, inf.data(), sizeof(int32_t) * inf.size());
-  memcpy(centres, cen.data(), sizeof(double) * cen.size());
-  if (!a.n_win) return EMAP_OK;
-  float* dst = out;
-  if (!out_is_device) {
-    const int rc = grow(h, h->d_export, (size_t)total, 0, false);
-    if (rc) return rc;
-    dst = h->d_export;
-  }
-  const auto kern = export_has_colour(a.L) ? k_submap<true> : k_submap<false>;
-  kern<<<dim3(tiles, n_layers), dim3(32, SUBMAP_ROWS), 0, h->stream>>>(h->dc, h->map, h->normal, dst, a, h->center[2],
-                                                                       h->cfg.use_only_above_for_upper_bound);
-  LAUNCH_CHECK();
-  if (!out_is_device) {
-    CK(cudaMemcpyAsync(out, dst, sizeof(float) * total, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-  }
-  return EMAP_OK;
-}
-
-static_assert(EMAP_TRANSFORM_TOLERANCE == TSUB_ORTHO_TOL && EMAP_TRANSFORMED_WINDOWS_PER_LAUNCH == TSUB_MAX_WINDOWS,
-              "emap.h states the transformed windows' limits");
-
-static bool transforms_ok(int64_t n, const double* transforms) {
-  for (int64_t w = 0; w < n; w++)
-    if (!tsub_transform_ok(transforms + 12 * w)) return false;
-  return true;
-}
-
-// The host part of emap_get_transformed_submaps on its own (no handle, no device): transformed_window for every request.
-int emap_transformed_submap_windows(int32_t cell_n, double resolution, const double center[2], int32_t n_windows,
-                                    const double* windows, const double* transforms, int32_t* info, double* geometry) {
-  if (!center || !windows || !transforms || !info || !geometry || cell_n < 3 ||
-      !(std::isfinite(resolution) && resolution > 0.0) || n_windows < 0 || !submap_lengths_ok(n_windows, windows) ||
-      !transforms_ok(n_windows, transforms))
-    return EMAP_ERR_INVALID;
-  for (int32_t w = 0; w < n_windows; w++) {
-    TSubGeom g;
-    transformed_window(cell_n, resolution, center, windows + 4 * w, transforms + 12 * w, g);
-    info[3 * w] = g.win[0]; info[3 * w + 1] = g.size[0]; info[3 * w + 2] = g.size[1];
-    for (int a = 0; a < 2; a++) { geometry[4 * w + a] = g.pos[a]; geometry[4 * w + 2 + a] = g.len[a]; }
-  }
-  return EMAP_OK;
-}
-
-// get_raw_submap with a request frame other than the map frame (elevation_mapping_ros.cpp:507-553 with grid_map's
-// getTransformedMap): the geometry on the host (transformed_window), then per launch of up to TSUB_MAX_WINDOWS windows
-// the two scatter passes and the gather (csrc/emap_submap.cuh), each launch's table in its parameters.  Output, stream
-// and graph rules as emap_get_submaps; every check runs before anything is written or launched.
-int emap_get_transformed_submaps(emap_handle* h, int32_t n_windows, const double* windows, const double* transforms,
-                                 double sample_ratio, int32_t n_layers, const char* const* names,
-                                 const float* const* planes_device, const int32_t* flags, float* out,
-                                 int32_t out_is_device, int64_t out_floats, int32_t* info, double* geometry) {
-  ENTER(h);
-  NvtxRange nv("emap:get_transformed_submaps");
-  if (!windows || !transforms || !names || !out || !info || !geometry)
-    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: null argument");
-  if (n_windows < 1 || n_windows > EMAP_SUBMAP_MAX_WINDOWS)
-    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: 1 to EMAP_SUBMAP_MAX_WINDOWS windows required");
-  if (n_layers < 1 || n_layers > EMAP_SUBMAP_MAX_LAYERS)
-    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: 1 to EMAP_SUBMAP_MAX_LAYERS layers required");
-  if (!submap_lengths_ok(n_windows, windows))
-    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: lengths must be finite and >= 0");
-  if (!transforms_ok(n_windows, transforms))
-    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: a transform is not finite or its R is not "
-                                     "orthonormal within EMAP_TRANSFORM_TOLERANCE");
-  if (!(std::isfinite(sample_ratio) && sample_ratio >= 0.0))
-    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: sample_ratio must be finite and >= 0");
-  ExportList L;
-  if (!export_list(h, n_layers, names, planes_device, flags, L)) return EMAP_ERR_INVALID;
-  const int W = h->dc.W;
-  const double res = h->cfg.resolution;
-  const double m[2] = {h->center[0], h->center[1]};
-  std::vector<TSubGeom> g(n_windows);
-  long long cells = 0;
-  for (int w = 0; w < n_windows; w++) {
-    transformed_window(W, res, m, windows + 4 * w, transforms + 12 * w, g[w]);
-    const long long n = (long long)g[w].size[0] * g[w].size[1];
-    if (n > INT32_MAX - TSUB_THREADS)
-      return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: a new map of 2^31 cells or more");
-    cells += n;
-  }
-  if (n_layers * cells > out_floats)
-    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: out_floats is below the layers times the new maps' cells");
-  for (int w = 0; w < n_windows; w++) {
-    info[3 * w] = g[w].win[0]; info[3 * w + 1] = g[w].size[0]; info[3 * w + 2] = g[w].size[1];
-    for (int a = 0; a < 2; a++) { geometry[4 * w + a] = g[w].pos[a]; geometry[4 * w + 2 + a] = g[w].len[a]; }
-  }
-  if (!cells) return EMAP_OK;
-  int rc;
-  if ((rc = grow(h, h->ts_key1, (size_t)cells, 0, true)) || (rc = grow(h, h->ts_key2, (size_t)cells, 0, true))) return rc;
-  float* dst = out;
-  if (!out_is_device) {
-    if ((rc = grow(h, h->d_export, (size_t)(n_layers * cells), 0, false))) return rc;
-    dst = h->d_export;
-  }
-  const bool colour = export_has_colour(L);
-  TSubArgs a;
-  a.L = L;
-  a.n_samples = sample_ratio > 0.0 ? 5 : 1;
-  a.res = res;
-  a.s = res * sample_ratio;
-  long long cell0 = 0;
-  for (int w0 = 0; w0 < n_windows;) {
-    a.n_win = 0;
-    int blk_src = 0, blk_dst = 0;
-    for (; w0 < n_windows && a.n_win < TSUB_MAX_WINDOWS; w0++) {
-      const TSubGeom& q = g[w0];
-      if (!q.win[0] || !q.size[0] || !q.size[1]) continue;
-      TSubWin& s = a.win[a.n_win++];
-      for (int k = 0; k < 9; k++) s.R[k] = transforms[12 * w0 + k];
-      for (int k = 0; k < 3; k++) s.t[k] = transforms[12 * w0 + 9 + k];
-      s.x0 = q.centre[0] + (0.5 * (q.win[3] * res) - 0.5 * res);
-      s.y0 = q.centre[1] + (0.5 * (q.win[4] * res) - 0.5 * res);
-      for (int k = 0; k < 2; k++) { s.pos[k] = q.pos[k]; s.len[k] = q.len[k]; }
-      s.r0 = (int16_t)(W - 2 - q.win[1]); s.c0 = (int16_t)(W - 2 - q.win[2]);
-      s.rows = (int16_t)q.win[3]; s.cols = (int16_t)q.win[4];
-      s.nrows = q.size[0]; s.ncols = q.size[1];
-      s.blk_src = blk_src; s.blk_dst = blk_dst; s.cell0 = cell0;
-      blk_src += cdiv((i64)q.win[3] * q.win[4], TSUB_THREADS);
-      blk_dst += cdiv((i64)q.size[0] * q.size[1], TSUB_THREADS);
-      cell0 += (long long)q.size[0] * q.size[1];
-    }
-    if (!a.n_win) continue;
-    k_tsub_scatter<1><<<blk_src, TSUB_THREADS, 0, h->stream>>>(h->dc, h->map, h->ts_key1, h->ts_key2, a, h->center[2]);
-    LAUNCH_CHECK();
-    k_tsub_scatter<2><<<blk_src, TSUB_THREADS, 0, h->stream>>>(h->dc, h->map, h->ts_key1, h->ts_key2, a, h->center[2]);
-    LAUNCH_CHECK();
-    const auto gather = colour ? k_tsub_gather<true> : k_tsub_gather<false>;
-    gather<<<blk_dst, TSUB_THREADS, 0, h->stream>>>(h->dc, h->map, h->normal, h->ts_key1, h->ts_key2, dst, a,
-                                                    h->center[2], h->cfg.use_only_above_for_upper_bound);
-    LAUNCH_CHECK();
-  }
-  if (!out_is_device) {
-    CK(cudaMemcpyAsync(out, dst, sizeof(float) * n_layers * cells, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-  }
-  return EMAP_OK;
-}
-
-// ---- plane segmentation of one window (emap_segment_planes, csrc/emap_planes.cuh) ----------------------------------
-
-// The scratch of a window of n cells with `slots` label slots, one block: the window, two image planes (fill / median
-// ping-pong), union-find parents, flags and ranks, fill keys, the planarity masks, scan block sums, the header words,
-// the label statistics and decisions, and the host output's staging (info, plane table, layers).
-namespace {
-
-struct PlaneScratch {
-  float *raw, *img[2];
-  int *parent, *flag, *rank, *lab, *bsum, *hdr, *keep;
-  unsigned* key;
-  unsigned char *bin, *tmp, *bg;
-  unsigned long long* st;
-  int32_t* info;
-  double* planes;
-  float* layers;
-};
-
-size_t carve_planes(int64_t n, int64_t slots, int64_t plane_rows, bool host_out, void* base, PlaneScratch& s) {
-  Carver c{(uintptr_t)base};
-  const int64_t m = std::max(n, slots);
-  s.raw = c.take<float>(n); s.img[0] = c.take<float>(n); s.img[1] = c.take<float>(n);
-  s.parent = c.take<int>(n); s.flag = c.take<int>(m); s.rank = c.take<int>(m); s.lab = c.take<int>(n);
-  s.bsum = c.take<int>(m / PL_SCAN + 1); s.hdr = c.take<int>(8); s.keep = c.take<int>(slots);
-  s.key = c.take<unsigned>(n);
-  s.bin = c.take<unsigned char>(n); s.tmp = c.take<unsigned char>(n); s.bg = c.take<unsigned char>(slots);
-  s.st = c.take<unsigned long long>(slots * PL_STAT);
-  s.info = c.take<int32_t>(host_out ? 8 : 0);
-  s.planes = c.take<double>(host_out ? 7 * plane_rows : 0);
-  s.layers = c.take<float>(host_out ? 4 * n : 0);
-  return c.bytes;
-}
-
-// Raster-order ranks of the n flags in s.flag into s.rank, the count into *total (three launches).
-int plane_scan(emap_handle* h, const PlaneScratch& s, int64_t n, int* total) {
-  const int nb = cdiv(n, PL_SCAN);
-  k_pl_scan_blocks<<<nb, PL_SCAN, 0, h->stream>>>(s.flag, (int)n, s.bsum);
-  LAUNCH_CHECK();
-  k_pl_scan_top<<<1, PL_SCAN, 0, h->stream>>>(s.bsum, nb, total);
-  LAUNCH_CHECK();
-  k_pl_scan_rank<<<nb, PL_SCAN, 0, h->stream>>>(s.flag, (int)n, s.bsum, s.rank);
-  LAUNCH_CHECK();
-  return 0;
-}
-
-// Union-find merge and flatten of the cells whose parent is >= 0.
-int plane_components(emap_handle* h, const PlaneScratch& s, int rows, int cols, int conn8) {
-  const int64_t n = (int64_t)rows * cols;
-  k_pl_uf_merge<<<cdiv(n, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.parent, rows, cols, conn8);
-  LAUNCH_CHECK();
-  k_pl_uf_flatten<<<cdiv(n, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.parent, (int)n);
-  LAUNCH_CHECK();
-  return 0;
-}
-
-}  // namespace
-
-static_assert(EMAP_PLANE_EIGEN_MIN == PL_EIG_MIN, "emap.h states the fit's threshold");
-
-// Why p is rejected (nullptr: accepted) for a map of resolution `res`.
-static const char* plane_params_error(const emap_plane_params& p, double res) {
-  if (p.ransac) return "emap_segment_planes: RANSAC refinement is not supported (ransac must be 0)";
-  const int mk = std::max(1, std::min(p.median_kernel, 5));
-  if (mk != 1 && mk != 3 && mk != 5) return "emap_segment_planes: the median kernel must clamp to 1, 3 or 5";
-  if (p.median_repeats < 0 || p.median_repeats > EMAP_PLANE_MAX_REPEATS)
-    return "emap_segment_planes: median_repeats must be in [0, EMAP_PLANE_MAX_REPEATS]";
-  if (std::isnan(p.resolution) || (p.resolution > 0.0 && !(std::fabs(res - p.resolution) < 1e-6)))
-    return "emap_segment_planes: resampling is not supported (resolution must be <= 0 or the map's)";
-  if (p.kernel_size < 3 || p.kernel_size % 2 == 0 || p.kernel_size > EMAP_PLANE_MAX_KERNEL)
-    return "emap_segment_planes: kernel_size must be odd, >= 3 and <= EMAP_PLANE_MAX_KERNEL";
-  if (p.opening < 0 || p.opening > EMAP_PLANE_MAX_OPENING)
-    return "emap_segment_planes: opening must be in [0, EMAP_PLANE_MAX_OPENING]";
-  if (p.connectivity != 4 && p.connectivity != 8) return "emap_segment_planes: connectivity must be 4 or 8";
-  if (!std::isfinite(p.plane_inclination_cos) || !std::isfinite(p.local_inclination_cos) ||
-      !std::isfinite(p.patch_error))
-    return "emap_segment_planes: the inclination cosines and the patch error must be finite";
-  return nullptr;
-}
-
-int64_t emap_plane_capacity(int64_t rows, int64_t cols, const emap_plane_params* params) {
-  if (!params || rows < 0 || cols < 0) return -1;
-  return rows * cols / std::max(params->min_points, 3);
-}
-
-// The plane decomposition node's segmented planes map for one window (ConvexPlaneDecompositionRos.cpp:115-149 up to
-// SlidingWindowPlaneExtractor, without RANSAC): the window by k_submap, then the passes of csrc/emap_planes.cuh.  Host
-// output: the copies and one synchronisation; device output: stream-ordered, no synchronisation.  Every check runs
-// before anything is written or launched.
-int emap_segment_planes(emap_handle* h, const double window[4], const emap_plane_params* params, float* layers_out,
-                        int32_t out_is_device, int64_t out_floats, double* planes_out, int64_t planes_capacity,
-                        int32_t* info) {
-  ENTER(h);
-  NvtxRange nv("emap:segment_planes");
-  if (!window || !params || !layers_out || !planes_out || !info)
-    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: null argument");
-  if (!submap_lengths_ok(1, window)) return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: lengths must be finite and >= 0");
-  const emap_plane_params p = *params;
-  const double res = h->cfg.resolution;
-  if (const char* e = plane_params_error(p, res)) return fail(h, EMAP_ERR_INVALID, e);
-  const int W = h->dc.W;
-  const double m[2] = {h->center[0], h->center[1]};
-  int32_t q[5];
-  double centre[2];
-  submap_window(W, res, m, window, q, centre);
-  const int rows = q[3], cols = q[4];
-  const int64_t n = (int64_t)rows * cols;
-  if (q[0] && out_floats < 4 * n)
-    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: out_floats is below 4 * rows * cols");
-  const int64_t plane_rows = emap_plane_capacity(rows, cols, &p);
-  if (q[0] && planes_capacity < plane_rows)
-    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: planes_capacity is below emap_plane_capacity()");
-  if (!q[0]) {
-    if (out_is_device) CK(cudaMemsetAsync(info, 0, 5 * sizeof(int32_t), h->stream));
-    else memset(info, 0, 5 * sizeof(int32_t));
-    return EMAP_OK;
-  }
-  // labels are at most ceil(n / 2) (a 4-connected checkerboard), plus 0.  The statistics are sized and zeroed for that
-  // worst case (128 bytes a slot) because the label count is known only on the device.
-  const int64_t slots = n / 2 + 2;
-  PlaneScratch s;
-  int rc = grow(h, h->pl_block, carve_planes(n, slots, plane_rows, !out_is_device, nullptr, s), 0, false);
-  if (rc) return rc;
-  const size_t used = carve_planes(n, slots, plane_rows, !out_is_device, h->pl_block, s);
-  float* dst = out_is_device ? layers_out : s.layers;
-  double* dst_planes = out_is_device ? planes_out : s.planes;
-  int32_t* dst_info = out_is_device ? info : s.info;
-  // the window: k_submap's elevation layer into s.raw
-  SubmapArgs a;
-  const char* elevation = "elevation";
-  if (!export_list(h, 1, &elevation, nullptr, nullptr, a.L)) return EMAP_ERR_CUDA;
-  a.n_win = 0;
-  int tiles = 0;
-  long long total = 0;
-  submap_add(a, W, q, 1, tiles, total);
-  k_submap<false><<<dim3(tiles, 1), dim3(32, SUBMAP_ROWS), 0, h->stream>>>(h->dc, h->map, h->normal, s.raw, a, h->center[2],
-                                                                           h->cfg.use_only_above_for_upper_bound);
-  LAUNCH_CHECK();
-  CK(cudaMemsetAsync(s.hdr, 0, 8 * sizeof(int), h->stream));
-  CK(cudaMemsetAsync(s.st, 0, sizeof(unsigned long long) * slots * PL_STAT, h->stream));
-  const int cb = cdiv(n, PL_THREADS);
-  // fill: minValues' fixed point per NaN component
-  k_pl_fill_init<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, s.hdr, (int)n);
-  LAUNCH_CHECK();
-  if ((rc = plane_components(h, s, rows, cols, 0))) return rc;
-  k_pl_fill_min<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, rows, cols);
-  LAUNCH_CHECK();
-  k_pl_fill_write<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, s.img[0], (int)n);
-  LAUNCH_CHECK();
-  // median, numberOfRepeats times
-  const int mk = std::max(1, std::min(p.median_kernel, 5));
-  int cur = 0;
-  if (mk > 1)
-    for (int r = 0; r < p.median_repeats; r++, cur ^= 1) {
-      (mk == 3 ? k_pl_median<3> : k_pl_median<5>)<<<cb, PL_THREADS, 0, h->stream>>>(s.img[cur], s.img[cur ^ 1], rows, cols);
-      LAUNCH_CHECK();
-    }
-  const float* img = s.img[cur];
-  // sliding-window planarity, opening, labels
-  k_pl_fit<<<cb, PL_THREADS, 0, h->stream>>>(img, s.bin, rows, cols, p.kernel_size, res, p.patch_error * p.patch_error,
-                                             p.local_inclination_cos);
-  LAUNCH_CHECK();
-  if (p.opening > 0) {
-    k_pl_morph<false><<<cb, PL_THREADS, 0, h->stream>>>(s.bin, s.tmp, rows, cols, p.opening);
-    LAUNCH_CHECK();
-    k_pl_morph<true><<<cb, PL_THREADS, 0, h->stream>>>(s.tmp, s.bin, rows, cols, p.opening);
-    LAUNCH_CHECK();
-  }
-  k_pl_cc_init<<<cb, PL_THREADS, 0, h->stream>>>(s.bin, s.parent, s.key, s.flag, (int)n);
-  LAUNCH_CHECK();
-  const bool conn8 = p.connectivity == 8;
-  if ((rc = plane_components(h, s, rows, cols, conn8))) return rc;
-  (conn8 ? k_pl_first<2> : k_pl_first<1>)<<<cb, PL_THREADS, 0, h->stream>>>(s.parent, s.key, rows, cols);
-  LAUNCH_CHECK();
-  k_pl_first_flag<<<cb, PL_THREADS, 0, h->stream>>>(s.parent, s.key, s.flag, (int)n);
-  LAUNCH_CHECK();
-  const int64_t n_blocks = conn8 ? (int64_t)cdiv(rows, 2) * cdiv(cols, 2) : n;
-  if ((rc = plane_scan(h, s, n_blocks, s.hdr + 1))) return rc;
-  k_pl_label<<<cb, PL_THREADS, 0, h->stream>>>(s.parent, s.key, s.rank, s.lab, (int)n);
-  LAUNCH_CHECK();
-  // per-label planes
-  k_pl_stats<<<cdiv(cdiv(n, PL_RUN), PL_THREADS), PL_THREADS, 0, h->stream>>>(img, s.lab, s.st, rows, cols);
-  LAUNCH_CHECK();
-  const PlaneLabelArgs la = {centre[0] + (0.5 * (rows * res) - 0.5 * res), centre[1] + (0.5 * (cols * res) - 0.5 * res),
-                             res, p.plane_inclination_cos, p.min_points};
-  k_pl_decide<<<cdiv(slots, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.st, s.hdr, s.flag, s.bg, (int)slots, la);
-  LAUNCH_CHECK();
-  if ((rc = plane_scan(h, s, slots, s.hdr + 2))) return rc;
-  k_pl_planes<<<cdiv(slots, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.st, s.rank, s.hdr, dst_planes, (int)slots, la);
-  LAUNCH_CHECK();
-  k_pl_out<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, img, s.lab, s.bg, s.hdr, dst, dst_info, rows, cols);
-  LAUNCH_CHECK();
-  if (!out_is_device) {
-    // info, the plane table and the layers are the block's tail: one copy, one synchronisation, and the caller's
-    // buffers take the layers and planes only when the window had a finite cell
-    const size_t off = (char*)s.info - (char*)h->pl_block, bytes = used - off;
-    if (h->pl_host.size() < bytes) CK(h->pl_host.alloc(bytes));
-    CK(cudaMemcpyAsync(h->pl_host, s.info, bytes, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    PlaneScratch t;
-    carve_planes(n, slots, plane_rows, true, (char*)h->pl_host - off, t);
-    memcpy(info, t.info, 5 * sizeof(int32_t));
-    if (info[0]) {
-      memcpy(planes_out, t.planes, sizeof(double) * 7 * info[4]);
-      memcpy(layers_out, t.layers, sizeof(float) * 4 * n);
-    }
-  }
-  return EMAP_OK;
-}
-
-// The node's publishAsPointCloud (elevation_mapping_ros.cpp:501-505): the points of the exported elevation (map_cloud).
-int emap_get_map_points(emap_handle* h, float* xyz_host, int64_t* n_points) {
-  ENTER(h);
-  NvtxRange nv("emap:get_map_points");
-  if (!n_points || *n_points < 0 || (*n_points > 0 && !xyz_host))
-    return fail(h, EMAP_ERR_INVALID, "emap_get_map_points: null argument or negative capacity");
-  return map_cloud<false>(h, n_points, xyz_host, nullptr, nullptr);
-}
-
-// The node's publishNormalAsArrow (elevation_mapping_ros.cpp:751-778): the arrows of the exported normals (map_cloud).
-int emap_get_normal_arrows(emap_handle* h, int32_t* ids_host, double* segments_host, int64_t* n_arrows) {
-  ENTER(h);
-  NvtxRange nv("emap:get_normal_arrows");
-  if (!n_arrows || *n_arrows < 0 || (*n_arrows > 0 && (!ids_host || !segments_host)))
-    return fail(h, EMAP_ERR_INVALID, "emap_get_normal_arrows: null argument or negative capacity");
-  return map_cloud<true>(h, n_arrows, nullptr, ids_host, segments_host);
-}
-
-int emap_layer_device_ptr(emap_handle* h, const char* name, void** ptr) {
-  ENTER(h);
-  if (!name || !ptr) return fail(h, EMAP_ERR_INVALID, "null argument");
-  const size_t C = (size_t)h->dc.C;
-  int li = layer_index(name);
-  if (li >= 0) { *ptr = h->map + li * C; return EMAP_OK; }
-  if (!strcmp(name, "elevation_map")) { *ptr = h->map; return EMAP_OK; }
-  if (!strcmp(name, "normal_map") || !strcmp(name, "normal_x")) { *ptr = h->normal; return EMAP_OK; }
-  if (!strcmp(name, "normal_y")) { *ptr = h->normal + C; return EMAP_OK; }
-  if (!strcmp(name, "normal_z")) { *ptr = h->normal + 2 * C; return EMAP_OK; }
-  if (!strcmp(name, "traversability_input")) { *ptr = h->trav_input; return EMAP_OK; }
-  h->err = std::string("Layer ") + name + " is not in the map";
-  return EMAP_ERR_NOLAYER;
-}
-
-int emap_exists_layer(const emap_handle* h, const char* name) {
-  if (!h || !name) return 0;
-  return layer_index(name) >= 0 ? 1 : 0;
-}
-
-// EM.py:837-889 get_polygon_traversability (WRAP:254-281): area, clip and bounding box on the host in fp32, then a
-// batch of one polygon whose work items are every tile of the grid (the mask is written everywhere, and the statistics
-// need no poison pass), one device-to-host copy and one synchronisation.
-int emap_polygon_traversability(emap_handle* h, const float* polygon_xy, int32_t n_vertices, const float* checker_plane,
-                                double safe_thresh, double safe_min_thresh, int32_t max_unsafe_n, double result[3],
-                                double* hull_xy, int32_t* n_hull, float* mask) {
-  ENTER(h);
-  if (!polygon_xy || !result || !n_hull || *n_hull < 0 || (*n_hull > 0 && !hull_xy))
-    return fail(h, EMAP_ERR_INVALID, "emap_polygon_traversability: null argument or negative hull capacity");
-  if (n_vertices < 3 || n_vertices > EMAP_POLYGON_MAX_VERTICES)
-    return fail(h, EMAP_ERR_INVALID, "emap_polygon_traversability: 3 to EMAP_POLYGON_MAX_VERTICES vertices required");
-  const int W = h->dc.W;
-  const dim3 g = polygon_grid(W);
-  const PolyStage st = poly_stage(1, n_vertices, ring_capacity(W));
-  PolySizes z;
-  z.up = st.up_bytes; z.items = (size_t)g.x * g.y; z.cols = W - 2; z.down = st.down_bytes;
-  PolyScratch s;
-  int rc = alloc_polygon_scratch(h, z, s);
-  if (rc) return rc;
-  const float area = shoelace_f32(polygon_xy, n_vertices);
-  PolyDesc d = {};
-  float2* xy = (float2*)(h->pg_host + st.xy);
-  clip_polygon(W, h->cfg.resolution, h->center, polygon_xy, n_vertices, xy, d.bbox);
-  const float clipped_area = shoelace_f32((const float*)xy, n_vertices);
-  d.v0 = 0; d.n = n_vertices; d.item0 = 0;
-  d.tr0 = 0; d.tc0 = 0; d.n_tr = g.y; d.n_tc = g.x;
-  d.col0 = 0; d.n_col = W - 2; d.col_off = 0; d.ring_off = 0;
-  memcpy(h->pg_host + st.desc, &d, sizeof(d));
-  rc = run_polygons(h, s, st, 1, (int)z.items, false, checker_plane, safe_thresh, safe_min_thresh, max_unsafe_n, mask,
-                    true, kRingHead);
-  if (rc) return rc;
-  const char* back = h->pg_host + h->pg_cap.up;
-  PolyResult r;
-  memcpy(&r, back, sizeof(r));
-  const double2* ring = (const double2*)(back + st.ring);
-  // EM.py:884-887: a polygon (almost) entirely outside the map is unsafe
-  result[0] = (r.is_safe && !(clipped_area < 0.001f)) ? 1.0 : 0.0;
-  result[1] = r.t;
-  result[2] = (double)area;
-  if (r.n_ring > *n_hull) {
-    *n_hull = r.n_ring;
-    return fail(h, EMAP_ERR_INVALID, "emap_polygon_traversability: hull capacity too small (needed length in *n_hull)");
-  }
-  for (int k = 0; k < r.n_ring; k++) { hull_xy[2 * k] = ring[k].x; hull_xy[2 * k + 1] = ring[k].y; }
-  *n_hull = r.n_ring;
-  return EMAP_OK;
-}
-
-// The check_safety service (CheckSafety.srv) in one call: every polygon's answer is emap_polygon_traversability's.  The
-// work items are only the tiles of each polygon's cell bounding box; k_poly_poison carries the map-wide NaN rule to
-// the cells outside them.  One upload, one read-back copy and one synchronisation (plus one for long rings).
-int emap_polygon_traversability_batch(emap_handle* h, int32_t n_polygons, const int32_t* n_vertices,
-                                      const float* polygon_xy, const float* checker_plane, double safe_thresh,
-                                      double safe_min_thresh, int32_t max_unsafe_n, double* results, double* hull_xy,
-                                      int64_t* hull_offsets, int64_t* hull_rows) {
-  ENTER(h);
-  if (n_polygons < 1 || n_polygons > EMAP_POLYGON_MAX_BATCH)
-    return fail(h, EMAP_ERR_INVALID, "emap_polygon_traversability_batch: 1 to EMAP_POLYGON_MAX_BATCH polygons required");
-  if (!n_vertices || !polygon_xy || !results || (hull_xy && (!hull_offsets || !hull_rows)) ||
-      (hull_rows && *hull_rows < 0))
-    return fail(h, EMAP_ERR_INVALID, "emap_polygon_traversability_batch: null argument or negative hull capacity");
-  size_t n_vert = 0;
-  for (int i = 0; i < n_polygons; i++) {
-    if (n_vertices[i] < 3 || n_vertices[i] > EMAP_POLYGON_MAX_VERTICES)
-      return fail(h, EMAP_ERR_INVALID,
-                  "emap_polygon_traversability_batch: 3 to EMAP_POLYGON_MAX_VERTICES vertices required per polygon");
-    n_vert += n_vertices[i];
-  }
-  const bool hulls = hull_xy != nullptr;
-  // traversability_polygon.py:25 compares the whole interior: with fp32(1 - safe_thresh) < 0 the masked 0 of every cell
-  // outside a polygon is over too, so its count and hull take the whole map.  Every polygon then brings every tile and
-  // the whole column window, as the single call does.
-  const bool whole_map = (float)(1.0 - safe_thresh) < 0.0f;
-  const dim3 g = polygon_grid(h->dc.W);
-  // each polygon's tiles (its work items and partials), column window and ring slot
-  std::vector<PolyDesc> desc(n_polygons);
-  size_t items = 0, cols = 0, rows = 0, v0 = 0;
-  for (int i = 0; i < n_polygons; i++) {
-    PolyDesc& d = desc[i];
-    clip_polygon(h->dc.W, h->cfg.resolution, h->center, polygon_xy + 2 * v0, n_vertices[i], nullptr, d.bbox);
-    polygon_tiles(h->dc.W, h->cfg.resolution, h->center, d);
-    if (whole_map) {
-      d.tr0 = 0; d.tc0 = 0; d.n_tr = g.y; d.n_tc = g.x;
-      d.col0 = 0; d.n_col = h->dc.W - 2;
-    }
-    if (!hulls) d.n_col = 0;
-    d.v0 = (int)v0; d.n = n_vertices[i]; d.item0 = (int)items; d.col_off = (int)cols; d.ring_off = (int)rows;
-    items += (size_t)d.n_tr * d.n_tc;
-    cols += d.n_col;
-    rows += d.n_col ? 2 * (size_t)d.n_col + 1 : 0;
-    v0 += n_vertices[i];
-  }
-  const PolyStage st = poly_stage(n_polygons, n_vert, rows);
-  PolySizes z;
-  z.up = st.up_bytes; z.items = items; z.cols = cols; z.down = st.down_bytes;
-  PolyScratch s;
-  int rc = alloc_polygon_scratch(h, z, s);
-  if (rc) return rc;
-  memset(h->pg_host, 0, st.desc);                                   // the poison counts start at zero
-  memcpy(h->pg_host + st.desc, desc.data(), sizeof(PolyDesc) * n_polygons);
-  float2* xy = (float2*)(h->pg_host + st.xy);
-  std::vector<float> area(n_polygons), clipped_area(n_polygons);
-  for (int i = 0; i < n_polygons; i++) {
-    const PolyDesc& d = desc[i];
-    area[i] = shoelace_f32(polygon_xy + 2 * (size_t)d.v0, d.n);
-    float bbox[4];
-    clip_polygon(h->dc.W, h->cfg.resolution, h->center, polygon_xy + 2 * (size_t)d.v0, d.n, xy + d.v0, bbox);
-    clipped_area[i] = shoelace_f32((const float*)(xy + d.v0), d.n);
-  }
-  rc = run_polygons(h, s, st, n_polygons, (int)items, true, checker_plane, safe_thresh, safe_min_thresh, max_unsafe_n,
-                    nullptr, hulls, kBatchRingHead);
-  if (rc) return rc;
-  const char* back = h->pg_host + h->pg_cap.up;
-  const PolyResult* r = (const PolyResult*)back;
-  const double2* ring = (const double2*)(back + st.ring);
-  int64_t total = 0;
-  for (int i = 0; i < n_polygons; i++) {
-    // EM.py:884-887: a polygon (almost) entirely outside the map is unsafe
-    results[3 * i] = (r[i].is_safe && !(clipped_area[i] < 0.001f)) ? 1.0 : 0.0;
-    results[3 * i + 1] = r[i].t;
-    results[3 * i + 2] = (double)area[i];
-    if (hull_offsets) hull_offsets[i] = total;
-    total += r[i].n_ring;
-  }
-  if (hull_offsets) hull_offsets[n_polygons] = total;
-  if (!hulls) {
-    if (hull_rows) *hull_rows = 0;
-    return EMAP_OK;
-  }
-  if (total > *hull_rows) {
-    *hull_rows = total;
-    return fail(h, EMAP_ERR_INVALID,
-                "emap_polygon_traversability_batch: hull capacity too small (needed rows in *hull_rows)");
-  }
-  for (int i = 0; i < n_polygons; i++) {
-    const double2* src = ring + desc[i].ring_off;
-    double* dst = hull_xy + 2 * hull_offsets[i];
-    for (int k = 0; k < r[i].n_ring; k++) { dst[2 * k] = src[k].x; dst[2 * k + 1] = src[k].y; }
-  }
-  *hull_rows = total;
   return EMAP_OK;
 }
 
@@ -2363,232 +987,6 @@ int emap_set_state(emap_handle* h, const float* map_host, const float* normal_ho
   if (normal_host) CK(cudaMemcpyAsync(h->normal, normal_host, sizeof(float) * 3 * C, cudaMemcpyHostToDevice, h->stream));
   if (center) for (int k = 0; k < 3; k++) h->center[k] = (float)center[k];
   CK(cudaStreamSynchronize(h->stream));
-  return EMAP_OK;
-}
-
-// ---- plugins ---------------------------------------------------------------------------------
-int emap_min_filter(emap_handle* h, const float* elevation, const float* is_valid, float* out, int32_t k, int32_t iteration_n,
-                    int32_t* iterations_run) {
-  ENTER(h);
-  return minmax_filter<false>(h, elevation, is_valid, out, k, iteration_n, iterations_run);
-}
-
-int emap_max_filter(emap_handle* h, const float* elevation, const float* is_valid, float* out, int32_t k, int32_t iteration_n,
-                    int32_t* iterations_run) {
-  ENTER(h);
-  return minmax_filter<true>(h, elevation, is_valid, out, k, iteration_n, iterations_run);
-}
-
-int emap_erode(emap_handle* h, const float* layer, float* out, int32_t kernel_size, int32_t iterations, int32_t reverse) {
-  ENTER(h);
-  if (!layer || !out || kernel_size < 1 || kernel_size > 31 || iterations < 1 || iterations > 64)
-    return fail(h, EMAP_ERR_INVALID, "emap_erode: bad argument");
-  int rc;
-  if ((rc = alloc_plugin_scratch(h)) || (rc = grow(h, h->pl_cnt, 2, 30, false))) return rc;
-  u32* const mm = (u32*)(int*)h->pl_cnt;      // min / max of the layer
-  const u32 init[2] = {0xffffffffu, 0u};
-  CK(cudaMemcpyAsync(mm, init, sizeof(init), cudaMemcpyHostToDevice, h->stream));
-  PER_CELL(k_layer_minmax, h->dc, layer, reverse, mm);
-  const int ks = kernel_size + (iterations - 1) * (kernel_size - 1), anchor = (kernel_size / 2) * iterations;
-  const float* src = layer;
-  if (layer == out) {        // in-place call: erode from a copy
-    CK(cudaMemcpyAsync(h->pl[0], layer, sizeof(float) * (size_t)h->dc.C, cudaMemcpyDeviceToDevice, h->stream));
-    src = h->pl[0];
-  }
-  PER_CELL(k_erode, h->dc, src, out, ks, anchor, reverse, (const u32*)mm);
-  return EMAP_OK;
-}
-
-int emap_robot_centric_elevation(emap_handle* h, const float* elevation, const float* is_valid, const float R[9], float* out,
-                                 double resolution, double threshold, int32_t use_threshold) {
-  ENTER(h);
-  if (!elevation || !is_valid || !R || !out) return fail(h, EMAP_ERR_INVALID, "null argument");
-  PER_CELL(k_robot_centric, h->dc, elevation, is_valid, out, R[6], R[7], R[8], resolution, threshold, use_threshold);
-  return EMAP_OK;
-}
-
-int emap_smooth_filter(emap_handle* h, const float* in, float* out) {
-  ENTER(h);
-  if (!in || !out) return fail(h, EMAP_ERR_INVALID, "null argument");
-  int rc = alloc_plugin_scratch(h);
-  if (rc) return rc;
-  PER_CELL(k_box3, h->dc, in, h->pl[0], 0);
-  PER_CELL(k_box3, h->dc, h->pl[0], h->pl[1], 1);
-  PER_CELL(k_box3, h->dc, h->pl[1], h->pl[0], 0);
-  PER_CELL(k_box3, h->dc, h->pl[0], out, 1);
-  return EMAP_OK;
-}
-
-// plugins/inpainting.py:53-63: 8-bit normalisation, cv.inpaint(h, mask, 1, INPAINT_TELEA), de-normalisation -- OpenCV's
-// fast-marching fill replayed on the device in parallel (emap_inpaint.cuh), bit-identical to cv2's result.
-int emap_inpaint(emap_handle* h, const float* elevation, const float* is_valid, float* out, int32_t method) {
-  ENTER(h);
-  NvtxRange nv("emap:inpaint");
-  if (!elevation || !is_valid || !out) return fail(h, EMAP_ERR_INVALID, "emap_inpaint: null argument");
-  if (method != 0) return fail(h, EMAP_ERR_INVALID, "emap_inpaint: only method 0 (telea) is implemented; 'ns' (Navier-Stokes) is not");
-  const int W = h->dc.W;
-  const size_t N = (size_t)(W + 2) * (W + 2), C = (size_t)W * W;
-  // zero-filled once: the march loads a pixel's child fields (ck, Tc, vc) speculatively, before it knows the pixel is a
-  // child of the running round; the values of non-children are never used, but they should not be uninitialised memory
-  int rc = grow(h, h->ip_block, inpaint_scratch(W, nullptr).bytes, 0, true);
-  if (rc) return rc;
-  if (!h->ip_grid) {
-    int nb = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_ip_march, IP_MARCH_THREADS, 0));
-    if (nb < 1) return fail(h, EMAP_ERR_CUDA, "emap_inpaint: the cooperative kernel does not fit on an SM");
-    h->ip_grid = h->n_sm;          // one CTA per SM: the fronts are thin, and a grid barrier costs less with fewer CTAs
-  }
-  InpaintScratch s = inpaint_scratch(W, h->ip_block);
-  InpaintView& v = s.v;
-  InpaintCtl* ctl = s.ctl;
-  InpaintCtl init;
-  memset(&init, 0, sizeof(init));
-  init.mm[0] = 0xffffffffu; init.mm[1] = 0u;
-  CK(cudaMemcpyAsync(ctl, &init, sizeof(init), cudaMemcpyHostToDevice, h->stream));     // pageable: staged before return
-  const int nbN = cdiv((i64)N, 256);
-  PER_CELL(k_ip_minmax, (int)C, elevation, is_valid, ctl);
-  k_ip_init<<<nbN, 256, 0, h->stream>>>(W, elevation, is_valid, v, (const InpaintCtl*)ctl); LAUNCH_CHECK();
-  k_ip_band<<<nbN, 256, 0, h->stream>>>(v, s.heap[0], ctl); LAUNCH_CHECK();
-  k_ip_band_flag<<<nbN, 256, 0, h->stream>>>(v, (const int*)s.heap[0], ctl); LAUNCH_CHECK();
-  {
-    int cap = 4096;
-    void* args[] = {(void*)&v, (void*)&s.heap[0], (void*)&s.heap[1], (void*)&s.children, (void*)&ctl, (void*)&cap};
-    CK(cudaLaunchCooperativeKernel((const void*)k_ip_march, dim3(h->ip_grid), dim3(IP_MARCH_THREADS), args, 0, h->stream));
-    h->launches++;
-  }
-  PER_CELL(k_ip_finish, (int)C, (const uint8_t*)v.img, elevation, out, (const InpaintCtl*)ctl);
-  return EMAP_OK;
-}
-
-// plugins/semantic_filter.py:89-133: argmax over the planes, palette entry of the class id (bits)
-int emap_semantic_filter(emap_handle* h, int32_t n_layers, const float* const* planes, float* out) {
-  ENTER(h);
-  if (!out || n_layers < 0 || n_layers > EMAP_SEMANTIC_FILTER_MAX_LAYERS || !planes_ok(n_layers, planes))
-    return fail(h, EMAP_ERR_INVALID, "emap_semantic_filter: 0 to EMAP_SEMANTIC_FILTER_MAX_LAYERS non-null planes and a non-null output required");
-  SemFilterArgs a;
-  memset(&a, 0, sizeof(a));
-  a.n = n_layers;
-  for (int l = 0; l < n_layers; l++) a.plane[l] = planes[l];
-  PER_CELL(k_semantic_filter, h->dc.C, a, (u32*)out);
-  return EMAP_OK;
-}
-
-// plugins/semantic_traversability.py:59-83: per-layer threshold votes (fp64 comparisons), fp32(0.1) or 1
-int emap_semantic_traversability(emap_handle* h, int32_t n_layers, const float* const* planes, const double* thresholds,
-                                 const int32_t* is_traversability_type, float* out) {
-  ENTER(h);
-  if (!out || n_layers < 0 || n_layers > EMAP_SEMANTIC_TRAVERSABILITY_MAX_LAYERS || !planes_ok(n_layers, planes) ||
-      (n_layers > 0 && (!thresholds || !is_traversability_type)))
-    return fail(h, EMAP_ERR_INVALID, "emap_semantic_traversability: 0 to EMAP_SEMANTIC_TRAVERSABILITY_MAX_LAYERS non-null planes, "
-                                     "thresholds, types and a non-null output required");
-  SemTravArgs a;
-  memset(&a, 0, sizeof(a));
-  a.n = n_layers;
-  for (int l = 0; l < n_layers; l++) {
-    a.plane[l] = planes[l];
-    a.thr[l] = thresholds[l];
-    if (is_traversability_type[l]) a.is_trav[l >> 5] |= 1u << (l & 31);
-  }
-  PER_CELL(k_semantic_traversability, h->dc.C, a, out);
-  return EMAP_OK;
-}
-
-// plugins/features_pca.py:44-96: exact 3-component PCA of the clipped features on the device, packed to colour bits.
-// Four launches and one synchronisation, at the end, to read the NaN flag.
-int emap_features_pca(emap_handle* h, int32_t n_features, const float* const* planes, float* out) {
-  ENTER(h);
-  NvtxRange nv("emap:features_pca");
-  if (!out || n_features < 3 || n_features > EMAP_PCA_MAX_FEATURES || !planes_ok(n_features, planes))
-    return fail(h, EMAP_ERR_INVALID, "emap_features_pca: 3 to EMAP_PCA_MAX_FEATURES non-null planes and a non-null output required");
-  PcaScratch s;
-  int rc = grow(h, h->pca_block, carve_pca(h, nullptr, s), 0, false);
-  if (rc) return rc;
-  carve_pca(h, h->pca_block, s);
-  const int C = h->dc.C, F = n_features;
-  PcaArgs a;
-  memset(&a, 0, sizeof(a));
-  a.F = F;
-  for (int f = 0; f < F; f++) a.plane[f] = planes[f];
-  const size_t eig_smem = sizeof(double) * 2 * F * (F + 1);
-  CK(cudaFuncSetAttribute(k_pca_eigen, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)eig_smem));
-  CK(cudaMemsetAsync(&s.res->nan, 0, sizeof(int), h->stream));
-  const int grid = pca_stats_grid(h);
-  k_pca_stats<<<grid, PCA_THREADS, 0, h->stream>>>(C, a, s.part, s.res);
-  LAUNCH_CHECK();
-  k_pca_eigen<<<1, PCA_THREADS, eig_smem, h->stream>>>(C, F, grid, s.part, s.res);
-  LAUNCH_CHECK();
-  PER_CELL(k_pca_project, C, a, s.res, s.proj);
-  PER_CELL(k_pca_pack, C, (const PcaResult*)s.res, (const double*)s.proj, (u32*)out);
-  int nan = 0;
-  CK(cudaMemcpyAsync(&nan, &s.res->nan, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  if (nan) return fail(h, EMAP_ERR_INVALID, "emap_features_pca: NaN in the input features");
-  return EMAP_OK;
-}
-
-// EM.py:468-562 input_image + semantic_map.py:261-309 update_layers_image: the host part (image_camera) and one
-// k_image_fuse launch.  A host image is copied into pinned staging and from there, once, to the device; a device image
-// is read in place, with no host synchronisation.
-int emap_input_image(emap_handle* h, int32_t n_planes, const float* image, int is_device_ptr, int32_t height, int32_t width,
-                     const float K[9], const float* D, int32_t n_D, const char* distortion_model, const float R[9],
-                     const float t[3], int32_t n_fused, const int32_t* plane, const int32_t* kind, const int32_t* layer,
-                     float* semantic_map_device, int32_t n_layers) {
-  ENTER(h);
-  NvtxRange nv("emap:input_image");
-  if (!image || !K || !R || !t || !distortion_model || (n_D > 0 && !D) || n_D < 0 ||
-      (n_fused > 0 && (!plane || !kind || !layer || !semantic_map_device)))
-    return fail(h, EMAP_ERR_INVALID, "emap_input_image: null argument");
-  if (n_planes < 1 || height < 1 || width < 1 || (int64_t)height * width > (1ll << 24))
-    return fail(h, EMAP_ERR_INVALID, "emap_input_image: n_planes >= 1 and 1 <= height * width <= 2^24 required");
-  if (n_fused < 0 || n_fused > EMAP_IMAGE_MAX_CHANNELS)
-    return fail(h, EMAP_ERR_INVALID, "emap_input_image: 0 to EMAP_IMAGE_MAX_CHANNELS fused channels required");
-  ImageArgs a;
-  memset(&a, 0, sizeof(a));
-  for (int k = 0; k < n_fused; k++) {
-    if (kind[k] != EMAP_IMAGE_COLOR && kind[k] != EMAP_IMAGE_EXPONENTIAL)
-      return fail(h, EMAP_ERR_INVALID, "emap_input_image: kind must be EMAP_IMAGE_COLOR or EMAP_IMAGE_EXPONENTIAL");
-    if (plane[k] < 0 || plane[k] >= n_planes || (kind[k] == EMAP_IMAGE_COLOR && n_planes < 3))
-      return fail(h, EMAP_ERR_INVALID, "emap_input_image: plane outside the image, or a colour channel with fewer than 3 planes");
-    if (layer[k] < 0 || layer[k] >= n_layers)
-      return fail(h, EMAP_ERR_INVALID, "emap_input_image: layer outside [0, n_layers)");
-    a.plane[k] = plane[k];
-    a.kind[k] = kind[k] == EMAP_IMAGE_COLOR ? IMG_COLOR : IMG_EXPONENTIAL;
-    a.layer[k] = layer[k];
-  }
-  const int cam = image_camera(K, D, n_D, distortion_model, R, t, h->center, h->dc.W, h->cfg.resolution, &a.cam);
-  if (cam == IMG_CAM_NONFINITE) return fail(h, EMAP_ERR_INVALID, "emap_input_image: non-finite K, R or t");
-  if (cam == IMG_CAM_OUTSIDE)
-    return fail(h, EMAP_ERR_INVALID, "emap_input_image: camera cell cell_n / 2 + t / resolution outside [0, 2^24)");
-  if (n_fused == 0) return EMAP_OK;       // the correspondence alone changes nothing
-  const size_t plane_sz = (size_t)height * width, n_img = plane_sz * n_planes;
-  const float* img = image;
-  if (!is_device_ptr) {
-    const size_t bytes = sizeof(float) * n_img;
-    if (int rc = h->img_up.room(h, bytes)) return rc;
-    memcpy(h->img_up.host, image, bytes);                // the caller's buffer is free from here on
-    if (int rc = h->img_up.send(h, bytes)) return rc;
-    img = (const float*)(char*)h->img_up.dev;
-  }
-  for (int k = 0; k < 3; k++) a.center[k] = h->center[k];
-  a.res = h->cfg.resolution;
-  a.W = h->dc.W; a.C = h->dc.C;
-  a.img_w = (float)width; a.img_h = (float)height;
-  a.n_img = (long long)n_img; a.plane_sz = (long long)plane_sz;
-  a.image = img; a.sem = semantic_map_device; a.n = n_fused;
-  PER_CELL(k_image_fuse, a, (const float*)h->map);
-  return EMAP_OK;
-}
-
-// rounds / Jacobi statistics of the last emap_inpaint call (diagnostics)
-int emap_inpaint_stats(emap_handle* h, int32_t* rounds, int32_t* max_jacobi, int32_t* not_converged) {
-  ENTER(h);
-  if (!h->ip_block) return fail(h, EMAP_ERR_STATE, "emap_inpaint has not run");
-  InpaintCtl c;
-  CK(cudaMemcpyAsync(&c, inpaint_scratch(h->dc.W, h->ip_block).ctl, sizeof(c), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  if (rounds) *rounds = c.rounds;
-  if (max_jacobi) *max_jacobi = c.max_jacobi;
-  if (not_converged) *not_converged = c.not_converged;
   return EMAP_OK;
 }
 

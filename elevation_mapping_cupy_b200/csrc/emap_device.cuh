@@ -82,6 +82,27 @@ struct FrameScalars {          // device-resident scalars of the running frame
   i64 nkept, nkept_last;       // kept pixels of a depth-image frame (DepthSource), and its copy
 };
 
+// per-cell scratch of a frame; all zero between frames (k_finalize re-zeroes what it consumed)
+struct CellScratch {
+  u64* cnt_ai;     // low word: newmap[4] all points of the cell (CK.py:336), high word: newmap[3] drift inliers (CK.py:334).
+                   // One 64-bit accumulation per point carries both (one multimem.red per run in sharded frames).
+  u64* cnt_fo;     // low word: newmap[2] fused points (CK.py:185), high word: atomicAdd(map[1], outlier_variance) count
+                   // of outlier points (CK.py:174)
+  u32* n_ray;      // ... by penetrating rays, CK.py:251
+  i64* SH;         // sum new_h   CK.py:183
+  i64* SV;         // sum new_v   CK.py:184
+  i64* DV;         // sum of validity decrements CK.py:250
+  u64* last;       // (global point index << 32 | bits(new_h)) max  -> upper_bound of a hit cell, CK.py:191
+  float* thr;      // first-level ray record, 4 B: a sample at height nz can only act on the cell if !(nz > thr)
+  uint2* rec;      // second-level ray record, 8 B: {valid cell ? bits(h') : upper-bound key, flags}; read-only for rays
+  u32* ukv;        // min over rays of the upper-bound key carved into the cell (UKEY_NONE between frames), CK.py:230-233,253-256
+  unsigned char* dirty;   // 1 = some kernel of this frame touched the cell's scratch (k_finalize takes its full path there
+                   // and clears it); nullptr in sharded frames, where the marker is derived from cnt_all / ukv
+  i64 mc_off;      // sharded frames: byte offset from a local scratch address to its NVLink MULTICAST alias
+                   // (0 = single GPU).  Non-zero: every accumulation is one multimem.red that the NVSwitch
+                   // applies to the replicas of ALL ranks (this one included) -- scatter and collective fused.
+};
+
 __device__ __forceinline__ float h16(float x) { return __half2float(__float2half_rn(x)); }
 
 // 2^-32 fixed point of one fp32 term, |x| saturated at 2^20 (oracle/emap_oracle.c fix32)

@@ -1,0 +1,594 @@
+// emap_export_api.cu -- the export calls of the C ABI (include/emap.h): layers, map windows (emap_get_submaps), windows
+// in a requester's frame (emap_get_transformed_submaps), plane segmentation of a window, the map point cloud and normal
+// arrows, and the layer pointers.
+#include "emap_handle.cuh"
+#include "emap_export.cuh"
+#include "emap_submap.cuh"
+#include "emap_planes.cuh"
+#include "emap_mapcloud.cuh"
+
+namespace {
+
+int layer_index(const char* name) {
+  static const char* names[] = {"elevation", "variance", "is_valid", "traversability", "time", "upper_bound", "is_upper_bound"};
+  for (int i = 0; i < 7; i++) if (!strcmp(name, names[i])) return i;
+  return -1;
+}
+// export_value's named kinds: kExportNames[k] is kind k, except the last, normal_color (kind EXPORT_KIND_PLANE is a
+// caller plane)
+const char* const kExportNames[] = {"elevation", "variance", "traversability", "time", "upper_bound", "is_upper_bound",
+                                    "normal_x", "normal_y", "normal_z", "normal_color"};
+constexpr int kNumExportNames = sizeof(kExportNames) / sizeof(kExportNames[0]);
+static_assert(kNumExportNames == EXPORT_KIND_PLANE + 1, "kinds 0..8 are named in order, then normal_color");
+inline int export_kind(int name_index) {
+  return name_index == kNumExportNames - 1 ? EXPORT_KIND_NORMAL_COLOR : name_index;
+}
+
+// The n (<= EXPORT_MAX_LAYERS) layers of an export call.  names[k]: a name of kExportNames, or planes[k] != NULL: a (W,W)
+// device plane exported with flags[k] (bit 0 fill_nan, bit 1 add the centre height).  Returns false, with the message
+// in h->err, for an unknown name.
+bool export_list(emap_handle* h, int32_t n, const char* const* names, const float* const* planes, const int32_t* flags,
+                 ExportList& L) {
+  memset(&L, 0, sizeof(L));
+  L.n = n;
+  for (int k = 0; k < n; k++) {
+    if (planes && planes[k]) {
+      L.kind[k] = EXPORT_KIND_PLANE; L.plane[k] = planes[k]; L.flags[k] = flags ? flags[k] : 0;
+      continue;
+    }
+    int kind = -1;
+    if (names && names[k])
+      for (int i = 0; i < kNumExportNames; i++) if (!strcmp(names[k], kExportNames[i])) kind = export_kind(i);
+    if (kind < 0) { h->err = std::string("Layer ") + (names && names[k] ? names[k] : "(null)") + " is not in the map"; return false; }
+    L.kind[k] = kind;
+  }
+  return true;
+}
+
+// Layers by one k_export_multi launch, one device-to-host copy and one synchronisation (layers as export_list).
+int export_layers(emap_handle* h, int32_t n, const char* const* names, const float* const* planes, const int32_t* flags,
+                  float* out_host, int64_t n_out_total) {
+  if (n < 1 || n > EXPORT_MAX_LAYERS || !out_host) return fail(h, EMAP_ERR_INVALID, "emap_get_layers: 1..24 layers, non-null output");
+  const int Wo = h->dc.W - 2;
+  const size_t per = (size_t)Wo * Wo;
+  if (n_out_total != (int64_t)(per * n)) return fail(h, EMAP_ERR_INVALID, "output must hold n * (cell_n-2)^2 floats");
+  ExportList L;
+  if (!export_list(h, n, names, planes, flags, L)) return EMAP_ERR_NOLAYER;
+  int rc = grow(h, h->d_export, per * n, 0, false);
+  if (rc) return rc;
+  const auto kern = export_has_colour(L) ? k_export_multi<true> : k_export_multi<false>;
+  kern<<<dim3(cdiv((i64)per, 256), n), 256, 0, h->stream>>>(h->dc, h->map, h->normal, h->d_export, L, h->center[2],
+                                                             h->cfg.use_only_above_for_upper_bound);
+  LAUNCH_CHECK();
+  CK(cudaMemcpyAsync(out_host, h->d_export, sizeof(float) * per * n, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return EMAP_OK;
+}
+
+// emap_get_map_points (ARROWS false) / emap_get_normal_arrows (true): the count pass and the scan, one synchronisation
+// for the total; then, if the caller's capacity holds it, the write pass, the payload's copies and one more
+// synchronisation.  Nothing reaches the caller's rows when the capacity is too small.
+template <bool ARROWS>
+int map_cloud(emap_handle* h, int64_t* n_rows, float* xyz, int32_t* ids, double* seg) {
+  const int Wo = h->dc.W - 2;
+  const int n_chunks = cdiv(Wo, MC_TILE), n_tiles = cdiv(Wo, MC_TILE);
+  const int n = Wo * n_chunks, span = MC_TILE * n_chunks;      // count entries; entries of one scan CTA
+  static_assert(MC_TILE % 4 == 0, "k_mapcloud_scan reads whole spans as int4");
+  // cell_n <= 2049 (emap_create): at most 64 chunks, a span of at most 2048 entries, two per scan thread
+  if (span > 2 * 1024) return fail(h, EMAP_ERR_INVALID, "map point cloud: cell_n too large for k_mapcloud_scan");
+  int rc = grow(h, h->mapcloud.table, 2 * (size_t)n + 1, 0, false);
+  if (rc) return rc;
+  if (!h->mapcloud.count) CK(h->mapcloud.count.alloc(1));
+  int* cnt = h->mapcloud.table;
+  int* off = cnt + n;
+  const dim3 grid(n_tiles, n_chunks);
+  const MapCloudGeom g = {(double)h->center[0], (double)h->center[1], h->cfg.resolution};
+  MapCloudOut o = {nullptr, nullptr, nullptr};
+  k_mapcloud<ARROWS, false><<<grid, MC_THREADS, 0, h->stream>>>(h->dc, h->map, h->normal, h->center[2], cnt, nullptr, g, o);
+  LAUNCH_CHECK();
+  k_mapcloud_scan<<<cdiv(n, span), 1024, 0, h->stream>>>(cnt, off, n, span);
+  LAUNCH_CHECK();
+  CK(cudaMemcpyAsync(h->mapcloud.count, off + n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  const int64_t total = *h->mapcloud.count;
+  if (total > *n_rows) {
+    *n_rows = total;
+    return fail(h, EMAP_ERR_INVALID, "map point cloud: capacity too small (needed rows in the count argument)");
+  }
+  *n_rows = total;
+  if (!total) return EMAP_OK;
+  const size_t id_bytes = ARROWS ? (sizeof(int32_t) * (size_t)total + 255) & ~(size_t)255 : 0;
+  const size_t row_bytes = ARROWS ? 6 * sizeof(double) : 3 * sizeof(float);
+  rc = grow(h, h->mapcloud.out, id_bytes + row_bytes * (size_t)total, 0, false);
+  if (rc) return rc;
+  char* base = h->mapcloud.out;
+  o.xyz = (float*)base; o.ids = (int32_t*)base; o.seg = (double*)(base + id_bytes);
+  k_mapcloud<ARROWS, true><<<grid, MC_THREADS, 0, h->stream>>>(h->dc, h->map, h->normal, h->center[2], cnt, off, g, o);
+  LAUNCH_CHECK();
+  if (ARROWS) {
+    CK(cudaMemcpyAsync(ids, o.ids, sizeof(int32_t) * total, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(seg, o.seg, 6 * sizeof(double) * total, cudaMemcpyDeviceToHost, h->stream));
+  } else {
+    CK(cudaMemcpyAsync(xyz, o.xyz, 3 * sizeof(float) * total, cudaMemcpyDeviceToHost, h->stream));
+  }
+  CK(cudaStreamSynchronize(h->stream));
+  return EMAP_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int emap_get_map_with_name(emap_handle* h, const char* name, float* out_host, int64_t n_out) {
+  ENTER(h);
+  if (!name || !out_host) return fail(h, EMAP_ERR_INVALID, "null argument");
+  return export_layers(h, 1, &name, nullptr, nullptr, out_host, n_out);
+}
+
+// Several layers in one launch, one device-to-host copy and one synchronisation (WRAP:213-252 get_grid_map exports a list
+// of layers per call).
+int emap_get_layers(emap_handle* h, int32_t n, const char* const* names, const float* const* planes, const int32_t* flags,
+                    float* out_host, int64_t n_out_total) {
+  ENTER(h);
+  return export_layers(h, n, names, planes, flags, out_host, n_out_total);
+}
+
+static_assert(EMAP_SUBMAP_MAX_WINDOWS == SUBMAP_MAX_WINDOWS && EMAP_SUBMAP_MAX_LAYERS == EXPORT_MAX_LAYERS,
+              "emap.h states the kernel's limits");
+
+static bool submap_lengths_ok(int64_t n, const double* windows) {
+  for (int64_t w = 0; w < n; w++)
+    for (int a = 2; a < 4; a++)
+      if (!(std::isfinite(windows[4 * w + a]) && windows[4 * w + a] >= 0.0)) return false;
+  return true;
+}
+
+// submap_window for each of n windows: info[5 w ..] and centres[2 w ..]
+static void submap_windows(int32_t cell_n, double res, const double m[2], int32_t n, const double* windows,
+                           int32_t* info, double* centres) {
+  for (int32_t w = 0; w < n; w++) submap_window(cell_n, res, m, windows + 4 * w, info + 5 * w, centres + 2 * w);
+}
+
+// The host part of emap_get_submaps on its own (no handle, no device).
+int emap_submap_windows(int32_t cell_n, double resolution, const double center[2], int32_t n_windows,
+                        const double* windows, int32_t* info, double* centres) {
+  if (!center || !windows || !info || !centres || cell_n < 3 || !(std::isfinite(resolution) && resolution > 0.0) ||
+      n_windows < 0 || !submap_lengths_ok(n_windows, windows))
+    return EMAP_ERR_INVALID;
+  submap_windows(cell_n, resolution, center, n_windows, windows, info, centres);
+  return EMAP_OK;
+}
+
+// Appends the successful window q = submap_window's info to k_submap's table: its first work item is `tiles` and its
+// first output float `total`, both advanced past it.
+static void submap_add(SubmapArgs& a, int W, const int32_t q[5], int n_layers, int& tiles, long long& total) {
+  SubmapWin& s = a.win[a.n_win++];
+  s.r0 = (int16_t)(W - 2 - q[1]); s.c0 = (int16_t)(W - 2 - q[2]);
+  s.rows = (int16_t)q[3]; s.cols = (int16_t)q[4];
+  s.tile0 = tiles; s.off = total;
+  tiles += cdiv(q[3], SUBMAP_ROWS);
+  total += (long long)n_layers * q[3] * q[4];
+}
+
+// The get_raw_submap service (elevation_mapping_ros.cpp:507-553) for a batch of windows: the windows on the host
+// (submap_window), every (window, layer, row) of the batch in one k_submap launch whose table is its parameters.  Host
+// output: one device-to-host copy and one synchronisation; device output: stream-ordered, no synchronisation.  Every
+// check runs before anything is written or launched.
+int emap_get_submaps(emap_handle* h, int32_t n_windows, const double* windows, int32_t n_layers, const char* const* names,
+                     const float* const* planes_device, const int32_t* flags, float* out, int32_t out_is_device,
+                     int64_t out_floats, int32_t* info, double* centres) {
+  ENTER(h);
+  NvtxRange nv("emap:get_submaps");
+  if (!windows || !names || !out || !info || !centres) return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: null argument");
+  if (n_windows < 1 || n_windows > EMAP_SUBMAP_MAX_WINDOWS)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: 1 to EMAP_SUBMAP_MAX_WINDOWS windows required");
+  if (n_layers < 1 || n_layers > EMAP_SUBMAP_MAX_LAYERS)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: 1 to EMAP_SUBMAP_MAX_LAYERS layers required");
+  if (!submap_lengths_ok(n_windows, windows))
+    return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: lengths must be finite and >= 0");
+  SubmapArgs a;
+  if (!export_list(h, n_layers, names, planes_device, flags, a.L)) return EMAP_ERR_INVALID;
+  const int W = h->dc.W;
+  const double m[2] = {h->center[0], h->center[1]};
+  std::vector<int32_t> inf(5 * (size_t)n_windows);
+  std::vector<double> cen(2 * (size_t)n_windows);
+  a.n_win = 0;
+  int tiles = 0;
+  long long total = 0;
+  submap_windows(W, h->cfg.resolution, m, n_windows, windows, inf.data(), cen.data());
+  for (int w = 0; w < n_windows; w++)
+    if (inf[5 * w]) submap_add(a, W, &inf[5 * w], n_layers, tiles, total);
+  if (total > out_floats)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_submaps: out_floats is below the layers times the windows' cells");
+  memcpy(info, inf.data(), sizeof(int32_t) * inf.size());
+  memcpy(centres, cen.data(), sizeof(double) * cen.size());
+  if (!a.n_win) return EMAP_OK;
+  float* dst = out;
+  if (!out_is_device) {
+    const int rc = grow(h, h->d_export, (size_t)total, 0, false);
+    if (rc) return rc;
+    dst = h->d_export;
+  }
+  const auto kern = export_has_colour(a.L) ? k_submap<true> : k_submap<false>;
+  kern<<<dim3(tiles, n_layers), dim3(32, SUBMAP_ROWS), 0, h->stream>>>(h->dc, h->map, h->normal, dst, a, h->center[2],
+                                                                       h->cfg.use_only_above_for_upper_bound);
+  LAUNCH_CHECK();
+  if (!out_is_device) {
+    CK(cudaMemcpyAsync(out, dst, sizeof(float) * total, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+  }
+  return EMAP_OK;
+}
+
+static_assert(EMAP_TRANSFORM_TOLERANCE == TSUB_ORTHO_TOL && EMAP_TRANSFORMED_WINDOWS_PER_LAUNCH == TSUB_MAX_WINDOWS,
+              "emap.h states the transformed windows' limits");
+
+// Why n windows and their transforms are rejected (nullptr: accepted); else the new maps' geometry (transformed_window)
+// in g.
+static const char* transformed_windows(int32_t cell_n, double res, const double m[2], int32_t n, const double* windows,
+                                       const double* transforms, std::vector<TSubGeom>& g) {
+  if (!submap_lengths_ok(n, windows)) return "lengths must be finite and >= 0";
+  for (int32_t w = 0; w < n; w++)
+    if (!tsub_transform_ok(transforms + 12 * w))
+      return "a transform is not finite or its R is not orthonormal within EMAP_TRANSFORM_TOLERANCE";
+  g.resize(n);
+  for (int32_t w = 0; w < n; w++) transformed_window(cell_n, res, m, windows + 4 * w, transforms + 12 * w, g[w]);
+  return nullptr;
+}
+
+// info {success, rows, cols} and geometry {centre, length} of every new map
+static void write_transformed(const std::vector<TSubGeom>& g, int32_t* info, double* geometry) {
+  for (size_t w = 0; w < g.size(); w++) {
+    info[3 * w] = g[w].win[0]; info[3 * w + 1] = g[w].size[0]; info[3 * w + 2] = g[w].size[1];
+    for (int a = 0; a < 2; a++) { geometry[4 * w + a] = g[w].pos[a]; geometry[4 * w + 2 + a] = g[w].len[a]; }
+  }
+}
+
+// The host part of emap_get_transformed_submaps on its own (no handle, no device).
+int emap_transformed_submap_windows(int32_t cell_n, double resolution, const double center[2], int32_t n_windows,
+                                    const double* windows, const double* transforms, int32_t* info, double* geometry) {
+  std::vector<TSubGeom> g;
+  if (!center || !windows || !transforms || !info || !geometry || cell_n < 3 ||
+      !(std::isfinite(resolution) && resolution > 0.0) || n_windows < 0 ||
+      transformed_windows(cell_n, resolution, center, n_windows, windows, transforms, g))
+    return EMAP_ERR_INVALID;
+  write_transformed(g, info, geometry);
+  return EMAP_OK;
+}
+
+// get_raw_submap with a request frame other than the map frame (elevation_mapping_ros.cpp:507-553 with grid_map's
+// getTransformedMap): the geometry on the host (transformed_window), then per launch of up to TSUB_MAX_WINDOWS windows
+// the two scatter passes and the gather (csrc/emap_submap.cuh), each launch's table in its parameters.  Output, stream
+// and graph rules as emap_get_submaps; every check runs before anything is written or launched.
+int emap_get_transformed_submaps(emap_handle* h, int32_t n_windows, const double* windows, const double* transforms,
+                                 double sample_ratio, int32_t n_layers, const char* const* names,
+                                 const float* const* planes_device, const int32_t* flags, float* out,
+                                 int32_t out_is_device, int64_t out_floats, int32_t* info, double* geometry) {
+  ENTER(h);
+  NvtxRange nv("emap:get_transformed_submaps");
+  if (!windows || !transforms || !names || !out || !info || !geometry)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: null argument");
+  if (n_windows < 1 || n_windows > EMAP_SUBMAP_MAX_WINDOWS)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: 1 to EMAP_SUBMAP_MAX_WINDOWS windows required");
+  if (n_layers < 1 || n_layers > EMAP_SUBMAP_MAX_LAYERS)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: 1 to EMAP_SUBMAP_MAX_LAYERS layers required");
+  const int W = h->dc.W;
+  const double res = h->cfg.resolution;
+  const double m[2] = {h->center[0], h->center[1]};
+  std::vector<TSubGeom> g;
+  if (const char* e = transformed_windows(W, res, m, n_windows, windows, transforms, g))
+    return fail(h, EMAP_ERR_INVALID, (std::string("emap_get_transformed_submaps: ") + e).c_str());
+  if (!(std::isfinite(sample_ratio) && sample_ratio >= 0.0))
+    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: sample_ratio must be finite and >= 0");
+  ExportList L;
+  if (!export_list(h, n_layers, names, planes_device, flags, L)) return EMAP_ERR_INVALID;
+  long long cells = 0;
+  for (int w = 0; w < n_windows; w++) {
+    const long long n = (long long)g[w].size[0] * g[w].size[1];
+    if (n > INT32_MAX - TSUB_THREADS)
+      return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: a new map of 2^31 cells or more");
+    cells += n;
+  }
+  if (n_layers * cells > out_floats)
+    return fail(h, EMAP_ERR_INVALID, "emap_get_transformed_submaps: out_floats is below the layers times the new maps' cells");
+  write_transformed(g, info, geometry);
+  if (!cells) return EMAP_OK;
+  int rc;
+  if ((rc = grow(h, h->tsub.key1, (size_t)cells, 0, true)) || (rc = grow(h, h->tsub.key2, (size_t)cells, 0, true))) return rc;
+  float* dst = out;
+  if (!out_is_device) {
+    if ((rc = grow(h, h->d_export, (size_t)(n_layers * cells), 0, false))) return rc;
+    dst = h->d_export;
+  }
+  const bool colour = export_has_colour(L);
+  TSubArgs a;
+  a.L = L;
+  a.n_samples = sample_ratio > 0.0 ? 5 : 1;
+  a.res = res;
+  a.s = res * sample_ratio;
+  long long cell0 = 0;
+  for (int w0 = 0; w0 < n_windows;) {
+    a.n_win = 0;
+    int blk_src = 0, blk_dst = 0;
+    for (; w0 < n_windows && a.n_win < TSUB_MAX_WINDOWS; w0++) {
+      const TSubGeom& q = g[w0];
+      if (!q.win[0] || !q.size[0] || !q.size[1]) continue;
+      TSubWin& s = a.win[a.n_win++];
+      for (int k = 0; k < 9; k++) s.R[k] = transforms[12 * w0 + k];
+      for (int k = 0; k < 3; k++) s.t[k] = transforms[12 * w0 + 9 + k];
+      s.x0 = q.centre[0] + (0.5 * (q.win[3] * res) - 0.5 * res);
+      s.y0 = q.centre[1] + (0.5 * (q.win[4] * res) - 0.5 * res);
+      for (int k = 0; k < 2; k++) { s.pos[k] = q.pos[k]; s.len[k] = q.len[k]; }
+      s.r0 = (int16_t)(W - 2 - q.win[1]); s.c0 = (int16_t)(W - 2 - q.win[2]);
+      s.rows = (int16_t)q.win[3]; s.cols = (int16_t)q.win[4];
+      s.nrows = q.size[0]; s.ncols = q.size[1];
+      s.blk_src = blk_src; s.blk_dst = blk_dst; s.cell0 = cell0;
+      blk_src += cdiv((i64)q.win[3] * q.win[4], TSUB_THREADS);
+      blk_dst += cdiv((i64)q.size[0] * q.size[1], TSUB_THREADS);
+      cell0 += (long long)q.size[0] * q.size[1];
+    }
+    if (!a.n_win) continue;
+    k_tsub_scatter<1><<<blk_src, TSUB_THREADS, 0, h->stream>>>(h->dc, h->map, h->tsub.key1, h->tsub.key2, a, h->center[2]);
+    LAUNCH_CHECK();
+    k_tsub_scatter<2><<<blk_src, TSUB_THREADS, 0, h->stream>>>(h->dc, h->map, h->tsub.key1, h->tsub.key2, a, h->center[2]);
+    LAUNCH_CHECK();
+    const auto gather = colour ? k_tsub_gather<true> : k_tsub_gather<false>;
+    gather<<<blk_dst, TSUB_THREADS, 0, h->stream>>>(h->dc, h->map, h->normal, h->tsub.key1, h->tsub.key2, dst, a,
+                                                    h->center[2], h->cfg.use_only_above_for_upper_bound);
+    LAUNCH_CHECK();
+  }
+  if (!out_is_device) {
+    CK(cudaMemcpyAsync(out, dst, sizeof(float) * n_layers * cells, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+  }
+  return EMAP_OK;
+}
+
+// ---- plane segmentation of one window (emap_segment_planes, csrc/emap_planes.cuh) ----------------------------------
+
+// The scratch of a window of n cells with `slots` label slots, one block: the window, two image planes (fill / median
+// ping-pong), union-find parents, flags and ranks, fill keys, the planarity masks, scan block sums, the header words,
+// the label statistics and decisions, and the host output's staging (info, plane table, layers).
+namespace {
+
+struct PlaneScratch {
+  float *raw, *img[2];
+  int *parent, *flag, *rank, *lab, *bsum, *hdr, *keep;
+  unsigned* key;
+  unsigned char *bin, *tmp, *bg;
+  unsigned long long* st;
+  int32_t* info;
+  double* planes;
+  float* layers;
+};
+
+size_t carve_planes(int64_t n, int64_t slots, int64_t plane_rows, bool host_out, void* base, PlaneScratch& s) {
+  Carver c{(uintptr_t)base};
+  const int64_t m = std::max(n, slots);
+  s.raw = c.take<float>(n); s.img[0] = c.take<float>(n); s.img[1] = c.take<float>(n);
+  s.parent = c.take<int>(n); s.flag = c.take<int>(m); s.rank = c.take<int>(m); s.lab = c.take<int>(n);
+  s.bsum = c.take<int>(m / PL_SCAN + 1); s.hdr = c.take<int>(8); s.keep = c.take<int>(slots);
+  s.key = c.take<unsigned>(n);
+  s.bin = c.take<unsigned char>(n); s.tmp = c.take<unsigned char>(n); s.bg = c.take<unsigned char>(slots);
+  s.st = c.take<unsigned long long>(slots * PL_STAT);
+  s.info = c.take<int32_t>(host_out ? 8 : 0);
+  s.planes = c.take<double>(host_out ? 7 * plane_rows : 0);
+  s.layers = c.take<float>(host_out ? 4 * n : 0);
+  return c.bytes;
+}
+
+// Raster-order ranks of the n flags in s.flag into s.rank, the count into *total (three launches).
+int plane_scan(emap_handle* h, const PlaneScratch& s, int64_t n, int* total) {
+  const int nb = cdiv(n, PL_SCAN);
+  k_pl_scan_blocks<<<nb, PL_SCAN, 0, h->stream>>>(s.flag, (int)n, s.bsum);
+  LAUNCH_CHECK();
+  k_pl_scan_top<<<1, PL_SCAN, 0, h->stream>>>(s.bsum, nb, total);
+  LAUNCH_CHECK();
+  k_pl_scan_rank<<<nb, PL_SCAN, 0, h->stream>>>(s.flag, (int)n, s.bsum, s.rank);
+  LAUNCH_CHECK();
+  return 0;
+}
+
+// Union-find merge and flatten of the cells whose parent is >= 0.
+int plane_components(emap_handle* h, const PlaneScratch& s, int rows, int cols, int conn8) {
+  const int64_t n = (int64_t)rows * cols;
+  k_pl_uf_merge<<<cdiv(n, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.parent, rows, cols, conn8);
+  LAUNCH_CHECK();
+  k_pl_uf_flatten<<<cdiv(n, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.parent, (int)n);
+  LAUNCH_CHECK();
+  return 0;
+}
+
+}  // namespace
+
+static_assert(EMAP_PLANE_EIGEN_MIN == PL_EIG_MIN, "emap.h states the fit's threshold");
+
+// Why p is rejected (nullptr: accepted) for a map of resolution `res`.
+static const char* plane_params_error(const emap_plane_params& p, double res) {
+  if (p.ransac) return "emap_segment_planes: RANSAC refinement is not supported (ransac must be 0)";
+  const int mk = std::max(1, std::min(p.median_kernel, 5));
+  if (mk != 1 && mk != 3 && mk != 5) return "emap_segment_planes: the median kernel must clamp to 1, 3 or 5";
+  if (p.median_repeats < 0 || p.median_repeats > EMAP_PLANE_MAX_REPEATS)
+    return "emap_segment_planes: median_repeats must be in [0, EMAP_PLANE_MAX_REPEATS]";
+  if (std::isnan(p.resolution) || (p.resolution > 0.0 && !(std::fabs(res - p.resolution) < 1e-6)))
+    return "emap_segment_planes: resampling is not supported (resolution must be <= 0 or the map's)";
+  if (p.kernel_size < 3 || p.kernel_size % 2 == 0 || p.kernel_size > EMAP_PLANE_MAX_KERNEL)
+    return "emap_segment_planes: kernel_size must be odd, >= 3 and <= EMAP_PLANE_MAX_KERNEL";
+  if (p.opening < 0 || p.opening > EMAP_PLANE_MAX_OPENING)
+    return "emap_segment_planes: opening must be in [0, EMAP_PLANE_MAX_OPENING]";
+  if (p.connectivity != 4 && p.connectivity != 8) return "emap_segment_planes: connectivity must be 4 or 8";
+  if (!std::isfinite(p.plane_inclination_cos) || !std::isfinite(p.local_inclination_cos) ||
+      !std::isfinite(p.patch_error))
+    return "emap_segment_planes: the inclination cosines and the patch error must be finite";
+  return nullptr;
+}
+
+int64_t emap_plane_capacity(int64_t rows, int64_t cols, const emap_plane_params* params) {
+  if (!params || rows < 0 || cols < 0) return -1;
+  return rows * cols / std::max(params->min_points, 3);
+}
+
+// The plane decomposition node's segmented planes map for one window (ConvexPlaneDecompositionRos.cpp:115-149 up to
+// SlidingWindowPlaneExtractor, without RANSAC): the window by k_submap, then the passes of csrc/emap_planes.cuh.  Host
+// output: the copies and one synchronisation; device output: stream-ordered, no synchronisation.  Every check runs
+// before anything is written or launched.
+int emap_segment_planes(emap_handle* h, const double window[4], const emap_plane_params* params, float* layers_out,
+                        int32_t out_is_device, int64_t out_floats, double* planes_out, int64_t planes_capacity,
+                        int32_t* info) {
+  ENTER(h);
+  NvtxRange nv("emap:segment_planes");
+  if (!window || !params || !layers_out || !planes_out || !info)
+    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: null argument");
+  if (!submap_lengths_ok(1, window)) return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: lengths must be finite and >= 0");
+  const emap_plane_params p = *params;
+  const double res = h->cfg.resolution;
+  if (const char* e = plane_params_error(p, res)) return fail(h, EMAP_ERR_INVALID, e);
+  const int W = h->dc.W;
+  const double m[2] = {h->center[0], h->center[1]};
+  int32_t q[5];
+  double centre[2];
+  submap_window(W, res, m, window, q, centre);
+  const int rows = q[3], cols = q[4];
+  const int64_t n = (int64_t)rows * cols;
+  if (q[0] && out_floats < 4 * n)
+    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: out_floats is below 4 * rows * cols");
+  const int64_t plane_rows = emap_plane_capacity(rows, cols, &p);
+  if (q[0] && planes_capacity < plane_rows)
+    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: planes_capacity is below emap_plane_capacity()");
+  if (!q[0]) {
+    if (out_is_device) CK(cudaMemsetAsync(info, 0, 5 * sizeof(int32_t), h->stream));
+    else memset(info, 0, 5 * sizeof(int32_t));
+    return EMAP_OK;
+  }
+  // labels are at most ceil(n / 2) (a 4-connected checkerboard), plus 0.  The statistics are sized and zeroed for that
+  // worst case (128 bytes a slot) because the label count is known only on the device.
+  const int64_t slots = n / 2 + 2;
+  PlaneScratch s;
+  int rc = grow(h, h->planes.block, carve_planes(n, slots, plane_rows, !out_is_device, nullptr, s), 0, false);
+  if (rc) return rc;
+  const size_t used = carve_planes(n, slots, plane_rows, !out_is_device, h->planes.block, s);
+  float* dst = out_is_device ? layers_out : s.layers;
+  double* dst_planes = out_is_device ? planes_out : s.planes;
+  int32_t* dst_info = out_is_device ? info : s.info;
+  // the window: k_submap's elevation layer into s.raw
+  SubmapArgs a;
+  const char* elevation = "elevation";
+  if (!export_list(h, 1, &elevation, nullptr, nullptr, a.L)) return EMAP_ERR_CUDA;
+  a.n_win = 0;
+  int tiles = 0;
+  long long total = 0;
+  submap_add(a, W, q, 1, tiles, total);
+  k_submap<false><<<dim3(tiles, 1), dim3(32, SUBMAP_ROWS), 0, h->stream>>>(h->dc, h->map, h->normal, s.raw, a, h->center[2],
+                                                                           h->cfg.use_only_above_for_upper_bound);
+  LAUNCH_CHECK();
+  CK(cudaMemsetAsync(s.hdr, 0, 8 * sizeof(int), h->stream));
+  CK(cudaMemsetAsync(s.st, 0, sizeof(unsigned long long) * slots * PL_STAT, h->stream));
+  const int cb = cdiv(n, PL_THREADS);
+  // fill: minValues' fixed point per NaN component
+  k_pl_fill_init<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, s.hdr, (int)n);
+  LAUNCH_CHECK();
+  if ((rc = plane_components(h, s, rows, cols, 0))) return rc;
+  k_pl_fill_min<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, rows, cols);
+  LAUNCH_CHECK();
+  k_pl_fill_write<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, s.img[0], (int)n);
+  LAUNCH_CHECK();
+  // median, numberOfRepeats times
+  const int mk = std::max(1, std::min(p.median_kernel, 5));
+  int cur = 0;
+  if (mk > 1)
+    for (int r = 0; r < p.median_repeats; r++, cur ^= 1) {
+      (mk == 3 ? k_pl_median<3> : k_pl_median<5>)<<<cb, PL_THREADS, 0, h->stream>>>(s.img[cur], s.img[cur ^ 1], rows, cols);
+      LAUNCH_CHECK();
+    }
+  const float* img = s.img[cur];
+  // sliding-window planarity, opening, labels
+  k_pl_fit<<<cb, PL_THREADS, 0, h->stream>>>(img, s.bin, rows, cols, p.kernel_size, res, p.patch_error * p.patch_error,
+                                             p.local_inclination_cos);
+  LAUNCH_CHECK();
+  if (p.opening > 0) {
+    k_pl_morph<false><<<cb, PL_THREADS, 0, h->stream>>>(s.bin, s.tmp, rows, cols, p.opening);
+    LAUNCH_CHECK();
+    k_pl_morph<true><<<cb, PL_THREADS, 0, h->stream>>>(s.tmp, s.bin, rows, cols, p.opening);
+    LAUNCH_CHECK();
+  }
+  k_pl_cc_init<<<cb, PL_THREADS, 0, h->stream>>>(s.bin, s.parent, s.key, s.flag, (int)n);
+  LAUNCH_CHECK();
+  const bool conn8 = p.connectivity == 8;
+  if ((rc = plane_components(h, s, rows, cols, conn8))) return rc;
+  (conn8 ? k_pl_first<2> : k_pl_first<1>)<<<cb, PL_THREADS, 0, h->stream>>>(s.parent, s.key, rows, cols);
+  LAUNCH_CHECK();
+  k_pl_first_flag<<<cb, PL_THREADS, 0, h->stream>>>(s.parent, s.key, s.flag, (int)n);
+  LAUNCH_CHECK();
+  const int64_t n_blocks = conn8 ? (int64_t)cdiv(rows, 2) * cdiv(cols, 2) : n;
+  if ((rc = plane_scan(h, s, n_blocks, s.hdr + 1))) return rc;
+  k_pl_label<<<cb, PL_THREADS, 0, h->stream>>>(s.parent, s.key, s.rank, s.lab, (int)n);
+  LAUNCH_CHECK();
+  // per-label planes
+  k_pl_stats<<<cdiv(cdiv(n, PL_RUN), PL_THREADS), PL_THREADS, 0, h->stream>>>(img, s.lab, s.st, rows, cols);
+  LAUNCH_CHECK();
+  const PlaneLabelArgs la = {centre[0] + (0.5 * (rows * res) - 0.5 * res), centre[1] + (0.5 * (cols * res) - 0.5 * res),
+                             res, p.plane_inclination_cos, p.min_points};
+  k_pl_decide<<<cdiv(slots, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.st, s.hdr, s.flag, s.bg, (int)slots, la);
+  LAUNCH_CHECK();
+  if ((rc = plane_scan(h, s, slots, s.hdr + 2))) return rc;
+  k_pl_planes<<<cdiv(slots, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.st, s.rank, s.hdr, dst_planes, (int)slots, la);
+  LAUNCH_CHECK();
+  k_pl_out<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, img, s.lab, s.bg, s.hdr, dst, dst_info, rows, cols);
+  LAUNCH_CHECK();
+  if (!out_is_device) {
+    // info, the plane table and the layers are the block's tail: one copy, one synchronisation, and the caller's
+    // buffers take the layers and planes only when the window had a finite cell
+    const size_t off = (char*)s.info - (char*)h->planes.block, bytes = used - off;
+    if (h->planes.host.size() < bytes) CK(h->planes.host.alloc(bytes));
+    CK(cudaMemcpyAsync(h->planes.host, s.info, bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    PlaneScratch t;
+    carve_planes(n, slots, plane_rows, true, (char*)h->planes.host - off, t);
+    memcpy(info, t.info, 5 * sizeof(int32_t));
+    if (info[0]) {
+      memcpy(planes_out, t.planes, sizeof(double) * 7 * info[4]);
+      memcpy(layers_out, t.layers, sizeof(float) * 4 * n);
+    }
+  }
+  return EMAP_OK;
+}
+
+// The node's publishAsPointCloud (elevation_mapping_ros.cpp:501-505): the points of the exported elevation (map_cloud).
+int emap_get_map_points(emap_handle* h, float* xyz_host, int64_t* n_points) {
+  ENTER(h);
+  NvtxRange nv("emap:get_map_points");
+  if (!n_points || *n_points < 0 || (*n_points > 0 && !xyz_host))
+    return fail(h, EMAP_ERR_INVALID, "emap_get_map_points: null argument or negative capacity");
+  return map_cloud<false>(h, n_points, xyz_host, nullptr, nullptr);
+}
+
+// The node's publishNormalAsArrow (elevation_mapping_ros.cpp:751-778): the arrows of the exported normals (map_cloud).
+int emap_get_normal_arrows(emap_handle* h, int32_t* ids_host, double* segments_host, int64_t* n_arrows) {
+  ENTER(h);
+  NvtxRange nv("emap:get_normal_arrows");
+  if (!n_arrows || *n_arrows < 0 || (*n_arrows > 0 && (!ids_host || !segments_host)))
+    return fail(h, EMAP_ERR_INVALID, "emap_get_normal_arrows: null argument or negative capacity");
+  return map_cloud<true>(h, n_arrows, nullptr, ids_host, segments_host);
+}
+
+int emap_layer_device_ptr(emap_handle* h, const char* name, void** ptr) {
+  ENTER(h);
+  if (!name || !ptr) return fail(h, EMAP_ERR_INVALID, "null argument");
+  const size_t C = (size_t)h->dc.C;
+  int li = layer_index(name);
+  if (li >= 0) { *ptr = h->map + li * C; return EMAP_OK; }
+  if (!strcmp(name, "elevation_map")) { *ptr = h->map; return EMAP_OK; }
+  if (!strcmp(name, "normal_map") || !strcmp(name, "normal_x")) { *ptr = h->normal; return EMAP_OK; }
+  if (!strcmp(name, "normal_y")) { *ptr = h->normal + C; return EMAP_OK; }
+  if (!strcmp(name, "normal_z")) { *ptr = h->normal + 2 * C; return EMAP_OK; }
+  if (!strcmp(name, "traversability_input")) { *ptr = h->trav_input; return EMAP_OK; }
+  h->err = std::string("Layer ") + name + " is not in the map";
+  return EMAP_ERR_NOLAYER;
+}
+
+int emap_exists_layer(const emap_handle* h, const char* name) {
+  if (!h || !name) return 0;
+  return layer_index(name) >= 0 ? 1 : 0;
+}
+
+}  // extern "C"

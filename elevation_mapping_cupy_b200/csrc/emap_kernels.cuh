@@ -14,31 +14,9 @@
 // makes every result independent of thread order, run-to-run deterministic and bit-identical to
 // oracle/emap_oracle.c; they are within one fp32 rounding of some order of the reference atomics.
 #pragma once
-#include <cuda.h>                 // CUtensorMap (type only; the encoder is fetched at run time, emap_api.cu)
+#include <cuda.h>                 // CUtensorMap (type only; the encoder is fetched at run time, make_post_tm)
 #include "emap_plan.cuh"         // RT, RayGrid, RC_STRIDE, RcLayout, PT_X, PT_Y
 #include "emap_sources.cuh"
-
-// ------------------------------------------------------------------------------------------
-// per-cell scratch of a frame; all zero between frames (k_finalize re-zeroes what it consumed)
-struct CellScratch {
-  u64* cnt_ai;     // low word: newmap[4] all points of the cell (CK.py:336), high word: newmap[3] drift inliers (CK.py:334).
-                   // One 64-bit accumulation per point carries both (one multimem.red per run in sharded frames).
-  u64* cnt_fo;     // low word: newmap[2] fused points (CK.py:185), high word: atomicAdd(map[1], outlier_variance) count
-                   // of outlier points (CK.py:174)
-  u32* n_ray;      // ... by penetrating rays, CK.py:251
-  i64* SH;         // sum new_h   CK.py:183
-  i64* SV;         // sum new_v   CK.py:184
-  i64* DV;         // sum of validity decrements CK.py:250
-  u64* last;       // (global point index << 32 | bits(new_h)) max  -> upper_bound of a hit cell, CK.py:191
-  float* thr;      // first-level ray record, 4 B: a sample at height nz can only act on the cell if !(nz > thr)
-  uint2* rec;      // second-level ray record, 8 B: {valid cell ? bits(h') : upper-bound key, flags}; read-only for rays
-  u32* ukv;        // min over rays of the upper-bound key carved into the cell (UKEY_NONE between frames), CK.py:230-233,253-256
-  unsigned char* dirty;   // 1 = some kernel of this frame touched the cell's scratch (k_finalize takes its full path there
-                   // and clears it); nullptr in sharded frames, where the marker is derived from cnt_all / ukv
-  i64 mc_off;      // sharded frames: byte offset from a local scratch address to its NVLink MULTICAST alias
-                   // (0 = single GPU).  Non-zero: every accumulation is one multimem.red that the NVSwitch
-                   // applies to the replicas of ALL ranks (this one included) -- scatter and collective fused.
-};
 
 // accumulate into the per-cell scratch: local L2 atomic, or one in-switch multicast reduction
 __device__ __forceinline__ void red_add(u32* p, u32 v, i64 mc) {
@@ -414,7 +392,7 @@ __device__ __forceinline__ float add_n_times(float v, float c, u32 n) {
 //              cells / upper-bound key for invalid ones, .y = RF_* flags.
 // The variance a ray needs (CK.py:239) is rebuilt on the second level from map[1] and n_out.
 // Only the cells a ray of this frame can reach are recorded: box = sensor cell +- (max_ray_length / resolution + slack),
-// rows [box.x, box.y) x columns [box.z, box.w) (columns a multiple of V), computed on the host (ray_box in emap_api.cu).
+// rows [box.x, box.y) x columns [box.z, box.w) (columns a multiple of V), computed on the host (ray_box in emap_plan.cuh).
 // Also reduces thr to the coarse map tmap: max over each 2^ts x 2^ts tile (order-preserving keys, atomicMax; zeroed
 // by k_drift) -- a ray above a tile's maximum cannot act on any of its cells (k_raycast).
 template <int V>
@@ -1146,232 +1124,4 @@ __global__ void __launch_bounds__(256) k_update_time(const DevCfg c, float* __re
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= c.C) return;
   map[4 * c.C + i] = __fadd_rn(map[4 * c.C + i], c.time_int_f);
-}
-
-// EM.py:913-922 after the map initialiser: dilation_filter_kernel (CK.py:392-449) of the elevation into invalid cells with
-// mask = is_valid -- the reference runs it IN PLACE (racy); here every pass reads the previous pass's planes (src) and
-// writes the map -- and update_upper_bound_with_valid_elevation (EM.py:428-432) on the last pass.
-__global__ void __launch_bounds__(256)
-k_init_dilate(const DevCfg c, const float* __restrict__ src_h, const float* __restrict__ src_valid, float* __restrict__ map,
-              int k, int last) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= c.C) return;
-  const int W = c.W, C = c.C;
-  float h = src_h[i], valid = src_valid[i];
-  if (valid < 0.5f) {
-    float distance = 100.f, near_value = 0.f;
-    for_window(W, C, i, k, [&](int idx, int dy, int dx) {
-      if ((src_valid[idx] > 0.5f) & ((float)(dx + dy) < distance)) { distance = (float)(dx + dy); near_value = src_h[idx]; }
-    });
-    if (distance < 100.f) { h = near_value; valid = 1.0f; }
-  }
-  map[i] = h; map[2 * C + i] = valid;
-  if (last && valid > 0.5f) { map[5 * C + i] = h; map[6 * C + i] = 0.f; }     // EM.py:430-432
-}
-
-// ------------------------------------------------------------------------------------------
-// export EM.py:579-670,720-775: NaN-fill, +center_z, crop the border ring, flip both axes.
-// kind: 0 elevation, 1 variance, 2 traversability, 3 time, 4 upper_bound, 5 is_upper_bound, 6..8 normal xyz,
-// 10 normal_color (normal_color_value)
-// kind 9: arbitrary plane with flags (bit0 fill_nan, bit1 add_z) = process_map_for_publish (EM.py:579-596)
-// export_cell: the value of state cell (r, cc); export_value: of exported cell o (row-major over the (W-2)^2 output).
-// COLOUR: whether kind 10 can occur.  Only a call that asks for normal_color runs the COLOUR instantiation, so every
-// other export runs the same code it ran before that kind existed.
-#define EXPORT_KIND_PLANE 9
-#define EXPORT_KIND_NORMAL_COLOR 10
-
-// The bridge's addNormalColorLayer (WRAP:296-314) for one cell, restated from grid_map's colorVectorToValue
-// (GridMapMath.cpp; not checked against a grid_map build): c = ((nx + 1) / 2, (ny + 1) / 2) in double, each rounded to
-// float, and nz; channel = int(c * 255.0f) (float product, truncated toward zero); the value is the float whose bits
-// are (r << 16) | (g << 8) | b.  A channel whose product is NaN is 0, one beyond the int32 range saturates (the
-// reference's int cast is undefined there; the frame only writes unit normals, whose channels are in [-255, 255]).
-__device__ __forceinline__ float normal_color_value(float nx, float ny, float nz) {
-  const float cx = __double2float_rn(__dmul_rn(__dadd_rn((double)nx, 1.0), 0.5));   // x / 2.0 == x * 0.5, exactly
-  const float cy = __double2float_rn(__dmul_rn(__dadd_rn((double)ny, 1.0), 0.5));
-  const unsigned r = (unsigned)__float2int_rz(__fmul_rn(cx, 255.0f));
-  const unsigned g = (unsigned)__float2int_rz(__fmul_rn(cy, 255.0f));
-  const unsigned b = (unsigned)__float2int_rz(__fmul_rn(nz, 255.0f));
-  return __uint_as_float((r << 16) | (g << 8) | b);
-}
-template <bool COLOUR = false>
-__device__ __forceinline__ float export_cell(const DevCfg& c, const float* __restrict__ map, const float* __restrict__ normal,
-                                             int r, int cc, int kind, float center_z, int only_above,
-                                             const float* __restrict__ plane, int flags) {
-  const int i = r * c.W + cc, C = c.C;
-  const float nanv = __int_as_float(0x7fc00000);
-  const float valid = map[2 * C + i], isup = map[6 * C + i], upper = map[5 * C + i];
-  float v;
-  switch (kind) {
-    case 0: v = (valid > 0.5f) ? __fadd_rn(map[i], center_z) : nanv; break;
-    case 1: v = map[C + i]; break;
-    case 2: {   // EM.py:615-628: NaN where neither valid nor upper-bounded; only [3:-3] is ever defined
-      const bool in33 = r >= 3 && r <= c.W - 4 && cc >= 3 && cc <= c.W - 4;
-      v = (in33 && __fadd_rn(valid, isup) > 0.5f) ? map[3 * C + i] : nanv; break; }
-    case 3: v = map[4 * C + i]; break;
-    case 4: case 5: {
-      const bool ok = only_above ? ((upper > 0.f && isup > 0.5f) || valid > 0.5f) : (valid > 0.5f || isup > 0.5f);
-      v = ok ? (kind == 4 ? __fadd_rn(upper, center_z) : isup) : nanv; break; }
-    case EXPORT_KIND_PLANE: {
-      v = plane[i];
-      if ((flags & 1) && !(valid > 0.5f)) v = nanv;
-      if (flags & 2) v = __fadd_rn(v, center_z);
-      break; }
-    default:
-      v = (COLOUR && kind == EXPORT_KIND_NORMAL_COLOR) ? normal_color_value(normal[i], normal[C + i], normal[2 * C + i])
-                                                       : normal[(size_t)(kind - 6) * C + i];
-      break;
-  }
-  return v;
-}
-template <bool COLOUR>
-__device__ __forceinline__ float export_value(const DevCfg& c, const float* __restrict__ map, const float* __restrict__ normal,
-                                              int o, int kind, float center_z, int only_above, const float* __restrict__ plane,
-                                              int flags) {
-  const int Wo = c.W - 2;
-  const int orow = o / Wo, ocol = o - orow * Wo;
-  const int r = Wo - 1 - orow + 1, cc = Wo - 1 - ocol + 1;         // flip(0), flip(1) of m[1:-1,1:-1]
-  return export_cell<COLOUR>(c, map, normal, r, cc, kind, center_z, only_above, plane, flags);
-}
-
-// One launch exports a list of layers (WRAP:213-252 get_grid_map asks for several): blockIdx.y = layer.
-#define EXPORT_MAX_LAYERS 24
-struct ExportList { int n; int kind[EXPORT_MAX_LAYERS]; int flags[EXPORT_MAX_LAYERS]; const float* plane[EXPORT_MAX_LAYERS]; };
-// Whether a list asks for normal_color: k_export_multi and k_submap run their COLOUR instantiation only then.
-inline bool export_has_colour(const ExportList& L) {
-  for (int k = 0; k < L.n; k++)
-    if (L.kind[k] == EXPORT_KIND_NORMAL_COLOR) return true;
-  return false;
-}
-template <bool COLOUR>
-__global__ void __launch_bounds__(256)
-k_export_multi(const DevCfg c, const float* __restrict__ map, const float* __restrict__ normal, float* __restrict__ out,
-               const ExportList L, float center_z, int only_above) {
-  const int Wo = c.W - 2;
-  const int o = blockIdx.x * blockDim.x + threadIdx.x;
-  const int l = blockIdx.y;
-  if (o >= Wo * Wo) return;
-  out[(size_t)l * Wo * Wo + o] =
-      export_value<COLOUR>(c, map, normal, o, L.kind[l], center_z, only_above, L.plane[l], L.flags[l]);
-}
-
-// ------------------------------------------------------------------------------------------
-// plugins
-// plugins/min_filter.py:57-82 with Jacobi order (reads iteration k-1, writes iteration k).
-// `unfilled[it]` counts cells whose mask is still <= 0.5 after iteration it; an iteration whose
-// predecessor left none is skipped on the device (min_filter.py:115 breaks on the host instead).
-// MAX: plugins/max_filter.py:68-88 -- same stencil with max, and the fill test looks at the CURRENT mask
-// (max_filter.py:102-108 passes copies of the running arrays), where min_filter keeps testing the ORIGINAL one.
-template <bool MAX>
-__global__ void __launch_bounds__(256)
-k_fill_filter_iter(const DevCfg c, int k, const float* __restrict__ mask0, const float* __restrict__ in_h,
-                   const float* __restrict__ in_m, float* __restrict__ out_h, float* __restrict__ out_m,
-                   int* __restrict__ unfilled, int it) {
-  if (it > 0 && unfilled[it - 1] == 0) { if (blockIdx.x == 0 && threadIdx.x == 0) unfilled[it] = 0; return; }
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  int miss = 0;
-  if (i < c.C) {
-    float h = in_h[i], m = in_m[i];
-    if ((MAX ? m : mask0[i]) < 0.5f) {
-      const float none = MAX ? -1000000.0f : 1000000.0f;
-      float mv = none;
-      for_window(c.W, c.C, i, k, [&](int idx, int, int) {
-        const float val = in_h[idx];
-        if (in_m[idx] > 0.5f && (MAX ? val > mv : val < mv)) mv = val;
-      });
-      if (MAX ? mv > none + 1.f : mv < none - 1.f) { h = mv; m = 0.6f; }
-    }
-    out_h[i] = h; out_m[i] = m;
-    miss = !(m > 0.5f);
-  }
-  miss = __syncthreads_count(miss);
-  if (threadIdx.x == 0 && miss) atomicAdd(unfilled + it, miss);
-}
-// final select: the result is in buffer parity (first it with unfilled[it]==0, else iteration_n-1)
-__global__ void __launch_bounds__(256)
-k_min_filter_final(const DevCfg c, const float* __restrict__ hA, const float* __restrict__ mA,
-                   const float* __restrict__ hB, const float* __restrict__ mB, const int* __restrict__ unfilled,
-                   int iteration_n, float* __restrict__ out, int* __restrict__ iters_run) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  int last = iteration_n - 1;
-  for (int it = 0; it < iteration_n; it++) if (unfilled[it] == 0) { last = it; break; }
-  if (i == 0 && iters_run) *iters_run = last + 1;
-  if (i >= c.C) return;
-  // iteration `it` wrote buffer (it & 1) ? A : B   (it 0 reads A(copy of input) -> writes B)
-  const float* h = (last & 1) ? hA : hB; const float* m = (last & 1) ? mA : mB;
-  out[i] = m[i] > 0.5f ? h[i] : __int_as_float(0x7fc00000);
-}
-
-// plugins/smooth_filter.py:57-58: one 1-D pass of a size-3 uniform filter, 'reflect' boundary,
-// double accumulation of x*(1/3) terms, fp32 store (cupyx.scipy.ndimage correlate1d).
-__global__ void __launch_bounds__(256)
-k_box3(const DevCfg c, const float* __restrict__ in, float* __restrict__ out, int axis) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= c.C) return;
-  const int W = c.W, r = i / W, cc = i - r * W;
-  const double w = 1.0 / 3.0;
-  int ia, ib;
-  if (axis == 0) { ia = (r == 0 ? 0 : r - 1) * W + cc; ib = (r == W - 1 ? W - 1 : r + 1) * W + cc; }
-  else { ia = r * W + (cc == 0 ? 0 : cc - 1); ib = r * W + (cc == W - 1 ? W - 1 : cc + 1); }
-  const double sacc = __dadd_rn(__dadd_rn(__dmul_rn((double)in[ia], w), __dmul_rn((double)in[i], w)), __dmul_rn((double)in[ib], w));
-  out[i] = (float)sacc;
-}
-
-// ------------------------------------------------------------------------------------------
-// plugins/erosion.py:96-113: min / max of the (optionally reversed) layer, 8-bit normalisation, cv.erode with a
-// ones(k,k) kernel (OpenCV folds `iterations` of a full rectangle into ONE erosion with a rectangle of side
-// k + (iterations-1)(k-1) anchored at (k/2)*iterations; pixels outside the image do not constrain the minimum),
-// de-normalisation.  mm = {min, max} as order-preserving keys.
-__global__ void __launch_bounds__(256)
-k_layer_minmax(const DevCfg c, const float* __restrict__ in, int reverse, u32* __restrict__ mm) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  u32 lo = 0xffffffffu, hi = 0u;
-  if (i < c.C) {
-    float x = in[i];
-    if (reverse) x = __fsub_rn(1.0f, x);
-    lo = hi = fkey(x);
-  }
-  lo = __reduce_min_sync(0xffffffffu, lo); hi = __reduce_max_sync(0xffffffffu, hi);
-  if ((threadIdx.x & 31) == 0) { atomicMin(mm, lo); atomicMax(mm + 1, hi); }
-}
-__global__ void __launch_bounds__(256)
-k_erode(const DevCfg c, const float* __restrict__ in, float* __restrict__ out, int ks, int anchor, int reverse,
-        const u32* __restrict__ mm) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= c.C) return;
-  const int W = c.W, r = i / W, cc = i - r * W;
-  const float mn = funkey(mm[0]), mx = funkey(mm[1]);
-  const float span = (float)((double)mx - (double)mn);            // python float difference, used as float32
-  int best = 255;
-  for (int dy = -anchor; dy < ks - anchor; dy++) {
-    const int rr = r + dy;
-    if (rr < 0 || rr >= W) continue;
-    for (int dx = -anchor; dx < ks - anchor; dx++) {
-      const int c2 = cc + dx;
-      if (c2 < 0 || c2 >= W) continue;
-      float x = in[rr * W + c2];
-      if (reverse) x = __fsub_rn(1.0f, x);
-      const int q = (int)(unsigned char)__float2int_rz(__fdiv_rn(__fmul_rn(__fsub_rn(x, mn), 255.0f), span));
-      best = min(best, q);
-    }
-  }
-  float y = __fadd_rn(__fdiv_rn(__fmul_rn((float)best, span), 255.0f), mn);
-  if (reverse) y = __fsub_rn(1.0f, y);
-  out[i] = y;
-}
-
-// plugins/robot_centric_elevation.py:66-83: z of the cell in the base frame, optionally thresholded.
-__global__ void __launch_bounds__(256)
-k_robot_centric(const DevCfg c, const float* __restrict__ elev, const float* __restrict__ valid, float* __restrict__ out,
-                float r6, float r7, float r8, double resolution, double threshold, int use_threshold) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= c.C) return;
-  const float rz = elev[i];
-  float o = rz;                                                   // self.min_filtered = elevation_map[0].copy()
-  if (valid[i] > 0.5f) {
-    const float rx = (float)((double)(i / c.W) * resolution), ry = (float)((double)(i % c.W) * resolution);
-    const float zb = __fmaf_rn(r8, rz, __fmaf_rn(r6, rx, __fmul_rn(r7, ry)));   // r0*x + r1*y + r2*z, nvcc contraction
-    if (use_threshold) o = ((double)zb >= threshold) ? 1.0f : 0.0f;
-    else o = zb;
-  }
-  out[i] = o;
 }

@@ -19,6 +19,8 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "emap_export.cuh"
+
 #define MC_TILE 32                 // exported rows of a chunk = exported columns of a tile (one warp's lanes)
 #define MC_THREADS 256             // 8 warps: each stages 4 tile rows, then walks 4 tile columns
 

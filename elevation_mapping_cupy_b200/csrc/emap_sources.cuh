@@ -10,6 +10,25 @@
 
 #define SEM_MAX_CH 16             // semantic channels of a frame (emap_semantic_configure)
 
+// The semantic point channels a frame fuses (emap_semantic_configure): which column of a point goes into which layer,
+// and how (emap_semantic.cuh).
+enum { SEM_AVERAGE = 0, SEM_CLASS_AVERAGE = 1, SEM_COLOR = 2, SEM_CLASS_BAYESIAN = 3, SEM_BAYESIAN_INFERENCE = 4,
+       SEM_CLASS_MAX = 5 };
+
+struct SemCfg {
+  int n_ch;                      // channels fused this frame (0: semantic fusion off)
+  int col[SEM_MAX_CH];           // column of the feature in a cloud row (>= 3)
+  int kind[SEM_MAX_CH];          // SEM_*
+  int layer[SEM_MAX_CH];         // layer of semantic_map the channel writes
+  int slot[SEM_MAX_CH];          // scratch slot: i64 sum plane (average and bayesian kinds) / first of 4 u32 planes
+                                 // (colour) / position among the class_max channels
+  double alpha;                  // parameter.py:163 average_weight (class_average)
+  int n_max;                     // class_max channels
+  float* sigma;                  // (n_layers, W, W) variance planes of bayesian_inference, caller-owned (or null)
+  int* id_max;                   // (n_id_max, W, W) class id of every class_max round, caller-owned (or null)
+  int n_id_max;
+};
+
 // One point's xyz.  fp32 rows padded to 4 floats (16-byte aligned): one 128-bit read-only load per point; other
 // layouts: three scalar loads (a warp's rows are contiguous, so they coalesce into the same sectors).
 template <typename T>

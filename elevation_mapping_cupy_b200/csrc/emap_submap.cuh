@@ -11,6 +11,8 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "emap_export.cuh"
+
 #define SUBMAP_MAX_WINDOWS 1024
 #define SUBMAP_ROWS 8              // output rows per work item: one warp per row
 
