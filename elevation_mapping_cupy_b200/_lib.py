@@ -39,6 +39,15 @@ class EmapPlaneParams(C.Structure):
                 ("local_inclination_cos", C.c_double), ("patch_error", C.c_double), ("ransac", C.c_int32)]
 
 
+class EmapRegionParams(C.Structure):
+    _fields_ = [("margin_size", C.c_int32), ("plane_height_offset", C.c_double)]
+
+
+class EmapRegionOut(C.Structure):
+    _fields_ = [("regions", C.c_void_p), ("regions_capacity", C.c_int64), ("polygons", C.c_void_p),
+                ("polygons_capacity", C.c_int64), ("vertices", C.c_void_p), ("vertices_capacity", C.c_int64)]
+
+
 class EmapDepthCamera(C.Structure):
     _fields_ = [("height", C.c_int32), ("width", C.c_int32), ("depth", C.c_void_p), ("confidence", C.c_void_p),
                 ("rgb", C.c_void_p), ("features", C.c_void_p), ("fx", C.c_double), ("fy", C.c_double),
@@ -111,6 +120,8 @@ SIGNATURES = {
     "emap_plane_capacity": (C.c_int64, [C.c_int64, C.c_int64, C.c_void_p]),
     "emap_segment_planes": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p,
                                       C.c_int64, C.c_void_p]),
+    "emap_extract_planar_regions": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
+                                              C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "emap_get_map_points": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_get_normal_arrows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_layer_device_ptr": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),

@@ -5,6 +5,7 @@
 #include "emap_export.cuh"
 #include "emap_submap.cuh"
 #include "emap_planes.cuh"
+#include "emap_regions.cuh"
 #include "emap_mapcloud.cuh"
 
 namespace {
@@ -348,7 +349,8 @@ int emap_get_transformed_submaps(emap_handle* h, int32_t n_windows, const double
 
 // The scratch of a window of n cells with `slots` label slots, one block: the window, two image planes (fill / median
 // ping-pong), union-find parents, flags and ranks, fill keys, the planarity masks, scan block sums, the header words,
-// the label statistics and decisions, and the host output's staging (info, plane table, layers).
+// the label statistics and decisions, and the host output's staging (info, plane table, layers, then `extra` bytes
+// that emap_extract_planar_regions stages its tables in).
 namespace {
 
 struct PlaneScratch {
@@ -360,9 +362,11 @@ struct PlaneScratch {
   int32_t* info;
   double* planes;
   float* layers;
+  char* extra;
 };
 
-size_t carve_planes(int64_t n, int64_t slots, int64_t plane_rows, bool host_out, void* base, PlaneScratch& s) {
+size_t carve_planes(int64_t n, int64_t slots, int64_t plane_rows, bool host_out, size_t extra, void* base,
+                    PlaneScratch& s) {
   Carver c{(uintptr_t)base};
   const int64_t m = std::max(n, slots);
   s.raw = c.take<float>(n); s.img[0] = c.take<float>(n); s.img[1] = c.take<float>(n);
@@ -371,22 +375,28 @@ size_t carve_planes(int64_t n, int64_t slots, int64_t plane_rows, bool host_out,
   s.key = c.take<unsigned>(n);
   s.bin = c.take<unsigned char>(n); s.tmp = c.take<unsigned char>(n); s.bg = c.take<unsigned char>(slots);
   s.st = c.take<unsigned long long>(slots * PL_STAT);
-  s.info = c.take<int32_t>(host_out ? 8 : 0);
+  s.info = c.take<int32_t>(host_out ? 16 : 0);
   s.planes = c.take<double>(host_out ? 7 * plane_rows : 0);
   s.layers = c.take<float>(host_out ? 4 * n : 0);
+  s.extra = c.take<char>(host_out ? extra : 0);
   return c.bytes;
 }
 
-// Raster-order ranks of the n flags in s.flag into s.rank, the count into *total (three launches).
-int plane_scan(emap_handle* h, const PlaneScratch& s, int64_t n, int* total) {
+// Raster-order ranks of the n values in flag into rank (exclusive sums where the value is not 0, else -1), their sum
+// into *total (three launches; bsum holds n / PL_SCAN + 1 words).
+int scan_ranks(emap_handle* h, const int* flag, int* rank, int* bsum, int64_t n, int* total) {
   const int nb = cdiv(n, PL_SCAN);
-  k_pl_scan_blocks<<<nb, PL_SCAN, 0, h->stream>>>(s.flag, (int)n, s.bsum);
+  k_pl_scan_blocks<<<nb, PL_SCAN, 0, h->stream>>>(flag, (int)n, bsum);
   LAUNCH_CHECK();
-  k_pl_scan_top<<<1, PL_SCAN, 0, h->stream>>>(s.bsum, nb, total);
+  k_pl_scan_top<<<1, PL_SCAN, 0, h->stream>>>(bsum, nb, total);
   LAUNCH_CHECK();
-  k_pl_scan_rank<<<nb, PL_SCAN, 0, h->stream>>>(s.flag, (int)n, s.bsum, s.rank);
+  k_pl_scan_rank<<<nb, PL_SCAN, 0, h->stream>>>(flag, (int)n, bsum, rank);
   LAUNCH_CHECK();
   return 0;
+}
+
+int plane_scan(emap_handle* h, const PlaneScratch& s, int64_t n, int* total) {
+  return scan_ranks(h, s.flag, s.rank, s.bsum, n, total);
 }
 
 // Union-find merge and flatten of the cells whose parent is >= 0.
@@ -399,27 +409,40 @@ int plane_components(emap_handle* h, const PlaneScratch& s, int rows, int cols, 
   return 0;
 }
 
+// One segmentation call's window and scratch, as plane_check and segment_window leave them.
+struct PlaneCall {
+  int32_t q[5];                    // submap_window: {success, r0, c0, rows, cols}
+  double centre[2];
+  int rows = 0, cols = 0;
+  int64_t n = 0, slots = 0, plane_rows = 0;
+  double ox = 0.0, oy = 0.0;       // the centre of window cell (0, 0)
+  PlaneScratch s;
+  size_t used = 0;
+  double* dst_planes = nullptr;    // where the plane table is written (the caller's or the staging)
+  int32_t* dst_info = nullptr;
+};
+
 }  // namespace
 
 static_assert(EMAP_PLANE_EIGEN_MIN == PL_EIG_MIN, "emap.h states the fit's threshold");
 
 // Why p is rejected (nullptr: accepted) for a map of resolution `res`.
 static const char* plane_params_error(const emap_plane_params& p, double res) {
-  if (p.ransac) return "emap_segment_planes: RANSAC refinement is not supported (ransac must be 0)";
+  if (p.ransac) return "RANSAC refinement is not supported (ransac must be 0)";
   const int mk = std::max(1, std::min(p.median_kernel, 5));
-  if (mk != 1 && mk != 3 && mk != 5) return "emap_segment_planes: the median kernel must clamp to 1, 3 or 5";
+  if (mk != 1 && mk != 3 && mk != 5) return "the median kernel must clamp to 1, 3 or 5";
   if (p.median_repeats < 0 || p.median_repeats > EMAP_PLANE_MAX_REPEATS)
-    return "emap_segment_planes: median_repeats must be in [0, EMAP_PLANE_MAX_REPEATS]";
+    return "median_repeats must be in [0, EMAP_PLANE_MAX_REPEATS]";
   if (std::isnan(p.resolution) || (p.resolution > 0.0 && !(std::fabs(res - p.resolution) < 1e-6)))
-    return "emap_segment_planes: resampling is not supported (resolution must be <= 0 or the map's)";
+    return "resampling is not supported (resolution must be <= 0 or the map's)";
   if (p.kernel_size < 3 || p.kernel_size % 2 == 0 || p.kernel_size > EMAP_PLANE_MAX_KERNEL)
-    return "emap_segment_planes: kernel_size must be odd, >= 3 and <= EMAP_PLANE_MAX_KERNEL";
+    return "kernel_size must be odd, >= 3 and <= EMAP_PLANE_MAX_KERNEL";
   if (p.opening < 0 || p.opening > EMAP_PLANE_MAX_OPENING)
-    return "emap_segment_planes: opening must be in [0, EMAP_PLANE_MAX_OPENING]";
-  if (p.connectivity != 4 && p.connectivity != 8) return "emap_segment_planes: connectivity must be 4 or 8";
+    return "opening must be in [0, EMAP_PLANE_MAX_OPENING]";
+  if (p.connectivity != 4 && p.connectivity != 8) return "connectivity must be 4 or 8";
   if (!std::isfinite(p.plane_inclination_cos) || !std::isfinite(p.local_inclination_cos) ||
       !std::isfinite(p.patch_error))
-    return "emap_segment_planes: the inclination cosines and the patch error must be finite";
+    return "the inclination cosines and the patch error must be finite";
   return nullptr;
 }
 
@@ -428,48 +451,56 @@ int64_t emap_plane_capacity(int64_t rows, int64_t cols, const emap_plane_params*
   return rows * cols / std::max(params->min_points, 3);
 }
 
-// The plane decomposition node's segmented planes map for one window (ConvexPlaneDecompositionRos.cpp:115-149 up to
-// SlidingWindowPlaneExtractor, without RANSAC): the window by k_submap, then the passes of csrc/emap_planes.cuh.  Host
-// output: the copies and one synchronisation; device output: stream-ordered, no synchronisation.  Every check runs
-// before anything is written or launched.
-int emap_segment_planes(emap_handle* h, const double window[4], const emap_plane_params* params, float* layers_out,
-                        int32_t out_is_device, int64_t out_floats, double* planes_out, int64_t planes_capacity,
-                        int32_t* info) {
-  ENTER(h);
-  NvtxRange nv("emap:segment_planes");
-  if (!window || !params || !layers_out || !planes_out || !info)
-    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: null argument");
-  if (!submap_lengths_ok(1, window)) return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: lengths must be finite and >= 0");
-  const emap_plane_params p = *params;
+// EMAP_ERR_INVALID with "<fn>: <msg>" as the handle's message.
+static int fail_in(emap_handle* h, const char* fn, const char* msg) {
+  h->err = std::string(fn) + ": " + msg;
+  return EMAP_ERR_INVALID;
+}
+
+// The checks both segmentation entry points make before anything is written or launched, and the window (c.q,
+// c.centre, c.rows, c.cols, c.n, c.plane_rows).  Returns the error's message (without the entry point's name), or nullptr.
+static const char* plane_check(emap_handle* h, const double window[4], const emap_plane_params& p, int64_t out_floats,
+                               int64_t planes_capacity, PlaneCall& c) {
+  if (!submap_lengths_ok(1, window)) return "lengths must be finite and >= 0";
   const double res = h->cfg.resolution;
-  if (const char* e = plane_params_error(p, res)) return fail(h, EMAP_ERR_INVALID, e);
-  const int W = h->dc.W;
+  if (const char* e = plane_params_error(p, res)) return e;
   const double m[2] = {h->center[0], h->center[1]};
-  int32_t q[5];
-  double centre[2];
-  submap_window(W, res, m, window, q, centre);
-  const int rows = q[3], cols = q[4];
-  const int64_t n = (int64_t)rows * cols;
-  if (q[0] && out_floats < 4 * n)
-    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: out_floats is below 4 * rows * cols");
-  const int64_t plane_rows = emap_plane_capacity(rows, cols, &p);
-  if (q[0] && planes_capacity < plane_rows)
-    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: planes_capacity is below emap_plane_capacity()");
-  if (!q[0]) {
-    if (out_is_device) CK(cudaMemsetAsync(info, 0, 5 * sizeof(int32_t), h->stream));
-    else memset(info, 0, 5 * sizeof(int32_t));
-    return EMAP_OK;
-  }
+  submap_window(h->dc.W, res, m, window, c.q, c.centre);
+  c.rows = c.q[3];
+  c.cols = c.q[4];
+  c.n = (int64_t)c.rows * c.cols;
+  if (c.q[0] && out_floats < 4 * c.n) return "out_floats is below 4 * rows * cols";
+  c.plane_rows = emap_plane_capacity(c.rows, c.cols, &p);
+  if (c.q[0] && planes_capacity < c.plane_rows)
+    return "planes_capacity is below emap_plane_capacity()";
+  return nullptr;
+}
+
+// The segmentation of a window that plane_check accepted and found inside the map (ConvexPlaneDecompositionRos.cpp:
+// 115-149 up to SlidingWindowPlaneExtractor, without RANSAC): the window by k_submap, then the passes of
+// csrc/emap_planes.cuh, queued on the handle's stream.  With host output the layers, plane table and info go to the
+// staging at the scratch's tail, which also holds `extra` bytes for the caller (c.s.extra).
+static int segment_window(emap_handle* h, const double window[4], const emap_plane_params& p, bool out_is_device,
+                          float* layers_out, double* planes_out, int32_t* info, size_t extra, PlaneCall& c) {
+  const int rows = c.rows, cols = c.cols;
+  const int64_t n = c.n;
+  const double res = h->cfg.resolution;
   // labels are at most ceil(n / 2) (a 4-connected checkerboard), plus 0.  The statistics are sized and zeroed for that
   // worst case (128 bytes a slot) because the label count is known only on the device.
-  const int64_t slots = n / 2 + 2;
-  PlaneScratch s;
-  int rc = grow(h, h->planes.block, carve_planes(n, slots, plane_rows, !out_is_device, nullptr, s), 0, false);
+  c.slots = n / 2 + 2;
+  const int64_t slots = c.slots;
+  PlaneScratch& s = c.s;
+  int rc = grow(h, h->planes.block, carve_planes(n, slots, c.plane_rows, !out_is_device, extra, nullptr, s), 0, false);
   if (rc) return rc;
-  const size_t used = carve_planes(n, slots, plane_rows, !out_is_device, h->planes.block, s);
+  c.used = carve_planes(n, slots, c.plane_rows, !out_is_device, extra, h->planes.block, s);
+  if (!out_is_device) {
+    // the pinned staging of the copy back, allocated before anything is launched
+    const size_t bytes = c.used - (size_t)((char*)s.info - (char*)h->planes.block);
+    if (h->planes.host.size() < bytes) CK(h->planes.host.alloc(bytes));
+  }
   float* dst = out_is_device ? layers_out : s.layers;
-  double* dst_planes = out_is_device ? planes_out : s.planes;
-  int32_t* dst_info = out_is_device ? info : s.info;
+  c.dst_planes = out_is_device ? planes_out : s.planes;
+  c.dst_info = out_is_device ? info : s.info;
   // the window: k_submap's elevation layer into s.raw
   SubmapArgs a;
   const char* elevation = "elevation";
@@ -477,7 +508,7 @@ int emap_segment_planes(emap_handle* h, const double window[4], const emap_plane
   a.n_win = 0;
   int tiles = 0;
   long long total = 0;
-  submap_add(a, W, q, 1, tiles, total);
+  submap_add(a, h->dc.W, c.q, 1, tiles, total);
   k_submap<false><<<dim3(tiles, 1), dim3(32, SUBMAP_ROWS), 0, h->stream>>>(h->dc, h->map, h->normal, s.raw, a, h->center[2],
                                                                            h->cfg.use_only_above_for_upper_bound);
   LAUNCH_CHECK();
@@ -526,28 +557,225 @@ int emap_segment_planes(emap_handle* h, const double window[4], const emap_plane
   // per-label planes
   k_pl_stats<<<cdiv(cdiv(n, PL_RUN), PL_THREADS), PL_THREADS, 0, h->stream>>>(img, s.lab, s.st, rows, cols);
   LAUNCH_CHECK();
-  const PlaneLabelArgs la = {centre[0] + (0.5 * (rows * res) - 0.5 * res), centre[1] + (0.5 * (cols * res) - 0.5 * res),
-                             res, p.plane_inclination_cos, p.min_points};
+  c.ox = c.centre[0] + (0.5 * (rows * res) - 0.5 * res);
+  c.oy = c.centre[1] + (0.5 * (cols * res) - 0.5 * res);
+  const PlaneLabelArgs la = {c.ox, c.oy, res, p.plane_inclination_cos, p.min_points};
   k_pl_decide<<<cdiv(slots, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.st, s.hdr, s.flag, s.bg, (int)slots, la);
   LAUNCH_CHECK();
   if ((rc = plane_scan(h, s, slots, s.hdr + 2))) return rc;
-  k_pl_planes<<<cdiv(slots, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.st, s.rank, s.hdr, dst_planes, (int)slots, la);
+  k_pl_planes<<<cdiv(slots, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.st, s.rank, s.hdr, c.dst_planes, (int)slots, la);
   LAUNCH_CHECK();
-  k_pl_out<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, img, s.lab, s.bg, s.hdr, dst, dst_info, rows, cols);
+  k_pl_out<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, img, s.lab, s.bg, s.hdr, dst, c.dst_info, rows, cols);
   LAUNCH_CHECK();
+  return 0;
+}
+
+// Host output: the staging (info, the plane table, the layers and the caller's extra bytes are the block's tail) in
+// one copy and one synchronisation; the caller's buffers take the layers and planes only when the window had a finite
+// cell.  Returns the staged copy of the scratch in t.
+static int plane_copy_back(emap_handle* h, PlaneCall& c, float* layers_out, double* planes_out, int32_t* info,
+                           int n_info, PlaneScratch& t) {
+  const size_t off = (char*)c.s.info - (char*)h->planes.block, bytes = c.used - off;
+  if (h->planes.host.size() < bytes) CK(h->planes.host.alloc(bytes));
+  CK(cudaMemcpyAsync(h->planes.host, c.s.info, bytes, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  carve_planes(c.n, c.slots, c.plane_rows, true, bytes, (char*)h->planes.host - off, t);
+  memcpy(info, t.info, n_info * sizeof(int32_t));
+  if (info[0]) {
+    memcpy(planes_out, t.planes, sizeof(double) * 7 * info[4]);
+    memcpy(layers_out, t.layers, sizeof(float) * 4 * c.n);
+  }
+  return 0;
+}
+
+// The plane decomposition node's segmented planes map for one window: segment_window.  Host output: the copies and
+// one synchronisation; device output: stream-ordered, no synchronisation.  Every check runs before anything is written
+// or launched.
+int emap_segment_planes(emap_handle* h, const double window[4], const emap_plane_params* params, float* layers_out,
+                        int32_t out_is_device, int64_t out_floats, double* planes_out, int64_t planes_capacity,
+                        int32_t* info) {
+  ENTER(h);
+  NvtxRange nv("emap:segment_planes");
+  if (!window || !params || !layers_out || !planes_out || !info)
+    return fail(h, EMAP_ERR_INVALID, "emap_segment_planes: null argument");
+  const emap_plane_params p = *params;
+  PlaneCall c;
+  if (const char* e = plane_check(h, window, p, out_floats, planes_capacity, c))
+    return fail_in(h, "emap_segment_planes", e);
+  if (!c.q[0]) {
+    if (out_is_device) CK(cudaMemsetAsync(info, 0, 5 * sizeof(int32_t), h->stream));
+    else memset(info, 0, 5 * sizeof(int32_t));
+    return EMAP_OK;
+  }
+  int rc = segment_window(h, window, p, out_is_device, layers_out, planes_out, info, 0, c);
+  if (rc) return rc;
+  PlaneScratch t;
+  if (!out_is_device && (rc = plane_copy_back(h, c, layers_out, planes_out, info, 5, t))) return rc;
+  return EMAP_OK;
+}
+
+// ---- planar regions of one window (emap_extract_planar_regions, csrc/emap_regions.cuh) -----------------------------
+
+namespace {
+
+// The region passes' scratch for U upsampled pixels, `rows` plane rows and n source cells (49 bytes per upsampled
+// pixel, EMAP_REGION_SCRATCH_PER_PIXEL): the mask bytes, the two images' union-find parents (U + 1 words: the edge
+// node), the point counts, the boundary marks, the kept flags and their ranks, the scan block sums, the polygon
+// records (key, point count, start) and the per-row tables.  After the two passes the parents, marks, flags and ranks
+// are reused as the output order's arrays (see emap_extract_planar_regions).
+struct RegionScratch {
+  unsigned char* mask;
+  int *pa, *pb, *cnt, *have, *flag, *rank, *bsum, *pr, *hdr, *ok, *lcnt, *lreg, *loff, *roff, *lfill;
+  unsigned long long *khi, *klo;
+  int *rn, *rcode;
+};
+
+size_t carve_regions(int64_t U, int64_t rows, int64_t n, void* base, RegionScratch& s) {
+  Carver c{(uintptr_t)base};
+  s.mask = c.take<unsigned char>(U);
+  s.pa = c.take<int>(U + 1); s.pb = c.take<int>(U + 1); s.cnt = c.take<int>(U); s.have = c.take<int>(U);
+  s.flag = c.take<int>(U); s.rank = c.take<int>(U); s.bsum = c.take<int>(U / PL_SCAN + 1);
+  s.pr = c.take<int>(n); s.hdr = c.take<int>(8); s.ok = c.take<int>(6 * (rows + 1));
+  s.lcnt = s.ok + (rows + 1); s.lreg = s.lcnt + (rows + 1); s.loff = s.lreg + (rows + 1);
+  s.roff = s.loff + (rows + 1); s.lfill = s.roff + (rows + 1);
+  s.khi = c.take<unsigned long long>(U); s.klo = c.take<unsigned long long>(U);
+  s.rn = c.take<int>(U); s.rcode = c.take<int>(U);
+  return c.bytes;
+}
+
+}  // namespace
+
+static_assert(EMAP_REGION_MAX_MARGIN == RG_MAX_MARGIN, "emap.h states the margin's bound");
+static_assert(EMAP_REGION_ROW == RG_ROW && EMAP_REGION_POLYGON == RG_POLY, "emap.h states the table rows");
+
+// ContourExtraction::extractPlanarRegions and addHeightOffset after segment_window: see include/emap.h and DESIGN.md
+// §4l.  The launches depend on the parameters and the window size only.
+int emap_extract_planar_regions(emap_handle* h, const double window[4], const emap_plane_params* plane_params,
+                                const emap_region_params* region_params, float* layers_out, int32_t out_is_device,
+                                int64_t out_floats, double* planes_out, int64_t planes_capacity,
+                                const emap_region_out* regions_out, int32_t* info) {
+  ENTER(h);
+  NvtxRange nv("emap:extract_planar_regions");
+  if (!window || !plane_params || !region_params || !layers_out || !planes_out || !regions_out || !info)
+    return fail(h, EMAP_ERR_INVALID, "emap_extract_planar_regions: null argument");
+  const emap_plane_params p = *plane_params;
+  const emap_region_params rp = *region_params;
+  const emap_region_out o = *regions_out;
+  if (rp.margin_size < 0 || rp.margin_size > EMAP_REGION_MAX_MARGIN)
+    return fail(h, EMAP_ERR_INVALID, "emap_extract_planar_regions: margin_size must be in [0, EMAP_REGION_MAX_MARGIN]");
+  if (!std::isfinite(rp.plane_height_offset))
+    return fail(h, EMAP_ERR_INVALID, "emap_extract_planar_regions: plane_height_offset must be finite");
+  if (o.regions_capacity > EMAP_REGION_MAX_ROWS || o.polygons_capacity > EMAP_REGION_MAX_ROWS ||
+      o.vertices_capacity > EMAP_REGION_MAX_ROWS)
+    return fail(h, EMAP_ERR_INVALID, "emap_extract_planar_regions: a table capacity is above EMAP_REGION_MAX_ROWS");
+  if (o.regions_capacity < 0 || o.polygons_capacity < 0 || o.vertices_capacity < 0 ||
+      (o.regions_capacity && !o.regions) || (o.polygons_capacity && !o.polygons) ||
+      (o.vertices_capacity && !o.vertices))
+    return fail(h, EMAP_ERR_INVALID,
+                "emap_extract_planar_regions: a table capacity is negative or a table with a capacity is null");
+  PlaneCall c;
+  if (const char* e = plane_check(h, window, p, out_floats, planes_capacity, c))
+    return fail_in(h, "emap_extract_planar_regions", e);
+  if (!c.q[0]) {
+    if (out_is_device) {
+      k_rg_none<<<1, 1, 0, h->stream>>>(info, 0);
+      LAUNCH_CHECK();
+    } else {
+      memset(info, 0, 8 * sizeof(int32_t));
+      info[8] = 1;
+    }
+    return EMAP_OK;
+  }
+  const bool regions = c.rows >= 2 && c.cols >= 2;
+  const size_t rb = sizeof(double) * RG_ROW * o.regions_capacity, pb = sizeof(int32_t) * RG_POLY * o.polygons_capacity,
+               vb = sizeof(double) * 2 * o.vertices_capacity;
+  const size_t extra = regions ? ((rb + 255) & ~size_t(255)) + ((pb + 255) & ~size_t(255)) + vb : 0;
+  int rc = segment_window(h, window, p, out_is_device, layers_out, planes_out, info, extra, c);
+  if (rc) return rc;
+  PlaneScratch& s = c.s;
+  char* stage = s.extra;
+  RgOut ro;
+  ro.regions = out_is_device ? o.regions : (double*)stage;
+  ro.polys = out_is_device ? o.polygons : (int32_t*)(stage + ((rb + 255) & ~size_t(255)));
+  ro.verts = out_is_device ? o.vertices : (double*)(stage + ((rb + 255) & ~size_t(255)) + ((pb + 255) & ~size_t(255)));
+  ro.planes = c.dst_planes;
+  ro.ox = c.ox;
+  ro.oy = c.oy;
+  ro.res3 = h->cfg.resolution / 3.0;
+  ro.offset = rp.plane_height_offset;
+  if (!regions) {
+    k_rg_none<<<1, 1, 0, h->stream>>>(c.dst_info, 5);   // upSample needs 2 x 2 cells: no region
+    LAUNCH_CHECK();
+  } else {
+    const RgGeom g = {c.rows, c.cols, 3 * c.rows - 2, 3 * c.cols - 2};
+    const int64_t U = (int64_t)g.UR * g.UC, prow = c.plane_rows;
+    RegionScratch r;
+    if ((rc = grow(h, h->regions, carve_regions(U, prow, c.n, nullptr, r), 0, false))) return rc;
+    carve_regions(U, prow, c.n, h->regions, r);
+    const int ub = cdiv(U, PL_THREADS);
+    CK(cudaMemsetAsync(r.hdr, 0, 8 * sizeof(int), h->stream));
+    CK(cudaMemsetAsync(r.ok, 0, 6 * (prow + 1) * sizeof(int), h->stream));   // ok, lcnt, lreg, loff, roff, lfill
+    k_rg_rows<<<cdiv(c.n, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.lab, s.rank, r.pr, (int)c.n);
+    LAUNCH_CHECK();
+    RgKernel kern[2];
+    kern[0].r = 1 + rp.margin_size;
+    for (int i = 0; i <= 2 * kern[0].r; i++) kern[0].half[i] = rg_ellipse_half(kern[0].r, i);
+    kern[1].r = 1;
+    kern[1].half[0] = 0; kern[1].half[1] = 1; kern[1].half[2] = 0;
+    // pass 0: the margin erosion; pass 1: the cross erosion of the plane rows pass 0 left without a region
+    for (int ph = 0; ph < 2; ph++) {
+      k_rg_erode<<<ub, PL_THREADS, 0, h->stream>>>(r.pr, r.ok, r.mask, g, kern[ph], ph);
+      LAUNCH_CHECK();
+      k_rg_inset<<<ub, PL_THREADS, 0, h->stream>>>(r.mask, g, ph);
+      LAUNCH_CHECK();
+      const int bo = 1 << (2 * ph);
+      int* par[2] = {r.pa, r.pb};
+      for (int im = 0; im < 2; im++) {
+        k_rg_uf_init<<<cdiv(U + 1, PL_THREADS), PL_THREADS, 0, h->stream>>>(par[im], (int)U);
+        LAUNCH_CHECK();
+        k_rg_uf_merge<<<ub, PL_THREADS, 0, h->stream>>>(r.mask, bo << im, par[im], g);
+        LAUNCH_CHECK();
+        k_pl_uf_flatten<<<cdiv(U + 1, PL_THREADS), PL_THREADS, 0, h->stream>>>(par[im], (int)U + 1);
+        LAUNCH_CHECK();
+      }
+      k_rg_count<<<ub, PL_THREADS, 0, h->stream>>>(r.mask, r.pa, r.pb, r.cnt, g, ph);
+      LAUNCH_CHECK();
+      CK(cudaMemsetAsync(r.have, 0, U * sizeof(int), h->stream));
+      k_rg_have<<<ub, PL_THREADS, 0, h->stream>>>(r.mask, r.pa, r.pb, r.cnt, r.have, g, ph);
+      LAUNCH_CHECK();
+      k_rg_keep<<<ub, PL_THREADS, 0, h->stream>>>(r.mask, r.pa, r.pb, r.cnt, r.have, r.pr, r.flag, r.ok, g, ph);
+      LAUNCH_CHECK();
+      if ((rc = scan_ranks(h, r.flag, r.rank, r.bsum, U, r.hdr + ph))) return rc;
+      k_rg_append<<<ub, PL_THREADS, 0, h->stream>>>(r.mask, r.pa, r.pb, r.cnt, r.pr, r.flag, r.rank, r.hdr, r.khi,
+                                                     r.klo, r.rn, r.rcode, r.lcnt, r.lreg, g, ph);
+      LAUNCH_CHECK();
+    }
+    // the output order: per plane row offsets of polygons and regions, buckets, and per record its position, region
+    // and inset; the arrays of the passes are reused for it (bucket: rank; sorted counts: flag; record, region,
+    // inset: pa, pb, have; first vertices: cnt)
+    if ((rc = scan_ranks(h, r.lcnt, r.loff, r.bsum, prow + 1, r.hdr + 2))) return rc;
+    if ((rc = scan_ranks(h, r.lreg, r.roff, r.bsum, prow + 1, r.hdr + 3))) return rc;
+    k_rg_bucket<<<ub, PL_THREADS, 0, h->stream>>>(r.khi, r.hdr, r.loff, r.lfill, r.rank, (int)U);
+    LAUNCH_CHECK();
+    CK(cudaMemsetAsync(r.flag, 0, U * sizeof(int), h->stream));
+    k_rg_rank<<<ub, PL_THREADS, 0, h->stream>>>(r.khi, r.klo, r.rn, r.hdr, r.lcnt, r.loff, r.roff, r.rank, r.flag,
+                                                 r.pa, r.pb, r.have, (int)U);
+    LAUNCH_CHECK();
+    if ((rc = scan_ranks(h, r.flag, r.cnt, r.bsum, U, r.hdr + 4))) return rc;
+    k_rg_info<<<1, 1, 0, h->stream>>>(r.hdr, c.dst_info, o.regions_capacity, o.polygons_capacity, o.vertices_capacity);
+    LAUNCH_CHECK();
+    k_rg_write<<<ub, PL_THREADS, 0, h->stream>>>(r.mask, r.khi, r.klo, r.rcode, r.hdr, r.flag, r.pa, r.pb, r.have,
+                                                  r.cnt, ro, g, (int)U);
+    LAUNCH_CHECK();
+  }
   if (!out_is_device) {
-    // info, the plane table and the layers are the block's tail: one copy, one synchronisation, and the caller's
-    // buffers take the layers and planes only when the window had a finite cell
-    const size_t off = (char*)s.info - (char*)h->planes.block, bytes = used - off;
-    if (h->planes.host.size() < bytes) CK(h->planes.host.alloc(bytes));
-    CK(cudaMemcpyAsync(h->planes.host, s.info, bytes, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
     PlaneScratch t;
-    carve_planes(n, slots, plane_rows, true, (char*)h->planes.host - off, t);
-    memcpy(info, t.info, 5 * sizeof(int32_t));
-    if (info[0]) {
-      memcpy(planes_out, t.planes, sizeof(double) * 7 * info[4]);
-      memcpy(layers_out, t.layers, sizeof(float) * 4 * n);
+    if ((rc = plane_copy_back(h, c, layers_out, planes_out, info, 9, t))) return rc;
+    if (regions && info[8]) {
+      const char* st = t.extra;
+      memcpy(o.regions, st, sizeof(double) * RG_ROW * info[5]);
+      memcpy(o.polygons, st + ((rb + 255) & ~size_t(255)), sizeof(int32_t) * RG_POLY * info[6]);
+      memcpy(o.vertices, st + ((rb + 255) & ~size_t(255)) + ((pb + 255) & ~size_t(255)), sizeof(double) * 2 * info[7]);
     }
   }
   return EMAP_OK;

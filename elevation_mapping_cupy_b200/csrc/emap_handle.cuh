@@ -199,6 +199,7 @@ struct emap_handle {
     DevBuf<char> block;            // carve_planes, and its host output's staging: info, plane table and layers, as one
     PinnedBuf<char> host;          // copy of the block's tail
   } planes;
+  DevBuf<char> regions;            // emap_extract_planar_regions' scratch (carve_regions), grown to the largest window
   struct {                         // emap_get_map_points / emap_get_normal_arrows: the count and offset tables, the
     DevBuf<int> table;             // kept cells' payload (grown to the largest call) and a pinned word for the count
     DevBuf<char> out;

@@ -122,6 +122,7 @@ class ElevationMap:
         self.layer_names = list(LAYER_NAMES)
         self.initial_variance = param.initial_variance
         self.map_lock = threading.Lock()
+        self._region_caps = (256, 1024, 16384)   # extract_planar_regions: the largest table counts seen (rows)
         self.device = device
         self._L = _lib.load()
         self._h = C.c_void_p()
@@ -596,6 +597,80 @@ class ElevationMap:
                 "origin": centre + (0.5 * (np.array([rows, cols]) * res) - 0.5 * res), "resolution": res,
                 "size": (rows, cols), "success": bool(info_h[0])}
 
+    def extract_planar_regions(self, position, length, params=None, out=None, capacities=None):
+        """The plane decomposition node's planar regions for the get_submap window around `position` (x, y) of `length`
+        (x, y) metres: segment_planes, then contour extraction and the height offset in one library call
+        (emap_extract_planar_regions; include/emap.h states every step).  `params` and `out` as in segment_planes
+        (the PlaneSegmentationParams' margin_size and extracted_planes_height_offset apply here).  Returns
+        segment_planes' dict plus "tables" (the flat "regions" (n, 17), "polygons" (n, 5) and "vertices" (n, 2)
+        tables: NumPy arrays, or torch CUDA tensors with a device `out`, of which only the info words are read back) and,
+        with host output, "regions": per region a dict of "label", "transform" (4 x 4 plane-to-world), "bbox" (xmin,
+        ymin, xmax, ymax in the plane frame), "boundary" {"outer", "holes"} and "insets" [{"outer", "holes"}], each
+        polygon an (n, 2) array of plane-frame points.  `capacities`: (regions, polygons, vertices) rows to start from;
+        None starts from the largest counts an earlier call of this map returned (a small default on the first call).
+        When a table is too small the call is repeated once with the exact sizes; "retried" says whether it was."""
+        from .plane_segmentation import PlaneSegmentationParams
+        prm = params or PlaneSegmentationParams()
+        p, rp = prm.to_c(), prm.regions_to_c()
+        req = np.array(_xy(position) + _xy(length), np.float64)
+        win = np.zeros(5, np.int32)
+        centre = np.zeros(2, np.float64)
+        device = out is not None and _is_device(out)
+        names = ["elevation_raw", "elevation", "segmentation", "plane_classification"]
+        caps = tuple(int(v) for v in (capacities or self._region_caps))
+        for attempt in range(2):
+            with self.map_lock:
+                c = self.center.astype(np.float64)
+                self._check(self._L.emap_submap_windows(self.cell_n, float(self.resolution), c.ctypes.data, 1,
+                                                        req.ctypes.data, win.ctypes.data, centre.ctypes.data))
+                rows, cols = int(win[3]), int(win[4])
+                cap = max(int(self._L.emap_plane_capacity(rows, cols, C.byref(p))), 1)
+                if device:
+                    import torch
+                    if out.dtype != torch.float32 or not out.is_contiguous():
+                        raise TypeError("a device `out` must be a contiguous float32 torch CUDA tensor")
+                    mk = lambda shape, dt: torch.empty(shape, dtype=dt, device=out.device)  # noqa: E731
+                    f64, i32 = torch.float64, torch.int32
+                    ptr = lambda a: a.data_ptr()  # noqa: E731
+                else:
+                    if out is None:
+                        out = np.zeros(4 * rows * cols, np.float32)
+                    if out.dtype != np.float32 or not out.flags.c_contiguous:
+                        raise TypeError("a host `out` must be a C-contiguous float32 NumPy array")
+                    mk = lambda shape, dt: np.zeros(shape, dt)  # noqa: E731
+                    f64, i32 = np.float64, np.int32
+                    ptr = lambda a: a.ctypes.data  # noqa: E731
+                planes, info = mk((cap, 7), f64), mk(9, i32)
+                tables = (mk((max(caps[0], 1), 17), f64), mk((max(caps[1], 1), 5), i32), mk((max(caps[2], 1), 2), f64))
+                ro = _lib.EmapRegionOut(ptr(tables[0]), caps[0], ptr(tables[1]), caps[1], ptr(tables[2]), caps[2])
+                lay = (out.data_ptr(), out.numel()) if device else (out.ctypes.data, out.size)
+                if device:
+                    self._after_framework()
+                self._check(self._L.emap_extract_planar_regions(self._h, req.ctypes.data, C.byref(p), C.byref(rp),
+                                                                lay[0], int(device), lay[1], ptr(planes), cap,
+                                                                C.byref(ro), ptr(info)))
+                if device:
+                    self._before_framework()
+            info_h = info.cpu().numpy() if device else info
+            if info_h[8]:
+                break
+            caps = (int(info_h[5]), int(info_h[6]), int(info_h[7]))
+        self._region_caps = tuple(max(a, int(b)) for a, b in zip(self._region_caps, info_h[5:8]))
+        n = rows * cols
+        flat = out.reshape(-1)
+        res = float(self.resolution)
+        nr, npoly, nv = (int(x) for x in info_h[5:8])
+        reg, poly, vert = tables[0][:nr], tables[1][:npoly], tables[2][:nv]
+        result = {"layers": {name: flat[k * n:(k + 1) * n].reshape(rows, cols) for k, name in enumerate(names)},
+                  "planes": planes[:int(info_h[4])], "highest_label": int(info_h[3]),
+                  "origin": centre + (0.5 * (np.array([rows, cols]) * res) - 0.5 * res), "resolution": res,
+                  "size": (rows, cols), "success": bool(info_h[0]), "complete": bool(info_h[8]),
+                  "tables": {"regions": reg, "polygons": poly, "vertices": vert}, "regions": None,
+                  "retried": attempt > 0}
+        if not device and info_h[8]:
+            result["regions"] = regions_from_tables(reg, poly, vert)
+        return result
+
     def _window_views(self, layers, out, cells, call, sizes):
         """What get_submaps and get_transformed_submaps share: checks the layer names (KeyError before anything runs),
         sizes a new host `out` with cells() (the host window arithmetic, which fills `sizes`), checks `out`, orders the
@@ -860,6 +935,28 @@ def _to_host(x):
     if hasattr(x, "get"):                                # cupy array
         return x.get()
     return np.asarray(x)
+
+
+def regions_from_tables(regions, polygons, vertices):
+    """extract_planar_regions' per-region dicts from the three flat tables (include/emap.h states their layout)."""
+    out = []
+    for r in regions:
+        T = np.eye(4)
+        T[:3, :] = r[1:13].reshape(3, 4)
+        out.append({"label": int(r[0]), "transform": T, "bbox": r[13:17].copy(),
+                    "boundary": {"outer": None, "holes": []}, "insets": []})
+    for region, role, inset, first, count in polygons:
+        pts = vertices[first:first + count].copy()
+        d = out[region]
+        if role == 0:
+            d["boundary"]["outer"] = pts
+        elif role == 1:
+            d["boundary"]["holes"].append(pts)
+        elif role == 2:
+            d["insets"].append({"outer": pts, "holes": []})
+        else:
+            d["insets"][inset]["holes"].append(pts)
+    return out
 
 
 def _is_device(x):

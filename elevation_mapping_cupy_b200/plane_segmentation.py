@@ -1,6 +1,7 @@
-"""Parameters of ElevationMap.segment_planes: the plane decomposition node's `preprocessing` and
-`sliding_window_plane_extractor` sections (convex_plane_decomposition_ros/config/parameters.yaml), with the two
-inclination thresholds as cosines, as ParameterLoading.cpp stores them."""
+"""Parameters of ElevationMap.segment_planes and ElevationMap.extract_planar_regions: the plane decomposition node's
+`preprocessing`, `sliding_window_plane_extractor`, `contour_extraction` and `postprocessing` sections
+(convex_plane_decomposition_ros/config/parameters.yaml), with the two inclination thresholds as cosines, as
+ParameterLoading.cpp stores them."""
 import math
 from dataclasses import dataclass
 
@@ -22,11 +23,15 @@ class PlaneSegmentationParams:
     min_number_points_per_label: int = 4
     connectivity: int = 4
     include_ransac_refinement: bool = False
+    # contour_extraction and postprocessing (extract_planar_regions only)
+    margin_size: int = 1
+    extracted_planes_height_offset: float = 0.0
 
     @classmethod
     def from_yaml(cls, path):
-        """Reads the `preprocessing` and `sliding_window_plane_extractor` sections of a node parameter file; keys that
-        are absent keep their defaults, and `*_degrees` become cosines (ParameterLoading.cpp:49-59)."""
+        """Reads the `preprocessing`, `sliding_window_plane_extractor`, `contour_extraction` (marginSize) and
+        `postprocessing` (extracted_planes_height_offset) sections of a node parameter file; keys that are absent keep
+        their defaults, and `*_degrees` become cosines (ParameterLoading.cpp:49-59)."""
         import yaml
         with open(path) as f:
             doc = yaml.safe_load(f) or {}
@@ -43,6 +48,10 @@ class PlaneSegmentationParams:
                           ("connectivity", "connectivity"), ("include_ransac_refinement", "include_ransac_refinement")):
             if key in sw:
                 setattr(p, name, sw[key])
+        if "marginSize" in (doc.get("contour_extraction") or {}):
+            p.margin_size = doc["contour_extraction"]["marginSize"]
+        if "extracted_planes_height_offset" in (doc.get("postprocessing") or {}):
+            p.extracted_planes_height_offset = doc["postprocessing"]["extracted_planes_height_offset"]
         if "plane_inclination_threshold_degrees" in sw:
             p.plane_inclination_cos = math.cos(sw["plane_inclination_threshold_degrees"] * math.pi / 180.0)
         if "local_plane_inclination_threshold_degrees" in sw:
@@ -55,3 +64,6 @@ class PlaneSegmentationParams:
                                     int(self.min_number_points_per_label), int(self.connectivity),
                                     float(self.plane_inclination_cos), float(self.local_plane_inclination_cos),
                                     float(self.plane_patch_error_threshold), int(bool(self.include_ransac_refinement)))
+
+    def regions_to_c(self):
+        return _lib.EmapRegionParams(int(self.margin_size), float(self.extracted_planes_height_offset))

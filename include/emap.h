@@ -457,6 +457,64 @@ int64_t emap_plane_capacity(int64_t rows, int64_t cols, const emap_plane_params*
 int emap_segment_planes(emap_handle* h, const double window[4], const emap_plane_params* params, float* layers_out,
                         int32_t out_is_device, int64_t out_floats, double* planes_out, int64_t planes_capacity,
                         int32_t* info);
+/* ---- planar regions: the plane decomposition node's PlanarTerrain.planarRegions for one window, on the device:
+ * ContourExtraction::extractPlanarRegions (plane_segmentation/convex_plane_decomposition) and
+ * Postprocessing::addHeightOffset, after emap_segment_planes.  DESIGN.md §4l gives the parallel restatement.
+ * Takes everything emap_segment_planes takes and writes the same layers_out, planes_out and info[0 .. 4], byte for
+ * byte; then, for a window of R x C >= 2 x 2 cells:
+ *  Upsampling: the label image becomes (3R - 2) x (3C - 2) pixels; the first and last source rows and columns take 2
+ *    pixels each, every inner one 3.  Pixel (x = column, y = row) is at world (ox - y res / 3, oy - x res / 3), (ox,
+ *    oy) the centre of window cell (0, 0).
+ *  Per plane row, labels ascending: binary = (up == label) eroded once, BORDER_REPLICATE, by MORPH_ELLIPSE of size
+ *    2 (1 + margin_size) + 1 (cv::getStructuringElement's shape).  Boundaries = its polygons; insets = the polygons of
+ *    its erosion by the 3 x 3 cross (BORDER_REPLICATE) with the first and last rows and columns cleared.  A polygon is
+ *    a cv::findContours(RETR_CCOMP, CHAIN_APPROX_SIMPLE) top-level contour with more than one point, with its child
+ *    contours as holes.  A boundary keeps, in inset order, the insets whose first outer vertex is inside it (on an
+ *    edge counts as inside); boundaries without an inset are dropped.  When no boundary of the label is kept, the
+ *    same is redone from (up == label) eroded once by the 3 x 3 cross (the fallback).
+ *  Order (cv2 4.13's RETR_CCOMP order, which the tests pin down): top-level contours by start pixel (the raster-first
+ *    pixel of the 8-connected component) descending in raster order, each followed by its holes by start pixel (the
+ *    pixel left of the raster-first pixel of the enclosed 4-connected background) descending.
+ *  Geometry, in double: every point is mapped to the world as above and projected along gravity into the plane frame
+ *    of getTransformLocalToGlobal(support, normal); the region's transform is that one with plane_height_offset added
+ *    to its translation z.  bbox = (xmin, ymin, xmax, ymax) of the boundary's outer points in the plane frame.
+ * Outputs (emap_region_out): regions, EMAP_REGION_ROW doubles per region: label, the 3 x 4 row-major plane-to-world
+ * transform [R | t], bbox.  polygons, EMAP_REGION_POLYGON int32 per polygon: {region, role, inset, first_vertex,
+ * n_vertices}; role 0 boundary outer, 1 boundary hole, 2 inset outer, 3 inset hole; inset = the inset's index in its
+ * region, -1 for the boundary; per region the boundary outer, its holes, then each inset's outer and its holes.
+ * vertices: (x, y) per point in the plane frame, in OpenCV's order.  info = {success, rows, cols, highest_label,
+ * n_planes, n_regions, n_polygons, n_vertices, complete}: the counts are always the required totals; when one exceeds
+ * its capacity, complete = 0 and no region, polygon or vertex is written (decided on the device).  A window outside
+ * the map gives info = {0, ..., 0, 1}; a window with fewer than 2 rows or columns gives n_regions = 0.
+ * Host and device output, stream order, graph capture, rejections and the map state as in emap_segment_planes; host
+ * output comes back in the same single copy and synchronisation.  The launches depend on the parameters and the
+ * window size only.  Scratch: EMAP_REGION_SCRATCH_PER_PIXEL bytes per upsampled pixel on top of emap_segment_planes'
+ * (about 1.9 GB for a 2047 x 2047 window).  EMAP_ERR_INVALID, with nothing written or launched, additionally for
+ * margin_size outside 0 .. EMAP_REGION_MAX_MARGIN, a non-finite plane_height_offset, a capacity below 0 or above
+ * EMAP_REGION_MAX_ROWS, or a NULL table whose capacity is above 0.  With host output the tables are staged at their
+ * capacities, so pass capacities near the counts (info[5 .. 7] of an earlier call); a staging that cannot be allocated
+ * returns EMAP_ERR_CUDA before anything is launched. */
+typedef struct emap_region_params {
+  int32_t margin_size;             /* contour_extraction/marginSize, 0 .. EMAP_REGION_MAX_MARGIN */
+  double plane_height_offset;      /* postprocessing/extracted_planes_height_offset [m] */
+} emap_region_params;
+typedef struct emap_region_out {
+  double* regions;                 /* EMAP_REGION_ROW doubles per region */
+  int64_t regions_capacity;        /* rows */
+  int32_t* polygons;               /* EMAP_REGION_POLYGON int32 per polygon */
+  int64_t polygons_capacity;
+  double* vertices;                /* 2 doubles per vertex */
+  int64_t vertices_capacity;
+} emap_region_out;
+#define EMAP_REGION_MAX_MARGIN 4
+#define EMAP_REGION_ROW 17
+#define EMAP_REGION_POLYGON 5
+#define EMAP_REGION_SCRATCH_PER_PIXEL 49
+#define EMAP_REGION_MAX_ROWS 2147483647  /* a table capacity above this (the counts are int32) is rejected */
+int emap_extract_planar_regions(emap_handle* h, const double window[4], const emap_plane_params* plane_params,
+                                const emap_region_params* region_params, float* layers_out, int32_t out_is_device,
+                                int64_t out_floats, double* planes_out, int64_t planes_capacity,
+                                const emap_region_out* regions_out, int32_t* info);
 /* ---- the exported map as a point cloud and as normal arrows: the ROS node's publishAsPointCloud
  * (elevation_mapping_ros.cpp:501-505, grid_map's toPointCloud(map, {"elevation"}, "elevation")) and publishNormalAsArrow
  * (:751-778), restated from grid_map's published source (not checked against a grid_map build).  Coordinates are those of
