@@ -43,6 +43,15 @@ class EmapRegionParams(C.Structure):
     _fields_ = [("margin_size", C.c_int32), ("plane_height_offset", C.c_double)]
 
 
+class EmapPostprocessParams(C.Structure):
+    _fields_ = [("nonplanar_height_offset", C.c_double), ("nonplanar_horizontal_offset", C.c_int32),
+                ("smoothing_dilation_size", C.c_double), ("smoothing_box_kernel_size", C.c_double),
+                ("smoothing_gauss_kernel_size", C.c_double)]
+
+
+EMAP_TERRAIN_LAYERS = 10
+
+
 class EmapRegionOut(C.Structure):
     _fields_ = [("regions", C.c_void_p), ("regions_capacity", C.c_int64), ("polygons", C.c_void_p),
                 ("polygons_capacity", C.c_int64), ("vertices", C.c_void_p), ("vertices_capacity", C.c_int64)]
@@ -122,6 +131,8 @@ SIGNATURES = {
                                       C.c_int64, C.c_void_p]),
     "emap_extract_planar_regions": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32,
                                               C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "emap_planar_terrain": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "emap_get_map_points": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_get_normal_arrows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_layer_device_ptr": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),

@@ -6,6 +6,7 @@
 #include "emap_submap.cuh"
 #include "emap_planes.cuh"
 #include "emap_regions.cuh"
+#include "emap_postprocess.cuh"
 #include "emap_mapcloud.cuh"
 
 namespace {
@@ -350,7 +351,8 @@ int emap_get_transformed_submaps(emap_handle* h, int32_t n_windows, const double
 // The scratch of a window of n cells with `slots` label slots, one block: the window, two image planes (fill / median
 // ping-pong), union-find parents, flags and ranks, fill keys, the planarity masks, scan block sums, the header words,
 // the label statistics and decisions, and the host output's staging (info, plane table, layers, then `extra` bytes
-// that emap_extract_planar_regions stages its tables in).
+// that emap_extract_planar_regions stages its tables in).  With the post-processing (emap_planar_terrain) the block
+// also holds its three fp32 planes and the box filter's double row sums, and the staging all EMAP_TERRAIN_LAYERS layers.
 namespace {
 
 struct PlaneScratch {
@@ -359,13 +361,15 @@ struct PlaneScratch {
   unsigned* key;
   unsigned char *bin, *tmp, *bg;
   unsigned long long* st;
+  float* pp;
+  double* pd;
   int32_t* info;
   double* planes;
   float* layers;
   char* extra;
 };
 
-size_t carve_planes(int64_t n, int64_t slots, int64_t plane_rows, bool host_out, size_t extra, void* base,
+size_t carve_planes(int64_t n, int64_t slots, int64_t plane_rows, bool host_out, bool post, size_t extra, void* base,
                     PlaneScratch& s) {
   Carver c{(uintptr_t)base};
   const int64_t m = std::max(n, slots);
@@ -375,9 +379,11 @@ size_t carve_planes(int64_t n, int64_t slots, int64_t plane_rows, bool host_out,
   s.key = c.take<unsigned>(n);
   s.bin = c.take<unsigned char>(n); s.tmp = c.take<unsigned char>(n); s.bg = c.take<unsigned char>(slots);
   s.st = c.take<unsigned long long>(slots * PL_STAT);
+  s.pp = c.take<float>(post ? 3 * n : 0);
+  s.pd = c.take<double>(post ? n : 0);
   s.info = c.take<int32_t>(host_out ? 16 : 0);
   s.planes = c.take<double>(host_out ? 7 * plane_rows : 0);
-  s.layers = c.take<float>(host_out ? 4 * n : 0);
+  s.layers = c.take<float>(host_out ? (post ? EMAP_TERRAIN_LAYERS : 4) * n : 0);
   s.extra = c.take<char>(host_out ? extra : 0);
   return c.bytes;
 }
@@ -415,6 +421,7 @@ struct PlaneCall {
   double centre[2];
   int rows = 0, cols = 0;
   int64_t n = 0, slots = 0, plane_rows = 0;
+  bool post = false;               // emap_planar_terrain: the post-processing's scratch and layers
   double ox = 0.0, oy = 0.0;       // the centre of window cell (0, 0)
   PlaneScratch s;
   size_t used = 0;
@@ -490,9 +497,10 @@ static int segment_window(emap_handle* h, const double window[4], const emap_pla
   c.slots = n / 2 + 2;
   const int64_t slots = c.slots;
   PlaneScratch& s = c.s;
-  int rc = grow(h, h->planes.block, carve_planes(n, slots, c.plane_rows, !out_is_device, extra, nullptr, s), 0, false);
+  int rc = grow(h, h->planes.block, carve_planes(n, slots, c.plane_rows, !out_is_device, c.post, extra, nullptr, s), 0,
+                false);
   if (rc) return rc;
-  c.used = carve_planes(n, slots, c.plane_rows, !out_is_device, extra, h->planes.block, s);
+  c.used = carve_planes(n, slots, c.plane_rows, !out_is_device, c.post, extra, h->planes.block, s);
   if (!out_is_device) {
     // the pinned staging of the copy back, allocated before anything is launched
     const size_t bytes = c.used - (size_t)((char*)s.info - (char*)h->planes.block);
@@ -579,11 +587,11 @@ static int plane_copy_back(emap_handle* h, PlaneCall& c, float* layers_out, doub
   if (h->planes.host.size() < bytes) CK(h->planes.host.alloc(bytes));
   CK(cudaMemcpyAsync(h->planes.host, c.s.info, bytes, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
-  carve_planes(c.n, c.slots, c.plane_rows, true, bytes, (char*)h->planes.host - off, t);
+  carve_planes(c.n, c.slots, c.plane_rows, true, c.post, bytes, (char*)h->planes.host - off, t);
   memcpy(info, t.info, n_info * sizeof(int32_t));
   if (info[0]) {
     memcpy(planes_out, t.planes, sizeof(double) * 7 * info[4]);
-    memcpy(layers_out, t.layers, sizeof(float) * 4 * c.n);
+    memcpy(layers_out, t.layers, sizeof(float) * (c.post ? EMAP_TERRAIN_LAYERS : 4) * c.n);
   }
   return 0;
 }
@@ -648,34 +656,123 @@ size_t carve_regions(int64_t U, int64_t rows, int64_t n, void* base, RegionScrat
 static_assert(EMAP_REGION_MAX_MARGIN == RG_MAX_MARGIN, "emap.h states the margin's bound");
 static_assert(EMAP_REGION_ROW == RG_ROW && EMAP_REGION_POLYGON == RG_POLY, "emap.h states the table rows");
 
-// ContourExtraction::extractPlanarRegions and addHeightOffset after segment_window: see include/emap.h and DESIGN.md
-// §4l.  The launches depend on the parameters and the window size only.
-int emap_extract_planar_regions(emap_handle* h, const double window[4], const emap_plane_params* plane_params,
-                                const emap_region_params* region_params, float* layers_out, int32_t out_is_device,
-                                int64_t out_floats, double* planes_out, int64_t planes_capacity,
-                                const emap_region_out* regions_out, int32_t* info) {
-  ENTER(h);
-  NvtxRange nv("emap:extract_planar_regions");
-  if (!window || !plane_params || !region_params || !layers_out || !planes_out || !regions_out || !info)
-    return fail(h, EMAP_ERR_INVALID, "emap_extract_planar_regions: null argument");
-  const emap_plane_params p = *plane_params;
-  const emap_region_params rp = *region_params;
-  const emap_region_out o = *regions_out;
+static_assert(EMAP_POST_MAX_KERNEL == PP_MAX_KERNEL && EMAP_POST_MAX_OFFSET == PP_MAX_OFFSET,
+              "emap.h states the post-processing's bounds");
+
+// The post-processing's kernel sizes and the final pass's arithmetic, as postprocess_window launches them.
+struct PostCall {
+  int dil = 0, box = 0, gauss = 0;  // the smoothing's kernel sizes (kernelSizeInPixels)
+  PpFinal fin;
+};
+
+// Why q is rejected (nullptr: accepted) for a map of resolution res; else pc.
+static const char* post_params_error(const emap_postprocess_params& q, double res, double ext_offset, PostCall& pc) {
+  pc.dil = pp_kernel_size(q.smoothing_dilation_size, res);
+  pc.box = pp_kernel_size(q.smoothing_box_kernel_size, res);
+  pc.gauss = pp_kernel_size(q.smoothing_gauss_kernel_size, res);
+  if (pc.dil < 0 || pc.box < 0 || pc.gauss < 0)
+    return "the smoothing sizes must be finite, >= 0 and give kernels of at most EMAP_POST_MAX_KERNEL cells";
+  if (q.nonplanar_horizontal_offset < 0 || q.nonplanar_horizontal_offset > EMAP_POST_MAX_OFFSET)
+    return "nonplanar_horizontal_offset must be in [0, EMAP_POST_MAX_OFFSET]";
+  if (!std::isfinite(q.nonplanar_height_offset)) return "nonplanar_height_offset must be finite";
+  // Eigen narrows a double scalar to the float matrix's scalar type before the fp32 operation (promote_scalar_arg)
+  pc.fin.dil = q.nonplanar_horizontal_offset > 0;
+  pc.fin.add_on = ext_offset != 0.0 || q.nonplanar_height_offset != 0.0;
+  pc.fin.sub_on = q.nonplanar_height_offset != 0.0;
+  pc.fin.add = (float)(ext_offset + q.nonplanar_height_offset);
+  pc.fin.sub = (float)q.nonplanar_height_offset;
+  return nullptr;
+}
+
+static PpEllipse pp_ellipse(int size) {
+  PpEllipse e;
+  e.r = (size - 1) / 2;
+  for (int i = 0; i < size; i++) e.half[i] = rg_ellipse_half(e.r, i);
+  return e;
+}
+
+// Postprocessing::postprocess on the layers segment_window left in dst (layer 1 is E, layer 3 M): layers 4 .. 9.  The
+// scratch is the block's three post planes (a: fill input, then the box output; b: fill output, then the dilated E; t:
+// the closing's and the Gaussian's intermediates) and its double row sums.  The launches depend on the parameters only.
+static int postprocess_window(emap_handle* h, PlaneCall& c, const emap_postprocess_params& q, const PostCall& pc, float* dst) {
+  PlaneScratch& s = c.s;
+  const int rows = c.rows, cols = c.cols, n = (int)c.n, cb = cdiv(c.n, PL_THREADS);
+  float *a = s.pp, *b = s.pp + c.n, *t = s.pp + 2 * c.n;
+  float* L[EMAP_TERRAIN_LAYERS];
+  for (int k = 0; k < EMAP_TERRAIN_LAYERS; k++) L[k] = dst + (int64_t)k * c.n;
+  int rc;
+  // elevationWithNaN, then minValues with the segmentation's fill; its finite-cell word is hdr[3], so the call's
+  // success (hdr[0]) stays the segmentation's
+  k_pp_mask<<<cb, PL_THREADS, 0, h->stream>>>(dst, a, L[4], s.hdr, n);
+  LAUNCH_CHECK();
+  k_pl_fill_init<<<cb, PL_THREADS, 0, h->stream>>>(a, s.parent, s.key, s.hdr + 3, n);
+  LAUNCH_CHECK();
+  if ((rc = plane_components(h, s, rows, cols, 0))) return rc;
+  k_pl_fill_min<<<cb, PL_THREADS, 0, h->stream>>>(a, s.parent, s.key, rows, cols);
+  LAUNCH_CHECK();
+  k_pl_fill_write<<<cb, PL_THREADS, 0, h->stream>>>(a, s.parent, s.key, b, n);
+  LAUNCH_CHECK();
+  // MORPH_CLOSE (its dilation also stores elevationWithNaN_i), then the sloped dilation
+  const PpEllipse ec = pp_ellipse(pc.dil);
+  k_pp_morph<true><<<cb, PL_THREADS, 0, h->stream>>>(b, t, L[5], s.hdr, rows, cols, ec);
+  LAUNCH_CHECK();
+  k_pp_morph<false><<<cb, PL_THREADS, 0, h->stream>>>(t, L[6], nullptr, s.hdr, rows, cols, ec);
+  LAUNCH_CHECK();
+  k_pp_slope<<<cb, PL_THREADS, 0, h->stream>>>(L[6], L[7], s.hdr, rows, cols, pc.dil, (float)h->cfg.resolution);
+  LAUNCH_CHECK();
+  // smooth_planar: boxFilter, then GaussianBlur (rows, then columns)
+  k_pp_box_rows<<<cb, PL_THREADS, 0, h->stream>>>(L[7], s.pd, s.hdr, rows, cols, pc.box / 2);
+  LAUNCH_CHECK();
+  k_pp_box_cols<<<cb, PL_THREADS, 0, h->stream>>>(s.pd, a, s.hdr, rows, cols, pc.box / 2,
+                                                   1.0 / ((double)pc.box * pc.box));
+  LAUNCH_CHECK();
+  PpGauss g;
+  g.h = pc.gauss / 2;
+  pp_gauss_coeffs(pc.gauss, g.c);
+  k_pp_gauss<true><<<cb, PL_THREADS, 0, h->stream>>>(a, t, s.hdr, rows, cols, g);
+  LAUNCH_CHECK();
+  k_pp_gauss<false><<<cb, PL_THREADS, 0, h->stream>>>(t, L[8], s.hdr, rows, cols, g);
+  LAUNCH_CHECK();
+  // dilationInNonplanarRegions and addHeightOffset
+  if (pc.fin.dil) {
+    k_pp_morph<true><<<cb, PL_THREADS, 0, h->stream>>>(L[1], b, nullptr, s.hdr, rows, cols,
+                                                        pp_ellipse(2 * q.nonplanar_horizontal_offset + 1));
+    LAUNCH_CHECK();
+  }
+  k_pp_final<<<cb, PL_THREADS, 0, h->stream>>>(dst, b, L[9], s.hdr, n, pc.fin);
+  LAUNCH_CHECK();
+  return 0;
+}
+
+// ContourExtraction::extractPlanarRegions and addHeightOffset after segment_window (both entry points), then, with
+// post != nullptr, Postprocessing::postprocess's map passes (emap_planar_terrain): see include/emap.h and DESIGN.md
+// §4l.  Every check runs before anything is written or launched; the launches depend on the parameters and the window
+// size only.  fn names the entry point in the messages.
+static int planar_regions(emap_handle* h, const char* fn, const double window[4], const emap_plane_params& p,
+                          const emap_region_params& rp, const emap_postprocess_params* post, float* layers_out,
+                          int32_t out_is_device, int64_t out_floats, double* planes_out, int64_t planes_capacity,
+                          const emap_region_out& o, int32_t* info) {
   if (rp.margin_size < 0 || rp.margin_size > EMAP_REGION_MAX_MARGIN)
-    return fail(h, EMAP_ERR_INVALID, "emap_extract_planar_regions: margin_size must be in [0, EMAP_REGION_MAX_MARGIN]");
-  if (!std::isfinite(rp.plane_height_offset))
-    return fail(h, EMAP_ERR_INVALID, "emap_extract_planar_regions: plane_height_offset must be finite");
+    return fail_in(h, fn, "margin_size must be in [0, EMAP_REGION_MAX_MARGIN]");
+  if (!std::isfinite(rp.plane_height_offset)) return fail_in(h, fn, "plane_height_offset must be finite");
   if (o.regions_capacity > EMAP_REGION_MAX_ROWS || o.polygons_capacity > EMAP_REGION_MAX_ROWS ||
       o.vertices_capacity > EMAP_REGION_MAX_ROWS)
-    return fail(h, EMAP_ERR_INVALID, "emap_extract_planar_regions: a table capacity is above EMAP_REGION_MAX_ROWS");
+    return fail_in(h, fn, "a table capacity is above EMAP_REGION_MAX_ROWS");
   if (o.regions_capacity < 0 || o.polygons_capacity < 0 || o.vertices_capacity < 0 ||
       (o.regions_capacity && !o.regions) || (o.polygons_capacity && !o.polygons) ||
       (o.vertices_capacity && !o.vertices))
-    return fail(h, EMAP_ERR_INVALID,
-                "emap_extract_planar_regions: a table capacity is negative or a table with a capacity is null");
+    return fail_in(h, fn, "a table capacity is negative or a table with a capacity is null");
   PlaneCall c;
-  if (const char* e = plane_check(h, window, p, out_floats, planes_capacity, c))
-    return fail_in(h, "emap_extract_planar_regions", e);
+  if (const char* e = plane_check(h, window, p, out_floats, planes_capacity, c)) return fail_in(h, fn, e);
+  PostCall pc;
+  if (post) {
+    if (const char* e = post_params_error(*post, h->cfg.resolution, rp.plane_height_offset, pc)) return fail_in(h, fn, e);
+    if (c.q[0] && out_floats < EMAP_TERRAIN_LAYERS * c.n)
+      return fail_in(h, fn, "out_floats is below EMAP_TERRAIN_LAYERS * rows * cols");
+    if (c.q[0] && (c.rows < pc.dil || c.cols < pc.dil))
+      return fail_in(h, fn, "the window has fewer rows or columns than the smoothing's dilation kernel");
+    c.post = true;
+  }
   if (!c.q[0]) {
     if (out_is_device) {
       k_rg_none<<<1, 1, 0, h->stream>>>(info, 0);
@@ -768,6 +865,7 @@ int emap_extract_planar_regions(emap_handle* h, const double window[4], const em
                                                   r.cnt, ro, g, (int)U);
     LAUNCH_CHECK();
   }
+  if (post && (rc = postprocess_window(h, c, *post, pc, out_is_device ? layers_out : s.layers))) return rc;
   if (!out_is_device) {
     PlaneScratch t;
     if ((rc = plane_copy_back(h, c, layers_out, planes_out, info, 9, t))) return rc;
@@ -779,6 +877,32 @@ int emap_extract_planar_regions(emap_handle* h, const double window[4], const em
     }
   }
   return EMAP_OK;
+}
+
+int emap_extract_planar_regions(emap_handle* h, const double window[4], const emap_plane_params* plane_params,
+                                const emap_region_params* region_params, float* layers_out, int32_t out_is_device,
+                                int64_t out_floats, double* planes_out, int64_t planes_capacity,
+                                const emap_region_out* regions_out, int32_t* info) {
+  ENTER(h);
+  NvtxRange nv("emap:extract_planar_regions");
+  if (!window || !plane_params || !region_params || !layers_out || !planes_out || !regions_out || !info)
+    return fail(h, EMAP_ERR_INVALID, "emap_extract_planar_regions: null argument");
+  return planar_regions(h, "emap_extract_planar_regions", window, *plane_params, *region_params, nullptr, layers_out,
+                        out_is_device, out_floats, planes_out, planes_capacity, *regions_out, info);
+}
+
+// Postprocessing::postprocess after extract_planar_regions' passes: see include/emap.h and DESIGN.md §4l.
+int emap_planar_terrain(emap_handle* h, const double window[4], const emap_plane_params* plane_params,
+                        const emap_region_params* region_params, const emap_postprocess_params* post_params,
+                        float* layers_out, int32_t out_is_device, int64_t out_floats, double* planes_out,
+                        int64_t planes_capacity, const emap_region_out* regions_out, int32_t* info) {
+  ENTER(h);
+  NvtxRange nv("emap:planar_terrain");
+  if (!window || !plane_params || !region_params || !post_params || !layers_out || !planes_out || !regions_out || !info)
+    return fail(h, EMAP_ERR_INVALID, "emap_planar_terrain: null argument");
+  const emap_postprocess_params q = *post_params;
+  return planar_regions(h, "emap_planar_terrain", window, *plane_params, *region_params, &q, layers_out, out_is_device,
+                        out_floats, planes_out, planes_capacity, *regions_out, info);
 }
 
 // The node's publishAsPointCloud (elevation_mapping_ros.cpp:501-505): the points of the exported elevation (map_cloud).

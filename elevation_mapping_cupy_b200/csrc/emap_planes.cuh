@@ -14,6 +14,7 @@
 using std::fabs;
 using std::floor;
 using std::isfinite;
+using std::rint;
 using std::sqrt;
 #endif
 
@@ -28,6 +29,16 @@ using std::sqrt;
 #else
 #define PL_HD inline
 #endif
+
+// cv::getStructuringElement(MORPH_ELLIPSE, (2 r + 1)^2): row i covers columns r - w .. r + w, w = the half width.  The
+// region erosions (emap_regions.cuh) and the post-processing's grey morphology (emap_postprocess.cuh) share it.  r = 0
+// is OpenCV's 1 x 1 element (it switches to MORPH_RECT there; the formula would divide by 0).
+PL_HD int rg_ellipse_half(int r, int i) {
+  if (r == 0) return 0;
+  const int dy = i - r;
+  const double inv_r2 = 1.0 / ((double)r * r);
+  return (int)rint(r * sqrt((double)(r * r - dy * dy) * inv_r2));
+}
 
 // A fit's result: the unit normal (z >= 0) and the squared error (the smallest eigenvalue, clamped at 0), or
 // (UnitZ, 1e30) when it is not defined.

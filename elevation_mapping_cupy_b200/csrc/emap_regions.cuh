@@ -3,19 +3,15 @@
 // Reference: plane_segmentation's convex_plane_decomposition ContourExtraction::extractPlanarRegions (upsampling,
 // margin erosion, boundaries and insets by cv::findContours(RETR_CCOMP, CHAIN_APPROX_SIMPLE), the cross-erosion
 // fallback, the projection to the plane frame) and Postprocessing::addHeightOffset.  include/emap.h states the
-// contract; DESIGN.md §4l the parallel restatement.  The upsampling index, the structuring element, the start-pixel
-// rule and the border following with CHAIN_APPROX_SIMPLE's compression are __host__ __device__ so that a native test
-// can check them against cv2.
+// contract; DESIGN.md §4l the parallel restatement.  The upsampling index, the start-pixel rule and the border
+// following with CHAIN_APPROX_SIMPLE's compression (and the structuring element, rg_ellipse_half in emap_planes.cuh)
+// are __host__ __device__ so that a native test can check them against cv2.
 #pragma once
 #include <cmath>
 #include <cstdint>
 #include <cuda_runtime.h>
 
 #include "emap_planes.cuh"
-
-#if !defined(__CUDACC__)
-using std::rint;
-#endif
 
 #define RG_MAX_MARGIN 4            // emap.h's EMAP_REGION_MAX_MARGIN: the margin ellipse is at most 11 x 11
 #define RG_KMAX (2 * (1 + RG_MAX_MARGIN) + 1)
@@ -29,13 +25,6 @@ using std::rint;
 PL_HD int rg_src(int u, int m) {
   const int s = u < 2 ? 0 : (u - 2) / 3 + 1;
   return s < m - 1 ? s : m - 1;
-}
-
-// cv::getStructuringElement(MORPH_ELLIPSE, (2 r + 1)^2): row i covers columns r - w .. r + w, w = the half width.
-PL_HD int rg_ellipse_half(int r, int i) {
-  const int dy = i - r;
-  const double inv_r2 = 1.0 / ((double)r * r);
-  return (int)rint(r * sqrt((double)(r * r - dy * dy) * inv_r2));
 }
 
 // Border-following start of pixel i of a binary image in Suzuki-Abe's scan (8-connected foreground, 4-connected

@@ -609,14 +609,36 @@ class ElevationMap:
         polygon an (n, 2) array of plane-frame points.  `capacities`: (regions, polygons, vertices) rows to start from;
         None starts from the largest counts an earlier call of this map returned (a small default on the first call).
         When a table is too small the call is repeated once with the exact sizes; "retried" says whether it was."""
+        return self._planar_regions(position, length, params, out, capacities, False)
+
+    def planar_terrain(self, position, length, params=None, out=None, capacities=None):
+        """The grid map and planar regions of the plane decomposition node's PlanarTerrain message for the get_submap
+        window around `position` (x, y) of `length` (x, y) metres: extract_planar_regions, then the node's
+        post-processing, in one library call (emap_planar_terrain; include/emap.h states every step).  `params`,
+        `capacities` and the returned dict as in extract_planar_regions (the PlaneSegmentationParams' postprocessing
+        fields apply here); a device `out` holds at least 10 * rows * cols floats.  "layers" maps the node's layer names
+        to (rows, cols) views: elevation_raw, elevation_before_postprocess (extract_planar_regions' "elevation"),
+        segmentation, plane_classification, elevationWithNaN, elevationWithNaN_i, elevationWithNaNClosed,
+        elevationWithNaNClosedDilated, smooth_planar and elevation.  Note that "elevation" here is the post-processed
+        layer (non-planar cells dilated and lifted), not the one segment_planes and extract_planar_regions return."""
+        return self._planar_regions(position, length, params, out, capacities, True)
+
+    def _planar_regions(self, position, length, params, out, capacities, post):
+        """extract_planar_regions (post False) and planar_terrain (post True): the call with the capacity retry."""
         from .plane_segmentation import PlaneSegmentationParams
         prm = params or PlaneSegmentationParams()
         p, rp = prm.to_c(), prm.regions_to_c()
+        pp = prm.postprocess_to_c() if post else None
+        n_layers = _lib.EMAP_TERRAIN_LAYERS if post else 4
         req = np.array(_xy(position) + _xy(length), np.float64)
         win = np.zeros(5, np.int32)
         centre = np.zeros(2, np.float64)
         device = out is not None and _is_device(out)
         names = ["elevation_raw", "elevation", "segmentation", "plane_classification"]
+        if post:
+            names = ["elevation_raw", "elevation_before_postprocess", "segmentation", "plane_classification",
+                     "elevationWithNaN", "elevationWithNaN_i", "elevationWithNaNClosed",
+                     "elevationWithNaNClosedDilated", "smooth_planar", "elevation"]
         caps = tuple(int(v) for v in (capacities or self._region_caps))
         for attempt in range(2):
             with self.map_lock:
@@ -634,7 +656,7 @@ class ElevationMap:
                     ptr = lambda a: a.data_ptr()  # noqa: E731
                 else:
                     if out is None:
-                        out = np.zeros(4 * rows * cols, np.float32)
+                        out = np.zeros(n_layers * rows * cols, np.float32)
                     if out.dtype != np.float32 or not out.flags.c_contiguous:
                         raise TypeError("a host `out` must be a C-contiguous float32 NumPy array")
                     mk = lambda shape, dt: np.zeros(shape, dt)  # noqa: E731
@@ -646,9 +668,14 @@ class ElevationMap:
                 lay = (out.data_ptr(), out.numel()) if device else (out.ctypes.data, out.size)
                 if device:
                     self._after_framework()
-                self._check(self._L.emap_extract_planar_regions(self._h, req.ctypes.data, C.byref(p), C.byref(rp),
-                                                                lay[0], int(device), lay[1], ptr(planes), cap,
-                                                                C.byref(ro), ptr(info)))
+                if post:
+                    self._check(self._L.emap_planar_terrain(self._h, req.ctypes.data, C.byref(p), C.byref(rp),
+                                                            C.byref(pp), lay[0], int(device), lay[1], ptr(planes), cap,
+                                                            C.byref(ro), ptr(info)))
+                else:
+                    self._check(self._L.emap_extract_planar_regions(self._h, req.ctypes.data, C.byref(p), C.byref(rp),
+                                                                    lay[0], int(device), lay[1], ptr(planes), cap,
+                                                                    C.byref(ro), ptr(info)))
                 if device:
                     self._before_framework()
             info_h = info.cpu().numpy() if device else info

@@ -1,4 +1,4 @@
-"""Parameters of ElevationMap.segment_planes and ElevationMap.extract_planar_regions: the plane decomposition node's
+"""Parameters of ElevationMap.segment_planes, extract_planar_regions and planar_terrain: the plane decomposition node's
 `preprocessing`, `sliding_window_plane_extractor`, `contour_extraction` and `postprocessing` sections
 (convex_plane_decomposition_ros/config/parameters.yaml), with the two inclination thresholds as cosines, as
 ParameterLoading.cpp stores them."""
@@ -26,12 +26,18 @@ class PlaneSegmentationParams:
     # contour_extraction and postprocessing (extract_planar_regions only)
     margin_size: int = 1
     extracted_planes_height_offset: float = 0.0
+    # postprocessing (planar_terrain only)
+    nonplanar_height_offset: float = 0.02
+    nonplanar_horizontal_offset: int = 1
+    smoothing_dilation_size: float = 0.2
+    smoothing_box_kernel_size: float = 0.1
+    smoothing_gauss_kernel_size: float = 0.05
 
     @classmethod
     def from_yaml(cls, path):
         """Reads the `preprocessing`, `sliding_window_plane_extractor`, `contour_extraction` (marginSize) and
-        `postprocessing` (extracted_planes_height_offset) sections of a node parameter file; keys that are absent keep
-        their defaults, and `*_degrees` become cosines (ParameterLoading.cpp:49-59)."""
+        `postprocessing` sections of a node parameter file; keys that are absent keep their defaults, and `*_degrees`
+        become cosines (ParameterLoading.cpp:49-59)."""
         import yaml
         with open(path) as f:
             doc = yaml.safe_load(f) or {}
@@ -50,8 +56,11 @@ class PlaneSegmentationParams:
                 setattr(p, name, sw[key])
         if "marginSize" in (doc.get("contour_extraction") or {}):
             p.margin_size = doc["contour_extraction"]["marginSize"]
-        if "extracted_planes_height_offset" in (doc.get("postprocessing") or {}):
-            p.extracted_planes_height_offset = doc["postprocessing"]["extracted_planes_height_offset"]
+        post = doc.get("postprocessing") or {}
+        for key in ("extracted_planes_height_offset", "nonplanar_height_offset", "nonplanar_horizontal_offset",
+                    "smoothing_dilation_size", "smoothing_box_kernel_size", "smoothing_gauss_kernel_size"):
+            if key in post:
+                setattr(p, key, post[key])
         if "plane_inclination_threshold_degrees" in sw:
             p.plane_inclination_cos = math.cos(sw["plane_inclination_threshold_degrees"] * math.pi / 180.0)
         if "local_plane_inclination_threshold_degrees" in sw:
@@ -67,3 +76,8 @@ class PlaneSegmentationParams:
 
     def regions_to_c(self):
         return _lib.EmapRegionParams(int(self.margin_size), float(self.extracted_planes_height_offset))
+
+    def postprocess_to_c(self):
+        return _lib.EmapPostprocessParams(float(self.nonplanar_height_offset), int(self.nonplanar_horizontal_offset),
+                                          float(self.smoothing_dilation_size), float(self.smoothing_box_kernel_size),
+                                          float(self.smoothing_gauss_kernel_size))

@@ -515,6 +515,63 @@ int emap_extract_planar_regions(emap_handle* h, const double window[4], const em
                                 const emap_region_params* region_params, float* layers_out, int32_t out_is_device,
                                 int64_t out_floats, double* planes_out, int64_t planes_capacity,
                                 const emap_region_out* regions_out, int32_t* info);
+/* ---- planar terrain: the grid map of the plane decomposition node's PlanarTerrain message for one window, on the
+ * device: Postprocessing::postprocess (convex_plane_decomposition) after emap_extract_planar_regions.  DESIGN.md §4l
+ * gives the restatement.  Takes everything emap_extract_planar_regions takes plus post_params and writes the same
+ * planes_out, regions, polygons, vertices and info, byte for byte, and layers 0 .. 3 of layers_out as that call does.
+ * With res the map's resolution, E layer 1 (elevation) and M layer 3 (plane_classification, 0 or 1):
+ *  Kernel sizes (kernelSizeInPixels): 2 (int) round(size / res) + 1 in double, halves away from zero (0.1 / 0.04 =
+ *    2.5 gives 7), for the dilation, box and Gauss sizes; each at most EMAP_POST_MAX_KERNEL.
+ *  Layer 4 elevationWithNaN = M == 1 ? E : NaN.  Layer 5 elevationWithNaN_i = grid_map's minValues of layer 4 (the fill
+ *    of emap_segment_planes; the sign of a filled zero as stated there).  Layer 6 elevationWithNaNClosed =
+ *    cv::morphologyEx(MORPH_CLOSE) of layer 5 by MORPH_ELLIPSE of the dilation size, BORDER_REPLICATE.
+ *  Layer 7 elevationWithNaNClosedDilated = grid_map_filters_rsl's applyKernelFunction of layer 6 with a k x k window
+ *    (k the dilation size, h = (k - 1) / 2) and (data - offsets).maxCoeffOfFinites(): offsets(i, j) =
+ *    float(double(float(res)) * sqrt(double((i - h)^2 + (j - h)^2))), the difference in fp32, the window's corner
+ *    max(cell - h, 0) moved back to rows - k (cols - k) where the window would overshoot, so a cell within h of the edge
+ *    uses a window that is not centred on it.  maxCoeffOfFinites, restated from grid_map's published source (not
+ *    checked against a grid_map build): the max over the finite values, NaN when there are none (only when the window
+ *    has no planar cell; then layers 4 .. 8 are all NaN).
+ *  Layer 8 smooth_planar = cv::boxFilter (normalised, BORDER_REPLICATE) of the box size on layer 7, then
+ *    cv::GaussianBlur(ksize, 0, 0, BORDER_REPLICATE) of the Gauss size: the box sums in double times 1 / k^2 (double),
+ *    rounded to fp32 (exact, like OpenCV's, while the summed values lie within 29 binary orders of magnitude); the
+ *    Gaussian with cv::getGaussianKernel(k, 0, CV_32F)'s coefficients c, rows then columns, each pass c0 x0 + sum over
+ *    j of c_j (x_+j + x_-j) in fp32 without contraction: bit-identical to cv2 4.13 for k <= 3.  For a longer kernel
+ *    OpenCV's evaluation order is not reproduced; the result differs from cv2's by at most EMAP_POST_GAUSS_ULPS(k) units
+ *    in the last place of layer 7's largest magnitude.  That is the worst-case fp32 rounding bound of a k-term sum,
+ *    applied to both passes of both evaluations, so it holds for every input and evaluation order (DESIGN.md §4l gives
+ *    the derivation and the deviations measured).
+ *  Layer 9 elevation: with nonplanar_horizontal_offset > 0, E = M E + (1 - M) D in fp32, D the grey dilation of E by
+ *    MORPH_ELLIPSE of 2 offset + 1 (BORDER_REPLICATE); then, when region_params' plane_height_offset (the node's
+ *    extracted_planes_height_offset) or nonplanar_height_offset is not 0, E += float(ext + nonpl) and, when nonpl is not
+ *    0, E -= float(nonpl) M, each in fp32.  Eigen narrows a double scalar to the float matrix's scalar type before the
+ *    operation (promote_scalar_arg in Eigen's XprHelper.h, from Eigen's published source).
+ * layers_out: EMAP_TERRAIN_LAYERS planes of rows x cols row-major, out_floats >= EMAP_TERRAIN_LAYERS * rows * cols.
+ * Windows outside the map, without a finite cell (nothing but info written) or below 2 x 2 behave as in
+ * emap_extract_planar_regions; host output comes back in the same single copy and synchronisation, device output is
+ * stream-ordered and can be captured; the launches depend on the parameters and the window size only; the map state is
+ * not changed.  The scratch grows emap_segment_planes' block by 20 bytes per cell; with host output the staging at the
+ * block's tail and the handle's pinned host buffer each grow by another 24 bytes per cell (six more layers).
+ * EMAP_ERR_INVALID, with nothing
+ * written or launched, additionally for a NULL post_params, a smoothing size that is not finite and >= 0 or gives a
+ * kernel above EMAP_POST_MAX_KERNEL, a horizontal offset outside 0 .. EMAP_POST_MAX_OFFSET, a non-finite
+ * nonplanar_height_offset, an out_floats below EMAP_TERRAIN_LAYERS * rows * cols, and a window inside the map with
+ * fewer rows or columns than the dilation size. */
+typedef struct emap_postprocess_params {
+  double nonplanar_height_offset;      /* postprocessing/nonplanar_height_offset [m] */
+  int32_t nonplanar_horizontal_offset; /* postprocessing/nonplanar_horizontal_offset [cells], 0 .. EMAP_POST_MAX_OFFSET */
+  double smoothing_dilation_size;      /* [m], >= 0 */
+  double smoothing_box_kernel_size;    /* [m], >= 0 */
+  double smoothing_gauss_kernel_size;  /* [m], >= 0 */
+} emap_postprocess_params;
+#define EMAP_TERRAIN_LAYERS 10
+#define EMAP_POST_MAX_KERNEL 63
+#define EMAP_POST_MAX_OFFSET 31
+#define EMAP_POST_GAUSS_ULPS(k) (4 * (k) + 1)   /* the bound for a k-tap Gaussian, k >= 5 */
+int emap_planar_terrain(emap_handle* h, const double window[4], const emap_plane_params* plane_params,
+                        const emap_region_params* region_params, const emap_postprocess_params* post_params,
+                        float* layers_out, int32_t out_is_device, int64_t out_floats, double* planes_out,
+                        int64_t planes_capacity, const emap_region_out* regions_out, int32_t* info);
 /* ---- the exported map as a point cloud and as normal arrows: the ROS node's publishAsPointCloud
  * (elevation_mapping_ros.cpp:501-505, grid_map's toPointCloud(map, {"elevation"}, "elevation")) and publishNormalAsArrow
  * (:751-778), restated from grid_map's published source (not checked against a grid_map build).  Coordinates are those of
