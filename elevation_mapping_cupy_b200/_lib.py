@@ -57,6 +57,19 @@ class EmapRegionOut(C.Structure):
                 ("polygons_capacity", C.c_int64), ("vertices", C.c_void_p), ("vertices_capacity", C.c_int64)]
 
 
+class EmapRegionTables(C.Structure):
+    _fields_ = [("regions", C.c_void_p), ("n_regions", C.c_int64), ("polygons", C.c_void_p),
+                ("n_polygons", C.c_int64), ("vertices", C.c_void_p), ("n_vertices", C.c_int64)]
+
+
+class EmapProjectionOut(C.Structure):
+    _fields_ = [("index", C.c_void_p), ("point", C.c_void_p), ("convex", C.c_void_p)]
+
+
+EMAP_CONVEX_MAX_VERTICES = 64
+PROJECTION_STATUS = ("grown", "zero_radius", "max_iter", "no_region", "invalid_query", "bad_table")
+
+
 class EmapDepthCamera(C.Structure):
     _fields_ = [("height", C.c_int32), ("width", C.c_int32), ("depth", C.c_void_p), ("confidence", C.c_void_p),
                 ("rgb", C.c_void_p), ("features", C.c_void_p), ("fx", C.c_double), ("fy", C.c_double),
@@ -133,6 +146,9 @@ SIGNATURES = {
                                               C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
     "emap_planar_terrain": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_int32, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]),
+    "emap_project_to_planar_regions": (C.c_int, [C.c_void_p, C.POINTER(EmapRegionTables), C.c_int32, C.c_int64,
+                                                 C.c_void_p, C.c_int32, C.c_double, C.c_int32, C.c_double,
+                                                 C.POINTER(EmapProjectionOut), C.c_int32]),
     "emap_get_map_points": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_get_normal_arrows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_layer_device_ptr": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),

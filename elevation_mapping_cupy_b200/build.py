@@ -9,11 +9,13 @@ from concurrent.futures import ThreadPoolExecutor
 PKG = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(PKG, "csrc")
 LIB = os.path.join(PKG, "libemap.so")
-SOURCES = ["emap_api.cu", "emap_export_api.cu", "emap_polygon_api.cu", "emap_plugins_api.cu"]
+SOURCES = ["emap_api.cu", "emap_export_api.cu", "emap_polygon_api.cu", "emap_plugins_api.cu",
+           "emap_terrain_query_api.cu"]
 HEADERS = ["emap_handle.cuh", "emap_kernels.cuh", "emap_export.cuh", "emap_plugins.cuh", "emap_device.cuh",
            "emap_inpaint.cuh", "emap_semantic.cuh", "emap_polygon.cuh", "emap_semantic_plugins.cuh", "emap_image.cuh",
            "emap_submap.cuh", "emap_mapcloud.cuh", "emap_initialize.cuh", "emap_sources.cuh", "emap_plan.cuh",
-           "emap_planes.cuh", "emap_regions.cuh", "emap_postprocess.cuh", os.path.join("..", "..", "include", "emap.h")]
+           "emap_planes.cuh", "emap_regions.cuh", "emap_postprocess.cuh", "emap_terrain_query.cuh",
+           os.path.join("..", "..", "include", "emap.h")]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMPILE_FLAGS = ["-O3", "-std=c++17"] + GENCODE + ["-lineinfo", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 LINK_FLAGS = GENCODE + ["-shared", "-cudart", "shared"]

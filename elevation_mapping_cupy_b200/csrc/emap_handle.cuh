@@ -219,6 +219,11 @@ struct emap_handle {
     int grid = 0;
   } inpaint;
   DevBuf<char> pca_block;          // emap_features_pca: one device block carved by carve_pca
+  struct {                         // emap_project_to_planar_regions (grown to the largest call): the device block
+    DevBuf<char> block;            // carved by carve_query, the upload of host tables and queries, and the pinned
+    StagedUpload up;               // staging of host output
+    PinnedBuf<char> down;
+  } query;
   StagedUpload img_up;             // emap_input_image with a host image
   StagedUpload init_up;            // emap_initialize_map's arrays
   // misc

@@ -623,6 +623,89 @@ class ElevationMap:
         layer (non-planar cells dilated and lifted), not the one segment_planes and extract_planar_regions return."""
         return self._planar_regions(position, length, params, out, capacities, True)
 
+    def project_to_planar_regions(self, terrain, queries, penalty_z_weight=0.0, convex_vertices=0, growth_factor=1.05,
+                                  out=None):
+        """The best planar region for each query point and the point projected onto it, optionally with a convex
+        polygon grown around it inside the region's boundary (convex_plane_decomposition's
+        getBestPlanarRegionAtPositionInWorld, searched exhaustively, and growConvexPolygonInsideShape), in one library
+        call (emap_project_to_planar_regions; include/emap.h states every step).  `terrain`: a dict returned by
+        extract_planar_regions or planar_terrain; its "tables" are read in place (NumPy or torch CUDA).  `queries`: (N,
+        3) world points, float64 NumPy or a CUDA tensor.  The cost of a region is the squared distance to the projected
+        point plus penalty_z_weight * |z| of that point.  `convex_vertices`: 0 (no growth) or 3 ..
+        EMAP_CONVEX_MAX_VERTICES.  `out`: None, or a dict of "index" (N, 3) int32, "point" (N, 6) float64 and, with
+        growth, "convex" (N, V, 5) float64, all NumPy or all torch CUDA tensors, written in place.  Device queries or a
+        device `out` keep everything on the device (stream-ordered after the caller's work, no host synchronisation).
+        Returns "region" (row, -1 for none), "label", "cost", "position_plane" (N, 2), "position_world" (N, 3), "status"
+        (0 grown, 1 zero radius, 2 max iterations, 3 no region, 4 invalid query, 5 bad table), "iterations" and, with
+        growth, "convex_plane" (N, V, 2) and "convex_world" (N, V, 3); all views of `out`."""
+        tabs = terrain["tables"]
+        reg, poly, vert = tabs["regions"], tabs["polygons"], tabs["vertices"]
+        tables_dev = _is_device(reg)
+        n_conv = int(convex_vertices)
+        device = _is_device(queries) or (out is not None and _is_device(out["index"]))
+        if device:
+            import torch
+            dev = (queries if _is_device(queries) else out["index"]).device
+            if not _is_device(queries):
+                queries = torch.as_tensor(np.asarray(queries, np.float64), device=dev)
+            queries = queries.to(torch.float64).contiguous()
+            n = int(queries.shape[0])
+            if out is None:
+                out = {"index": torch.empty((n, 3), dtype=torch.int32, device=dev),
+                       "point": torch.empty((n, 6), dtype=torch.float64, device=dev)}
+                if n_conv:
+                    out["convex"] = torch.empty((n, n_conv, 5), dtype=torch.float64, device=dev)
+            ptr = lambda a: a.data_ptr() if a is not None else None  # noqa: E731
+            q_ptr = queries.data_ptr()
+        else:
+            queries = np.ascontiguousarray(queries, np.float64)
+            n = int(queries.shape[0])
+            if out is None:
+                out = {"index": np.zeros((n, 3), np.int32), "point": np.zeros((n, 6), np.float64)}
+                if n_conv:
+                    out["convex"] = np.zeros((n, n_conv, 5), np.float64)
+            ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
+            q_ptr = queries.ctypes.data
+        if queries.shape != (n, 3):
+            raise ValueError("queries must be (N, 3)")
+        shapes = {"index": (n, 3), "point": (n, 6), "convex": (n, n_conv, 5)}
+        for k in ("index", "point") + (("convex",) if n_conv else ()):
+            a = out[k]
+            if tuple(a.shape) != shapes[k] or _is_device(a) != device or not (
+                    a.is_contiguous() if device else a.flags.c_contiguous):
+                raise TypeError("out[%r] must be a contiguous %s array of shape %s" % (
+                    k, "CUDA" if device else "NumPy", shapes[k]))
+        tptr = (lambda a: a.data_ptr()) if tables_dev else (lambda a: np.ascontiguousarray(a).ctypes.data)  # noqa: E731
+        if not tables_dev:
+            reg, poly, vert = (np.ascontiguousarray(a, dt) for a, dt in ((reg, np.float64), (poly, np.int32),
+                                                                        (vert, np.float64)))
+        t = _lib.EmapRegionTables(tptr(reg), len(reg), tptr(poly), len(poly), tptr(vert), len(vert))
+        o = _lib.EmapProjectionOut(ptr(out["index"]), ptr(out["point"]), ptr(out.get("convex") if n_conv else None))
+        if device or tables_dev:
+            self._after_framework()
+        self._check(self._L.emap_project_to_planar_regions(self._h, C.byref(t), int(tables_dev), n, q_ptr,
+                                                           int(_is_device(queries)), float(penalty_z_weight), n_conv,
+                                                           float(growth_factor), C.byref(o), int(device)))
+        if device:
+            self._before_framework()
+        index, point = out["index"], out["point"]
+        region = index[:, 0]
+        if device:
+            import torch
+            labels = (reg[:, 0] if tables_dev else torch.as_tensor(reg[:, 0])).to(point.device)
+            lab = torch.full((n,), float("nan"), dtype=torch.float64, device=point.device)
+            if len(reg):
+                lab = torch.where(region >= 0, labels[region.clamp(min=0).long()], lab)
+        else:
+            labels = reg[:, 0].cpu().numpy() if tables_dev else reg[:, 0]
+            lab = np.where(region >= 0, labels[np.clip(region, 0, None)] if len(reg) else np.nan, np.nan)
+        res = {"region": region, "label": lab, "cost": point[:, 0], "position_plane": point[:, 1:3],
+               "position_world": point[:, 3:6], "status": index[:, 1], "iterations": index[:, 2]}
+        if n_conv:
+            res["convex_plane"] = out["convex"][:, :, :2]
+            res["convex_world"] = out["convex"][:, :, 2:]
+        return res
+
     def _planar_regions(self, position, length, params, out, capacities, post):
         """extract_planar_regions (post False) and planar_terrain (post True): the call with the capacity retry."""
         from .plane_segmentation import PlaneSegmentationParams

@@ -572,6 +572,88 @@ int emap_planar_terrain(emap_handle* h, const double window[4], const emap_plane
                         const emap_region_params* region_params, const emap_postprocess_params* post_params,
                         float* layers_out, int32_t out_is_device, int64_t out_floats, double* planes_out,
                         int64_t planes_capacity, const emap_region_out* regions_out, int32_t* info);
+/* ---- projection onto the planar regions and convex footholds: convex_plane_decomposition's SegmentedPlaneProjection
+ * (getBestPlanarRegionAtPositionInWorld, searched exhaustively as testConvexApproximation.cpp's naive version) and
+ * ConvexRegionGrowing (growConvexPolygonInsideShape), for a batch of query points on the device.  DESIGN.md §4l gives
+ * the restatement.  tables: the regions, polygons and vertices tables as emap_extract_planar_regions /
+ * emap_planar_terrain wrote them (info[8] = complete = 1), in host (tables_on_device 0) or device memory.
+ * queries: n_queries world (x, y, z) doubles, host or device.  The handle's map state is not read or changed; the call
+ * uses the handle's stream, staging and scratch only.
+ * Per query p and region row r (ascending), with [R | t] the region's plane-to-world transform:
+ *  Plane frame: q = T^-1 p as Eigen's Isometry3d::inverse() computes it: linear R^T, translation -(R^T t); q_i =
+ *    ((A_i0 p0 + A_i1 p1) + A_i2 p2) + u_i, A = R^T, u_i = -((A_i0 t0 + A_i1 t1) + A_i2 t2).
+ *  projectToPlanarRegion of (q.x, q.y): the first inset (table order) whose outer polygon contains the point (bounded
+ *    side, the boundary counts as inside) keeps it, unless it lies in one of that inset's holes (its boundary counts
+ *    as in the hole): then it goes to the first such hole's closest edge.  Inside no inset, it goes to the closest edge
+ *    of each inset outer; the inset whose projection c has the least (c.x - q.x)^2 + (c.y - q.y)^2 wins (strict <, the
+ *    first from DBL_MAX).  Closest edge of a polygon: the first least CGAL squared distance over its edges in vertex
+ *    order (edge k from vertex k to k + 1, the last closing the polygon).  Onto an edge s -> e: v = e - s, L =
+ *    sqrt(v.x^2 + v.y^2), n = v / L, coefficient = std::min(std::max(0.0, n . (p - s)), L), result coefficient n + s.
+ *  World: w_i = (t_i + x R_i0) + y R_i1.  Cost: ((dx^2 + dy^2) + dz^2) + penalty_z_weight |w_z|, d = p - w.
+ *  Result: the first region of least cost (std::min_element over the rows: ties to the lowest row).  The reference's
+ *    bounding-box pruning and sort can differ from it only at exact cost ties or sub-ulp violations of its bound; the
+ *    device does not prune.
+ * Convex growth (n_convex > 0), inside the chosen region's BOUNDARY (outer and holes), around the projected plane
+ * point c, with ConvexRegionGrowing.cpp's steps: radius = 0.999 distance(c, boundary) (sqrt of the least squared
+ * edge distance, 0 when it is 0); createRegularPolygon (vertex i = (radius cos_i + c.x, radius sin_i + c.y), cos_i and
+ * sin_i the host C library's cos / sin of i * ((2 pi) / n_convex)); then at most EMAP_GROW_MAX_ITER sweeps over the
+ * unblocked vertices in order: candidate = growth (v - c) + c; it moves when the 5-point sub-polygon (2nd and 1st
+ * clockwise neighbours, candidate, 1st and 2nd counter-clockwise neighbours) is convex (CGAL's is_convex_2) and either
+ * both neighbours and the candidate lie in the vertex's free circle (squared distance <= squared radius) or neither
+ * neighbour-to-candidate segment meets a boundary edge (closed segments); in the second case the free circle becomes
+ * (candidate, least squared edge distance).  A move updates the centre c += (1.0 / n) (candidate - v) before v is
+ * replaced; a vertex that cannot move is blocked.
+ * Arithmetic: every predicate (orientation, bounded side, closed segment intersection, is_convex_2, comparisons) is
+ * exact for finite coordinates whose products neither overflow nor underflow (magnitudes and non-zero differences
+ * within 2^-480 .. 2^480): a double filter with Shewchuk's orient2d error bound, then expansion arithmetic with
+ * TwoSum / TwoProduct (fma).  Bounded side: on a closed edge is the boundary, else the even-odd rule.  Every
+ * construction is double arithmetic in the order written here, without contraction.  CGAL's squared distance from a
+ * point p to segment s -> e (Distance_2/Point_2_Segment_2.h, line_from_pointsC2, Point_2_Line_2.h) is restated from
+ * CGAL's published source and not checked against a CGAL build: d = (p - s) . (e - s); d <= 0 gives |p - s|^2;
+ * otherwise with f = |e - s|^2, d > f gives (p.x - e.x)^2 + (p.y - e.y)^2; otherwise (a p.x + b p.y + c)^2 / (a^2 +
+ * b^2) with (a, b, c) = (0, 1, -s.y) for a horizontal edge to +x, (0, -1, s.y) to -x, (-1, 0, s.x) for a vertical edge
+ * to +y, (1, 0, -s.x) to -y, else (s.y - e.y, e.x - s.x, -s.x a - s.y b).  Eigen's sum orders above are restated from
+ * Eigen's published source, not checked against an Eigen build.  The same inputs give the same bits on every call.
+ * Outputs (emap_projection_out): index, 3 int32 per query: {region row (-1: none), status, sweeps}; point, 6 doubles:
+ * {cost, plane x, y, world x, y, z}; convex (NULL when n_convex is 0), 5 doubles per query and vertex: {plane x, y,
+ * world x, y, z} (the world point as above).  Status EMAP_PROJECTION_*: GROWN (also without growth), ZERO_RADIUS (the
+ * point is on the boundary: every vertex is the centre, as the reference returns), MAX_ITER (EMAP_GROW_MAX_ITER
+ * sweeps ran), NO_REGION (no region), INVALID_QUERY (a non-finite coordinate), BAD_TABLE (device tables that break
+ * the layout: see below).  The last three write region -1, cost +inf, NaN positions and NaN vertices.
+ * Host tables are checked before anything launches: every polygon row needs a region in range, regions ascending
+ * without a gap, roles in the order boundary outer, its holes, then each inset outer followed by its holes (so every
+ * region has an inset), inset -1 for the boundary and the running inset index otherwise, at least one vertex and a
+ * vertex range inside n_vertices.  Device tables get the same checks on the device; any failure makes every query
+ * BAD_TABLE, and no kernel reads outside the counts passed in.
+ * Host output comes back in one device-to-host copy and one synchronisation; device output (index, point and convex
+ * device memory) is stream-ordered with no host synchronisation and can be captured into a CUDA graph (with device
+ * tables and queries; capture after an eager call of the largest size: growing the scratch synchronises).  Host
+ * tables or queries are staged and uploaded in one copy.  Kernels: none for n_queries = 0, else 2, plus 1 with
+ * n_convex > 0.  One warp per query; the work is the edges of every region's insets per query, plus the boundary's
+ * edges per growth step that leaves a free circle.
+ * EMAP_ERR_INVALID, with nothing written or launched: a NULL tables / out, a NULL table with a count above 0, NULL
+ * queries or outputs with n_queries > 0 (convex with n_convex > 0), a negative count, n_regions, n_polygons or
+ * n_queries above 2^31 - 1, n_convex outside 0, 3 .. EMAP_CONVEX_MAX_VERTICES, a growth_factor that is not finite and
+ * > 1, a penalty_z_weight that is not finite and >= 0 (the reference's bound needs a non-negative penalty), and host
+ * tables that fail the checks above. */
+typedef struct emap_region_tables {
+  const double* regions;   int64_t n_regions;      /* EMAP_REGION_ROW doubles per region */
+  const int32_t* polygons; int64_t n_polygons;     /* EMAP_REGION_POLYGON int32 per polygon */
+  const double* vertices;  int64_t n_vertices;     /* 2 doubles per vertex */
+} emap_region_tables;
+typedef struct emap_projection_out {
+  int32_t* index;          /* 3 per query: region row (-1: none), status, growth sweeps */
+  double* point;           /* 6 per query: cost, plane-frame x y, world x y z */
+  double* convex;          /* 5 per query and vertex: plane-frame x y, world x y z; NULL when n_convex == 0 */
+} emap_projection_out;
+#define EMAP_CONVEX_MAX_VERTICES 64
+#define EMAP_GROW_MAX_ITER 1000   /* ConvexRegionGrowing.cpp's maxIter */
+enum { EMAP_PROJECTION_GROWN = 0, EMAP_PROJECTION_ZERO_RADIUS = 1, EMAP_PROJECTION_MAX_ITER = 2,
+       EMAP_PROJECTION_NO_REGION = 3, EMAP_PROJECTION_INVALID_QUERY = 4, EMAP_PROJECTION_BAD_TABLE = 5 };
+int emap_project_to_planar_regions(emap_handle* h, const emap_region_tables* tables, int32_t tables_on_device,
+                                   int64_t n_queries, const double* queries, int32_t queries_on_device,
+                                   double penalty_z_weight, int32_t n_convex, double growth_factor,
+                                   const emap_projection_out* out, int32_t out_is_device);
 /* ---- the exported map as a point cloud and as normal arrows: the ROS node's publishAsPointCloud
  * (elevation_mapping_ros.cpp:501-505, grid_map's toPointCloud(map, {"elevation"}, "elevation")) and publishNormalAsArrow
  * (:751-778), restated from grid_map's published source (not checked against a grid_map build).  Coordinates are those of
