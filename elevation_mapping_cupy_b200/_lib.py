@@ -70,6 +70,27 @@ EMAP_CONVEX_MAX_VERTICES = 64
 PROJECTION_STATUS = ("grown", "zero_radius", "max_iter", "no_region", "invalid_query", "bad_table")
 
 
+class EmapGrid(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("rows", C.c_int64), ("cols", C.c_int64), ("position", C.c_double * 2),
+                ("resolution", C.c_double)]
+
+
+class EmapLineMaxOut(C.Structure):
+    _fields_ = [("index", C.c_void_p), ("value", C.c_void_p)]
+
+
+class EmapLineValuesOut(C.Structure):
+    _fields_ = [("rows", C.c_void_p), ("capacity", C.c_int64), ("counts", C.c_void_p), ("first", C.c_void_p),
+                ("info", C.c_void_p)]
+
+
+class EmapDerivativeOut(C.Structure):
+    _fields_ = [("index", C.c_void_p), ("value", C.c_void_p)]
+
+
+EMAP_DERIVATIVE_INSIDE, EMAP_DERIVATIVE_OUTSIDE = 0, 1
+
+
 class EmapDepthCamera(C.Structure):
     _fields_ = [("height", C.c_int32), ("width", C.c_int32), ("depth", C.c_void_p), ("confidence", C.c_void_p),
                 ("rgb", C.c_void_p), ("features", C.c_void_p), ("fx", C.c_double), ("fy", C.c_double),
@@ -149,6 +170,12 @@ SIGNATURES = {
     "emap_project_to_planar_regions": (C.c_int, [C.c_void_p, C.POINTER(EmapRegionTables), C.c_int32, C.c_int64,
                                                  C.c_void_p, C.c_int32, C.c_double, C.c_int32, C.c_double,
                                                  C.POINTER(EmapProjectionOut), C.c_int32]),
+    "emap_max_values_between": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
+                                          C.POINTER(EmapLineMaxOut), C.c_int32]),
+    "emap_values_between": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
+                                      C.POINTER(EmapLineValuesOut), C.c_int32]),
+    "emap_grid_derivatives": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
+                                        C.c_int32, C.POINTER(EmapDerivativeOut), C.c_int32]),
     "emap_get_map_points": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_get_normal_arrows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_layer_device_ptr": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),

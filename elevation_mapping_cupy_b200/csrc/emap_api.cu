@@ -459,7 +459,7 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   h->stream = h->own_stream;
   for (Event* ev : {&h->in.staging_free[0], &h->in.staging_free[1], &h->in.copied, &h->in.host_free, &h->ev_fork,
                     &h->ev_join, &h->ev_order, &h->img_up.staged, &h->init_up.staged,
-                    &h->query.up.staged})
+                    &h->query.up.staged, &h->lookup.up.staged})
     if ((e = ev->create(cudaEventDisableTiming)) != cudaSuccess) return bail("event", e);
   for (Event& ev : h->st.ev) if ((e = ev.create(cudaEventDefault)) != cudaSuccess) return bail("event", e);
 #define ALLOC(buf, n) if ((e = (buf).alloc(n)) != cudaSuccess) return bail("cudaMalloc", e)

@@ -224,6 +224,12 @@ struct emap_handle {
     StagedUpload up;               // staging of host output
     PinnedBuf<char> down;
   } query;
+  struct {                         // the grid lookups (grown to the largest call): the device block carved by
+    DevBuf<char> block;            // carve_lookup, emap_values_between's host-bound rows, the upload of a host grid and
+    DevBuf<double> rows;           // queries, and the pinned staging of host output
+    StagedUpload up;
+    PinnedBuf<char> down;
+  } lookup;
   StagedUpload img_up;             // emap_input_image with a host image
   StagedUpload init_up;            // emap_initialize_map's arrays
   // misc

@@ -12,6 +12,7 @@
 #include <cuda_runtime.h>
 
 #include "emap_export.cuh"
+#include "emap_grid.cuh"
 
 #define SUBMAP_MAX_WINDOWS 1024
 #define SUBMAP_ROWS 8              // output rows per work item: one warp per row
@@ -223,9 +224,8 @@ __device__ __forceinline__ float tsub_funkey(u32 k) {
 
 // Sample k of window cell (row, col) with exported elevation h, through T, in double with every operation rounded
 // on its own (no contraction): p = (x, y, h), then for k = 1..4 (x - s, y), (x + s, y), (x, y - s), (x, y + s).
-// Returns its key / output cell, or -1 when (q.x, q.y) is outside the new map: with o = 0.5 * len per axis, inside is
-// 0 <= -((q - pos) - o) < len (checkIfPositionWithinMap), and the index is trunc(-(((q - o) - pos) / res))
-// (getIndexFromPosition), clamped to [0, size - 1].
+// Returns its key / output cell, or -1 when (q.x, q.y) is outside the new map (grid_axis_index: checkIfPositionWithinMap
+// and getIndexFromPosition).
 __device__ __forceinline__ long long tsub_sample(const TSubWin& w, const TSubArgs& a, int row, int col, double h, int k,
                                                  double& qz) {
   double p[3] = {__dadd_rn(w.x0, -__dmul_rn(a.res, (double)row)), __dadd_rn(w.y0, -__dmul_rn(a.res, (double)col)), h};
@@ -243,14 +243,8 @@ __device__ __forceinline__ long long tsub_sample(const TSubWin& w, const TSubArg
   qz = q[2];
   int idx[2];
 #pragma unroll
-  for (int ax = 0; ax < 2; ax++) {
-    const double o = __dmul_rn(0.5, w.len[ax]);
-    const double u = -__dadd_rn(__dadd_rn(q[ax], -w.pos[ax]), -o);
-    if (!(u >= 0.0 && u < w.len[ax])) return -1;
-    const int n = ax ? w.ncols : w.nrows;
-    const int i = __double2int_rz(-__ddiv_rn(__dadd_rn(__dadd_rn(q[ax], -o), -w.pos[ax]), a.res));
-    idx[ax] = min(max(i, 0), n - 1);
-  }
+  for (int ax = 0; ax < 2; ax++)
+    if (!grid_axis_index(q[ax], w.pos[ax], w.len[ax], a.res, ax ? w.ncols : w.nrows, idx[ax])) return -1;
   return w.cell0 + (long long)idx[0] * w.ncols + idx[1];
 }
 

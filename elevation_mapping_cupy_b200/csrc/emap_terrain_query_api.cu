@@ -1,7 +1,9 @@
-// emap_terrain_query_api.cu -- queries on the planar terrain of the C ABI (include/emap.h):
-// emap_project_to_planar_regions, over the kernels of emap_terrain_query.cuh.
+// emap_terrain_query_api.cu -- queries on the planar terrain and its layers of the C ABI (include/emap.h):
+// emap_project_to_planar_regions over the kernels of emap_terrain_query.cuh, and emap_max_values_between,
+// emap_values_between and emap_grid_derivatives over those of emap_grid_lookup.cuh.
 #include <algorithm>
 
+#include "emap_grid_lookup.cuh"
 #include "emap_handle.cuh"
 #include "emap_terrain_query.cuh"
 
@@ -47,7 +49,57 @@ const char* check_arguments(const emap_region_tables* t, int32_t tables_on_devic
   return nullptr;
 }
 
+// The grid and query checks the three lookups share (min_cells: the fewest rows and columns the call takes).
+const char* check_lookup(const emap_grid* g, int64_t min_cells, int64_t n, const double* queries, bool outputs) {
+  if (const char* e = gl_check_grid(g->data, g->rows, g->cols, g->position, g->resolution, min_cells)) return e;
+  if (n < 0 || n > INT32_MAX) return "n_queries must be 0 .. 2^31 - 1";
+  if (n && (!queries || !outputs)) return "null queries or output";
+  return nullptr;
+}
+
+// The grid and queries as the kernels read them: a host grid and host queries (per_query doubles each) staged and
+// uploaded in one copy.
+int lookup_inputs(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, int64_t n, const double* queries,
+                  int32_t queries_on_device, int per_query, GlGrid& g, const double*& q) {
+  g.data = grid->data;
+  g.rows = (int)grid->rows;
+  g.cols = (int)grid->cols;
+  g.res = grid->resolution;
+  for (int a = 0; a < 2; a++) {
+    g.pos[a] = grid->position[a];
+    g.len[a] = (double)(a ? grid->cols : grid->rows) * grid->resolution;
+  }
+  q = queries;
+  const size_t grid_bytes = grid_on_device ? 0 : sizeof(float) * grid->rows * grid->cols;
+  const size_t q_off = (grid_bytes + 255) & ~(size_t)255;
+  const size_t q_bytes = queries_on_device ? 0 : sizeof(double) * per_query * n;
+  if (!grid_bytes && !q_bytes) return 0;
+  const size_t up = q_off + q_bytes;
+  if (int rc = h->lookup.up.room(h, up)) return rc;
+  if (grid_bytes) {
+    memcpy(h->lookup.up.host, grid->data, grid_bytes);
+    g.data = (const float*)(char*)h->lookup.up.dev;
+  }
+  if (q_bytes) {
+    memcpy(h->lookup.up.host + q_off, queries, q_bytes);
+    q = (const double*)(h->lookup.up.dev + q_off);
+  }
+  return h->lookup.up.send(h, up);
+}
+
+// Host output: `bytes` of the device block back into the pinned staging, one synchronisation.
+int lookup_back(emap_handle* h, size_t bytes) {
+  if (h->lookup.down.size() < bytes) CK(h->lookup.down.alloc(bytes));
+  CK(cudaMemcpyAsync(h->lookup.down, h->lookup.block, bytes, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
+
 }  // namespace
+
+static_assert(EMAP_GRID_MAX_EXTENT == GL_MAX_EXTENT && EMAP_GRID_MIN_RESOLUTION == GL_MIN_RES, "the grid bounds");
+static_assert((int)EMAP_DERIVATIVE_INSIDE == (int)GL_INSIDE && (int)EMAP_DERIVATIVE_OUTSIDE == (int)GL_OUTSIDE,
+              "the derivative statuses");
 
 static_assert(EMAP_REGION_ROW == PQ_ROW && EMAP_REGION_POLYGON == PQ_POLY, "the region table layout");
 static_assert(EMAP_CONVEX_MAX_VERTICES == PQ_MAX_CONVEX && EMAP_GROW_MAX_ITER == PQ_MAX_ITER, "the growth limits");
@@ -128,6 +180,140 @@ int emap_project_to_planar_regions(emap_handle* h, const emap_region_tables* tab
     memcpy(out->point, h->query.down, pt_bytes);
     if (n_convex) memcpy(out->convex, h->query.down + pt_bytes, cv_bytes);
     memcpy(out->index, h->query.down + pt_bytes + cv_bytes, sizeof(int32_t) * 3 * N);
+  }
+  return EMAP_OK;
+}
+
+int emap_max_values_between(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, int64_t n_queries,
+                            const double* lines, int32_t lines_on_device, const emap_line_max_out* out,
+                            int32_t out_is_device) {
+  ENTER(h);
+  const char* e = !grid || !out ? "null argument"
+                                : check_lookup(grid, 1, n_queries, lines, out->index && out->value);
+  if (e) return fail(h, EMAP_ERR_INVALID, (std::string("emap_max_values_between: ") + e).c_str());
+  if (n_queries == 0) return EMAP_OK;
+  NvtxRange nv("max_values_between");
+  const int64_t N = n_queries;
+  const size_t vb = sizeof(double) * 3 * N, ib = sizeof(int32_t) * 3 * N;
+  if (!out_is_device)
+    if (int rc = grow(h, h->lookup.block, vb + ib, 0, false)) return rc;
+  GlGrid g;
+  const double* q;
+  if (int rc = lookup_inputs(h, grid, grid_on_device, N, lines, lines_on_device, 4, g, q)) return rc;
+  double* value = out_is_device ? out->value : (double*)(char*)h->lookup.block;
+  int32_t* index = out_is_device ? out->index : (int32_t*)(h->lookup.block + vb);
+  k_gl_max<<<cdiv(N, GL_WARPS), 32 * GL_WARPS, 0, h->stream>>>(g, q, N, index, value);
+  LAUNCH_CHECK();
+  if (!out_is_device) {
+    if (int rc = lookup_back(h, vb + ib)) return rc;
+    memcpy(out->value, h->lookup.down, vb);
+    memcpy(out->index, h->lookup.down + vb, ib);
+  }
+  return EMAP_OK;
+}
+
+int emap_values_between(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, int64_t n_queries,
+                        const double* lines, int32_t lines_on_device, const emap_line_values_out* out,
+                        int32_t out_is_device) {
+  ENTER(h);
+  const char* e = !grid || !out ? "null argument"
+                                : check_lookup(grid, 1, n_queries, lines, out->counts && out->first);
+  if (!e && !out->info) e = "null info";
+  if (!e && out->capacity < 0) e = "capacity must be >= 0";
+  if (!e && out->capacity > 0 && !out->rows) e = "null rows with a capacity above 0";
+  if (e) return fail(h, EMAP_ERR_INVALID, (std::string("emap_values_between: ") + e).c_str());
+  if (n_queries == 0) {
+    if (out_is_device) {
+      CK(cudaMemsetAsync(out->info, 0, 2 * sizeof(int64_t), h->stream));
+      CK(cudaMemsetAsync((char*)(out->info + 1), 1, 1, h->stream));     // complete = 1 (little-endian)
+    } else {
+      out->info[0] = 0;
+      out->info[1] = 1;
+    }
+    return EMAP_OK;
+  }
+  NvtxRange nv("values_between");
+  const int64_t N = n_queries, nb = cdiv(N, GL_WARPS);
+  // the block: per-block sums (then offsets), then what host output copies back in one piece: info, first, counts
+  Carver c0{0};
+  c0.take<int64_t>(nb);
+  const size_t back0 = c0.bytes;
+  c0.take<int64_t>(2);
+  c0.take<int64_t>(N);
+  c0.take<int32_t>(N);
+  if (int rc = grow(h, h->lookup.block, c0.bytes, 0, false)) return rc;
+  Carver c{(uintptr_t)(char*)h->lookup.block};
+  int64_t* block_sum = c.take<int64_t>(nb);
+  int64_t* info = c.take<int64_t>(2);
+  int64_t* first = c.take<int64_t>(N);
+  int32_t* counts = c.take<int32_t>(N);
+  const size_t back_bytes = c.bytes - back0;
+  if (out_is_device) {
+    info = out->info;
+    first = out->first;
+    counts = out->counts;
+  }
+  GlGrid g;
+  const double* q;
+  if (int rc = lookup_inputs(h, grid, grid_on_device, N, lines, lines_on_device, 4, g, q)) return rc;
+  k_gl_count<<<nb, 32 * GL_WARPS, 0, h->stream>>>(g, q, N, counts, block_sum);
+  LAUNCH_CHECK();
+  k_gl_scan<<<1, GL_SCAN_THREADS, 0, h->stream>>>(block_sum, nb, out->capacity, info);
+  LAUNCH_CHECK();
+  if (out_is_device) {
+    k_gl_values<<<nb, 32 * GL_WARPS, 0, h->stream>>>(g, q, N, counts, block_sum, info, first, out->rows);
+    LAUNCH_CHECK();
+    return EMAP_OK;
+  }
+  // host output: the total sizes the rows' staging, then the rows and the per-line words come back together
+  int64_t tc[2];
+  CK(cudaMemcpyAsync(tc, info, sizeof(tc), cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  const size_t row_doubles = tc[1] ? 3 * (size_t)tc[0] : 0;
+  if (int rc = grow(h, h->lookup.rows, row_doubles, 0, false)) return rc;
+  k_gl_values<<<nb, 32 * GL_WARPS, 0, h->stream>>>(g, q, N, counts, block_sum, info, first, h->lookup.rows);
+  LAUNCH_CHECK();
+  const size_t rows_off = (back_bytes + 255) & ~(size_t)255, total_bytes = rows_off + sizeof(double) * row_doubles;
+  if (h->lookup.down.size() < total_bytes) CK(h->lookup.down.alloc(total_bytes));
+  CK(cudaMemcpyAsync(h->lookup.down, (char*)info, back_bytes, cudaMemcpyDeviceToHost, h->stream));
+  if (row_doubles)
+    CK(cudaMemcpyAsync(h->lookup.down + rows_off, h->lookup.rows, sizeof(double) * row_doubles,
+                       cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  const char* d = h->lookup.down;
+  memcpy(out->info, d, 2 * sizeof(int64_t));
+  memcpy(out->first, d + ((char*)first - (char*)info), sizeof(int64_t) * N);
+  memcpy(out->counts, d + ((char*)counts - (char*)info), sizeof(int32_t) * N);
+  if (row_doubles) memcpy(out->rows, d + rows_off, sizeof(double) * row_doubles);
+  return EMAP_OK;
+}
+
+int emap_grid_derivatives(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, int64_t n_queries,
+                          const double* positions, int32_t positions_on_device, int32_t curvature,
+                          const emap_derivative_out* out, int32_t out_is_device) {
+  ENTER(h);
+  const char* e = !grid || !out ? "null argument"
+                                : check_lookup(grid, 5, n_queries, positions, out->index && out->value);
+  if (e) return fail(h, EMAP_ERR_INVALID, (std::string("emap_grid_derivatives: ") + e).c_str());
+  if (n_queries == 0) return EMAP_OK;
+  NvtxRange nv("grid_derivatives");
+  const int64_t N = n_queries;
+  const int nv_per = curvature ? 5 : 2;
+  const size_t vb = sizeof(double) * nv_per * N, ib = sizeof(int32_t) * 3 * N;
+  if (!out_is_device)
+    if (int rc = grow(h, h->lookup.block, vb + ib, 0, false)) return rc;
+  GlGrid g;
+  const double* q;
+  if (int rc = lookup_inputs(h, grid, grid_on_device, N, positions, positions_on_device, 2, g, q)) return rc;
+  double* value = out_is_device ? out->value : (double*)(char*)h->lookup.block;
+  int32_t* index = out_is_device ? out->index : (int32_t*)(h->lookup.block + vb);
+  k_gl_derivatives<<<cdiv(N, GL_THREADS), GL_THREADS, 0, h->stream>>>(g, gl_kernels(grid->resolution), q, N,
+                                                                      curvature ? 1 : 0, index, value);
+  LAUNCH_CHECK();
+  if (!out_is_device) {
+    if (int rc = lookup_back(h, vb + ib)) return rc;
+    memcpy(out->value, h->lookup.down, vb);
+    memcpy(out->index, h->lookup.down + vb, ib);
   }
   return EMAP_OK;
 }

@@ -123,6 +123,7 @@ class ElevationMap:
         self.initial_variance = param.initial_variance
         self.map_lock = threading.Lock()
         self._region_caps = (256, 1024, 16384)   # extract_planar_regions: the largest table counts seen (rows)
+        self._values_cap = 4096                  # values_between_locations: the largest total seen (rows)
         self.device = device
         self._L = _lib.load()
         self._h = C.c_void_p()
@@ -553,7 +554,8 @@ class ElevationMap:
         and the plane table stay on the device, and only the five info words are read back.  Returns a dict: "layers"
         maps elevation_raw, elevation, segmentation and plane_classification to (rows, cols) views; "planes" is an
         (n, 7) float64 array (label, support xyz, normal xyz); "highest_label", "origin" (the centre of window cell
-        (0, 0)), "resolution", "size" and "success" (False when the window is outside the map or has no finite cell;
+        (0, 0)), "centre" (the centre of the window's cells, as get_submaps returns it), "resolution", "size" and
+        "success" (False when the window is outside the map or has no finite cell;
         its layers are then not written)."""
         from .plane_segmentation import PlaneSegmentationParams
         p = (params or PlaneSegmentationParams()).to_c()
@@ -594,8 +596,8 @@ class ElevationMap:
         res = float(self.resolution)
         return {"layers": {name: flat[k * n:(k + 1) * n].reshape(rows, cols) for k, name in enumerate(names)},
                 "planes": planes[:int(info_h[4])], "highest_label": int(info_h[3]),
-                "origin": centre + (0.5 * (np.array([rows, cols]) * res) - 0.5 * res), "resolution": res,
-                "size": (rows, cols), "success": bool(info_h[0])}
+                "origin": centre + (0.5 * (np.array([rows, cols]) * res) - 0.5 * res), "centre": centre.copy(),
+                "resolution": res, "size": (rows, cols), "success": bool(info_h[0])}
 
     def extract_planar_regions(self, position, length, params=None, out=None, capacities=None):
         """The plane decomposition node's planar regions for the get_submap window around `position` (x, y) of `length`
@@ -706,6 +708,113 @@ class ElevationMap:
             res["convex_world"] = out["convex"][:, :, 2:]
         return res
 
+    def max_value_between_locations(self, grid, layer, starts, ends, out=None):
+        """The largest finite value of `layer` on each line from starts[i] to ends[i] (grid_map_filters_rsl's
+        maxValueBetweenLocations, quirks preserved), in one library call (emap_max_values_between; include/emap.h
+        states every step).  `grid`: a dict returned by segment_planes, extract_planar_regions, planar_terrain or
+        get_submap(s); `layer` names one of its layers, read in place (NumPy or torch CUDA).  `starts`, `ends`: (N, 2)
+        map-frame points, float64 NumPy or CUDA tensors.  `out`: None, or a dict of "index" (N, 3) int32 and "value"
+        (N, 3) float64, both NumPy or both torch CUDA, written in place.  Device queries or a device `out` keep
+        everything on the device.  Returns "valid", "value", "index" (N, 2: the LAST finite cell of the line, as the
+        reference returns) and "position" (N, 2: that cell's position); all views of `out`."""
+        g, g_dev, lines, n, device, mk, ptr = self._lookup_args(grid, layer, (starts, ends), 4, out, ("index",))
+        if out is None:
+            out = {"index": mk((n, 3), "int32"), "value": mk((n, 3), "float64")}
+        _check_out(out, {"index": (n, 3), "value": (n, 3)}, device)
+        o = _lib.EmapLineMaxOut(ptr(out["index"]), ptr(out["value"]))
+        self._lookup_call(self._L.emap_max_values_between, g, g_dev, n, lines, C.byref(o), device)
+        index, value = out["index"], out["value"]
+        return {"valid": index[:, 0] != 0, "value": value[:, 0], "index": index[:, 1:], "position": value[:, 1:]}
+
+    def values_between_locations(self, grid, layer, starts, ends, capacity=None):
+        """Every finite value of `layer` on each line from starts[i] to ends[i] with its cell's position
+        (grid_map_filters_rsl's valuesBetweenLocations), in one library call (emap_values_between; include/emap.h
+        states every step).  `grid`, `layer`, `starts` and `ends` as in max_value_between_locations; with device queries
+        or a device layer the results stay on the device.  `capacity`: the rows to start from (None: the largest total
+        this map has returned before).  When it is too small the call is repeated once with the exact total.  Returns
+        "rows" (total, 3: x, y, value), "counts" (N) and "first" (N: where line i's rows start), "retried"."""
+        g, g_dev, lines, n, device, mk, ptr = self._lookup_args(grid, layer, (starts, ends), 4, None, (), True)
+        cap = int(capacity if capacity is not None else self._values_cap)
+        counts, first, info = mk((n,), "int32"), mk((n,), "int64"), mk((2,), "int64")
+        for attempt in range(2):
+            rows = mk((max(cap, 1), 3), "float64")
+            o = _lib.EmapLineValuesOut(ptr(rows), cap, ptr(counts), ptr(first), ptr(info))
+            self._lookup_call(self._L.emap_values_between, g, g_dev, n, lines, C.byref(o), device)
+            info_h = info.cpu().numpy() if device else info
+            if info_h[1]:
+                break
+            cap = int(info_h[0])
+        self._values_cap = max(self._values_cap, int(info_h[0]))
+        return {"rows": rows[:int(info_h[0])], "counts": counts, "first": first, "retried": attempt > 0}
+
+    def grid_derivatives(self, grid, layer, positions, curvature=False, out=None):
+        """The gradient and, with `curvature`, the curvature of `layer` at each position (grid_map_filters_rsl's
+        GridMapDerivative::estimateGradient / estimateGradientAndCurvature at the position's cell), in one library call
+        (emap_grid_derivatives; include/emap.h states every step).  `grid` and `layer` as in max_value_between_locations
+        (at least 5 x 5 cells); `positions`: (N, 2) map-frame points.  `out`: None, or a dict of "index" (N, 3) int32
+        and "value" (N, 2 or 5) float64.  Returns "status" (0 inside, 1 outside: zero derivatives), "index" (N, 2),
+        "gradient" (N, 2: x, y) and, with curvature, "curvature" (N, 3: xx, xy, yy); all views of `out`."""
+        g, g_dev, pos, n, device, mk, ptr = self._lookup_args(grid, layer, (positions,), 2, out, ("index",))
+        nv = 5 if curvature else 2
+        if out is None:
+            out = {"index": mk((n, 3), "int32"), "value": mk((n, nv), "float64")}
+        _check_out(out, {"index": (n, 3), "value": (n, nv)}, device)
+        o = _lib.EmapDerivativeOut(ptr(out["index"]), ptr(out["value"]))
+        call = lambda *a: self._L.emap_grid_derivatives(*a[:6], int(bool(curvature)), *a[6:])  # noqa: E731
+        self._lookup_call(call, g, g_dev, n, pos, C.byref(o), device)
+        index, value = out["index"], out["value"]
+        res = {"status": index[:, 0], "index": index[:, 1:], "gradient": value[:, :2]}
+        if curvature:
+            res["curvature"] = value[:, 2:]
+        return res
+
+    def _lookup_args(self, grid, layer, parts, width, out, out_keys, follow_grid=False):
+        """What the three lookups share: the layer's emap_grid (the grid dict's "centre", its "resolution" or the map's),
+        the queries as one contiguous (N, width) float64 array (NumPy, or a CUDA tensor when any part is one), whether
+        the call writes device output (device queries, a device `out` or, with follow_grid, a device layer), and an
+        array maker and pointer getter for that side."""
+        data = grid["layers"][layer]
+        g_dev = _is_device(data)
+        if g_dev:
+            import torch
+            if data.dtype != torch.float32 or not data.is_contiguous():
+                raise TypeError("a device layer must be a contiguous float32 torch CUDA tensor")
+            d_ptr = data.data_ptr()
+        else:
+            data = np.ascontiguousarray(data, np.float32)
+            d_ptr = data.ctypes.data
+        rows, cols = (int(s) for s in data.shape)
+        res = float(grid.get("resolution", self.resolution))
+        centre = np.asarray(_to_host(grid["centre"]), np.float64)
+        g = _lib.EmapGrid(d_ptr, rows, cols, (C.c_double * 2)(*centre.tolist()), res)
+        g._keep = data
+        q_dev = any(_is_device(p) for p in parts)
+        out_dev = [out[k] for k in out_keys if _is_device(out[k])] if out is not None else []
+        device = q_dev or bool(out_dev) or (follow_grid and g_dev)
+        dev = None
+        if q_dev:
+            import torch
+            dev = next(p.device for p in parts if _is_device(p))
+            q = torch.cat([torch.as_tensor(p, device=dev).to(torch.float64).reshape(-1, width // len(parts))
+                           for p in parts], 1).contiguous()
+        else:
+            q = np.ascontiguousarray(np.concatenate([np.asarray(p, np.float64).reshape(-1, width // len(parts))
+                                                     for p in parts], 1))
+        n = int(q.shape[0])
+        if device and dev is None:
+            dev = out_dev[0].device if out_dev else data.device
+        mk, ptr = _array_maker(dev if device else None)
+        return g, g_dev, q, n, device, mk, ptr
+
+    def _lookup_call(self, fn, g, g_dev, n, queries, out, device):
+        q_dev = _is_device(queries)
+        q_ptr = queries.data_ptr() if q_dev else queries.ctypes.data
+        if device or g_dev or q_dev:
+            self._after_framework()
+        self._check(fn(self._h, C.byref(g), int(g_dev), n, q_ptr, int(q_dev), out, int(device)))
+        if device:
+            self._before_framework()
+
     def _planar_regions(self, position, length, params, out, capacities, post):
         """extract_planar_regions (post False) and planar_terrain (post True): the call with the capacity retry."""
         from .plane_segmentation import PlaneSegmentationParams
@@ -773,8 +882,8 @@ class ElevationMap:
         reg, poly, vert = tables[0][:nr], tables[1][:npoly], tables[2][:nv]
         result = {"layers": {name: flat[k * n:(k + 1) * n].reshape(rows, cols) for k, name in enumerate(names)},
                   "planes": planes[:int(info_h[4])], "highest_label": int(info_h[3]),
-                  "origin": centre + (0.5 * (np.array([rows, cols]) * res) - 0.5 * res), "resolution": res,
-                  "size": (rows, cols), "success": bool(info_h[0]), "complete": bool(info_h[8]),
+                  "origin": centre + (0.5 * (np.array([rows, cols]) * res) - 0.5 * res), "centre": centre.copy(),
+                  "resolution": res, "size": (rows, cols), "success": bool(info_h[0]), "complete": bool(info_h[8]),
                   "tables": {"regions": reg, "polygons": poly, "vertices": vert}, "regions": None,
                   "retried": attempt > 0}
         if not device and info_h[8]:
@@ -1067,6 +1176,25 @@ def regions_from_tables(regions, polygons, vertices):
         else:
             d["insets"][inset]["holes"].append(pts)
     return out
+
+
+def _array_maker(device):
+    """(make(shape, dtype name), pointer(array)) for new NumPy arrays (device None) or torch tensors on `device`."""
+    if device is None:
+        return (lambda shape, dt: np.zeros(shape, dt)), (lambda a: a.ctypes.data)
+    import torch
+    return (lambda shape, dt: torch.empty(shape, dtype=getattr(torch, dt), device=device)), (lambda a: a.data_ptr())
+
+
+def _check_out(out, shapes, device):
+    """Every out[k] is a contiguous array of shapes[k] on the call's side (NumPy for host output, CUDA for device)."""
+    dtypes = {"index": "int32", "value": "float64"}
+    for k, shape in shapes.items():
+        a = out[k]
+        if tuple(a.shape) != shape or _is_device(a) != device or str(a.dtype).split(".")[-1] != dtypes[k] or not (
+                a.is_contiguous() if device else a.flags.c_contiguous):
+            raise TypeError("out[%r] must be a contiguous %s %s array of shape %s" % (
+                k, dtypes[k], "CUDA" if device else "NumPy", shape))
 
 
 def _is_device(x):

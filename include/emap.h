@@ -654,6 +654,103 @@ int emap_project_to_planar_regions(emap_handle* h, const emap_region_tables* tab
                                    int64_t n_queries, const double* queries, int32_t queries_on_device,
                                    double penalty_z_weight, int32_t n_convex, double growth_factor,
                                    const emap_projection_out* out, int32_t out_is_device);
+/* ---- lookups along lines and derivatives at points on one grid layer: grid_map_filters_rsl's lookup.cpp
+ * (maxValueBetweenLocations, valuesBetweenLocations, projectToMapWithMargin) and GridMapDerivative.cpp
+ * (estimateGradient, estimateGradientAndCurvature), for a batch of queries on the device.  DESIGN.md §4l gives the
+ * restatement.  The handle's map state is not read or changed; the calls use the handle's stream, staging and scratch.
+ * Grid (emap_grid): one fp32 layer of rows x cols cells, row-major, grid_map index (r, c) at r * cols + c (row 0 the +x
+ * edge, column 0 the +y edge, as every window of this library), in host (grid_on_device 0) or device memory; grid_map
+ * geometry position = `position` (the centre of the cells: emap_submap_windows' centre), length L = (rows, cols) *
+ * resolution, buffer start index 0.  Index and position arithmetic, restated from grid_map's published GridMapMath.cpp
+ * (not checked against a grid_map build), per axis with p the position and o = 0.5 L: a point v is inside when
+ * 0 <= -((v - p) - o) < L (checkIfPositionWithinMap), its index is trunc(-(((v - o) - p) / resolution)) clamped to
+ * [0, n - 1] (getIndexFromPosition; the same code as emap_get_transformed_submaps'), and index i is at
+ * (p + (0.5 L - 0.5 resolution)) - resolution * i (getPositionFromIndex).
+ * Lines: queries are n_queries (x0, y0, x1, y1) doubles in the map frame, host or device.  Per line:
+ *  Ends: projectToMapWithMargin with the default margin: m = min(1e-6, L.x / 2, L.y / 2), each coordinate
+ *    fmax(fmin(v, (p + 0.5 L) - m), (p - 0.5 L) + m).  A NaN coordinate lands on the upper bound (fmin returns the other
+ *    operand), +-inf on its bound.  For an accepted grid (|p| + L <= EMAP_GRID_MAX_EXTENT and resolution >=
+ *    EMAP_GRID_MIN_RESOLUTION per axis) a projected end is always inside: every intermediate lies below 2^20 in
+ *    magnitude, so each of the four roundings between the bound and the inside test is off by at most 2^-33, while
+ *    m >= min(1e-6, 2^-21) keeps the exact value at least 4.7e-7 inside.  So LineIterator's getIndexLimitedToMapRange
+ *    never steps and its ends are the getIndex cells of the projected ends (tests/test_grid_lookup_cpu.py checks this
+ *    at the bounds, edges and corners of extreme grids).
+ *  Walk: grid_map's LineIterator (LineIterator.cpp, restated from grid_map's published source, not checked against a
+ *    grid_map build): Bresenham from the start cell to the end cell; d = |end - start| per axis, each axis steps +1 when
+ *    end >= start, else -1; the major axis is the rows when d.rows >= d.cols; den = d.major, numerator = den / 2, add =
+ *    d.minor, den + 1 cells; each step adds `add` to the numerator and, when it is >= den, subtracts den and steps the
+ *    minor axis; it always steps the major axis.  Cell i is computed directly: major start + i, minor start +
+ *    floor((den / 2 + i add) / den) steps (64-bit; the start cell alone when den is 0).
+ *  emap_max_values_between (maxValueBetweenLocations), quirks preserved: value = std::max(value, v) from -FLT_MAX over
+ *    the finite cells in order, so on equal values the first is kept (the sign of a largest zero is that of the first
+ *    such zero); valid = value > -FLT_MAX (a line whose only finite values are -FLT_MAX is invalid); the returned cell is
+ *    the LAST finite cell of the line, not the maximum's (maxIndex is set at every finite cell), and (0, 0) when there
+ *    is none; x, y its position.  Outputs (emap_line_max_out): index, 3 int32 per line {valid, row, col}; value, 3
+ *    doubles {value (the float widened), x, y}.
+ *  emap_values_between (valuesBetweenLocations): (x, y, value) per finite cell, in iterator order, value the float
+ *    widened.  Outputs (emap_line_values_out): counts (int32 per line: its rows), first (int64 per line: the exclusive
+ *    prefix sum of the counts, where its rows start) and info = {total rows, complete} are always written; rows
+ *    (3 doubles per row) only when total <= capacity (complete = 1), decided on the device; otherwise nothing is
+ *    written to rows.  Host output reads the total back first (one synchronisation), so the rows' staging is sized
+ *    by the total, not the capacity; the rows and the per-line words then come back together (a second one).
+ * Derivatives (emap_grid_derivatives): positions are n_queries (x, y) doubles, host or device.  Per position, its
+ *  index (r, c) as above; outside the map: status EMAP_DERIVATIVE_OUTSIDE, row = col = -1, zero gradient and curvature
+ *  (as GridMapDerivative.hpp documents).  Inside: the kernels d1 = float(-1/12, 2/3, 0, -2/3, 1/12) / float(resolution)
+ *  and d2 = float(-1/12, 4/3, -5/2, 4/3, -1/12) / (float(resolution) * float(resolution)), each literal a double rounded
+ *  to float, the divisions in float; getKernelCenter's taps rows r0 .. r0 + 4 with r0 = r - 2 - min(r - 2, 0) -
+ *  max(r + 2 - (rows - 1), 0), columns c0 .. c0 + 4 likewise (an edge cell gets an off-centre stencil); H(a, b) the
+ *  layer.  gx = d1 . H(r0.., c), gy = d1 . H(r, c0..), cxx = d2 . H(r0.., c), cyy = d2 . H(r, c0..), cxy = d1 . g with
+ *  g_j = d1 . H(r0.., c0 + j).  Every product and sum is in float without contraction, widened to double at the end (a NaN as the quiet NaN
+ *  0x7ff8000000000000, whatever its payload in float).
+ *  Eigen's sum orders (restated from Eigen's published source for an SSE build without FMA, not checked against an
+ *  Eigen build): a contiguous 5-vector (a column block of the column-major matrix, and g) sums
+ *  ((p0 + p2) + (p1 + p3)) + p4; a strided one (a row block) (p0 + p1) + (p2 + (p3 + p4)).  Outputs
+ *  (emap_derivative_out): index, 3 int32 per position {status, row, col}; value, 2 doubles {gx, gy}, or with
+ *  curvature != 0 5 doubles {gx, gy, cxx, cxy, cyy}.
+ * Host grids and queries are staged and uploaded in one copy.  Host output comes back in one copy and synchronisation
+ * (emap_values_between: two); device output (every output pointer device memory) is stream-ordered with no host
+ * synchronisation and can be captured into a CUDA graph (with a device grid and queries; capture after an eager call of
+ * the largest size: growing the scratch synchronises).  Kernels: none for n_queries = 0 (emap_values_between then
+ * writes info = {0, 1}); else emap_max_values_between 1 (one warp per line), emap_values_between 3 (count, scan,
+ * write; one warp per line), emap_grid_derivatives 1 (one thread per position).
+ * EMAP_ERR_INVALID, with nothing written or launched: a NULL grid, out or grid data; rows or cols below 1 (below 5 for
+ * emap_grid_derivatives, where the reference's stencil would read outside the layer); rows * cols >= 2^31; a
+ * resolution that is not finite or below EMAP_GRID_MIN_RESOLUTION; a position that is not finite; |position| + length
+ * above EMAP_GRID_MAX_EXTENT on an axis; n_queries below 0 or above 2^31 - 1; NULL queries or outputs with
+ * n_queries > 0; for emap_values_between a NULL info, a capacity below 0 and NULL rows with a capacity above 0. */
+typedef struct emap_grid {
+  const float* data;       /* rows x cols, row-major */
+  int64_t rows, cols;
+  double position[2];      /* the centre of the cells, map frame [m] */
+  double resolution;       /* [m] */
+} emap_grid;
+typedef struct emap_line_max_out {
+  int32_t* index;          /* 3 per line: valid, row, col */
+  double* value;           /* 3 per line: value, x, y */
+} emap_line_max_out;
+typedef struct emap_line_values_out {
+  double* rows;            /* 3 per row: x, y, value */
+  int64_t capacity;        /* rows */
+  int32_t* counts;         /* 1 per line */
+  int64_t* first;          /* 1 per line */
+  int64_t* info;           /* {total rows, complete} */
+} emap_line_values_out;
+typedef struct emap_derivative_out {
+  int32_t* index;          /* 3 per position: status, row, col */
+  double* value;           /* 2 per position (gx, gy), or 5 with curvature (gx, gy, cxx, cxy, cyy) */
+} emap_derivative_out;
+#define EMAP_GRID_MAX_EXTENT 1048576.0              /* 2^20 m */
+#define EMAP_GRID_MIN_RESOLUTION 9.5367431640625e-07 /* 2^-20 m */
+enum { EMAP_DERIVATIVE_INSIDE = 0, EMAP_DERIVATIVE_OUTSIDE = 1 };
+int emap_max_values_between(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, int64_t n_queries,
+                            const double* lines, int32_t lines_on_device, const emap_line_max_out* out,
+                            int32_t out_is_device);
+int emap_values_between(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, int64_t n_queries,
+                        const double* lines, int32_t lines_on_device, const emap_line_values_out* out,
+                        int32_t out_is_device);
+int emap_grid_derivatives(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, int64_t n_queries,
+                          const double* positions, int32_t positions_on_device, int32_t curvature,
+                          const emap_derivative_out* out, int32_t out_is_device);
 /* ---- the exported map as a point cloud and as normal arrows: the ROS node's publishAsPointCloud
  * (elevation_mapping_ros.cpp:501-505, grid_map's toPointCloud(map, {"elevation"}, "elevation")) and publishNormalAsArrow
  * (:751-778), restated from grid_map's published source (not checked against a grid_map build).  Coordinates are those of
