@@ -176,6 +176,10 @@ SIGNATURES = {
                                       C.POINTER(EmapLineValuesOut), C.c_int32]),
     "emap_grid_derivatives": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
                                         C.c_int32, C.POINTER(EmapDerivativeOut), C.c_int32]),
+    "emap_plane_grid_geometry": (C.c_int, [C.c_int64, C.c_int64, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "emap_plane_decomposition": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_void_p, C.c_void_p,
+                                           C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int64,
+                                           C.c_void_p, C.c_void_p]),
     "emap_get_map_points": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_get_normal_arrows": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "emap_layer_device_ptr": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(C.c_void_p)]),

@@ -7,6 +7,8 @@
 #include "emap_planes.cuh"
 #include "emap_regions.cuh"
 #include "emap_postprocess.cuh"
+#include "emap_resample.cuh"
+#include "emap_grid.cuh"
 #include "emap_mapcloud.cuh"
 
 namespace {
@@ -353,6 +355,8 @@ int emap_get_transformed_submaps(emap_handle* h, int32_t n_windows, const double
 // the label statistics and decisions, and the host output's staging (info, plane table, layers, then `extra` bytes
 // that emap_extract_planar_regions stages its tables in).  With the post-processing (emap_planar_terrain) the block
 // also holds its three fp32 planes and the box filter's double row sums, and the staging all EMAP_TERRAIN_LAYERS layers.
+// n is the larger of the input and the resampled grid (emap_plane_decomposition), n_out the resampled one the staged
+// layers have; a window is not resampled (n == n_out).
 namespace {
 
 struct PlaneScratch {
@@ -369,8 +373,8 @@ struct PlaneScratch {
   char* extra;
 };
 
-size_t carve_planes(int64_t n, int64_t slots, int64_t plane_rows, bool host_out, bool post, size_t extra, void* base,
-                    PlaneScratch& s) {
+size_t carve_planes(int64_t n, int64_t n_out, int64_t slots, int64_t plane_rows, bool host_out, bool post,
+                    size_t extra, void* base, PlaneScratch& s) {
   Carver c{(uintptr_t)base};
   const int64_t m = std::max(n, slots);
   s.raw = c.take<float>(n); s.img[0] = c.take<float>(n); s.img[1] = c.take<float>(n);
@@ -383,7 +387,7 @@ size_t carve_planes(int64_t n, int64_t slots, int64_t plane_rows, bool host_out,
   s.pd = c.take<double>(post ? n : 0);
   s.info = c.take<int32_t>(host_out ? 16 : 0);
   s.planes = c.take<double>(host_out ? 7 * plane_rows : 0);
-  s.layers = c.take<float>(host_out ? (post ? EMAP_TERRAIN_LAYERS : 4) * n : 0);
+  s.layers = c.take<float>(host_out ? (post ? EMAP_TERRAIN_LAYERS : 4) * n_out : 0);
   s.extra = c.take<char>(host_out ? extra : 0);
   return c.bytes;
 }
@@ -415,12 +419,18 @@ int plane_components(emap_handle* h, const PlaneScratch& s, int rows, int cols, 
   return 0;
 }
 
-// One segmentation call's window and scratch, as plane_check and segment_window leave them.
+// One segmentation call's grid and scratch, as plane_check (a window) or grid_plane_check (a caller's grid) and
+// segment_window leave them.  The pipeline runs on rows x cols cells of resolution res from the fill's output on: the
+// input's in_rows x in_cols resampled, or the input itself.
 struct PlaneCall {
-  int32_t q[5];                    // submap_window: {success, r0, c0, rows, cols}
-  double centre[2];
-  int rows = 0, cols = 0;
-  int64_t n = 0, slots = 0, plane_rows = 0;
+  int32_t q[5];                    // submap_window: {success, r0, c0, rows, cols}; a grid: {1, 0, 0, in_rows, in_cols}
+  double centre[2];                // the centre of the cells (kept by the resampling)
+  const float* grid = nullptr;     // the caller's grid (emap_plane_decomposition), else the window by k_submap
+  bool grid_on_device = false;
+  int in_rows = 0, in_cols = 0;    // the input
+  int rows = 0, cols = 0;          // the pipeline's grid
+  double res = 0.0;
+  int64_t n = 0, n_in = 0, slots = 0, plane_rows = 0;
   bool post = false;               // emap_planar_terrain: the post-processing's scratch and layers
   double ox = 0.0, oy = 0.0;       // the centre of window cell (0, 0)
   PlaneScratch s;
@@ -433,14 +443,15 @@ struct PlaneCall {
 
 static_assert(EMAP_PLANE_EIGEN_MIN == PL_EIG_MIN, "emap.h states the fit's threshold");
 
-// Why p is rejected (nullptr: accepted) for a map of resolution `res`.
-static const char* plane_params_error(const emap_plane_params& p, double res) {
+// Why p is rejected (nullptr: accepted) for a map of resolution `res`; a resampling only when `resample` is false.
+static const char* plane_params_error(const emap_plane_params& p, double res, bool resample) {
   if (p.ransac) return "RANSAC refinement is not supported (ransac must be 0)";
   const int mk = std::max(1, std::min(p.median_kernel, 5));
   if (mk != 1 && mk != 3 && mk != 5) return "the median kernel must clamp to 1, 3 or 5";
   if (p.median_repeats < 0 || p.median_repeats > EMAP_PLANE_MAX_REPEATS)
     return "median_repeats must be in [0, EMAP_PLANE_MAX_REPEATS]";
-  if (std::isnan(p.resolution) || (p.resolution > 0.0 && !(std::fabs(res - p.resolution) < 1e-6)))
+  if (std::isnan(p.resolution)) return "resolution must not be NaN";
+  if (!resample && p.resolution > 0.0 && !(std::fabs(res - p.resolution) < 1e-6))
     return "resampling is not supported (resolution must be <= 0 or the map's)";
   if (p.kernel_size < 3 || p.kernel_size % 2 == 0 || p.kernel_size > EMAP_PLANE_MAX_KERNEL)
     return "kernel_size must be odd, >= 3 and <= EMAP_PLANE_MAX_KERNEL";
@@ -470,12 +481,13 @@ static const char* plane_check(emap_handle* h, const double window[4], const ema
                                int64_t planes_capacity, PlaneCall& c) {
   if (!submap_lengths_ok(1, window)) return "lengths must be finite and >= 0";
   const double res = h->cfg.resolution;
-  if (const char* e = plane_params_error(p, res)) return e;
+  if (const char* e = plane_params_error(p, res, false)) return e;
   const double m[2] = {h->center[0], h->center[1]};
   submap_window(h->dc.W, res, m, window, c.q, c.centre);
-  c.rows = c.q[3];
-  c.cols = c.q[4];
-  c.n = (int64_t)c.rows * c.cols;
+  c.rows = c.in_rows = c.q[3];
+  c.cols = c.in_cols = c.q[4];
+  c.res = res;
+  c.n = c.n_in = (int64_t)c.rows * c.cols;
   if (c.q[0] && out_floats < 4 * c.n) return "out_floats is below 4 * rows * cols";
   c.plane_rows = emap_plane_capacity(c.rows, c.cols, &p);
   if (c.q[0] && planes_capacity < c.plane_rows)
@@ -483,24 +495,59 @@ static const char* plane_check(emap_handle* h, const double window[4], const ema
   return nullptr;
 }
 
-// The segmentation of a window that plane_check accepted and found inside the map (ConvexPlaneDecompositionRos.cpp:
-// 115-149 up to SlidingWindowPlaneExtractor, without RANSAC): the window by k_submap, then the passes of
-// csrc/emap_planes.cuh, queued on the handle's stream.  With host output the layers, plane table and info go to the
-// staging at the scratch's tail, which also holds `extra` bytes for the caller (c.s.extra).
-static int segment_window(emap_handle* h, const double window[4], const emap_plane_params& p, bool out_is_device,
-                          float* layers_out, double* planes_out, int32_t* info, size_t extra, PlaneCall& c) {
+// The largest grid side emap_plane_decomposition takes, before and after the resampling: the largest window (cell_n <=
+// 2049 exports at most 2047 rows), so its scratch never exceeds the window calls'.
+constexpr int64_t kPlaneGridMax = 2047;
+
+// emap_plane_decomposition's checks of the grid and its resampling, before anything is written or launched, and the
+// call's geometry (c.q, c.centre, c.in_rows / c.in_cols, c.rows / c.cols the resampled size, c.res, c.n, c.n_in,
+// c.plane_rows).  Returns the error's message, or nullptr.
+static const char* grid_plane_check(const emap_grid& g, int32_t grid_on_device, const emap_plane_params& p,
+                                    int64_t out_floats, int64_t planes_capacity, PlaneCall& c) {
+  if (const char* e = gl_check_grid(g.data, g.rows, g.cols, g.position, g.resolution, 1)) return e;
+  if (g.rows > kPlaneGridMax || g.cols > kPlaneGridMax) return "the grid has more than 2047 rows or columns";
+  if (const char* e = plane_params_error(p, g.resolution, true)) return e;
+  int64_t size[2];
+  rs_geometry(g.rows, g.cols, g.resolution, p.resolution, size, &c.res);
+  if (!size[0] || !size[1]) return "the resampled grid has no rows or no columns";
+  if (size[0] > kPlaneGridMax || size[1] > kPlaneGridMax) return "the resampled grid has more than 2047 rows or columns";
+  c.grid = g.data;
+  c.grid_on_device = grid_on_device != 0;
+  c.in_rows = (int)g.rows;
+  c.in_cols = (int)g.cols;
+  c.rows = (int)size[0];
+  c.cols = (int)size[1];
+  c.q[0] = 1; c.q[1] = c.q[2] = 0; c.q[3] = c.in_rows; c.q[4] = c.in_cols;
+  c.centre[0] = g.position[0];
+  c.centre[1] = g.position[1];
+  c.n_in = g.rows * g.cols;
+  c.n = (int64_t)c.rows * c.cols;
+  c.plane_rows = emap_plane_capacity(c.rows, c.cols, &p);
+  if (out_floats < EMAP_TERRAIN_LAYERS * c.n) return "out_floats is below EMAP_TERRAIN_LAYERS * rows * cols (resampled)";
+  if (planes_capacity < c.plane_rows) return "planes_capacity is below emap_plane_capacity() of the resampled grid";
+  return nullptr;
+}
+
+// The segmentation of a window that plane_check accepted and found inside the map, or of a grid that grid_plane_check
+// accepted (ConvexPlaneDecompositionRos.cpp:115-149 up to SlidingWindowPlaneExtractor, without RANSAC): the window by
+// k_submap or the grid copied in, the fill and the median on the input, the resampling when the sizes differ
+// (csrc/emap_resample.cuh), then the passes of csrc/emap_planes.cuh on the pipeline's grid, queued on the handle's
+// stream.  With host output the layers, plane table and info go to the staging at the scratch's tail, which also holds
+// `extra` bytes for the caller (c.s.extra).  Layer 0 is the input; a grid's is not written (it is the caller's).
+static int segment_window(emap_handle* h, const emap_plane_params& p, bool out_is_device, float* layers_out,
+                          double* planes_out, int32_t* info, size_t extra, PlaneCall& c) {
   const int rows = c.rows, cols = c.cols;
-  const int64_t n = c.n;
-  const double res = h->cfg.resolution;
+  const int64_t n = c.n, n_in = c.n_in, n_scratch = std::max(n, n_in);
+  const double res = c.res;
   // labels are at most ceil(n / 2) (a 4-connected checkerboard), plus 0.  The statistics are sized and zeroed for that
   // worst case (128 bytes a slot) because the label count is known only on the device.
   c.slots = n / 2 + 2;
   const int64_t slots = c.slots;
   PlaneScratch& s = c.s;
-  int rc = grow(h, h->planes.block, carve_planes(n, slots, c.plane_rows, !out_is_device, c.post, extra, nullptr, s), 0,
-                false);
+  int rc = grow(h, h->planes.block,
+                carve_planes(n_scratch, n, slots, c.plane_rows, !out_is_device, c.post, extra, nullptr, s), 0, false);
   if (rc) return rc;
-  c.used = carve_planes(n, slots, c.plane_rows, !out_is_device, c.post, extra, h->planes.block, s);
+  c.used = carve_planes(n_scratch, n, slots, c.plane_rows, !out_is_device, c.post, extra, h->planes.block, s);
   if (!out_is_device) {
     // the pinned staging of the copy back, allocated before anything is launched
     const size_t bytes = c.used - (size_t)((char*)s.info - (char*)h->planes.block);
@@ -509,36 +556,52 @@ static int segment_window(emap_handle* h, const double window[4], const emap_pla
   float* dst = out_is_device ? layers_out : s.layers;
   c.dst_planes = out_is_device ? planes_out : s.planes;
   c.dst_info = out_is_device ? info : s.info;
-  // the window: k_submap's elevation layer into s.raw
-  SubmapArgs a;
-  const char* elevation = "elevation";
-  if (!export_list(h, 1, &elevation, nullptr, nullptr, a.L)) return EMAP_ERR_CUDA;
-  a.n_win = 0;
-  int tiles = 0;
-  long long total = 0;
-  submap_add(a, h->dc.W, c.q, 1, tiles, total);
-  k_submap<false><<<dim3(tiles, 1), dim3(32, SUBMAP_ROWS), 0, h->stream>>>(h->dc, h->map, h->normal, s.raw, a, h->center[2],
-                                                                           h->cfg.use_only_above_for_upper_bound);
-  LAUNCH_CHECK();
+  if (c.grid) {
+    // the caller's grid into s.raw: one copy (a host grid is staged by the driver before the call returns)
+    CK(cudaMemcpyAsync(s.raw, c.grid, sizeof(float) * n_in,
+                       c.grid_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
+  } else {
+    // the window: k_submap's elevation layer into s.raw
+    SubmapArgs a;
+    const char* elevation = "elevation";
+    if (!export_list(h, 1, &elevation, nullptr, nullptr, a.L)) return EMAP_ERR_CUDA;
+    a.n_win = 0;
+    int tiles = 0;
+    long long total = 0;
+    submap_add(a, h->dc.W, c.q, 1, tiles, total);
+    k_submap<false><<<dim3(tiles, 1), dim3(32, SUBMAP_ROWS), 0, h->stream>>>(h->dc, h->map, h->normal, s.raw, a,
+                                                                             h->center[2],
+                                                                             h->cfg.use_only_above_for_upper_bound);
+    LAUNCH_CHECK();
+  }
   CK(cudaMemsetAsync(s.hdr, 0, 8 * sizeof(int), h->stream));
   CK(cudaMemsetAsync(s.st, 0, sizeof(unsigned long long) * slots * PL_STAT, h->stream));
-  const int cb = cdiv(n, PL_THREADS);
-  // fill: minValues' fixed point per NaN component
-  k_pl_fill_init<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, s.hdr, (int)n);
+  // fill: minValues' fixed point per NaN component, on the input
+  const int ib = cdiv(n_in, PL_THREADS);
+  k_pl_fill_init<<<ib, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, s.hdr, (int)n_in);
   LAUNCH_CHECK();
-  if ((rc = plane_components(h, s, rows, cols, 0))) return rc;
-  k_pl_fill_min<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, rows, cols);
+  if ((rc = plane_components(h, s, c.in_rows, c.in_cols, 0))) return rc;
+  k_pl_fill_min<<<ib, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, c.in_rows, c.in_cols);
   LAUNCH_CHECK();
-  k_pl_fill_write<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, s.img[0], (int)n);
+  k_pl_fill_write<<<ib, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, s.img[0], (int)n_in);
   LAUNCH_CHECK();
   // median, numberOfRepeats times
   const int mk = std::max(1, std::min(p.median_kernel, 5));
   int cur = 0;
   if (mk > 1)
     for (int r = 0; r < p.median_repeats; r++, cur ^= 1) {
-      (mk == 3 ? k_pl_median<3> : k_pl_median<5>)<<<cb, PL_THREADS, 0, h->stream>>>(s.img[cur], s.img[cur ^ 1], rows, cols);
+      (mk == 3 ? k_pl_median<3> : k_pl_median<5>)<<<ib, PL_THREADS, 0, h->stream>>>(s.img[cur], s.img[cur ^ 1],
+                                                                                    c.in_rows, c.in_cols);
       LAUNCH_CHECK();
     }
+  // changeResolution: inpainting::resample to the pipeline's grid
+  if (rows != c.in_rows || cols != c.in_cols) {
+    k_rs_resample<<<cdiv(n, RS_THREADS), RS_THREADS, 0, h->stream>>>(s.img[cur], c.in_rows, c.in_cols, s.img[cur ^ 1],
+                                                                     rows, cols);
+    LAUNCH_CHECK();
+    cur ^= 1;
+  }
+  const int cb = cdiv(n, PL_THREADS);
   const float* img = s.img[cur];
   // sliding-window planarity, opening, labels
   k_pl_fit<<<cb, PL_THREADS, 0, h->stream>>>(img, s.bin, rows, cols, p.kernel_size, res, p.patch_error * p.patch_error,
@@ -573,7 +636,8 @@ static int segment_window(emap_handle* h, const double window[4], const emap_pla
   if ((rc = plane_scan(h, s, slots, s.hdr + 2))) return rc;
   k_pl_planes<<<cdiv(slots, PL_THREADS), PL_THREADS, 0, h->stream>>>(s.st, s.rank, s.hdr, c.dst_planes, (int)slots, la);
   LAUNCH_CHECK();
-  k_pl_out<<<cb, PL_THREADS, 0, h->stream>>>(s.raw, img, s.lab, s.bg, s.hdr, dst, c.dst_info, rows, cols);
+  k_pl_out<<<cb, PL_THREADS, 0, h->stream>>>(c.grid ? nullptr : s.raw, img, s.lab, s.bg, s.hdr, dst, c.dst_info, rows,
+                                             cols);
   LAUNCH_CHECK();
   return 0;
 }
@@ -587,11 +651,12 @@ static int plane_copy_back(emap_handle* h, PlaneCall& c, float* layers_out, doub
   if (h->planes.host.size() < bytes) CK(h->planes.host.alloc(bytes));
   CK(cudaMemcpyAsync(h->planes.host, c.s.info, bytes, cudaMemcpyDeviceToHost, h->stream));
   CK(cudaStreamSynchronize(h->stream));
-  carve_planes(c.n, c.slots, c.plane_rows, true, c.post, bytes, (char*)h->planes.host - off, t);
+  carve_planes(std::max(c.n, c.n_in), c.n, c.slots, c.plane_rows, true, c.post, bytes, (char*)h->planes.host - off, t);
   memcpy(info, t.info, n_info * sizeof(int32_t));
   if (info[0]) {
     memcpy(planes_out, t.planes, sizeof(double) * 7 * info[4]);
-    memcpy(layers_out, t.layers, sizeof(float) * (c.post ? EMAP_TERRAIN_LAYERS : 4) * c.n);
+    const int64_t skip = c.grid ? c.n : 0;      // a grid's layer 0 is the caller's
+    memcpy(layers_out + skip, t.layers + skip, sizeof(float) * ((c.post ? EMAP_TERRAIN_LAYERS : 4) * c.n - skip));
   }
   return 0;
 }
@@ -615,7 +680,7 @@ int emap_segment_planes(emap_handle* h, const double window[4], const emap_plane
     else memset(info, 0, 5 * sizeof(int32_t));
     return EMAP_OK;
   }
-  int rc = segment_window(h, window, p, out_is_device, layers_out, planes_out, info, 0, c);
+  int rc = segment_window(h, p, out_is_device, layers_out, planes_out, info, 0, c);
   if (rc) return rc;
   PlaneScratch t;
   if (!out_is_device && (rc = plane_copy_back(h, c, layers_out, planes_out, info, 5, t))) return rc;
@@ -718,7 +783,7 @@ static int postprocess_window(emap_handle* h, PlaneCall& c, const emap_postproce
   LAUNCH_CHECK();
   k_pp_morph<false><<<cb, PL_THREADS, 0, h->stream>>>(t, L[6], nullptr, s.hdr, rows, cols, ec);
   LAUNCH_CHECK();
-  k_pp_slope<<<cb, PL_THREADS, 0, h->stream>>>(L[6], L[7], s.hdr, rows, cols, pc.dil, (float)h->cfg.resolution);
+  k_pp_slope<<<cb, PL_THREADS, 0, h->stream>>>(L[6], L[7], s.hdr, rows, cols, pc.dil, (float)c.res);
   LAUNCH_CHECK();
   // smooth_planar: boxFilter, then GaussianBlur (rows, then columns)
   k_pp_box_rows<<<cb, PL_THREADS, 0, h->stream>>>(L[7], s.pd, s.hdr, rows, cols, pc.box / 2);
@@ -744,11 +809,13 @@ static int postprocess_window(emap_handle* h, PlaneCall& c, const emap_postproce
   return 0;
 }
 
-// ContourExtraction::extractPlanarRegions and addHeightOffset after segment_window (both entry points), then, with
-// post != nullptr, Postprocessing::postprocess's map passes (emap_planar_terrain): see include/emap.h and DESIGN.md
-// §4l.  Every check runs before anything is written or launched; the launches depend on the parameters and the window
-// size only.  fn names the entry point in the messages.
-static int planar_regions(emap_handle* h, const char* fn, const double window[4], const emap_plane_params& p,
+// ContourExtraction::extractPlanarRegions and addHeightOffset after segment_window (the window entry points with
+// `window`, emap_plane_decomposition with `grid`), then, with post != nullptr, Postprocessing::postprocess's map passes
+// (emap_planar_terrain, emap_plane_decomposition): see include/emap.h and DESIGN.md §4l.  Every check runs before
+// anything is written or launched; the launches depend on the parameters and the grid sizes only.  fn names the entry
+// point in the messages.
+static int planar_regions(emap_handle* h, const char* fn, const double* window, const emap_grid* grid,
+                          int32_t grid_on_device, const emap_plane_params& p,
                           const emap_region_params& rp, const emap_postprocess_params* post, float* layers_out,
                           int32_t out_is_device, int64_t out_floats, double* planes_out, int64_t planes_capacity,
                           const emap_region_out& o, int32_t* info) {
@@ -763,14 +830,17 @@ static int planar_regions(emap_handle* h, const char* fn, const double window[4]
       (o.vertices_capacity && !o.vertices))
     return fail_in(h, fn, "a table capacity is negative or a table with a capacity is null");
   PlaneCall c;
-  if (const char* e = plane_check(h, window, p, out_floats, planes_capacity, c)) return fail_in(h, fn, e);
+  if (const char* e = grid ? grid_plane_check(*grid, grid_on_device, p, out_floats, planes_capacity, c)
+                           : plane_check(h, window, p, out_floats, planes_capacity, c))
+    return fail_in(h, fn, e);
   PostCall pc;
   if (post) {
-    if (const char* e = post_params_error(*post, h->cfg.resolution, rp.plane_height_offset, pc)) return fail_in(h, fn, e);
+    if (const char* e = post_params_error(*post, c.res, rp.plane_height_offset, pc)) return fail_in(h, fn, e);
     if (c.q[0] && out_floats < EMAP_TERRAIN_LAYERS * c.n)
       return fail_in(h, fn, "out_floats is below EMAP_TERRAIN_LAYERS * rows * cols");
     if (c.q[0] && (c.rows < pc.dil || c.cols < pc.dil))
-      return fail_in(h, fn, "the window has fewer rows or columns than the smoothing's dilation kernel");
+      return fail_in(h, fn, grid ? "the resampled grid has fewer rows or columns than the smoothing's dilation kernel"
+                                 : "the window has fewer rows or columns than the smoothing's dilation kernel");
     c.post = true;
   }
   if (!c.q[0]) {
@@ -787,7 +857,7 @@ static int planar_regions(emap_handle* h, const char* fn, const double window[4]
   const size_t rb = sizeof(double) * RG_ROW * o.regions_capacity, pb = sizeof(int32_t) * RG_POLY * o.polygons_capacity,
                vb = sizeof(double) * 2 * o.vertices_capacity;
   const size_t extra = regions ? ((rb + 255) & ~size_t(255)) + ((pb + 255) & ~size_t(255)) + vb : 0;
-  int rc = segment_window(h, window, p, out_is_device, layers_out, planes_out, info, extra, c);
+  int rc = segment_window(h, p, out_is_device, layers_out, planes_out, info, extra, c);
   if (rc) return rc;
   PlaneScratch& s = c.s;
   char* stage = s.extra;
@@ -798,7 +868,7 @@ static int planar_regions(emap_handle* h, const char* fn, const double window[4]
   ro.planes = c.dst_planes;
   ro.ox = c.ox;
   ro.oy = c.oy;
-  ro.res3 = h->cfg.resolution / 3.0;
+  ro.res3 = c.res / 3.0;
   ro.offset = rp.plane_height_offset;
   if (!regions) {
     k_rg_none<<<1, 1, 0, h->stream>>>(c.dst_info, 5);   // upSample needs 2 x 2 cells: no region
@@ -887,8 +957,8 @@ int emap_extract_planar_regions(emap_handle* h, const double window[4], const em
   NvtxRange nv("emap:extract_planar_regions");
   if (!window || !plane_params || !region_params || !layers_out || !planes_out || !regions_out || !info)
     return fail(h, EMAP_ERR_INVALID, "emap_extract_planar_regions: null argument");
-  return planar_regions(h, "emap_extract_planar_regions", window, *plane_params, *region_params, nullptr, layers_out,
-                        out_is_device, out_floats, planes_out, planes_capacity, *regions_out, info);
+  return planar_regions(h, "emap_extract_planar_regions", window, nullptr, 0, *plane_params, *region_params, nullptr,
+                        layers_out, out_is_device, out_floats, planes_out, planes_capacity, *regions_out, info);
 }
 
 // Postprocessing::postprocess after extract_planar_regions' passes: see include/emap.h and DESIGN.md §4l.
@@ -901,8 +971,35 @@ int emap_planar_terrain(emap_handle* h, const double window[4], const emap_plane
   if (!window || !plane_params || !region_params || !post_params || !layers_out || !planes_out || !regions_out || !info)
     return fail(h, EMAP_ERR_INVALID, "emap_planar_terrain: null argument");
   const emap_postprocess_params q = *post_params;
-  return planar_regions(h, "emap_planar_terrain", window, *plane_params, *region_params, &q, layers_out, out_is_device,
-                        out_floats, planes_out, planes_capacity, *regions_out, info);
+  return planar_regions(h, "emap_planar_terrain", window, nullptr, 0, *plane_params, *region_params, &q, layers_out,
+                        out_is_device, out_floats, planes_out, planes_capacity, *regions_out, info);
+}
+
+// The resampled size and resolution emap_plane_decomposition runs at (rs_geometry): see include/emap.h.
+int emap_plane_grid_geometry(int64_t rows, int64_t cols, double resolution, const emap_plane_params* params,
+                             int64_t out_size[2], double* out_resolution) {
+  if (!params || !out_size || !out_resolution || rows < 1 || cols < 1 ||
+      !(std::isfinite(resolution) && resolution > 0.0) || std::isnan(params->resolution))
+    return EMAP_ERR_INVALID;
+  rs_geometry(rows, cols, resolution, params->resolution, out_size, out_resolution);
+  return EMAP_OK;
+}
+
+// PlaneDecompositionPipeline::update's grid map part on a caller's grid: GridMapPreprocessing with its resampling, the
+// segmentation, the regions and the post-processing (planar_regions), at the resampled size.  See include/emap.h.
+int emap_plane_decomposition(emap_handle* h, const emap_grid* grid, int32_t grid_on_device,
+                             const emap_plane_params* plane_params, const emap_region_params* region_params,
+                             const emap_postprocess_params* post_params, float* layers_out, int32_t out_is_device,
+                             int64_t out_floats, double* planes_out, int64_t planes_capacity,
+                             const emap_region_out* regions_out, int32_t* info) {
+  ENTER(h);
+  NvtxRange nv("emap:plane_decomposition");
+  if (!grid || !plane_params || !region_params || !post_params || !layers_out || !planes_out || !regions_out || !info)
+    return fail(h, EMAP_ERR_INVALID, "emap_plane_decomposition: null argument");
+  const emap_grid g = *grid;
+  const emap_postprocess_params q = *post_params;
+  return planar_regions(h, "emap_plane_decomposition", nullptr, &g, grid_on_device, *plane_params, *region_params, &q,
+                        layers_out, out_is_device, out_floats, planes_out, planes_capacity, *regions_out, info);
 }
 
 // The node's publishAsPointCloud (elevation_mapping_ros.cpp:501-505): the points of the exported elevation (map_cloud).

@@ -1,11 +1,13 @@
-// emap_grid.cuh -- grid_map's index and position arithmetic on one axis, __host__ __device__ (kernel-free, so both the
-// windows of emap_submap.cuh and the lookups of emap_grid_lookup.cuh include it).
+// emap_grid.cuh -- grid_map's index and position arithmetic on one axis, __host__ __device__, and the check of a caller's
+// grid (kernel-free, so the windows of emap_submap.cuh, the lookups of emap_grid_lookup.cuh and the plane decomposition
+// of a grid in emap_export_api.cu include it).
 //
 // Restated from grid_map_core's published GridMapMath.cpp (not checked against a grid_map build), for a map whose
 // buffer start index is 0.  Per axis: pos the map's position (the centre of its cells), len its length (cells * res),
 // n its cells; index 0 is the +x (+y) edge.  Every operation is rounded on its own (no contraction), so the host and
 // the device give the same bits.
 #pragma once
+#include <cmath>
 #include <cstdint>
 #include <cuda_runtime.h>
 
@@ -14,6 +16,9 @@
 #else
 #define GRID_HD inline
 #endif
+
+#define GL_MAX_EXTENT 1048576.0    // emap.h's EMAP_GRID_MAX_EXTENT: |position| + length per axis, 2^20 m
+#define GL_MIN_RES 9.5367431640625e-07   // emap.h's EMAP_GRID_MIN_RESOLUTION, 2^-20 m
 
 #if defined(__CUDA_ARCH__)
 #define GRID_ADD(a, b) __dadd_rn((a), (b))
@@ -46,4 +51,21 @@ GRID_HD double grid_axis_origin(double pos, double len, double res) {
 GRID_HD double grid_axis_at(double origin, double res, int64_t i) { return GRID_ADD(origin, -GRID_MUL(res, (double)i)); }
 GRID_HD double grid_axis_position(double pos, double len, double res, int64_t i) {
   return grid_axis_at(grid_axis_origin(pos, len, res), res, i);
+}
+
+// The grids the calls accept (min_cells: the fewest rows and columns): nullptr, or why not.  Within these bounds a
+// projected line end is always inside the map (include/emap.h).
+inline const char* gl_check_grid(const float* data, int64_t rows, int64_t cols, const double pos[2], double res,
+                                 int64_t min_cells) {
+  if (!data) return "null grid data";
+  if (rows < min_cells || cols < min_cells)
+    return min_cells > 1 ? "rows and cols must be >= 5" : "rows and cols must be >= 1";
+  if (rows > INT32_MAX || cols > INT32_MAX || rows * cols > INT32_MAX) return "rows * cols must be below 2^31";
+  if (!(std::isfinite(res) && res >= GL_MIN_RES)) return "resolution must be finite and >= EMAP_GRID_MIN_RESOLUTION";
+  for (int a = 0; a < 2; a++) {
+    if (!std::isfinite(pos[a])) return "position must be finite";
+    if (!(std::fabs(pos[a]) + (double)(a ? cols : rows) * res <= GL_MAX_EXTENT))
+      return "|position| + length must be at most EMAP_GRID_MAX_EXTENT";
+  }
+  return nullptr;
 }

@@ -23,8 +23,6 @@
 #define GL_THREADS 256             // queries per block of k_gl_derivatives
 #define GL_SCAN_THREADS 1024       // k_gl_scan's single block
 #define GL_MARGIN 1e-6             // projectToMapWithMargin's default margin
-#define GL_MAX_EXTENT 1048576.0    // emap.h's EMAP_GRID_MAX_EXTENT: |position| + length per axis, 2^20 m
-#define GL_MIN_RES 9.5367431640625e-07   // emap.h's EMAP_GRID_MIN_RESOLUTION, 2^-20 m
 
 #if defined(__CUDA_ARCH__)
 #define GL_LANE ((int)(threadIdx.x & 31))
@@ -47,23 +45,6 @@ struct GlGrid {
   int rows, cols;
   double pos[2], len[2], res;
 };
-
-// The grids the calls accept (min_cells: the fewest rows and columns): nullptr, or why not.  Within these bounds a
-// projected line end is always inside the map (include/emap.h).
-inline const char* gl_check_grid(const float* data, int64_t rows, int64_t cols, const double pos[2], double res,
-                                 int64_t min_cells) {
-  if (!data) return "null grid data";
-  if (rows < min_cells || cols < min_cells)
-    return min_cells > 1 ? "rows and cols must be >= 5" : "rows and cols must be >= 1";
-  if (rows > INT32_MAX || cols > INT32_MAX || rows * cols > INT32_MAX) return "rows * cols must be below 2^31";
-  if (!(std::isfinite(res) && res >= GL_MIN_RES)) return "resolution must be finite and >= EMAP_GRID_MIN_RESOLUTION";
-  for (int a = 0; a < 2; a++) {
-    if (!std::isfinite(pos[a])) return "position must be finite";
-    if (!(std::fabs(pos[a]) + (double)(a ? cols : rows) * res <= GL_MAX_EXTENT))
-      return "|position| + length must be at most EMAP_GRID_MAX_EXTENT";
-  }
-  return nullptr;
-}
 
 GRID_HD float gl_at(const GlGrid& g, int r, int c) { return g.data[(int64_t)r * g.cols + c]; }
 

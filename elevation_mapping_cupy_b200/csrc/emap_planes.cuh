@@ -505,7 +505,7 @@ __global__ void k_pl_planes(const unsigned long long* __restrict__ st, const int
 }
 
 // The four output layers and info {success, rows, cols, highest_label, n_planes}; nothing but info when the window has
-// no finite cell.
+// no finite cell.  raw == nullptr leaves layer 0 unwritten (a caller's grid is its own elevation_raw).
 __global__ void k_pl_out(const float* __restrict__ raw, const float* __restrict__ img, const int* __restrict__ lab,
                          const unsigned char* __restrict__ bg, const int* __restrict__ hdr, float* __restrict__ out,
                          int32_t* __restrict__ info, int rows, int cols) {
@@ -519,7 +519,7 @@ __global__ void k_pl_out(const float* __restrict__ raw, const float* __restrict_
   if (i >= n || !ok) return;
   int l = lab[i];
   if (l > 0 && bg[l]) l = 0;
-  out[i] = raw[i];
+  if (raw) out[i] = raw[i];
   out[n + i] = img[i];
   out[2 * n + i] = (float)l;
   out[3 * n + i] = l > 0 ? 1.f : 0.f;

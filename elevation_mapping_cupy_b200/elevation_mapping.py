@@ -815,14 +815,58 @@ class ElevationMap:
         if device:
             self._before_framework()
 
-    def _planar_regions(self, position, length, params, out, capacities, post):
-        """extract_planar_regions (post False) and planar_terrain (post True): the call with the capacity retry."""
+    def plane_decomposition(self, grid, layer="elevation", params=None, out=None, capacities=None):
+        """The plane decomposition node's pipeline (PlaneDecompositionPipeline::update without RANSAC refinement) on a
+        grid rather than a window of this map, with the preprocessing's resampling to params.resolution, in one library
+        call (emap_plane_decomposition; include/emap.h states every step).  `grid`: a dict returned by get_submap(s),
+        get_transformed_submap(s) or planar_terrain; `layer` names one of its layers, read in place (NumPy or torch
+        CUDA).  `params`, `out` and `capacities` as in planar_terrain, with a device `out` of at least 10 * rows *
+        cols floats of the resampled grid.  Returns planar_terrain's dict for the resampled grid: "size",
+        "resolution", "origin" and "centre" are its geometry, and "elevation_raw" is the input layer itself (the node's
+        submap before the preprocessing, at its own size).  The result feeds project_to_planar_regions and the
+        lookups as planar_terrain's does."""
+        data = grid["layers"][layer]
+        g_dev = _is_device(data)
+        if g_dev:
+            import torch
+            if data.dtype != torch.float32 or not data.is_contiguous():
+                raise TypeError("a device layer must be a contiguous float32 torch CUDA tensor")
+            d_ptr = data.data_ptr()
+        else:
+            data = np.ascontiguousarray(data, np.float32)
+            d_ptr = data.ctypes.data
+        rows_in, cols_in = (int(v) for v in data.shape)
+        res_in = float(grid.get("resolution", self.resolution))
+        centre = np.asarray(_to_host(grid["centre"] if "centre" in grid else grid["frame_centre"]), np.float64)
+        g = _lib.EmapGrid(d_ptr, rows_in, cols_in, (C.c_double * 2)(*centre.tolist()), res_in)
+        from .plane_segmentation import PlaneSegmentationParams
+        p = (params or PlaneSegmentationParams()).to_c()
+        size = np.zeros(2, np.int64)
+        res = C.c_double(0.0)
+        self._check(self._L.emap_plane_grid_geometry(rows_in, cols_in, res_in, C.byref(p), size.ctypes.data,
+                                                     C.addressof(res)))
+        geometry = (int(size[0]), int(size[1]), res.value, centre)
+
+        def call(p, rp, pp, lay, device, planes, cap, ro, info):
+            return self._L.emap_plane_decomposition(self._h, C.byref(g), int(g_dev), C.byref(p), C.byref(rp),
+                                                    C.byref(pp), lay[0], int(device), lay[1], planes, cap,
+                                                    C.byref(ro), info)
+        result = self._planar_regions(None, None, params, out, capacities, True, geometry, call, g_dev)
+        result["layers"]["elevation_raw"] = data
+        return result
+
+    def _planar_regions(self, position, length, params, out, capacities, post, geometry=None, call=None,
+                        grid_dev=False):
+        """extract_planar_regions (post False), planar_terrain (post True) and plane_decomposition (geometry = the
+        resampled (rows, cols, resolution, centre), `call` its library call and grid_dev whether it reads device
+        memory): the call with the capacity retry."""
         from .plane_segmentation import PlaneSegmentationParams
         prm = params or PlaneSegmentationParams()
         p, rp = prm.to_c(), prm.regions_to_c()
         pp = prm.postprocess_to_c() if post else None
         n_layers = _lib.EMAP_TERRAIN_LAYERS if post else 4
-        req = np.array(_xy(position) + _xy(length), np.float64)
+        if geometry is None:
+            req = np.array(_xy(position) + _xy(length), np.float64)
         win = np.zeros(5, np.int32)
         centre = np.zeros(2, np.float64)
         device = out is not None and _is_device(out)
@@ -834,10 +878,14 @@ class ElevationMap:
         caps = tuple(int(v) for v in (capacities or self._region_caps))
         for attempt in range(2):
             with self.map_lock:
-                c = self.center.astype(np.float64)
-                self._check(self._L.emap_submap_windows(self.cell_n, float(self.resolution), c.ctypes.data, 1,
-                                                        req.ctypes.data, win.ctypes.data, centre.ctypes.data))
-                rows, cols = int(win[3]), int(win[4])
+                if geometry is None:
+                    c = self.center.astype(np.float64)
+                    self._check(self._L.emap_submap_windows(self.cell_n, float(self.resolution), c.ctypes.data, 1,
+                                                            req.ctypes.data, win.ctypes.data, centre.ctypes.data))
+                    rows, cols = int(win[3]), int(win[4])
+                    res = float(self.resolution)
+                else:
+                    rows, cols, res, centre = geometry
                 cap = max(int(self._L.emap_plane_capacity(rows, cols, C.byref(p))), 1)
                 if device:
                     import torch
@@ -858,9 +906,11 @@ class ElevationMap:
                 tables = (mk((max(caps[0], 1), 17), f64), mk((max(caps[1], 1), 5), i32), mk((max(caps[2], 1), 2), f64))
                 ro = _lib.EmapRegionOut(ptr(tables[0]), caps[0], ptr(tables[1]), caps[1], ptr(tables[2]), caps[2])
                 lay = (out.data_ptr(), out.numel()) if device else (out.ctypes.data, out.size)
-                if device:
+                if device or grid_dev:
                     self._after_framework()
-                if post:
+                if call is not None:
+                    self._check(call(p, rp, pp, lay, device, ptr(planes), cap, ro, ptr(info)))
+                elif post:
                     self._check(self._L.emap_planar_terrain(self._h, req.ctypes.data, C.byref(p), C.byref(rp),
                                                             C.byref(pp), lay[0], int(device), lay[1], ptr(planes), cap,
                                                             C.byref(ro), ptr(info)))
@@ -877,7 +927,6 @@ class ElevationMap:
         self._region_caps = tuple(max(a, int(b)) for a, b in zip(self._region_caps, info_h[5:8]))
         n = rows * cols
         flat = out.reshape(-1)
-        res = float(self.resolution)
         nr, npoly, nv = (int(x) for x in info_h[5:8])
         reg, poly, vert = tables[0][:nr], tables[1][:npoly], tables[2][:nv]
         result = {"layers": {name: flat[k * n:(k + 1) * n].reshape(rows, cols) for k, name in enumerate(names)},

@@ -13,7 +13,7 @@ class PlaneSegmentationParams:
     # preprocessing
     median_kernel: int = 3
     median_repeats: int = 1
-    resolution: float = 0.04           # resampling resolution: <= 0 or the map's (resampling is not supported)
+    resolution: float = 0.04           # resampled by plane_decomposition; the window calls take <= 0 or the map's
     # sliding_window_plane_extractor
     kernel_size: int = 3
     planarity_opening_filter: int = 0

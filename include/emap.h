@@ -751,6 +751,52 @@ int emap_values_between(emap_handle* h, const emap_grid* grid, int32_t grid_on_d
 int emap_grid_derivatives(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, int64_t n_queries,
                           const double* positions, int32_t positions_on_device, int32_t curvature,
                           const emap_derivative_out* out, int32_t out_is_device);
+/* ---- plane decomposition of a caller's grid: PlaneDecompositionPipeline::update's grid map part
+ * (ConvexPlaneDecompositionRos.cpp:88-162 without RANSAC refinement) on any grid, such as a window of
+ * emap_get_submaps or a new map of emap_get_transformed_submaps, with GridMapPreprocessing's resampling
+ * (inpainting::resample, grid_map_filters_rsl inpainting.cpp:244-288).  DESIGN.md §4l gives the restatement.
+ *  Grid (emap_grid, as the lookups take it): rows x cols fp32 cells, row-major, host (grid_on_device 0: staged in one
+ *    upload) or device memory, position = the centre of its cells, resolution res.
+ *  Geometry (emap_plane_grid_geometry): with params->resolution <= 0 or within 1e-6 of res the grid is not resampled;
+ *    otherwise scaling = res / new_res (double), rows' = int(rows * scaling) and cols' = int(cols * scaling)
+ *    (truncating), and the true resolution res' = 0.5 * ((rows * res) / rows' + (cols * res) / cols').  The position is
+ *    kept; origin = the centre of cell (0, 0) = position + (0.5 * (n' * res') - 0.5 * res') per axis.
+ *  Steps: the fill and the median of emap_segment_planes on the input; then, when the size changes, the resampling
+ *    below; then every later step of emap_planar_terrain on the rows' x cols' grid at res' and that origin (the per-cell
+ *    fit's res, the per-label origin, the regions' res' / 3 upsampling, kernelSizeInPixels and the sloped dilation's
+ *    offsets).
+ *  Resampling (cv::resize INTER_LINEAR, as cv2 4.13's default path computes it on x86; DESIGN.md §4l): per axis, for
+ *    output index d of m from n cells, f = (d + 0.5) * (n / m) - 0.5 in double, s = floor(f), f -= s; s < 0 or
+ *    s >= n - 1 is an edge position that takes cell clamp(s, 0, n - 1) alone; otherwise v = a + float(f) * (b - a) in
+ *    fp32 without contraction, a, b cells s and s + 1.  Columns first, on the two source rows of the row taps, then the
+ *    rows.  An exact 2x downscale in both axes is this same formula with f = 0.5 everywhere, which is what cv2's
+ *    default path computes there, bit for bit.  Against cv2's default path the result is within EMAP_RESAMPLE_ULPS
+ *    units in the last place of the input's largest finite magnitude; cv2 takes its scalar path for a source of one
+ *    row or column of n cells, and the bound there is EMAP_RESAMPLE_ULPS_LINE(n).  DESIGN.md §4l derives both.  +-inf
+ *    inside the grid propagates as in cv2 (inf - inf and 0 * inf are NaN); at edge positions cv2's default path
+ *    mixes single and two-tap evaluation, which this restatement does not reproduce.
+ * Outputs: emap_planar_terrain's, at rows' x cols': layers_out holds EMAP_TERRAIN_LAYERS planes of rows' x cols' with
+ * layer 0 (elevation_raw) left unwritten (in the node it is the grid before the preprocessing, at its own size: the
+ * caller's grid); planes, regions, polygons, vertices and info = {success, rows', cols', ...} as there.  A grid with
+ * no finite cell gives info[0] = 0.  Host and device output, stream order, graph capture (with a device grid), the
+ * capacity rule and the map state as in emap_planar_terrain; the launches depend on the parameters and the sizes
+ * only, one more than emap_planar_terrain's when the grid is resampled, and the grid's copy replaces k_submap.
+ * EMAP_ERR_INVALID, with nothing written or launched, for everything emap_planar_terrain rejects except the
+ * resampling (a NaN resolution is still rejected), the lookups' emap_grid checks, a grid or resampled grid of more
+ * than 2047 rows or columns (the largest window, so the scratch never exceeds the window calls'), a resampled size of
+ * 0, and a resampled grid with fewer rows or columns than the dilation size. */
+#define EMAP_RESAMPLE_ULPS 13
+#define EMAP_RESAMPLE_ULPS_LINE(n) (2 * (n) + 6)
+/* The resampled size (out_size = {rows', cols'}) and resolution emap_plane_decomposition runs a rows x cols grid of
+ * `resolution` at, for params->resolution; out_resolution is 0 when a size is 0.  EMAP_ERR_INVALID for a NULL
+ * argument, rows or cols below 1, a resolution that is not finite and > 0, or a NaN params->resolution. */
+int emap_plane_grid_geometry(int64_t rows, int64_t cols, double resolution, const emap_plane_params* params,
+                             int64_t out_size[2], double* out_resolution);
+int emap_plane_decomposition(emap_handle* h, const emap_grid* grid, int32_t grid_on_device,
+                             const emap_plane_params* plane_params, const emap_region_params* region_params,
+                             const emap_postprocess_params* post_params, float* layers_out, int32_t out_is_device,
+                             int64_t out_floats, double* planes_out, int64_t planes_capacity,
+                             const emap_region_out* regions_out, int32_t* info);
 /* ---- the exported map as a point cloud and as normal arrows: the ROS node's publishAsPointCloud
  * (elevation_mapping_ros.cpp:501-505, grid_map's toPointCloud(map, {"elevation"}, "elevation")) and publishNormalAsArrow
  * (:751-778), restated from grid_map's published source (not checked against a grid_map build).  Coordinates are those of

@@ -35,8 +35,8 @@ def _device_ms(call, reps):
     return e0.elapsed_time(e1) / reps
 
 
-def _kernels_ms(call, reps=3):
-    """Device time per call of each kernel (torch.profiler, CUDA activities), largest first."""
+def _kernels_ms(call, reps=3, top=12):
+    """Device time per call of each kernel (torch.profiler, CUDA activities), the `top` largest first (None: all)."""
     import torch
     from torch.profiler import ProfilerActivity, profile
     call()
@@ -53,7 +53,7 @@ def _kernels_ms(call, reps=3):
         if t > 0:
             name = e.key.split("(")[0].replace("void ", "")
             tot[name] = tot.get(name, 0.0) + t / 1e3 / reps
-    return {k: round(v, 4) for k, v in sorted(tot.items(), key=lambda kv: -kv[1])[:12]}
+    return {k: round(v, 4) for k, v in sorted(tot.items(), key=lambda kv: -kv[1])[:top]}
 
 
 def _lattice(n):
