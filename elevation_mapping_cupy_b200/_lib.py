@@ -91,6 +91,14 @@ class EmapDerivativeOut(C.Structure):
 EMAP_DERIVATIVE_INSIDE, EMAP_DERIVATIVE_OUTSIDE = 0, 1
 
 
+class EmapSdf(C.Structure):
+    _fields_ = [("data", C.c_void_p), ("rows", C.c_int64), ("cols", C.c_int64), ("n_z", C.c_int64),
+                ("position", C.c_double * 2), ("resolution", C.c_double), ("z_min", C.c_double)]
+
+
+EMAP_SDF_MAX_D2 = 1 << 24
+
+
 class EmapDepthCamera(C.Structure):
     _fields_ = [("height", C.c_int32), ("width", C.c_int32), ("depth", C.c_void_p), ("confidence", C.c_void_p),
                 ("rgb", C.c_void_p), ("features", C.c_void_p), ("fx", C.c_double), ("fy", C.c_double),
@@ -176,6 +184,10 @@ SIGNATURES = {
                                       C.POINTER(EmapLineValuesOut), C.c_int32]),
     "emap_grid_derivatives": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
                                         C.c_int32, C.POINTER(EmapDerivativeOut), C.c_int32]),
+    "emap_signed_distance_field": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_double, C.c_int64,
+                                             C.c_void_p, C.c_int64, C.c_int32]),
+    "emap_sdf_values": (C.c_int, [C.c_void_p, C.POINTER(EmapSdf), C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
+                                  C.c_void_p, C.c_int32]),
     "emap_plane_grid_geometry": (C.c_int, [C.c_int64, C.c_int64, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
     "emap_plane_decomposition": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int64,

@@ -224,9 +224,10 @@ struct emap_handle {
     StagedUpload up;               // staging of host output
     PinnedBuf<char> down;
   } query;
-  struct {                         // the grid lookups (grown to the largest call): the device block carved by
-    DevBuf<char> block;            // carve_lookup, emap_values_between's host-bound rows, the upload of a host grid and
-    DevBuf<double> rows;           // queries, and the pinned staging of host output
+  struct {                         // the grid lookups and the distance field (grown to the largest call): the device
+    DevBuf<char> block;            // block (the lookups' outputs, the field's fill key and host-bound volume),
+    DevBuf<double> rows;           // emap_values_between's host-bound rows, the upload of a host grid or field and
+                                   // queries, and the pinned staging of host output
     StagedUpload up;
     PinnedBuf<char> down;
   } lookup;

@@ -1,10 +1,12 @@
 // emap_terrain_query_api.cu -- queries on the planar terrain and its layers of the C ABI (include/emap.h):
-// emap_project_to_planar_regions over the kernels of emap_terrain_query.cuh, and emap_max_values_between,
-// emap_values_between and emap_grid_derivatives over those of emap_grid_lookup.cuh.
+// emap_project_to_planar_regions over the kernels of emap_terrain_query.cuh, emap_max_values_between,
+// emap_values_between and emap_grid_derivatives over those of emap_grid_lookup.cuh, and emap_signed_distance_field and
+// emap_sdf_values over those of emap_sdf.cuh.
 #include <algorithm>
 
 #include "emap_grid_lookup.cuh"
 #include "emap_handle.cuh"
+#include "emap_sdf.cuh"
 #include "emap_terrain_query.cuh"
 
 namespace {
@@ -57,11 +59,28 @@ const char* check_lookup(const emap_grid* g, int64_t min_cells, int64_t n, const
   return nullptr;
 }
 
+// Host inputs staged and uploaded in one copy: `data_bytes` of data (0: on the device already), then `q_bytes` of
+// queries (0: likewise); data and q are pointed at their device copies.
+int stage_inputs(emap_handle* h, const void*& data, size_t data_bytes, const double*& q, size_t q_bytes) {
+  const size_t q_off = (data_bytes + 255) & ~(size_t)255;
+  if (!data_bytes && !q_bytes) return 0;
+  const size_t up = q_off + q_bytes;
+  if (int rc = h->lookup.up.room(h, up)) return rc;
+  if (data_bytes) {
+    memcpy(h->lookup.up.host, data, data_bytes);
+    data = (const void*)(char*)h->lookup.up.dev;
+  }
+  if (q_bytes) {
+    memcpy(h->lookup.up.host + q_off, q, q_bytes);
+    q = (const double*)(h->lookup.up.dev + q_off);
+  }
+  return h->lookup.up.send(h, up);
+}
+
 // The grid and queries as the kernels read them: a host grid and host queries (per_query doubles each) staged and
 // uploaded in one copy.
 int lookup_inputs(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, int64_t n, const double* queries,
                   int32_t queries_on_device, int per_query, GlGrid& g, const double*& q) {
-  g.data = grid->data;
   g.rows = (int)grid->rows;
   g.cols = (int)grid->cols;
   g.res = grid->resolution;
@@ -70,21 +89,12 @@ int lookup_inputs(emap_handle* h, const emap_grid* grid, int32_t grid_on_device,
     g.len[a] = (double)(a ? grid->cols : grid->rows) * grid->resolution;
   }
   q = queries;
+  const void* data = grid->data;
   const size_t grid_bytes = grid_on_device ? 0 : sizeof(float) * grid->rows * grid->cols;
-  const size_t q_off = (grid_bytes + 255) & ~(size_t)255;
   const size_t q_bytes = queries_on_device ? 0 : sizeof(double) * per_query * n;
-  if (!grid_bytes && !q_bytes) return 0;
-  const size_t up = q_off + q_bytes;
-  if (int rc = h->lookup.up.room(h, up)) return rc;
-  if (grid_bytes) {
-    memcpy(h->lookup.up.host, grid->data, grid_bytes);
-    g.data = (const float*)(char*)h->lookup.up.dev;
-  }
-  if (q_bytes) {
-    memcpy(h->lookup.up.host + q_off, queries, q_bytes);
-    q = (const double*)(h->lookup.up.dev + q_off);
-  }
-  return h->lookup.up.send(h, up);
+  const int rc = stage_inputs(h, data, grid_bytes, q, q_bytes);
+  g.data = (const float*)data;
+  return rc;
 }
 
 // Host output: `bytes` of the device block back into the pinned staging, one synchronisation.
@@ -95,11 +105,24 @@ int lookup_back(emap_handle* h, size_t bytes) {
   return 0;
 }
 
+// The volumes the field calls accept, after the lookups' grid checks: nullptr, or why not
+const char* check_volume(int64_t rows, int64_t cols, int64_t n_z, double z_min) {
+  if (n_z < 1) return "n_z must be >= 1";
+  if (!std::isfinite(z_min)) return "z_min must be finite";
+  if (rows > SDF_MAX_LINE || cols > SDF_MAX_LINE || n_z > SDF_MAX_LINE ||
+      (rows - 1) * (rows - 1) + (cols - 1) * (cols - 1) + (n_z - 1) * (n_z - 1) >= SDF_MAX_D2)
+    return "(rows - 1)^2 + (cols - 1)^2 + (n_z - 1)^2 must be below 2^24";
+  if (rows * cols * n_z > INT32_MAX) return "rows * cols * n_z must be below 2^31";
+  return nullptr;
+}
+
 }  // namespace
 
 static_assert(EMAP_GRID_MAX_EXTENT == GL_MAX_EXTENT && EMAP_GRID_MIN_RESOLUTION == GL_MIN_RES, "the grid bounds");
 static_assert((int)EMAP_DERIVATIVE_INSIDE == (int)GL_INSIDE && (int)EMAP_DERIVATIVE_OUTSIDE == (int)GL_OUTSIDE,
               "the derivative statuses");
+
+static_assert(EMAP_SDF_MAX_D2 == SDF_MAX_D2, "the field's limit");
 
 static_assert(EMAP_REGION_ROW == PQ_ROW && EMAP_REGION_POLYGON == PQ_POLY, "the region table layout");
 static_assert(EMAP_CONVEX_MAX_VERTICES == PQ_MAX_CONVEX && EMAP_GROW_MAX_ITER == PQ_MAX_ITER, "the growth limits");
@@ -314,6 +337,83 @@ int emap_grid_derivatives(emap_handle* h, const emap_grid* grid, int32_t grid_on
     if (int rc = lookup_back(h, vb + ib)) return rc;
     memcpy(out->value, h->lookup.down, vb);
     memcpy(out->index, h->lookup.down + vb, ib);
+  }
+  return EMAP_OK;
+}
+
+int emap_signed_distance_field(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, double z_min,
+                               int64_t n_z, float* out, int64_t capacity, int32_t out_is_device) {
+  ENTER(h);
+  const char* e = !grid || !out ? "null argument" : gl_check_grid(grid->data, grid->rows, grid->cols, grid->position,
+                                                                 grid->resolution, 1);
+  if (!e) e = check_volume(grid->rows, grid->cols, n_z, z_min);
+  if (!e && capacity < grid->rows * grid->cols * n_z) e = "capacity below rows * cols * n_z";
+  if (e) return fail(h, EMAP_ERR_INVALID, (std::string("emap_signed_distance_field: ") + e).c_str());
+  NvtxRange nv("signed_distance_field");
+  const int rows = (int)grid->rows, cols = (int)grid->cols, nz = (int)n_z;
+  const size_t vol_bytes = sizeof(float) * rows * cols * nz;
+  // the block: the fill key, then (host output) the volume
+  const size_t vol_off = 256;
+  if (int rc = grow(h, h->lookup.block, vol_off + (out_is_device ? 0 : vol_bytes), 0, false)) return rc;
+  uint32_t* key = (uint32_t*)(char*)h->lookup.block;
+  int32_t* vol = out_is_device ? (int32_t*)out : (int32_t*)(h->lookup.block + vol_off);
+  const void* data = grid->data;
+  const double* no_q = nullptr;
+  if (int rc = stage_inputs(h, data, grid_on_device ? 0 : sizeof(float) * rows * cols, no_q, 0)) return rc;
+  CK(cudaMemsetAsync(key, 0xff, sizeof(uint32_t), h->stream));     // SDF_KEY_NONE
+  const int64_t cells = (int64_t)rows * cols;
+  k_sdf_min<<<std::min(cdiv(cells, SDF_THREADS * 8), 1024), SDF_THREADS, 0, h->stream>>>((const float*)data, cells,
+                                                                                           key);
+  LAUNCH_CHECK();
+  k_sdf_cols<<<dim3(rows, nz), SDF_LINE_THREADS, sdf_line_smem(cols), h->stream>>>(
+      (const float*)data, rows, cols, nz, z_min, grid->resolution, key, vol);
+  LAUNCH_CHECK();
+  k_sdf_rows<<<dim3(cols, nz), SDF_LINE_THREADS, sdf_line_smem(rows), h->stream>>>(rows, cols,
+                                                                                  (float)grid->resolution, vol);
+  LAUNCH_CHECK();
+  if (!out_is_device) {
+    if (h->lookup.down.size() < vol_bytes) CK(h->lookup.down.alloc(vol_bytes));
+    CK(cudaMemcpyAsync(h->lookup.down, vol, vol_bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    memcpy(out, h->lookup.down, vol_bytes);
+  }
+  return EMAP_OK;
+}
+
+int emap_sdf_values(emap_handle* h, const emap_sdf* field, int32_t field_on_device, int64_t n, const double* points,
+                    int32_t points_on_device, double* out, int32_t out_is_device) {
+  ENTER(h);
+  const char* e = !field ? "null argument" : gl_check_grid(field->data, field->rows, field->cols, field->position,
+                                                          field->resolution, 1);
+  if (!e) e = check_volume(field->rows, field->cols, field->n_z, field->z_min);
+  if (!e && (n < 0 || n > INT32_MAX)) e = "n must be 0 .. 2^31 - 1";
+  if (!e && n && (!points || !out)) e = "null points or output";
+  if (e) return fail(h, EMAP_ERR_INVALID, (std::string("emap_sdf_values: ") + e).c_str());
+  if (n == 0) return EMAP_OK;
+  NvtxRange nv("sdf_values");
+  const size_t ob = sizeof(double) * 4 * n;
+  if (!out_is_device)
+    if (int rc = grow(h, h->lookup.block, ob, 0, false)) return rc;
+  SdfVol f;
+  f.rows = (int)field->rows;
+  f.cols = (int)field->cols;
+  f.n_z = (int)field->n_z;
+  f.pos[0] = field->position[0];
+  f.pos[1] = field->position[1];
+  f.res = field->resolution;
+  f.z_min = field->z_min;
+  const void* data = field->data;
+  const double* q = points;
+  if (int rc = stage_inputs(h, data, field_on_device ? 0 : sizeof(float) * f.rows * f.cols * f.n_z, q,
+                            points_on_device ? 0 : sizeof(double) * 3 * n))
+    return rc;
+  f.data = (const float*)data;
+  double* o = out_is_device ? out : (double*)(char*)h->lookup.block;
+  k_sdf_values<<<cdiv(n, SDF_THREADS), SDF_THREADS, 0, h->stream>>>(f, q, n, o);
+  LAUNCH_CHECK();
+  if (!out_is_device) {
+    if (int rc = lookup_back(h, ob)) return rc;
+    memcpy(out, h->lookup.down, ob);
   }
   return EMAP_OK;
 }

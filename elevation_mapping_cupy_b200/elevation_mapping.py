@@ -26,6 +26,7 @@ frame reads the depth, confidence, rgb and feature planes itself (csrc/emap_sour
 Out of scope (SURVEY.md section 8): the image feature extractors.
 """
 import ctypes as C
+import math
 import threading
 from typing import List
 
@@ -768,9 +769,94 @@ class ElevationMap:
             res["curvature"] = value[:, 2:]
         return res
 
+    def signed_distance_field(self, grid, layer="elevation", height_clearance=0.1, z_range=None, out=None):
+        """A signed distance field of `layer` over the grid's box (metres to the terrain surface: positive above it,
+        negative below), in one library call (emap_signed_distance_field; include/emap.h states every step).  `grid`
+        and `layer` as in max_value_between_locations (a dict of segment_planes, planar_terrain, plane_decomposition,
+        get_submap(s) or the caller's own with "layers", "centre" and optionally "resolution").  The slices are res
+        apart from z_min: with `z_range` = (z_low, z_high), z_min = z_low and n_z = floor((z_high - z_low) / res) + 1;
+        without it, z_min = lowest finite value - height_clearance and n_z = floor(((highest finite value +
+        height_clearance) - z_min) / res) + 1, which reads two scalars back (a host synchronisation for a device
+        layer), and a layer with no finite cell raises ValueError.  `out`: None, or an (n_z, rows, cols) contiguous
+        float32 NumPy array or CUDA tensor, written in place; a device layer or `out` keeps the volume on the device
+        (stream-ordered, no host synchronisation with `z_range`).  Returns "volume" (n_z, rows, cols), "rows", "cols",
+        "n_z", "position", "resolution" and "z_min": the dict sdf_values takes."""
+        g, g_dev, _, _, device, mk, ptr = self._lookup_args(grid, layer, (), 0, None if out is None else {"volume": out},
+                                                            ("volume",), True)
+        res = float(g.resolution)
+        if z_range is None:
+            data = g._keep
+            if g_dev:
+                import torch
+                fin = data[torch.isfinite(data)]
+                if fin.numel() == 0:
+                    raise ValueError("the layer has no finite cell: pass z_range")
+                lo, hi = (float(v) for v in torch.aminmax(fin))
+            else:
+                fin = data[np.isfinite(data)]
+                if fin.size == 0:
+                    raise ValueError("the layer has no finite cell: pass z_range")
+                lo, hi = float(fin.min()), float(fin.max())
+            z_min = lo - float(height_clearance)
+            n_z = int(math.floor(((hi + float(height_clearance)) - z_min) / res)) + 1
+        else:
+            z_min = float(z_range[0])
+            n_z = int(math.floor((float(z_range[1]) - z_min) / res)) + 1
+        shape = (n_z, int(g.rows), int(g.cols))
+        if out is None:
+            out = mk(shape, "float32")
+        _check_out({"volume": out}, {"volume": shape}, device)
+        if device or g_dev:
+            self._after_framework()
+        self._check(self._L.emap_signed_distance_field(self._h, C.byref(g), int(g_dev), z_min, n_z, ptr(out),
+                                                       out.numel() if device else out.size, int(device)))
+        if device:
+            self._before_framework()
+        return {"volume": out, "rows": int(g.rows), "cols": int(g.cols), "n_z": n_z,
+                "position": np.array(g.position[:], np.float64), "resolution": res, "z_min": z_min}
+
+    def sdf_values(self, field, points, out=None):
+        """The field's value and gradient at each point, in one library call (emap_sdf_values; include/emap.h states
+        every step): trilinear inside the box, plus the distance to the box outside it.  `field`: a dict returned by
+        signed_distance_field (its "volume" read in place, NumPy or torch CUDA).  `points`: (N, 3) map-frame points,
+        float64 NumPy or a CUDA tensor.  `out`: None, or an (N, 4) float64 array, NumPy or torch CUDA, written in place.
+        Device points or a device `out` keep everything on the device.  Returns (N, 4): value, d/dx, d/dy, d/dz."""
+        vol = field["volume"]
+        f_dev = _is_device(vol)
+        if f_dev:
+            import torch
+            if vol.dtype != torch.float32 or not vol.is_contiguous():
+                raise TypeError("a device volume must be a contiguous float32 torch CUDA tensor")
+            v_ptr = vol.data_ptr()
+        else:
+            vol = np.ascontiguousarray(vol, np.float32)
+            v_ptr = vol.ctypes.data
+        n_z, rows, cols = (int(field[k]) for k in ("n_z", "rows", "cols"))
+        if tuple(vol.shape) != (n_z, rows, cols):
+            raise ValueError("the volume must be (n_z, rows, cols)")
+        pos = np.asarray(_to_host(field["position"]), np.float64)
+        f = _lib.EmapSdf(v_ptr, rows, cols, n_z, (C.c_double * 2)(*pos.tolist()), float(field["resolution"]),
+                         float(field["z_min"]))
+        f._keep = vol
+        q_dev = _is_device(points)
+        device = q_dev or (out is not None and _is_device(out))
+        if q_dev:
+            import torch
+            q = points.to(torch.float64).reshape(-1, 3).contiguous()
+        else:
+            q = np.ascontiguousarray(np.asarray(points, np.float64).reshape(-1, 3))
+        n = int(q.shape[0])
+        if out is None:
+            out = _array_maker(points.device if device else None)[0]((n, 4), "float64")
+        _check_out({"value": out}, {"value": (n, 4)}, device)
+        ptr = (lambda a: a.data_ptr()) if device else (lambda a: a.ctypes.data)  # noqa: E731
+        self._lookup_call(self._L.emap_sdf_values, f, f_dev, n, q, ptr(out), device)
+        return out
+
     def _lookup_args(self, grid, layer, parts, width, out, out_keys, follow_grid=False):
-        """What the three lookups share: the layer's emap_grid (the grid dict's "centre", its "resolution" or the map's),
-        the queries as one contiguous (N, width) float64 array (NumPy, or a CUDA tensor when any part is one), whether
+        """What the lookups and the distance field share: the layer's emap_grid (the grid dict's "centre", its
+        "resolution" or the map's), the queries as one contiguous (N, width) float64 array (NumPy, or a CUDA tensor when
+        any part is one; None without parts), whether
         the call writes device output (device queries, a device `out` or, with follow_grid, a device layer), and an
         array maker and pointer getter for that side."""
         data = grid["layers"][layer]
@@ -792,7 +878,9 @@ class ElevationMap:
         out_dev = [out[k] for k in out_keys if _is_device(out[k])] if out is not None else []
         device = q_dev or bool(out_dev) or (follow_grid and g_dev)
         dev = None
-        if q_dev:
+        if not parts:
+            q = None
+        elif q_dev:
             import torch
             dev = next(p.device for p in parts if _is_device(p))
             q = torch.cat([torch.as_tensor(p, device=dev).to(torch.float64).reshape(-1, width // len(parts))
@@ -800,7 +888,7 @@ class ElevationMap:
         else:
             q = np.ascontiguousarray(np.concatenate([np.asarray(p, np.float64).reshape(-1, width // len(parts))
                                                      for p in parts], 1))
-        n = int(q.shape[0])
+        n = int(q.shape[0]) if parts else 0
         if device and dev is None:
             dev = out_dev[0].device if out_dev else data.device
         mk, ptr = _array_maker(dev if device else None)
@@ -1237,7 +1325,7 @@ def _array_maker(device):
 
 def _check_out(out, shapes, device):
     """Every out[k] is a contiguous array of shapes[k] on the call's side (NumPy for host output, CUDA for device)."""
-    dtypes = {"index": "int32", "value": "float64"}
+    dtypes = {"index": "int32", "value": "float64", "volume": "float32"}
     for k, shape in shapes.items():
         a = out[k]
         if tuple(a.shape) != shape or _is_device(a) != device or str(a.dtype).split(".")[-1] != dtypes[k] or not (

@@ -751,6 +751,63 @@ int emap_values_between(emap_handle* h, const emap_grid* grid, int32_t grid_on_d
 int emap_grid_derivatives(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, int64_t n_queries,
                           const double* positions, int32_t positions_on_device, int32_t curvature,
                           const emap_derivative_out* out, int32_t out_is_device);
+/* ---- a signed distance field of one grid layer and distance queries against it, on the device (a legged robot's
+ * swing-leg clearance: how far a point is from the terrain and in which direction that distance grows).  DESIGN.md
+ * §4l (continued) gives the algorithm.  The handle's map state is not read or changed; the calls use the handle's
+ * stream, staging and scratch of the lookups.
+ * Field (emap_signed_distance_field): the grid is an emap_grid exactly as the lookups take it (host or device, the same
+ *  checks), res its resolution.  Slice k (0 <= k < n_z) lies at z_k = z_min + k * res in double (one multiply, then
+ *  one add); the voxels are res apart on all three axes.
+ *  Occupancy: a non-finite cell takes the layer's lowest finite value (one device reduction, no host synchronisation;
+ *    a layer with no finite cell has no occupied voxel).  Voxel (r, c, k) is occupied iff (double)e(r, c) >= z_k, else
+ *    free.  A column's top slice T (the highest occupied slice, -1 for none) is floor((e - z_min) / res) corrected by
+ *    the exact comparison, so it agrees with it for every k.
+ *  Value: with d2 the exact integer squared Euclidean distance in voxel units between voxel centres, over the voxels
+ *    of the volume only, a free voxel holds +fl(sqrt(float(d2)) * float(res)) (correctly rounded float square root and
+ *    product) for its nearest occupied voxel, an occupied voxel minus that for its nearest free voxel; +INFINITY
+ *    (-INFINITY) when the volume has no voxel of the other kind.
+ *  Output: n_z x rows x cols floats, slice after slice, each slice in the grid's row-major layout (slice k reads like a
+ *    layer of the grid), in host (out_is_device 0) or device memory; capacity is out's size in floats.
+ *  Kernels: 3 (the lowest finite value; the z pass with the envelopes along the columns of every row, one CTA per
+ *    row and slice; the envelopes along the rows, one CTA per column and slice, in place in the output).
+ * Queries (emap_sdf_values): n points (x, y, z) as doubles, host or device, against a field (emap_sdf: a volume as
+ *  emap_signed_distance_field writes it with its grid's geometry and z_min, in host (field_on_device 0) or device
+ *  memory).  out: 4 doubles per point {value, d/dx, d/dy, d/dz}.  Every operation is in double, rounded on its own (no
+ *  contraction).  Per point:
+ *   fractional indices fr = ((p_x + (0.5 L_x - 0.5 res)) - x) / res (the inverse of getPositionFromIndex),
+ *     fc = ((p_y + (0.5 L_y - 0.5 res)) - y) / res, fk = (z - z_min) / res, with L = (rows, cols) * res;
+ *   per axis of n cells, u = the index clamped to [0, n - 1] (f < 0: 0; f > n - 1: n - 1), i0 = min(floor(u), n - 2)
+ *     and i1 = i0 + 1 (both 0 when n = 1), t = u - i0, and off = f - u;
+ *   V(k, r, c) the voxel value widened to double; lerp(a, b, t) = a + t * (b - a);
+ *   columns: X(k, r) = lerp(V(k, r, c0), V(k, r, c1), tc) and D(k, r) = V(k, r, c1) - V(k, r, c0);
+ *   rows: Y(k) = lerp(X(k, r0), X(k, r1), tr), R(k) = X(k, r1) - X(k, r0), E(k) = lerp(D(k, r0), D(k, r1), tr);
+ *   slices: value = lerp(Y(k0), Y(k1), tk) + sqrt((off_r^2 + off_c^2) + off_k^2) * res (the distance in metres from the
+ *     point to its clamped point, 0 inside the box);
+ *   gradient of the interpolant: d/dx = -(lerp(R(k0), R(k1), tk) / res) (the row index grows toward -x),
+ *     d/dy = -(lerp(E(k0), E(k1), tk) / res), d/dz = (Y(k1) - Y(k0)) / res; 0 along an axis of one cell.
+ *  A NaN coordinate gives four NaNs.  Infinite voxel values (a volume with no voxel of one kind) propagate by IEEE
+ *  arithmetic, so such a volume gives infinite or NaN values and NaN gradients.  Every NaN is written as the quiet NaN
+ *  0x7ff8000000000000.  Kernels: 1 (one thread per point), none for n = 0.
+ * Host grids, fields and points are staged and uploaded in one copy; host output comes back in one copy and
+ * synchronisation.  Device output is stream-ordered with no host synchronisation and can be captured into a CUDA graph
+ * (with device inputs; capture after an eager call of the largest size: growing the scratch synchronises).
+ * EMAP_ERR_INVALID, with nothing written or launched: everything the lookups reject for their grid (emap_sdf_values:
+ * for the field's rows, cols, position, resolution and data), n_z below 1, a non-finite z_min,
+ * (rows - 1)^2 + (cols - 1)^2 + (n_z - 1)^2 >= EMAP_SDF_MAX_D2 (so that every d2 converts to float exactly),
+ * rows * cols * n_z >= 2^31, a NULL out, a capacity below rows * cols * n_z, n below 0 or above 2^31 - 1, and NULL
+ * points or out with n > 0. */
+#define EMAP_SDF_MAX_D2 16777216   /* 2^24 */
+typedef struct emap_sdf {
+  const float* data;       /* n_z x rows x cols */
+  int64_t rows, cols, n_z;
+  double position[2];      /* the centre of the cells, map frame [m] */
+  double resolution;       /* [m], also the slice spacing */
+  double z_min;            /* the height of slice 0 [m] */
+} emap_sdf;
+int emap_signed_distance_field(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, double z_min,
+                               int64_t n_z, float* out, int64_t capacity, int32_t out_is_device);
+int emap_sdf_values(emap_handle* h, const emap_sdf* field, int32_t field_on_device, int64_t n, const double* points,
+                    int32_t points_on_device, double* out, int32_t out_is_device);
 /* ---- plane decomposition of a caller's grid: PlaneDecompositionPipeline::update's grid map part
  * (ConvexPlaneDecompositionRos.cpp:88-162 without RANSAC refinement) on any grid, such as a window of
  * emap_get_submaps or a new map of emap_get_transformed_submaps, with GridMapPreprocessing's resampling
