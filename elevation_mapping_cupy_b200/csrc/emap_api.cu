@@ -470,7 +470,7 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   ALLOC(h->trav_input, C);
   ALLOC(h->xscratch, exchange_bytes(C));
   ALLOC(h->thr, C);
-  ALLOC(h->dirty, C + 16);
+  ALLOC(h->dirty, 2 * (C + 16));
   ALLOC(h->ukey_x, C);
   ALLOC(h->lut, 65536);
   ALLOC(h->tmap, RT * RT);
@@ -481,7 +481,7 @@ int emap_create(const emap_config* cfg, int device, emap_handle** out) {
   h->sc.dirty = h->dirty;
   TRY(place_exchange(h, h->xscratch));
   TRY(cudaMemsetAsync(h->thr, 0, sizeof(float) * C, h->stream));
-  TRY(cudaMemsetAsync(h->dirty, 0, C + 16, h->stream));
+  TRY(cudaMemsetAsync(h->dirty, 0, 2 * (C + 16), h->stream));
   TRY(cudaMemsetAsync(h->tmap, 0, sizeof(u32) * RT * RT, h->stream));
   TRY(cudaMemsetAsync(h->normal, 0, sizeof(float) * 3 * C, h->stream));
   TRY(cudaMemsetAsync(h->trav_input, 0, sizeof(float) * C, h->stream));

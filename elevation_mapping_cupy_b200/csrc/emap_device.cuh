@@ -96,8 +96,10 @@ struct CellScratch {
   float* thr;      // first-level ray record, 4 B: a sample at height nz can only act on the cell if !(nz > thr)
   uint2* rec;      // second-level ray record, 8 B: {valid cell ? bits(h') : upper-bound key, flags}; read-only for rays
   u32* ukv;        // min over rays of the upper-bound key carved into the cell (UKEY_NONE between frames), CK.py:230-233,253-256
-  unsigned char* dirty;   // 1 = some kernel of this frame touched the cell's scratch (k_finalize takes its full path there
-                   // and clears it); nullptr in sharded frames, where the marker is derived from cnt_all / ukv
+  unsigned char* dirty;   // two marker bytes per cell: [2i] = 1 when the point passes accumulated into cell i (k_index_error,
+                   // k_fuse), [2i + 1] = 1 when the ray-cast did (k_raycast).  k_finalize takes its full path where
+                   // either is set, reads only the flagged scratch groups, and clears both; nullptr in sharded frames,
+                   // where the markers are derived from cnt_all / ukv
   i64 mc_off;      // sharded frames: byte offset from a local scratch address to its NVLink MULTICAST alias
                    // (0 = single GPU).  Non-zero: every accumulation is one multimem.red that the NVSwitch
                    // applies to the replicas of ALL ranks (this one included) -- scatter and collective fused.

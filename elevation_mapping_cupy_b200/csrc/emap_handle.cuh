@@ -156,7 +156,7 @@ struct emap_handle {
   DevBuf<float> steps;        // device march table: [0] dummy, [1 + k] = s_k, +inf padded to plan.n_tab entries
   DevBuf<unsigned short> lut;        // cell of every fp16 bit pattern (k_build_lut)
   DevBuf<unsigned short> step_cnt;   // march steps below every non-negative fp16 value (k_build_step_cnt)
-  DevBuf<unsigned char> dirty;       // per-cell dirty bytes of single-GPU frames (CellScratch::dirty)
+  DevBuf<unsigned char> dirty;       // two marker bytes per cell of single-GPU frames, points and rays (CellScratch::dirty)
   DevBuf<float> thr;                 // CellScratch::thr
   DevBuf<u32> tmap;                  // coarse ray map of the frame: RT x RT tile maxima of thr (keys)
   // points

@@ -169,7 +169,7 @@ k_index_error(const DevCfg c, const Pose q, const Src src, const i64 n,
           is_inl = true;
         }
         cell_key = idx;
-        if (s.dirty) s.dirty[idx] = 1;
+        if (s.dirty) s.dirty[2 * idx] = 1;                        // points marker: exactly the cells k_fuse may touch
       }
     }
     xyzv[i] = o; pidx[i] = rec;
@@ -656,7 +656,7 @@ k_raycast(const DevCfg c, const Pose q, const Ray* __restrict__ rays, int* __res
           const u32 key = fkey(nz);
           if (key < rc.x && key < __ldcg(s.ukv + nidx)) {
             red_min(s.ukv + nidx, key, s.mc_off);                 // true min over all rays (and ranks)
-            if (s.dirty) s.dirty[nidx] = 1;
+            if (s.dirty) s.dirty[2 * nidx + 1] = 1;
           }
           continue;
         }
@@ -675,7 +675,7 @@ k_raycast(const DevCfg c, const Pose q, const Ray* __restrict__ rays, int* __res
         red_add((u64*)(s.DV + nidx), (u64)dec_fix, s.mc_off);     // CK.py:250
         red_add(s.n_ray + nidx, 1u, s.mc_off);                    // CK.py:251
         red_min(s.ukv + nidx, fkey(nz), s.mc_off);                // CK.py:253-256
-        if (s.dirty) s.dirty[nidx] = 1;
+        if (s.dirty) s.dirty[2 * nidx + 1] = 1;
       }
     }
    }
@@ -695,19 +695,24 @@ k_raycast(const DevCfg c, const Pose q, const Ray* __restrict__ rays, int* __res
 
 // Apply every side effect of the frame to the state planes, then average_map_kernel
 // (CK.py:362-384) and clear_overlap_map (EM.py:393-410); re-zero the consumed scratch.
-// One cell, full path: everything the frame may have done to it.
+// One cell, full path: everything the frame may have done to it.  The scratch falls into two groups, each written by one
+// side of the frame: `pts` (cnt_fo, cnt_ai, SH, SV, last: the point passes) and `rays` (n_ray, ukv, DV: the ray-cast).  A
+// group whose flag is clear still holds its between-frames value (zero; UKEY_NONE for ukv), so it is neither read nor
+// re-zeroed.  cnt_ai is re-zeroed without being read: it is non-zero exactly where `pts` is set.  An overlap-window cell
+// with neither flag reads only the map planes.
 __device__ __forceinline__ void finalize_cell(const DevCfg& c, float* __restrict__ map, const CellScratch& s, const int i,
-                                              const int rr, const int cc, const int applied, const float shift,
-                                              const float hmin, const float hmax, const int rays_ran) {
+                                              const int applied, const float shift,
+                                              const float hmin, const float hmax, const bool pts, const bool rays) {
   const size_t C = (size_t)c.C;
-  // every load up front, also the ones only some cells need (last / sums: cells hit by points; DV: cells acted on by rays):
-  // the kernel is bound by dependent round trips to L2 / DRAM, not by bytes, so one wave of 14 loads beats two dependent ones
-  const u64 fo = s.cnt_fo[i], ca = s.cnt_ai[i];
+  // every load the flagged groups need up front, also the ones only some of their cells need (last / sums: fused points;
+  // DV: rays that decrement): the kernel is bound by dependent round trips to L2 / DRAM, not by bytes, so one wave of loads
+  // beats two dependent ones
+  u64 fo = 0, last_key = 0;
+  i64 sh_fix = 0, sv_fix = 0;
+  if (pts) { fo = s.cnt_fo[i]; last_key = s.last[i]; sh_fix = s.SH[i]; sv_fix = s.SV[i]; }
   u32 nr = 0, kv = UKEY_NONE;
   i64 dv_fix = 0;
-  if (rays_ran) { nr = s.n_ray[i]; kv = s.ukv[i]; dv_fix = s.DV[i]; }
-  const u64 last_key = s.last[i];
-  const i64 sh_fix = s.SH[i], sv_fix = s.SV[i];
+  if (rays) { nr = s.n_ray[i]; kv = s.ukv[i]; dv_fix = s.DV[i]; }
   const u32 cf = (u32)fo, no = (u32)(fo >> 32);
   const float h0 = map[i], v0 = map[C + i], va0 = map[2 * C + i], ti0 = map[4 * C + i], up0 = map[5 * C + i], iu0 = map[6 * C + i];
   float h = h0, v = v0, valid = va0, time = ti0, upper = up0, isup = iu0;
@@ -717,7 +722,7 @@ __device__ __forceinline__ void finalize_cell(const DevCfg& c, float* __restrict
     valid = 1.f; time = 0.f; isup = 0.f;
     upper = __uint_as_float((u32)(last_key & 0xffffffffull));
   }
-  if (rays_ran) {
+  if (rays) {
     const u32 key0 = (isup < 0.5f) ? UKEY_NONE : fkey(upper);
     if (nr > 0) {
       valid = __fadd_rn(valid, (float)unfix32(dv_fix));           // CK.py:250
@@ -737,6 +742,7 @@ __device__ __forceinline__ void finalize_cell(const DevCfg& c, float* __restrict
   }
   if (valid_in < 0.5f) { h = 0.f; v = c.init_var; valid = 0.f; }
   // clear_overlap_map EM.py:393-410
+  const int rr = (int)((u32)i / (u32)c.W), cc = i - rr * c.W;
   if (c.overlap && rr >= c.cell_min && rr < c.cell_max && cc >= c.cell_min && cc < c.cell_max) {
     if (h < hmin || h > hmax) { h = 0.f; v = c.init_var; valid = 0.f; }
     if (upper < hmin || upper > hmax) { upper = 0.f; isup = 0.f; }
@@ -751,15 +757,16 @@ __device__ __forceinline__ void finalize_cell(const DevCfg& c, float* __restrict
   if (cf) { s.SH[i] = 0; s.SV[i] = 0; s.last[i] = 0; }
   if (fo) s.cnt_fo[i] = 0;
   if (nr) { s.DV[i] = 0; s.n_ray[i] = 0; }
-  if (ca) s.cnt_ai[i] = 0;
+  if (pts) s.cnt_ai[i] = 0;                                       // every point that sets the flag counts into cnt_ai
   if (kv != UKEY_NONE) s.ukv[i] = UKEY_NONE;
 }
 
-// V consecutive cells per thread.  A frame touches few cells (< 15 % at config B): the dirty marker (one byte per cell,
-// set by whichever kernel accumulated into the cell's scratch; in sharded frames derived from the all-reduced cnt_all / ukv)
-// selects the full path; everywhere else only the drift shift (EM.py:357) and the reset of invalid cells
-// (CK.py:380-384) remain: 3 planes read, at most 3 written, as vectors.  The cells that need the full path are
-// compacted per warp (shared-memory list) and then finalised one per LANE, so the rare path runs converged.
+// V consecutive cells per thread.  A frame touches few cells (< 15 % at config B): the two markers of a cell (a points
+// byte set by k_index_error, a rays byte set by k_raycast; in sharded frames derived from the all-reduced cnt_all / ukv)
+// select the full path and which scratch groups it reads; everywhere else only the drift shift (EM.py:357) and the reset
+// of invalid cells (CK.py:380-384) remain: 3 planes read, at most 3 written, as vectors.  The cells that need the full
+// path are compacted per warp (shared-memory list, index << 2 | group flags) and then finalised one per LANE, so the rare
+// path runs converged.
 #ifndef FIN_MINB
 #define FIN_MINB 4
 #endif
@@ -775,29 +782,42 @@ k_finalize(const DevCfg c, float* __restrict__ map, const CellScratch s, const F
     if (threadIdx.x == 0) { fs_reset->E = 0; fs_reset->ecnt = 0; fs_reset->nvalid = 0; fs_reset->nkept = 0; }
   }
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int i0 = (blockIdx.x * blockDim.x + threadIdx.x) * V;
+  // blocks in centre-first order (bmid, bmid + 1, bmid - 1, bmid + 2, ...): the map is centred on the robot, so the rows the
+  // frame touches (the points near the sensor, the overlap window) are the middle ones, and their blocks, which take the
+  // full path, start in the first wave instead of finishing the last
+  const int bmid = gridDim.x / 2, boff = (blockIdx.x + 1) / 2;
+  const int blk = (blockIdx.x & 1) ? bmid - boff : bmid + boff;
+  const int i0 = (blk * blockDim.x + threadIdx.x) * V;
   const size_t C = (size_t)c.C;
   const int applied = fs->applied;
   const float shift = fs->shift;
-  u32 full = 0;                                                    // bit j: cell i0 + j takes the full path
+  static_assert(V == 1 || V == 4, "k_finalize: 1 or 4 cells per thread");
+  u32 full = 0, pm = 0, rm = 0;      // bit j: cell i0 + j takes the full path / its points group / its rays group is read
   int r = 0, col0 = 0;
   if (i0 < c.C) {
     r = i0 / c.W; col0 = i0 - r * c.W;                             // V == 4 only when W % 4 == 0: one row per thread
     if (s.dirty) {
-      if (V == 4) {
-        const u32 d = *reinterpret_cast<const u32*>(s.dirty + i0);
-        if (d) {
-          *reinterpret_cast<u32*>(s.dirty + i0) = 0u;
-          full = ((d & 0xffu) ? 1u : 0u) | ((d & 0xff00u) ? 2u : 0u) | ((d & 0xff0000u) ? 4u : 0u) | ((d & 0xff000000u) ? 8u : 0u);
+      unsigned char* mk = s.dirty + 2 * (size_t)i0;                // the V cells' markers: one 8-byte (V = 4) or 2-byte load
+      const u64 d = V == 4 ? *reinterpret_cast<const u64*>(mk) : (u64)*reinterpret_cast<const unsigned short*>(mk);
+      if (d) {
+        if (V == 4) *reinterpret_cast<u64*>(mk) = 0ull; else *reinterpret_cast<unsigned short*>(mk) = 0;
+#pragma unroll
+        for (int j = 0; j < V; j++) {
+          if ((d >> (16 * j)) & 0xffu) pm |= 1u << j;
+          if ((d >> (16 * j + 8)) & 0xffu) rm |= 1u << j;
         }
-      } else {
-        for (int j = 0; j < V; j++) if (s.dirty[i0 + j]) { full |= 1u << j; s.dirty[i0 + j] = 0; }
       }
     } else {
+      // DV and n_ray are only ever accumulated together with a red_min on ukv: ukv != UKEY_NONE covers the rays group
       u64 ca[V]; u32 kv[V];
       ldv64<V>(s.cnt_ai + i0, ca); ldv<V>(s.ukv + i0, kv);
-      for (int j = 0; j < V; j++) if (ca[j] != 0ull || kv[j] != UKEY_NONE) full |= 1u << j;
+      for (int j = 0; j < V; j++) {
+        if (ca[j] != 0ull) pm |= 1u << j;
+        if (kv[j] != UKEY_NONE) rm |= 1u << j;
+      }
     }
+    if (!rays_ran) rm = 0;
+    full = pm | rm;
     if (c.overlap && r >= c.cell_min && r < c.cell_max)            // clear_overlap_map window (EM.py:393-410)
       for (int j = 0; j < V; j++) if (col0 + j >= c.cell_min && col0 + j < c.cell_max) full |= 1u << j;
     if (full != (1u << V) - 1u) {
@@ -833,13 +853,13 @@ k_finalize(const DevCfg c, float* __restrict__ map, const CellScratch s, const F
   const int total = __shfl_sync(0xffffffffu, incl, 31);
   if (total == 0) return;
   int pos = incl - nfull;
-  for (int j = 0; j < V; j++) if ((full >> j) & 1u) s_list[wid][pos++] = i0 + j;
+  for (int j = 0; j < V; j++)      // C <= 2049^2 < 2^23: the index shifted by 2 fits an int
+    if ((full >> j) & 1u) s_list[wid][pos++] = ((i0 + j) << 2) | (int)((pm >> j) & 1u) | (int)(((rm >> j) & 1u) << 1);
   __syncwarp();
   const float hmin = __fsub_rn(fs->overlap_tz, c.overlap_z_f), hmax = __fadd_rn(fs->overlap_tz, c.overlap_z_f);
   for (int e = lane; e < total; e += 32) {
-    const int i = s_list[wid][e];
-    const int rr = i / c.W;
-    finalize_cell(c, map, s, i, rr, i - rr * c.W, applied, shift, hmin, hmax, rays_ran);
+    const int ent = s_list[wid][e];
+    finalize_cell(c, map, s, ent >> 2, applied, shift, hmin, hmax, ent & 1, (ent >> 1) & 1);
   }
 }
 
