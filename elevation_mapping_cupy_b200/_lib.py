@@ -188,6 +188,10 @@ SIGNATURES = {
                                              C.c_void_p, C.c_int64, C.c_int32]),
     "emap_sdf_values": (C.c_int, [C.c_void_p, C.POINTER(EmapSdf), C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
                                   C.c_void_p, C.c_int32]),
+    "emap_inpaint_image": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_double, C.c_int32,
+                                     C.c_void_p, C.c_int32]),
+    "emap_nonlinear_interpolation": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_double, C.c_void_p,
+                                               C.c_int32]),
     "emap_plane_grid_geometry": (C.c_int, [C.c_int64, C.c_int64, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
     "emap_plane_decomposition": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int64,

@@ -218,6 +218,7 @@ struct emap_handle {
     DevBuf<char> block;            // cooperative march's grid
     int grid = 0;
   } inpaint;
+  DevBuf<char> inpaint_image;      // emap_inpaint_image / emap_nonlinear_interpolation: their own inpaint_scratch block
   DevBuf<char> pca_block;          // emap_features_pca: one device block carved by carve_pca
   struct {                         // emap_project_to_planar_regions (grown to the largest call): the device block
     DevBuf<char> block;            // carved by carve_query, the upload of host tables and queries, and the pinned

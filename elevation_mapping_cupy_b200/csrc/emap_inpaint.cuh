@@ -20,6 +20,7 @@
 #pragma once
 #include <math.h>
 #include <stdint.h>
+#include <stdlib.h>
 
 #if defined(__CUDACC__)
 #define IP_HD __host__ __device__ __forceinline__
@@ -389,6 +390,138 @@ IP_HD bool ip_eval_child_fast(const InpaintView& v, int c, int cur, bool first, 
   return changed;
 }
 
+// ---------------------------------------------------------------------------------------------
+// cv2.inpaint(INPAINT_NS) at radius 1 (icvNSInpaintFMM, one 8-bit channel).  The sweep is Telea's -- the same queue and
+// the same FastMarching_solve T update, and at radius 1 Telea's march outside the mask covers no pixel -- so the rounds,
+// children and event order above carry over unchanged; only the per-pixel estimate differs.  It reads T nowhere: each
+// known 4-neighbour n of the filled pixel adds w * value(n) with w = dst * dir, dst = 1 / (|r|^4 + 1), and dir the
+// alignment of r with n's image-gradient estimate (sums of absolute differences of its known 4-neighbours' values).
+// Those neighbours lie within distance 2 of the filled pixel: the same 13-pixel stencil and cached event masks as Telea.
+// Restated from the published routine and pinned against the cv2 binary by tests/test_inpaint_ns_cpu.py (the sequential
+// restatement is tests/ns_inpaint_oracle.py).
+enum { IP_TELEA = 0, IP_NS = 1 };
+
+// One known neighbour n's term: r = (rx, ry) from the filled pixel to n; kd / ku / kr / kl: n's down / up / right / left
+// pixel is known at the event.  The 8-bit values are the ones the reference reads: a, b, cc down the image column lm at
+// rows kp+1, kp, km-1 (its gradI.x), d, e, g along the image row km at columns lp+1, lm, lm-1 (its gradI.y), and n's own
+// value `val`.  Float arithmetic of the x86-64 build (sqrt and fabs resolve to their float overloads).
+IP_HD void ip_ns_term(float rx, float ry, bool kd, bool ku, bool kr, bool kl, int a, int b, int cc, int d, int e, int g,
+                      int val, float& Ia, float& s) {
+  const float vl = IP_FADD(IP_FMUL(rx, rx), IP_FMUL(ry, ry));                     // VectorLength: the SQUARED length
+  const float dst = IP_FDIV(1.0f, IP_FADD(IP_FMUL(vl, vl), 1.0f));
+  float gx, gy;
+  if (kd) gx = ku ? (float)(abs(a - b) + abs(b - cc)) : IP_FMUL((float)abs(a - b), 2.0f);
+  else gx = ku ? IP_FMUL((float)abs(b - cc), 2.0f) : 0.f;
+  if (kr) gy = kl ? (float)(abs(d - e) + abs(e - g)) : IP_FMUL((float)abs(d - e), 2.0f);
+  else gy = kl ? IP_FMUL((float)abs(e - g), 2.0f) : 0.f;
+  gx = -gx;
+  float dir = IP_FADD(IP_FMUL(rx, gx), IP_FMUL(ry, gy));
+  if (fabs((double)dir) <= 0.01) dir = 0.000001f;
+  else dir = fabsf(IP_FDIV(dir, IP_FSQRT(IP_FMUL(vl, IP_FADD(IP_FMUL(gx, gx), IP_FMUL(gy, gy))))));
+  const float w = IP_FMUL(dst, dir);
+  Ia = IP_FADD(Ia, IP_FMUL(w, (float)val));
+  s = IP_FADD(s, w);
+}
+
+// saturate_cast<uchar>((double)Ia / s): cvRound (nearest even) of the double quotient, clamped
+IP_HD uint8_t ip_ns_round(float Ia, float s) {
+  int iv = (int)rint(IP_DDIV((double)Ia, (double)s));                               // Ia / s lies in [0, 255]
+  return (uint8_t)(iv < 0 ? 0 : (iv > 255 ? 255 : iv));
+}
+
+// 8-bit value of IMAGE pixel (row, col) as child c sees it, the coordinates clamped to the image.  Only a one-row or
+// one-column image needs the clamp: the reference's shifted indices then leave the image and it reads memory outside it
+// (its result is not even repeatable between calls there), which this replaces by the nearest image row / column.
+IP_HD int ip_ns_val(const InpaintView& v, int c, int row, int col, int cur) {
+  row = row < 0 ? 0 : (row > v.rows - 3 ? v.rows - 3 : row);
+  col = col < 0 ? 0 : (col > v.cols - 3 ? v.cols - 3 : col);
+  return ip_val(v, c, row + 1, col + 1, cur);
+}
+
+// Border-aware evaluation of child c (any position): the reference's loop over (k, l) in the 3x3 window, of which only
+// the 4-neighbours are within radius 1.
+IP_HD bool ip_eval_child_ns(const InpaintView& v, int c, int cur, float* t_out, uint8_t* val_out) {
+  const int cols = v.cols, rows = v.rows;
+  const int i = c / cols, j = c - i * cols;
+  const IpNb up = ip_at_event(v, c, c - cols, cur), dn = ip_at_event(v, c, c + cols, cur);
+  const IpNb lf = ip_at_event(v, c, c - 1, cur), rt = ip_at_event(v, c, c + 1, cur);
+  float dist = ip_solve(up, lf);
+  { const float d2 = ip_solve(dn, lf); if (d2 < dist) dist = d2; }
+  { const float d3 = ip_solve(up, rt); if (d3 < dist) dist = d3; }
+  { const float d4 = ip_solve(dn, rt); if (d4 < dist) dist = d4; }
+  float Ia = 0.f, s = 1.0e-20f;
+  const int dk[4] = {-1, 0, 0, 1}, dl[4] = {0, -1, 1, 0};
+  for (int n = 0; n < 4; n++) {
+    const int k = i + dk[n], l = j + dl[n];
+    if (!(k > 0 && l > 0 && k < rows - 1 && l < cols - 1)) continue;
+    const IpNb& nb = (n == 0) ? up : (n == 1) ? lf : (n == 2) ? rt : dn;
+    if (!nb.known) continue;
+    // image rows / columns of the reference (UNPADDED coordinates, shifted next to the border)
+    const int km = k - 1 + (k == 1), kp = k - 1 - (k == rows - 2);
+    const int lm = l - 1 + (l == 1), lp = l - 1 - (l == cols - 2);
+    const int x = k * cols + l;
+    const bool kd = ip_at_event(v, c, x + cols, cur).known, ku = ip_at_event(v, c, x - cols, cur).known;
+    const bool kr = ip_at_event(v, c, x + 1, cur).known, kl = ip_at_event(v, c, x - 1, cur).known;
+    ip_ns_term((float)(l - j), (float)(k - i), kd, ku, kr, kl, ip_ns_val(v, c, kp + 1, lm, cur),
+               ip_ns_val(v, c, kp, lm, cur), ip_ns_val(v, c, km - 1, lm, cur), ip_ns_val(v, c, km, lp + 1, cur),
+               ip_ns_val(v, c, km, lm, cur), ip_ns_val(v, c, km, lm - 1, cur), ip_val(v, c, k, l, cur), Ia, s);
+  }
+  const uint8_t iv = ip_ns_round(Ia, s);
+  const bool changed = (dist != v.Tc[cur][c]) || (iv != v.vc[cur][c]);
+  *t_out = dist; *val_out = iv;
+  return changed;
+}
+
+// The same for a child at least 3 pixels from the border (no shifted index applies), gather-then-compute over the 13
+// stencil slots and the cached event masks of ip_eval_child_fast.  Bit-identical to ip_eval_child_ns by construction;
+// tests/native/inpaint_ns_host.cpp cross-checks both.
+IP_HD bool ip_eval_child_ns_fast(const InpaintView& v, int c, int cur, bool first, float* t_out, uint8_t* val_out) {
+  const int cols = v.cols, W = cols - 2;
+  const int off[13] = {0, -cols, -1, 1, cols, -2 * cols, -cols - 1, -cols + 1, -2, 2, cols - 1, cols + 1, 2 * cols};
+  uint8_t VC[13], IM[13];
+  float TT[13], TC[13];
+  const int ci = c / cols, cj = c - ci * cols;
+  const int cimg = (ci - 1) * W + (cj - 1);
+  const int offi[13] = {0, -W, -1, 1, W, -2 * W, -W - 1, -W + 1, -2, 2, W - 1, W + 1, 2 * W};
+#pragma unroll
+  for (int n = 0; n < 13; n++) {                                   // one wave of independent loads
+    const int x = c + off[n];
+    TT[n] = v.T[x]; TC[n] = v.Tc[cur][x]; VC[n] = v.vc[cur][x]; IM[n] = v.img[cimg + offi[n]];
+  }
+  uint32_t m;
+  if (first) { m = ip_child_masks(v, c); v.em[c] = m; } else m = v.em[c];
+  bool kn[13]; float Tn[13]; int val[13];
+  kn[0] = false; Tn[0] = IP_TBIG; val[0] = IM[0];
+#pragma unroll
+  for (int n = 1; n < 13; n++) {
+    const bool earlier = (m >> (16 + n)) & 1u;
+    kn[n] = (m >> n) & 1u;
+    Tn[n] = (kn[n] && !earlier) ? TT[n] : (earlier ? TC[n] : IP_TBIG);
+    val[n] = earlier ? (int)VC[n] : (int)IM[n];
+  }
+  IpNb up, lf, rt, dn;
+  up.known = kn[1]; up.T = Tn[1]; lf.known = kn[2]; lf.T = Tn[2]; rt.known = kn[3]; rt.T = Tn[3]; dn.known = kn[4]; dn.T = Tn[4];
+  float dist = ip_solve(up, lf);
+  { const float d2 = ip_solve(dn, lf); if (d2 < dist) dist = d2; }
+  { const float d3 = ip_solve(up, rt); if (d3 < dist) dist = d3; }
+  { const float d4 = ip_solve(dn, rt); if (d4 < dist) dist = d4; }
+  float Ia = 0.f, s = 1.0e-20f;
+  // per cross neighbour n (order up, left, right, down): slots of ITS left / right / up / down pixel, and r = n - c
+  const int nL[4] = {6, 8, 0, 10}, nR[4] = {7, 0, 9, 11}, nU[4] = {5, 6, 7, 0}, nD[4] = {0, 10, 11, 12};
+  const float rxs[4] = {0.f, -1.f, 1.f, 0.f}, rys[4] = {-1.f, 0.f, 0.f, 1.f};
+#pragma unroll
+  for (int n = 0; n < 4; n++) {
+    const int sl = n + 1;
+    if (!kn[sl]) continue;
+    ip_ns_term(rxs[n], rys[n], kn[nD[n]], kn[nU[n]], kn[nR[n]], kn[nL[n]], val[nD[n]], val[sl], val[nU[n]], val[nR[n]],
+               val[sl], val[nL[n]], val[sl], Ia, s);
+  }
+  const uint8_t iv = ip_ns_round(Ia, s);
+  const bool changed = (dist != TC[0]) || (iv != VC[0]);
+  *t_out = dist; *val_out = iv;
+  return changed;
+}
+
 // =============================================================================================
 #if defined(__CUDACC__)
 #include <cooperative_groups.h>
@@ -477,8 +610,10 @@ __device__ __forceinline__ bool ip_claim(uint8_t* f, int c) {
   }
 }
 
-// The whole fast-marching replay: one cooperative launch, grid barriers between the passes of a round.
+// The whole fast-marching replay: one cooperative launch, grid barriers between the passes of a round.  METHOD selects
+// the per-pixel estimate (IP_TELEA or IP_NS); the rounds are the same for both.
 #define IP_MARCH_THREADS 256
+template <int METHOD>
 __global__ void __launch_bounds__(IP_MARCH_THREADS, 1)
 k_ip_march(InpaintView v, int* __restrict__ heapA, int* __restrict__ heapB, int* __restrict__ children, InpaintCtl* ctl,
            int jacobi_cap) {
@@ -520,7 +655,10 @@ k_ip_march(InpaintView v, int* __restrict__ heapA, int* __restrict__ heapB, int*
       for (int e = gtid; e < nchild; e += gsz) {
         const int c = children[e];
         float t; uint8_t val;
-        changed |= ip_interior(v, c) ? ip_eval_child_fast(v, c, cur, it == 0, &t, &val) : ip_eval_child(v, c, cur, &t, &val);
+        if (METHOD == IP_NS)
+          changed |= ip_interior(v, c) ? ip_eval_child_ns_fast(v, c, cur, it == 0, &t, &val) : ip_eval_child_ns(v, c, cur, &t, &val);
+        else
+          changed |= ip_interior(v, c) ? ip_eval_child_fast(v, c, cur, it == 0, &t, &val) : ip_eval_child(v, c, cur, &t, &val);
         v.Tc[cur ^ 1][c] = t; v.vc[cur ^ 1][c] = val;
       }
       if (changed) atomicOr(&ctl->chg[it % 3], 1);
@@ -556,6 +694,83 @@ k_ip_march(InpaintView v, int* __restrict__ heapA, int* __restrict__ heapB, int*
     p ^= 1;
   }
   if (gtid == 0) { ctl->rounds = round; ctl->max_jacobi = max_j; ctl->not_converged = not_conv; }
+}
+
+// cv2.inpaint's setup for an 8-bit image (rows x cols) and its mask: the image copied in, INSIDE where the mask is
+// non-zero, everything else (padding ring included) KNOWN with T = 1e6.  The control block is zeroed before.
+__global__ void __launch_bounds__(256)
+k_ip_image_init(const uint8_t* __restrict__ img, const uint8_t* __restrict__ mask, InpaintView v) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= v.rows * v.cols) return;
+  const int i = p / v.cols, j = p - i * v.cols, W = v.cols - 2;
+  uint8_t f = IP_KNOWN;
+  if (i >= 1 && j >= 1 && i <= v.rows - 2 && j <= W) {
+    const int ci = (i - 1) * W + (j - 1);
+    v.img[ci] = img[ci];
+    if (mask[ci]) f = IP_INSIDE;
+  }
+  v.f[p] = f; v.T[p] = IP_TBIG; v.ord[p] = IP_ROOT;
+}
+
+// ---- inpainting::nonlinearInterpolation (grid_map_filters_rsl inpainting.cpp:205-242) on a rows x cols grid
+// minCoeffOfFinites / maxCoeffOfFinites and the count of finite cells, into a zeroed control block: mm[0] holds the
+// complement of the lowest order-preserving key (so that 0 means "none", as for mm[1])
+__global__ void __launch_bounds__(256)
+k_ip_finite_range(int C, const float* __restrict__ h, InpaintCtl* ctl) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  unsigned int lo_c = 0u, hi = 0u; int nv = 0;
+  if (i < C && isfinite(h[i])) {
+    const unsigned int u = __float_as_uint(h[i]);
+    hi = (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+    lo_c = ~hi;
+    nv = 1;
+  }
+  lo_c = __reduce_max_sync(0xffffffffu, lo_c); hi = __reduce_max_sync(0xffffffffu, hi); nv = __reduce_add_sync(0xffffffffu, nv);
+  if ((threadIdx.x & 31) == 0 && nv) { atomicMax(&ctl->mm[0], lo_c); atomicMax(&ctl->mm[1], hi); atomicAdd(&ctl->n_valid, nv); }
+}
+
+__device__ __forceinline__ void ip_grid_range(const InpaintCtl* ctl, float& lo, float& hi) {
+  lo = ip_unkey(~ctl->mm[0]); hi = ip_unkey(ctl->mm[1]);
+}
+
+// grid_map_cv's toImage<uchar, 1>(lo, hi) and the inpainting mask (isnan): a NaN cell is INSIDE with image value 0,
+// every other cell is clamped to [lo, hi] and quantised in float, truncated (a NaN quotient -- lo == hi, or an
+// infinite hi - lo -- converts to 0 as on x86).  Nothing finite: lo / hi are +-FLT_MAX, as in the reference.
+__global__ void __launch_bounds__(256)
+k_ip_grid_init(const float* __restrict__ h, InpaintView v, const InpaintCtl* __restrict__ ctl) {
+  const int p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= v.rows * v.cols) return;
+  const int i = p / v.cols, j = p - i * v.cols, W = v.cols - 2;
+  uint8_t f = IP_KNOWN;
+  if (i >= 1 && j >= 1 && i <= v.rows - 2 && j <= W) {
+    const int ci = (i - 1) * W + (j - 1);
+    float lo = 3.402823466e38f, hi = -3.402823466e38f;
+    if (ctl->n_valid) ip_grid_range(ctl, lo, hi);
+    float x = h[ci];
+    uint8_t q = 0;
+    if (x != x) f = IP_INSIDE;
+    else {
+      x = x < lo ? lo : (x > hi ? hi : x);
+      const float r = __fmul_rn(__fdiv_rn(__fsub_rn(x, lo), __fsub_rn(hi, lo)), 255.0f);
+      q = (r == r) ? (uint8_t)(int)r : (uint8_t)0;
+    }
+    v.img[ci] = q;
+  }
+  v.f[p] = f; v.T[p] = IP_TBIG; v.ord[p] = IP_ROOT;
+}
+
+// convertTo(CV_32F, (hi - lo) / 255, lo) -- fused multiply-add, as cv::Mat::convertTo's x86 path computes it -- copied
+// into the NaN cells only; every other cell is the input bit for bit.  Nothing finite: the input.
+__global__ void __launch_bounds__(256)
+k_ip_grid_out(int C, const uint8_t* __restrict__ img, const float* __restrict__ h, float* __restrict__ out,
+              const InpaintCtl* __restrict__ ctl) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= C) return;
+  const float x = h[i];
+  if (x == x || ctl->n_valid == 0) { out[i] = x; return; }
+  float lo, hi;
+  ip_grid_range(ctl, lo, hi);
+  out[i] = __fmaf_rn((float)img[i], __fdiv_rn(__fsub_rn(hi, lo), 255.0f), lo);
 }
 
 // plugins/inpainting.py:60: dst.astype(float32) * (h_max - h_min) / 255 + h_min

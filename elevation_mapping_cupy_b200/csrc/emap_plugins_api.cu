@@ -1,6 +1,7 @@
 // emap_plugins_api.cu -- the plugin calls of the C ABI (include/emap.h): min / max filter, erode, robot-centric
 // elevation, smooth, inpainting and its statistics, semantic filter and traversability, PCA, camera image fusion and
 // map initialisation.
+#include "emap_grid.cuh"
 #include "emap_handle.cuh"
 #include "emap_plugins.cuh"
 #include "emap_inpaint.cuh"
@@ -10,7 +11,7 @@
 
 namespace {
 
-// The inpainting scratch of a W x W map, one block; N = (W + 2)^2 padded pixels.
+// The inpainting scratch of an H x W image (a W x W map), one block; N = (H + 2) * (W + 2) padded pixels.
 struct InpaintScratch {
   InpaintView v;
   int* heap[2];
@@ -19,13 +20,14 @@ struct InpaintScratch {
   size_t bytes;
 };
 
-InpaintScratch inpaint_scratch(int W, void* base) {
-  const size_t N = (size_t)(W + 2) * (W + 2);
+InpaintScratch inpaint_scratch(int H, int W, void* base) {
+  const size_t N = (size_t)(H + 2) * (W + 2);
   Carver b{(uintptr_t)base};
   InpaintScratch s;
-  s.v.rows = s.v.cols = W + 2;
+  s.v.rows = H + 2;
+  s.v.cols = W + 2;
   s.v.f = b.take<uint8_t>(N); s.v.ck = b.take<uint8_t>(N); s.v.vc[0] = b.take<uint8_t>(N); s.v.vc[1] = b.take<uint8_t>(N);
-  s.v.img = b.take<uint8_t>((size_t)W * W);
+  s.v.img = b.take<uint8_t>((size_t)H * W);
   s.v.T = b.take<float>(N); s.v.Tc[0] = b.take<float>(N); s.v.Tc[1] = b.take<float>(N);
   s.v.ord = b.take<uint32_t>(N);
   s.heap[0] = b.take<int>(N); s.heap[1] = b.take<int>(N); s.children = b.take<int>(N);
@@ -33,6 +35,35 @@ InpaintScratch inpaint_scratch(int W, void* base) {
   s.v.em = b.take<uint32_t>(N);
   s.bytes = b.bytes;
   return s;
+}
+InpaintScratch inpaint_scratch(int W, void* base) { return inpaint_scratch(W, W, base); }
+
+// The fast-marching replay of an H x W image whose state k_ip_image_init / k_ip_grid_init and the control block's
+// zeroing have queued: band, band flags and the cooperative march with METHOD's estimate, one CTA per SM.
+template <int METHOD>
+int inpaint_march(emap_handle* h, InpaintScratch& s) {
+  int nb = 0;
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_ip_march<METHOD>, IP_MARCH_THREADS, 0));
+  if (nb < 1) return fail(h, EMAP_ERR_CUDA, "inpainting: the cooperative kernel does not fit on an SM");
+  const int nbN = cdiv((i64)s.v.rows * s.v.cols, 256);
+  k_ip_band<<<nbN, 256, 0, h->stream>>>(s.v, s.heap[0], s.ctl); LAUNCH_CHECK();
+  k_ip_band_flag<<<nbN, 256, 0, h->stream>>>(s.v, (const int*)s.heap[0], s.ctl); LAUNCH_CHECK();
+  int cap = 4096;
+  void* args[] = {(void*)&s.v, (void*)&s.heap[0], (void*)&s.heap[1], (void*)&s.children, (void*)&s.ctl, (void*)&cap};
+  CK(cudaLaunchCooperativeKernel((const void*)k_ip_march<METHOD>, dim3(h->n_sm), dim3(IP_MARCH_THREADS), args, 0, h->stream));
+  h->launches++;
+  return 0;
+}
+
+// cv::inpaint's radius (cvRound, half to even, then at least 1) is 1: the one radius provided
+bool inpaint_radius_ok(double r) { return std::isfinite(r) && std::nearbyint(r) <= 1.0; }
+
+// The block of the image calls, carved for H x W, zeroed when it grows (see emap_inpaint), its control block zeroed.
+int image_scratch(emap_handle* h, int H, int W, InpaintScratch& s) {
+  if (int rc = grow(h, h->inpaint_image, inpaint_scratch(H, W, nullptr).bytes, 0, true)) return rc;
+  s = inpaint_scratch(H, W, h->inpaint_image);
+  CK(cudaMemsetAsync(s.ctl, 0, sizeof(InpaintCtl), h->stream));
+  return 0;
 }
 
 int alloc_plugin_scratch(emap_handle* h) {
@@ -302,7 +333,7 @@ int emap_inpaint(emap_handle* h, const float* elevation, const float* is_valid, 
   if (rc) return rc;
   if (!h->inpaint.grid) {
     int nb = 0;
-    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_ip_march, IP_MARCH_THREADS, 0));
+    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_ip_march<IP_TELEA>, IP_MARCH_THREADS, 0));
     if (nb < 1) return fail(h, EMAP_ERR_CUDA, "emap_inpaint: the cooperative kernel does not fit on an SM");
     h->inpaint.grid = h->n_sm;          // one CTA per SM: the fronts are thin, and a grid barrier costs less with fewer CTAs
   }
@@ -321,10 +352,90 @@ int emap_inpaint(emap_handle* h, const float* elevation, const float* is_valid, 
   {
     int cap = 4096;
     void* args[] = {(void*)&v, (void*)&s.heap[0], (void*)&s.heap[1], (void*)&s.children, (void*)&ctl, (void*)&cap};
-    CK(cudaLaunchCooperativeKernel((const void*)k_ip_march, dim3(h->inpaint.grid), dim3(IP_MARCH_THREADS), args, 0, h->stream));
+    CK(cudaLaunchCooperativeKernel((const void*)k_ip_march<IP_TELEA>, dim3(h->inpaint.grid), dim3(IP_MARCH_THREADS), args, 0, h->stream));
     h->launches++;
   }
   PER_CELL(k_ip_finish, (int)C, (const uint8_t*)v.img, elevation, out, (const InpaintCtl*)ctl);
+  return EMAP_OK;
+}
+
+// cv2.inpaint for one 8-bit channel: Telea (the replay emap_inpaint runs) or Navier-Stokes, radius 1 (include/emap.h)
+int emap_inpaint_image(emap_handle* h, const uint8_t* img, const uint8_t* mask, int64_t rows, int64_t cols,
+                       double radius, int32_t method, uint8_t* out, int32_t on_device) {
+  ENTER(h);
+  const char* e = nullptr;
+  if (!img || !mask || !out) e = "null argument";
+  else if (method != 0 && method != 1) e = "method must be 0 (telea) or 1 (ns)";
+  else if (rows < (method ? 1 : 2) || cols < (method ? 1 : 2) || rows > EMAP_INPAINT_MAX_SIDE || cols > EMAP_INPAINT_MAX_SIDE)
+    e = method ? "rows and cols must be 1 .. EMAP_INPAINT_MAX_SIDE" : "rows and cols must be 2 .. EMAP_INPAINT_MAX_SIDE for telea";
+  else if (!inpaint_radius_ok(radius)) e = "radius must be finite and round to at most 1 (only radius 1 is provided)";
+  if (e) return fail(h, EMAP_ERR_INVALID, (std::string("emap_inpaint_image: ") + e).c_str());
+  NvtxRange nv("emap:inpaint_image");
+  const int H = (int)rows, W = (int)cols;
+  const size_t n = (size_t)H * W, mask_off = (n + 255) & ~(size_t)255;
+  InpaintScratch s;
+  if (int rc = image_scratch(h, H, W, s)) return rc;
+  if (!on_device) {                                // image and mask staged and uploaded in one copy
+    if (int rc = h->lookup.up.room(h, mask_off + n)) return rc;
+    memcpy(h->lookup.up.host, img, n);
+    memcpy(h->lookup.up.host + mask_off, mask, n);
+    if (int rc = h->lookup.up.send(h, mask_off + n)) return rc;
+    img = (const uint8_t*)(char*)h->lookup.up.dev;
+    mask = (const uint8_t*)(h->lookup.up.dev + mask_off);
+  }
+  k_ip_image_init<<<cdiv((i64)s.v.rows * s.v.cols, 256), 256, 0, h->stream>>>(img, mask, s.v); LAUNCH_CHECK();
+  if (int rc = method ? inpaint_march<IP_NS>(h, s) : inpaint_march<IP_TELEA>(h, s)) return rc;
+  if (on_device) {
+    CK(cudaMemcpyAsync(out, s.v.img, n, cudaMemcpyDeviceToDevice, h->stream));
+  } else {
+    if (h->lookup.down.size() < n) CK(h->lookup.down.alloc(n));
+    CK(cudaMemcpyAsync(h->lookup.down, s.v.img, n, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    memcpy(out, h->lookup.down, n);
+  }
+  return EMAP_OK;
+}
+
+// grid_map_filters_rsl's inpainting::nonlinearInterpolation on a caller's grid (include/emap.h)
+int emap_nonlinear_interpolation(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, double inpaint_radius,
+                                 float* out, int32_t out_is_device) {
+  ENTER(h);
+  const char* e = !grid || !out ? "null argument" : gl_check_grid(grid->data, grid->rows, grid->cols, grid->position,
+                                                                 grid->resolution, 1);
+  if (!e && (grid->rows > EMAP_INPAINT_MAX_SIDE || grid->cols > EMAP_INPAINT_MAX_SIDE))
+    e = "rows and cols must be at most EMAP_INPAINT_MAX_SIDE";
+  if (!e && !inpaint_radius_ok(inpaint_radius / grid->resolution))
+    e = "inpaint_radius / resolution must be finite and round to at most 1 (only radius 1 is provided)";
+  if (e) return fail(h, EMAP_ERR_INVALID, (std::string("emap_nonlinear_interpolation: ") + e).c_str());
+  NvtxRange nv("emap:nonlinear_interpolation");
+  const int H = (int)grid->rows, W = (int)grid->cols;
+  const size_t bytes = sizeof(float) * H * W;
+  InpaintScratch s;
+  if (int rc = image_scratch(h, H, W, s)) return rc;
+  // host output goes through the lookups' block
+  if (!out_is_device)
+    if (int rc = grow(h, h->lookup.block, bytes, 0, false)) return rc;
+  const float* data = grid->data;
+  if (!grid_on_device) {
+    if (int rc = h->lookup.up.room(h, bytes)) return rc;
+    memcpy(h->lookup.up.host, data, bytes);
+    if (int rc = h->lookup.up.send(h, bytes)) return rc;
+    data = (const float*)(char*)h->lookup.up.dev;
+  }
+  k_ip_finite_range<<<cdiv((i64)H * W, 256), 256, 0, h->stream>>>(H * W, data, s.ctl); LAUNCH_CHECK();
+  k_ip_grid_init<<<cdiv((i64)s.v.rows * s.v.cols, 256), 256, 0, h->stream>>>(data, s.v, (const InpaintCtl*)s.ctl);
+  LAUNCH_CHECK();
+  if (int rc = inpaint_march<IP_NS>(h, s)) return rc;
+  float* o = out_is_device ? out : (float*)(char*)h->lookup.block;
+  k_ip_grid_out<<<cdiv((i64)H * W, 256), 256, 0, h->stream>>>(H * W, (const uint8_t*)s.v.img, data, o,
+                                                              (const InpaintCtl*)s.ctl);
+  LAUNCH_CHECK();
+  if (!out_is_device) {
+    if (h->lookup.down.size() < bytes) CK(h->lookup.down.alloc(bytes));
+    CK(cudaMemcpyAsync(h->lookup.down, o, bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    memcpy(out, h->lookup.down, bytes);
+  }
   return EMAP_OK;
 }
 

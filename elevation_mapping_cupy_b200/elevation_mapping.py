@@ -853,6 +853,63 @@ class ElevationMap:
         self._lookup_call(self._L.emap_sdf_values, f, f_dev, n, q, ptr(out), device)
         return out
 
+    def inpaint_image(self, image, mask, radius=1, method="ns", out=None):
+        """cv2.inpaint(image, mask, radius, INPAINT_NS or INPAINT_TELEA) for one 8-bit channel, bit for bit, in one
+        library call (emap_inpaint_image; include/emap.h states every step).  `image`, `mask`: (rows, cols) uint8, NumPy
+        or torch CUDA; a pixel is filled where its mask is non-zero.  `radius` is rounded as cv2 rounds it; only radius 1
+        is provided.  `method`: "ns" (Navier-Stokes) or "telea" (at least 2 x 2 pixels).  `out`: None, or a contiguous
+        (rows, cols) uint8 array, written in place.  A CUDA image, mask or `out` keeps everything on the device
+        (stream-ordered, no host synchronisation); host inputs are then uploaded first.  Returns `out`."""
+        methods = {"telea": 0, "ns": 1}
+        if method not in methods:
+            raise ValueError("method must be 'ns' or 'telea'")
+        device = _is_device(image) or _is_device(mask) or (out is not None and _is_device(out))
+        if device:
+            import torch
+            dev = next(a.device for a in (image, mask, out) if a is not None and _is_device(a))
+            image, mask = (torch.as_tensor(a, device=dev).to(torch.uint8).contiguous() for a in (image, mask))
+        else:
+            image, mask = (np.ascontiguousarray(_to_host(a), np.uint8) for a in (image, mask))
+        if image.ndim != 2 or tuple(mask.shape) != tuple(image.shape):
+            raise ValueError("image and mask must be (rows, cols) of the same shape")
+        rows, cols = (int(v) for v in image.shape)
+        mk, ptr = _array_maker(dev if device else None)
+        if out is None:
+            out = mk((rows, cols), "uint8")
+        _check_out({"image": out}, {"image": (rows, cols)}, device)
+        if device:
+            self._after_framework()
+        self._check(self._L.emap_inpaint_image(self._h, ptr(image), ptr(mask), rows, cols, float(radius),
+                                               methods[method], ptr(out), int(device)))
+        if device:
+            self._before_framework()
+        return out
+
+    def nonlinear_interpolation(self, grid, layer="elevation", inpaint_radius=None, out=None):
+        """grid_map_filters_rsl's inpainting::nonlinearInterpolation: the NaN cells of `layer` filled by cv2's
+        Navier-Stokes inpainting of the layer quantised to 8 bits between its finite minimum and maximum, every other cell
+        copied bit for bit, in one library call (emap_nonlinear_interpolation; include/emap.h states every step and the
+        edge cases).  `grid` and `layer` as in max_value_between_locations (a dict of get_submap(s),
+        get_transformed_submap(s), planar_terrain, plane_decomposition or the caller's own).  `inpaint_radius` [m]
+        (None: the grid's resolution) must round to 1 pixel.  `out`: None (on the layer's side), or a contiguous (rows,
+        cols) float32 NumPy array or CUDA tensor, written in place; device output is stream-ordered with no host
+        synchronisation.  Returns `out`."""
+        g, g_dev, _, _, _, _, _ = self._lookup_args(grid, layer, (), 0, None, (), True)
+        device = _is_device(out) if out is not None else g_dev
+        mk, ptr = _array_maker((out.device if out is not None else g._keep.device) if device else None)
+        shape = (int(g.rows), int(g.cols))
+        if out is None:
+            out = mk(shape, "float32")
+        _check_out({"layer": out}, {"layer": shape}, device)
+        radius = float(g.resolution if inpaint_radius is None else inpaint_radius)
+        if device or g_dev:
+            self._after_framework()
+        self._check(self._L.emap_nonlinear_interpolation(self._h, C.byref(g), int(g_dev), radius, ptr(out),
+                                                         int(device)))
+        if device:
+            self._before_framework()
+        return out
+
     def _lookup_args(self, grid, layer, parts, width, out, out_keys, follow_grid=False):
         """What the lookups and the distance field share: the layer's emap_grid (the grid dict's "centre", its
         "resolution" or the map's), the queries as one contiguous (N, width) float64 array (NumPy, or a CUDA tensor when
@@ -1325,7 +1382,7 @@ def _array_maker(device):
 
 def _check_out(out, shapes, device):
     """Every out[k] is a contiguous array of shapes[k] on the call's side (NumPy for host output, CUDA for device)."""
-    dtypes = {"index": "int32", "value": "float64", "volume": "float32"}
+    dtypes = {"index": "int32", "value": "float64", "volume": "float32", "image": "uint8", "layer": "float32"}
     for k, shape in shapes.items():
         a = out[k]
         if tuple(a.shape) != shape or _is_device(a) != device or str(a.dtype).split(".")[-1] != dtypes[k] or not (

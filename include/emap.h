@@ -808,6 +808,41 @@ int emap_signed_distance_field(emap_handle* h, const emap_grid* grid, int32_t gr
                                int64_t n_z, float* out, int64_t capacity, int32_t out_is_device);
 int emap_sdf_values(emap_handle* h, const emap_sdf* field, int32_t field_on_device, int64_t n, const double* points,
                     int32_t points_on_device, double* out, int32_t out_is_device);
+/* ---- inpainting of an 8-bit image and of a grid layer on the device.  DESIGN.md §4c gives the algorithm.  The
+ * handle's map state is not read or changed; the calls use the handle's stream, the lookups' staging and one inpainting
+ * scratch block of their own (grown to the largest image, about 37 bytes per padded pixel).
+ * emap_inpaint_image: cv2.inpaint(img, mask, radius, flags) for one 8-bit channel, bit for bit.  img, mask and out are
+ *  rows x cols bytes, row-major, all three in host (on_device 0) or all three in device memory; a pixel is filled where
+ *  its mask byte is non-zero, every other pixel is copied.  radius is rounded as cv::inpaint does (half to even, then at
+ *  least 1); only radius 1 is provided, so a radius that rounds above 1 is rejected.
+ *   method 0: Telea (INPAINT_TELEA), the device replay emap_inpaint runs; rows and cols >= 2.
+ *   method 1: Navier-Stokes (INPAINT_NS); rows and cols >= 1.  On a one-row or one-column image cv2 reads memory
+ *     outside the image next to its border and its result is not repeatable; there the reads are clamped to the image.
+ *  An image with no masked pixel, or with every pixel masked (no known pixel to start from), comes back unchanged.
+ * emap_nonlinear_interpolation: grid_map_filters_rsl's inpainting::nonlinearInterpolation (inpainting.cpp:205-242) on an
+ *  emap_grid exactly as the lookups take it (host or device, the same checks), into out (rows x cols floats, host or
+ *  device as out_is_device says).  Per call:
+ *   mask = isnan(cell); lo / hi = the lowest / highest finite cell (float);
+ *   image = grid_map_cv's toImage<uchar, 1>(lo, hi) (restated from its published source, not checked against a
+ *     grid_map build): a NaN cell gives 0; every other cell is clamped to [lo, hi] (±inf becomes lo or hi) and gives
+ *     (uchar)(((v - lo) / (hi - lo)) * 255.0f) in float, truncated, a NaN quotient giving 0 (x86's conversion);
+ *   filled = emap_inpaint_image(image, mask, inpaint_radius / resolution, method 1);
+ *   out = fma(filled, (hi - lo) / 255.0f, lo) in float (cv::Mat::convertTo's fused x86 path) in the NaN cells, and
+ *     the input bit for bit in every other cell (±inf cells included: they are not NaN, so they are not masked).
+ *  Edge cases: a grid with no finite cell comes back unchanged (the reference's scale is then -inf and every filled
+ *  value NaN); lo == hi fills every NaN cell with lo (the image is all 0).
+ * Host inputs are staged and uploaded in one copy; host output comes back in one copy and synchronisation.  Device output
+ * is stream-ordered with no host synchronisation.  Kernels: emap_inpaint_image 4 (setup, band, band flags, one
+ * cooperative march), emap_nonlinear_interpolation 6 (the finite range and the image, then those 4, then the write-back).
+ * EMAP_ERR_INVALID, with nothing written or launched: a NULL img, mask or out; rows or cols below 1 (below 2 for method
+ * 0) or above EMAP_INPAINT_MAX_SIDE; a method other than 0 and 1; a radius that is not finite or rounds above 1; for
+ * emap_nonlinear_interpolation everything the lookups reject for their grid, a NULL out, a grid side above
+ * EMAP_INPAINT_MAX_SIDE and an inpaint_radius / resolution that is not finite or rounds above 1. */
+#define EMAP_INPAINT_MAX_SIDE 8192
+int emap_inpaint_image(emap_handle* h, const uint8_t* img, const uint8_t* mask, int64_t rows, int64_t cols,
+                       double radius, int32_t method, uint8_t* out, int32_t on_device);
+int emap_nonlinear_interpolation(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, double inpaint_radius,
+                                 float* out, int32_t out_is_device);
 /* ---- plane decomposition of a caller's grid: PlaneDecompositionPipeline::update's grid map part
  * (ConvexPlaneDecompositionRos.cpp:88-162 without RANSAC refinement) on any grid, such as a window of
  * emap_get_submaps or a new map of emap_get_transformed_submaps, with GridMapPreprocessing's resampling
