@@ -352,9 +352,9 @@ int emap_get_transformed_submaps(emap_handle* h, int32_t n_windows, const double
 
 // The scratch of a window of n cells with `slots` label slots, one block: the window, two image planes (fill / median
 // ping-pong), union-find parents, flags and ranks, fill keys, the planarity masks, scan block sums, the header words,
-// the label statistics and decisions, and the host output's staging (info, plane table, layers, then `extra` bytes
-// that emap_extract_planar_regions stages its tables in).  With the post-processing (emap_planar_terrain) the block
-// also holds its three fp32 planes and the box filter's double row sums, and the staging all EMAP_TERRAIN_LAYERS layers.
+// the label statistics and decisions, and the host outputs (carve_plane_out).  With the post-processing
+// (emap_planar_terrain) the block also holds its three fp32 planes and the box filter's double row sums, and the host
+// outputs all EMAP_TERRAIN_LAYERS layers.
 // n is the larger of the input and the resampled grid (emap_plane_decomposition), n_out the resampled one the staged
 // layers have; a window is not resampled (n == n_out).
 namespace {
@@ -370,11 +370,27 @@ struct PlaneScratch {
   int32_t* info;
   double* planes;
   float* layers;
-  char* extra;
+  double* regions;
+  int32_t* polys;
+  double* verts;
 };
 
+// The host outputs, carved alike at the block's tail and in the pinned staging they are read back into: info, the
+// plane table, the layers, then the region tables at the capacities of `tables` (none if null).
+size_t carve_plane_out(void* base, int64_t n_out, int64_t plane_rows, bool post, const emap_region_out* tables,
+                       PlaneScratch& s) {
+  Carver c{(uintptr_t)base};
+  s.info = c.take<int32_t>(16);
+  s.planes = c.take<double>(7 * plane_rows);
+  s.layers = c.take<float>((post ? EMAP_TERRAIN_LAYERS : 4) * n_out);
+  s.regions = c.take<double>(tables ? RG_ROW * tables->regions_capacity : 0);
+  s.polys = c.take<int32_t>(tables ? RG_POLY * tables->polygons_capacity : 0);
+  s.verts = c.take<double>(tables ? 2 * tables->vertices_capacity : 0);
+  return c.bytes;
+}
+
 size_t carve_planes(int64_t n, int64_t n_out, int64_t slots, int64_t plane_rows, bool host_out, bool post,
-                    size_t extra, void* base, PlaneScratch& s) {
+                    const emap_region_out* tables, void* base, PlaneScratch& s) {
   Carver c{(uintptr_t)base};
   const int64_t m = std::max(n, slots);
   s.raw = c.take<float>(n); s.img[0] = c.take<float>(n); s.img[1] = c.take<float>(n);
@@ -385,10 +401,7 @@ size_t carve_planes(int64_t n, int64_t n_out, int64_t slots, int64_t plane_rows,
   s.st = c.take<unsigned long long>(slots * PL_STAT);
   s.pp = c.take<float>(post ? 3 * n : 0);
   s.pd = c.take<double>(post ? n : 0);
-  s.info = c.take<int32_t>(host_out ? 16 : 0);
-  s.planes = c.take<double>(host_out ? 7 * plane_rows : 0);
-  s.layers = c.take<float>(host_out ? (post ? EMAP_TERRAIN_LAYERS : 4) * n_out : 0);
-  s.extra = c.take<char>(host_out ? extra : 0);
+  if (host_out) c.bytes += carve_plane_out((void*)(c.base + c.bytes), n_out, plane_rows, post, tables, s);
   return c.bytes;
 }
 
@@ -432,9 +445,9 @@ struct PlaneCall {
   double res = 0.0;
   int64_t n = 0, n_in = 0, slots = 0, plane_rows = 0;
   bool post = false;               // emap_planar_terrain: the post-processing's scratch and layers
+  const emap_region_out* tables = nullptr;   // host output: the region tables to stage (their capacities)
   double ox = 0.0, oy = 0.0;       // the centre of window cell (0, 0)
   PlaneScratch s;
-  size_t used = 0;
   double* dst_planes = nullptr;    // where the plane table is written (the caller's or the staging)
   int32_t* dst_info = nullptr;
 };
@@ -530,12 +543,12 @@ static const char* grid_plane_check(const emap_grid& g, int32_t grid_on_device, 
 
 // The segmentation of a window that plane_check accepted and found inside the map, or of a grid that grid_plane_check
 // accepted (ConvexPlaneDecompositionRos.cpp:115-149 up to SlidingWindowPlaneExtractor, without RANSAC): the window by
-// k_submap or the grid copied in, the fill and the median on the input, the resampling when the sizes differ
-// (csrc/emap_resample.cuh), then the passes of csrc/emap_planes.cuh on the pipeline's grid, queued on the handle's
-// stream.  With host output the layers, plane table and info go to the staging at the scratch's tail, which also holds
-// `extra` bytes for the caller (c.s.extra).  Layer 0 is the input; a grid's is not written (it is the caller's).
+// k_submap or the caller's grid (staged if on the host), the fill and the median on the input, the resampling when the
+// sizes differ (csrc/emap_resample.cuh), then the passes of csrc/emap_planes.cuh on the pipeline's grid, queued on the
+// handle's stream.  With host output the layers, plane table and info go to the host outputs at the scratch's tail, which also
+// hold the region tables of c.tables.  Layer 0 is the input; a grid's is not written (it is the caller's).
 static int segment_window(emap_handle* h, const emap_plane_params& p, bool out_is_device, float* layers_out,
-                          double* planes_out, int32_t* info, size_t extra, PlaneCall& c) {
+                          double* planes_out, int32_t* info, PlaneCall& c) {
   const int rows = c.rows, cols = c.cols;
   const int64_t n = c.n, n_in = c.n_in, n_scratch = std::max(n, n_in);
   const double res = c.res;
@@ -545,21 +558,17 @@ static int segment_window(emap_handle* h, const emap_plane_params& p, bool out_i
   const int64_t slots = c.slots;
   PlaneScratch& s = c.s;
   int rc = grow(h, h->planes.block,
-                carve_planes(n_scratch, n, slots, c.plane_rows, !out_is_device, c.post, extra, nullptr, s), 0, false);
+                carve_planes(n_scratch, n, slots, c.plane_rows, !out_is_device, c.post, c.tables, nullptr, s), 0, false);
   if (rc) return rc;
-  c.used = carve_planes(n_scratch, n, slots, c.plane_rows, !out_is_device, c.post, extra, h->planes.block, s);
-  if (!out_is_device) {
-    // the pinned staging of the copy back, allocated before anything is launched
-    const size_t bytes = c.used - (size_t)((char*)s.info - (char*)h->planes.block);
-    if (h->planes.host.size() < bytes) CK(h->planes.host.alloc(bytes));
-  }
+  carve_planes(n_scratch, n, slots, c.plane_rows, !out_is_device, c.post, c.tables, h->planes.block, s);
   float* dst = out_is_device ? layers_out : s.layers;
   c.dst_planes = out_is_device ? planes_out : s.planes;
   c.dst_info = out_is_device ? info : s.info;
+  const float* raw = s.raw;
   if (c.grid) {
-    // the caller's grid into s.raw: one copy (a host grid is staged by the driver before the call returns)
-    CK(cudaMemcpyAsync(s.raw, c.grid, sizeof(float) * n_in,
-                       c.grid_on_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, h->stream));
+    // the caller's grid, read in place on the device and from its staged copy if on the host
+    raw = c.grid;
+    if ((rc = stage_inputs(h, h->planes.up, raw, c.grid_on_device ? 0 : sizeof(float) * n_in))) return rc;
   } else {
     // the window: k_submap's elevation layer into s.raw
     SubmapArgs a;
@@ -578,12 +587,12 @@ static int segment_window(emap_handle* h, const emap_plane_params& p, bool out_i
   CK(cudaMemsetAsync(s.st, 0, sizeof(unsigned long long) * slots * PL_STAT, h->stream));
   // fill: minValues' fixed point per NaN component, on the input
   const int ib = cdiv(n_in, PL_THREADS);
-  k_pl_fill_init<<<ib, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, s.hdr, (int)n_in);
+  k_pl_fill_init<<<ib, PL_THREADS, 0, h->stream>>>(raw, s.parent, s.key, s.hdr, (int)n_in);
   LAUNCH_CHECK();
   if ((rc = plane_components(h, s, c.in_rows, c.in_cols, 0))) return rc;
-  k_pl_fill_min<<<ib, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, c.in_rows, c.in_cols);
+  k_pl_fill_min<<<ib, PL_THREADS, 0, h->stream>>>(raw, s.parent, s.key, c.in_rows, c.in_cols);
   LAUNCH_CHECK();
-  k_pl_fill_write<<<ib, PL_THREADS, 0, h->stream>>>(s.raw, s.parent, s.key, s.img[0], (int)n_in);
+  k_pl_fill_write<<<ib, PL_THREADS, 0, h->stream>>>(raw, s.parent, s.key, s.img[0], (int)n_in);
   LAUNCH_CHECK();
   // median, numberOfRepeats times
   const int mk = std::max(1, std::min(p.median_kernel, 5));
@@ -642,16 +651,13 @@ static int segment_window(emap_handle* h, const emap_plane_params& p, bool out_i
   return 0;
 }
 
-// Host output: the staging (info, the plane table, the layers and the caller's extra bytes are the block's tail) in
-// one copy and one synchronisation; the caller's buffers take the layers and planes only when the window had a finite
-// cell.  Returns the staged copy of the scratch in t.
-static int plane_copy_back(emap_handle* h, PlaneCall& c, float* layers_out, double* planes_out, int32_t* info,
+// Host output: the block's tail (carve_plane_out) in one read-back; the caller's buffers take the layers and planes
+// only when the window had a finite cell.  Returns the read-back outputs in t.
+static int plane_copy_back(emap_handle* h, const PlaneCall& c, float* layers_out, double* planes_out, int32_t* info,
                            int n_info, PlaneScratch& t) {
-  const size_t off = (char*)c.s.info - (char*)h->planes.block, bytes = c.used - off;
-  if (h->planes.host.size() < bytes) CK(h->planes.host.alloc(bytes));
-  CK(cudaMemcpyAsync(h->planes.host, c.s.info, bytes, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  carve_planes(std::max(c.n, c.n_in), c.n, c.slots, c.plane_rows, true, c.post, bytes, (char*)h->planes.host - off, t);
+  const size_t bytes = carve_plane_out(nullptr, c.n, c.plane_rows, c.post, c.tables, t);
+  if (int rc = read_back(h, h->planes, c.s.info, bytes)) return rc;
+  carve_plane_out(h->planes.down, c.n, c.plane_rows, c.post, c.tables, t);
   memcpy(info, t.info, n_info * sizeof(int32_t));
   if (info[0]) {
     memcpy(planes_out, t.planes, sizeof(double) * 7 * info[4]);
@@ -680,7 +686,7 @@ int emap_segment_planes(emap_handle* h, const double window[4], const emap_plane
     else memset(info, 0, 5 * sizeof(int32_t));
     return EMAP_OK;
   }
-  int rc = segment_window(h, p, out_is_device, layers_out, planes_out, info, 0, c);
+  int rc = segment_window(h, p, out_is_device, layers_out, planes_out, info, c);
   if (rc) return rc;
   PlaneScratch t;
   if (!out_is_device && (rc = plane_copy_back(h, c, layers_out, planes_out, info, 5, t))) return rc;
@@ -854,17 +860,14 @@ static int planar_regions(emap_handle* h, const char* fn, const double* window, 
     return EMAP_OK;
   }
   const bool regions = c.rows >= 2 && c.cols >= 2;
-  const size_t rb = sizeof(double) * RG_ROW * o.regions_capacity, pb = sizeof(int32_t) * RG_POLY * o.polygons_capacity,
-               vb = sizeof(double) * 2 * o.vertices_capacity;
-  const size_t extra = regions ? ((rb + 255) & ~size_t(255)) + ((pb + 255) & ~size_t(255)) + vb : 0;
-  int rc = segment_window(h, p, out_is_device, layers_out, planes_out, info, extra, c);
+  if (regions) c.tables = &o;
+  int rc = segment_window(h, p, out_is_device, layers_out, planes_out, info, c);
   if (rc) return rc;
   PlaneScratch& s = c.s;
-  char* stage = s.extra;
   RgOut ro;
-  ro.regions = out_is_device ? o.regions : (double*)stage;
-  ro.polys = out_is_device ? o.polygons : (int32_t*)(stage + ((rb + 255) & ~size_t(255)));
-  ro.verts = out_is_device ? o.vertices : (double*)(stage + ((rb + 255) & ~size_t(255)) + ((pb + 255) & ~size_t(255)));
+  ro.regions = out_is_device ? o.regions : s.regions;
+  ro.polys = out_is_device ? o.polygons : s.polys;
+  ro.verts = out_is_device ? o.vertices : s.verts;
   ro.planes = c.dst_planes;
   ro.ox = c.ox;
   ro.oy = c.oy;
@@ -940,10 +943,9 @@ static int planar_regions(emap_handle* h, const char* fn, const double* window, 
     PlaneScratch t;
     if ((rc = plane_copy_back(h, c, layers_out, planes_out, info, 9, t))) return rc;
     if (regions && info[8]) {
-      const char* st = t.extra;
-      memcpy(o.regions, st, sizeof(double) * RG_ROW * info[5]);
-      memcpy(o.polygons, st + ((rb + 255) & ~size_t(255)), sizeof(int32_t) * RG_POLY * info[6]);
-      memcpy(o.vertices, st + ((rb + 255) & ~size_t(255)) + ((pb + 255) & ~size_t(255)), sizeof(double) * 2 * info[7]);
+      memcpy(o.regions, t.regions, sizeof(double) * RG_ROW * info[5]);
+      memcpy(o.polygons, t.polys, sizeof(int32_t) * RG_POLY * info[6]);
+      memcpy(o.vertices, t.verts, sizeof(double) * 2 * info[7]);
     }
   }
   return EMAP_OK;

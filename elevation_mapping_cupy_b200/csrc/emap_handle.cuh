@@ -4,6 +4,7 @@
 // emap_plugins_api.cu (plugins, inpainting, PCA, image fusion, map initialisation).  Each includes the kernel headers of
 // its own area only, so that every kernel is compiled into exactly one module; this header includes none.
 #pragma once
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -84,6 +85,15 @@ struct StagedUpload {
   int send(emap_handle* h, size_t n);      // queues the upload of the first n staged bytes on the handle's stream
 };
 
+// The per-call scratch of one call family: the device block its kernels carve, the upload of its host inputs
+// (stage_inputs, or room / send where a call builds its upload in the staging) and the pinned staging its host outputs
+// come back through (read_back).  Each buffer grows to the family's largest call.
+struct Staging {
+  DevBuf<char> block;
+  StagedUpload up;
+  PinnedBuf<char> down;
+};
+
 // The input of a frame: where its kernels read every sensor's points, and when the caller may reuse its host memory.
 // A frame describes it (kind, rows, the caller's buffers); stage() makes the buffers readable by the kernels, each()
 // hands every sensor's point source to a launch, read_done() follows each pass that reads them, and wait_free()
@@ -123,9 +133,9 @@ struct FrameInput {
 // index / fusion / ray-cast pass queued, or exchange 3 took the upper-bound keys (the finish merges them back first)
 enum class Progress { IDLE, BEGUN, INDEXED, FUSED, RAYS_CAST, KEYS_EXCHANGED };
 
-// sizes of the polygon check's scratch (carve_polygon): upload bytes, partials, column extremes, read-back bytes
+// sizes of the polygon check's device block (carve_polygon): partials, column extremes, read-back bytes
 struct PolySizes {
-  size_t up = 0, items = 0, cols = 0, down = 0;
+  size_t items = 0, cols = 0, down = 0;
 };
 
 struct emap_handle {
@@ -188,28 +198,23 @@ struct emap_handle {
   // class_max scratch (SemMax): per-cell words (cnt, off, occ), control words + bitmaps + U list, the per-record table
   DevBuf<u32> cm_cell, cm_ctl, cm_key, cm_flag;
   DevBuf<i64> cm_sum;
-  // The per-call scratch of the other calls, one member per feature.  Each is allocated on first use and grown by its
-  // own feature only, so a call's growth (and the host synchronisation it costs) never depends on another feature.
+  // The per-call scratch of the other calls.  Each member belongs to one call family, is allocated on first use and is
+  // grown by that family only, so a call's growth (and the host synchronisation it costs) never depends on another's.
   DevBuf<float> d_export;          // host-bound layers and windows, staged on the device (grown to the largest call)
   struct {                         // emap_get_transformed_submaps' per-cell keys (grown to the largest call, zero
     DevBuf<u32> key1;              // between calls: k_tsub_gather resets them)
     DevBuf<u64> key2;
   } tsub;
-  struct {                         // emap_segment_planes (grown to the largest window): one device block carved by
-    DevBuf<char> block;            // carve_planes, and its host output's staging: info, plane table and layers, as one
-    PinnedBuf<char> host;          // copy of the block's tail
-  } planes;
+  Staging planes;                  // emap_segment_planes, the planar regions and terrain, emap_plane_decomposition:
+                                   // the block carved by carve_planes, a host grid, the host outputs (carve_plane_out)
   DevBuf<char> regions;            // emap_extract_planar_regions' scratch (carve_regions), grown to the largest window
   struct {                         // emap_get_map_points / emap_get_normal_arrows: the count and offset tables, the
     DevBuf<int> table;             // kept cells' payload (grown to the largest call) and a pinned word for the count
     DevBuf<char> out;
     PinnedBuf<int> count;
   } mapcloud;
-  struct {                         // the polygon checks (grown to the largest call): one device block carved by
-    DevBuf<char> block;            // carve_polygon, and its pinned host staging (the upload region on the way in, the
-    PolySizes cap{};               // read-back region on the way out)
-    PinnedBuf<char> host;
-  } poly;
+  Staging poly;                    // the polygon checks: the block carved by carve_polygon for poly_cap, the poison
+  PolySizes poly_cap;              // counts, descriptors and clipped vertices (PolyStage), the results and rings
   struct {                         // min / max filter, erode, smooth and the map initialiser's dilation: four planes
     DevBuf<float> plane[4];        // and the per-iteration counters
     DevBuf<int> cnt;
@@ -218,20 +223,15 @@ struct emap_handle {
     DevBuf<char> block;            // cooperative march's grid
     int grid = 0;
   } inpaint;
-  DevBuf<char> inpaint_image;      // emap_inpaint_image / emap_nonlinear_interpolation: their own inpaint_scratch block
+  Staging inpaint_image;           // emap_inpaint_image / emap_nonlinear_interpolation: inpaint_scratch's block (and a
+                                   // host-bound grid), a host image and mask or grid, the host output
   DevBuf<char> pca_block;          // emap_features_pca: one device block carved by carve_pca
-  struct {                         // emap_project_to_planar_regions (grown to the largest call): the device block
-    DevBuf<char> block;            // carved by carve_query, the upload of host tables and queries, and the pinned
-    StagedUpload up;               // staging of host output
-    PinnedBuf<char> down;
-  } query;
-  struct {                         // the grid lookups and the distance field (grown to the largest call): the device
-    DevBuf<char> block;            // block (the lookups' outputs, the field's fill key and host-bound volume),
-    DevBuf<double> rows;           // emap_values_between's host-bound rows, the upload of a host grid or field and
-                                   // queries, and the pinned staging of host output
-    StagedUpload up;
-    PinnedBuf<char> down;
-  } lookup;
+  Staging query;                   // emap_project_to_planar_regions: the block carved by carve_query, host tables and
+                                   // queries, the host outputs
+  Staging lookup;                  // the grid lookups and the distance field: the block (the lookups' outputs, the
+                                   // field's fill key and host-bound volume), a host grid or field and queries, the
+                                   // host outputs
+  DevBuf<double> line_rows;        // emap_values_between's host-bound line offsets, then its rows
   StagedUpload img_up;             // emap_input_image with a host image
   StagedUpload init_up;            // emap_initialize_map's arrays
   // misc
@@ -314,8 +314,10 @@ int grow(emap_handle* h, DevBuf<T>& b, size_t n, size_t slack, bool zero) {
   return 0;
 }
 
-// Waits only for the previous upload (a staged event that was never recorded is complete) and when a buffer grows.
+// Waits only for the previous upload (a staged event that was never recorded is complete; one not yet created is
+// created here) and when a buffer grows.
 inline int StagedUpload::room(emap_handle* h, size_t n) {
+  if (!(cudaEvent_t)staged) CK(staged.create(cudaEventDisableTiming));
   CK(cudaEventSynchronize(staged));
   if (host.size() < n) CK(host.alloc(n));
   return grow(h, dev, n, 0, false);
@@ -339,6 +341,44 @@ struct Carver {
     return p;
   }
 };
+
+// A call's host inputs uploaded through `up` in one copy.  The arguments are (pointer, bytes) pairs, one per input, with
+// 0 bytes for an input already on the device.  The host inputs are laid out by Carver, copied into the staging and sent,
+// and each of their pointers is repointed at its device copy; the caller may reuse its buffers once this returns.
+inline void stage_each(Carver&, size_t&, char*, char*) {}
+template <typename T, typename... More>
+void stage_each(Carver& c, size_t& end, char* host, char* dev, const T*& p, size_t bytes, More&&... more) {
+  if (bytes) {
+    const size_t o = (size_t)c.take<char>(bytes);
+    end = o + bytes;
+    if (host) {
+      memcpy(host + o, p, bytes);
+      p = (const T*)(dev + o);
+    }
+  }
+  stage_each(c, end, host, dev, more...);
+}
+template <typename... Inputs>
+int stage_inputs(emap_handle* h, StagedUpload& up, Inputs&&... in) {
+  Carver layout{0};
+  size_t end = 0;
+  stage_each(layout, end, nullptr, nullptr, in...);
+  if (!end) return 0;
+  if (int rc = up.room(h, end)) return rc;
+  Carver c{0};
+  stage_each(c, end, up.host, up.dev, in...);
+  return up.send(h, end);
+}
+
+// A call's host outputs: `bytes` of device memory at src back into s.down (grown to hold at least `room` bytes) in one
+// copy and one synchronisation.  The caller takes its pieces out of s.down.
+inline int read_back(emap_handle* h, Staging& s, const void* src, size_t bytes, size_t room = 0) {
+  room = std::max(room, bytes);
+  if (s.down.size() < room) CK(s.down.alloc(room));
+  CK(cudaMemcpyAsync(s.down, src, bytes, cudaMemcpyDeviceToHost, h->stream));
+  CK(cudaStreamSynchronize(h->stream));
+  return 0;
+}
 
 // NVTX range around the launches of one stage or call (visible in nsys / ncu timelines; a no-op without a tool attached)
 struct NvtxRange {

@@ -58,10 +58,11 @@ int inpaint_march(emap_handle* h, InpaintScratch& s) {
 // cv::inpaint's radius (cvRound, half to even, then at least 1) is 1: the one radius provided
 bool inpaint_radius_ok(double r) { return std::isfinite(r) && std::nearbyint(r) <= 1.0; }
 
-// The block of the image calls, carved for H x W, zeroed when it grows (see emap_inpaint), its control block zeroed.
-int image_scratch(emap_handle* h, int H, int W, InpaintScratch& s) {
-  if (int rc = grow(h, h->inpaint_image, inpaint_scratch(H, W, nullptr).bytes, 0, true)) return rc;
-  s = inpaint_scratch(H, W, h->inpaint_image);
+// The block of the image calls, carved for H x W with `out_bytes` of host-bound output behind the scratch (at s.bytes),
+// zeroed when it grows (see emap_inpaint), its control block zeroed.
+int image_scratch(emap_handle* h, int H, int W, size_t out_bytes, InpaintScratch& s) {
+  if (int rc = grow(h, h->inpaint_image.block, inpaint_scratch(H, W, nullptr).bytes + out_bytes, 0, true)) return rc;
+  s = inpaint_scratch(H, W, h->inpaint_image.block);
   CK(cudaMemsetAsync(s.ctl, 0, sizeof(InpaintCtl), h->stream));
   return 0;
 }
@@ -372,26 +373,17 @@ int emap_inpaint_image(emap_handle* h, const uint8_t* img, const uint8_t* mask, 
   if (e) return fail(h, EMAP_ERR_INVALID, (std::string("emap_inpaint_image: ") + e).c_str());
   NvtxRange nv("emap:inpaint_image");
   const int H = (int)rows, W = (int)cols;
-  const size_t n = (size_t)H * W, mask_off = (n + 255) & ~(size_t)255;
+  const size_t n = (size_t)H * W;
   InpaintScratch s;
-  if (int rc = image_scratch(h, H, W, s)) return rc;
-  if (!on_device) {                                // image and mask staged and uploaded in one copy
-    if (int rc = h->lookup.up.room(h, mask_off + n)) return rc;
-    memcpy(h->lookup.up.host, img, n);
-    memcpy(h->lookup.up.host + mask_off, mask, n);
-    if (int rc = h->lookup.up.send(h, mask_off + n)) return rc;
-    img = (const uint8_t*)(char*)h->lookup.up.dev;
-    mask = (const uint8_t*)(h->lookup.up.dev + mask_off);
-  }
+  if (int rc = image_scratch(h, H, W, 0, s)) return rc;
+  if (int rc = stage_inputs(h, h->inpaint_image.up, img, on_device ? 0 : n, mask, on_device ? 0 : n)) return rc;
   k_ip_image_init<<<cdiv((i64)s.v.rows * s.v.cols, 256), 256, 0, h->stream>>>(img, mask, s.v); LAUNCH_CHECK();
   if (int rc = method ? inpaint_march<IP_NS>(h, s) : inpaint_march<IP_TELEA>(h, s)) return rc;
   if (on_device) {
     CK(cudaMemcpyAsync(out, s.v.img, n, cudaMemcpyDeviceToDevice, h->stream));
   } else {
-    if (h->lookup.down.size() < n) CK(h->lookup.down.alloc(n));
-    CK(cudaMemcpyAsync(h->lookup.down, s.v.img, n, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    memcpy(out, h->lookup.down, n);
+    if (int rc = read_back(h, h->inpaint_image, s.v.img, n)) return rc;
+    memcpy(out, h->inpaint_image.down, n);
   }
   return EMAP_OK;
 }
@@ -411,30 +403,20 @@ int emap_nonlinear_interpolation(emap_handle* h, const emap_grid* grid, int32_t 
   const int H = (int)grid->rows, W = (int)grid->cols;
   const size_t bytes = sizeof(float) * H * W;
   InpaintScratch s;
-  if (int rc = image_scratch(h, H, W, s)) return rc;
-  // host output goes through the lookups' block
-  if (!out_is_device)
-    if (int rc = grow(h, h->lookup.block, bytes, 0, false)) return rc;
+  if (int rc = image_scratch(h, H, W, out_is_device ? 0 : bytes, s)) return rc;
   const float* data = grid->data;
-  if (!grid_on_device) {
-    if (int rc = h->lookup.up.room(h, bytes)) return rc;
-    memcpy(h->lookup.up.host, data, bytes);
-    if (int rc = h->lookup.up.send(h, bytes)) return rc;
-    data = (const float*)(char*)h->lookup.up.dev;
-  }
+  if (int rc = stage_inputs(h, h->inpaint_image.up, data, grid_on_device ? 0 : bytes)) return rc;
   k_ip_finite_range<<<cdiv((i64)H * W, 256), 256, 0, h->stream>>>(H * W, data, s.ctl); LAUNCH_CHECK();
   k_ip_grid_init<<<cdiv((i64)s.v.rows * s.v.cols, 256), 256, 0, h->stream>>>(data, s.v, (const InpaintCtl*)s.ctl);
   LAUNCH_CHECK();
   if (int rc = inpaint_march<IP_NS>(h, s)) return rc;
-  float* o = out_is_device ? out : (float*)(char*)h->lookup.block;
+  float* o = out_is_device ? out : (float*)(h->inpaint_image.block + s.bytes);
   k_ip_grid_out<<<cdiv((i64)H * W, 256), 256, 0, h->stream>>>(H * W, (const uint8_t*)s.v.img, data, o,
                                                               (const InpaintCtl*)s.ctl);
   LAUNCH_CHECK();
   if (!out_is_device) {
-    if (h->lookup.down.size() < bytes) CK(h->lookup.down.alloc(bytes));
-    CK(cudaMemcpyAsync(h->lookup.down, o, bytes, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    memcpy(out, h->lookup.down, bytes);
+    if (int rc = read_back(h, h->inpaint_image, o, bytes)) return rc;
+    memcpy(out, h->inpaint_image.down, bytes);
   }
   return EMAP_OK;
 }
@@ -541,13 +523,7 @@ int emap_input_image(emap_handle* h, int32_t n_planes, const float* image, int i
   if (n_fused == 0) return EMAP_OK;       // the correspondence alone changes nothing
   const size_t plane_sz = (size_t)height * width, n_img = plane_sz * n_planes;
   const float* img = image;
-  if (!is_device_ptr) {
-    const size_t bytes = sizeof(float) * n_img;
-    if (int rc = h->img_up.room(h, bytes)) return rc;
-    memcpy(h->img_up.host, image, bytes);                // the caller's buffer is free from here on
-    if (int rc = h->img_up.send(h, bytes)) return rc;
-    img = (const float*)(char*)h->img_up.dev;
-  }
+  if (int rc = stage_inputs(h, h->img_up, img, is_device_ptr ? 0 : sizeof(float) * n_img)) return rc;
   for (int k = 0; k < 3; k++) a.center[k] = h->center[k];
   a.res = h->cfg.resolution;
   a.W = h->dc.W; a.C = h->dc.C;

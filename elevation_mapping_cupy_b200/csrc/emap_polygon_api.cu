@@ -10,14 +10,13 @@ constexpr size_t kBatchRingHead = 4096;    // ring rows of a batch read back wit
 // (longer rings take a second copy)
 
 struct PolyScratch {
-  char* up;                        // upload region: poison counts, descriptors, clipped vertices (PolyStage)
   PolyPartial* part;               // one per k_polygon work item
   int *col_min, *col_max;          // the polygons' column windows, back to back
   char* down;                      // read-back region: one PolyResult per polygon, then the rings (PolyStage)
 };
 
-// One call's layout of the upload and read-back regions, the same in device and in pinned host memory, so that each
-// region moves in one copy.  The two poison counts sit at offset 0 of the upload, the results at offset 0 of the read-back.
+// One call's layout of the upload (h->poly.up) and of the read-back region (at the block's tail and in h->poly.down),
+// each moved in one copy.  The two poison counts sit at offset 0 of the upload, the results at offset 0 of the read-back.
 struct PolyStage {
   size_t desc, xy, up_bytes;
   size_t ring, down_bytes;
@@ -37,7 +36,6 @@ dim3 polygon_grid(int W) { return dim3(cdiv(W, PG_COLS), cdiv(W, PG_ROWS)); }
 
 size_t carve_polygon(const PolySizes& z, void* base, PolyScratch& s) {
   Carver b{(uintptr_t)base};
-  s.up = b.take<char>(z.up);
   s.part = b.take<PolyPartial>(z.items);
   s.col_min = b.take<int>(z.cols);
   s.col_max = b.take<int>(z.cols);
@@ -45,28 +43,23 @@ size_t carve_polygon(const PolySizes& z, void* base, PolyScratch& s) {
   return b.bytes;
 }
 
-// Carves the scratch of a call of sizes z, growing the device block and the pinned staging (upload region, then
-// read-back region) to the largest call so far.
+// Carves the device block of a call of sizes z, growing it to the largest call so far.
 int alloc_polygon_scratch(emap_handle* h, const PolySizes& z, PolyScratch& s) {
-  PolySizes& c = h->poly.cap;
-  if (!h->poly.block || z.up > c.up || z.items > c.items || z.cols > c.cols || z.down > c.down) {
-    // the read-back region follows the upload region in pinned memory: keep it aligned for its double2 rings
-    c.up = std::max(c.up, (z.up + 255) & ~(size_t)255); c.items = std::max(c.items, z.items);
-    c.cols = std::max(c.cols, z.cols); c.down = std::max(c.down, z.down);
+  PolySizes& c = h->poly_cap;
+  if (!h->poly.block || z.items > c.items || z.cols > c.cols || z.down > c.down) {
+    c.items = std::max(c.items, z.items); c.cols = std::max(c.cols, z.cols); c.down = std::max(c.down, z.down);
     CK(h->poly.block.alloc(carve_polygon(c, nullptr, s)));
     carve_polygon(c, h->poly.block, s);
     CK(cudaMemsetAsync(s.col_min, 0x7f, sizeof(int) * c.cols, h->stream));    // "no cell yet": k_hull restores it
     CK(cudaMemsetAsync(s.col_max, 0xff, sizeof(int) * c.cols, h->stream));
   }
-  if (h->poly.host.size() < c.up + c.down) CK(h->poly.host.alloc(c.up + c.down));
   carve_polygon(c, h->poly.block, s);
   return 0;
 }
 
-// The device part of a call whose n_poly polygons (n_items work items) are staged in the upload region of h->poly.host:
-// one upload copy, k_poly_poison (with `poison`), k_polygon, k_hull, one copy of the results and the first `head` ring
-// rows into the read-back region of h->poly.host, one synchronisation; one more copy and synchronisation only if a ring
-// ends beyond `head`.
+// The device part of a call whose n_poly polygons (n_items work items) are staged in h->poly.up's host side: one upload
+// copy, k_poly_poison (with `poison`), k_polygon, k_hull, one copy of the results and the first `head` ring rows into
+// h->poly.down, one synchronisation; one more copy and synchronisation only if a ring ends beyond `head`.
 int run_polygons(emap_handle* h, const PolyScratch& s, const PolyStage& st, int n_poly, int n_items, bool poison,
                  const float* checker_plane, double safe_thresh, double safe_min_thresh, int32_t max_unsafe_n,
                  float* mask, bool hulls, size_t head) {
@@ -75,16 +68,17 @@ int run_polygons(emap_handle* h, const PolyScratch& s, const PolyStage& st, int 
   const dim3 g = polygon_grid(W);
   const float* valid = h->map + L_VALID * C;
   const float* checker = checker_plane ? checker_plane : h->map + L_TRAV * C;
+  const char* up = h->poly.up.dev;
   PolyArgs a;
-  a.poly = (const PolyDesc*)(s.up + st.desc); a.n_poly = n_poly; a.xy = (const float2*)(s.up + st.xy);
+  a.poly = (const PolyDesc*)(up + st.desc); a.n_poly = n_poly; a.xy = (const float2*)(up + st.xy);
   a.cx = h->center[0]; a.cy = h->center[1];
   a.thr_over = (float)(1.0 - safe_thresh); a.thr_max = (float)(1.0 - safe_min_thresh);    // traversability_polygon.py:25-26
   a.max_unsafe_n = max_unsafe_n;
-  a.poison = poison ? (const int*)s.up : nullptr;
-  memcpy(&a.one, h->poly.host + st.desc, sizeof(PolyDesc));
-  CK(cudaMemcpyAsync(s.up, h->poly.host, st.up_bytes, cudaMemcpyHostToDevice, h->stream));
+  a.poison = poison ? (const int*)up : nullptr;
+  memcpy(&a.one, h->poly.up.host + st.desc, sizeof(PolyDesc));
+  if (int rc = h->poly.up.send(h, st.up_bytes)) return rc;
   if (poison) {
-    k_poly_poison<<<std::min(cdiv((i64)C, 256), 4 * h->n_sm), 256, 0, h->stream>>>(W, valid, checker, (int*)s.up);
+    k_poly_poison<<<std::min(cdiv((i64)C, 256), 4 * h->n_sm), 256, 0, h->stream>>>(W, valid, checker, (int*)up);
     LAUNCH_CHECK();
   }
   (poison ? k_polygon<true> : k_polygon<false>)<<<n_items, PG_THREADS, 0, h->stream>>>(
@@ -94,12 +88,11 @@ int run_polygons(emap_handle* h, const PolyScratch& s, const PolyStage& st, int 
                                                  s.col_max, (PolyResult*)s.down,
                                                  hulls ? (double2*)(s.down + st.ring) : nullptr);
   LAUNCH_CHECK();
-  char* back = h->poly.host + h->poly.cap.up;
   head = std::min(head, (st.down_bytes - st.ring) / sizeof(double2));
-  CK(cudaMemcpyAsync(back, s.down, st.ring + sizeof(double2) * head, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
+  if (int rc = read_back(h, h->poly, s.down, st.ring + sizeof(double2) * head, st.down_bytes)) return rc;
+  char* back = h->poly.down;
   const PolyResult* r = (const PolyResult*)back;
-  const PolyDesc* d = (const PolyDesc*)(h->poly.host + st.desc);
+  const PolyDesc* d = (const PolyDesc*)(h->poly.up.host + st.desc);
   size_t end = 0;
   for (int i = 0; i < n_poly; i++)
     if (r[i].n_ring) end = std::max(end, (size_t)d[i].ring_off + r[i].n_ring);
@@ -142,13 +135,14 @@ int check_polygons(emap_handle* h, int n_polygons, const int32_t* n_vertices, co
   }
   st = poly_stage(n_polygons, v0, rows);
   PolySizes z;
-  z.up = st.up_bytes; z.items = items; z.cols = cols; z.down = st.down_bytes;
+  z.items = items; z.cols = cols; z.down = st.down_bytes;
   PolyScratch s;
   int rc = alloc_polygon_scratch(h, z, s);
-  if (rc) return rc;
-  memset(h->poly.host, 0, st.desc);                                 // the poison counts start at zero
-  memcpy(h->poly.host + st.desc, desc.data(), sizeof(PolyDesc) * n_polygons);
-  float2* xy = (float2*)(h->poly.host + st.xy);
+  if (rc || (rc = h->poly.up.room(h, st.up_bytes))) return rc;
+  char* up = h->poly.up.host;
+  memset(up, 0, st.desc);                                           // the poison counts start at zero
+  memcpy(up + st.desc, desc.data(), sizeof(PolyDesc) * n_polygons);
+  float2* xy = (float2*)(up + st.xy);
   std::vector<float> area(n_polygons), clipped_area(n_polygons);
   for (int i = 0; i < n_polygons; i++) {
     const PolyDesc& d = desc[i];
@@ -160,7 +154,7 @@ int check_polygons(emap_handle* h, int n_polygons, const int32_t* n_vertices, co
   rc = run_polygons(h, s, st, n_polygons, (int)items, poison, checker_plane, safe_thresh, safe_min_thresh, max_unsafe_n,
                     mask, hulls, head);
   if (rc) return rc;
-  const PolyResult* r = (const PolyResult*)(h->poly.host + h->poly.cap.up);
+  const PolyResult* r = (const PolyResult*)(char*)h->poly.down;
   total = 0;
   for (int i = 0; i < n_polygons; i++) {
     // EM.py:884-887: a polygon (almost) entirely outside the map is unsafe
@@ -176,9 +170,9 @@ int check_polygons(emap_handle* h, int n_polygons, const int32_t* n_vertices, co
 
 // The hull of every polygon of the last check_polygons (layout st) to hull_xy + 2 hull_offsets[i], as (x, y) rows.
 void copy_hulls(emap_handle* h, const PolyStage& st, int n_polygons, const int64_t* hull_offsets, double* hull_xy) {
-  const char* back = h->poly.host + h->poly.cap.up;
+  const char* back = h->poly.down;
   const PolyResult* r = (const PolyResult*)back;
-  const PolyDesc* d = (const PolyDesc*)(h->poly.host + st.desc);
+  const PolyDesc* d = (const PolyDesc*)(h->poly.up.host + st.desc);
   const double2* ring = (const double2*)(back + st.ring);
   for (int i = 0; i < n_polygons; i++) {
     const double2* src = ring + d[i].ring_off;

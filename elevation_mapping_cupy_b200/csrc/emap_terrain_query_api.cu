@@ -59,24 +59,6 @@ const char* check_lookup(const emap_grid* g, int64_t min_cells, int64_t n, const
   return nullptr;
 }
 
-// Host inputs staged and uploaded in one copy: `data_bytes` of data (0: on the device already), then `q_bytes` of
-// queries (0: likewise); data and q are pointed at their device copies.
-int stage_inputs(emap_handle* h, const void*& data, size_t data_bytes, const double*& q, size_t q_bytes) {
-  const size_t q_off = (data_bytes + 255) & ~(size_t)255;
-  if (!data_bytes && !q_bytes) return 0;
-  const size_t up = q_off + q_bytes;
-  if (int rc = h->lookup.up.room(h, up)) return rc;
-  if (data_bytes) {
-    memcpy(h->lookup.up.host, data, data_bytes);
-    data = (const void*)(char*)h->lookup.up.dev;
-  }
-  if (q_bytes) {
-    memcpy(h->lookup.up.host + q_off, q, q_bytes);
-    q = (const double*)(h->lookup.up.dev + q_off);
-  }
-  return h->lookup.up.send(h, up);
-}
-
 // The grid and queries as the kernels read them: a host grid and host queries (per_query doubles each) staged and
 // uploaded in one copy.
 int lookup_inputs(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, int64_t n, const double* queries,
@@ -88,21 +70,10 @@ int lookup_inputs(emap_handle* h, const emap_grid* grid, int32_t grid_on_device,
     g.pos[a] = grid->position[a];
     g.len[a] = (double)(a ? grid->cols : grid->rows) * grid->resolution;
   }
+  g.data = grid->data;
   q = queries;
-  const void* data = grid->data;
-  const size_t grid_bytes = grid_on_device ? 0 : sizeof(float) * grid->rows * grid->cols;
-  const size_t q_bytes = queries_on_device ? 0 : sizeof(double) * per_query * n;
-  const int rc = stage_inputs(h, data, grid_bytes, q, q_bytes);
-  g.data = (const float*)data;
-  return rc;
-}
-
-// Host output: `bytes` of the device block back into the pinned staging, one synchronisation.
-int lookup_back(emap_handle* h, size_t bytes) {
-  if (h->lookup.down.size() < bytes) CK(h->lookup.down.alloc(bytes));
-  CK(cudaMemcpyAsync(h->lookup.down, h->lookup.block, bytes, cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  return 0;
+  return stage_inputs(h, h->lookup.up, g.data, grid_on_device ? 0 : sizeof(float) * grid->rows * grid->cols, q,
+                      queries_on_device ? 0 : sizeof(double) * per_query * n);
 }
 
 // The volumes the field calls accept, after the lookups' grid checks: nullptr, or why not
@@ -142,43 +113,20 @@ int emap_project_to_planar_regions(emap_handle* h, const emap_region_tables* tab
   if (n_queries == 0) return EMAP_OK;
   NvtxRange nv("project_to_planar_regions");
   const int64_t N = n_queries, R = tables->n_regions;
-  // uploads: the host tables and the host queries, back to back in one staged copy
-  const size_t tab_bytes[3] = {sizeof(double) * PQ_ROW * R, sizeof(int32_t) * PQ_POLY * tables->n_polygons,
-                               sizeof(double) * 2 * tables->n_vertices};
-  size_t up_off[4] = {0, 0, 0, 0};     // regions, polygons, vertices, queries
-  size_t up = 0;
-  for (int k = 0; k < 4; k++) {
-    up_off[k] = up;
-    if (k < 3 ? !tables_on_device : !queries_on_device)
-      up = (up + (k < 3 ? tab_bytes[k] : sizeof(double) * 3 * N) + 255) & ~(size_t)255;
-  }
   const size_t pt_bytes = sizeof(double) * 6 * N, cv_bytes = sizeof(double) * 5 * n_convex * N;
   const size_t back_bytes = out_is_device ? 0 : pt_bytes + cv_bytes + sizeof(int32_t) * 3 * N;
   QueryScratch s;
   const size_t need = carve_query(nullptr, R, back_bytes, s);
   if (int rc = grow(h, h->query.block, need, 0, false)) return rc;
   carve_query(h->query.block, R, back_bytes, s);
-  if (!out_is_device && h->query.down.size() < back_bytes) CK(h->query.down.alloc(back_bytes));
   PqTables t{tables->regions, tables->polygons, tables->vertices, R, tables->n_polygons, tables->n_vertices};
   const double* q = queries;
-  if (up) {
-    if (int rc = h->query.up.room(h, up)) return rc;
-    char* st = h->query.up.host;
-    char* dev = h->query.up.dev;
-    if (!tables_on_device) {
-      memcpy(st + up_off[0], tables->regions, tab_bytes[0]);
-      memcpy(st + up_off[1], tables->polygons, tab_bytes[1]);
-      memcpy(st + up_off[2], tables->vertices, tab_bytes[2]);
-      t.regions = (const double*)(dev + up_off[0]);
-      t.polygons = (const int32_t*)(dev + up_off[1]);
-      t.vertices = (const double*)(dev + up_off[2]);
-    }
-    if (!queries_on_device) {
-      memcpy(st + up_off[3], queries, sizeof(double) * 3 * N);
-      q = (const double*)(dev + up_off[3]);
-    }
-    if (int rc = h->query.up.send(h, up)) return rc;
-  }
+  const bool host_tables = !tables_on_device;
+  if (int rc = stage_inputs(h, h->query.up, t.regions, host_tables ? sizeof(double) * PQ_ROW * R : 0, t.polygons,
+                            host_tables ? sizeof(int32_t) * PQ_POLY * t.n_polygons : 0, t.vertices,
+                            host_tables ? sizeof(double) * 2 * t.n_vertices : 0, q,
+                            queries_on_device ? 0 : sizeof(double) * 3 * N))
+    return rc;
   double* point = out_is_device ? out->point : (double*)s.back;
   double* convex = !n_convex ? nullptr : out_is_device ? out->convex : (double*)(s.back + pt_bytes);
   int32_t* index = out_is_device ? out->index : (int32_t*)(s.back + pt_bytes + cv_bytes);
@@ -198,8 +146,7 @@ int emap_project_to_planar_regions(emap_handle* h, const emap_region_tables* tab
     LAUNCH_CHECK();
   }
   if (!out_is_device) {
-    CK(cudaMemcpyAsync(h->query.down, s.back, back_bytes, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    if (int rc = read_back(h, h->query, s.back, back_bytes)) return rc;
     memcpy(out->point, h->query.down, pt_bytes);
     if (n_convex) memcpy(out->convex, h->query.down + pt_bytes, cv_bytes);
     memcpy(out->index, h->query.down + pt_bytes + cv_bytes, sizeof(int32_t) * 3 * N);
@@ -228,7 +175,7 @@ int emap_max_values_between(emap_handle* h, const emap_grid* grid, int32_t grid_
   k_gl_max<<<cdiv(N, GL_WARPS), 32 * GL_WARPS, 0, h->stream>>>(g, q, N, index, value);
   LAUNCH_CHECK();
   if (!out_is_device) {
-    if (int rc = lookup_back(h, vb + ib)) return rc;
+    if (int rc = read_back(h, h->lookup, h->lookup.block, vb + ib)) return rc;
     memcpy(out->value, h->lookup.down, vb);
     memcpy(out->index, h->lookup.down + vb, ib);
   }
@@ -257,25 +204,16 @@ int emap_values_between(emap_handle* h, const emap_grid* grid, int32_t grid_on_d
   }
   NvtxRange nv("values_between");
   const int64_t N = n_queries, nb = cdiv(N, GL_WARPS);
-  // the block: per-block sums (then offsets), then what host output copies back in one piece: info, first, counts
+  // the block: per-block sums (then offsets), then what host output copies back first, in one piece: info, counts
   Carver c0{0};
   c0.take<int64_t>(nb);
-  const size_t back0 = c0.bytes;
   c0.take<int64_t>(2);
-  c0.take<int64_t>(N);
   c0.take<int32_t>(N);
   if (int rc = grow(h, h->lookup.block, c0.bytes, 0, false)) return rc;
   Carver c{(uintptr_t)(char*)h->lookup.block};
   int64_t* block_sum = c.take<int64_t>(nb);
-  int64_t* info = c.take<int64_t>(2);
-  int64_t* first = c.take<int64_t>(N);
-  int32_t* counts = c.take<int32_t>(N);
-  const size_t back_bytes = c.bytes - back0;
-  if (out_is_device) {
-    info = out->info;
-    first = out->first;
-    counts = out->counts;
-  }
+  int64_t* info = out_is_device ? out->info : c.take<int64_t>(2);
+  int32_t* counts = out_is_device ? out->counts : c.take<int32_t>(N);
   GlGrid g;
   const double* q;
   if (int rc = lookup_inputs(h, grid, grid_on_device, N, lines, lines_on_device, 4, g, q)) return rc;
@@ -284,30 +222,23 @@ int emap_values_between(emap_handle* h, const emap_grid* grid, int32_t grid_on_d
   k_gl_scan<<<1, GL_SCAN_THREADS, 0, h->stream>>>(block_sum, nb, out->capacity, info);
   LAUNCH_CHECK();
   if (out_is_device) {
-    k_gl_values<<<nb, 32 * GL_WARPS, 0, h->stream>>>(g, q, N, counts, block_sum, info, first, out->rows);
+    k_gl_values<<<nb, 32 * GL_WARPS, 0, h->stream>>>(g, q, N, counts, block_sum, info, out->first, out->rows);
     LAUNCH_CHECK();
     return EMAP_OK;
   }
-  // host output: the total sizes the rows' staging, then the rows and the per-line words come back together
-  int64_t tc[2];
-  CK(cudaMemcpyAsync(tc, info, sizeof(tc), cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  const size_t row_doubles = tc[1] ? 3 * (size_t)tc[0] : 0;
-  if (int rc = grow(h, h->lookup.rows, row_doubles, 0, false)) return rc;
-  k_gl_values<<<nb, 32 * GL_WARPS, 0, h->stream>>>(g, q, N, counts, block_sum, info, first, h->lookup.rows);
+  // host output: info and the counts come back first, and the total sizes the second buffer; then the line offsets
+  // and the rows, which k_gl_values writes into it back to back, come back together
+  if (int rc = read_back(h, h->lookup, info, (char*)(counts + N) - (char*)info)) return rc;
+  memcpy(out->info, h->lookup.down, 2 * sizeof(int64_t));
+  memcpy(out->counts, h->lookup.down + ((char*)counts - (char*)info), sizeof(int32_t) * N);
+  const size_t row_doubles = out->info[1] ? 3 * (size_t)out->info[0] : 0;
+  if (int rc = grow(h, h->line_rows, N + row_doubles, 0, false)) return rc;
+  k_gl_values<<<nb, 32 * GL_WARPS, 0, h->stream>>>(g, q, N, counts, block_sum, info, (int64_t*)(double*)h->line_rows,
+                                                   h->line_rows + N);
   LAUNCH_CHECK();
-  const size_t rows_off = (back_bytes + 255) & ~(size_t)255, total_bytes = rows_off + sizeof(double) * row_doubles;
-  if (h->lookup.down.size() < total_bytes) CK(h->lookup.down.alloc(total_bytes));
-  CK(cudaMemcpyAsync(h->lookup.down, (char*)info, back_bytes, cudaMemcpyDeviceToHost, h->stream));
-  if (row_doubles)
-    CK(cudaMemcpyAsync(h->lookup.down + rows_off, h->lookup.rows, sizeof(double) * row_doubles,
-                       cudaMemcpyDeviceToHost, h->stream));
-  CK(cudaStreamSynchronize(h->stream));
-  const char* d = h->lookup.down;
-  memcpy(out->info, d, 2 * sizeof(int64_t));
-  memcpy(out->first, d + ((char*)first - (char*)info), sizeof(int64_t) * N);
-  memcpy(out->counts, d + ((char*)counts - (char*)info), sizeof(int32_t) * N);
-  if (row_doubles) memcpy(out->rows, d + rows_off, sizeof(double) * row_doubles);
+  if (int rc = read_back(h, h->lookup, h->line_rows, sizeof(double) * (N + row_doubles))) return rc;
+  memcpy(out->first, h->lookup.down, sizeof(int64_t) * N);
+  if (row_doubles) memcpy(out->rows, h->lookup.down + sizeof(int64_t) * N, sizeof(double) * row_doubles);
   return EMAP_OK;
 }
 
@@ -334,7 +265,7 @@ int emap_grid_derivatives(emap_handle* h, const emap_grid* grid, int32_t grid_on
                                                                       curvature ? 1 : 0, index, value);
   LAUNCH_CHECK();
   if (!out_is_device) {
-    if (int rc = lookup_back(h, vb + ib)) return rc;
+    if (int rc = read_back(h, h->lookup, h->lookup.block, vb + ib)) return rc;
     memcpy(out->value, h->lookup.down, vb);
     memcpy(out->index, h->lookup.down + vb, ib);
   }
@@ -357,24 +288,20 @@ int emap_signed_distance_field(emap_handle* h, const emap_grid* grid, int32_t gr
   if (int rc = grow(h, h->lookup.block, vol_off + (out_is_device ? 0 : vol_bytes), 0, false)) return rc;
   uint32_t* key = (uint32_t*)(char*)h->lookup.block;
   int32_t* vol = out_is_device ? (int32_t*)out : (int32_t*)(h->lookup.block + vol_off);
-  const void* data = grid->data;
-  const double* no_q = nullptr;
-  if (int rc = stage_inputs(h, data, grid_on_device ? 0 : sizeof(float) * rows * cols, no_q, 0)) return rc;
+  const float* data = grid->data;
+  if (int rc = stage_inputs(h, h->lookup.up, data, grid_on_device ? 0 : sizeof(float) * rows * cols)) return rc;
   CK(cudaMemsetAsync(key, 0xff, sizeof(uint32_t), h->stream));     // SDF_KEY_NONE
   const int64_t cells = (int64_t)rows * cols;
-  k_sdf_min<<<std::min(cdiv(cells, SDF_THREADS * 8), 1024), SDF_THREADS, 0, h->stream>>>((const float*)data, cells,
-                                                                                           key);
+  k_sdf_min<<<std::min(cdiv(cells, SDF_THREADS * 8), 1024), SDF_THREADS, 0, h->stream>>>(data, cells, key);
   LAUNCH_CHECK();
   k_sdf_cols<<<dim3(rows, nz), SDF_LINE_THREADS, sdf_line_smem(cols), h->stream>>>(
-      (const float*)data, rows, cols, nz, z_min, grid->resolution, key, vol);
+      data, rows, cols, nz, z_min, grid->resolution, key, vol);
   LAUNCH_CHECK();
   k_sdf_rows<<<dim3(cols, nz), SDF_LINE_THREADS, sdf_line_smem(rows), h->stream>>>(rows, cols,
                                                                                   (float)grid->resolution, vol);
   LAUNCH_CHECK();
   if (!out_is_device) {
-    if (h->lookup.down.size() < vol_bytes) CK(h->lookup.down.alloc(vol_bytes));
-    CK(cudaMemcpyAsync(h->lookup.down, vol, vol_bytes, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    if (int rc = read_back(h, h->lookup, vol, vol_bytes)) return rc;
     memcpy(out, h->lookup.down, vol_bytes);
   }
   return EMAP_OK;
@@ -402,17 +329,16 @@ int emap_sdf_values(emap_handle* h, const emap_sdf* field, int32_t field_on_devi
   f.pos[1] = field->position[1];
   f.res = field->resolution;
   f.z_min = field->z_min;
-  const void* data = field->data;
+  f.data = field->data;
   const double* q = points;
-  if (int rc = stage_inputs(h, data, field_on_device ? 0 : sizeof(float) * f.rows * f.cols * f.n_z, q,
+  if (int rc = stage_inputs(h, h->lookup.up, f.data, field_on_device ? 0 : sizeof(float) * f.rows * f.cols * f.n_z, q,
                             points_on_device ? 0 : sizeof(double) * 3 * n))
     return rc;
-  f.data = (const float*)data;
   double* o = out_is_device ? out : (double*)(char*)h->lookup.block;
   k_sdf_values<<<cdiv(n, SDF_THREADS), SDF_THREADS, 0, h->stream>>>(f, q, n, o);
   LAUNCH_CHECK();
   if (!out_is_device) {
-    if (int rc = lookup_back(h, ob)) return rc;
+    if (int rc = read_back(h, h->lookup, h->lookup.block, ob)) return rc;
     memcpy(out, h->lookup.down, ob);
   }
   return EMAP_OK;
