@@ -112,6 +112,9 @@ class EmapExchange(C.Structure):
     _fields_ = [("ptr", C.c_void_p), ("count", C.c_int64), ("kind", C.c_int32)]
 
 
+EMAP_SHARD_MAX_EXCHANGES = 5
+
+
 # every symbol include/emap.h declares, with its argument types
 SIGNATURES = {
     "emap_create": (C.c_int, [C.POINTER(EmapConfig), C.c_int, C.POINTER(C.c_void_p)]),
@@ -138,6 +141,9 @@ SIGNATURES = {
     "emap_stream_wait_for": (C.c_int, [C.c_void_p, C.c_void_p]),
     "emap_shard_begin": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int64,
                                    C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_float]),
+    "emap_shard_begin_depth_images": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(EmapDepthCamera), C.c_int, C.c_int32,
+                                                C.c_void_p, C.c_int32, C.c_float, C.c_float, C.c_int64, C.c_float,
+                                                C.c_float]),
     "emap_shard_scratch_bytes": (C.c_int64, [C.c_void_p]),
     "emap_shard_attach": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]),
     "emap_shard_set_overlap_z": (C.c_int, [C.c_void_p, C.c_float]),
@@ -147,6 +153,9 @@ SIGNATURES = {
     "emap_comm_init": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32]),
     "emap_input_sensors_sharded": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_void_p), C.POINTER(C.c_int64), C.c_int64,
                                              C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_float, C.c_float]),
+    "emap_input_depth_images_sharded": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(EmapDepthCamera), C.c_int, C.c_int32,
+                                                  C.c_void_p, C.c_int32, C.c_float, C.c_float, C.c_int64, C.c_float,
+                                                  C.c_float, C.c_float]),
     "emap_move_to": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
     "emap_move": (C.c_int, [C.c_void_p, C.c_void_p]),
     "emap_clear": (C.c_int, [C.c_void_p]),

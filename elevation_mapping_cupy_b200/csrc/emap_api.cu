@@ -97,6 +97,26 @@ size_t exchange_bytes(size_t C) {
   return carve_exchange(C, nullptr, sc, fs);
 }
 
+bool sem_on(const emap_handle* h) { return h->sem.n_ch > 0 && h->sem_map; }
+
+// The semantic sum planes of h's configuration carved at `base`: the 2^-32 fixed-point planes, then the r, g, b, count
+// planes of each colour channel.  Returns their size (0 without a configuration).
+size_t carve_sem(const emap_handle* h, uintptr_t base, i64*& fsum, u32*& csum) {
+  const size_t C = (size_t)h->dc.C;
+  const bool on = sem_on(h);
+  Carver b{base};
+  fsum = b.take<i64>(on ? C * h->sem_nf : 0);
+  csum = b.take<u32>(on ? 4 * C * h->sem_nc : 0);
+  return b.bytes;
+}
+
+// Where the frame's semantic sums are: the handle's planes, or behind the exchange scratch of an attached block (where
+// every rank's k_sem_sum adds into all replicas)
+void sem_sums(emap_handle* h, i64*& fsum, u32*& csum) {
+  if (h->attached) carve_sem(h, (uintptr_t)h->attach_base + exchange_bytes((size_t)h->dc.C), fsum, csum);
+  else { fsum = h->sem_fsum; csum = h->sem_csum; }
+}
+
 // Moves the exchange scratch of h to `base` in its between-frames state: all zero, upper-bound keys UKEY_NONE.
 cudaError_t place_exchange(emap_handle* h, void* base) {
   const size_t C = (size_t)h->dc.C;
@@ -228,8 +248,15 @@ template <typename Src>
 int launch_sem_sum(emap_handle* h, const Src& src, int s) {
   const i64 n = h->in.n[s];
   if (n <= 0) return 0;
-  k_sem_sum<Src><<<cdiv(n, 256), 256, 0, h->stream>>>(h->dc, h->sem, src, n, (const int*)(h->pidx + h->offs[s]),
-                                                       h->sem_fsum, h->sem_csum, sem_max(h));
+  i64* fsum;
+  u32* csum;
+  sem_sums(h, fsum, csum);
+  if (h->sc.mc_off)
+    k_sem_sum<Src, true><<<cdiv(n, 256), 256, 0, h->stream>>>(h->dc, h->sem, src, n, (const int*)(h->pidx + h->offs[s]),
+                                                              fsum, csum, sem_max(h), h->sc.mc_off);
+  else
+    k_sem_sum<Src, false><<<cdiv(n, 256), 256, 0, h->stream>>>(h->dc, h->sem, src, n, (const int*)(h->pidx + h->offs[s]),
+                                                               fsum, csum, sem_max(h), (i64)0);
   LAUNCH_CHECK();
   return 0;
 }
@@ -392,28 +419,61 @@ __global__ void k_ukey_merge(int C, u32* __restrict__ ukv, const int* __restrict
   ukv[i] = ((u32)x[i]) ^ 0x80000000u;
 }
 
-// The arrays the ranks of a sharded frame reduce after phase 1..3 (kinds: see emap_exchange in emap.h).  Phase 3 first
-// extracts the upper-bound keys in s32 order; without visibility cleanup it exchanges nothing.
-int exchange_list(emap_handle* h, int phase, emap_exchange out[3], int32_t* n_out) {
+// The arrays the ranks of a sharded frame reduce after phase 1..3 (kinds: see emap_exchange in emap.h); returns their
+// count.  Phase 3 lists the upper-bound keys in s32 order (exchange_keys); without visibility cleanup it lists nothing.
+int exchange_list(emap_handle* h, int phase, emap_exchange out[EMAP_SHARD_MAX_EXCHANGES]) {
   const i64 C = h->dc.C;
   if (phase == 1) {          // after begin: counts (CK.py:334,336) and the drift statistics (CK.py:332-333)
     out[0] = {h->sc.cnt_ai, 2 * C, 3};          // two 32-bit counters per cell: an int32 SUM keeps them apart
     out[1] = {&h->fs->E, 2, 0};
-    *n_out = 2;
-  } else if (phase == 2) {   // after fusion: sums, counts, last-writer keys
+    return 2;
+  }
+  if (phase == 2) {          // after fusion: sums, counts (listed second: the only array phase 2 reads), last-writer keys
     out[0] = {h->sc.SH, 2 * C, 0};
     out[1] = {h->sc.cnt_fo, 2 * C, 3};
     out[2] = {h->sc.last, C, 1};
-    *n_out = 3;
-  } else if (h->dc.visibility) {   // after the ray-cast: decrements, counts, upper-bound keys
-    k_ukey_extract<<<cdiv(C, 256), 256, 0, h->stream>>>((int)C, h->sc.ukv, h->ukey_x);
-    LAUNCH_CHECK();
-    out[0] = {h->sc.DV, C, 0};
-    out[1] = {h->sc.n_ray, C, 3};
-    out[2] = {h->ukey_x, C, 2};
-    *n_out = 3;
-    h->progress = Progress::KEYS_EXCHANGED;
-  } else *n_out = 0;
+    int n = 3;
+    if (sem_on(h)) {         // the semantic sums of phase 1, read in phase 3 like the height sums
+      i64* fsum;
+      u32* csum;
+      sem_sums(h, fsum, csum);
+      if (h->sem_nf) out[n++] = {fsum, h->sem_nf * C, 0};
+      if (h->sem_nc) out[n++] = {csum, 4 * h->sem_nc * C, 3};
+    }
+    return n;
+  }
+  if (!h->dc.visibility) return 0;
+  out[0] = {h->sc.DV, C, 0};   // after the ray-cast: decrements, counts, upper-bound keys
+  out[1] = {h->sc.n_ray, C, 3};
+  out[2] = {h->ukey_x, C, 2};
+  return 3;
+}
+
+// Before exchange 3: the upper-bound keys in the s32 order an int32 MIN all-reduce needs (shard_finish merges them back)
+int exchange_keys(emap_handle* h) {
+  if (!h->dc.visibility) return 0;
+  k_ukey_extract<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc.C, h->sc.ukv, h->ukey_x);
+  LAUNCH_CHECK();
+  h->progress = Progress::KEYS_EXCHANGED;
+  return 0;
+}
+
+// A sharded frame's semantic passes: this rank's sums in phase 1, after which the caller may reuse its host input, and
+// the layers from the reduced sums and counts in phase 3, before k_finalize re-zeroes the counts
+int shard_sem_sum(emap_handle* h) {
+  if (!sem_on(h)) return 0;
+  NvtxRange nv("emap:semantic");
+  int rc;
+  if ((rc = h->in.each([h](auto pts, int s) { return launch_sem_sum(h, pts, s); })) || (rc = h->in.read_done(h))) return rc;
+  return h->in.wait_free(h);
+}
+
+int shard_sem_apply(emap_handle* h) {
+  if (!sem_on(h)) return 0;
+  i64* fsum;
+  u32* csum;
+  sem_sums(h, fsum, csum);
+  PER_CELL(k_sem_apply, h->dc, h->sem, (const u64*)h->sc.cnt_fo, fsum, csum, h->sem_map, sem_max(h));
   return 0;
 }
 
@@ -423,7 +483,8 @@ int shard_finish(emap_handle* h) {
     k_ukey_merge<<<cdiv(h->dc.C, 256), 256, 0, h->stream>>>(h->dc.C, h->sc.ukv, h->ukey_x);
     LAUNCH_CHECK();
   }
-  return frame_finish(h);
+  const int rc = shard_sem_apply(h);
+  return rc ? rc : frame_finish(h);
 }
 
 }  // namespace
@@ -542,6 +603,71 @@ int clear_map(emap_handle* h) {
   return EMAP_OK;
 }
 
+// A frame of depth cameras (emap_input_depth_images, its sharded twins): the argument checks, then the frame's input.
+// Its rows are the pixels, camera after camera, so a sharded frame's global_off counts the pixels of lower ranks.
+int depth_begin(emap_handle* h, const char* fn, int32_t n_cameras, const emap_depth_camera* cams, int is_device_ptr,
+                int32_t n_channels, const int32_t* channel_source, int32_t n_features, float confidence_threshold,
+                float max_depth, int64_t global_off, float pn, float on, bool sharded) {
+  char msg[200];
+#define DMSG(text) (snprintf(msg, sizeof(msg), "%s: " text, fn), msg)
+  if (!cams || n_cameras < 1 || n_cameras > EMAP_DEPTH_MAX_CAMERAS)
+    return fail(h, EMAP_ERR_INVALID, DMSG("1 <= n_cameras <= EMAP_DEPTH_MAX_CAMERAS cameras required"));
+  if (n_channels < 0 || n_channels > SEM_MAX_CH || (n_channels > 0 && !channel_source) || n_features < 0 ||
+      n_features > EMAP_DEPTH_MAX_FEATURES)
+    return fail(h, EMAP_ERR_INVALID, DMSG("0..16 channels with their sources, 0..255 feature planes required"));
+  int n_color = 0, n_feat_used = 0;
+  for (int j = 0; j < n_channels; j++) {
+    if (channel_source[j] < -1 || channel_source[j] >= n_features)
+      return fail(h, EMAP_ERR_INVALID, DMSG("a channel source outside [-1, n_features)"));
+    n_color += channel_source[j] == -1;
+    n_feat_used += channel_source[j] >= 0;
+  }
+  if (n_color > 1) return fail(h, EMAP_ERR_INVALID, DMSG("more than one colour channel"));
+  if (h->sem.n_ch > 0 && h->sem_map)
+    for (int k = 0; k < h->sem.n_ch; k++)
+      if (h->sem.col[k] >= 3 + n_channels)
+        return fail(h, EMAP_ERR_INVALID, DMSG("a configured semantic column beyond 3 + n_channels"));
+  int64_t n[EMAP_DEPTH_MAX_CAMERAS];      // at most 16 * 2^24 = 2^28 pixels: below the frame's 2^31 rows
+  float R[9 * EMAP_DEPTH_MAX_CAMERAS], t[3 * EMAP_DEPTH_MAX_CAMERAS];
+  for (int s = 0; s < n_cameras; s++) {
+    const emap_depth_camera& c = cams[s];
+    bool finite = std::isfinite(c.fx) && std::isfinite(c.fy) && c.fx != 0.0 && c.fy != 0.0 && std::isfinite(c.cx) &&
+                  std::isfinite(c.cy);
+    for (int k = 0; k < 9; k++) finite = finite && std::isfinite(c.R[k]);
+    for (int k = 0; k < 3; k++) finite = finite && std::isfinite(c.t[k]);
+    if (!c.depth || c.height <= 0 || c.width <= 0 || (i64)c.height * c.width > (1ll << 24))
+      return fail(h, EMAP_ERR_INVALID, DMSG("a depth image, 0 < height * width <= 2^24 required"));
+    if (!finite) return fail(h, EMAP_ERR_INVALID, DMSG("non-finite or zero fx / fy, or non-finite cx, cy, R, t"));
+    if ((n_color && !c.rgb) || (n_feat_used && !c.features))
+      return fail(h, EMAP_ERR_INVALID, DMSG("a colour channel needs rgb, a feature channel the feature planes"));
+    n[s] = (i64)c.height * c.width;
+    memcpy(R + 9 * s, c.R, sizeof(c.R));
+    memcpy(t + 3 * s, c.t, sizeof(c.t));
+  }
+  i64 N = 0;
+  for (int s = 0; s < n_cameras; s++) N += n[s];
+  if (global_off + N >= (1ll << 31)) return fail(h, EMAP_ERR_INVALID, DMSG("more than 2^31 rows up to this rank's last pixel"));
+#undef DMSG
+  // per camera: depth, confidence, rgb, feature planes (the ones the channels read)
+  FrameInput& in = h->in;
+  in.kind = FrameInput::DEPTH; in.n.assign(n, n + n_cameras);
+  in.bufs.resize(4 * n_cameras); in.bytes.resize(4 * n_cameras); in.cams.assign(n_cameras, DepthSource{});
+  for (int s = 0; s < n_cameras; s++) {
+    const emap_depth_camera& c = cams[s];
+    const size_t P = (size_t)n[s];
+    in.bufs[4 * s] = c.depth; in.bytes[4 * s] = 4 * P;
+    in.bufs[4 * s + 1] = c.confidence; in.bytes[4 * s + 1] = c.confidence ? 4 * P : 0;
+    in.bufs[4 * s + 2] = c.rgb; in.bytes[4 * s + 2] = n_color ? 3 * P : 0;
+    in.bufs[4 * s + 3] = c.features; in.bytes[4 * s + 3] = n_feat_used ? 4 * P * n_features : 0;
+    DepthSource& d = in.cams[s];
+    d.conf = c.confidence; d.plane = n[s]; d.width = c.width;
+    d.conf_min = confidence_threshold; d.max_depth = max_depth;
+    d.fx = c.fx; d.fy = c.fy; d.cx = c.cx; d.cy = c.cy;
+    for (int j = 0; j < n_channels; j++) d.src[j / 8] |= (u64)(channel_source[j] + 1) << (8 * (j % 8));
+  }
+  return frame_start(h, is_device_ptr, R, t, global_off, pn, on, sharded);
+}
+
 // The frame after frame_start: every pass, then the wait after which the caller may reuse its host memory
 int frame_run(emap_handle* h) {
   int rc;
@@ -585,58 +711,8 @@ int emap_input_depth_images(emap_handle* h, int32_t n_cameras, const emap_depth_
                             float confidence_threshold, float max_depth, float pn, float on) {
   ENTER(h);
   if (h->attached) return fail(h, EMAP_ERR_STATE, "handle is attached to a sharded scratch: use the emap_shard_* calls");
-  if (!cams || n_cameras < 1 || n_cameras > EMAP_DEPTH_MAX_CAMERAS)
-    return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: 1 <= n_cameras <= EMAP_DEPTH_MAX_CAMERAS cameras required");
-  if (n_channels < 0 || n_channels > SEM_MAX_CH || (n_channels > 0 && !channel_source) || n_features < 0 ||
-      n_features > EMAP_DEPTH_MAX_FEATURES)
-    return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: 0..16 channels with their sources, 0..255 feature planes required");
-  int n_color = 0, n_feat_used = 0;
-  for (int j = 0; j < n_channels; j++) {
-    if (channel_source[j] < -1 || channel_source[j] >= n_features)
-      return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: a channel source outside [-1, n_features)");
-    n_color += channel_source[j] == -1;
-    n_feat_used += channel_source[j] >= 0;
-  }
-  if (n_color > 1) return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: more than one colour channel");
-  if (h->sem.n_ch > 0 && h->sem_map)
-    for (int k = 0; k < h->sem.n_ch; k++)
-      if (h->sem.col[k] >= 3 + n_channels)
-        return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: a configured semantic column beyond 3 + n_channels");
-  int64_t n[EMAP_DEPTH_MAX_CAMERAS];      // at most 16 * 2^24 = 2^28 pixels: below the frame's 2^31 rows
-  float R[9 * EMAP_DEPTH_MAX_CAMERAS], t[3 * EMAP_DEPTH_MAX_CAMERAS];
-  for (int s = 0; s < n_cameras; s++) {
-    const emap_depth_camera& c = cams[s];
-    bool finite = std::isfinite(c.fx) && std::isfinite(c.fy) && c.fx != 0.0 && c.fy != 0.0 && std::isfinite(c.cx) &&
-                  std::isfinite(c.cy);
-    for (int k = 0; k < 9; k++) finite = finite && std::isfinite(c.R[k]);
-    for (int k = 0; k < 3; k++) finite = finite && std::isfinite(c.t[k]);
-    if (!c.depth || c.height <= 0 || c.width <= 0 || (i64)c.height * c.width > (1ll << 24))
-      return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: a depth image, 0 < height * width <= 2^24 required");
-    if (!finite) return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: non-finite or zero fx / fy, or non-finite cx, cy, R, t");
-    if ((n_color && !c.rgb) || (n_feat_used && !c.features))
-      return fail(h, EMAP_ERR_INVALID, "emap_input_depth_images: a colour channel needs rgb, a feature channel the feature planes");
-    n[s] = (i64)c.height * c.width;
-    memcpy(R + 9 * s, c.R, sizeof(c.R));
-    memcpy(t + 3 * s, c.t, sizeof(c.t));
-  }
-  // per camera: depth, confidence, rgb, feature planes (the ones the channels read)
-  FrameInput& in = h->in;
-  in.kind = FrameInput::DEPTH; in.n.assign(n, n + n_cameras);
-  in.bufs.resize(4 * n_cameras); in.bytes.resize(4 * n_cameras); in.cams.assign(n_cameras, DepthSource{});
-  for (int s = 0; s < n_cameras; s++) {
-    const emap_depth_camera& c = cams[s];
-    const size_t P = (size_t)n[s];
-    in.bufs[4 * s] = c.depth; in.bytes[4 * s] = 4 * P;
-    in.bufs[4 * s + 1] = c.confidence; in.bytes[4 * s + 1] = c.confidence ? 4 * P : 0;
-    in.bufs[4 * s + 2] = c.rgb; in.bytes[4 * s + 2] = n_color ? 3 * P : 0;
-    in.bufs[4 * s + 3] = c.features; in.bytes[4 * s + 3] = n_feat_used ? 4 * P * n_features : 0;
-    DepthSource& d = in.cams[s];
-    d.conf = c.confidence; d.plane = n[s]; d.width = c.width;
-    d.conf_min = confidence_threshold; d.max_depth = max_depth;
-    d.fx = c.fx; d.fy = c.fy; d.cx = c.cx; d.cy = c.cy;
-    for (int j = 0; j < n_channels; j++) d.src[j / 8] |= (u64)(channel_source[j] + 1) << (8 * (j % 8));
-  }
-  const int rc = frame_start(h, is_device_ptr, R, t, 0, pn, on, false);
+  const int rc = depth_begin(h, "emap_input_depth_images", n_cameras, cams, is_device_ptr, n_channels, channel_source,
+                             n_features, confidence_threshold, max_depth, 0, pn, on, false);
   return rc ? rc : frame_run(h);
 }
 
@@ -653,7 +729,7 @@ int semantic_configure(emap_handle* h, const char* fn, int max_kind, int32_t n_c
                        const int32_t* kind, const int32_t* layer, float* semantic_map_device, int32_t n_layers,
                        double average_weight, float* variance_device, int32_t* id_max_device, int32_t n_id_max) {
   char msg[200];
-  if (n_channels <= 0) { h->sem.n_ch = 0; h->sem_map = nullptr; return EMAP_OK; }
+  if (n_channels <= 0) { h->sem.n_ch = 0; h->sem_map = nullptr; h->sem_nf = h->sem_nc = 0; return EMAP_OK; }
   if (n_channels > SEM_MAX_CH || !column || !kind || !layer || !semantic_map_device || n_layers < 1) {
     snprintf(msg, sizeof(msg), "%s: 1..16 channels, non-null arrays and layer buffer", fn);
     return fail(h, EMAP_ERR_INVALID, msg);
@@ -679,11 +755,13 @@ int semantic_configure(emap_handle* h, const char* fn, int max_kind, int32_t n_c
   c.id_max = nm ? id_max_device : nullptr; c.n_id_max = nm ? n_id_max : 0;
   const size_t C = (size_t)h->dc.C;
   int rc;
-  if ((rc = grow(h, h->sem_fsum, C * nf, 0, true)) || (rc = grow(h, h->sem_csum, C * 4 * nc, 0, true))) return rc;
+  // an attached handle keeps its sums in the symmetric block (sem_sums)
+  if (!h->attached && ((rc = grow(h, h->sem_fsum, C * nf, 0, true)) || (rc = grow(h, h->sem_csum, C * 4 * nc, 0, true))))
+    return rc;
   if (nm > 0 && ((rc = grow(h, h->cm_cell, 3 * C, 0, true)) ||
                  (rc = grow(h, h->cm_ctl, (size_t)CM_CTL + (1 + SEM_MAX_CH) * CM_WORDS + 65536, 0, true))))
     return rc;
-  h->sem = c; h->sem_map = semantic_map_device;
+  h->sem = c; h->sem_map = semantic_map_device; h->sem_nf = nf; h->sem_nc = nc;
   return EMAP_OK;
 }
 }  // namespace
@@ -713,23 +791,66 @@ int emap_point_record_device_ptr(emap_handle* h, const int32_t** packed, int64_t
 }
 
 // ---- sharded frame ---------------------------------------------------------------------------
+namespace {
+// What a sharded frame refuses before anything is queued: a class_max channel (its per-cell tables and class set do not
+// reduce as fixed-size sums), and an attached block too small for the sums of the semantic configuration
+int shard_check(emap_handle* h, const char* fn) {
+  char msg[200];
+  if (sem_on(h) && h->sem.n_max > 0) {
+    snprintf(msg, sizeof(msg), "%s: class_max channels are not fused by sharded frames", fn);
+    return fail(h, EMAP_ERR_INVALID, msg);
+  }
+  if (h->attached && h->attach_bytes < emap_shard_scratch_bytes(h)) {
+    snprintf(msg, sizeof(msg), "%s: the semantic configuration outgrew the attached block: attach a block of "
+             "emap_shard_scratch_bytes()", fn);
+    return fail(h, EMAP_ERR_STATE, msg);
+  }
+  return 0;
+}
+
+// A sharded frame after its input is described and staged: NCCL mode indexes at once, an attached handle in phase 0
+// (after the caller's barrier).  The caller may reuse its host input on return, or after phase 1 when the semantic sums
+// read it there.
+int shard_begun(emap_handle* h) {
+  int rc = h->in.wait_free(h);
+  if (rc || h->attached || (rc = frame_index(h))) return rc;
+  return sem_on(h) ? 0 : h->in.wait_free(h);
+}
+}  // namespace
 
 int emap_shard_begin(emap_handle* h, int32_t n_sensors, const void* const* points, const int64_t* n, int64_t row_stride,
                      int dtype, int is_device_ptr, const float* R, const float* t, int64_t global_point_offset, float pn,
                      float on) {
   ENTER(h);
   if (!points || !n || !R || !t) return fail(h, EMAP_ERR_INVALID, "emap_shard_begin: null argument");
-  int rc = frame_begin(h, n_sensors, points, n, row_stride, dtype, is_device_ptr, R, t, global_point_offset, pn, on, true);
-  if (rc || (rc = h->in.wait_free(h))) return rc;
+  int rc;
+  if ((rc = shard_check(h, "emap_shard_begin")) ||
+      (rc = frame_begin(h, n_sensors, points, n, row_stride, dtype, is_device_ptr, R, t, global_point_offset, pn, on, true)))
+    return rc;
   // multicast mode: every rank must have reset its frame scalars before anyone pushes -> the caller runs a
   // cross-rank barrier and then emap_shard_phase(h, 0); NCCL mode: index right away
-  if (h->attached) return 0;
-  return (rc = frame_index(h)) ? rc : h->in.wait_free(h);
+  return shard_begun(h);
+}
+
+int emap_shard_begin_depth_images(emap_handle* h, int32_t n_cameras, const emap_depth_camera* cams, int is_device_ptr,
+                                  int32_t n_channels, const int32_t* channel_source, int32_t n_features,
+                                  float confidence_threshold, float max_depth, int64_t global_point_offset, float pn,
+                                  float on) {
+  ENTER(h);
+  const char* fn = "emap_shard_begin_depth_images";
+  int rc;
+  if ((rc = shard_check(h, fn)) ||
+      (rc = depth_begin(h, fn, n_cameras, cams, is_device_ptr, n_channels, channel_source, n_features,
+                        confidence_threshold, max_depth, global_point_offset, pn, on, true)))
+    return rc;
+  return shard_begun(h);
 }
 
 int64_t emap_shard_scratch_bytes(const emap_handle* h) {
   if (!h) return EMAP_ERR_INVALID;
-  return (int64_t)exchange_bytes((size_t)h->dc.C);
+  i64* fsum;
+  u32* csum;
+  return (int64_t)(exchange_bytes((size_t)h->dc.C) + carve_sem(h, 0, fsum, csum));
 }
 
 int emap_shard_attach(emap_handle* h, void* local_base, void* multicast_base, int64_t bytes) {
@@ -742,6 +863,9 @@ int emap_shard_attach(emap_handle* h, void* local_base, void* multicast_base, in
   // the library's own scratch is released; the symmetric block (owned by the caller) replaces it
   h->xscratch.reset();
   CK(place_exchange(h, local_base));
+  const size_t xb = exchange_bytes((size_t)h->dc.C);       // the semantic sum planes: zero between frames
+  CK(cudaMemsetAsync((char*)local_base + xb, 0, (size_t)bytes - xb, h->stream));
+  h->attach_base = (char*)local_base; h->attach_bytes = bytes;
   h->sc.mc_off = (i64)((char*)multicast_base - (char*)local_base);
   CK(cudaMemcpyAsync(h->fs, &keep, sizeof(keep), cudaMemcpyHostToDevice, h->stream));
   CK(cudaStreamSynchronize(h->stream));
@@ -765,7 +889,16 @@ int emap_shard_exchange(emap_handle* h, int32_t phase, emap_exchange* out, int32
                                 "exchange 3 must follow phase 2"};
   static const Progress after[] = {Progress::IDLE, Progress::INDEXED, Progress::FUSED, Progress::RAYS_CAST};
   if (h->progress != after[phase]) return fail(h, EMAP_ERR_STATE, order[phase]);
-  return exchange_list(h, phase, out, n_out);
+  emap_exchange ex[EMAP_SHARD_MAX_EXCHANGES];
+  const int n = exchange_list(h, phase, ex);
+  if (*n_out < n) {
+    *n_out = n;
+    return fail(h, EMAP_ERR_INVALID, "emap_shard_exchange: capacity below the listed arrays (*n_out: the count needed)");
+  }
+  if (phase == 3) if (int rc = exchange_keys(h)) return rc;
+  std::copy(ex, ex + n, out);
+  *n_out = n;
+  return 0;
 }
 
 int emap_shard_phase(emap_handle* h, int32_t phase) {
@@ -773,11 +906,12 @@ int emap_shard_phase(emap_handle* h, int32_t phase) {
   if (phase == 0) {
     if (h->progress != Progress::BEGUN) return fail(h, EMAP_ERR_STATE, "phase 0 must follow emap_shard_begin on an attached handle");
     const int rc = frame_index(h);
-    return rc ? rc : h->in.wait_free(h);
+    return rc || sem_on(h) ? rc : h->in.wait_free(h);
   }
   if (phase == 1) {
     if (h->progress != Progress::INDEXED) return fail(h, EMAP_ERR_STATE, "phase 1 must follow emap_shard_begin");
-    return frame_fuse(h);
+    const int rc = frame_fuse(h);
+    return rc ? rc : shard_sem_sum(h);
   }
   if (phase == 2) {
     if (h->progress != Progress::FUSED) return fail(h, EMAP_ERR_STATE, "phase 2 must follow phase 1");
@@ -845,10 +979,9 @@ int emap_comm_init(emap_handle* h, const emap_nccl_id* id, int32_t rank, int32_t
 }
 
 static int comm_exchange(emap_handle* h, int phase) {
-  emap_exchange ex[3];
-  int32_t n = 0;
-  int rc = exchange_list(h, phase, ex, &n);
-  if (rc) return rc;
+  emap_exchange ex[EMAP_SHARD_MAX_EXCHANGES];
+  const int n = exchange_list(h, phase, ex);
+  if (phase == 3) if (int rc = exchange_keys(h)) return rc;
   NcclApi& a = nccl_api();
   for (int k = 0; k < n; k++) {
     const int dt = (ex[k].kind == 0 || ex[k].kind == 1) ? kNcclInt64 : kNcclInt32;
@@ -859,24 +992,53 @@ static int comm_exchange(emap_handle* h, int phase) {
   return 0;
 }
 
-// One sharded frame, collective over the communicator of emap_comm_init: this rank's sensors are fused into the
-// replicated grid together with every other rank's (integer NCCL all-reduces between the phases; replicas stay bit-identical).
+// The phases of a sharded frame after its begin, collective over the communicator of emap_comm_init (integer NCCL
+// all-reduces between them; the replicas stay bit-identical)
+static int comm_frame(emap_handle* h, float overlap_sensor_z_absolute) {
+  int rc;
+  h->overlap_override = true; h->overlap_z_override = overlap_sensor_z_absolute - h->center[2];
+  if ((rc = comm_exchange(h, 1)) || (rc = frame_fuse(h)) || (rc = shard_sem_sum(h)) || (rc = comm_exchange(h, 2)) ||
+      (rc = frame_rays(h)) || (rc = comm_exchange(h, 3)))
+    return rc;
+  return shard_finish(h);
+}
+
+static int comm_check(emap_handle* h, const char* fn) {
+  char msg[200];
+  snprintf(msg, sizeof(msg), "%s: call emap_comm_init first", fn);
+  if (!h->nccl_comm) return fail(h, EMAP_ERR_STATE, msg);
+  if (h->attached) return fail(h, EMAP_ERR_STATE, "handle is attached to a multicast scratch: use the emap_shard_* calls");
+  return shard_check(h, fn);
+}
+
+// One sharded frame: this rank's sensors are fused into the replicated grid together with every other rank's.
 int emap_input_sensors_sharded(emap_handle* h, int32_t n_sensors, const void* const* points, const int64_t* n, int64_t row_stride,
                                int dtype, int is_device_ptr, const float* R, const float* t, int64_t global_point_offset,
                                float overlap_sensor_z_absolute, float pn, float on) {
   ENTER(h);
-  if (!h->nccl_comm) return fail(h, EMAP_ERR_STATE, "emap_input_sensors_sharded: call emap_comm_init first");
-  if (h->attached) return fail(h, EMAP_ERR_STATE, "handle is attached to a multicast scratch: use the emap_shard_* calls");
+  int rc;
+  if ((rc = comm_check(h, "emap_input_sensors_sharded"))) return rc;
   if (!points || !n || !R || !t) return fail(h, EMAP_ERR_INVALID, "emap_input_sensors_sharded: null argument");
-  int rc = frame_begin(h, n_sensors, points, n, row_stride, dtype, is_device_ptr, R, t, global_point_offset, pn, on, true);
-  if (rc || (rc = h->in.wait_free(h)) || (rc = frame_index(h)) || (rc = h->in.wait_free(h))) return rc;
-  h->overlap_override = true; h->overlap_z_override = overlap_sensor_z_absolute - h->center[2];
-  if ((rc = comm_exchange(h, 1))) return rc;
-  if ((rc = frame_fuse(h))) return rc;
-  if ((rc = comm_exchange(h, 2))) return rc;
-  if ((rc = frame_rays(h))) return rc;
-  if ((rc = comm_exchange(h, 3))) return rc;
-  return shard_finish(h);
+  if ((rc = frame_begin(h, n_sensors, points, n, row_stride, dtype, is_device_ptr, R, t, global_point_offset, pn, on, true)) ||
+      (rc = shard_begun(h)))
+    return rc;
+  return comm_frame(h, overlap_sensor_z_absolute);
+}
+
+// One sharded frame of this rank's depth cameras (global_point_offset: the pixels of the lower ranks' cameras)
+int emap_input_depth_images_sharded(emap_handle* h, int32_t n_cameras, const emap_depth_camera* cams, int is_device_ptr,
+                                    int32_t n_channels, const int32_t* channel_source, int32_t n_features,
+                                    float confidence_threshold, float max_depth, int64_t global_point_offset,
+                                    float overlap_sensor_z_absolute, float pn, float on) {
+  ENTER(h);
+  const char* fn = "emap_input_depth_images_sharded";
+  int rc;
+  if ((rc = comm_check(h, fn)) ||
+      (rc = depth_begin(h, fn, n_cameras, cams, is_device_ptr, n_channels, channel_source, n_features,
+                        confidence_threshold, max_depth, global_point_offset, pn, on, true)) ||
+      (rc = shard_begun(h)))
+    return rc;
+  return comm_frame(h, overlap_sensor_z_absolute);
 }
 
 // ---- read-backs ------------------------------------------------------------------------------

@@ -185,8 +185,11 @@ struct emap_handle {
   float pos_noise = 0, ori_noise = 0;
   Progress progress = Progress::IDLE;
   bool fused_drift = false;   // single-GPU frame: no k_drift launch (k_fuse decides, k_finalize resets)
-  // multicast-attached scratch (sharded frames over NVLink multicast, emap_shard_attach)
+  // multicast-attached scratch (sharded frames over NVLink multicast, emap_shard_attach): the caller's symmetric block,
+  // the exchange scratch then the semantic sum planes (carve_sem)
   bool attached = false;
+  char* attach_base = nullptr;
+  int64_t attach_bytes = 0;
   // C-side communicator of sharded frames (emap_comm_init): NCCL, loaded at run time
   void* nccl_comm = nullptr;
   int comm_rank = 0, comm_nranks = 1;
@@ -195,6 +198,7 @@ struct emap_handle {
   float* sem_map = nullptr;        // (n_layers, W, W) fp32, device, caller-owned
   DevBuf<i64> sem_fsum;            // one 2^-32 fixed-point sum plane per averaged channel
   DevBuf<u32> sem_csum;            // r, g, b, count planes per colour channel
+  int sem_nf = 0, sem_nc = 0;      // the configuration's averaged and colour channels (its sum planes: sem_fsum, sem_csum)
   // class_max scratch (SemMax): per-cell words (cnt, off, occ), control words + bitmaps + U list, the per-record table
   DevBuf<u32> cm_cell, cm_ctl, cm_key, cm_flag;
   DevBuf<i64> cm_sum;

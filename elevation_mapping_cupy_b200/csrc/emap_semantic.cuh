@@ -16,6 +16,7 @@
 // zeroed everywhere for the later rounds), so it adds its own passes between them, see "class_max" below.  DESIGN §4d
 // defines all three where the reference crashes or degenerates.
 #pragma once
+#include "emap_kernels.cuh"       // red_add
 #include "emap_sources.cuh"
 
 // ---- class_max scratch ------------------------------------------------------------------------------------------------
@@ -52,11 +53,14 @@ __device__ __forceinline__ float cm_value(u32 f, i64 s) {
 
 // scatter: fusion/pointcloud_average.py:41-52 (sum_kernel), fusion/pointcloud_color.py:51-61 (add_color_kernel)
 // fusion/pointcloud_class_bayesian.py alpha_kernel (theta >= 0 only), pointcloud_bayesian_inference.py
-// sum_compact_kernel and pointcloud_class_max.py sum_max_kernel (into the cell's hash table), every (point, channel)
-template <typename Src>
+// sum_compact_kernel and pointcloud_class_max.py sum_max_kernel (into the cell's hash table), every (point, channel).
+// MC (sharded frames on a multicast-attached block): the sums go to every rank's replica through red_add at mc_off;
+// otherwise mc_off is unused and the sums are local atomics.
+template <typename Src, bool MC>
 __global__ void __launch_bounds__(256)
 k_sem_sum(const DevCfg c, const SemCfg sc, const Src src, const i64 n,
-          const int* __restrict__ pidx, i64* __restrict__ fsum, u32* __restrict__ csum, const SemMax ms) {
+          const int* __restrict__ pidx, i64* __restrict__ fsum, u32* __restrict__ csum, const SemMax ms, const i64 mc_off) {
+  const i64 mc = MC ? mc_off : 0;
   const i64 i = blockIdx.x * (i64)blockDim.x + threadIdx.x;
   if (i >= n) return;
   const int rec = pidx[i];
@@ -68,10 +72,10 @@ k_sem_sum(const DevCfg c, const SemCfg sc, const Src src, const i64 n,
     if (sc.kind[k] == SEM_COLOR) {
       const u32 color = __float_as_uint(feat);                    // pointcloud_color.py:56-60
       u32* p = csum + (size_t)sc.slot[k] * C + idx;
-      atomicAdd(p, (color >> 16) & 0xffu);
-      atomicAdd(p + C, (color >> 8) & 0xffu);
-      atomicAdd(p + 2 * C, color & 0xffu);
-      atomicAdd(p + 3 * C, 1u);
+      red_add(p, (color >> 16) & 0xffu, mc);
+      red_add(p + C, (color >> 8) & 0xffu, mc);
+      red_add(p + 2 * C, color & 0xffu, mc);
+      red_add(p + 3 * C, 1u, mc);
     } else if (sc.kind[k] == SEM_CLASS_MAX) {
       const u32 bits = __float_as_uint(feat);                     // decode_max: fp16 probability | class id << 16
       const u32 id = bits >> 16;
@@ -88,7 +92,7 @@ k_sem_sum(const DevCfg c, const SemCfg sc, const Src src, const i64 n,
       else atomicAdd((u64*)(ms.sum + base + s), (u64)__float2ll_rn(__fmul_rn(prob, 16777216.0f)));
     } else {
       if (sc.kind[k] == SEM_CLASS_BAYESIAN && !(feat >= 0.f)) continue;     // alpha_kernel: `if (theta >= theta_max)`
-      atomicAdd((u64*)(fsum + (size_t)sc.slot[k] * C + idx), (u64)fix32(feat));
+      red_add((u64*)(fsum + (size_t)sc.slot[k] * C + idx), (u64)fix32(feat), mc);
     }
   }
 }

@@ -289,8 +289,7 @@ class ElevationMap:
         (torch CUDA / cupy) array.  Channels beyond x, y, z are fused into semantic layers inside the frame
         (semantic_map.py:223-259; algorithms average / class_average / color / class_bayesian / bayesian_inference /
         class_max)."""
-        if channels is not None and (len(channels) > 3 or self.semantic_map._configured is not None):
-            self.semantic_map.configure_for(list(channels))
+        self._configure_cloud_channels(channels)
         Rm = np.ascontiguousarray(_to_host(R), dtype=np.float32).reshape(9)
         tv = np.ascontiguousarray(_to_host(t), dtype=np.float32).reshape(3)
         dev = _device_pointer(raw_points)
@@ -299,6 +298,11 @@ class ElevationMap:
             self._after_framework()       # framework work writing the cloud or reading the aliased layers comes first
             self._check(self._L.emap_input_pointcloud(self._h, ptr, n, row, dt, int(dev is not None), Rm.ctypes.data,
                                                       tv.ctypes.data, float(position_noise), float(orientation_noise)))
+
+    def _configure_cloud_channels(self, channels):
+        """The semantic fusion of a cloud with these channel names (x, y, z first); None keeps the configuration."""
+        if channels is not None and (len(channels) > 3 or self.semantic_map._configured is not None):
+            self.semantic_map.configure_for(list(channels))
 
     # the pure-Python ROS node of the reference still calls `.input(...)` (elevation_mapping_ros.py:212)
     input = input_pointcloud
@@ -332,6 +336,21 @@ class ElevationMap:
         """Several depth cameras of one time slice fused against the same snapshot, as input_sensors fuses clouds.
         `cameras`: dicts with the keys depth, P, R, t and optionally rgb, features, confidence (see input_depth_image);
         `channels` is shared by every camera."""
+        depth = self._depth_frame(cameras, channels)
+        with self.map_lock:
+            self._after_framework()       # framework work writing the images or reading the aliased layers comes first
+            rc = self._L.emap_input_depth_images(self._h, *depth.args, float(confidence_threshold), float(max_depth),
+                                                 float(position_noise), float(orientation_noise))
+            # framework work queued from here on sees the fused map, and the device images (the caller's, or the
+            # converted copies in `keep`, freed on return) are released or rewritten only after the frame has read them
+            # (no host sync)
+            self._before_framework()
+            self._check(rc)
+
+    def _depth_frame(self, cameras, channels):
+        """The depth cameras of one frame as the library takes them (_DepthFrame), with `channels` configured as the
+        extra channels of every camera (the semantic sensor node's rule: the `color` channel reads rgb, the others the
+        feature planes in order)."""
         channels = list(channels)
         if channels or self.semantic_map._configured is not None:
             self.semantic_map.configure_for(["x", "y", "z"] + channels)
@@ -368,16 +387,8 @@ class ElevationMap:
             c.R[:] = np.asarray(_to_host(cam["R"]), np.float32).reshape(9).tolist()
             c.t[:] = np.asarray(_to_host(cam["t"]), np.float32).reshape(3).tolist()
         src = (C.c_int32 * max(len(sources), 1))(*sources)
-        with self.map_lock:
-            self._after_framework()       # framework work writing the images or reading the aliased layers comes first
-            rc = self._L.emap_input_depth_images(self._h, n, cams, int(dev), len(sources), src, n_features,
-                                                 float(confidence_threshold), float(max_depth), float(position_noise),
-                                                 float(orientation_noise))
-            # framework work queued from here on sees the fused map, and the device images (the caller's, or the
-            # converted copies in `keep`, freed on return) are released or rewritten only after the frame has read them
-            # (no host sync)
-            self._before_framework()
-            self._check(rc)
+        return _DepthFrame((n, cams, int(dev), len(sources), src, n_features), keep,
+                           sum(int(c.height) * int(c.width) for c in cams), float(cams[0].t[2]))
 
     # ---- queries -------------------------------------------------------------------------------
     def get_additive_mean_error(self):
@@ -1338,6 +1349,15 @@ class ElevationMap:
                 self._h, pts.ctypes.data, pts.shape[0], INIT_METHODS[method], None if tri is None else tri.ctypes.data,
                 0 if tri is None else tri.shape[0], None if grad is None else grad.ctypes.data,
                 float(self.param.initialized_variance), int(self.param.dilation_size_initialize)))
+
+
+class _DepthFrame:
+    """The depth cameras of one frame: `args` (n_cameras, cameras, is_device_ptr, n_channels, channel_source, n_features)
+    of emap_input_depth_images and its sharded twins, the converted inputs they point at (`keep`), the frame's rows (its
+    pixels) and its first camera's t[2]."""
+
+    def __init__(self, args, keep, pixels, first_z):
+        self.args, self.keep, self.pixels, self.first_z = args, keep, pixels, first_z
 
 
 def _to_host(x):

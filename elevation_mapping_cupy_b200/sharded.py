@@ -9,6 +9,11 @@ NCCL / NVLink between the phases of the frame:
                                                 upper-bound keys (int32 MIN)
     phase 3 (finalise + dilation + traversability + normals), identical on every rank.
 
+Semantic channels of the kinds that reduce as sums (average, class_average, color, class_bayesian, bayesian_inference)
+are summed by each rank in phase 1, reduced with exchange 2 (int64 / int32 SUM) and written to every replica's layers in
+phase 3; class_max is refused.  Depth cameras shard like clouds: a rank's rows are its cameras' pixels, offset by the
+pixels of the lower ranks' cameras.
+
 Every reduction is over integers, so the replicas stay bit-identical and the result equals the
 single-GPU `input_sensors` of the concatenated clouds bit for bit (which tests/ check against the oracle).
 The reference has no multi-GPU path (SURVEY 2.1); sensors there are fused sequentially.
@@ -42,6 +47,30 @@ def all_reduce_buffers(tensors_and_ops, group=None):
     ops = {"SUM": dist.ReduceOp.SUM, "MAX": dist.ReduceOp.MAX, "MIN": dist.ReduceOp.MIN}
     for t, op in tensors_and_ops:
         dist.all_reduce(t, op=ops[op], group=group)
+
+
+def split_exchange2(todo):
+    """Exchange 2's arrays as (critical, deferred): only the fused counts, listed second, gate the ray-cast of phase 2;
+    the height sums, last-writer keys and semantic sums are read in phase 3 (pure host logic, unit-tested on CPU)."""
+    return todo[1:2], todo[:1] + todo[2:]
+
+
+def depth_frame_offsets(pixels, first_z, group=None, static_offsets=None, overlap_z=None):
+    """(row offset, overlap z) of this rank's cameras in a sharded depth frame: the pixels (height * width summed) of the
+    lower ranks' cameras, or static_offsets[0]; `overlap_z`, or rank 0's first camera's t[2].  One all_gather of
+    (pixels, first_z) when either has to be found."""
+    if static_offsets is not None and overlap_z is not None:
+        return int(static_offsets[0]), float(overlap_z)
+    import torch
+    import torch.distributed as dist
+    ws, rk = dist.get_world_size(group), dist.get_rank(group)
+    dev = "cuda" if dist.get_backend(group) == "nccl" else "cpu"
+    mine = torch.tensor([float(pixels), float(first_z)], dtype=torch.float64, device=dev)     # exact below 2^53 pixels
+    allv = [torch.zeros_like(mine) for _ in range(ws)]
+    dist.all_gather(allv, mine, group=group)
+    rows = [v.tolist() for v in allv]
+    off = int(static_offsets[0]) if static_offsets is not None else int(sum(r[0] for r in rows[:rk]))
+    return off, float(overlap_z) if overlap_z is not None else rows[0][1]
 
 
 def global_point_offsets(local_count, group=None):
@@ -83,7 +112,9 @@ class ShardedElevationMap:
             if not ok and mode == "multicast":
                 raise RuntimeError("NVLink multicast is not available on this fabric")
 
-    def _attach_multicast(self):
+    def _attach_multicast(self, required=False):
+        """Attaches a symmetric block of emap_shard_scratch_bytes() (collective).  Without multicast support: False, or
+        an error when `required` (a re-attach of a handle that was attached)."""
         import torch.distributed as dist
         torch = self.torch
         em = self.em
@@ -95,22 +126,33 @@ class ShardedElevationMap:
             hdl = symm_mem.rendezvous(buf, grp.group_name)
             mc = int(hdl.multicast_ptr)
         except Exception as e:          # no symmetric-memory support in this build / fabric
+            if required:
+                raise
             print(f"[sharded] multicast unavailable ({type(e).__name__}: {e}); using NCCL all-reduces")
             return False
         if mc == 0:
+            if required:
+                raise RuntimeError("NVLink multicast is not available for the re-attached block")
             return False
         torch.cuda.synchronize()
         em._check(em._L.emap_shard_attach(em._h, C.c_void_p(buf.data_ptr()), C.c_void_p(mc), nbytes))
         hdl.barrier()
         torch.cuda.synchronize()
-        self._symm = (buf, hdl)
+        self._symm = (buf, hdl, nbytes)        # the block it replaces is released here, after the attach
         self.mode = "multicast"
         return True
 
+    def _fit_block(self):
+        """Multicast mode: a new block when the semantic configuration outgrew the attached one.  Collective, like the
+        configuration itself: every rank configures the same channels in the same call."""
+        em = self.em
+        if self.mode == "multicast" and int(em._L.emap_shard_scratch_bytes(em._h)) > self._symm[2]:
+            self._attach_multicast(required=True)
+
     def _plan(self, phase):
         em = self.em
-        arr = (_lib.EmapExchange * 4)()
-        n = C.c_int32(4)
+        arr = (_lib.EmapExchange * _lib.EMAP_SHARD_MAX_EXCHANGES)()
+        n = C.c_int32(_lib.EMAP_SHARD_MAX_EXCHANGES)
         em._check(em._L.emap_shard_exchange(em._h, phase, arr, C.byref(n)))
         plan = reduce_plan([(arr[i].ptr, arr[i].count, arr[i].kind) for i in range(n.value)])
         todo = []
@@ -127,14 +169,12 @@ class ShardedElevationMap:
         all_reduce_buffers(self._plan(phase), self.group)
 
     def _exchange2_overlapped(self):
-        """Exchange 2: only the int32 counts (cnt_fused | n_out) gate the ray-cast; the fixed-point sums and the
-        last-writer keys are consumed by the finalise pass, so their all-reduces run on a side stream under the
-        ray-cast.  Returns the pending work handles."""
+        """Exchange 2: only the counts (cnt_fused | n_out) gate the ray-cast; the fixed-point sums, the last-writer keys
+        and the semantic sums are consumed in phase 3, so their all-reduces run on a side stream under the ray-cast.
+        Returns the pending work handles."""
         import torch.distributed as dist
         ops = {"SUM": dist.ReduceOp.SUM, "MAX": dist.ReduceOp.MAX, "MIN": dist.ReduceOp.MIN}
-        todo = self._plan(2)
-        critical = [(t, op) for t, op in todo if t.dtype == self.torch.int32]
-        deferred = [(t, op) for t, op in todo if t.dtype != self.torch.int32]
+        critical, deferred = split_exchange2(self._plan(2))
         all_reduce_buffers(critical, self.group)
         self.side.wait_stream(self.stream)
         works = []
@@ -143,10 +183,13 @@ class ShardedElevationMap:
                 works.append(dist.all_reduce(t, op=ops[op], group=self.group, async_op=True))
         return works
 
-    def input_sensors(self, clouds, Rs, ts, position_noise, orientation_noise, device_ptrs=False, overlap_z=None):
-        """`overlap_z`: absolute z of the frame's first sensor (rank 0's), the same value on every rank."""
+    def input_sensors(self, clouds, Rs, ts, position_noise, orientation_noise, device_ptrs=False, overlap_z=None,
+                      channels=None):
+        """`overlap_z`: absolute z of the frame's first sensor (rank 0's), the same value on every rank.  `channels`:
+        the clouds' channel names as ElevationMap.input_pointcloud takes them, the same on every rank."""
         em = self.em
         from .elevation_mapping import _clouds, _to_host
+        em._configure_cloud_channels(channels)
         ptrs, counts, stride, dt, _keep = _clouds(clouds, device_ptrs)
         ns = len(counts)
         total_local = sum(int(c) for c in counts)
@@ -156,15 +199,35 @@ class ShardedElevationMap:
         L, h = em._L, em._h
         self.stream.wait_stream(self.torch.cuda.current_stream())
         with self.torch.cuda.stream(self.stream):
-            self._frame(L, h, ns, ptrs, counts, stride, dt, device_ptrs, Rm, tm, off, position_noise, orientation_noise,
+            self._frame(lambda: L.emap_shard_begin(h, ns, ptrs, counts, stride, dt, int(bool(device_ptrs)), Rm.ctypes.data,
+                                                   tm.ctypes.data, off, float(position_noise), float(orientation_noise)),
                         overlap_z)
         self.torch.cuda.current_stream().wait_stream(self.stream)
 
-    def _frame(self, L, h, ns, ptrs, counts, stride, dt, device_ptrs, Rm, tm, off, position_noise, orientation_noise,
-               overlap_z):
+    def input_depth_images(self, cameras, position_noise, orientation_noise, channels=(), confidence_threshold=10.0,
+                           max_depth=8.0, overlap_z=None):
+        """This rank's depth cameras of one sharded frame, collective over `group`: cameras and channels as
+        ElevationMap.input_depth_images (the same channels on every rank).  The frame's rows are the pixels of every
+        rank's cameras in rank order (static_offsets, if given, count pixels); `overlap_z` defaults to rank 0's first
+        camera's t[2]."""
         em = self.em
-        em._check(L.emap_shard_begin(h, ns, ptrs, counts, stride, dt, int(bool(device_ptrs)), Rm.ctypes.data,
-                                     tm.ctypes.data, off, float(position_noise), float(orientation_noise)))
+        depth = em._depth_frame(cameras, channels)
+        off, z = depth_frame_offsets(depth.pixels, depth.first_z, self.group, self.static_offsets, overlap_z)
+        L, h = em._L, em._h
+        self.stream.wait_stream(self.torch.cuda.current_stream())
+        with self.torch.cuda.stream(self.stream):
+            self._frame(lambda: L.emap_shard_begin_depth_images(h, *depth.args, float(confidence_threshold),
+                                                                float(max_depth), off, float(position_noise),
+                                                                float(orientation_noise)), z)
+        # the converted images in depth.keep are freed on return: their stream's later work follows the frame's
+        self.torch.cuda.current_stream().wait_stream(self.stream)
+
+    def _frame(self, begin, overlap_z):
+        """One sharded frame after `begin()` (an emap_shard_begin* call) on the library's stream."""
+        em = self.em
+        L, h = em._L, em._h
+        self._fit_block()
+        em._check(begin())
         if overlap_z is not None:
             em._check(L.emap_shard_set_overlap_z(h, float(overlap_z)))
         if self.mode == "multicast":

@@ -128,7 +128,7 @@ int emap_set_ray_counting(emap_handle* h, int enable);
  * emap_input_pointcloud / emap_input_sensors then also fuses the configured feature columns of the cloud into the caller's
  * (n_layers, W, W) fp32 device buffer.  kind: 0 = fusion/pointcloud_average.py, 1 = fusion/pointcloud_class_average.py
  * (average_weight = parameter.py:163), 2 = fusion/pointcloud_color.py (feature = packed 0x00RRGGBB bits in a float).
- * n_channels = 0 switches it off.  Not applied to sharded frames. */
+ * n_channels = 0 switches it off.  Sharded frames fuse kinds 0..4 too (emap_shard_begin); they refuse kind 5. */
 int emap_semantic_configure(emap_handle* h, int32_t n_channels, const int32_t* column, const int32_t* kind,
                             const int32_t* layer, float* semantic_map_device, int32_t n_layers, double average_weight);
 /* The kinds of emap_semantic_configure (0..2) and of emap_semantic_configure_ext (0..5). */
@@ -181,7 +181,8 @@ int emap_point_record_device_ptr(emap_handle* h, const int32_t** packed_device, 
  * (no host synchronisation, capturable into a CUDA graph under the rules of emap_set_stream, which binds the image
  * pointers, sizes, intrinsics and channel sources too), page-locked host images over PCIe, pageable ones are staged;
  * host images are free to reuse on return.  Kernel launches: those of the cloud frame with the same channel
- * configuration.  Not applied to sharded frames.
+ * configuration.  emap_shard_begin_depth_images and emap_input_depth_images_sharded spread the cameras of one frame over
+ * ranks.
  * EMAP_ERR_INVALID, with nothing launched and the state unchanged, for: n_cameras outside [1, EMAP_DEPTH_MAX_CAMERAS], a
  * NULL depth, height or width <= 0 or height * width > 2^24 (so a frame has fewer than 2^31 pixels), non-finite or zero fx / fy,
  * non-finite cx / cy / R / t, n_channels outside [0, EMAP_DEPTH_MAX_CHANNELS], n_features outside
@@ -217,21 +218,43 @@ typedef struct emap_exchange {
   int64_t count;    /* number of elements */
   int32_t kind;     /* 0: int64 SUM, 1: int64 MAX (keys < 2^63), 2: int32 MIN (keys offset to signed order), 3: int32 SUM */
 } emap_exchange;
+/* Semantic channels (emap_semantic_configure*) of kinds 0..4 are fused by sharded frames: each rank sums its own points'
+ * channels in phase 1, the sums are reduced with the others (exchange 2, or the multicast block), and every replica
+ * writes the layers in phase 3, bit for bit those of the single-GPU frame of all ranks' inputs.  A class_max channel
+ * (kind 5) is refused: any sharded begin returns EMAP_ERR_INVALID with nothing queued while one is configured. */
 int emap_shard_begin(emap_handle* h, int32_t n_sensors, const void* const* points, const int64_t* n,
                      int64_t row_stride, int dtype, int is_device_ptr, const float* R, const float* t,
                      int64_t global_point_offset, float position_noise, float orientation_noise);
+/* emap_shard_begin for depth cameras: arguments, checks and rows as emap_input_depth_images.  The rows are the pixels,
+ * camera after camera (masked pixels are dropped rows), so global_point_offset is the number of PIXELS (height * width
+ * summed) of the cameras on lower ranks; then the upper-bound keys ("last point in input order") are those of a single-GPU
+ * emap_input_depth_images of all ranks' cameras in rank order.  global_point_offset + this rank's pixels < 2^31.  The
+ * phases, barriers and exchanges that follow are those of emap_shard_begin. */
+int emap_shard_begin_depth_images(emap_handle* h, int32_t n_cameras, const emap_depth_camera* cameras, int is_device_ptr,
+                                  int32_t n_channels, const int32_t* channel_source, int32_t n_features,
+                                  float confidence_threshold, float max_depth, int64_t global_point_offset,
+                                  float position_noise, float orientation_noise);
 /* NVLink-multicast mode (replaces the three all-reduces): the caller allocates one symmetric block of
  * emap_shard_scratch_bytes() per rank (e.g. torch.distributed._symmetric_memory), rendezvouses it and hands
  * the library its own base and the MULTICAST alias.  From then on every per-cell accumulation of the frame
  * kernels is a single `multimem.red` that the NVSwitch applies to the replicas of all ranks -- the scatter and
  * the collective are one instruction.  Frame = emap_shard_begin, barrier, phase 0 (index), barrier, phase 1,
- * barrier, phase 2, barrier, phase 3; the barriers are the caller's (stream-ordered, cross-rank). */
+ * barrier, phase 2, barrier, phase 3; the barriers are the caller's (stream-ordered, cross-rank).
+ * The block holds the exchange scratch and then the semantic sum planes of the current configuration, so its size
+ * depends on that configuration: a sharded begin on a handle whose block is smaller than emap_shard_scratch_bytes()
+ * returns EMAP_ERR_STATE; attach a new block of that size (every rank, collectively) and begin again. */
 int64_t emap_shard_scratch_bytes(const emap_handle* h);
 int emap_shard_attach(emap_handle* h, void* local_base, void* multicast_base, int64_t bytes);
 /* Height reference of clear_overlap_map (EM.py:400-401) for a sharded frame: the absolute z of the
  * FIRST sensor of the whole frame (rank 0's), so that every replica clears the same cells.  Call
  * between emap_shard_begin and phase 3; without it a rank uses its own first sensor. */
 int emap_shard_set_overlap_z(emap_handle* h, float sensor_z_absolute);
+/* The arrays to reduce after phase `phase` (1..3): phase 1 the counts and drift statistics; phase 2 the height sums,
+ * the fused counts (listed second: the only array phase 2 reads, the others are read in phase 3), the last-writer keys,
+ * then the semantic sums where the configuration has them (int64 SUM of the averaged channels, int32 SUM of the colour
+ * channels); phase 3 the decrements, ray counts and upper-bound keys.  *n_out: the capacity on entry (>= 3), the count
+ * on return; a capacity below the count returns EMAP_ERR_INVALID with *n_out set to the count. */
+#define EMAP_SHARD_MAX_EXCHANGES 5
 int emap_shard_exchange(emap_handle* h, int32_t phase, emap_exchange* out, int32_t* n_out /*in: capacity*/);
 int emap_shard_phase(emap_handle* h, int32_t phase);   /* 0: index (attached handles only), 1: fusion, 2: ray-cast, 3: finalise+post */
 
@@ -248,6 +271,12 @@ int emap_input_sensors_sharded(emap_handle* h, int32_t n_sensors, const void* co
                                int64_t row_stride, int dtype, int is_device_ptr, const float* R, const float* t,
                                int64_t global_point_offset, float overlap_sensor_z_absolute, float position_noise,
                                float orientation_noise);
+/* emap_input_sensors_sharded for depth cameras: arguments as emap_shard_begin_depth_images, plus the absolute z of the
+ * frame's first camera overall (rank 0's first). */
+int emap_input_depth_images_sharded(emap_handle* h, int32_t n_cameras, const emap_depth_camera* cameras, int is_device_ptr,
+                                    int32_t n_channels, const int32_t* channel_source, int32_t n_features,
+                                    float confidence_threshold, float max_depth, int64_t global_point_offset,
+                                    float overlap_sensor_z_absolute, float position_noise, float orientation_noise);
 
 /* ---- pose / time: EM.py:139-170 move, move_to (WRAP:180-186); EM.py:119-128 clear (WRAP:188-191);
  * EM.py:420-426 update_variance, update_time (WRAP:193-203) ---- */
