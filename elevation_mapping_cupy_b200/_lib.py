@@ -91,6 +91,15 @@ class EmapDerivativeOut(C.Structure):
 EMAP_DERIVATIVE_INSIDE, EMAP_DERIVATIVE_OUTSIDE = 0, 1
 
 
+class EmapValuesOut(C.Structure):
+    _fields_ = [("values", C.c_void_p), ("status", C.c_void_p)]
+
+
+EMAP_VALUES_MAX_LAYERS = 24
+EMAP_VALUES_METHODS = {"nearest": 0, "linear": 1, "cubic": 2}
+VALUE_STATUS = ("outside", "nearest", "linear", "cubic")
+
+
 class EmapSdf(C.Structure):
     _fields_ = [("data", C.c_void_p), ("rows", C.c_int64), ("cols", C.c_int64), ("n_z", C.c_int64),
                 ("position", C.c_double * 2), ("resolution", C.c_double), ("z_min", C.c_double)]
@@ -193,6 +202,11 @@ SIGNATURES = {
                                       C.POINTER(EmapLineValuesOut), C.c_int32]),
     "emap_grid_derivatives": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_int64, C.c_void_p, C.c_int32,
                                         C.c_int32, C.POINTER(EmapDerivativeOut), C.c_int32]),
+    "emap_grid_values_at": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(EmapGrid), C.c_int32, C.c_int64, C.c_void_p,
+                                      C.c_int32, C.c_int32, C.POINTER(EmapValuesOut), C.c_int32]),
+    "emap_map_values_at": (C.c_int, [C.c_void_p, C.c_int32, C.POINTER(C.c_char_p), C.POINTER(C.c_void_p),
+                                     C.POINTER(C.c_int32), C.c_int64, C.c_void_p, C.c_int32, C.c_int32,
+                                     C.POINTER(EmapValuesOut), C.c_int32]),
     "emap_signed_distance_field": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_double, C.c_int64,
                                              C.c_void_p, C.c_int64, C.c_int32]),
     "emap_sdf_values": (C.c_int, [C.c_void_p, C.POINTER(EmapSdf), C.c_int32, C.c_int64, C.c_void_p, C.c_int32,

@@ -1,6 +1,6 @@
 // emap_export_api.cu -- the export calls of the C ABI (include/emap.h): layers, map windows (emap_get_submaps), windows
 // in a requester's frame (emap_get_transformed_submaps), plane segmentation of a window, the map point cloud and normal
-// arrows, and the layer pointers.
+// arrows, the layer pointers, and the layers' values at points (emap_map_values_at).
 #include "emap_handle.cuh"
 #include "emap_export.cuh"
 #include "emap_submap.cuh"
@@ -10,6 +10,7 @@
 #include "emap_resample.cuh"
 #include "emap_grid.cuh"
 #include "emap_mapcloud.cuh"
+#include "emap_values_at.cuh"
 
 namespace {
 
@@ -119,6 +120,41 @@ int map_cloud(emap_handle* h, int64_t* n_rows, float* xyz, int32_t* ids, double*
   return EMAP_OK;
 }
 
+// emap_map_values_at's cells: cell (r, c) of the full export (the (W-2)^2 planes of emap_get_layers, flipped on both
+// axes) is state cell (W - 2 - r, W - 2 - c), read through export_cell like every export.  value() picks the layer's
+// kind once, so each cell read is that kind's alone (KIND -1: the kind read at run time, for the normal planes and
+// normal_color).
+template <bool COLOUR>
+struct VaMapSrc {
+  int n;
+  DevCfg c;
+  const float* map;
+  const float* normal;
+  ExportList L;
+  float center_z;
+  int only_above;
+  template <int KIND>
+  struct Cell {
+    const VaMapSrc& s;
+    __device__ __forceinline__ float at(int l, int r, int cc) const {
+      return export_cell<COLOUR>(s.c, s.map, s.normal, s.c.W - 2 - r, s.c.W - 2 - cc, KIND < 0 ? s.L.kind[l] : KIND,
+                                 s.center_z, s.only_above, s.L.plane[l], s.L.flags[l]);
+    }
+  };
+  __device__ __forceinline__ float value(const VaPoint& p, int l) const {
+    switch (L.kind[l]) {
+      case 0: return va_value(p, Cell<0>{*this}, l);
+      case 1: return va_value(p, Cell<1>{*this}, l);
+      case 2: return va_value(p, Cell<2>{*this}, l);
+      case 3: return va_value(p, Cell<3>{*this}, l);
+      case 4: return va_value(p, Cell<4>{*this}, l);
+      case 5: return va_value(p, Cell<5>{*this}, l);
+      case EXPORT_KIND_PLANE: return va_value(p, Cell<EXPORT_KIND_PLANE>{*this}, l);
+      default: return va_value(p, Cell<-1>{*this}, l);
+    }
+  }
+};
+
 }  // namespace
 
 extern "C" {
@@ -222,6 +258,38 @@ int emap_get_submaps(emap_handle* h, int32_t n_windows, const double* windows, i
     CK(cudaStreamSynchronize(h->stream));
   }
   return EMAP_OK;
+}
+
+// The live map's layers at points: emap_grid_values_at on the full export (rows = cols = cell_n - 2, position = the map
+// centre's x and y widened to double, the handle's resolution), its cells read in place.  The centre travels in the
+// kernel's parameters.
+int emap_map_values_at(emap_handle* h, int32_t n_layers, const char* const* names, const float* const* planes_device,
+                       const int32_t* flags, int64_t n_points, const double* positions, int32_t positions_on_device,
+                       int32_t method, const emap_values_out* out, int32_t out_is_device) {
+  ENTER(h);
+  const char* e = !names ? "null argument" : va_check(n_layers, n_points, positions, method, out);
+  if (e) return fail(h, EMAP_ERR_INVALID, (std::string("emap_map_values_at: ") + e).c_str());
+  ExportList L;
+  if (!export_list(h, n_layers, names, planes_device, flags, L)) return EMAP_ERR_INVALID;
+  if (n_points == 0) return EMAP_OK;
+  NvtxRange nv("map_values_at");
+  if (int rc = va_room(h, n_layers, n_points, out_is_device)) return rc;
+  const double* xy = positions;
+  if (int rc = stage_inputs(h, h->lookup.up, xy, positions_on_device ? 0 : sizeof(double) * 2 * n_points)) return rc;
+  const int Wo = h->dc.W - 2;
+  VaGeom g;
+  g.rows = g.cols = Wo;
+  g.res = h->cfg.resolution;
+  for (int a = 0; a < 2; a++) {
+    g.pos[a] = (double)h->center[a];
+    g.len[a] = (double)Wo * h->cfg.resolution;
+  }
+  if (export_has_colour(L)) {
+    const VaMapSrc<true> s{n_layers, h->dc, h->map, h->normal, L, h->center[2], h->cfg.use_only_above_for_upper_bound};
+    return va_launch(h, g, s, method, n_points, xy, out, out_is_device);
+  }
+  const VaMapSrc<false> s{n_layers, h->dc, h->map, h->normal, L, h->center[2], h->cfg.use_only_above_for_upper_bound};
+  return va_launch(h, g, s, method, n_points, xy, out, out_is_device);
 }
 
 static_assert(EMAP_TRANSFORM_TOLERANCE == TSUB_ORTHO_TOL && EMAP_TRANSFORMED_WINDOWS_PER_LAUNCH == TSUB_MAX_WINDOWS,

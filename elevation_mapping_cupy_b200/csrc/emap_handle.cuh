@@ -232,9 +232,9 @@ struct emap_handle {
   DevBuf<char> pca_block;          // emap_features_pca: one device block carved by carve_pca
   Staging query;                   // emap_project_to_planar_regions: the block carved by carve_query, host tables and
                                    // queries, the host outputs
-  Staging lookup;                  // the grid lookups and the distance field: the block (the lookups' outputs, the
-                                   // field's fill key and host-bound volume), a host grid or field and queries, the
-                                   // host outputs
+  Staging lookup;                  // the grid lookups, the point values and the distance field: the block (the
+                                   // lookups' and point values' outputs, the field's fill key and host-bound volume),
+                                   // host grids or a field and queries, the host outputs
   DevBuf<double> line_rows;        // emap_values_between's host-bound line offsets, then its rows
   StagedUpload img_up;             // emap_input_image with a host image
   StagedUpload init_up;            // emap_initialize_map's arrays
@@ -371,6 +371,25 @@ int stage_inputs(emap_handle* h, StagedUpload& up, Inputs&&... in) {
   if (int rc = up.room(h, end)) return rc;
   Carver c{0};
   stage_each(c, end, up.host, up.dev, in...);
+  return up.send(h, end);
+}
+
+// stage_inputs for a list of n inputs known at run time: p[k] and bytes[k] as the (pointer, bytes) pairs above.
+template <typename T>
+int stage_input_list(emap_handle* h, StagedUpload& up, int n, const T** p, const size_t* bytes) {
+  Carver layout{0};
+  size_t end = 0;
+  for (int k = 0; k < n; k++)
+    if (bytes[k]) end = (size_t)layout.take<char>(bytes[k]) + bytes[k];
+  if (!end) return 0;
+  if (int rc = up.room(h, end)) return rc;
+  Carver c{0};
+  for (int k = 0; k < n; k++)
+    if (bytes[k]) {
+      const size_t o = (size_t)c.take<char>(bytes[k]);
+      memcpy(up.host + o, p[k], bytes[k]);
+      p[k] = (const T*)(up.dev + o);
+    }
   return up.send(h, end);
 }
 

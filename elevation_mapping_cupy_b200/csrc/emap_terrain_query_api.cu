@@ -1,13 +1,14 @@
 // emap_terrain_query_api.cu -- queries on the planar terrain and its layers of the C ABI (include/emap.h):
 // emap_project_to_planar_regions over the kernels of emap_terrain_query.cuh, emap_max_values_between,
-// emap_values_between and emap_grid_derivatives over those of emap_grid_lookup.cuh, and emap_signed_distance_field and
-// emap_sdf_values over those of emap_sdf.cuh.
+// emap_values_between and emap_grid_derivatives over those of emap_grid_lookup.cuh, emap_grid_values_at over
+// emap_values_at.cuh's, and emap_signed_distance_field and emap_sdf_values over those of emap_sdf.cuh.
 #include <algorithm>
 
 #include "emap_grid_lookup.cuh"
 #include "emap_handle.cuh"
 #include "emap_sdf.cuh"
 #include "emap_terrain_query.cuh"
+#include "emap_values_at.cuh"
 
 namespace {
 
@@ -94,6 +95,13 @@ static_assert((int)EMAP_DERIVATIVE_INSIDE == (int)GL_INSIDE && (int)EMAP_DERIVAT
               "the derivative statuses");
 
 static_assert(EMAP_SDF_MAX_D2 == SDF_MAX_D2, "the field's limit");
+
+static_assert(EMAP_VALUES_MAX_LAYERS == VA_MAX_LAYERS && (int)EMAP_VALUES_NEAREST == (int)VA_NEAREST &&
+                  (int)EMAP_VALUES_LINEAR == (int)VA_LINEAR && (int)EMAP_VALUES_CUBIC == (int)VA_CUBIC,
+              "the point values' limits and methods");
+static_assert((int)EMAP_VALUE_OUTSIDE == (int)VA_OUT && (int)EMAP_VALUE_NEAREST == (int)VA_BY_NEAREST &&
+                  (int)EMAP_VALUE_LINEAR == (int)VA_BY_LINEAR && (int)EMAP_VALUE_CUBIC == (int)VA_BY_CUBIC,
+              "the point values' statuses");
 
 static_assert(EMAP_REGION_ROW == PQ_ROW && EMAP_REGION_POLYGON == PQ_POLY, "the region table layout");
 static_assert(EMAP_CONVEX_MAX_VERTICES == PQ_MAX_CONVEX && EMAP_GROW_MAX_ITER == PQ_MAX_ITER, "the growth limits");
@@ -270,6 +278,48 @@ int emap_grid_derivatives(emap_handle* h, const emap_grid* grid, int32_t grid_on
     memcpy(out->index, h->lookup.down + vb, ib);
   }
   return EMAP_OK;
+}
+
+int emap_grid_values_at(emap_handle* h, int32_t n_layers, const emap_grid* grids, int32_t grids_on_device,
+                        int64_t n_points, const double* positions, int32_t positions_on_device, int32_t method,
+                        const emap_values_out* out, int32_t out_is_device) {
+  ENTER(h);
+  const char* e = !grids ? "null argument" : va_check(n_layers, n_points, positions, method, out);
+  for (int k = 0; !e && k < n_layers; k++) {
+    const emap_grid &a = grids[k], &b = grids[0];
+    e = gl_check_grid(a.data, a.rows, a.cols, a.position, a.resolution, 1);
+    if (!e && (a.rows != b.rows || a.cols != b.cols || a.position[0] != b.position[0] ||
+               a.position[1] != b.position[1] || a.resolution != b.resolution))
+      e = "the layers must share rows, cols, position and resolution";
+  }
+  if (e) return fail(h, EMAP_ERR_INVALID, (std::string("emap_grid_values_at: ") + e).c_str());
+  if (n_points == 0) return EMAP_OK;
+  NvtxRange nv("grid_values_at");
+  if (int rc = va_room(h, n_layers, n_points, out_is_device)) return rc;
+  const emap_grid& g0 = grids[0];
+  // the layers and the positions, host ones uploaded in one copy
+  const void* in[VA_MAX_LAYERS + 1];
+  size_t bytes[VA_MAX_LAYERS + 1];
+  for (int k = 0; k < n_layers; k++) {
+    in[k] = grids[k].data;
+    bytes[k] = grids_on_device ? 0 : sizeof(float) * g0.rows * g0.cols;
+  }
+  in[n_layers] = positions;
+  bytes[n_layers] = positions_on_device ? 0 : sizeof(double) * 2 * n_points;
+  if (int rc = stage_input_list(h, h->lookup.up, n_layers + 1, in, bytes)) return rc;
+  VaGeom g;
+  g.rows = (int)g0.rows;
+  g.cols = (int)g0.cols;
+  g.res = g0.resolution;
+  for (int a = 0; a < 2; a++) {
+    g.pos[a] = g0.position[a];
+    g.len[a] = (double)(a ? g0.cols : g0.rows) * g0.resolution;
+  }
+  VaGridSrc s;
+  s.n = n_layers;
+  s.cols = g.cols;
+  for (int k = 0; k < VA_MAX_LAYERS; k++) s.data[k] = k < n_layers ? (const float*)in[k] : nullptr;
+  return va_launch(h, g, s, method, n_points, (const double*)in[n_layers], out, out_is_device);
 }
 
 int emap_signed_distance_field(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, double z_min,

@@ -780,6 +780,78 @@ class ElevationMap:
             res["curvature"] = value[:, 2:]
         return res
 
+    def values_at(self, positions, layers=("elevation",), method="linear", grid=None, out=None):
+        """The value of each layer at each point, as grid_map's GridMap::atPosition gives it with "nearest", "linear" or
+        "cubic" (cubic convolution), in one library call (emap_map_values_at / emap_grid_values_at; include/emap.h
+        states the rule, its fallbacks at the edges and its operation order).  `positions`: (N, 2) map-frame points,
+        float64 NumPy or a CUDA tensor.  `layers`: up to 24 names.  `grid`: None for the live map (layers named as for
+        get_maps_with_names_ref, each evaluated once; the map's exported geometry at its current centre), or a dict of
+        get_submap(s), get_transformed_submap(s), planar_terrain, plane_decomposition or the caller's own with
+        "layers", "centre" and optionally "resolution", its layers read in place (all NumPy or all torch CUDA).
+        `out`: None, or a dict of "values" (len(layers), N) float32 and "status" (N,) int32, both NumPy or both torch
+        CUDA, written in place.  Device positions or a device `out` keep everything on the device (stream-ordered, no
+        host synchronisation).  Returns "values" (a dict of (N,) views per layer name; NaN outside the grid) and
+        "status" (N,): the method that produced each point's values after the fallbacks, 0 outside, 1 nearest,
+        2 linear, 3 cubic."""
+        if isinstance(layers, str):
+            layers = (layers,)
+        names = list(layers)
+        if method not in _lib.EMAP_VALUES_METHODS:
+            raise ValueError("method must be 'nearest', 'linear' or 'cubic'")
+        if not 1 <= len(names) <= _lib.EMAP_VALUES_MAX_LAYERS:
+            raise ValueError("1 to %d layers" % _lib.EMAP_VALUES_MAX_LAYERS)
+        nl, m = len(names), _lib.EMAP_VALUES_METHODS[method]
+        if grid is not None:
+            g, g_dev, q, n, device, mk, ptr = self._lookup_args(grid, names[0], (positions,), 2, out,
+                                                                ("values", "status"))
+            grids = [g] + [self._lookup_args(grid, name, (), 0, None, ())[0] for name in names[1:]]
+            if any(_is_device(x._keep) != g_dev for x in grids):
+                raise TypeError("the grid's layers must be all NumPy or all torch CUDA")
+        else:
+            for name in names:
+                if not (name in EXPORT_NAMES or name in self.semantic_map.layer_names
+                        or name in self.plugin_manager.layer_names):
+                    raise KeyError("Layer {} is not in the map".format(name))
+            g_dev = False
+            q_dev = _is_device(positions)
+            out_dev = [a for a in (out or {}).values() if _is_device(a)]
+            device = q_dev or bool(out_dev)
+            if q_dev:
+                import torch
+                q = positions.to(torch.float64).reshape(-1, 2).contiguous()
+            else:
+                q = np.ascontiguousarray(np.asarray(_to_host(positions), np.float64).reshape(-1, 2))
+            n = int(q.shape[0])
+            mk, ptr = _array_maker((positions.device if q_dev else out_dev[0].device) if device else None)
+        if out is None:
+            out = {"values": mk((nl, n), "float32"), "status": mk((n,), "int32")}
+        _check_out(out, {"values": (nl, n), "status": (n,)}, device)
+        o = _lib.EmapValuesOut(ptr(out["values"]), ptr(out["status"]))
+        q_dev = _is_device(q)
+        q_ptr = q.data_ptr() if q_dev else q.ctypes.data
+        if grid is not None:
+            arr = (_lib.EmapGrid * nl)(*grids)
+            if device or g_dev or q_dev:
+                self._after_framework()
+            self._check(self._L.emap_grid_values_at(self._h, nl, arr, int(g_dev), n, q_ptr, int(q_dev), m, C.byref(o),
+                                                    int(device)))
+            if device:
+                self._before_framework()
+        else:
+            with self.map_lock:
+                sources = [self._export_source(name) for name in names]
+                c_names = (C.c_char_p * nl)(*[s[0].encode() for s in sources])
+                planes = (C.c_void_p * nl)(*[s[1] for s in sources])
+                flags = (C.c_int32 * nl)(*[s[2] for s in sources])
+                if device or q_dev or any(s[3] is not None for s in sources):
+                    self._after_framework()
+                self._check(self._L.emap_map_values_at(self._h, nl, c_names, planes, flags, n, q_ptr, int(q_dev), m,
+                                                       C.byref(o), int(device)))
+                if device:
+                    self._before_framework()
+        values = out["values"]
+        return {"values": {name: values[k] for k, name in enumerate(names)}, "status": out["status"]}
+
     def signed_distance_field(self, grid, layer="elevation", height_clearance=0.1, z_range=None, out=None):
         """A signed distance field of `layer` over the grid's box (metres to the terrain surface: positive above it,
         negative below), in one library call (emap_signed_distance_field; include/emap.h states every step).  `grid`
@@ -1402,7 +1474,8 @@ def _array_maker(device):
 
 def _check_out(out, shapes, device):
     """Every out[k] is a contiguous array of shapes[k] on the call's side (NumPy for host output, CUDA for device)."""
-    dtypes = {"index": "int32", "value": "float64", "volume": "float32", "image": "uint8", "layer": "float32"}
+    dtypes = {"index": "int32", "value": "float64", "volume": "float32", "image": "uint8", "layer": "float32",
+              "values": "float32", "status": "int32"}
     for k, shape in shapes.items():
         a = out[k]
         if tuple(a.shape) != shape or _is_device(a) != device or str(a.dtype).split(".")[-1] != dtypes[k] or not (

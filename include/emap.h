@@ -780,6 +780,75 @@ int emap_values_between(emap_handle* h, const emap_grid* grid, int32_t grid_on_d
 int emap_grid_derivatives(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, int64_t n_queries,
                           const double* positions, int32_t positions_on_device, int32_t curvature,
                           const emap_derivative_out* out, int32_t out_is_device);
+/* ---- layer values at points: grid_map's GridMap::atPosition(layer, position, method) with nearest, linear and cubic
+ * convolution interpolation (GridMap.cpp's atPositionLinearInterpolated, CubicInterpolation.cpp's bicubic_conv;
+ * restated from grid_map's published source), for a batch of points and up to EMAP_VALUES_MAX_LAYERS layers of one
+ * geometry, on the device.  The cell choice and the operation order below are this library's definition and are
+ * tested exactly; bit parity with a grid_map build is not claimed (none was available).
+ * Geometry: an emap_grid's, with the lookups' index and position arithmetic above: per axis, a point v is inside when
+ *  0 <= -((v - p) - o) < L, its index is trunc(-(((v - o) - p) / resolution)) clamped to [0, n - 1], and index i is at
+ *  (p + (0.5 L - 0.5 resolution)) - resolution * i; X(r) and Y(c) below are these positions of row r and column c.
+ * Per point (x, y), in IEEE double, every operation rounded on its own (no contraction), the result rounded once to
+ * float; F(r, c) is the layer's cell widened to double:
+ *  Outside (on either axis, which includes a NaN or infinite coordinate): status EMAP_VALUE_OUTSIDE and every layer the
+ *   quiet NaN 0x7fc00000 (grid_map throws here).
+ *  (r, c) = the point's cell.  method EMAP_VALUES_NEAREST: F(r, c), status EMAP_VALUE_NEAREST.
+ *  Linear (EMAP_VALUES_LINEAR, and the fallback of cubic): r' = r - 1 when x >= X(r), else r + 1; c' = c - 1 when
+ *   y >= Y(c), else c + 1.  If r' or c' lies outside [0, rows - 1] / [0, cols - 1], the point falls back to nearest.
+ *   Otherwise the corner of lowest x and y is r0 = max(r, r'), c0 = max(c, c'); tx = (x - X(r0)) / resolution,
+ *   ty = (y - Y(c0)) / resolution, ux = 1 - tx, uy = 1 - ty; with f0 = F(r0, c0), f1 = F(r0 - 1, c0),
+ *   f2 = F(r0, c0 - 1), f3 = F(r0 - 1, c0 - 1):
+ *     value = (((f0 ux) uy + (f1 tx) uy) + (f2 ux) ty) + (f3 tx) ty      (grid_map's order), status EMAP_VALUE_LINEAR.
+ *   grid_map bounds-checks the four cells by their linear buffer index, so at its edges it can read a wrapped row where
+ *   this rule falls back to nearest; that departure is deliberate and not reproduced.
+ *  Cubic convolution (EMAP_VALUES_CUBIC; grid_map's INTER_CUBIC_CONVOLUTION, Keys with a = -0.5): r0, c0, tx and ty as
+ *   for linear; it needs rows r0 + 1 .. r0 - 2 and columns c0 + 1 .. c0 - 2 inside the grid, else the point falls back
+ *   to linear (and from there possibly to nearest).  Weights per axis, t = tx or ty, with grid_map's matrix
+ *   M = [[0, 2, 0, 0], [-1, 0, 1, 0], [2, -5, 4, -1], [-1, 3, -3, 1]], t2 = t t, t3 = t2 t:
+ *     w_j = 0.5 (((M[0][j] + M[1][j] t) + M[2][j] t2) + M[3][j] t3)           (j = 0 .. 3: f(-1), f(0), f(1), f(2)).
+ *   The 1-D pass runs along y for each of the four rows i = 0 .. 3 (row r0 + 1 - i), then along x:
+ *     g_i = ((wy_0 F(r, c0 + 1) + wy_1 F(r, c0)) + wy_2 F(r, c0 - 1)) + wy_3 F(r, c0 - 2),
+ *     value = ((wx_0 g_0 + wx_1 g_1) + wx_2 g_2) + wx_3 g_3,                              status EMAP_VALUE_CUBIC.
+ *  Non-finite cells are not masked: a NaN or +-inf among the cells used propagates by IEEE arithmetic as it does in
+ *   grid_map, including 0 * inf = NaN for a zero weight (a point at a cell centre next to an infinite cell is NaN).
+ *   Every NaN value is written as 0x7fc00000 (the host and the device give NaNs different payloads).
+ *  So at a cell centre with finite neighbours linear and cubic return the cell's value (up to the sign of a zero).
+ * Outputs (emap_values_out): values, n_layers x n_points floats, layer-major (layer k of point i at k n_points + i);
+ *  status, one int32 per point: the method that produced its values after the fallbacks.
+ * emap_grid_values_at: n_layers emap_grids that share rows, cols, position and resolution, every layer's data in host
+ *  (grids_on_device 0) or every one in device memory.  Checks: each grid as the lookups check theirs (rows and cols
+ *  >= 1).
+ * emap_map_values_at: the live map.  The layers are named as for emap_get_layers (a basic name, or planes_device[k] !=
+ *  NULL with flags[k]).  The result equals emap_grid_values_at on the full export, bit for bit: the (cell_n - 2)^2
+ *  planes of emap_get_layers with position = the map centre's x and y (float) widened to double and the handle's
+ *  resolution.  A get_submaps window that covers the whole exported area (at the map centre, lengths >= (cell_n - 2) *
+ *  resolution) is that grid: emap_submap_windows reports its centre as center + (0.5 (top + bottom + 1) - 0.5 cell_n)
+ *  * resolution with top + bottom + 1 = cell_n, i.e. exactly the map centre.  The cells are read from the map state
+ *  (the export is not materialised).  The centre travels in the kernel's parameters, so a captured call is valid only
+ *  at its capture centre, as for frames and windows.
+ * Both: positions are n_points (x, y) doubles in the map frame, host (positions_on_device 0) or device memory.  One
+ *  kernel (one thread per point: the cell, the fallbacks and the weights once, then 1, 4 or 16 cells per layer), none
+ *  for n_points = 0.  Host inputs are uploaded in one copy; host output comes back in one copy and one
+ *  synchronisation; device output (values and status device memory) is stream-ordered with no host synchronisation and
+ *  can be captured into a CUDA graph (with device positions; capture after an eager call of the largest size: growing
+ *  the scratch synchronises).  The handle's map state is not changed; the calls use the lookups' staging and scratch.
+ *  EMAP_ERR_INVALID, with nothing written or launched: a NULL grids / names / out; n_layers outside
+ *  [1, EMAP_VALUES_MAX_LAYERS]; a method other than EMAP_VALUES_*; n_points below 0 or above 2^31 - 1; NULL positions,
+ *  values or status with n_points > 0; what the lookups reject for a grid and layers whose geometries differ
+ *  (emap_grid_values_at); an unknown layer name (emap_map_values_at). */
+#define EMAP_VALUES_MAX_LAYERS 24
+enum { EMAP_VALUES_NEAREST = 0, EMAP_VALUES_LINEAR = 1, EMAP_VALUES_CUBIC = 2 };
+enum { EMAP_VALUE_OUTSIDE = 0, EMAP_VALUE_NEAREST = 1, EMAP_VALUE_LINEAR = 2, EMAP_VALUE_CUBIC = 3 };
+typedef struct emap_values_out {
+  float* values;           /* n_layers x n_points, layer-major */
+  int32_t* status;         /* 1 per point: EMAP_VALUE_* */
+} emap_values_out;
+int emap_grid_values_at(emap_handle* h, int32_t n_layers, const emap_grid* grids, int32_t grids_on_device,
+                        int64_t n_points, const double* positions, int32_t positions_on_device, int32_t method,
+                        const emap_values_out* out, int32_t out_is_device);
+int emap_map_values_at(emap_handle* h, int32_t n_layers, const char* const* names, const float* const* planes_device,
+                       const int32_t* flags, int64_t n_points, const double* positions, int32_t positions_on_device,
+                       int32_t method, const emap_values_out* out, int32_t out_is_device);
 /* ---- a signed distance field of one grid layer and distance queries against it, on the device (a legged robot's
  * swing-leg clearance: how far a point is from the terrain and in which direction that distance grows).  DESIGN.md
  * §4l (continued) gives the algorithm.  The handle's map state is not read or changed; the calls use the handle's
