@@ -190,6 +190,18 @@ class ElevationMap:
         if st is not None:
             self._check(self._L.emap_stream_wait_for(self._h, C.c_void_p(st)))
 
+    def _ordered_call(self, fn, *args, after=False, before=False):
+        """fn(*args), a library call, ordered with the caller's framework: after the work it has queued when `after` (the
+        call reads memory the framework writes, or writes memory it reads) and before the work it queues next when
+        `before` (the call writes device memory the framework reads).  That second wait is queued before a failure
+        raises, so framework work that frees or rewrites the call's device inputs still runs after what the call queued."""
+        if after:
+            self._after_framework()
+        rc = fn(*args)
+        if before:
+            self._before_framework()
+        self._check(rc)
+
     def _ptr(self, name):
         p = C.c_void_p()
         self._check(self._L.emap_layer_device_ptr(self._h, name.encode(), C.byref(p)))
@@ -338,14 +350,11 @@ class ElevationMap:
         `channels` is shared by every camera."""
         depth = self._depth_frame(cameras, channels)
         with self.map_lock:
-            self._after_framework()       # framework work writing the images or reading the aliased layers comes first
-            rc = self._L.emap_input_depth_images(self._h, *depth.args, float(confidence_threshold), float(max_depth),
-                                                 float(position_noise), float(orientation_noise))
-            # framework work queued from here on sees the fused map, and the device images (the caller's, or the
-            # converted copies in `keep`, freed on return) are released or rewritten only after the frame has read them
-            # (no host sync)
-            self._before_framework()
-            self._check(rc)
+            # the frame runs after the framework work writing the images or reading the aliased layers; framework work
+            # queued from here on sees the fused map, and the device images (the caller's, or the converted copies in
+            # `keep`, freed on return) are released or rewritten only after the frame has read them (no host sync)
+            self._ordered_call(self._L.emap_input_depth_images, self._h, *depth.args, float(confidence_threshold),
+                               float(max_depth), float(position_noise), float(orientation_noise), after=True, before=True)
 
     def _depth_frame(self, cameras, channels):
         """The depth cameras of one frame as the library takes them (_DepthFrame), with `channels` configured as the
@@ -426,35 +435,47 @@ class ElevationMap:
         self.plugin_manager.update_with_name(name, self.elevation_map, self.layer_names, self.semantic_map.semantic_map,
                                              self.semantic_map.layer_names, self.base_rotation, self.semantic_map.elements_to_shift)
 
+    def _exportable(self, name):
+        return name in EXPORT_NAMES or name in self.semantic_map.layer_names or name in self.plugin_manager.layer_names
+
     def _export_source(self, name):
-        """(name, device plane, flags, tensor to keep alive) of an exportable layer, None if the map has none by that name.
-        Basic layers are exported by name; semantic layers as they are (EM.py:747-748: cropped, flipped, no NaN fill, no z
-        offset); plugin layers with their fill_nan / is_height_layer (EM.py:762-775: flags bit 0 / bit 1)."""
+        """(name, device plane, flags, tensor to keep alive) of an exportable layer (_exportable).  Basic layers are
+        exported by name; semantic layers as they are (EM.py:747-748: cropped, flipped, no NaN fill, no z offset); plugin
+        layers with their fill_nan / is_height_layer (EM.py:762-775: flags bit 0 / bit 1)."""
         if name in EXPORT_NAMES:
             return name, None, 0, None
         if name in self.semantic_map.layer_names:
             m = self.semantic_map.semantic_map[self.semantic_map.layer_names.index(name)]
             return name, m.data_ptr(), 0, m
-        if name in self.plugin_manager.layer_names:
-            self._update_plugin(name)
-            m = self.plugin_manager.get_map_with_name(name)
-            p = self.plugin_manager.get_param_with_name(name)
-            return name, m.data_ptr(), int(bool(p.fill_nan)) | (int(bool(p.is_height_layer)) << 1), m
-        return None
+        self._update_plugin(name)
+        m = self.plugin_manager.get_map_with_name(name)
+        p = self.plugin_manager.get_param_with_name(name)
+        return name, m.data_ptr(), int(bool(p.fill_nan)) | (int(bool(p.is_height_layer)) << 1), m
 
-    def _export(self, sources, data):
-        """Writes the layers of `sources` (_export_source results) into `data`, a caller-owned (len(sources), cell_n-2,
-        cell_n-2) float32 array: one kernel, one D2H copy, one sync.  Runs under map_lock."""
+    def _layer_sources(self, names):
+        """The (names, planes, flags) arrays the library takes for the live-map layers `names` (_export_source each), and
+        whether any plane is framework memory.  Every name is checked before any source is evaluated (a plugin layer runs
+        its plugin): KeyError for a layer the map does not have.  Runs under map_lock."""
+        for name in names:
+            if not self._exportable(name):
+                raise KeyError("Layer {} is not in the map".format(name))
+        sources = [self._export_source(name) for name in names]
         n = len(sources)
+        planes = (C.c_void_p * n)(*[s[1] for s in sources])
+        planes._keep = [s[3] for s in sources]
+        return ((C.c_char_p * n)(*[s[0].encode() for s in sources]), planes, (C.c_int32 * n)(*[s[2] for s in sources]),
+                any(s[3] is not None for s in sources))
+
+    def _export(self, names, data):
+        """Writes the layers `names` (_layer_sources) into `data`, a caller-owned (len(names), cell_n-2, cell_n-2) float32
+        array: one kernel, one D2H copy, one sync.  Runs under map_lock."""
+        n = len(names)
         n_out = (self.cell_n - 2) ** 2
         direct = isinstance(data, np.ndarray) and data.dtype == np.float32 and data.flags.c_contiguous and data.size == n * n_out
         buf = data if direct else (self._export_tmp if n == 1 else np.zeros((n, n_out), np.float32))
-        c_names = (C.c_char_p * n)(*[s[0].encode() for s in sources])
-        planes = (C.c_void_p * n)(*[s[1] for s in sources])
-        flags = (C.c_int32 * n)(*[s[2] for s in sources])
-        if any(s[3] is not None for s in sources):
-            self._after_framework()
-        self._check(self._L.emap_get_layers(self._h, n, c_names, planes, flags, buf.ctypes.data, n * n_out))
+        c_names, planes, flags, framework = self._layer_sources(names)
+        self._ordered_call(self._L.emap_get_layers, self._h, n, c_names, planes, flags, buf.ctypes.data, n * n_out,
+                           after=framework)
         if not direct:
             data[...] = buf.reshape(data.shape)
 
@@ -462,23 +483,16 @@ class ElevationMap:
         """EM.py:720-775: write layer `name` (NaN-filled, z-shifted, cropped, flipped) into `data`,
         a caller-owned (cell_n-2, cell_n-2) float32 array."""
         with self.map_lock:
-            src = self._export_source(name)
-            if src is None:
+            if not self._exportable(name):
                 print("Layer {} is not in the map".format(name))
                 return
-            self._export([src], data)
+            self._export([name], data)
 
     def get_maps_with_names_ref(self, names, data):
         """Several layers at once (what the C++ bridge's get_grid_map does one by one, elevation_mapping_wrapper.cpp:213-252):
         `data` is a caller-owned (len(names), cell_n-2, cell_n-2) float32 array.  One kernel, one D2H copy, one sync."""
         with self.map_lock:
-            sources = []
-            for name in names:
-                src = self._export_source(name)
-                if src is None:
-                    raise KeyError("Layer {} is not in the map".format(name))
-                sources.append(src)
-            self._export(sources, data)
+            self._export(list(names), data)
 
     def get_submap(self, position, length, layers, out=None):
         """The get_raw_submap service (elevation_mapping_ros.cpp:507-553) in the map frame: the window of the exported
@@ -508,8 +522,8 @@ class ElevationMap:
             return int((info[:, 3].astype(np.int64) * info[:, 4]).sum())
 
         def call(nl, c_names, planes, flags, ptr, device, size):
-            self._check(self._L.emap_get_submaps(self._h, n, req.ctypes.data, nl, c_names, planes, flags, ptr,
-                                                 device, size, info.ctypes.data, centres.ctypes.data))
+            return self._L.emap_get_submaps(self._h, n, req.ctypes.data, nl, c_names, planes, flags, ptr, device, size,
+                                            info.ctypes.data, centres.ctypes.data)
 
         views = self._window_views(layers, out, cells, call, info[:, 3:5])
         return [{"layers": views[w], "index": (int(info[w, 1]), int(info[w, 2])),
@@ -549,9 +563,9 @@ class ElevationMap:
             return int((info[:, 1].astype(np.int64) * info[:, 2]).sum())
 
         def call(nl, c_names, planes, flags, ptr, device, size):
-            self._check(self._L.emap_get_transformed_submaps(self._h, n, req.ctypes.data, tf.ctypes.data,
-                                                             float(sample_ratio), nl, c_names, planes, flags, ptr,
-                                                             device, size, info.ctypes.data, geometry.ctypes.data))
+            return self._L.emap_get_transformed_submaps(self._h, n, req.ctypes.data, tf.ctypes.data, float(sample_ratio),
+                                                        nl, c_names, planes, flags, ptr, device, size, info.ctypes.data,
+                                                        geometry.ctypes.data)
 
         views = self._window_views(layers, out, cells, call, info[:, 1:3])
         return [{"layers": views[w], "size": (int(info[w, 1]), int(info[w, 2])),
@@ -572,44 +586,18 @@ class ElevationMap:
         from .plane_segmentation import PlaneSegmentationParams
         p = (params or PlaneSegmentationParams()).to_c()
         req = np.array(_xy(position) + _xy(length), np.float64)
-        win = np.zeros(5, np.int32)
-        centre = np.zeros(2, np.float64)
         device = out is not None and _is_device(out)
-        names = ["elevation_raw", "elevation", "segmentation", "plane_classification"]
+        size = None if out is None else _flat_out(out)
         with self.map_lock:
-            c = self.center.astype(np.float64)
-            self._check(self._L.emap_submap_windows(self.cell_n, float(self.resolution), c.ctypes.data, 1,
-                                                    req.ctypes.data, win.ctypes.data, centre.ctypes.data))
-            rows, cols = int(win[3]), int(win[4])
-            cap = max(int(self._L.emap_plane_capacity(rows, cols, C.byref(p))), 1)
-            if device:
-                import torch
-                if out.dtype != torch.float32 or not out.is_contiguous():
-                    raise TypeError("a device `out` must be a contiguous float32 torch CUDA tensor")
-                planes = torch.empty((cap, 7), dtype=torch.float64, device=out.device)
-                info = torch.zeros(5, dtype=torch.int32, device=out.device)
-                ptrs = (out.data_ptr(), out.numel(), planes.data_ptr(), info.data_ptr())
-                self._after_framework()
-            else:
-                if out is None:
-                    out = np.zeros(4 * rows * cols, np.float32)
-                if out.dtype != np.float32 or not out.flags.c_contiguous:
-                    raise TypeError("a host `out` must be a C-contiguous float32 NumPy array")
-                planes = np.zeros((cap, 7), np.float64)
-                info = np.zeros(5, np.int32)
-                ptrs = (out.ctypes.data, out.size, planes.ctypes.data, info.ctypes.data)
-            self._check(self._L.emap_segment_planes(self._h, req.ctypes.data, C.byref(p), ptrs[0], int(device),
-                                                    ptrs[1], ptrs[2], cap, ptrs[3]))
-            if device:
-                self._before_framework()
-        info_h = info.cpu().numpy() if device else info
-        n = rows * cols
-        flat = out.reshape(-1)
-        res = float(self.resolution)
-        return {"layers": {name: flat[k * n:(k + 1) * n].reshape(rows, cols) for k, name in enumerate(names)},
-                "planes": planes[:int(info_h[4])], "highest_label": int(info_h[3]),
-                "origin": centre + (0.5 * (np.array([rows, cols]) * res) - 0.5 * res), "centre": centre.copy(),
-                "resolution": res, "size": (rows, cols), "success": bool(info_h[0])}
+            rows, cols, res, centre, cap = self._plane_window(p, req)
+            if out is None:
+                out = np.zeros(len(_PLANE_LAYERS) * rows * cols, np.float32)
+                size = out.size
+            mk = _array_maker(out.device if device else None)
+            planes, info = mk((cap, 7), "float64"), mk(5, "int32")
+            self._ordered_call(self._L.emap_segment_planes, self._h, req.ctypes.data, C.byref(p), _address(out),
+                               int(device), size, _address(planes), cap, _address(info), after=device, before=device)
+        return _plane_result(_PLANE_LAYERS, out, rows, cols, res, centre, planes, info.cpu().numpy() if device else info)
 
     def extract_planar_regions(self, position, length, params=None, out=None, capacities=None):
         """The plane decomposition node's planar regions for the get_submap window around `position` (x, y) of `length`
@@ -653,55 +641,27 @@ class ElevationMap:
         (0 grown, 1 zero radius, 2 max iterations, 3 no region, 4 invalid query, 5 bad table), "iterations" and, with
         growth, "convex_plane" (N, V, 2) and "convex_world" (N, V, 3); all views of `out`."""
         tabs = terrain["tables"]
-        reg, poly, vert = tabs["regions"], tabs["polygons"], tabs["vertices"]
+        reg, poly, vert = (_input_array(tabs[k], dt, k[:-1] + " table", cols)
+                           for k, dt, cols in (("regions", "float64", 17), ("polygons", "int32", 5),
+                                               ("vertices", "float64", 2)))
         tables_dev = _is_device(reg)
-        n_conv = int(convex_vertices)
-        device = _is_device(queries) or (out is not None and _is_device(out["index"]))
-        if device:
-            import torch
-            dev = (queries if _is_device(queries) else out["index"]).device
-            if not _is_device(queries):
-                queries = torch.as_tensor(np.asarray(queries, np.float64), device=dev)
-            queries = queries.to(torch.float64).contiguous()
-            n = int(queries.shape[0])
-            if out is None:
-                out = {"index": torch.empty((n, 3), dtype=torch.int32, device=dev),
-                       "point": torch.empty((n, 6), dtype=torch.float64, device=dev)}
-                if n_conv:
-                    out["convex"] = torch.empty((n, n_conv, 5), dtype=torch.float64, device=dev)
-            ptr = lambda a: a.data_ptr() if a is not None else None  # noqa: E731
-            q_ptr = queries.data_ptr()
-        else:
-            queries = np.ascontiguousarray(queries, np.float64)
-            n = int(queries.shape[0])
-            if out is None:
-                out = {"index": np.zeros((n, 3), np.int32), "point": np.zeros((n, 6), np.float64)}
-                if n_conv:
-                    out["convex"] = np.zeros((n, n_conv, 5), np.float64)
-            ptr = lambda a: a.ctypes.data if a is not None else None  # noqa: E731
-            q_ptr = queries.ctypes.data
-        if queries.shape != (n, 3):
+        if _is_device(poly) != tables_dev or _is_device(vert) != tables_dev:
+            raise TypeError("the region tables must be all NumPy or all torch CUDA")
+        if np.ndim(queries) != 2 or np.shape(queries)[1] != 3:
             raise ValueError("queries must be (N, 3)")
-        shapes = {"index": (n, 3), "point": (n, 6), "convex": (n, n_conv, 5)}
-        for k in ("index", "point") + (("convex",) if n_conv else ()):
-            a = out[k]
-            if tuple(a.shape) != shapes[k] or _is_device(a) != device or not (
-                    a.is_contiguous() if device else a.flags.c_contiguous):
-                raise TypeError("out[%r] must be a contiguous %s array of shape %s" % (
-                    k, "CUDA" if device else "NumPy", shapes[k]))
-        tptr = (lambda a: a.data_ptr()) if tables_dev else (lambda a: np.ascontiguousarray(a).ctypes.data)  # noqa: E731
-        if not tables_dev:
-            reg, poly, vert = (np.ascontiguousarray(a, dt) for a, dt in ((reg, np.float64), (poly, np.int32),
-                                                                        (vert, np.float64)))
-        t = _lib.EmapRegionTables(tptr(reg), len(reg), tptr(poly), len(poly), tptr(vert), len(vert))
-        o = _lib.EmapProjectionOut(ptr(out["index"]), ptr(out["point"]), ptr(out.get("convex") if n_conv else None))
-        if device or tables_dev:
-            self._after_framework()
-        self._check(self._L.emap_project_to_planar_regions(self._h, C.byref(t), int(tables_dev), n, q_ptr,
-                                                           int(_is_device(queries)), float(penalty_z_weight), n_conv,
-                                                           float(growth_factor), C.byref(o), int(device)))
-        if device:
-            self._before_framework()
+        q = _queries((queries,), 3)
+        n, n_conv = int(q.shape[0]), int(convex_vertices)
+        dev = _output_device([q, *(out or {}).values()])
+        device = dev is not None
+        specs = {"index": ((n, 3), "int32"), "point": ((n, 6), "float64")}
+        if n_conv:
+            specs["convex"] = ((n, n_conv, 5), "float64")
+        out = _outputs(out, specs, dev)
+        t = _lib.EmapRegionTables(_address(reg), len(reg), _address(poly), len(poly), _address(vert), len(vert))
+        o = _lib.EmapProjectionOut(_address(out["index"]), _address(out["point"]), _address(out["convex"]) if n_conv else None)
+        self._ordered_call(self._L.emap_project_to_planar_regions, self._h, C.byref(t), int(tables_dev), n, _address(q),
+                           int(_is_device(q)), float(penalty_z_weight), n_conv, float(growth_factor), C.byref(o),
+                           int(device), after=device or tables_dev, before=device)
         index, point = out["index"], out["point"]
         region = index[:, 0]
         if device:
@@ -729,12 +689,13 @@ class ElevationMap:
         (N, 3) float64, both NumPy or both torch CUDA, written in place.  Device queries or a device `out` keep
         everything on the device.  Returns "valid", "value", "index" (N, 2: the LAST finite cell of the line, as the
         reference returns) and "position" (N, 2: that cell's position); all views of `out`."""
-        g, g_dev, lines, n, device, mk, ptr = self._lookup_args(grid, layer, (starts, ends), 4, out, ("index",))
-        if out is None:
-            out = {"index": mk((n, 3), "int32"), "value": mk((n, 3), "float64")}
-        _check_out(out, {"index": (n, 3), "value": (n, 3)}, device)
-        o = _lib.EmapLineMaxOut(ptr(out["index"]), ptr(out["value"]))
-        self._lookup_call(self._L.emap_max_values_between, g, g_dev, n, lines, C.byref(o), device)
+        g = self._grid(grid, layer)
+        lines = _queries((starts, ends), 4)
+        n = int(lines.shape[0])
+        dev = _output_device([lines, *(out or {}).values()])
+        out = _outputs(out, {"index": ((n, 3), "int32"), "value": ((n, 3), "float64")}, dev)
+        o = _lib.EmapLineMaxOut(_address(out["index"]), _address(out["value"]))
+        self._lookup_call(self._L.emap_max_values_between, g, lines, C.byref(o), dev is not None)
         index, value = out["index"], out["value"]
         return {"valid": index[:, 0] != 0, "value": value[:, 0], "index": index[:, 1:], "position": value[:, 1:]}
 
@@ -745,14 +706,18 @@ class ElevationMap:
         or a device layer the results stay on the device.  `capacity`: the rows to start from (None: the largest total
         this map has returned before).  When it is too small the call is repeated once with the exact total.  Returns
         "rows" (total, 3: x, y, value), "counts" (N) and "first" (N: where line i's rows start), "retried"."""
-        g, g_dev, lines, n, device, mk, ptr = self._lookup_args(grid, layer, (starts, ends), 4, None, (), True)
+        g = self._grid(grid, layer)
+        lines = _queries((starts, ends), 4)
+        n = int(lines.shape[0])
+        dev = _output_device([lines, g._keep])
+        mk = _array_maker(dev)
         cap = int(capacity if capacity is not None else self._values_cap)
         counts, first, info = mk((n,), "int32"), mk((n,), "int64"), mk((2,), "int64")
         for attempt in range(2):
             rows = mk((max(cap, 1), 3), "float64")
-            o = _lib.EmapLineValuesOut(ptr(rows), cap, ptr(counts), ptr(first), ptr(info))
-            self._lookup_call(self._L.emap_values_between, g, g_dev, n, lines, C.byref(o), device)
-            info_h = info.cpu().numpy() if device else info
+            o = _lib.EmapLineValuesOut(_address(rows), cap, _address(counts), _address(first), _address(info))
+            self._lookup_call(self._L.emap_values_between, g, lines, C.byref(o), dev is not None)
+            info_h = info.cpu().numpy() if dev is not None else info
             if info_h[1]:
                 break
             cap = int(info_h[0])
@@ -766,14 +731,14 @@ class ElevationMap:
         (at least 5 x 5 cells); `positions`: (N, 2) map-frame points.  `out`: None, or a dict of "index" (N, 3) int32
         and "value" (N, 2 or 5) float64.  Returns "status" (0 inside, 1 outside: zero derivatives), "index" (N, 2),
         "gradient" (N, 2: x, y) and, with curvature, "curvature" (N, 3: xx, xy, yy); all views of `out`."""
-        g, g_dev, pos, n, device, mk, ptr = self._lookup_args(grid, layer, (positions,), 2, out, ("index",))
-        nv = 5 if curvature else 2
-        if out is None:
-            out = {"index": mk((n, 3), "int32"), "value": mk((n, nv), "float64")}
-        _check_out(out, {"index": (n, 3), "value": (n, nv)}, device)
-        o = _lib.EmapDerivativeOut(ptr(out["index"]), ptr(out["value"]))
+        g = self._grid(grid, layer)
+        pos = _queries((positions,), 2)
+        n = int(pos.shape[0])
+        dev = _output_device([pos, *(out or {}).values()])
+        out = _outputs(out, {"index": ((n, 3), "int32"), "value": ((n, 5 if curvature else 2), "float64")}, dev)
+        o = _lib.EmapDerivativeOut(_address(out["index"]), _address(out["value"]))
         call = lambda *a: self._L.emap_grid_derivatives(*a[:6], int(bool(curvature)), *a[6:])  # noqa: E731
-        self._lookup_call(call, g, g_dev, n, pos, C.byref(o), device)
+        self._lookup_call(call, g, pos, C.byref(o), dev is not None)
         index, value = out["index"], out["value"]
         res = {"status": index[:, 0], "index": index[:, 1:], "gradient": value[:, :2]}
         if curvature:
@@ -802,53 +767,26 @@ class ElevationMap:
             raise ValueError("1 to %d layers" % _lib.EMAP_VALUES_MAX_LAYERS)
         nl, m = len(names), _lib.EMAP_VALUES_METHODS[method]
         if grid is not None:
-            g, g_dev, q, n, device, mk, ptr = self._lookup_args(grid, names[0], (positions,), 2, out,
-                                                                ("values", "status"))
-            grids = [g] + [self._lookup_args(grid, name, (), 0, None, ())[0] for name in names[1:]]
+            grids = [self._grid(grid, name) for name in names]
+            g_dev = _is_device(grids[0]._keep)
             if any(_is_device(x._keep) != g_dev for x in grids):
                 raise TypeError("the grid's layers must be all NumPy or all torch CUDA")
-        else:
-            for name in names:
-                if not (name in EXPORT_NAMES or name in self.semantic_map.layer_names
-                        or name in self.plugin_manager.layer_names):
-                    raise KeyError("Layer {} is not in the map".format(name))
-            g_dev = False
-            q_dev = _is_device(positions)
-            out_dev = [a for a in (out or {}).values() if _is_device(a)]
-            device = q_dev or bool(out_dev)
-            if q_dev:
-                import torch
-                q = positions.to(torch.float64).reshape(-1, 2).contiguous()
-            else:
-                q = np.ascontiguousarray(np.asarray(_to_host(positions), np.float64).reshape(-1, 2))
-            n = int(q.shape[0])
-            mk, ptr = _array_maker((positions.device if q_dev else out_dev[0].device) if device else None)
-        if out is None:
-            out = {"values": mk((nl, n), "float32"), "status": mk((n,), "int32")}
-        _check_out(out, {"values": (nl, n), "status": (n,)}, device)
-        o = _lib.EmapValuesOut(ptr(out["values"]), ptr(out["status"]))
-        q_dev = _is_device(q)
-        q_ptr = q.data_ptr() if q_dev else q.ctypes.data
+        q = _queries((positions,), 2)
+        n, q_dev = int(q.shape[0]), _is_device(q)
+        dev = _output_device([q, *(out or {}).values()])
+        device = dev is not None
+        out = _outputs(out, {"values": ((nl, n), "float32"), "status": ((n,), "int32")}, dev)
+        o = _lib.EmapValuesOut(_address(out["values"]), _address(out["status"]))
         if grid is not None:
-            arr = (_lib.EmapGrid * nl)(*grids)
-            if device or g_dev or q_dev:
-                self._after_framework()
-            self._check(self._L.emap_grid_values_at(self._h, nl, arr, int(g_dev), n, q_ptr, int(q_dev), m, C.byref(o),
-                                                    int(device)))
-            if device:
-                self._before_framework()
+            self._ordered_call(self._L.emap_grid_values_at, self._h, nl, (_lib.EmapGrid * nl)(*grids), int(g_dev), n,
+                               _address(q), int(q_dev), m, C.byref(o), int(device), after=device or g_dev or q_dev,
+                               before=device)
         else:
             with self.map_lock:
-                sources = [self._export_source(name) for name in names]
-                c_names = (C.c_char_p * nl)(*[s[0].encode() for s in sources])
-                planes = (C.c_void_p * nl)(*[s[1] for s in sources])
-                flags = (C.c_int32 * nl)(*[s[2] for s in sources])
-                if device or q_dev or any(s[3] is not None for s in sources):
-                    self._after_framework()
-                self._check(self._L.emap_map_values_at(self._h, nl, c_names, planes, flags, n, q_ptr, int(q_dev), m,
-                                                       C.byref(o), int(device)))
-                if device:
-                    self._before_framework()
+                c_names, planes, flags, framework = self._layer_sources(names)
+                self._ordered_call(self._L.emap_map_values_at, self._h, nl, c_names, planes, flags, n, _address(q),
+                                   int(q_dev), m, C.byref(o), int(device), after=device or q_dev or framework,
+                                   before=device)
         values = out["values"]
         return {"values": {name: values[k] for k, name in enumerate(names)}, "status": out["status"]}
 
@@ -864,8 +802,10 @@ class ElevationMap:
         float32 NumPy array or CUDA tensor, written in place; a device layer or `out` keeps the volume on the device
         (stream-ordered, no host synchronisation with `z_range`).  Returns "volume" (n_z, rows, cols), "rows", "cols",
         "n_z", "position", "resolution" and "z_min": the dict sdf_values takes."""
-        g, g_dev, _, _, device, mk, ptr = self._lookup_args(grid, layer, (), 0, None if out is None else {"volume": out},
-                                                            ("volume",), True)
+        g = self._grid(grid, layer)
+        g_dev = _is_device(g._keep)
+        dev = _output_device([out, g._keep])
+        device = dev is not None
         res = float(g.resolution)
         if z_range is None:
             data = g._keep
@@ -887,14 +827,11 @@ class ElevationMap:
             n_z = int(math.floor((float(z_range[1]) - z_min) / res)) + 1
         shape = (n_z, int(g.rows), int(g.cols))
         if out is None:
-            out = mk(shape, "float32")
-        _check_out({"volume": out}, {"volume": shape}, device)
-        if device or g_dev:
-            self._after_framework()
-        self._check(self._L.emap_signed_distance_field(self._h, C.byref(g), int(g_dev), z_min, n_z, ptr(out),
-                                                       out.numel() if device else out.size, int(device)))
-        if device:
-            self._before_framework()
+            out = _array_maker(dev)(shape, "float32")
+        _check_out({"volume": out}, {"volume": (shape, "float32")}, device)
+        self._ordered_call(self._L.emap_signed_distance_field, self._h, C.byref(g), int(g_dev), z_min, n_z,
+                           _address(out), out.numel() if device else out.size, int(device), after=device or g_dev,
+                           before=device)
         return {"volume": out, "rows": int(g.rows), "cols": int(g.cols), "n_z": n_z,
                 "position": np.array(g.position[:], np.float64), "resolution": res, "z_min": z_min}
 
@@ -904,36 +841,21 @@ class ElevationMap:
         signed_distance_field (its "volume" read in place, NumPy or torch CUDA).  `points`: (N, 3) map-frame points,
         float64 NumPy or a CUDA tensor.  `out`: None, or an (N, 4) float64 array, NumPy or torch CUDA, written in place.
         Device points or a device `out` keep everything on the device.  Returns (N, 4): value, d/dx, d/dy, d/dz."""
-        vol = field["volume"]
-        f_dev = _is_device(vol)
-        if f_dev:
-            import torch
-            if vol.dtype != torch.float32 or not vol.is_contiguous():
-                raise TypeError("a device volume must be a contiguous float32 torch CUDA tensor")
-            v_ptr = vol.data_ptr()
-        else:
-            vol = np.ascontiguousarray(vol, np.float32)
-            v_ptr = vol.ctypes.data
+        vol = _input_array(field["volume"], "float32", "volume")
         n_z, rows, cols = (int(field[k]) for k in ("n_z", "rows", "cols"))
         if tuple(vol.shape) != (n_z, rows, cols):
             raise ValueError("the volume must be (n_z, rows, cols)")
         pos = np.asarray(_to_host(field["position"]), np.float64)
-        f = _lib.EmapSdf(v_ptr, rows, cols, n_z, (C.c_double * 2)(*pos.tolist()), float(field["resolution"]),
+        f = _lib.EmapSdf(_address(vol), rows, cols, n_z, (C.c_double * 2)(*pos.tolist()), float(field["resolution"]),
                          float(field["z_min"]))
         f._keep = vol
-        q_dev = _is_device(points)
-        device = q_dev or (out is not None and _is_device(out))
-        if q_dev:
-            import torch
-            q = points.to(torch.float64).reshape(-1, 3).contiguous()
-        else:
-            q = np.ascontiguousarray(np.asarray(points, np.float64).reshape(-1, 3))
+        q = _queries((points,), 3)
         n = int(q.shape[0])
+        dev = _output_device([q, out])
         if out is None:
-            out = _array_maker(points.device if device else None)[0]((n, 4), "float64")
-        _check_out({"value": out}, {"value": (n, 4)}, device)
-        ptr = (lambda a: a.data_ptr()) if device else (lambda a: a.ctypes.data)  # noqa: E731
-        self._lookup_call(self._L.emap_sdf_values, f, f_dev, n, q, ptr(out), device)
+            out = _array_maker(dev)((n, 4), "float64")
+        _check_out({"value": out}, {"value": ((n, 4), "float64")}, dev is not None)
+        self._lookup_call(self._L.emap_sdf_values, f, q, _address(out), dev is not None)
         return out
 
     def inpaint_image(self, image, mask, radius=1, method="ns", out=None):
@@ -946,26 +868,21 @@ class ElevationMap:
         methods = {"telea": 0, "ns": 1}
         if method not in methods:
             raise ValueError("method must be 'ns' or 'telea'")
-        device = _is_device(image) or _is_device(mask) or (out is not None and _is_device(out))
+        dev = _output_device([image, mask, out])
+        device = dev is not None
         if device:
             import torch
-            dev = next(a.device for a in (image, mask, out) if a is not None and _is_device(a))
             image, mask = (torch.as_tensor(a, device=dev).to(torch.uint8).contiguous() for a in (image, mask))
         else:
             image, mask = (np.ascontiguousarray(_to_host(a), np.uint8) for a in (image, mask))
         if image.ndim != 2 or tuple(mask.shape) != tuple(image.shape):
             raise ValueError("image and mask must be (rows, cols) of the same shape")
         rows, cols = (int(v) for v in image.shape)
-        mk, ptr = _array_maker(dev if device else None)
         if out is None:
-            out = mk((rows, cols), "uint8")
-        _check_out({"image": out}, {"image": (rows, cols)}, device)
-        if device:
-            self._after_framework()
-        self._check(self._L.emap_inpaint_image(self._h, ptr(image), ptr(mask), rows, cols, float(radius),
-                                               methods[method], ptr(out), int(device)))
-        if device:
-            self._before_framework()
+            out = _array_maker(dev)((rows, cols), "uint8")
+        _check_out({"image": out}, {"image": ((rows, cols), "uint8")}, device)
+        self._ordered_call(self._L.emap_inpaint_image, self._h, _address(image), _address(mask), rows, cols,
+                           float(radius), methods[method], _address(out), int(device), after=device, before=device)
         return out
 
     def nonlinear_interpolation(self, grid, layer="elevation", inpaint_radius=None, out=None):
@@ -977,71 +894,36 @@ class ElevationMap:
         (None: the grid's resolution) must round to 1 pixel.  `out`: None (on the layer's side), or a contiguous (rows,
         cols) float32 NumPy array or CUDA tensor, written in place; device output is stream-ordered with no host
         synchronisation.  Returns `out`."""
-        g, g_dev, _, _, _, _, _ = self._lookup_args(grid, layer, (), 0, None, (), True)
-        device = _is_device(out) if out is not None else g_dev
-        mk, ptr = _array_maker((out.device if out is not None else g._keep.device) if device else None)
+        g = self._grid(grid, layer)
+        g_dev = _is_device(g._keep)
+        dev = _output_device([g._keep if out is None else out])
+        device = dev is not None
         shape = (int(g.rows), int(g.cols))
         if out is None:
-            out = mk(shape, "float32")
-        _check_out({"layer": out}, {"layer": shape}, device)
+            out = _array_maker(dev)(shape, "float32")
+        _check_out({"layer": out}, {"layer": (shape, "float32")}, device)
         radius = float(g.resolution if inpaint_radius is None else inpaint_radius)
-        if device or g_dev:
-            self._after_framework()
-        self._check(self._L.emap_nonlinear_interpolation(self._h, C.byref(g), int(g_dev), radius, ptr(out),
-                                                         int(device)))
-        if device:
-            self._before_framework()
+        self._ordered_call(self._L.emap_nonlinear_interpolation, self._h, C.byref(g), int(g_dev), radius, _address(out),
+                           int(device), after=device or g_dev, before=device)
         return out
 
-    def _lookup_args(self, grid, layer, parts, width, out, out_keys, follow_grid=False):
-        """What the lookups and the distance field share: the layer's emap_grid (the grid dict's "centre", its
-        "resolution" or the map's), the queries as one contiguous (N, width) float64 array (NumPy, or a CUDA tensor when
-        any part is one; None without parts), whether
-        the call writes device output (device queries, a device `out` or, with follow_grid, a device layer), and an
-        array maker and pointer getter for that side."""
-        data = grid["layers"][layer]
-        g_dev = _is_device(data)
-        if g_dev:
-            import torch
-            if data.dtype != torch.float32 or not data.is_contiguous():
-                raise TypeError("a device layer must be a contiguous float32 torch CUDA tensor")
-            d_ptr = data.data_ptr()
-        else:
-            data = np.ascontiguousarray(data, np.float32)
-            d_ptr = data.ctypes.data
+    def _grid(self, grid, layer):
+        """The EmapGrid of grid["layers"][layer] (_input_array, kept alive as g._keep), centred at the dict's "centre" or,
+        in a get_transformed_submap(s) dict, its "frame_centre", with its "resolution" or the map's."""
+        data = _input_array(grid["layers"][layer], "float32", "layer")
         rows, cols = (int(s) for s in data.shape)
-        res = float(grid.get("resolution", self.resolution))
-        centre = np.asarray(_to_host(grid["centre"]), np.float64)
-        g = _lib.EmapGrid(d_ptr, rows, cols, (C.c_double * 2)(*centre.tolist()), res)
+        centre = np.asarray(_to_host(grid["centre"] if "centre" in grid else grid["frame_centre"]), np.float64)
+        g = _lib.EmapGrid(_address(data), rows, cols, (C.c_double * 2)(*centre.tolist()),
+                          float(grid.get("resolution", self.resolution)))
         g._keep = data
-        q_dev = any(_is_device(p) for p in parts)
-        out_dev = [out[k] for k in out_keys if _is_device(out[k])] if out is not None else []
-        device = q_dev or bool(out_dev) or (follow_grid and g_dev)
-        dev = None
-        if not parts:
-            q = None
-        elif q_dev:
-            import torch
-            dev = next(p.device for p in parts if _is_device(p))
-            q = torch.cat([torch.as_tensor(p, device=dev).to(torch.float64).reshape(-1, width // len(parts))
-                           for p in parts], 1).contiguous()
-        else:
-            q = np.ascontiguousarray(np.concatenate([np.asarray(p, np.float64).reshape(-1, width // len(parts))
-                                                     for p in parts], 1))
-        n = int(q.shape[0]) if parts else 0
-        if device and dev is None:
-            dev = out_dev[0].device if out_dev else data.device
-        mk, ptr = _array_maker(dev if device else None)
-        return g, g_dev, q, n, device, mk, ptr
+        return g
 
-    def _lookup_call(self, fn, g, g_dev, n, queries, out, device):
-        q_dev = _is_device(queries)
-        q_ptr = queries.data_ptr() if q_dev else queries.ctypes.data
-        if device or g_dev or q_dev:
-            self._after_framework()
-        self._check(fn(self._h, C.byref(g), int(g_dev), n, q_ptr, int(q_dev), out, int(device)))
-        if device:
-            self._before_framework()
+    def _lookup_call(self, fn, g, queries, out, device):
+        """fn(handle, grid, grid on device, n, queries, queries on device, out, device output), the lookup on `g` (an
+        EmapGrid or EmapSdf whose array is g._keep) of the (n, k) `queries` (_queries), stream-ordered."""
+        g_dev, q_dev = _is_device(g._keep), _is_device(queries)
+        self._ordered_call(fn, self._h, C.byref(g), int(g_dev), int(queries.shape[0]), _address(queries), int(q_dev),
+                           out, int(device), after=device or g_dev or q_dev, before=device)
 
     def plane_decomposition(self, grid, layer="elevation", params=None, out=None, capacities=None):
         """The plane decomposition node's pipeline (PlaneDecompositionPipeline::update without RANSAC refinement) on a
@@ -1053,154 +935,94 @@ class ElevationMap:
         "resolution", "origin" and "centre" are its geometry, and "elevation_raw" is the input layer itself (the node's
         submap before the preprocessing, at its own size).  The result feeds project_to_planar_regions and the
         lookups as planar_terrain's does."""
-        data = grid["layers"][layer]
-        g_dev = _is_device(data)
-        if g_dev:
-            import torch
-            if data.dtype != torch.float32 or not data.is_contiguous():
-                raise TypeError("a device layer must be a contiguous float32 torch CUDA tensor")
-            d_ptr = data.data_ptr()
-        else:
-            data = np.ascontiguousarray(data, np.float32)
-            d_ptr = data.ctypes.data
-        rows_in, cols_in = (int(v) for v in data.shape)
-        res_in = float(grid.get("resolution", self.resolution))
-        centre = np.asarray(_to_host(grid["centre"] if "centre" in grid else grid["frame_centre"]), np.float64)
-        g = _lib.EmapGrid(d_ptr, rows_in, cols_in, (C.c_double * 2)(*centre.tolist()), res_in)
-        from .plane_segmentation import PlaneSegmentationParams
-        p = (params or PlaneSegmentationParams()).to_c()
-        size = np.zeros(2, np.int64)
-        res = C.c_double(0.0)
-        self._check(self._L.emap_plane_grid_geometry(rows_in, cols_in, res_in, C.byref(p), size.ctypes.data,
-                                                     C.addressof(res)))
-        geometry = (int(size[0]), int(size[1]), res.value, centre)
-
-        def call(p, rp, pp, lay, device, planes, cap, ro, info):
-            return self._L.emap_plane_decomposition(self._h, C.byref(g), int(g_dev), C.byref(p), C.byref(rp),
-                                                    C.byref(pp), lay[0], int(device), lay[1], planes, cap,
-                                                    C.byref(ro), info)
-        result = self._planar_regions(None, None, params, out, capacities, True, geometry, call, g_dev)
-        result["layers"]["elevation_raw"] = data
+        g = self._grid(grid, layer)
+        result = self._planar_regions(None, None, params, out, capacities, True, g)
+        result["layers"]["elevation_raw"] = g._keep
         return result
 
-    def _planar_regions(self, position, length, params, out, capacities, post, geometry=None, call=None,
-                        grid_dev=False):
-        """extract_planar_regions (post False), planar_terrain (post True) and plane_decomposition (geometry = the
-        resampled (rows, cols, resolution, centre), `call` its library call and grid_dev whether it reads device
-        memory): the call with the capacity retry."""
+    def _plane_window(self, p, req=None, grid=None):
+        """(rows, cols, resolution, centre, plane-table rows) of a plane call with the emap_plane_params `p`: the
+        get_submap window `req` of this map, or the EmapGrid `grid` resampled to p's resolution."""
+        if grid is None:
+            win, centre = np.zeros(5, np.int32), np.zeros(2, np.float64)
+            c = self.center.astype(np.float64)
+            self._check(self._L.emap_submap_windows(self.cell_n, float(self.resolution), c.ctypes.data, 1,
+                                                    req.ctypes.data, win.ctypes.data, centre.ctypes.data))
+            rows, cols, res = int(win[3]), int(win[4]), float(self.resolution)
+        else:
+            size, r = np.zeros(2, np.int64), C.c_double(0.0)
+            self._check(self._L.emap_plane_grid_geometry(grid.rows, grid.cols, grid.resolution, C.byref(p),
+                                                         size.ctypes.data, C.addressof(r)))
+            rows, cols, res, centre = int(size[0]), int(size[1]), r.value, np.array(grid.position[:], np.float64)
+        return rows, cols, res, centre, max(int(self._L.emap_plane_capacity(rows, cols, C.byref(p))), 1)
+
+    def _planar_regions(self, position, length, params, out, capacities, post, grid=None):
+        """extract_planar_regions (post False), planar_terrain (post True) and plane_decomposition (post True, `grid` the
+        EmapGrid it reads): the call with the capacity retry."""
         from .plane_segmentation import PlaneSegmentationParams
         prm = params or PlaneSegmentationParams()
         p, rp = prm.to_c(), prm.regions_to_c()
         pp = prm.postprocess_to_c() if post else None
-        n_layers = _lib.EMAP_TERRAIN_LAYERS if post else 4
-        if geometry is None:
-            req = np.array(_xy(position) + _xy(length), np.float64)
-        win = np.zeros(5, np.int32)
-        centre = np.zeros(2, np.float64)
         device = out is not None and _is_device(out)
-        names = ["elevation_raw", "elevation", "segmentation", "plane_classification"]
-        if post:
-            names = ["elevation_raw", "elevation_before_postprocess", "segmentation", "plane_classification",
-                     "elevationWithNaN", "elevationWithNaN_i", "elevationWithNaNClosed",
-                     "elevationWithNaNClosedDilated", "smooth_planar", "elevation"]
+        size = None if out is None else _flat_out(out)
+        names = _TERRAIN_LAYERS if post else _PLANE_LAYERS
+        if grid is None:
+            req = np.array(_xy(position) + _xy(length), np.float64)
+            fn = self._L.emap_planar_terrain if post else self._L.emap_extract_planar_regions
+            head = (req.ctypes.data, C.byref(p), C.byref(rp)) + ((C.byref(pp),) if post else ())
+            reads_framework = device
+        else:
+            req = None
+            fn = self._L.emap_plane_decomposition
+            head = (C.byref(grid), int(_is_device(grid._keep)), C.byref(p), C.byref(rp), C.byref(pp))
+            reads_framework = device or _is_device(grid._keep)
         caps = tuple(int(v) for v in (capacities or self._region_caps))
         for attempt in range(2):
             with self.map_lock:
-                if geometry is None:
-                    c = self.center.astype(np.float64)
-                    self._check(self._L.emap_submap_windows(self.cell_n, float(self.resolution), c.ctypes.data, 1,
-                                                            req.ctypes.data, win.ctypes.data, centre.ctypes.data))
-                    rows, cols = int(win[3]), int(win[4])
-                    res = float(self.resolution)
-                else:
-                    rows, cols, res, centre = geometry
-                cap = max(int(self._L.emap_plane_capacity(rows, cols, C.byref(p))), 1)
-                if device:
-                    import torch
-                    if out.dtype != torch.float32 or not out.is_contiguous():
-                        raise TypeError("a device `out` must be a contiguous float32 torch CUDA tensor")
-                    mk = lambda shape, dt: torch.empty(shape, dtype=dt, device=out.device)  # noqa: E731
-                    f64, i32 = torch.float64, torch.int32
-                    ptr = lambda a: a.data_ptr()  # noqa: E731
-                else:
-                    if out is None:
-                        out = np.zeros(n_layers * rows * cols, np.float32)
-                    if out.dtype != np.float32 or not out.flags.c_contiguous:
-                        raise TypeError("a host `out` must be a C-contiguous float32 NumPy array")
-                    mk = lambda shape, dt: np.zeros(shape, dt)  # noqa: E731
-                    f64, i32 = np.float64, np.int32
-                    ptr = lambda a: a.ctypes.data  # noqa: E731
-                planes, info = mk((cap, 7), f64), mk(9, i32)
-                tables = (mk((max(caps[0], 1), 17), f64), mk((max(caps[1], 1), 5), i32), mk((max(caps[2], 1), 2), f64))
-                ro = _lib.EmapRegionOut(ptr(tables[0]), caps[0], ptr(tables[1]), caps[1], ptr(tables[2]), caps[2])
-                lay = (out.data_ptr(), out.numel()) if device else (out.ctypes.data, out.size)
-                if device or grid_dev:
-                    self._after_framework()
-                if call is not None:
-                    self._check(call(p, rp, pp, lay, device, ptr(planes), cap, ro, ptr(info)))
-                elif post:
-                    self._check(self._L.emap_planar_terrain(self._h, req.ctypes.data, C.byref(p), C.byref(rp),
-                                                            C.byref(pp), lay[0], int(device), lay[1], ptr(planes), cap,
-                                                            C.byref(ro), ptr(info)))
-                else:
-                    self._check(self._L.emap_extract_planar_regions(self._h, req.ctypes.data, C.byref(p), C.byref(rp),
-                                                                    lay[0], int(device), lay[1], ptr(planes), cap,
-                                                                    C.byref(ro), ptr(info)))
-                if device:
-                    self._before_framework()
+                rows, cols, res, centre, cap = self._plane_window(p, req, grid)
+                if out is None:
+                    out = np.zeros(len(names) * rows * cols, np.float32)
+                    size = out.size
+                mk = _array_maker(out.device if device else None)
+                planes, info = mk((cap, 7), "float64"), mk(9, "int32")
+                tables = (mk((max(caps[0], 1), 17), "float64"), mk((max(caps[1], 1), 5), "int32"),
+                          mk((max(caps[2], 1), 2), "float64"))
+                ro = _lib.EmapRegionOut(_address(tables[0]), caps[0], _address(tables[1]), caps[1], _address(tables[2]),
+                                        caps[2])
+                self._ordered_call(fn, self._h, *head, _address(out), int(device), size, _address(planes), cap,
+                                   C.byref(ro), _address(info), after=reads_framework, before=device)
             info_h = info.cpu().numpy() if device else info
             if info_h[8]:
                 break
             caps = (int(info_h[5]), int(info_h[6]), int(info_h[7]))
         self._region_caps = tuple(max(a, int(b)) for a, b in zip(self._region_caps, info_h[5:8]))
-        n = rows * cols
-        flat = out.reshape(-1)
         nr, npoly, nv = (int(x) for x in info_h[5:8])
         reg, poly, vert = tables[0][:nr], tables[1][:npoly], tables[2][:nv]
-        result = {"layers": {name: flat[k * n:(k + 1) * n].reshape(rows, cols) for k, name in enumerate(names)},
-                  "planes": planes[:int(info_h[4])], "highest_label": int(info_h[3]),
-                  "origin": centre + (0.5 * (np.array([rows, cols]) * res) - 0.5 * res), "centre": centre.copy(),
-                  "resolution": res, "size": (rows, cols), "success": bool(info_h[0]), "complete": bool(info_h[8]),
-                  "tables": {"regions": reg, "polygons": poly, "vertices": vert}, "regions": None,
-                  "retried": attempt > 0}
+        result = _plane_result(names, out, rows, cols, res, centre, planes, info_h)
+        result.update(complete=bool(info_h[8]), tables={"regions": reg, "polygons": poly, "vertices": vert},
+                      regions=None, retried=attempt > 0)
         if not device and info_h[8]:
             result["regions"] = regions_from_tables(reg, poly, vert)
         return result
 
     def _window_views(self, layers, out, cells, call, sizes):
-        """What get_submaps and get_transformed_submaps share: checks the layer names (KeyError before anything runs),
-        sizes a new host `out` with cells() (the host window arithmetic, which fills `sizes`), checks `out`, orders the
-        library call `call(n_layers, names, planes, flags, out pointer, is device, out floats)` after the caller's
-        stream and the caller's later work after it (device output), and returns per window a dict of (rows, cols)
-        views of `out` per layer, rows and cols read from `sizes` after the call."""
+        """What get_submaps and get_transformed_submaps share: checks `out` and the layer names before anything runs,
+        sizes a new host `out` with cells() (the host window arithmetic, which fills `sizes`), runs the library call
+        `call(n_layers, names, planes, flags, out pointer, is device, out floats)` stream-ordered and returns per window
+        a dict of (rows, cols) views of `out` per layer, rows and cols read from `sizes` after the call."""
         names = list(layers)
-        for name in names:
-            if not (name in EXPORT_NAMES or name in self.semantic_map.layer_names
-                    or name in self.plugin_manager.layer_names):
-                raise KeyError("Layer {} is not in the map".format(name))
         nl = len(names)
         device = out is not None and _is_device(out)
+        size = None if out is None else _flat_out(out)
         with self.map_lock:
+            c_names, planes, flags, framework = self._layer_sources(names)
             if out is None:
                 out = np.zeros(nl * cells(), np.float32)
-            if device:
-                import torch
-                if out.dtype != torch.float32 or not out.is_contiguous():
-                    raise TypeError("a device `out` must be a contiguous float32 torch CUDA tensor")
-                ptr, size = out.data_ptr(), out.numel()
-            else:
-                if out.dtype != np.float32 or not out.flags.c_contiguous:
-                    raise TypeError("a host `out` must be a C-contiguous float32 NumPy array")
-                ptr, size = out.ctypes.data, out.size
-            sources = [self._export_source(name) for name in names]
-            c_names = (C.c_char_p * nl)(*[s[0].encode() for s in sources])
-            planes = (C.c_void_p * nl)(*[s[1] for s in sources])
-            flags = (C.c_int32 * nl)(*[s[2] for s in sources])
-            if device or any(s[3] is not None for s in sources):
-                self._after_framework()       # the planes and the output buffer are complete / free
-            call(nl, c_names, planes, flags, ptr, int(device), size)
-            if device:
-                self._before_framework()      # framework reads of `out` run after the kernel (no host sync)
+                size = out.size
+            # after: the planes and the output buffer are complete / free; before: framework reads of `out` run after
+            # the kernel (no host sync)
+            self._ordered_call(call, nl, c_names, planes, flags, _address(out), int(device), size,
+                               after=device or framework, before=device)
         flat = out.reshape(-1)
         result, off = [], 0
         for rows, cols in sizes:
@@ -1218,7 +1040,7 @@ class ElevationMap:
         n = self.cell_n - 2
         maps = np.zeros((3, n, n), np.float32)
         with self.map_lock:
-            self._export([self._export_source(name) for name in ("normal_x", "normal_y", "normal_z")], maps)
+            self._export(["normal_x", "normal_y", "normal_z"], maps)
         return maps
 
     def get_normal_ref(self, normal_x_data, normal_y_data, normal_z_data):
@@ -1303,16 +1125,14 @@ class ElevationMap:
             n = len(planes)
             arr = lambda v: (C.c_int32 * max(n, 1))(*v)
             sem = self.semantic_map.semantic_map
-            self._after_framework()       # the stacked image and any layer the channels added are complete
-            rc = self._L.emap_input_image(
-                self._h, n_planes, img.data_ptr() if dev else img.ctypes.data, int(dev), H, W, Km.ctypes.data,
-                Dv.ctypes.data if Dv.size else None, int(Dv.size), str(distortion_model).encode(), Rm.ctypes.data,
-                tv.ctypes.data, n, arr(planes), arr(kinds), arr(layers), None if sem is None else sem.data_ptr(),
-                len(self.semantic_map.layer_names))
-            # framework work queued from here on sees the fused layers, and releases or rewrites a device image only after
-            # the kernel has read it (no host sync)
-            self._before_framework()
-            self._check(rc)
+            # the kernel runs after the stacked image and any layer the channels added are complete; framework work
+            # queued from here on sees the fused layers, and releases or rewrites a device image only after the kernel
+            # has read it (no host sync)
+            self._ordered_call(
+                self._L.emap_input_image, self._h, n_planes, img.data_ptr() if dev else img.ctypes.data, int(dev), H, W,
+                Km.ctypes.data, Dv.ctypes.data if Dv.size else None, int(Dv.size), str(distortion_model).encode(),
+                Rm.ctypes.data, tv.ctypes.data, n, arr(planes), arr(kinds), arr(layers),
+                None if sem is None else sem.data_ptr(), len(self.semantic_map.layer_names), after=True, before=True)
 
     # ---- not on the per-frame path ---------------------------------------------------------------
 
@@ -1464,24 +1284,99 @@ def regions_from_tables(regions, polygons, vertices):
     return out
 
 
+_PLANE_LAYERS = ["elevation_raw", "elevation", "segmentation", "plane_classification"]
+_TERRAIN_LAYERS = ["elevation_raw", "elevation_before_postprocess", "segmentation", "plane_classification",
+                   "elevationWithNaN", "elevationWithNaN_i", "elevationWithNaNClosed", "elevationWithNaNClosedDilated",
+                   "smooth_planar", "elevation"]
+
+
+def _plane_result(names, out, rows, cols, res, centre, planes, info):
+    """What segment_planes and the planar-region calls return alike, from the flat layers `out`, the plane table and
+    the first five info words: the (rows, cols) views per layer name, the planes, the window's geometry and success."""
+    n = rows * cols
+    flat = out.reshape(-1)
+    return {"layers": {name: flat[k * n:(k + 1) * n].reshape(rows, cols) for k, name in enumerate(names)},
+            "planes": planes[:int(info[4])], "highest_label": int(info[3]),
+            "origin": centre + (0.5 * (np.array([rows, cols]) * res) - 0.5 * res), "centre": centre.copy(),
+            "resolution": res, "size": (rows, cols), "success": bool(info[0])}
+
+
 def _array_maker(device):
-    """(make(shape, dtype name), pointer(array)) for new NumPy arrays (device None) or torch tensors on `device`."""
+    """make(shape, dtype name) for new NumPy arrays (device None) or torch tensors on `device`."""
     if device is None:
-        return (lambda shape, dt: np.zeros(shape, dt)), (lambda a: a.ctypes.data)
+        return lambda shape, dt: np.zeros(shape, dt)
     import torch
-    return (lambda shape, dt: torch.empty(shape, dtype=getattr(torch, dt), device=device)), (lambda a: a.data_ptr())
+    return lambda shape, dt: torch.empty(shape, dtype=getattr(torch, dt), device=device)
 
 
-def _check_out(out, shapes, device):
-    """Every out[k] is a contiguous array of shapes[k] on the call's side (NumPy for host output, CUDA for device)."""
-    dtypes = {"index": "int32", "value": "float64", "volume": "float32", "image": "uint8", "layer": "float32",
-              "values": "float32", "status": "int32"}
-    for k, shape in shapes.items():
+def _output_device(arrays):
+    """The device of the first CUDA array among `arrays` (None entries skipped): where a call that writes to the side of
+    these arrays puts its output; None for host output."""
+    return next((a.device for a in arrays if a is not None and _is_device(a)), None)
+
+
+def _contiguous(a, dtype, device):
+    """Is `a` a contiguous `dtype` torch CUDA tensor (device) or a C-contiguous `dtype` NumPy array (host)?"""
+    if device:
+        return str(getattr(a, "dtype", "")) == "torch." + dtype and a.is_contiguous()
+    return isinstance(a, np.ndarray) and a.dtype == dtype and a.flags.c_contiguous
+
+
+def _outputs(out, specs, dev):
+    """The caller's `out` dict, checked against specs (_check_out), or new arrays of specs[k] = (shape, dtype name) on
+    the device `dev` (None: NumPy) when it is None."""
+    if out is None:
+        return {k: _array_maker(dev)(shape, dt) for k, (shape, dt) in specs.items()}
+    _check_out(out, specs, dev is not None)
+    return out
+
+
+def _check_out(out, specs, device):
+    """Every out[k] is a contiguous array of specs[k] = (shape, dtype name) on the call's side (NumPy for host output,
+    CUDA for device)."""
+    for k, (shape, dtype) in specs.items():
         a = out[k]
-        if tuple(a.shape) != shape or _is_device(a) != device or str(a.dtype).split(".")[-1] != dtypes[k] or not (
-                a.is_contiguous() if device else a.flags.c_contiguous):
+        if tuple(a.shape) != shape or _is_device(a) != device or not _contiguous(a, dtype, device):
             raise TypeError("out[%r] must be a contiguous %s %s array of shape %s" % (
-                k, dtypes[k], "CUDA" if device else "NumPy", shape))
+                k, dtype, "CUDA" if device else "NumPy", shape))
+
+
+def _flat_out(out):
+    """The float count of the flat float32 `out` of the window and plane calls, which must be contiguous."""
+    if _is_device(out):
+        if not _contiguous(out, "float32", True):
+            raise TypeError("a device `out` must be a contiguous float32 torch CUDA tensor")
+        return out.numel()
+    if not _contiguous(out, "float32", False):
+        raise TypeError("a host `out` must be a C-contiguous float32 NumPy array")
+    return out.size
+
+
+def _input_array(a, dtype, what, columns=None):
+    """A grid layer, distance volume or region table (`what`) as the library reads it: a torch CUDA tensor is read in
+    place and must be contiguous `dtype`; a host array becomes a C-contiguous NumPy array of `dtype`.  A table must have
+    `columns` columns."""
+    if _is_device(a):
+        if not _contiguous(a, dtype, True):
+            raise TypeError("a device %s must be a contiguous %s torch CUDA tensor" % (what, dtype))
+    else:
+        a = np.ascontiguousarray(a, dtype)
+    if columns is not None and (a.ndim != 2 or a.shape[1] != columns):
+        raise TypeError("a %s must have %d columns" % (what, columns))
+    return a
+
+
+def _queries(parts, width):
+    """The query arrays `parts` side by side as one contiguous (N, width) float64 array: a torch CUDA tensor when any
+    part is one, else NumPy."""
+    k = width // len(parts)
+    dev = _output_device(parts)
+    if dev is not None:
+        import torch
+        parts = [torch.as_tensor(p, device=dev).to(torch.float64).reshape(-1, k) for p in parts]
+        return (torch.cat(parts, 1) if len(parts) > 1 else parts[0]).contiguous()
+    parts = [np.asarray(_to_host(p), np.float64).reshape(-1, k) for p in parts]
+    return np.ascontiguousarray(np.concatenate(parts, 1) if len(parts) > 1 else parts[0])
 
 
 def _is_device(x):
@@ -1535,6 +1430,9 @@ def _on_device(x):
 
 
 def _address(a):
+    """The data pointer of a NumPy array or torch tensor; None for None."""
+    if a is None:
+        return None
     return a.data_ptr() if hasattr(a, "data_ptr") else a.ctypes.data
 
 

@@ -1,5 +1,5 @@
 """Helpers shared by the built-in plugins: call a libemap.so stencil on torch CUDA tensors.
-Ordering with the caller's torch stream is by stream waits (ElevationMap._after_framework / _before_framework), never a host sync."""
+Ordering with the caller's torch stream is by stream waits (ElevationMap._ordered_call), never a host sync."""
 
 
 def require_engine(engine, who):
@@ -25,9 +25,8 @@ def run_plugin(eng, entry, planes, *args, ptrs=(), like=None):
     import torch
     planes = [as_plane(p) for p in planes]
     out = torch.empty_like(as_plane(planes[0] if planes else like))
-    eng._after_framework()
-    eng._check(getattr(eng._L, entry)(eng._h, *(p.data_ptr() for p in planes), *ptrs, out.data_ptr(), *args))
-    eng._before_framework()
+    eng._ordered_call(getattr(eng._L, entry), eng._h, *(p.data_ptr() for p in planes), *ptrs, out.data_ptr(), *args,
+                      after=True, before=True)
     return out
 
 
