@@ -75,6 +75,15 @@ class EmapGrid(C.Structure):
                 ("resolution", C.c_double)]
 
 
+class EmapFilterOp(C.Structure):
+    _fields_ = [("op", C.c_int32), ("kernel_size", C.c_int32), ("delta_kernel_size", C.c_int32),
+                ("number_of_repeats", C.c_int32), ("sigma", C.c_double), ("inpaint", C.c_int32)]
+
+
+EMAP_FILTER_OPS = {"min_values": 0, "median": 1, "box_blur": 2, "gaussian_blur": 3, "dilate": 4, "erode": 5,
+                   "outline": 6}
+
+
 class EmapLineMaxOut(C.Structure):
     _fields_ = [("index", C.c_void_p), ("value", C.c_void_p)]
 
@@ -215,6 +224,8 @@ SIGNATURES = {
                                      C.c_void_p, C.c_int32]),
     "emap_nonlinear_interpolation": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_double, C.c_void_p,
                                                C.c_int32]),
+    "emap_grid_filter": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.POINTER(EmapFilterOp), C.c_void_p,
+                                   C.c_void_p, C.c_int32]),
     "emap_plane_grid_geometry": (C.c_int, [C.c_int64, C.c_int64, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
     "emap_plane_decomposition": (C.c_int, [C.c_void_p, C.POINTER(EmapGrid), C.c_int32, C.c_void_p, C.c_void_p,
                                            C.c_void_p, C.c_void_p, C.c_int32, C.c_int64, C.c_void_p, C.c_int64,

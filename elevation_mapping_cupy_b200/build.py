@@ -15,7 +15,7 @@ HEADERS = ["emap_handle.cuh", "emap_kernels.cuh", "emap_export.cuh", "emap_plugi
            "emap_inpaint.cuh", "emap_semantic.cuh", "emap_polygon.cuh", "emap_semantic_plugins.cuh", "emap_image.cuh",
            "emap_submap.cuh", "emap_mapcloud.cuh", "emap_initialize.cuh", "emap_sources.cuh", "emap_plan.cuh",
            "emap_planes.cuh", "emap_regions.cuh", "emap_postprocess.cuh", "emap_terrain_query.cuh",
-           "emap_grid.cuh", "emap_grid_lookup.cuh", "emap_resample.cuh", "emap_sdf.cuh", "emap_values_at.cuh", os.path.join("..", "..", "include", "emap.h")]
+           "emap_grid.cuh", "emap_grid_lookup.cuh", "emap_resample.cuh", "emap_sdf.cuh", "emap_values_at.cuh", "emap_filters.cuh", os.path.join("..", "..", "include", "emap.h")]
 GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMPILE_FLAGS = ["-O3", "-std=c++17"] + GENCODE + ["-lineinfo", "-Xcompiler", "-fPIC", "-Xptxas", "-v"]
 LINK_FLAGS = GENCODE + ["-shared", "-cudart", "shared"]

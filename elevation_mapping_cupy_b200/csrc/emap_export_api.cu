@@ -11,6 +11,7 @@
 #include "emap_grid.cuh"
 #include "emap_mapcloud.cuh"
 #include "emap_values_at.cuh"
+#include "emap_filters.cuh"
 
 namespace {
 
@@ -860,7 +861,7 @@ static int postprocess_window(emap_handle* h, PlaneCall& c, const emap_postproce
   k_pp_slope<<<cb, PL_THREADS, 0, h->stream>>>(L[6], L[7], s.hdr, rows, cols, pc.dil, (float)c.res);
   LAUNCH_CHECK();
   // smooth_planar: boxFilter, then GaussianBlur (rows, then columns)
-  k_pp_box_rows<<<cb, PL_THREADS, 0, h->stream>>>(L[7], s.pd, s.hdr, rows, cols, pc.box / 2);
+  k_pp_box_rows<<<cb, PL_THREADS, 0, h->stream>>>(L[7], s.pd, s.hdr, rows, cols, pc.box);
   LAUNCH_CHECK();
   k_pp_box_cols<<<cb, PL_THREADS, 0, h->stream>>>(s.pd, a, s.hdr, rows, cols, pc.box / 2,
                                                    1.0 / ((double)pc.box * pc.box));
@@ -1108,6 +1109,198 @@ int emap_layer_device_ptr(emap_handle* h, const char* name, void** ptr) {
 int emap_exists_layer(const emap_handle* h, const char* name) {
   if (!h || !name) return 0;
   return layer_index(name) >= 0 ? 1 : 0;
+}
+
+// ---- layer filters on a caller's grid (emap_grid_filter, csrc/emap_filters.cuh) -------------------------------------
+
+static_assert(EMAP_FILTER_MAX_KERNEL == PP_MAX_KERNEL, "the Gaussian's coefficients hold EMAP_FILTER_MAX_KERNEL taps");
+
+// The Gaussian's kernel size: kernel_size, or for 0 cv::GaussianBlur's size from sigma on a float image,
+// cvRound(sigma * 4 * 2 + 1) | 1 (cvRound rounds half to even); 0 when that is not in [1, EMAP_FILTER_MAX_KERNEL].
+static int gauss_kernel_size(const emap_filter_op& f) {
+  if (f.kernel_size != 0) return f.kernel_size;
+  if (!(f.sigma > 0.0)) return 0;
+  const double q = std::nearbyint(f.sigma * 4 * 2 + 1);
+  return q <= EMAP_FILTER_MAX_KERNEL ? ((int)q | 1) : 0;
+}
+
+// Why f is rejected for a rows x cols grid (nullptr: accepted).
+static const char* filter_error(const emap_filter_op& f, int64_t rows, int64_t cols) {
+  const int k = f.kernel_size;
+  const bool sized = f.op != EMAP_FILTER_MIN_VALUES && f.op != EMAP_FILTER_OUTLINE;
+  if (f.op < EMAP_FILTER_MIN_VALUES || f.op > EMAP_FILTER_OUTLINE) return "unknown op";
+  const bool from_sigma = f.op == EMAP_FILTER_GAUSSIAN_BLUR && k == 0;
+  if (sized && !from_sigma && (k < 1 || k > EMAP_FILTER_MAX_KERNEL))
+    return "kernel_size must be in [1, EMAP_FILTER_MAX_KERNEL]";
+  if ((f.op == EMAP_FILTER_MEDIAN || f.op == EMAP_FILTER_BOX_BLUR) && f.number_of_repeats < 1)
+    return "number_of_repeats must be >= 1";
+  if (f.op == EMAP_FILTER_MEDIAN) {
+    const int64_t last = (int64_t)k + (int64_t)f.delta_kernel_size * (f.number_of_repeats - 1);
+    const int64_t top = last <= 5 ? 5 : EMAP_FILTER_MAX_KERNEL;
+    if (!(k & 1) || (f.delta_kernel_size & 1) || last < 1 || last > top || (last <= 5 && k > 5))
+      return "every median kernel must be odd, 1, 3 or 5 on the float path and at most EMAP_FILTER_MAX_KERNEL on the "
+             "8-bit path";
+  }
+  if (f.op == EMAP_FILTER_GAUSSIAN_BLUR) {
+    if (!std::isfinite(f.sigma)) return "sigma must be finite";
+    if (!(gauss_kernel_size(f) & 1))
+      return "the Gaussian's kernel_size must be odd, or 0 with a sigma above 0 that gives at most EMAP_FILTER_MAX_KERNEL";
+  }
+  if ((f.op == EMAP_FILTER_DILATE || f.op == EMAP_FILTER_ERODE) && (rows < k || cols < k))
+    return "the grid has fewer rows or columns than kernel_size";
+  if (f.op == EMAP_FILTER_OUTLINE && (rows < 3 || cols < 3)) return "outline needs at least 3 rows and 3 columns";
+  return nullptr;
+}
+
+namespace {
+// emap_grid_filter's scratch for n cells: the fill's parents and keys, header words (the Gaussian's flag, the 8-bit
+// path's range), two float planes, the box's double row sums, two 8-bit images, and the host-bound output.
+struct FilterScratch {
+  int *parent, *hdr;
+  unsigned* key;
+  float* f[2];
+  double* rs;
+  uint8_t* u[2];
+  float* out;
+};
+
+size_t carve_filter(int64_t n, bool host_out, void* base, FilterScratch& s) {
+  Carver c{(uintptr_t)base};
+  s.parent = c.take<int>(n); s.key = c.take<unsigned>(n); s.hdr = c.take<int>(8);
+  s.f[0] = c.take<float>(n); s.f[1] = c.take<float>(n); s.rs = c.take<double>(n);
+  s.u[0] = c.take<uint8_t>(n); s.u[1] = c.take<uint8_t>(n);
+  s.out = c.take<float>(host_out ? n : 0);
+  return c.bytes;
+}
+}  // namespace
+
+// The passes of one accepted filter from `in` into `o` (include/emap.h lists them per op).
+static int filter_passes(emap_handle* h, const emap_filter_op& f, const float* in, const float* mask, float* o,
+                         int rows, int cols, FilterScratch& s) {
+  const int n = rows * cols, cb = cdiv(n, GF_THREADS), k = f.kernel_size;
+  switch (f.op) {
+    case EMAP_FILTER_MIN_VALUES: {
+      PlaneScratch p{};
+      p.parent = s.parent; p.key = s.key;
+      k_pl_fill_init<<<cb, PL_THREADS, 0, h->stream>>>(in, s.parent, s.key, s.hdr, n);
+      LAUNCH_CHECK();
+      if (int rc = plane_components(h, p, rows, cols, 0)) return rc;
+      k_pl_fill_min<<<cb, PL_THREADS, 0, h->stream>>>(in, s.parent, s.key, rows, cols);
+      LAUNCH_CHECK();
+      k_pl_fill_write<<<cb, PL_THREADS, 0, h->stream>>>(in, s.parent, s.key, o, n);
+      LAUNCH_CHECK();
+      return 0;
+    }
+    case EMAP_FILTER_MEDIAN: {
+      const int R = f.number_of_repeats, d = f.delta_kernel_size;
+      if (k + d * (R - 1) <= 5) {
+        const float* src = in;
+        for (int r = 0; r < R; r++) {
+          float* dst = r == R - 1 ? o : s.f[r & 1];
+          const int kr = k + d * r;
+          if (kr == 1) CK(cudaMemcpyAsync(dst, src, sizeof(float) * n, cudaMemcpyDeviceToDevice, h->stream));
+          else {
+            (kr == 3 ? k_pl_median<3, true> : k_pl_median<5, true>)<<<cb, PL_THREADS, 0, h->stream>>>(src, dst, rows,
+                                                                                                    cols);
+            LAUNCH_CHECK();
+          }
+          src = dst;
+        }
+        return 0;
+      }
+      unsigned* w = (unsigned*)s.hdr;
+      CK(cudaMemsetAsync(w, 0, 3 * sizeof(unsigned), h->stream));
+      k_gf_range<<<cb, GF_THREADS, 0, h->stream>>>(in, w, n);
+      LAUNCH_CHECK();
+      k_gf_quantise<<<cb, GF_THREADS, 0, h->stream>>>(in, w, s.u[0], n);
+      LAUNCH_CHECK();
+      int cur = 0;
+      for (int r = 0; r < R; r++) {
+        const int kr = k + d * r;
+        if (kr == 1) continue;
+        k_gf_median_u8<<<dim3(cdiv(cols, GF_MED_COLS), cdiv(rows, GF_MED_ROWS)), GF_MED_COLS, 0, h->stream>>>(
+            s.u[cur], s.u[cur ^ 1], rows, cols, kr);
+        LAUNCH_CHECK();
+        cur ^= 1;
+      }
+      k_gf_dequantise<<<cb, GF_THREADS, 0, h->stream>>>(s.u[cur], w, o, n);
+      LAUNCH_CHECK();
+      return 0;
+    }
+    case EMAP_FILTER_BOX_BLUR: {
+      const float* src = in;
+      if (k <= 5) CK(cudaMemsetAsync(s.hdr, 0xff, sizeof(int), h->stream));     // k_pp_box_rows runs where hdr[0] != 0
+      for (int r = 0; r < f.number_of_repeats; r++) {
+        float* dst = r == f.number_of_repeats - 1 ? o : s.f[r & 1];
+        if (k <= 5) k_pp_box_rows<true><<<cb, PL_THREADS, 0, h->stream>>>(src, s.rs, s.hdr, rows, cols, k);
+        else k_gf_box_rows<<<cdiv(rows, 128), 128, 0, h->stream>>>(src, s.rs, rows, cols, k);
+        LAUNCH_CHECK();
+        k_gf_box_cols<<<cdiv(cols, 128), 128, 0, h->stream>>>(s.rs, dst, rows, cols, k, 1.0 / ((double)k * k));
+        LAUNCH_CHECK();
+        src = dst;
+      }
+      return 0;
+    }
+    case EMAP_FILTER_GAUSSIAN_BLUR: {
+      const int kg = gauss_kernel_size(f);
+      PpGauss g;
+      g.h = kg / 2;
+      pp_gauss_coeffs(kg, g.c, f.sigma);
+      CK(cudaMemsetAsync(s.hdr, 0xff, sizeof(int), h->stream));     // k_pp_gauss runs where hdr[0] != 0
+      k_pp_gauss<true, true><<<cb, PL_THREADS, 0, h->stream>>>(in, s.f[0], s.hdr, rows, cols, g);
+      LAUNCH_CHECK();
+      k_pp_gauss<false, true><<<cb, PL_THREADS, 0, h->stream>>>(s.f[0], o, s.hdr, rows, cols, g);
+      LAUNCH_CHECK();
+      return 0;
+    }
+    case EMAP_FILTER_DILATE:
+    case EMAP_FILTER_ERODE: {
+      const bool mx = f.op == EMAP_FILTER_DILATE;
+      (mx ? k_gf_morph_cols<true> : k_gf_morph_cols<false>)<<<cb, GF_THREADS, 0, h->stream>>>(in, mask, s.f[0], rows,
+                                                                                               cols, k);
+      LAUNCH_CHECK();
+      (mx ? k_gf_morph_rows<true> : k_gf_morph_rows<false>)<<<cb, GF_THREADS, 0, h->stream>>>(
+          in, mask, s.f[0], o, rows, cols, k, f.inpaint != 0);
+      LAUNCH_CHECK();
+      return 0;
+    }
+    default:
+      k_gf_outline<<<cb, GF_THREADS, 0, h->stream>>>(in, o, rows, cols);
+      LAUNCH_CHECK();
+      return 0;
+  }
+}
+
+// grid_map_filters_rsl's layer filters on a caller's grid (include/emap.h).  Every check runs before anything is
+// written or launched.
+int emap_grid_filter(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, const emap_filter_op* f,
+                     const float* mask, float* out, int32_t out_is_device) {
+  ENTER(h);
+  const char* e = !grid || !f || !out ? "null argument"
+                                      : gl_check_grid(grid->data, grid->rows, grid->cols, grid->position,
+                                                      grid->resolution, 1);
+  if (!e) e = filter_error(*f, grid->rows, grid->cols);
+  if (e) return fail_in(h, "emap_grid_filter", e);
+  NvtxRange nv("emap:grid_filter");
+  const emap_filter_op op = *f;
+  const int rows = (int)grid->rows, cols = (int)grid->cols;
+  const int64_t n = (int64_t)rows * cols;
+  const size_t bytes = sizeof(float) * n;
+  FilterScratch s;
+  if (int rc = grow(h, h->filters.block, carve_filter(n, !out_is_device, nullptr, s), 0, false)) return rc;
+  carve_filter(n, !out_is_device, h->filters.block, s);
+  const bool morph = op.op == EMAP_FILTER_DILATE || op.op == EMAP_FILTER_ERODE;
+  const float* data = grid->data;
+  const float* m = morph ? mask : nullptr;
+  if (int rc = stage_inputs(h, h->filters.up, data, grid_on_device ? 0 : bytes, m, m && !grid_on_device ? bytes : 0))
+    return rc;
+  float* o = out_is_device ? out : s.out;
+  if (int rc = filter_passes(h, op, data, m, o, rows, cols, s)) return rc;
+  if (!out_is_device) {
+    if (int rc = read_back(h, h->filters, o, bytes)) return rc;
+    memcpy(out, h->filters.down, bytes);
+  }
+  return EMAP_OK;
 }
 
 }  // extern "C"

@@ -53,6 +53,22 @@ GRID_HD double grid_axis_position(double pos, double len, double res, int64_t i)
   return grid_axis_at(grid_axis_origin(pos, len, res), res, i);
 }
 
+// grid_map_cv's toImage<uchar, 1>(lo, hi) of one non-NaN cell: clamped to [lo, hi] and (uchar)(((v - lo) / (hi - lo)) *
+// 255.0f) in float, truncated, a NaN quotient giving 0 (x86's conversion).  emap_nonlinear_interpolation and
+// emap_grid_filter's 8-bit median quantise with it.
+#if defined(__CUDACC__)
+__device__ __forceinline__ uint8_t grid_to_u8(float x, float lo, float hi) {
+  x = x < lo ? lo : (x > hi ? hi : x);
+  const float r = __fmul_rn(__fdiv_rn(__fsub_rn(x, lo), __fsub_rn(hi, lo)), 255.0f);
+  return (r == r) ? (uint8_t)(int)r : (uint8_t)0;
+}
+
+// convertTo(CV_32F, (hi - lo) / 255, lo) of one 8-bit value: a fused multiply-add, as cv::Mat::convertTo's x86 path.
+__device__ __forceinline__ float grid_from_u8(uint8_t u, float lo, float hi) {
+  return __fmaf_rn((float)u, __fdiv_rn(__fsub_rn(hi, lo), 255.0f), lo);
+}
+#endif
+
 // The grids the calls accept (min_cells: the fewest rows and columns): nullptr, or why not.  Within these bounds a
 // projected line end is always inside the map (include/emap.h).
 inline const char* gl_check_grid(const float* data, int64_t rows, int64_t cols, const double pos[2], double res,

@@ -229,6 +229,8 @@ struct emap_handle {
   } inpaint;
   Staging inpaint_image;           // emap_inpaint_image / emap_nonlinear_interpolation: inpaint_scratch's block (and a
                                    // host-bound grid), a host image and mask or grid, the host output
+  Staging filters;                 // emap_grid_filter: the block carved by carve_filter (and a host-bound output), a
+                                   // host grid and mask, the host output
   DevBuf<char> pca_block;          // emap_features_pca: one device block carved by carve_pca
   Staging query;                   // emap_project_to_planar_regions: the block carved by carve_query, host tables and
                                    // queries, the host outputs

@@ -526,6 +526,8 @@ IP_HD bool ip_eval_child_ns_fast(const InpaintView& v, int c, int cur, bool firs
 #if defined(__CUDACC__)
 #include <cooperative_groups.h>
 
+#include "emap_grid.cuh"
+
 // device-resident control block of one inpainting run
 struct InpaintCtl {
   int heap_cnt[2];                // entries of the two heap lists (ping-pong)
@@ -746,14 +748,10 @@ k_ip_grid_init(const float* __restrict__ h, InpaintView v, const InpaintCtl* __r
     const int ci = (i - 1) * W + (j - 1);
     float lo = 3.402823466e38f, hi = -3.402823466e38f;
     if (ctl->n_valid) ip_grid_range(ctl, lo, hi);
-    float x = h[ci];
+    const float x = h[ci];
     uint8_t q = 0;
     if (x != x) f = IP_INSIDE;
-    else {
-      x = x < lo ? lo : (x > hi ? hi : x);
-      const float r = __fmul_rn(__fdiv_rn(__fsub_rn(x, lo), __fsub_rn(hi, lo)), 255.0f);
-      q = (r == r) ? (uint8_t)(int)r : (uint8_t)0;
-    }
+    else q = grid_to_u8(x, lo, hi);
     v.img[ci] = q;
   }
   v.f[p] = f; v.T[p] = IP_TBIG; v.ord[p] = IP_ROOT;
@@ -770,7 +768,7 @@ k_ip_grid_out(int C, const uint8_t* __restrict__ img, const float* __restrict__ 
   if (x == x || ctl->n_valid == 0) { out[i] = x; return; }
   float lo, hi;
   ip_grid_range(ctl, lo, hi);
-  out[i] = __fmaf_rn((float)img[i], __fdiv_rn(__fsub_rn(hi, lo), 255.0f), lo);
+  out[i] = grid_from_u8(img[i], lo, hi);
 }
 
 // plugins/inpainting.py:60: dst.astype(float32) * (h_max - h_min) / 255 + h_min

@@ -305,8 +305,9 @@ __global__ void k_pl_fill_write(const float* __restrict__ raw, const int* __rest
   out[i] = parent[i] >= 0 ? tsub_funkey(key[parent[i]]) : raw[i];
 }
 
-// cv::medianBlur on CV_32F: the exact median of the K x K values around each cell, border replicated.
-template <int K>
+// cv::medianBlur on CV_32F: the exact median of the K x K values around each cell, border replicated.  With KEEP_NAN a
+// NaN cell stays NaN, as in cv2 (emap_grid_filter); the fminf / fmaxf network itself passes over NaN operands.
+template <int K, bool KEEP_NAN = false>
 __global__ void k_pl_median(const float* __restrict__ src, float* __restrict__ dst, int rows, int cols) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= rows * cols) return;
@@ -327,7 +328,7 @@ __global__ void k_pl_median(const float* __restrict__ src, float* __restrict__ d
       v[b - 1] = fminf(x, y);
       v[b] = fmaxf(x, y);
     }
-  dst[i] = v[K * K / 2];
+  dst[i] = KEEP_NAN && isnan(src[i]) ? src[i] : v[K * K / 2];
 }
 
 // runSlidingWindowDetector: planar iff the centre is finite, error < thr2 and n.z > cos_local.

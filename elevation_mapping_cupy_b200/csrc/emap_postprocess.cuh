@@ -25,19 +25,21 @@ inline int pp_kernel_size(double size, double res) {
   return 2 * (int)q + 1;
 }
 
-// cv::getGaussianKernel(k, 0, CV_32F) for odd k <= PP_MAX_KERNEL: OpenCV's fixed tables up to k = 9, else
-// exp(-x^2 / (2 sigma^2)) with sigma = 0.3 ((k - 1) / 2 - 1) + 0.8, scaled by 1 / its sum, in double, rounded to float.
-inline void pp_gauss_coeffs(int k, float* out) {
+// cv::getGaussianKernel(k, sigma, CV_32F) for odd k <= PP_MAX_KERNEL: with sigma <= 0 OpenCV's fixed tables up to
+// k = 9, else exp(-x^2 / (2 sigma^2)) with sigma = 0.3 ((k - 1) / 2 - 1) + 0.8 when sigma <= 0, scaled by 1 / its sum,
+// in double, rounded to float.
+inline void pp_gauss_coeffs(int k, float* out, double sigma = 0.0) {
   static const float t1[] = {1.f}, t3[] = {0.25f, 0.5f, 0.25f}, t5[] = {0.0625f, 0.25f, 0.375f, 0.25f, 0.0625f},
                      t7[] = {0.03125f, 0.109375f, 0.21875f, 0.28125f, 0.21875f, 0.109375f, 0.03125f},
                      t9[] = {4 / 256.f, 13 / 256.f, 30 / 256.f, 51 / 256.f, 60 / 256.f, 51 / 256.f, 30 / 256.f,
                              13 / 256.f, 4 / 256.f};
   const float* tab[] = {t1, t3, t5, t7, t9};
-  if (k <= 9) {
+  if (k <= 9 && !(sigma > 0.0)) {
     for (int i = 0; i < k; i++) out[i] = tab[k / 2][i];
     return;
   }
-  const double sigma = ((k - 1) * 0.5 - 1) * 0.3 + 0.8, scale2x = -0.5 / (sigma * sigma);
+  if (!(sigma > 0.0)) sigma = ((k - 1) * 0.5 - 1) * 0.3 + 0.8;
+  const double scale2x = -0.5 / (sigma * sigma);
   double w[PP_MAX_KERNEL], sum = 0.0;
   for (int i = 0; i < k; i++) {
     const double x = i - (k - 1) * 0.5;
@@ -72,6 +74,24 @@ struct PpGauss {
 // replicated (clamped) like BORDER_REPLICATE.
 
 __device__ __forceinline__ int pp_clamp(int v, int hi) { return min(max(v, 0), hi); }
+
+// grid_map_filters_rsl's window corner on one axis of n cells (processing.cpp:37-48): max(v - (k - 1) / 2, 0), pulled
+// back to n - k where the window would overshoot.  n >= k (checked on the host).
+__device__ __forceinline__ int pp_corner(int v, int n, int k) {
+  const int c = max(v - (k - 1) / 2, 0);
+  return c + k > n ? n - k : c;
+}
+
+// cv::borderInterpolate(v, hi + 1, BORDER_REFLECT_101): reflected about the edge cells, as often as needed.
+__device__ __forceinline__ int pp_reflect101(int v, int hi) {
+  if (hi == 0) return 0;
+  while (v < 0 || v > hi) v = v < 0 ? -v : 2 * hi - v;
+  return v;
+}
+
+// The index of row or column v of an axis of hi + 1 cells: border replicated (clamped), or BORDER_REFLECT_101.
+template <bool REFLECT>
+__device__ __forceinline__ int pp_border(int v, int hi) { return REFLECT ? pp_reflect101(v, hi) : pp_clamp(v, hi); }
 
 // elevationWithNaN = plane_classification == 1 ? elevation : NaN (layers 1 and 3 of lay) into the fill's input a and
 // into layer 4.
@@ -116,10 +136,7 @@ __global__ void k_pp_slope(const float* __restrict__ src, float* __restrict__ ds
   __syncthreads();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= rows * cols || !hdr[0]) return;
-  const int r = i / cols, c = i - r * cols;
-  int r0 = max(r - h, 0), c0 = max(c - h, 0);
-  if (r0 + k > rows) r0 = rows - k;
-  if (c0 + k > cols) c0 = cols - k;
+  const int r0 = pp_corner(i / cols, rows, k), c0 = pp_corner(i % cols, cols, k);
   float best = __int_as_float(0x7fc00000);
   bool any = false;
   for (int a = 0; a < k; a++) {
@@ -136,16 +153,18 @@ __global__ void k_pp_slope(const float* __restrict__ src, float* __restrict__ ds
 }
 
 // cv::boxFilter's sums in double (exact for fp32 values within 29 binary orders of magnitude of each other, so the
-// order does not matter): ROWS sums 2 h + 1 cells along the row into rs; the column pass sums 2 h + 1 of those and
-// rounds sum * scale (OpenCV's double 1 / k^2) to float.
+// order does not matter): ROWS sums the k cells c - k / 2 .. c - k / 2 + k - 1 of the row into rs, left to right; the
+// column pass sums 2 h + 1 of those and rounds sum * scale (OpenCV's double 1 / k^2) to float.  The border is
+// replicated, or BORDER_REFLECT_101 with REFLECT (emap_grid_filter's cv::blur row sums for k <= 5).
+template <bool REFLECT = false>
 __global__ void k_pp_box_rows(const float* __restrict__ src, double* __restrict__ rs, const int* __restrict__ hdr,
-                              int rows, int cols, int h) {
+                              int rows, int cols, int k) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= rows * cols || !hdr[0]) return;
   const int r = i / cols, c = i - r * cols;
   const float* row = src + (long long)r * cols;
   double s = 0.0;
-  for (int d = -h; d <= h; d++) s += (double)__ldg(row + pp_clamp(c + d, cols - 1));
+  for (int d = -(k / 2); d < k - k / 2; d++) s += (double)__ldg(row + pp_border<REFLECT>(c + d, cols - 1));
   rs[i] = s;
 }
 
@@ -161,8 +180,9 @@ __global__ void k_pp_box_cols(const double* __restrict__ rs, float* __restrict__
 
 // One pass of the separable Gaussian, along the row (ROW) or the column: s = c[h] x0, then s += c[h + j] (x+j + x-j)
 // for j = 1 .. h, each operation rounded to fp32 on its own (no contraction).  Bit-identical to cv::GaussianBlur for
-// k = 3 (rows first); DESIGN.md §4l states the bound for longer kernels.
-template <bool ROW>
+// k = 3 (rows first); DESIGN.md §4l states the bound for longer kernels.  The border is replicated, or BORDER_REFLECT_101
+// (cv::GaussianBlur's default, emap_grid_filter) with REFLECT.
+template <bool ROW, bool REFLECT = false>
 __global__ void k_pp_gauss(const float* __restrict__ src, float* __restrict__ dst, const int* __restrict__ hdr, int rows,
                            int cols, const __grid_constant__ PpGauss g) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -170,10 +190,10 @@ __global__ void k_pp_gauss(const float* __restrict__ src, float* __restrict__ ds
   const int r = i / cols, c = i - r * cols;
   float s = __fmul_rn(g.c[g.h], src[i]);
   for (int j = 1; j <= g.h; j++) {
-    const float a = ROW ? __ldg(src + (long long)r * cols + pp_clamp(c + j, cols - 1))
-                        : __ldg(src + (long long)pp_clamp(r + j, rows - 1) * cols + c);
-    const float b = ROW ? __ldg(src + (long long)r * cols + pp_clamp(c - j, cols - 1))
-                        : __ldg(src + (long long)pp_clamp(r - j, rows - 1) * cols + c);
+    const float a = ROW ? __ldg(src + (long long)r * cols + pp_border<REFLECT>(c + j, cols - 1))
+                        : __ldg(src + (long long)pp_border<REFLECT>(r + j, rows - 1) * cols + c);
+    const float b = ROW ? __ldg(src + (long long)r * cols + pp_border<REFLECT>(c - j, cols - 1))
+                        : __ldg(src + (long long)pp_border<REFLECT>(r - j, rows - 1) * cols + c);
     s = __fadd_rn(s, __fmul_rn(g.c[g.h + j], __fadd_rn(a, b)));
   }
   dst[i] = s;

@@ -907,6 +907,68 @@ class ElevationMap:
                            int(device), after=device or g_dev, before=device)
         return out
 
+    def min_values(self, grid, layer="elevation", out=None):
+        """grid_map_filters_rsl's inpainting::minValues: every NaN cell of `layer` takes the least non-NaN value next to
+        its NaN region.  `grid`, `layer` and `out` as in nonlinear_interpolation; include/emap.h (emap_grid_filter)
+        states every filter's rule.  Returns `out`."""
+        return self._grid_filter("min_values", grid, layer, out)
+
+    def median(self, grid, layer="elevation", *, kernel_size, delta_kernel_size=2, number_of_repeats=1, out=None):
+        """smoothing::median: cv2.medianBlur on the float layer while kernel_size + delta_kernel_size *
+        (number_of_repeats - 1) <= 5, else on the layer quantised to 8 bits between its finite minimum and maximum; the
+        kernel grows by delta_kernel_size per repeat.  The float path is not cv2's on a layer with NaN holes: only
+        windows without a NaN are (include/emap.h)."""
+        return self._grid_filter("median", grid, layer, out, kernel_size=kernel_size,
+                                 delta_kernel_size=delta_kernel_size, number_of_repeats=number_of_repeats)
+
+    def box_blur(self, grid, layer="elevation", *, kernel_size, number_of_repeats=1, out=None):
+        """smoothing::boxBlur: number_of_repeats of cv2.blur((kernel_size, kernel_size)), bit for bit."""
+        return self._grid_filter("box_blur", grid, layer, out, kernel_size=kernel_size,
+                                 number_of_repeats=number_of_repeats)
+
+    def gaussian_blur(self, grid, layer="elevation", *, kernel_size, sigma, out=None):
+        """smoothing::gaussianBlur: cv2.GaussianBlur((kernel_size, kernel_size), sigma); kernel_size 0 takes cv2's size
+        from sigma."""
+        return self._grid_filter("gaussian_blur", grid, layer, out, kernel_size=kernel_size, sigma=sigma)
+
+    def dilate(self, grid, layer="elevation", *, kernel_size, mask=None, inpaint=True, out=None):
+        """processing::dilate: the max of the finite values of layer * mask (a (rows, cols) float32 array on the
+        layer's side; None, the reference's empty mask, reads the layer alone) in grid_map's clamped kernel_size
+        window."""
+        return self._grid_filter("dilate", grid, layer, out, kernel_size=kernel_size, mask=mask, inpaint=inpaint)
+
+    def erode(self, grid, layer="elevation", *, kernel_size, mask=None, inpaint=True, out=None):
+        """processing::erode: as dilate, with the min."""
+        return self._grid_filter("erode", grid, layer, out, kernel_size=kernel_size, mask=mask, inpaint=inpaint)
+
+    def outline(self, grid, layer="elevation", out=None):
+        """processing::outline: the cells next to a NaN keep their value, every other cell becomes NaN."""
+        return self._grid_filter("outline", grid, layer, out)
+
+    def _grid_filter(self, op, grid, layer, out, kernel_size=1, delta_kernel_size=0, number_of_repeats=1, sigma=0.0,
+                     mask=None, inpaint=True):
+        """One emap_grid_filter call: `op` on grid["layers"][layer] into `out` (None: a new array on the layer's side,
+        else a contiguous (rows, cols) float32 NumPy array or CUDA tensor, written in place; device output is
+        stream-ordered with no host synchronisation).  Returns `out`."""
+        g = self._grid(grid, layer)
+        g_dev = _is_device(g._keep)
+        shape = (int(g.rows), int(g.cols))
+        m = None
+        if mask is not None:
+            m = _input_array(mask, "float32", "mask")
+            if tuple(m.shape) != shape or _is_device(m) != g_dev:
+                raise ValueError("mask must be a (rows, cols) float32 array on the layer's side")
+        dev = _output_device([g._keep if out is None else out])
+        device = dev is not None
+        if out is None:
+            out = _array_maker(dev)(shape, "float32")
+        _check_out({"layer": out}, {"layer": (shape, "float32")}, device)
+        f = _lib.EmapFilterOp(_lib.EMAP_FILTER_OPS[op], int(kernel_size), int(delta_kernel_size),
+                              int(number_of_repeats), float(sigma), int(bool(inpaint)))
+        self._ordered_call(self._L.emap_grid_filter, self._h, C.byref(g), int(g_dev), C.byref(f), _address(m),
+                           _address(out), int(device), after=device or g_dev, before=device)
+        return out
+
     def _grid(self, grid, layer):
         """The EmapGrid of grid["layers"][layer] (_input_array, kept alive as g._keep), centred at the dict's "centre" or,
         in a get_transformed_submap(s) dict, its "frame_centre", with its "resolution" or the map's."""

@@ -1136,6 +1136,78 @@ int emap_stream(emap_handle* h, void** cuda_stream);
  * before it, a new semantic configuration, more class_max slots): run an eager frame of the largest size and
  * configuration first, then capture.  Cannot be captured: pageable host clouds (staged with a synchronising copy). */
 int emap_set_stream(emap_handle* h, void* cuda_stream);
+/* ---- layer filters on a caller's grid: grid_map_filters_rsl's inpainting::minValues (inpainting.cpp:25-94),
+ * smoothing::median, boxBlur and gaussianBlur (smoothing.cpp) and processing::dilate, erode and outline (processing.cpp)
+ * on an emap_grid exactly as the lookups take it (host or device, the same checks), into out (rows x cols floats, host or
+ * device as out_is_device says; it must not overlap the grid or the mask).  The handle's map is neither read nor
+ * changed.  Results are compared NaN-aware: every non-NaN cell bit for bit, NaN where the reference has NaN (the
+ * device's NaN payload is its own).  f->op and its parameters (k = kernel_size):
+ *  EMAP_FILTER_MIN_VALUES: every NaN cell takes the least value (±inf included, -0.0 before +0.0) of the non-NaN cells
+ *   4-adjacent to its 4-connected NaN component: the fixed point of the reference's in-place sweep.  A component with
+ *   no such neighbour (a grid with no non-NaN cell) stays NaN.  Kernels: 5.
+ *  EMAP_FILTER_MEDIAN (k, delta_kernel_size, number_of_repeats): with k + delta (repeats - 1) <= 5, repeats of
+ *   cv::medianBlur on CV_32F with the kernel k + delta i of repeat i (each 1, 3 or 5; 1 copies), border replicated: the
+ *   exact median of each window's values, bit-identical to cv2 where the window holds no NaN.  On a layer with NaN
+ *   holes this path is NOT cv2's: every cell whose window holds a NaN may differ (on a grid a quarter NaN, about half
+ *   the cells at k = 3).  cv2's sorting network moves a NaN by its SIMD or scalar code path, so its own result there
+ *   depends on the column; here a NaN cell stays NaN and the network passes over the other NaNs.
+ *   Otherwise toImage<uchar, 1> between the finite minimum lo and maximum hi (emap_nonlinear_interpolation's
+ *   quantisation; nothing finite: lo = FLT_MAX, hi = -FLT_MAX), repeats of the 8-bit cv::medianBlur (each kernel odd,
+ *   1 .. EMAP_FILTER_MAX_KERNEL) and out = fma(u8, (hi - lo) / 255.0f, lo) into every cell, NaN cells included, as the
+ *   reference converts back.  Kernels: one per repeat with a kernel above 1, plus 3 on the 8-bit path.
+ *  EMAP_FILTER_BOX_BLUR (k, number_of_repeats): repeats of cv::blur((k, k)), BORDER_REFLECT_101, in OpenCV's order:
+ *   row sums in double (k <= 5: each window left to right; else the running sum s += x[c + k] - x[c]), then one
+ *   running double sum per column from the top border row down, float(s * (1.0 / k^2)).  NaN and inf propagate down a
+ *   column as in cv2.  k may be even (anchor k / 2).  Kernels: 2 per repeat.
+ *  EMAP_FILTER_GAUSSIAN_BLUR (k odd, or 0 with sigma > 0, sigma): cv::GaussianBlur((k, k), sigma), BORDER_REFLECT_101;
+ *   k = 0 takes cv2's size for a float image, cvRound(8 sigma + 1) | 1.  The coefficients of
+ *   cv::getGaussianKernel(k, sigma, CV_32F) (sigma <= 0: from k), rows then columns, c0 x0 + sum c_j (x_+j + x_-j) in
+ *   fp32 without contraction.  Bit-identical to cv2 4.13 for k <= 3 with sigma <= 0, NaN and ±inf included; otherwise
+ *   within EMAP_POST_GAUSS_ULPS(k) units in the last place of the grid's largest finite magnitude (finite grids).
+ *   Kernels: 2.
+ *  EMAP_FILTER_DILATE / EMAP_FILTER_ERODE (k, mask, inpaint): processing.cpp's k x k window, its corner max(cell -
+ *   (k - 1) / 2, 0) pulled back to rows - k (cols - k) where it would overshoot, over in * mask (fp32; in alone with a
+ *   NULL mask).  m = block.maxCoeffOfFinites() (minCoeffOfFinites) as Eigen's redux computes it: grid_map's functor
+ *   op(a, b) (restated from its published FunctorsPlugin.hpp: the finite operand when only one is finite, else
+ *   std::max(a, b) = a < b ? b : a, or std::min(a, b) = b < a ? b : a) folded over the window's cells from its first,
+ *   down each column, column after column.  So m is the window's largest (least) finite value, the earliest in that
+ *   order on a tie (the sign of a zero is the earliest zero's); a window with no finite value gives NaN when its first
+ *   cell is NaN, else the window's largest (least) infinity.  out = m, or the cell's own value where m is NaN; with
+ *   inpaint = 0 a NaN cell stays NaN.  rows and cols must be >= k.  Kernels: 2 (the columns' folds, then the rows'; a
+ *   window with no finite value is folded cell by cell in the second).
+ *  EMAP_FILTER_OUTLINE: a cell whose clamped 3 x 3 window holds a NaN keeps its value; every other cell becomes NaN.
+ *   rows and cols must be >= 3.  Kernels: 1.
+ * mask: NULL or rows x cols floats on the grid's side; only dilate and erode read it.  Host inputs (grid, mask) are
+ * uploaded in one copy; host output comes back in one copy and one synchronisation.  Device output is stream-ordered
+ * with no host synchronisation.
+ * EMAP_ERR_INVALID, with nothing written or launched: everything the lookups reject for their grid; a NULL f or out; an
+ * unknown op; a kernel size below 1 (a Gaussian's 0 with sigma > 0 excepted) or above EMAP_FILTER_MAX_KERNEL (for the
+ * Gaussian's 0, the size from sigma above it), or even where cv2 needs it odd (median, Gaussian;
+ * a median kernel sequence that leaves 1 .. EMAP_FILTER_MAX_KERNEL, or a float median kernel other than 1, 3 and 5); a
+ * non-positive number_of_repeats (median, box); a sigma that is not finite; a dilate, erode or outline window larger
+ * than the grid.
+ * Not provided: inpainting::biLinearInterpolation (its weights come from Eigen's float colPivHouseholderQr and its
+ * fallback runs nonlinearInterpolation at 2 pixels, which emap_nonlinear_interpolation rejects),
+ * processing::applyKernelFunction (it takes a C++ callable) and any plugin or parameter-file wiring. */
+#define EMAP_FILTER_MIN_VALUES 0
+#define EMAP_FILTER_MEDIAN 1
+#define EMAP_FILTER_BOX_BLUR 2
+#define EMAP_FILTER_GAUSSIAN_BLUR 3
+#define EMAP_FILTER_DILATE 4
+#define EMAP_FILTER_ERODE 5
+#define EMAP_FILTER_OUTLINE 6
+#define EMAP_FILTER_MAX_KERNEL 63
+typedef struct emap_filter_op {
+  int32_t op;                  /* EMAP_FILTER_* */
+  int32_t kernel_size;         /* median, box, Gaussian, dilate, erode */
+  int32_t delta_kernel_size;   /* median: the kernel's growth per repeat */
+  int32_t number_of_repeats;   /* median, box */
+  double sigma;                /* Gaussian */
+  int32_t inpaint;             /* dilate, erode */
+} emap_filter_op;
+int emap_grid_filter(emap_handle* h, const emap_grid* grid, int32_t grid_on_device, const emap_filter_op* f,
+                     const float* mask, float* out, int32_t out_is_device);
+
 /* Stream ordering WITHOUT host synchronisation between the handle's stream and a stream of the caller's framework
  * (torch / CuPy current stream; NULL = the legacy default stream): after emap_wait_for_stream the handle's next work runs
  * after everything queued on `cuda_stream` so far (the caller wrote a buffer the library will read); after
